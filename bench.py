@@ -2,7 +2,7 @@
 """Benchmark of the DD3D inference hot path (contract: see the task statement / DESIGN.md "Measurement").
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload v2_99|dla34|nusc_v2_99]
-                    [--batch B] [--dtype bf16|fp16] [--input mapped|raw] [--sweep 8,16,32,64]
+                    [--batch B] [--dtype bf16|fp16] [--input mapped|raw] [--sweep 8,16,32,64] [--dump-outputs DIR]
 
 A step = one DD3D.forward over one batch of synthetic images per GPU:
   v2_99 (default, the config BASELINE.json's metric is quoted on): V2-99 DD3D, 32 x 900x1600 per GPU;
@@ -17,6 +17,10 @@ forward of step k+1 and no host synchronisation happens inside the timed region.
 it needs detectron2/pytorch3d, not installable offline) on rank 0 with all host threads, following BASELINE.md 3
 (batch = min(B, 8) images per forward, bounded so that the run ends within minutes).
 `--sweep` (BASELINE.json configs[4]): per-GPU batch sweep; prints one JSON line per batch size.
+`--dump-outputs DIR`: after the timed steps, writes what the last timed step returned (the packed detections and their
+counts -- with N > 1 the all-gathered buffer of every rank; NuscenesDD3D also rank 0's aggregated global boxes) as
+DIR/<name>.npy, or DIR/batch<B>/<name>.npy per batch size of a --sweep.  Inputs and weights are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -42,13 +46,19 @@ WORKLOADS = {
 
 
 def load_peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            p = json.load(f)
-        return dict(tflops=p.get("bf16_tflops_sustained", p.get("bf16_tflops", 1400.0)), gbs=p.get("hbm_gbs", 6650.0),
-                    source="measured (MEASURED_PEAKS.json: bf16_tflops_sustained / hbm_gbs)")
-    return dict(tflops=1400.0, gbs=6650.0, source="fallback (B200_PROFILING.md: 1.4 PFLOP/s sustained, 6.65 TB/s)")
+    return dict(tflops=989.0, gbs=3350.0,
+                source="NVIDIA H100 SXM data sheet (700 W): 989 TFLOP/s dense bf16, 3.35 TB/s HBM3; not a measured peak")
+
+
+def gpu_info(index):
+    """Card name and power limit, read in the same run as the measurement (a power-limited card clocks lower)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30).stdout
+        name, power, clk = [c.strip() for c in out.strip().split(",")]
+        return {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(clk)}
+    except Exception:  # noqa: BLE001
+        return {"name": None, "power_limit_w": None, "sm_max_mhz": None}
 
 
 class ClockSampler:
@@ -191,7 +201,31 @@ def run_reference(args, rank):
     print(json.dumps(line), flush=True)
 
 
-def run_workload(args, workload, batch, rank, local_rank, world, gatherer_cache, with_cpu=True, steps=None, warmup=None):
+def dump_outputs(out_dir, d_out, d_counts, d_glob=None, glob_counts=None):
+    """The detections a caller of the timed path receives, as float arrays: rows past each image's count are zeroed (the
+    buffer keeps stale words there), and the int32 words of dd3d_det (class, FPN level, candidate index) become float64."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    out = d_out.detach().cpu().clone()  # [images][cap][DET_WORDS] fp32 words
+    counts = d_counts.detach().cpu().to(torch.int64)
+    B, cap, _ = out.shape
+    valid = torch.arange(cap)[None, :] < counts[:, None]
+    out[~valid] = 0.0
+    int_words = [6, 7, 20, 21, 23]  # dd3d_det (include/dd3d_b200.h): cls, level, index, attr, pad
+    ints = out.view(torch.int32)[..., int_words].clone()
+    out[..., int_words] = 0.0
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "det_float_words.npy"), out.numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "det_int_words.npy"), ints[..., :4].numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "det_counts.npy"), counts.numpy().astype(np.float64))
+    if d_glob is not None:
+        g = d_glob.detach().cpu().clone()
+        g[~(torch.arange(cap)[None, :] < glob_counts.detach().cpu().to(torch.int64)[:, None])] = 0.0
+        np.save(os.path.join(out_dir, "global_boxes.npy"), g.numpy().astype(np.float32))
+
+
+def run_workload(args, workload, batch, rank, local_rank, world, gatherer_cache, with_cpu=True, dump=True):
     """Times one workload on this rank's GPU; returns the JSON line (dict).  All ranks must call it together."""
     import torch
     import torch.distributed as dist
@@ -201,8 +235,7 @@ def run_workload(args, workload, batch, rank, local_rank, world, gatherer_cache,
     from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200, group_indices
     from dd3d_b200.synthetic import make_inputs, make_nusc_inputs, make_state_dict
 
-    steps = steps or args.steps
-    warmup = warmup or args.warmup
+    steps, warmup = args.steps, args.warmup
     arch, ds, B, H, W, focal, gflop_img = WORKLOADS[workload]
     nusc = workload.startswith("nusc")
     if batch:
@@ -229,6 +262,7 @@ def run_workload(args, workload, batch, rank, local_rank, world, gatherer_cache,
         d_raw = h_raw.to(dev)
         raw_sizes = torch.tensor([[H, W]] * B, dtype=torch.int32)
         h_K_scaled = torch.empty((B, 9), dtype=torch.float32)
+    free0 = torch.cuda.mem_get_info(dev)[0]
     model._plan(*shape)
     L, handle = lib.load(), model._handle
     cap = model._desc.out_cap
@@ -261,6 +295,7 @@ def run_workload(args, workload, batch, rank, local_rank, world, gatherer_cache,
         d_flags = torch.zeros(1, dtype=torch.int32, device=dev)
 
     state = {"k": 0}
+    mem_used = free0 - torch.cuda.mem_get_info(dev)[0]  # the plan's activation buffers + the step's I/O tensors
 
     def begin_slot():
         slot = state["k"] & 1
@@ -399,6 +434,17 @@ def run_workload(args, workload, batch, rank, local_rank, world, gatherer_cache,
         return finish_timing(e0, e1, tag), clocks
 
     ms_dev, clocks = timed(step_device, "value", ClockSampler(local_rank))
+    if dump and args.dump_outputs:
+        last = (state["k"] - 1) & 1
+        if gat is not None:  # what the timed path hands back under --gpus > 1: every rank's detections, all-gathered
+            drain()
+            torch.cuda.synchronize(dev)
+            d_out, d_cnt, _ = split_gathered(recv[last], world, B, cap)
+        else:
+            d_out, d_cnt = packed[last].out, packed[last].counts
+        if rank == 0:
+            out_dir = os.path.join(args.dump_outputs, f"batch{B}") if args.sweep else args.dump_outputs
+            dump_outputs(out_dir, d_out, d_cnt, d_glob if nusc else None, packed[last].counts)
     ms_host, _ = timed(step_host, "e2e_serial")
     ms_host_serial = ms_host
     if not nusc and not raw_mode:  # double-buffered host path (H2D of the next step overlaps this step's kernels)
@@ -437,13 +483,6 @@ def run_workload(args, workload, batch, rank, local_rank, world, gatherer_cache,
     conv = acc["conv_igemm"]
     conv_tflops = conv["flops"] / (conv["ms"] * 1e-3) / 1e12 if conv["ms"] > 0 else 0.0
     step_ms = sum(v["ms"] for v in acc.values())
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, "profiles", "conv_igemm_traffic.json")
-    if os.path.exists(tpath) and args.dtype == "bf16" and not batch:
-        with open(tpath) as f:
-            tj = json.load(f)
-        traffic = tj.get(workload)
-        traffic_src = tj.get("source", "ncu dram__bytes_read.sum + dram__bytes_write.sum over the conv launches of one step")
 
     images = world * B * steps
     value = images / (ms_dev * 1e-3)
@@ -457,13 +496,15 @@ def run_workload(args, workload, batch, rank, local_rank, world, gatherer_cache,
                         f"(padded to /{model.backbone.size_divisibility})" +
                         (f", raw HWC input resized on the GPU to {shape[1]}x{shape[2]}" if raw_mode else ""),
             "global_batch": world * B, "parallelism": f"dp{world}",
-            "l2": "inputs (%.0f MB uint8) and activations (GBs) exceed the 126 MB L2; no explicit flush" %
+            "l2": "inputs (%.0f MB uint8) and activations (GBs) exceed the 50 MB L2; no explicit flush" %
                   (batch_t.numel() / 1e6),
+            "device_memory_used_gb": round(mem_used / 1e9, 2),
             "collective": ("1 ncclAllGather per step of the packed [dets | counts | flags] buffer (%d B per rank) through "
                            "dd3d_allgather, on a side stream (overlaps the next forward; no host sync in the timed region)"
                            % packed[0].nbytes) if world > 1 else "none",
             "detections_per_step": n_det,
         },
+        "gpu": gpu_info(local_rank),
         "clocks": clocks,
         "e2e": {"value": e2e, "unit": "images/s", "ms_per_step": ms_host / steps,
                 "path": "dd3d_submit_host / dd3d_wait_host (double-buffered: H2D of step k+1 overlaps the kernels of step "
@@ -474,10 +515,9 @@ def run_workload(args, workload, batch, rank, local_rank, world, gatherer_cache,
                 "d2h_bytes_per_step": int(h_out[0].numel() * 4 + h_cnt[0].numel() * 4 + (h_glob.numel() * 4 if nusc else 0))},
         "gpu_launches": (model.launches_per_forward() + (2 if nusc else 0)) * steps,
         "roofline": {
-            "kernel": "conv_igemm_kernel (tcgen05 implicit GEMM, %d launches/step)" % conv["launches"],
+            "kernel": "conv_igemm_kernel (wgmma implicit GEMM, %d launches/step)" % conv["launches"],
             "bound": "tensor", "achieved": conv_tflops, "peak": peaks["tflops"], "unit": "TFLOP/s",
-            "frac": conv_tflops / peaks["tflops"], "traffic": traffic,
-            "traffic_source": ("static: " + traffic_src) if traffic is not None else "not captured for this configuration",
+            "frac": conv_tflops / peaks["tflops"],
             "peak_source": peaks["source"],
             "algorithmic_flops_per_step": conv["flops"], "kernel_ms_per_step": conv["ms"],
             "share_of_step": conv["ms"] / step_ms if step_ms else None,
@@ -516,6 +556,8 @@ def main():
     ap.add_argument("--sweep", default="", help="comma list of per-GPU batch sizes: one JSON line per size (configs[4])")
     ap.add_argument("--cpu-images", type=int, default=2, help="0 disables the cpu_baseline leg")
     ap.add_argument("--no-secondary", action="store_true", help="skip the DLA-34 (configs[1]) leg of the default run")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32 / float64, < 64 MB in all)")
     ap.add_argument("--input", default="mapped", choices=["mapped", "raw"],
                     help="raw: steps start from raw HWC uint8 dataset images (dd3d_forward_raw: ResizeShortestEdge to "
                          "INPUT.RESIZE.MIN_SIZE_TEST + intrinsics rescale on the GPU); not the BASELINE configuration")
@@ -547,8 +589,7 @@ def main():
         if default_run and world == 1 and not args.no_secondary:
             # BASELINE.json configs[1] (DLA-34 bf16, batch 8, 384x1280) measured in the same process, so that the driver's
             # single `bench.py` run records it too
-            sec = run_workload(args, "dla34", 0, rank, local_rank, world, gatherers, with_cpu=False, steps=max(args.steps, 20),
-                               warmup=max(args.warmup, 5))
+            sec = run_workload(args, "dla34", 0, rank, local_rank, world, gatherers, with_cpu=False, dump=False)
             line["secondary"] = {k: sec[k] for k in ("metric", "value", "unit", "ms_per_step", "steps", "dtype", "config",
                                                       "clocks", "e2e", "gpu_launches", "roofline", "kernels_ms_per_step")}
         if rank == 0:

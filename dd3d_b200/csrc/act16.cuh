@@ -1,6 +1,6 @@
 // 16-bit activation / weight storage of the engine: bf16 (default) or fp16 (dd3d_model_desc.act_dtype, the reference's
 // mixed-precision path is fp16 autocast, scripts/train.py:121).  Layouts and kernels are identical; only the conversion
-// instructions, the UMMA instruction descriptor and the TMA element type differ, selected by a warp-uniform flag.
+// instructions, the wgmma operand type and the TMA element type differ, selected by a template flag or a warp-uniform flag.
 // Buffers are typed __nv_bfloat16* throughout as "opaque 16-bit elements".
 #pragma once
 #include <cuda_bf16.h>

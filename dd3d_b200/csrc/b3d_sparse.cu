@@ -2,7 +2,7 @@
 // 102-135 `box3d_quat/ctr/depth/size/conf`, applied in forward fcos3d.py:160-188, per-level Scale / Offset folded into the
 // epilogue) evaluated ONLY at the pixels that survived the 2-D threshold + per-level top-k (fcos2d.py:280-310) -- the 3-D
 // outputs of every other pixel are never read by the reference's inference either (fcos3d.py:328-399 indexes them with the
-// 2-D candidates).  Dense, the layer is 0.53 TFLOP and 1.75 ms of a V2-99 step (32 x 127 875 pixels x 2304 x 110); the
+// 2-D candidates).  Dense, the layer is 0.53 TFLOP of a V2-99 step (32 x 127 875 pixels x 2304 x 110); the
 // bench batch keeps ~1 100 candidates per image: 115 x fewer rows.
 //
 // Gathered GEMM: row = one final candidate (image b, level l, slot) of decode.cu's `fin` list, K = 9 taps x 256 channels read

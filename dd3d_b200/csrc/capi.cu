@@ -41,7 +41,7 @@ int cuda_status(cudaError_t e, std::string* err) {
 }
 
 int device_sms() {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     return sms;
 }
@@ -117,10 +117,6 @@ int dd3d_forward_host(dd3d_handle h, const void* h_images, int img_dtype, const 
 
 int dd3d_set_conv_policy(const char* name, int value) {
     if (!name) return DD3D_ERR_INVALID;
-    if (!strcmp(name, "cta2")) {
-        conv_set_cta2(value);
-        return DD3D_OK;
-    }
     if (!strcmp(name, "nms_class_parallel")) {
         nms_set_class_parallel(value);
         return DD3D_OK;
@@ -346,7 +342,6 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
     g.W = Wo;
     choose_tile(Ho, Wo, &g.th, &g.tw);
     bool ok = true;
-    p.cta2 = conv_use_cta2();
     p.halo = conv_prefer_halo(taps, stride, block_n, 1, &Ho, &Wo) ? conv_halo_mode() : 0;
     if (p.halo) {
         g.th = kHaloTh;
@@ -391,7 +386,7 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
             cudaFree(d_w_taps);
             return DD3D_ERR_CUDA;
         }
-    } else if (!make_weight_map(&p.w_map, d_w, taps * kchunks * kBlockK, cout_pad, p.cta2 ? block_n / 2 : block_n, g_op_fp16)) {
+    } else if (!make_weight_map(&p.w_map, d_w, taps * kchunks * kBlockK, cout_pad, block_n, g_op_fp16)) {
         fprintf(stderr, "dd3d_op_conv2d: %s\n", conv_last_error());
         return DD3D_ERR_CUDA;
     }

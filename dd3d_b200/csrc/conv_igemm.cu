@@ -1,815 +1,47 @@
-// Implicit-GEMM convolution on tcgen05 tensor cores (sm_100a).
-//
-// Replaces every cuDNN conv + FrozenBN/BN + ReLU (+residual, +FPN upsample-add) launch of the reference's
-// DD3D.forward (SURVEY.md 2.1 K1/K2/K3/K6; reference call sites dla.py:27-46,149-157,229-231, vovnet.py:129-157,
-// detectron2 FPN, fcos2d.py:81-98, fcos3d.py:90-126).
-//
-// GEMM view:  D[m][n] = sum_k A[m][k] * W[n][k]
-//   m : 128 output pixels of one th x tw patch of one image          (UMMA M = 128, one TMEM lane per pixel)
-//   n : output channels, block_n <= 256 per tile                       (UMMA N)
-//   k : taps x input channels, 64 channels (128 B) per k-block         (UMMA K = 16, 4 MMAs per k-block)
-// A is never materialised: for tap (r,s) the k-block is ONE tiled TMA box [1][th][tw][64ch] of the NHWC bf16
-// input at spatial offset (r-1, s-1); TMA zero-fills out-of-image pixels (= conv zero padding) and channels
-// beyond C (ragged C such as 160/224).  Stride-2 convs read a parity-split 5-D view of the same tensor.
-// Concats are free: producers TMA-store into channel slices of one wide NHWC buffer, the 1x1 reads it whole.
-//
-// Halo variant (3x3, stride 1): the A operand of a 64-channel block is ONE box [18][10][64ch] (tile + halo); the nine
-// taps are descriptor views of it shifted by whole 128-byte pixel rows, so A is fetched once instead of nine times.
-//
-// Warp roles (352 threads, 1 CTA/SM, persistent over tiles); every role loop is warp-converged and only the issue
-// instructions are predicated on elect.sync, which keeps TMA / UMMA operands in uniform registers:
-//   warp 0 : TMA producer of the activation tiles (generic) / of the weight tiles (halo)
-//   warp 2 : TMA producer of the weight tiles (generic) / of the halo patches (halo)
-//   warp 1 : tcgen05.mma issuer (accumulators double-buffered in TMEM: 2 x block_n columns)
-//   warps 3..10 : epilogue, TWO warps per TMEM lane quarter (a warp reads lanes 32 * (warp % 4) ..): the pair splits every
-//                64-column chunk into its two 32-column steps (tcgen05.ld -> scale/bias/residual/ReLU -> bf16/fp16 ->
-//                swizzled smem -> TMA store, optional eSE pooling partial sums; or fp32 direct stores for the predictor
-//                heads).  With one epilogue warp per scheduler every dependent instruction paid its full latency and the
-//                small-K layers (stem, OSA2, 1x1 concats / laterals) were epilogue-bound (profiles/r02_epilogue.md).
-// Launched with programmatic dependent launch: the prologue overlaps the previous kernel's tail.
-#include "conv_igemm.cuh"
-
-#include <math.h>
+// Implicit-GEMM convolution: host side (tensor maps, tiling policy, launch) and the taps-in-N kernel.  The main kernel and its
+// design notes are in conv_igemm_kernel.cuh.
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
 #include <string>
 
-#include "act16.cuh"
+#include "conv_igemm_kernel.cuh"
 #include "device_once.cuh"
-#include "ptx.cuh"
 
 namespace dd3d {
 
 namespace {
 
-constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KiB
-constexpr int kStagingBytes = kBlockM * 128;    // one 64-channel bf16 output chunk
-constexpr int kMaxStages = 8;
-constexpr int kSmemBudget = 227 * 1024;
-// halo variant: per 64-channel block the A operand is ONE (16+2)x(8+2)-pixel patch = 180 rows of 128 B (64 channels),
-// 128B-swizzled by TMA; the slot is rounded up to a multiple of 1024 B so every patch keeps the swizzle-atom alignment
-constexpr int kHaloPW = kHaloTw + 2, kHaloPH = kHaloTh + 2;
-constexpr int kHaloABytes = (kHaloPW * kHaloPH * 128 + 1023) / 1024 * 1024;  // 23552
-constexpr int kHaloAStages = 3;   // default number of A patches in flight
-constexpr int kMaxAStages = 5;    // weight-stationary layers (ConvParams::wstat) spend the freed B ring on deeper A prefetch
-constexpr int kBarBytes = 512;
-constexpr int kSbBytes = 2 * 256 * 4;  // staged (scale, bias) vectors of the current (segment, n-block)
-constexpr int kFirstEpiWarp = 3, kEpiWarps = 8, kEpiThreads = kEpiWarps * 32;
-
-struct TileCoord {
-    int seg, img, y0, x0, n_blk;
-    bool valid;  // false: the padding tile of an odd CTA pair (coordinates beyond the batch: loads zero-fill, stores skip)
-};
-
-// x / d for 0 <= x < 2^24 without the ~40-instruction integer division: fp32 reciprocal estimate, corrected by one.
-// (every warp decodes every tile; the divisions were 10 % of the epilogue warps' samples, profiles/r01d_cta2_ab.md)
-__device__ __forceinline__ int fast_div(int x, int d, float inv_d) {
-    int q = __float2int_rz(__int2float_rz(x) * inv_d);
-    const int r = x - q * d;
-    q += (r >= d) ? 1 : 0;
-    q -= (r < 0) ? 1 : 0;
-    return q;
-}
-
-// CTA pair (CTA2): work item = (pair of consecutive M-tiles, n-block); CTA `rank` of the pair owns tile 2 * pair + rank.
-template <bool CTA2>
-__device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int work, int rank) {
-    TileCoord t;
-    int mt = work;
-    t.n_blk = 0;
-    if (p.n_blocks > 1) {
-        mt = fast_div(work, p.n_blocks, p.inv_n_blocks);
-        t.n_blk = work - mt * p.n_blocks;
-    }
-    if (CTA2) mt = 2 * mt + rank;
-    t.valid = mt < p.total_tiles;
-    int s = 0;
-#pragma unroll
-    for (int i = 1; i < kMaxSeg; ++i) {
-        if (i < p.nseg && mt >= p.seg[i].tile_begin) s = i;
-    }
-    t.seg = s;
-    const ConvSeg& g = p.seg[s];
-    int local = mt - g.tile_begin;
-    int per_img = g.tiles_x * g.tiles_y;
-    t.img = fast_div(local, per_img, g.inv_per_img);
-    int r = local - t.img * per_img;
-    int ty = fast_div(r, g.tiles_x, g.inv_tiles_x);
-    int tx = r - ty * g.tiles_x;
-    t.y0 = ty * g.th;
-    t.x0 = tx * g.tw;
-    return t;
-}
-
-// (a, b) -> packed 16-bit pair; MODE bit 0: ReLU fused into the conversion (cvt.rn.relu), bit 1: fp16 instead of bf16.
-template <int MODE>
-__device__ __forceinline__ uint32_t pack2_mode(float a, float b) {
-    uint32_t r;
-    if (MODE == 0) {
-        asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
-    } else if (MODE == 1) {
-        asm("cvt.rn.relu.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
-    } else if (MODE == 2) {
-        asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
-    } else {
-        asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
-    }
-    return r;
-}
-
-// One full 32-column epilogue step of the 16-bit output path: v = this thread's accumulator row (32 fp32 columns, already
-// loaded from TMEM), y = v * scale + bias (+ residual) -> (ReLU) -> bf16 / fp16 -> the thread's row of the 128B-swizzled
-// staging tile.  (scale, bias) come from shared memory as broadcast LDS.128; two sub-steps of 16 columns keep the live
-// register set small (168-register cap with 11 warps).  MODE as in pack2_mode; HAS_RES: rpre holds the 32 residual values.
-template <int MODE, bool HAS_RES>
-__device__ __forceinline__ void epi_fast_step(uint32_t (&v)[32], uint32_t ssc, uint32_t sbi, const uint4 (&rpre)[4],
-                                              uint32_t stag_row, int c16_0, int row7) {
-    float4 sc[4], bi[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        sc[i] = ptx::ld_shared_f4(ssc + 16 * i);
-        bi[i] = ptx::ld_shared_f4(sbi + 16 * i);
-    }
-    ptx::tmem_ld_wait(v);  // the LDS above are in flight together with the TMEM load
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-        float y[16];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            y[4 * i + 0] = fmaf(__uint_as_float(v[16 * hh + 4 * i + 0]), sc[i].x, bi[i].x);
-            y[4 * i + 1] = fmaf(__uint_as_float(v[16 * hh + 4 * i + 1]), sc[i].y, bi[i].y);
-            y[4 * i + 2] = fmaf(__uint_as_float(v[16 * hh + 4 * i + 2]), sc[i].z, bi[i].z);
-            y[4 * i + 3] = fmaf(__uint_as_float(v[16 * hh + 4 * i + 3]), sc[i].w, bi[i].w);
-        }
-        if (hh == 0) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                sc[i] = ptx::ld_shared_f4(ssc + 64 + 16 * i);
-                bi[i] = ptx::ld_shared_f4(sbi + 64 + 16 * i);
-            }
-        }
-        if (HAS_RES) {
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const uint32_t* rb = reinterpret_cast<const uint32_t*>(&rpre[2 * hh + i]);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const float2 f = (MODE & 2) ? unpack2_f16(rb[j]) : unpack2_bf16(rb[j]);
-                    y[8 * i + 2 * j] += f.x;
-                    y[8 * i + 2 * j + 1] += f.y;
-                }
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            uint4 o;
-            o.x = pack2_mode<MODE>(y[8 * i + 0], y[8 * i + 1]);
-            o.y = pack2_mode<MODE>(y[8 * i + 2], y[8 * i + 3]);
-            o.z = pack2_mode<MODE>(y[8 * i + 4], y[8 * i + 5]);
-            o.w = pack2_mode<MODE>(y[8 * i + 6], y[8 * i + 7]);
-            const int c16 = c16_0 + 2 * hh + i;  // 16-byte chunk within the 128-byte row
-            ptx::st_shared_v4(stag_row + ((c16 ^ row7) << 4), o);
-        }
-    }
-}
-
-// elect.sync: exactly one lane of the (converged) warp gets true.  Keeping the role loops warp-converged and
-// predicating only the issue instructions on the elected lane lets the compiler keep TMA / UMMA operands in
-// uniform registers; a `lane == 0` branch instead forces an R2UR + election loop around every UTMALDG / UTCHMMA
-// (measured: ~220 ns per TMA box and ~245 ns per MMA from a single divergent thread).
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-        "elect.sync rx|px, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, px;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-
-template <bool HALO, bool CTA2>
-__global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    // 128B-swizzled tiles need 1024-byte alignment
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    // generic: num_stages x [A 16 KiB | B block_n*128].  halo: num_stages x [B block_n*128], then 3 x [A patch 23 KiB]
-    // CTA pair: one tcgen05.mma.cta_group::2 (M = 256) covers the two CTAs' pixel tiles; each CTA stages its own A tile
-    // and HALF of the weight tile (b_rows rows), which halves the shared-memory traffic per MMA -- the limiter of the
-    // single-CTA kernel (operand reads + TMA writes exceed 128 B/clk for N <= 256, DESIGN.md 3).
-    const int rank = CTA2 ? static_cast<int>(ptx::cluster_ctarank()) : 0;
-    const bool leader = rank == 0;
-    const int w_first = CTA2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-    const int w_step = CTA2 ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-    const int w_total = CTA2 ? p.pair_work : p.total_work;
-    const int b_rows = CTA2 ? p.block_n / 2 : p.block_n;
-    const int stage_bytes = (HALO ? 0 : kABytes) + b_rows * 128;
-    // weight-stationary (HALO, single CTA, one n-block, cin <= 64): ALL k-blocks of the weight tensor stay resident in the B
-    // region (loaded once per CTA) instead of cycling through the stage ring for every tile
-    const bool wstat = HALO && !CTA2 && p.wstat != 0;
-    const int a_stages = HALO ? p.a_stages : 0;
-    uint8_t* halo_a = smem + (wstat ? p.taps * p.kchunks : p.num_stages) * stage_bytes;
-    uint8_t* staging = halo_a + a_stages * kHaloABytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 2 * kStagingBytes);
-    uint64_t* full_bar = bars;                     // [kMaxStages]
-    uint64_t* empty_bar = bars + kMaxStages;       // [kMaxStages]
-    uint64_t* tfull_bar = bars + 2 * kMaxStages;   // [2]
-    uint64_t* tempty_bar = tfull_bar + 2;          // [2]
-    uint64_t* afull_bar = tempty_bar + 2;          // [kMaxAStages]
-    uint64_t* aempty_bar = afull_bar + kMaxAStages;
-    uint64_t* wfull_bar = aempty_bar + kMaxAStages;  // [1] resident weights landed (wstat)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull_bar + 1);
-    // shared-window addresses of the epilogue's staging tiles and of the staged folded-BN vectors (explicit LDS / STS)
-    const uint32_t staging_u32 = ptx::smem_u32(staging);
-    const uint32_t s_scale_u32 = ptx::smem_u32(reinterpret_cast<uint8_t*>(bars) + kBarBytes);  // [256] fp32 scale
-    const uint32_t s_bias_u32 = s_scale_u32 + 256 * 4;                                          // [256] fp32 bias
-
-    const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);  // provably warp-uniform
-    const int lane = threadIdx.x & 31;
-
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&p.w_map);
-        for (int s = 0; s < p.nseg; ++s) {
-            ptx::prefetch_tensormap(&p.seg[s].in_map[0]);
-            if (p.out_mode == 0) ptx::prefetch_tensormap(&p.seg[s].out_map);
-        }
-        for (int i = 0; i < p.num_stages; ++i) {
-            ptx::mbar_init(&full_bar[i], HALO ? 1 : 2);  // generic: A (warp 0) + B (warp 2) each arrive.expect_tx
-            ptx::mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            ptx::mbar_init(&tfull_bar[i], 1);
-            ptx::mbar_init(&tempty_bar[i], (CTA2 ? 2 : 1) * kEpiWarps);  // one arrival per epilogue warp (of both CTAs of a pair)
-        }
-        for (int i = 0; i < kMaxAStages; ++i) {
-            ptx::mbar_init(&afull_bar[i], 1);
-            ptx::mbar_init(&aempty_bar[i], 1);
-        }
-        ptx::mbar_init(wfull_bar, 1);
-        ptx::fence_barrier_init();
-    }
-    if (warp == 1) {
-        if (CTA2) {
-            ptx::tmem_alloc2(tmem_slot, p.tmem_cols);
-            ptx::tmem_relinquish2();
-        } else {
-            ptx::tmem_alloc(tmem_slot, p.tmem_cols);
-            ptx::tmem_relinquish();
-        }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (CTA2) ptx::cluster_sync();  // the peer's barriers and TMEM must exist before anything targets them
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // the leader's barriers as seen from either CTA of the pair (shared::cluster addresses; 8 bytes per barrier)
-    const uint32_t full0 = CTA2 ? ptx::mapa(&full_bar[0], 0) : 0;
-    const uint32_t afull0 = CTA2 ? ptx::mapa(&afull_bar[0], 0) : 0;
-    const uint32_t tempty0 = CTA2 ? ptx::mapa(&tempty_bar[0], 0) : 0;
-    // Programmatic dependent launch: everything above (barrier init, TMEM alloc, descriptor prefetch) overlapped the
-    // tail of the previous kernel in the stream; from here on we touch its outputs, so wait for it, and let the next
-    // kernel start its own prologue as our CTAs retire.
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-
-    const int kblocks = p.taps * p.kchunks;
-
-    if (warp == 0) {
-        // ---------------------------------------------------------------- warp 0: activation (A) producer in the
-        // generic variant, weight (B) producer in the halo variant.  Whole warp runs the loop; one elected lane issues.
-        int stage = 0;
-        uint32_t phase = 0;
-        if (wstat) {
-            // the whole weight tensor (<= 9 x 8 KiB), once: one barrier, one transaction count
-            if (elect_one()) {
-                ptx::mbar_expect_tx(wfull_bar, kblocks * p.block_n * 128);
-                for (int kb = 0; kb < kblocks; ++kb)
-                    ptx::tma_load_2d(smem + kb * stage_bytes, &p.w_map, wfull_bar, kb * kBlockK, 0);
-            }
-            __syncwarp();
-        }
-        for (int work = w_first; work < w_total && !wstat; work += w_step) {
-            const TileCoord t = decode_tile<CTA2>(p, work, rank);
-            const ConvSeg& g = p.seg[t.seg];
-            if (HALO) {
-                for (int kc = 0; kc < p.kchunks; ++kc) {
-                    for (int tap = 0; tap < 9; ++tap) {
-                        ptx::mbar_wait(&empty_bar[stage], phase ^ 1, 1);
-                        if (elect_one()) {
-                            if (CTA2) {  // the leader arms the barrier for both halves of the weight tile
-                                if (leader) ptx::mbar_expect_tx(&full_bar[stage], p.block_n * 128);
-                                ptx::tma2_load_2d(smem + stage * stage_bytes, &p.w_map, full0 + stage * 8,
-                                                  (tap * p.kchunks + kc) * kBlockK, t.n_blk * p.block_n + rank * b_rows);
-                            } else {
-                                ptx::mbar_expect_tx(&full_bar[stage], p.block_n * 128);
-                                ptx::tma_load_2d(smem + stage * stage_bytes, &p.w_map, &full_bar[stage],
-                                                 (tap * p.kchunks + kc) * kBlockK, t.n_blk * p.block_n);
-                            }
-                        }
-                        __syncwarp();
-                        if (++stage == p.num_stages) {
-                            stage = 0;
-                            phase ^= 1;
-                        }
-                    }
-                }
-                continue;
-            }
-            for (int tap = 0; tap < p.taps; ++tap) {
-                const int r = (p.taps == 9) ? tap / 3 : 1;
-                const int s = (p.taps == 9) ? tap - 3 * (tap / 3) : 1;
-                for (int kc = 0; kc < p.kchunks; ++kc) {
-                    ptx::mbar_wait(&empty_bar[stage], phase ^ 1, 1);
-                    if (elect_one()) {
-                        uint8_t* a_dst = smem + stage * stage_bytes;
-                        // the weight tile is armed + issued by warp 2; in a CTA pair the leader arms for both CTAs
-                        if (!CTA2 || leader) ptx::mbar_expect_tx(&full_bar[stage], CTA2 ? 2 * kABytes : kABytes);
-                        // stride 2: input (2*oy + r - 1, 2*ox + s - 1) in the parity-split view [B][H/2][2][W/2][wp*C..]
-                        const int wp = (s == 1) ? 0 : 1;
-                        const int dw = (s == 0) ? -1 : 0;
-                        const int hp = (r == 1) ? 0 : 1;
-                        const int dh = (r == 0) ? -1 : 0;
-                        if (CTA2) {
-                            if (p.stride == 1) {
-                                ptx::tma2_load_4d(a_dst, &g.in_map[0], full0 + stage * 8, kc * kBlockK, t.x0 + s - 1,
-                                                  t.y0 + r - 1, t.img);
-                            } else {
-                                ptx::tma2_load_5d(a_dst, &g.in_map[wp], full0 + stage * 8, kc * kBlockK, t.x0 + dw, hp,
-                                                  t.y0 + dh, t.img);
-                            }
-                        } else if (p.stride == 1) {
-                            ptx::tma_load_4d(a_dst, &g.in_map[0], &full_bar[stage], kc * kBlockK, t.x0 + s - 1,
-                                             t.y0 + r - 1, t.img);
-                        } else {
-                            ptx::tma_load_5d(a_dst, &g.in_map[wp], &full_bar[stage], kc * kBlockK, t.x0 + dw, hp,
-                                             t.y0 + dh, t.img);
-                        }
-                    }
-                    __syncwarp();
-                    if (++stage == p.num_stages) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-            }
-        }
-    } else if (warp == 2) {
-        if (!HALO) {
-            // ------------------------------------------------------------ warp 2: weight-tile (B) producer (generic)
-            int stage = 0;
-            uint32_t phase = 0;
-            const uint32_t b_bytes = p.block_n * 128;
-            for (int work = w_first; work < w_total; work += w_step) {
-                const int n0 = (work % p.n_blocks) * p.block_n;
-                for (int kb = 0; kb < kblocks; ++kb) {
-                    ptx::mbar_wait(&empty_bar[stage], phase ^ 1, 7);
-                    if (elect_one()) {
-                        if (CTA2) {
-                            if (leader) ptx::mbar_expect_tx(&full_bar[stage], b_bytes);  // both halves
-                            ptx::tma2_load_2d(smem + stage * stage_bytes + kABytes, &p.w_map, full0 + stage * 8,
-                                              kb * kBlockK, n0 + rank * b_rows);
-                        } else {
-                            ptx::mbar_expect_tx(&full_bar[stage], b_bytes);
-                            ptx::tma_load_2d(smem + stage * stage_bytes + kABytes, &p.w_map, &full_bar[stage],
-                                             kb * kBlockK, n0);
-                        }
-                    }
-                    __syncwarp();
-                    if (++stage == p.num_stages) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-            }
-        } else {
-            // ------------------------------------------------------------ warp 2: halo A-patch producer: one box
-            // [18][10][64 ch] (180 rows of 128 B, 128B-swizzled, zero-filled outside the image) per 64-channel block
-            int as = 0;
-            uint32_t aphase = 0;
-            for (int work = w_first; work < w_total; work += w_step) {
-                const TileCoord t = decode_tile<CTA2>(p, work, rank);
-                const ConvSeg& g = p.seg[t.seg];
-                for (int kc = 0; kc < p.kchunks; ++kc) {
-                    ptx::mbar_wait(&aempty_bar[as], aphase ^ 1, 5);
-                    if (elect_one()) {
-                        if (CTA2) {
-                            if (leader) ptx::mbar_expect_tx(&afull_bar[as], 2 * kHaloPW * kHaloPH * 128);
-                            ptx::tma2_load_4d(halo_a + as * kHaloABytes, &g.in_map[0], afull0 + as * 8, kc * kBlockK,
-                                              t.x0 - 1, t.y0 - 1, t.img);
-                        } else {
-                            ptx::mbar_expect_tx(&afull_bar[as], kHaloPW * kHaloPH * 128);
-                            ptx::tma_load_4d(halo_a + as * kHaloABytes, &g.in_map[0], &afull_bar[as], kc * kBlockK,
-                                             t.x0 - 1, t.y0 - 1, t.img);
-                        }
-                    }
-                    __syncwarp();
-                    if (++as == a_stages) {
-                        as = 0;
-                        aphase ^= 1;
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-      if (!CTA2 || leader) {  // CTA pair: only the leader issues; its MMAs read both CTAs' smem and write both TMEMs
-        // -------------------------------------------------------------------- warp 1: tcgen05.mma issuer
-        // Descriptor high word is constant; the low word is (addr >> 4) | LBO, advanced by 2 (= 32 bytes) per K=16 step.
-        const uint32_t idesc = ptx::make_idesc_f16(CTA2 ? 2 * kBlockM : kBlockM, p.block_n, p.fp16);
-        constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);                   // SBO 1024, v1, SW128
-        constexpr uint32_t kHaloDescHi = ((kHaloPW * 128u) >> 4) | (1u << 14) | (2u << 29);     // SBO = 10 pixels
-        const uint32_t lo0 = (ptx::smem_u32(smem) >> 4) | (1u << 16);
-        const uint32_t halo_lo0 = (ptx::smem_u32(halo_a) >> 4) | (1u << 16);
-        const uint32_t stage_units = static_cast<uint32_t>(stage_bytes) >> 4;
-        int stage = 0;
-        uint32_t phase = 0;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        int as = 0;
-        uint32_t aphase = 0;
-        if (wstat) {
-            ptx::mbar_wait(wfull_bar, 0, 4);
-            ptx::tc_fence_after();
-        }
-        for (int work = w_first; work < w_total; work += w_step) {
-            ptx::mbar_wait(&tempty_bar[acc], acc_phase ^ 1, 2);
-            ptx::tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * p.block_n;
-            if (HALO) {
-                for (int kc = 0; kc < p.kchunks; ++kc) {
-                    ptx::mbar_wait(&afull_bar[as], aphase, 6);
-                    const uint32_t a_lo = halo_lo0 + static_cast<uint32_t>(as) * (kHaloABytes >> 4);
-                    for (int tap = 0; tap < 9; ++tap) {
-                        if (!wstat) ptx::mbar_wait(&full_bar[stage], phase, 3);
-                        ptx::tc_fence_after();
-                        const int r = tap / 3, s = tap - 3 * r;
-                        const uint32_t a_tap = a_lo + (r * kHaloPW + s) * 8;  // whole pixels: 128 B = 8 x 16 B
-                        const uint32_t b_lo = lo0 + static_cast<uint32_t>(wstat ? tap * p.kchunks + kc : stage) * stage_units;
-                        const int ksteps = (kc == p.kchunks - 1) ? p.last_ksteps : kBlockK / 16;
-                        if (elect_one()) {
-#pragma unroll
-                            for (int k = 0; k < kBlockK / 16; ++k) {
-                                if (k < ksteps) {  // channels beyond cin are zero padding: skip their K steps
-                                    const uint64_t adesc = (static_cast<uint64_t>(kHaloDescHi) << 32) | (a_tap + 2 * k);
-                                    const uint64_t bdesc = (static_cast<uint64_t>(kDescHi) << 32) | (b_lo + 2 * k);
-                                    if (CTA2) {
-                                        ptx::umma2_bf16(d_tmem, adesc, bdesc, idesc, (kc | tap | k) != 0 ? 1u : 0u);
-                                    } else {
-                                        ptx::umma_bf16(d_tmem, adesc, bdesc, idesc, (kc | tap | k) != 0 ? 1u : 0u);
-                                    }
-                                }
-                            }
-                            if (CTA2) {
-                                ptx::umma_commit2(&empty_bar[stage], 3);
-                                if (tap == 8) ptx::umma_commit2(&aempty_bar[as], 3);
-                            } else {
-                                if (!wstat) ptx::umma_commit(&empty_bar[stage]);
-                                if (tap == 8) ptx::umma_commit(&aempty_bar[as]);  // patch free once its 36 MMAs retire
-                            }
-                        }
-                        __syncwarp();
-                        if (!wstat && ++stage == p.num_stages) {
-                            stage = 0;
-                            phase ^= 1;
-                        }
-                    }
-                    if (++as == a_stages) {
-                        as = 0;
-                        aphase ^= 1;
-                    }
-                }
-            } else {
-                int kc_gen = 0;  // channel block of k-block kb (k-blocks run tap-major: kb = tap * kchunks + kc)
-                for (int kb = 0; kb < kblocks; ++kb) {
-                    ptx::mbar_wait(&full_bar[stage], phase, 3);
-                    ptx::tc_fence_after();
-                    const uint32_t a_lo = lo0 + static_cast<uint32_t>(stage) * stage_units;
-                    const uint32_t b_lo = a_lo + (kABytes >> 4);
-                    if (++kc_gen == p.kchunks) kc_gen = 0;
-                    const int ksteps = (kc_gen == 0) ? p.last_ksteps : kBlockK / 16;  // kc_gen == 0: this was the last block
-                    if (elect_one()) {
-#pragma unroll
-                        for (int k = 0; k < kBlockK / 16; ++k) {
-                            if (k < ksteps) {  // channels beyond cin are zero padding: skip their K steps
-                                const uint64_t adesc = (static_cast<uint64_t>(kDescHi) << 32) | (a_lo + 2 * k);
-                                const uint64_t bdesc = (static_cast<uint64_t>(kDescHi) << 32) | (b_lo + 2 * k);
-                                if (CTA2) {
-                                    ptx::umma2_bf16(d_tmem, adesc, bdesc, idesc, (kb | k) != 0 ? 1u : 0u);
-                                } else {
-                                    ptx::umma_bf16(d_tmem, adesc, bdesc, idesc, (kb | k) != 0 ? 1u : 0u);
-                                }
-                            }
-                        }
-                        // frees the smem slot (of both CTAs of a pair) once these MMAs retire
-                        if (CTA2) {
-                            ptx::umma_commit2(&empty_bar[stage], 3);
-                        } else {
-                            ptx::umma_commit(&empty_bar[stage]);
-                        }
-                    }
-                    __syncwarp();
-                    if (++stage == p.num_stages) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-            }
-            if (elect_one()) {  // accumulator complete -> epilogue (of both CTAs of a pair)
-                if (CTA2) {
-                    ptx::umma_commit2(&tfull_bar[acc], 3);
-                } else {
-                    ptx::umma_commit(&tfull_bar[acc]);
-                }
-            }
-            __syncwarp();
-            if (++acc == p.acc_stages) {
-                acc = 0;
-                acc_phase ^= 1;
-            }
-        }
-      }
-    } else if (warp >= kFirstEpiWarp) {
-        // ---------------------------------------------------------------- epilogue (warps 3..10)
-        const int q = warp & 3;                       // TMEM lane quarter this warp may access (hardware: warp id % 4)
-        const int half = (warp - kFirstEpiWarp) >> 2;  // which 32-column step of every 64-column chunk this warp owns
-        const int row = q * 32 + lane;
-        const int et = static_cast<int>(threadIdx.x) - kFirstEpiWarp * 32;  // 0 .. kEpiThreads - 1
-        const bool store_leader = (et == 0);
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        int sbuf = 0;
-        int sb_key = -1;  // (segment, n-block) whose folded-BN vectors are staged in s_scale / s_bias
-        for (int work = w_first; work < w_total; work += w_step) {
-            const TileCoord t = decode_tile<CTA2>(p, work, rank);
-            const ConvSeg& g = p.seg[t.seg];
-            const int ly = row / g.tw;
-            const int lx = row - ly * g.tw;
-            const int oy = t.y0 + ly, ox = t.x0 + lx;
-            const bool in_img = t.valid && (oy < g.H) && (ox < g.W);
-            const int n_base = t.n_blk * p.block_n;
-
-            // bf16 output path: the per-channel (scale, bias) of this (segment, n-block) live in shared memory -- 16
-            // broadcast LDS.128 per 32-column step instead of 16 LDG.128 with their 64-bit address arithmetic.  All epilogue
-            // threads are past the last use of the previous vectors (the closing named barrier of the previous tile), and
-            // the opening named barrier of the first chunk below publishes the new ones.
-            if (p.out_mode == 0) {
-                const int key = t.seg * 8 + t.n_blk;
-                if (key != sb_key) {
-                    sb_key = key;
-                    if (et < p.block_n) {
-                        ptx::st_shared_f32(s_scale_u32 + et * 4, __ldg(g.scale + n_base + et));
-                        ptx::st_shared_f32(s_bias_u32 + et * 4, __ldg(g.bias + n_base + et));
-                    }
-                }
-            }
-
-            const __nv_bfloat16* res_ptr = nullptr;
-            if (g.residual != nullptr && in_img) {
-                const int ry = g.res_up2 ? (oy >> 1) : oy;
-                const int rx = g.res_up2 ? (ox >> 1) : ox;
-                res_ptr = g.residual + (static_cast<size_t>(t.img * g.res_H + ry) * g.res_W + rx) * g.res_pitch + n_base;
-            }
-            float* f32_ptr = nullptr;
-            if (p.out_mode == 1 && in_img) {
-                f32_ptr = g.out_f32 + (static_cast<size_t>(t.img * g.H + oy) * g.W + ox) * g.out_pitch + n_base;
-            }
-            // residual (BasicBlock identity / FPN top-down map) of this warp's FIRST step, fetched before the accumulator
-            // wait; every later step's columns are fetched one step ahead (L2 / DRAM latency paid once per tile)
-            // NOTE: every branch that contains a warp-collective instruction (tcgen05.ld / tcgen05.wait::ld are .sync.aligned)
-            // must be WARP-UNIFORM.  `res_ptr` is per thread (null for pixels outside a ragged map), so the code below
-            // branches on `has_res` (per segment) and lets the out-of-image threads carry zeros.
-            const bool has_res = g.residual != nullptr;
-            uint4 rpre[4];
-            auto load_res = [&](int col) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    rpre[i] = (res_ptr != nullptr && col + 8 * i < p.block_n)
-                                  ? __ldg(reinterpret_cast<const uint4*>(res_ptr + col + 8 * i))
-                                  : make_uint4(0u, 0u, 0u, 0u);
-                }
-            };
-            if (has_res && half * 32 < p.block_n) load_res(half * 32);
-
-            ptx::mbar_wait(&tfull_bar[acc], acc_phase, 4);
-            ptx::tc_fence_after();
-            const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * p.block_n;
-
-            for (int c0 = 0; c0 < p.block_n; c0 += 64) {
-                const int chunk_cols = min(64, p.block_n - c0);
-                uint8_t* stag = staging + sbuf * kStagingBytes;
-                const uint32_t stag_u32 = staging_u32 + sbuf * kStagingBytes;
-                if (p.out_mode == 0) {
-                    // the TMA store that last read this staging buffer must have drained
-                    if (store_leader) ptx::tma_store_wait_read<1>();
-                    ptx::named_bar_sync(1, kEpiThreads);
-                }
-                const int h = half * 32;  // this warp's step of the chunk
-                if (h < chunk_cols) {
-                    const int cols = min(32, chunk_cols - h);
-                    const int n0 = n_base + c0 + h;  // absolute output channel of v[0]
-                    uint32_t v[32];
-                    if (cols == 32) {
-                        ptx::tmem_ld32(t_addr + c0 + h, v);
-                    } else {
-                        ptx::tmem_ld16(t_addr + c0 + h, v);
-                    }
-                    if (p.out_mode == 0 && cols == 32) {
-                        // ---- fast path: full 32-column step, bf16 / fp16 output through the staging tile
-                        const uint32_t ssc = s_scale_u32 + (c0 + h) * 4, sbi = s_bias_u32 + (c0 + h) * 4;
-                        const uint32_t stag_row = stag_u32 + row * 128;
-                        const int mode = (p.relu ? 1 : 0) | (p.fp16 ? 2 : 0);  // warp-uniform: one branch per step
-                        if (has_res) {
-                            switch (mode) {
-                                case 0: epi_fast_step<0, true>(v, ssc, sbi, rpre, stag_row, h >> 3, row & 7); break;
-                                case 1: epi_fast_step<1, true>(v, ssc, sbi, rpre, stag_row, h >> 3, row & 7); break;
-                                case 2: epi_fast_step<2, true>(v, ssc, sbi, rpre, stag_row, h >> 3, row & 7); break;
-                                default: epi_fast_step<3, true>(v, ssc, sbi, rpre, stag_row, h >> 3, row & 7); break;
-                            }
-                            if (c0 + 64 + h < p.block_n) load_res(c0 + 64 + h);  // this warp's step of the next chunk
-                        } else {
-                            switch (mode) {
-                                case 0: epi_fast_step<0, false>(v, ssc, sbi, rpre, stag_row, h >> 3, row & 7); break;
-                                case 1: epi_fast_step<1, false>(v, ssc, sbi, rpre, stag_row, h >> 3, row & 7); break;
-                                case 2: epi_fast_step<2, false>(v, ssc, sbi, rpre, stag_row, h >> 3, row & 7); break;
-                                default: epi_fast_step<3, false>(v, ssc, sbi, rpre, stag_row, h >> 3, row & 7); break;
-                            }
-                        }
-                    } else {
-                        // ---- general path: fp32 predictor outputs, 16-column tails
-                        ptx::tmem_ld_wait(v);
-                        float y[32];
-#pragma unroll
-                        for (int i = 0; i < 32; i += 4) {
-                            if (i < cols) {
-                                const float4 sc = __ldg(reinterpret_cast<const float4*>(g.scale + n0 + i));
-                                const float4 bi = __ldg(reinterpret_cast<const float4*>(g.bias + n0 + i));
-                                y[i + 0] = fmaf(__uint_as_float(v[i + 0]), sc.x, bi.x);
-                                y[i + 1] = fmaf(__uint_as_float(v[i + 1]), sc.y, bi.y);
-                                y[i + 2] = fmaf(__uint_as_float(v[i + 2]), sc.z, bi.z);
-                                y[i + 3] = fmaf(__uint_as_float(v[i + 3]), sc.w, bi.w);
-                            }
-                        }
-                        if (has_res) {
-#pragma unroll
-                            for (int i = 0; i < 32; i += 8) {
-                                if (i < cols) {
-                                    const uint32_t* rb = reinterpret_cast<const uint32_t*>(&rpre[i >> 3]);
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j) {
-                                        const float2 f = unpack2_act(rb[j], p.fp16);
-                                        y[i + 2 * j] += f.x;
-                                        y[i + 2 * j + 1] += f.y;
-                                    }
-                                }
-                            }
-                            if (c0 + 64 + h < p.block_n) load_res(c0 + 64 + h);
-                        }
-                        if (p.relu) {
-#pragma unroll
-                            for (int i = 0; i < 32; ++i) y[i] = fmaxf(y[i], 0.0f);
-                        }
-                        if (p.out_mode == 0) {
-#pragma unroll
-                            for (int i = 0; i < 32; i += 8) {
-                                if (i < cols) {
-                                    uint4 o;
-                                    o.x = pack2_act(y[i + 0], y[i + 1], p.fp16);
-                                    o.y = pack2_act(y[i + 2], y[i + 3], p.fp16);
-                                    o.z = pack2_act(y[i + 4], y[i + 5], p.fp16);
-                                    o.w = pack2_act(y[i + 6], y[i + 7], p.fp16);
-                                    const int c16 = (h + i) >> 3;  // 16-byte chunk within the 128-byte row
-                                    ptx::st_shared_v4(stag_u32 + row * 128 + ((c16 ^ (row & 7)) << 4), o);
-                                }
-                            }
-                        } else if (f32_ptr != nullptr) {
-#pragma unroll
-                            for (int i = 0; i < 32; i += 4) {
-                                if (i < cols) {
-                                    float4 o = make_float4(y[i], y[i + 1], y[i + 2], y[i + 3]);
-                                    if (g.lo != nullptr) {
-                                        const float4 lo = __ldg(reinterpret_cast<const float4*>(g.lo + n0 + i));
-                                        o.x = fmaxf(o.x, lo.x);
-                                        o.y = fmaxf(o.y, lo.y);
-                                        o.z = fmaxf(o.z, lo.z);
-                                        o.w = fmaxf(o.w, lo.w);
-                                    }
-                                    *reinterpret_cast<float4*>(f32_ptr + c0 + h + i) = o;
-                                }
-                            }
-                        }
-                    }
-                }
-                if (p.out_mode == 0) {
-                    ptx::fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the TMA engine
-                    ptx::named_bar_sync(1, kEpiThreads);
-                    if (store_leader) {
-                        if (t.valid) ptx::tma_store_4d(&g.out_map, stag, n_base + c0, t.x0, t.y0, t.img);
-                        ptx::tma_store_commit();
-                    }
-                    if (g.pool_partial != nullptr && t.valid && et < 128) {
-                        // eSE global-average-pool, fused: per-tile channel sums of the 16-bit tile just staged (exactly the
-                        // values the reference pools, vovnet.py:181).  Thread e covers channels 8*(e&7).. of rows
-                        // (e>>3) + 16*i; the 4 row-groups of a warp are shuffle-reduced; one fp32 partial per
-                        // (tile, warp, channel) -> deterministic reduction later (no atomics).
-                        const int e = et;
-                        const int cg = e & 7;
-                        float ps[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const int r = (e >> 3) + 16 * i;
-                            const int ry = t.y0 + (r >> g.tw_shift), rx = t.x0 + (r & (g.tw - 1));
-                            if (ry < g.H && rx < g.W) {
-                                const uint4 u = ptx::ld_shared_v4(stag_u32 + r * 128 + ((cg ^ (r & 7)) << 4));
-                                const uint32_t* b2 = reinterpret_cast<const uint32_t*>(&u);
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    const float2 f = unpack2_act(b2[j], p.fp16);
-                                    ps[2 * j] += f.x;
-                                    ps[2 * j + 1] += f.y;
-                                }
-                            }
-                        }
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            ps[j] += __shfl_xor_sync(0xffffffffu, ps[j], 8);
-                            ps[j] += __shfl_xor_sync(0xffffffffu, ps[j], 16);
-                        }
-                        if (lane < 8 && c0 + cg * 8 < p.block_n) {
-                            const int tile_in_img = (t.y0 / g.th) * g.tiles_x + (t.x0 / g.tw);
-                            float* dst = g.pool_partial +
-                                         ((static_cast<size_t>(t.img) * (g.tiles_x * g.tiles_y) + tile_in_img) * 4 + (et >> 5)) *
-                                             g.pool_pitch +
-                                         n_base + c0 + cg * 8;
-                            *reinterpret_cast<float4*>(dst) = make_float4(ps[0], ps[1], ps[2], ps[3]);
-                            *reinterpret_cast<float4*>(dst + 4) = make_float4(ps[4], ps[5], ps[6], ps[7]);
-                        }
-                    }
-                    sbuf ^= 1;
-                }
-            }
-            // all TMEM reads of this accumulator are done -> hand it back to the MMA warp
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (CTA2) {
-                    ptx::mbar_arrive_cluster(tempty0 + acc * 8);  // the leader's MMA warp waits for both CTAs' epilogues
-                } else {
-                    ptx::mbar_arrive(&tempty_bar[acc]);
-                }
-            }
-            if (++acc == p.acc_stages) {
-                acc = 0;
-                acc_phase ^= 1;
-            }
-        }
-        if (store_leader) ptx::tma_store_wait_all();
-    }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (CTA2) ptx::cluster_sync();  // neither CTA may retire while the other can still target its smem / TMEM / barriers
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        if (CTA2) {
-            ptx::tmem_dealloc2(tmem_base, p.tmem_cols);
-        } else {
-            ptx::tmem_dealloc(tmem_base, p.tmem_cols);
-        }
-    }
-}
-
 // =========================================================================================== taps-in-N variant
 // 3x3 stride-1 convolutions with <= 16 output channels (FCOS predictors cls / [box2d_reg | centerness], DLA level0).
-// As nine N = 16 GEMMs per 64-channel block they sit at the UMMA instruction floor (~50-90 cycles for 128x16x16 instead of
-// 8) and reach 9 % tensor-pipe activity (profiles/r01d_conv_launches_v2_99.csv, launches 119/120).  Here the taps are GEMM
-// COLUMNS:  P[pixel of the (16+2)x(8+2) halo patch][tap * 16 + co] = sum_c in[pixel][c] * W[co][tap][c]  -- two
-// M128 x N144 x K16 UMMAs per K step over the SAME halo patch the halo variant stages -- and the output is the shifted sum
+// As nine N = 16 GEMMs per 64-channel block they sit at the tensor-core instruction floor.  Here the taps are GEMM COLUMNS:
+//   P[pixel of the (16+2)x(8+2) halo patch][tap * 16 + co] = sum_c in[pixel][c] * W[co][tap][c]
+// -- three M64 x N144 x K16 wgmmas per K step (one per consumer warpgroup: patch rows 0..63, 64..127, 128..191) over the
+// SAME halo patch the halo variant stages -- and the output is the shifted sum
 //   out[y][x][co] = sum_{r,s} P[(y + r) * 10 + (x + s)][(3 r + s) * 16 + co]
 // taken from shared memory in a fixed order (deterministic).  9x fewer tensor cycles, no extra HBM traffic.
-constexpr int kTapsThreads = 192;                 // warp 0 TMA, warp 1 MMA, warps 2..5 epilogue
+constexpr int kTapsThreads = 512;                 // warpgroup 0: TMA (warp 0); warpgroups 1..3: wgmma + epilogue
 constexpr int kTapsStages = 2;
 constexpr int kTapsBBytes = kTapsN * 128;         // 18 KiB weight tile per 64-channel block
 constexpr int kTapsPStride = 148;                 // fp32 words per patch pixel in P (144 + 4: conflict-free 128-bit access)
 constexpr int kTapsPRows = kHaloPW * kHaloPH;     // 180
 constexpr int kTapsPBytes = (kTapsPRows * kTapsPStride * 4 + 1023) / 1024 * 1024;
 constexpr int kTapsSmem = kTapsStages * (kHaloABytes + kTapsBBytes) + kTapsPBytes + kBarBytes + 1024;
-constexpr int kTapsAcc1Col = 256;                 // TMEM column of the second accumulator (patch rows 128..255)
+constexpr int kTapsConsumerWarps = 12;
 
+template <bool F16>
 __global__ void __launch_bounds__(kTapsThreads, 1) conv_taps_kernel(const __grid_constant__ ConvParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    // [A patches x stages | B tiles x stages | P | barriers].  The second UMMA of a K step reads patch rows 128..255; rows
-    // 180..255 lie past the patch (in the next slot / the B tiles): finite garbage that only reaches accumulator rows the
-    // epilogue never reads.
+    // [A patches x stages | B tiles x stages | P | barriers].  The third warpgroup reads patch rows 128..191; rows 180..191
+    // lie past the patch (in the next slot / the B tiles): finite values that only reach accumulator rows never stored.
     uint8_t* a_base = smem;
     uint8_t* b_base = smem + kTapsStages * kHaloABytes;
     const uint32_t p_u32 = ptx::smem_u32(b_base + kTapsStages * kTapsBBytes);
     uint64_t* bars = reinterpret_cast<uint64_t*>(b_base + kTapsStages * kTapsBBytes + kTapsPBytes);
     uint64_t* full_bar = bars;                   // [kTapsStages]
     uint64_t* empty_bar = bars + kTapsStages;    // [kTapsStages]
-    uint64_t* tfull_bar = empty_bar + kTapsStages;
-    uint64_t* tempty_bar = tfull_bar + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 1);
 
     const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
     const int lane = threadIdx.x & 31;
@@ -818,20 +50,11 @@ __global__ void __launch_bounds__(kTapsThreads, 1) conv_taps_kernel(const __grid
         for (int s = 0; s < p.nseg; ++s) ptx::prefetch_tensormap(&p.seg[s].in_map[0]);
         for (int i = 0; i < kTapsStages; ++i) {
             ptx::mbar_init(&full_bar[i], 1);
-            ptx::mbar_init(&empty_bar[i], 1);
+            ptx::mbar_init(&empty_bar[i], kTapsConsumerWarps);
         }
-        ptx::mbar_init(tfull_bar, 1);
-        ptx::mbar_init(tempty_bar, 4);  // one arrival per epilogue warp
         ptx::fence_barrier_init();
     }
-    if (warp == 1) {
-        ptx::tmem_alloc(tmem_slot, 512);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
@@ -841,10 +64,10 @@ __global__ void __launch_bounds__(kTapsThreads, 1) conv_taps_kernel(const __grid
         int stage = 0;
         uint32_t phase = 0;
         for (int work = w_first; work < w_total; work += w_step) {
-            const TileCoord t = decode_tile<false>(p, work, 0);
+            const TileCoord t = decode_tile(p, work);
             const ConvSeg& g = p.seg[t.seg];
             for (int kc = 0; kc < p.kchunks; ++kc) {
-                ptx::mbar_wait(&empty_bar[stage], phase ^ 1, 11);
+                ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
                 if (elect_one()) {
                     ptx::mbar_expect_tx(&full_bar[stage], kHaloPW * kHaloPH * 128 + kTapsBBytes);
                     ptx::tma_load_4d(a_base + stage * kHaloABytes, &g.in_map[0], &full_bar[stage], kc * kBlockK, t.x0 - 1,
@@ -858,158 +81,114 @@ __global__ void __launch_bounds__(kTapsThreads, 1) conv_taps_kernel(const __grid
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------ UMMA issuer
-        const uint32_t idesc = ptx::make_idesc_f16(kBlockM, kTapsN, p.fp16);
-        constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);  // SBO 1024, v1, SW128
-        const uint32_t a_lo0 = (ptx::smem_u32(a_base) >> 4) | (1u << 16);
-        const uint32_t b_lo0 = (ptx::smem_u32(b_base) >> 4) | (1u << 16);
+    } else if (warp >= 4) {
+        // ------------------------------------------------------------ consumers: wgmma into registers, dump P, shifted sum
+        const int slice = (warp >> 2) - 1;  // patch rows 64 * slice ..
+        const int et = static_cast<int>(threadIdx.x) - 128;
+        const int wl = (et >> 5) & 3;
+        const uint64_t desc_hi = ptx::make_sw128_desc(0) & ~0x3FFFull;
+        const uint32_t a_lo0 = (ptx::smem_u32(a_base) >> 4) + slice * (64 * 128 / 16);
+        const uint32_t b_lo0 = ptx::smem_u32(b_base) >> 4;
+        float acc[kTapsN / 2];
         int stage = 0;
-        uint32_t phase = 0, tphase = 0;
+        uint32_t phase = 0;
         for (int work = w_first; work < w_total; work += w_step) {
-            ptx::mbar_wait(tempty_bar, tphase ^ 1, 12);  // the previous tile's accumulators have been dumped
-            ptx::tc_fence_after();
+            const TileCoord t = decode_tile(p, work);
+            const ConvSeg& g = p.seg[t.seg];
             for (int kc = 0; kc < p.kchunks; ++kc) {
-                ptx::mbar_wait(&full_bar[stage], phase, 13);
-                ptx::tc_fence_after();
+                ptx::mbar_wait(&full_bar[stage], phase);
                 const uint32_t a_lo = a_lo0 + static_cast<uint32_t>(stage) * (kHaloABytes >> 4);
                 const uint32_t b_lo = b_lo0 + static_cast<uint32_t>(stage) * (kTapsBBytes >> 4);
-                const int ksteps = (kc == p.kchunks - 1) ? p.last_ksteps : kBlockK / 16;
-                if (elect_one()) {
-#pragma unroll
-                    for (int k = 0; k < kBlockK / 16; ++k) {
-                        if (k < ksteps) {
-                            const uint64_t bdesc = (static_cast<uint64_t>(kDescHi) << 32) | (b_lo + 2 * k);
-                            const uint64_t a0 = (static_cast<uint64_t>(kDescHi) << 32) | (a_lo + 2 * k);
-                            const uint64_t a1 = (static_cast<uint64_t>(kDescHi) << 32) | (a_lo + (16384 >> 4) + 2 * k);
-                            const uint32_t accumulate = (kc | k) != 0 ? 1u : 0u;
-                            ptx::umma_bf16(tmem_base, a0, bdesc, idesc, accumulate);                 // patch rows 0..127
-                            ptx::umma_bf16(tmem_base + kTapsAcc1Col, a1, bdesc, idesc, accumulate);  // patch rows 128..
-                        }
-                    }
-                    ptx::umma_commit(&empty_bar[stage]);
-                }
-                __syncwarp();
+                mma_kblock<kTapsN, F16>(acc, desc_hi | a_lo, desc_hi | b_lo, kc == 0);
+                wg::wait<0>();
+                if (lane == 0) ptx::mbar_arrive(&empty_bar[stage]);
                 if (++stage == kTapsStages) {
                     stage = 0;
                     phase ^= 1;
                 }
             }
-            if (elect_one()) ptx::umma_commit(tfull_bar);
-            __syncwarp();
-            tphase ^= 1;
-        }
-    } else {
-        // ------------------------------------------------------------ epilogue (warps 2..5): dump P, then shifted 9-tap sum
-        const int q = warp & 3;
-        const int m = q * 32 + lane;  // TMEM lane = patch row (first accumulator) and output pixel of the tile
-        uint32_t tphase = 0;
-        for (int work = w_first; work < w_total; work += w_step) {
-            const TileCoord t = decode_tile<false>(p, work, 0);
-            const ConvSeg& g = p.seg[t.seg];
-            ptx::mbar_wait(tfull_bar, tphase, 14);
-            ptx::tc_fence_after();
-            tphase ^= 1;
-            // ---- 1. TMEM -> P (fp32 [180][148]); patch rows 128..179 live in the second accumulator (warps of quarter 0 / 1)
+            wg::fence_regs(acc);
+            // ---- 1. registers -> P (fp32 [180][148])
 #pragma unroll
-            for (int a = 0; a < 2; ++a) {
-                const int prow = a * 128 + m;
-                if (a == 1 && q >= 2) break;  // warp-uniform: rows 192.. do not exist
-                const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + a * kTapsAcc1Col;
-                const uint32_t dst = p_u32 + prow * (kTapsPStride * 4);
+            for (int h = 0; h < 2; ++h) {
+                const int prow = 64 * slice + 16 * wl + (lane >> 2) + 8 * h;
+                if (prow < kTapsPRows) {
+                    const uint32_t dst = p_u32 + prow * (kTapsPStride * 4) + 2 * (lane & 3) * 4;
 #pragma unroll
-                for (int c0 = 0; c0 < kTapsN; c0 += 32) {
-                    uint32_t v[32];
-                    if (c0 + 32 <= kTapsN) {
-                        ptx::tmem_ld32(t_addr + c0, v);
-                    } else {
-                        ptx::tmem_ld16(t_addr + c0, v);
-                    }
-                    ptx::tmem_ld_wait(v);
-                    if (prow < kTapsPRows) {
-#pragma unroll
-                        for (int i = 0; i < 32; i += 4)
-                            if (c0 + i < kTapsN) ptx::st_shared_v4(dst + (c0 + i) * 4, make_uint4(v[i], v[i + 1], v[i + 2], v[i + 3]));
-                    }
+                    for (int j = 0; j < kTapsN / 8; ++j)
+                        ptx::st_shared_f2(dst + 8 * j * 4, make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
                 }
             }
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(tempty_bar);  // TMEM drained: the next tile's UMMAs may start
-            ptx::named_bar_sync(1, 128);                  // P complete
-            // ---- 2. out[y][x][:] = sum over the nine taps of the shifted partial sums (fixed order r, s)
-            const int ly = m >> 3, lx = m & 7;
-            const int oy = t.y0 + ly, ox = t.x0 + lx;
-            float acc[16];
+            ptx::named_bar_sync(1, kTapsConsumerWarps * 32);  // P complete
+            if (et < 128) {
+                // ---- 2. out[y][x][:] = sum over the nine taps of the shifted partial sums (fixed order r, s)
+                const int m = et;
+                const int ly = m >> 3, lx = m & 7;
+                const int oy = t.y0 + ly, ox = t.x0 + lx;
+                float sum[16];
 #pragma unroll
-            for (int i = 0; i < 16; ++i) acc[i] = 0.f;
+                for (int i = 0; i < 16; ++i) sum[i] = 0.f;
 #pragma unroll
-            for (int tap = 0; tap < 9; ++tap) {
-                const int r = tap / 3, s = tap - 3 * r;
-                const uint32_t src = p_u32 + ((ly + r) * kHaloPW + lx + s) * (kTapsPStride * 4) + tap * 64;
+                for (int tap = 0; tap < 9; ++tap) {
+                    const int r = tap / 3, s = tap - 3 * r;
+                    const uint32_t src = p_u32 + ((ly + r) * kHaloPW + lx + s) * (kTapsPStride * 4) + tap * 64;
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float4 f = ptx::ld_shared_f4(src + 16 * i);
-                    acc[4 * i + 0] += f.x;
-                    acc[4 * i + 1] += f.y;
-                    acc[4 * i + 2] += f.z;
-                    acc[4 * i + 3] += f.w;
+                    for (int i = 0; i < 4; ++i) {
+                        const float4 f = ptx::ld_shared_f4(src + 16 * i);
+                        sum[4 * i + 0] += f.x;
+                        sum[4 * i + 1] += f.y;
+                        sum[4 * i + 2] += f.z;
+                        sum[4 * i + 3] += f.w;
+                    }
                 }
-            }
-            if (t.valid && oy < g.H && ox < g.W) {
-                float y[16];
-#pragma unroll
-                for (int i = 0; i < 16; i += 4) {
-                    const float4 sc = __ldg(reinterpret_cast<const float4*>(g.scale + i));
-                    const float4 bi = __ldg(reinterpret_cast<const float4*>(g.bias + i));
-                    y[i + 0] = fmaf(acc[i + 0], sc.x, bi.x);
-                    y[i + 1] = fmaf(acc[i + 1], sc.y, bi.y);
-                    y[i + 2] = fmaf(acc[i + 2], sc.z, bi.z);
-                    y[i + 3] = fmaf(acc[i + 3], sc.w, bi.w);
-                }
-                if (p.relu) {
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) y[i] = fmaxf(y[i], 0.f);
-                }
-                const size_t pix = static_cast<size_t>(t.img * g.H + oy) * g.W + ox;
-                if (p.out_mode == 1) {
-                    float* dst = g.out_f32 + pix * g.out_pitch;
+                if (oy < g.H && ox < g.W) {
+                    float y[16];
 #pragma unroll
                     for (int i = 0; i < 16; i += 4) {
-                        float4 o = make_float4(y[i], y[i + 1], y[i + 2], y[i + 3]);
-                        if (g.lo != nullptr) {
-                            const float4 lo = __ldg(reinterpret_cast<const float4*>(g.lo + i));
-                            o.x = fmaxf(o.x, lo.x);
-                            o.y = fmaxf(o.y, lo.y);
-                            o.z = fmaxf(o.z, lo.z);
-                            o.w = fmaxf(o.w, lo.w);
-                        }
-                        *reinterpret_cast<float4*>(dst + i) = o;
+                        const float4 sc = __ldg(reinterpret_cast<const float4*>(g.scale + i));
+                        const float4 bi = __ldg(reinterpret_cast<const float4*>(g.bias + i));
+                        y[i + 0] = fmaf(sum[i + 0], sc.x, bi.x);
+                        y[i + 1] = fmaf(sum[i + 1], sc.y, bi.y);
+                        y[i + 2] = fmaf(sum[i + 2], sc.z, bi.z);
+                        y[i + 3] = fmaf(sum[i + 3], sc.w, bi.w);
                     }
-                } else {
-                    uint4 o0, o1;
-                    o0.x = pack2_act(y[0], y[1], p.fp16);
-                    o0.y = pack2_act(y[2], y[3], p.fp16);
-                    o0.z = pack2_act(y[4], y[5], p.fp16);
-                    o0.w = pack2_act(y[6], y[7], p.fp16);
-                    o1.x = pack2_act(y[8], y[9], p.fp16);
-                    o1.y = pack2_act(y[10], y[11], p.fp16);
-                    o1.z = pack2_act(y[12], y[13], p.fp16);
-                    o1.w = pack2_act(y[14], y[15], p.fp16);
-                    uint4* dst = reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(g.out16) + pix * g.out_pitch);
-                    dst[0] = o0;
-                    dst[1] = o1;
+                    if (p.relu) {
+#pragma unroll
+                        for (int i = 0; i < 16; ++i) y[i] = fmaxf(y[i], 0.f);
+                    }
+                    const size_t pix = static_cast<size_t>(t.img * g.H + oy) * g.W + ox;
+                    if (p.out_mode == 1) {
+                        float* dst = g.out_f32 + pix * g.out_pitch;
+#pragma unroll
+                        for (int i = 0; i < 16; i += 4) {
+                            float4 o = make_float4(y[i], y[i + 1], y[i + 2], y[i + 3]);
+                            if (g.lo != nullptr) {
+                                const float4 lo = __ldg(reinterpret_cast<const float4*>(g.lo + i));
+                                o.x = fmaxf(o.x, lo.x);
+                                o.y = fmaxf(o.y, lo.y);
+                                o.z = fmaxf(o.z, lo.z);
+                                o.w = fmaxf(o.w, lo.w);
+                            }
+                            *reinterpret_cast<float4*>(dst + i) = o;
+                        }
+                    } else {
+                        uint4 o0, o1;
+                        o0.x = pack2_act(y[0], y[1], F16 ? 1 : 0);
+                        o0.y = pack2_act(y[2], y[3], F16 ? 1 : 0);
+                        o0.z = pack2_act(y[4], y[5], F16 ? 1 : 0);
+                        o0.w = pack2_act(y[6], y[7], F16 ? 1 : 0);
+                        o1.x = pack2_act(y[8], y[9], F16 ? 1 : 0);
+                        o1.y = pack2_act(y[10], y[11], F16 ? 1 : 0);
+                        o1.z = pack2_act(y[12], y[13], F16 ? 1 : 0);
+                        o1.w = pack2_act(y[14], y[15], F16 ? 1 : 0);
+                        uint4* dst = reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(g.out16) + pix * g.out_pitch);
+                        dst[0] = o0;
+                        dst[1] = o1;
+                    }
                 }
             }
-            ptx::named_bar_sync(1, 128);  // every thread is done with P before the next tile's dump overwrites it
+            ptx::named_bar_sync(1, kTapsConsumerWarps * 32);  // every thread is done with P before the next tile's dump
         }
-    }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, 512);
     }
 }
 
@@ -1171,43 +350,14 @@ void conv_finalize_params(ConvParams* p) {
     }
     p->inv_n_blocks = 1.0f / static_cast<float>(p->n_blocks);
     p->total_work = tile * p->n_blocks;
-    p->total_tiles = tile;
-    // CTA pairs pay off where the weight tile is large (measured per layer, profiles/r01d_cta2_ab.md): N >= 160 and at
-    // least two waves of tiles; small-N layers (stem, OSA2) are issue/epilogue-bound and lose a few % to the pairing.
-    if (p->cta2 == 2) {  // auto
-        static int min_n = -1;
-        if (min_n < 0) {
-            const char* e = getenv("DD3D_CONV_CTA2_MINN");
-            min_n = e ? atoi(e) : 160;
-        }
-        // ... or where the weight stream itself is the limiter: a deep-K layer re-reads its whole weight tensor from L2 for
-        // every 128-pixel tile (N x K x 2 B; 516 KB for the box3d predictor, N = 112, K = 2304 -> 16 GB per launch), a pair
-        // reads it once per 256 pixels.
-        static int deep_k = -1;
-        if (deep_k < 0) {
-            const char* e = getenv("DD3D_CONV_CTA2_DEEPK");
-            deep_k = e ? atoi(e) : 1;
-        }
-        const bool deep = deep_k && p->block_n >= 96 && p->taps * p->kchunks >= 36;
-        // ... or a 3x3 stride-1 layer with N = 128: per UMMA the tensor core reads A (4 KB) + B (4 KB) from shared memory in
-        // the 64 cycles the MMA takes -- the whole smem bandwidth before TMA refills it (59.6 % tensor pipe); in a pair each
-        // CTA reads half of B.  Same box, alternating: OSA2 3x3 0.82 -> 0.71 ms; the stride-2 generic N = 128 layer
-        // (stem_3) loses 47 % to pairing and stays single (profiles/r02_ab.md).
-        const bool n128_halo = p->halo && p->block_n >= 128;
-        p->cta2 = ((p->block_n >= min_n || deep || n128_halo) && tile >= 4 * 74) ? 1 : 0;
-    }
-    if (p->cta2 && (tile < 2 || (p->block_n % 16) != 0)) p->cta2 = 0;
-    if (p->taps_n) p->cta2 = 0;
-    p->pair_work = ((tile + 1) / 2) * p->n_blocks;
-    const int stage_bytes = (p->halo ? 0 : kABytes) + (p->cta2 ? p->block_n / 2 : p->block_n) * 128;
+    const int stage_bytes = (p->halo ? 0 : kABytes) + p->block_n * 128;
     const int base = 2 * kStagingBytes + 1024 /*alignment slack*/ + kBarBytes + kSbBytes;
     p->a_stages = p->halo ? kHaloAStages : 0;
     p->wstat = 0;
     // Weight-stationary: a 3x3 layer whose whole weight tensor is a few k-blocks (64 -> 64: 9 x 8 KiB; DLA-34 level2, VoVNet
-    // stem_2) re-streamed it through the 8-deep B ring for every 128-pixel tile -- barely one tile of lookahead against a TMA
-    // round trip of ~2 tiles' worth of MMAs, so the MMA warp waited on weights (ncu: 5.4 k cycles per tile for 1.2 k cycles
-    // of MMAs).  The tensor stays resident instead and the freed barriers / shared memory go to deeper A-patch prefetch.
-    if (p->halo && !p->cta2 && !p->taps_n && p->n_blocks == 1 && conv_wstat_enabled()) {
+    // stem_2) would re-stream it through the B ring for every 128-pixel tile -- barely one tile of lookahead against a TMA
+    // round trip.  The tensor stays resident instead and the freed barriers / shared memory go to deeper A-patch prefetch.
+    if (p->halo && !p->taps_n && p->n_blocks == 1 && conv_wstat_enabled()) {
         const int resident = p->taps * p->kchunks * stage_bytes;
         for (int a = kMaxAStages; a >= kHaloAStages; --a) {
             if (base + resident + a * kHaloABytes <= kSmemBudget) {
@@ -1220,19 +370,8 @@ void conv_finalize_params(ConvParams* p) {
     const int fixed = base + p->a_stages * kHaloABytes;
     int stages = (kSmemBudget - fixed) / stage_bytes;
     p->num_stages = p->wstat ? 2 : std::max(2, std::min(kMaxStages, stages));
-    const int chains = 1;  // split-K accumulator chains were measured and dropped (DESIGN.md 7); field kept = 1
-    p->chains = chains;
-    p->acc_stages = (2 * chains * p->block_n <= 512) ? 2 : 1;
-    {
-        const int rem = p->cin - kBlockK * (p->kchunks - 1);
-        p->last_ksteps = (p->cin > 0 && rem > 0 && chains == 1) ? std::min(kBlockK / 16, (rem + 15) / 16) : kBlockK / 16;
-    }
-    int cols = 32;
-    while (cols < p->acc_stages * chains * p->block_n) cols *= 2;
-    p->tmem_cols = cols;
 }
 
-static int g_cta2_mode = -1;
 static int g_n_split = -1;
 static int g_wstat = -1;
 
@@ -1254,30 +393,32 @@ bool conv_n_split_enabled() {
 }
 void conv_set_n_split(int mode) { g_n_split = (mode == 0 || mode == 1) ? mode : -1; }
 
-int conv_use_cta2() {  // 0 never, 1 always (where legal), 2 auto (per-layer rule in conv_finalize_params)
-    if (g_cta2_mode < 0) {
-        const char* e = getenv("DD3D_CONV_CTA2");
-        g_cta2_mode = e ? (!strcmp(e, "auto") ? 2 : (atoi(e) != 0)) : kConvCta2Default;
-    }
-    return g_cta2_mode;
-}
-
-void conv_set_cta2(int mode) { g_cta2_mode = (mode >= 0 && mode <= 2) ? mode : -1; }
-
 cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
-    const int stage_bytes = (p.halo ? 0 : kABytes) + (p.cta2 ? p.block_n / 2 : p.block_n) * 128;
+    const int stage_bytes = (p.halo ? 0 : kABytes) + p.block_n * 128;
     const int smem_bytes = (p.wstat ? p.taps * p.kchunks : p.num_stages) * stage_bytes + 2 * kStagingBytes + 1024 + kBarBytes +
                            kSbBytes + p.a_stages * kHaloABytes;
+    ConvKernel kernel = nullptr;
+    for (auto group : {conv_kernel_n16_64, conv_kernel_n80_128, conv_kernel_n144_192, conv_kernel_n208_256}) {
+        if (kernel == nullptr) kernel = group(p.halo != 0, p.fp16 != 0, p.block_n);
+    }
+    if (kernel == nullptr) return cudaErrorInvalidValue;  // block_n must be a multiple of 16 in [16, 256] (the wgmma N)
     static uint64_t attr_devices = 0;  // per-device opt-in to > 48 KB dynamic shared memory
     if (first_use_on_device(&attr_devices)) {
-        cudaError_t e = cudaFuncSetAttribute(conv_igemm_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             kSmemBudget);
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(conv_igemm_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(conv_igemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(conv_igemm_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
+        cudaError_t e = cudaSuccess;
+        for (bool halo : {false, true}) {
+            for (bool fp16 : {false, true}) {
+                for (int n = 16; n <= 256; n += 16) {
+                    ConvKernel k = nullptr;
+                    for (auto group : {conv_kernel_n16_64, conv_kernel_n80_128, conv_kernel_n144_192, conv_kernel_n208_256}) {
+                        if (k == nullptr) k = group(halo, fp16, n);
+                    }
+                    if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
+                }
+            }
+        }
+        for (auto fn : {conv_taps_kernel<false>, conv_taps_kernel<true>}) {
+            if (e == cudaSuccess) e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kTapsSmem);
+        }
         if (e != cudaSuccess) return e;
     }
     if (p.total_work <= 0) return cudaSuccess;
@@ -1287,52 +428,19 @@ cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
         const char* e = getenv("DD3D_NO_PDL");
         use_pdl = (e && atoi(e)) ? 0 : 1;
     }
-    if (p.taps_n) {
-        static uint64_t taps_devices = 0;
-        if (first_use_on_device(&taps_devices)) {
-            cudaError_t e = cudaFuncSetAttribute(conv_taps_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTapsSmem);
-            if (e != cudaSuccess) return e;
-        }
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(std::min(p.total_work, num_sms));
-        cfg.blockDim = dim3(kTapsThreads);
-        cfg.dynamicSmemBytes = kTapsSmem;
-        cfg.stream = stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = use_pdl ? 1 : 0;
-        return cudaLaunchKernelEx(&cfg, conv_taps_kernel, p);
-    }
-    // CTA pairs: an even grid of 2-CTA clusters (one pair per TPC), each pair loops over pair-work items
-    const int grid = p.cta2 ? 2 * std::min(p.pair_work, num_sms / 2) : std::min(p.total_work, num_sms);
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kConvThreads);
-    cfg.dynamicSmemBytes = smem_bytes;
+    cfg.gridDim = dim3(std::min(p.total_work, num_sms));
+    cfg.blockDim = dim3(p.taps_n ? kTapsThreads : kConvThreads);
+    cfg.dynamicSmemBytes = p.taps_n ? kTapsSmem : smem_bytes;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (use_pdl) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    if (p.cta2) {
-        attr[na].id = cudaLaunchAttributeClusterDimension;
-        attr[na].val.clusterDim.x = 2;
-        attr[na].val.clusterDim.y = 1;
-        attr[na].val.clusterDim.z = 1;
-        ++na;
-    }
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = na;
-    if (p.cta2)
-        return p.halo ? cudaLaunchKernelEx(&cfg, conv_igemm_kernel<true, true>, p)
-                      : cudaLaunchKernelEx(&cfg, conv_igemm_kernel<false, true>, p);
-    return p.halo ? cudaLaunchKernelEx(&cfg, conv_igemm_kernel<true, false>, p)
-                  : cudaLaunchKernelEx(&cfg, conv_igemm_kernel<false, false>, p);
+    cfg.numAttrs = use_pdl ? 1 : 0;
+    if (p.taps_n)
+        return p.fp16 ? cudaLaunchKernelEx(&cfg, conv_taps_kernel<true>, p) : cudaLaunchKernelEx(&cfg, conv_taps_kernel<false>, p);
+    return cudaLaunchKernelEx(&cfg, kernel, p);
 }
 
 }  // namespace dd3d

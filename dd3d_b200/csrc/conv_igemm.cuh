@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution on tcgen05 tensor cores (sm_100a): interface.
+// Implicit-GEMM convolution on Hopper tensor cores (sm_90a, wgmma): interface.
 //
 // One launch covers up to kMaxSeg "segments" (FPN levels) that share one weight tensor (the FCOS towers share
 // weights across levels, reference fcos2d.py:74-91 / fcos3d.py:81-100) but have their own activation tensors,
@@ -14,7 +14,7 @@ namespace dd3d {
 constexpr int kMaxSeg = 5;
 constexpr int kBlockM = 128;  // output pixels per tile (th * tw)
 constexpr int kBlockK = 64;   // bf16 channels per k-block = one 128-byte swizzle row
-constexpr int kConvThreads = 352;  // warps: 0 TMA, 1 MMA, 2 second TMA producer, 3-10 epilogue (two per TMEM lane quarter)
+constexpr int kConvThreads = 384;  // warpgroup 0: TMA producers (warps 0, 2); warpgroups 1, 2: wgmma + epilogue, 64 rows each
 
 struct ConvSeg {
     CUtensorMap in_map[2];  // NHWC bf16 input.  stride 1: [0] (4-D).  stride 2: [w-parity] (5-D parity split)
@@ -46,20 +46,13 @@ struct ConvParams {
     int stride;    // 1 or 2 (3x3 only)
     int kchunks;   // ceil(cin / 64)
     int n_blocks;  // cout_pad / block_n
-    int block_n;   // UMMA N (multiple of 16, <= 256)
+    int block_n;   // wgmma N (multiple of 16, <= 256)
     int relu;
     int out_mode;  // 0: bf16 via TMA store, 1: fp32 direct
     int total_work;  // (sum of M-tiles) * n_blocks
     int num_stages;
-    int tmem_cols;
-    int chains;      // split-K accumulator chains per tile (independent TMEM accumulators, summed in the epilogue)
-    int acc_stages;  // 2: accumulators double-buffered against the epilogue, 1: single-buffered
-    int cin;          // real input channels (the zero-padded K steps of the last 64-channel block are skipped)
-    int last_ksteps;  // K=16 steps of the last channel block: ceil((cin - 64*(kchunks-1)) / 16)
+    int cin;          // real input channels
     int halo;  // 1: 3x3 stride-1 halo-reuse variant (tile 16x8, A patch loaded once per 64-channel block)
-    int cta2;         // 1: CTA-pair variant (cluster of 2, tcgen05.mma.cta_group::2, M = 256); w_map box = block_n / 2 rows
-    int total_tiles;  // sum of M-tiles over the segments
-    int pair_work;    // ceil(total_tiles / 2) * n_blocks
     float inv_n_blocks;
     int taps_n;       // 1: taps-in-N variant for 3x3 stride-1 convs with <= 16 output channels (conv_taps_kernel)
     int fp16;         // 16-bit storage type of activations and weights: 0 bf16, 1 fp16 (act16.cuh)
@@ -67,7 +60,6 @@ struct ConvParams {
     int a_stages;     // halo variants: A patches in flight (3, or up to 5 with wstat)
 };
 static_assert(sizeof(ConvParams) <= 4096, "kernel parameter space");
-constexpr int kConvCta2Default = 2;  // auto; DD3D_CONV_CTA2=0|1|auto overrides
 
 // Host helpers (conv_igemm.cu)
 const char* conv_last_error();
@@ -75,10 +67,6 @@ bool make_act_map(CUtensorMap* map, const void* base, int B, int H, int W, int C
 bool make_act_map_s2(CUtensorMap* map, const void* base, int wp, int B, int H, int W, int C, int pitch, int th,
                      int tw, int fp16 = 0);
 bool make_weight_map(CUtensorMap* map, const void* base, int ktot, int cout_pad, int block_n, int fp16 = 0);
-// CTA-pair policy for ConvParams::cta2 before conv_finalize_params: 0 never, 1 always, 2 auto (finalize decides; the
-// w_map box must then be block_n / 2 rows iff the finalized cta2 is 1)
-int conv_use_cta2();
-void conv_set_cta2(int mode);  // process-wide override (plans built afterwards); -1: back to the environment / default
 void choose_tile(int H, int W, int* th, int* tw);
 int conv_tiles_per_image(int H, int W);  // M-tiles per image of the generic tiling
 // Halo variant (3x3, stride 1): one 128B-swizzled [18][10][64 ch] patch per 64-channel block serves all nine taps.
@@ -89,7 +77,7 @@ bool make_act_map_halo(CUtensorMap* map, const void* base, int B, int H, int W, 
 // tiling over all segments (env DD3D_CONV_MODE=generic|halo overrides, for tests).
 bool conv_prefer_halo(int taps, int stride, int block_n, int nseg, const int* Hs, const int* Ws);
 // Taps-in-N variant (3x3, stride 1, cout_pad == 16): the nine taps become GEMM columns -- ONE [180 patch pixels] x [9 x 16]
-// GEMM per 64-channel block instead of nine N = 16 GEMMs (the N = 16 UMMA costs ~50-90 cycles, the N = 144 one 72), then the
+// GEMM per 64-channel block instead of nine N = 16 GEMMs (an N = 16 wgmma runs far below the tensor-core rate), then the
 // nine shifted partial sums are added from shared memory.  Weights: bf16 [9 * 16][cin_pad64] (row = tap * 16 + cout).
 constexpr int kTapsN = 144;
 bool make_weight_map_taps(CUtensorMap* map, const void* base, int cin_pad, int fp16 = 0);
@@ -100,7 +88,7 @@ bool conv_wstat_enabled();       // weight-stationary halo layers: on by default
 void conv_set_wstat(int mode);   // 0 off, 1 on, -1 environment / default
 bool conv_n_split_enabled();
 void conv_set_n_split(int mode);  // 0 off, 1 on, -1 environment / default (on)
-// Fills num_stages / tmem_cols / total_work / tile bookkeeping from the already-set fields.
+// Fills num_stages / total_work / tile bookkeeping from the already-set fields.
 void conv_finalize_params(ConvParams* p);
 cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream);
 

@@ -2,9 +2,9 @@
 // conv + FrozenBN + ReLU (reference dla.py:271-283 `base_layer`, `level0`, `level1`, forward dla.py:346-350), plus the 2x2
 // max-pool of level1's output that level2's Tree takes as `bottom` (dla.py:235).
 //
-// Why a separate kernel.  The three layers carry 4 % of DLA-34's FLOPs but, run one by one, 0.64 ms of a 2.66 ms forward
+// Why a separate kernel.  The three layers carry 4 % of DLA-34's FLOPs but, run one by one, a large share of the forward
 // (B = 8, 384x1280): each writes and re-reads a full-resolution 16-channel map (126 MB) and none has enough K (<= 16 per
-// tap) or N (<= 32) for a tcgen05 tile -- a 128x16 A tile costs the same shared-memory read whatever N is, and the
+// tap) or N (<= 32) for a wgmma tile -- a 64x16 A tile costs the same shared-memory read whatever N is, and the
 // taps-in-N form pays a 576 B/pixel fp32 round trip through shared memory.  Here the two full-resolution intermediates
 // never leave the SM: a CTA owns an 8x32 tile of level1's output, recomputes the 19x67 / 17x65 halo regions of base_layer /
 // level0 in shared memory and writes only level1 (+ its pooled copy).  HBM traffic per image pixel: 8 B in, 16 B + 4 B out
@@ -13,8 +13,8 @@
 // Arithmetic: warp-level mma.sync.m16n8k16 (bf16 or fp16 operands, fp32 accumulate) on purpose -- the operand fragments
 // are gathered straight from the shared-memory patches (LDS.64 of whole input pixels for the 7x7, ldmatrix of 16-channel
 // pixels for the 3x3s, any shift / stride for free), the accumulators live in registers and the BN + ReLU + 16-bit
-// rounding happens there, so there is no im2col copy, no TMEM round trip and no CTA-wide barrier inside a layer.  The
-// kernel is bound by shared-memory wavefronts (~10.6 k per tile) and the legacy tensor path, not by HBM or tcgen05 peak.
+// rounding happens there, so there is no im2col copy, no shared-memory round trip of the accumulators and no CTA-wide
+// barrier inside a layer.  The kernel is bound by shared-memory wavefronts and the mma.sync path, not by HBM or wgmma peak.
 //
 // Numerics are those of the layer-by-layer path (and of the oracle's 16-bit emulation): every intermediate is rounded to
 // the storage type, conv padding is zero OUTSIDE THE IMAGE (halo positions beyond the border are forced to 0 after the

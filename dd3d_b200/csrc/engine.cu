@@ -46,8 +46,8 @@ Engine::Engine(const dd3d_model_desc& d) : desc(d) {
     cuda_check(cudaGetDevice(&device), "cudaGetDevice");
     cudaDeviceProp prop;
     cuda_check(cudaGetDeviceProperties(&prop, device), "cudaGetDeviceProperties");
-    if (prop.major != 10) {
-        fail(DD3D_ERR_CUDA, std::string("dd3d_b200 needs an sm_100 (B200) device, found ") + prop.name + " sm_" +
+    if (prop.major != 9) {
+        fail(DD3D_ERR_CUDA, std::string("dd3d_b200 needs an sm_90 (H100) device, found ") + prop.name + " sm_" +
                                 std::to_string(prop.major) + std::to_string(prop.minor));
     }
     num_sms = prop.multiProcessorCount;
@@ -144,7 +144,6 @@ const ConvLayer& Engine::conv_layer(const std::string& key, const std::vector<st
     L.d_w = static_cast<__nv_bfloat16*>(dev_alloc(packed.size() * 2));
     cuda_check(cudaMemcpy(L.d_w, packed.data(), packed.size() * 2, cudaMemcpyHostToDevice), "upload conv weights");
     if (!make_weight_map(&L.w_map, L.d_w, L.ktot, L.cout_pad, L.block_n, fp16)) fail(DD3D_ERR_CUDA, conv_last_error());
-    if (!make_weight_map(&L.w_map_half, L.d_w, L.ktot, L.cout_pad, L.block_n / 2, fp16)) fail(DD3D_ERR_CUDA, conv_last_error());
     if (L.taps == 9 && L.cout_pad == 16) {
         // taps-in-N copy (conv_taps_kernel): row = tap * 16 + cout, K = channels
         std::vector<uint16_t> tp(static_cast<size_t>(kTapsN) * cin_pad, 0);
@@ -291,7 +290,6 @@ struct Builder {
         op.type = Op::CONV;
         ConvParams& p = op.conv;
         memset(&p, 0, sizeof(p));
-        p.cta2 = conv_use_cta2();  // policy; conv_finalize_params turns it into the per-layer decision
         p.nseg = static_cast<int>(segs.size());
         p.B = B;
         p.taps = L.taps;
@@ -361,8 +359,8 @@ struct Builder {
                 g.res_W = sp.res.W;
             }
         }
-        // Under-filled launches (DLA-34 level5 at B = 8: 30 M-tiles x 2 N-blocks on 148 SMs; p6 / p7): split N until the grid
-        // covers the machine.  Each CTA's serial MMA chain shrinks with N (128 -> 64 -> 32 cycles per K = 16 step) while the
+        // Under-filled launches (DLA-34 level5 at B = 8: 30 M-tiles x 2 N-blocks on 132 SMs; p6 / p7): split N until the grid
+        // covers the machine.  Each CTA's serial MMA chain shrinks with N while the
         // A tiles it re-reads are tiny; K order per output element is unchanged, so results are bit-identical.
         bool n_split = false;
         if (!p.taps_n && conv_n_split_enabled()) {
@@ -379,10 +377,10 @@ struct Builder {
         }
         conv_finalize_params(&p);
         if (n_split) {
-            if (!make_weight_map(&p.w_map, L.d_w, L.ktot, L.cout_pad, p.cta2 ? p.block_n / 2 : p.block_n, E->fp16))
+            if (!make_weight_map(&p.w_map, L.d_w, L.ktot, L.cout_pad, p.block_n, E->fp16))
                 fail(DD3D_ERR_CUDA, conv_last_error());
         } else {
-            p.w_map = p.taps_n ? L.w_map_taps : (p.cta2 ? L.w_map_half : L.w_map);
+            p.w_map = p.taps_n ? L.w_map_taps : L.w_map;
         }
         for (int s = 0; s < p.nseg; ++s)
             op.flops += 2.0 * B * p.seg[s].H * p.seg[s].W * static_cast<double>(L.cout) * L.cin * L.taps;
@@ -739,9 +737,8 @@ struct Builder {
         const bool per_level = E->desc.per_level_predictors != 0, box3d_on = E->desc.box3d_on != 0;
         const int C3 = E->desc.class_agnostic_box3d ? 1 : C;
         const int cls_pitch = round_up(C + (nusc ? kNumAttributes + 1 : 0), 16), b3d_pitch = round_up(11 * C3, 16);
-        // sparse box3d predictor: forced (1), off (0) or auto (2, default).  The dense launch costs ~0.45 us per 1 000 head
-        // pixels, the gathered one a near-constant 0.08 - 0.12 ms of latency-bound K loop: V2-99 at B = 32 (4.1 M pixels)
-        // 1.75 ms dense vs 0.12 ms sparse; DLA-34 at B = 8 (82 k pixels) 0.05 ms dense vs 0.08 ms sparse.  The rule looks at
+        // sparse box3d predictor: forced (1), off (0) or auto (2, default).  The dense launch costs time in proportion to the
+        // head pixels, the gathered one a near-constant latency-bound K loop, so large heads go sparse.  The rule looks at
         // the head pixels of ONE image, not of the batch, so that an image gives bit-identical detections whatever batch it
         // rides in (the two predictors differ in fp32 summation order): 900x1600 V2-99 = 127 875 pixels -> sparse at every
         // batch size, 384x1280 DLA-34 = 10 230 -> dense.

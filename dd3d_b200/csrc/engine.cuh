@@ -47,7 +47,6 @@ struct ConvLayer {
     int cin, cout, ksize, taps, kchunks, ktot, cout_pad, block_n, n_blocks;
     __nv_bfloat16* d_w;
     CUtensorMap w_map;
-    CUtensorMap w_map_half;  // box of block_n / 2 rows: each CTA of a pair loads half of the weight tile
     __nv_bfloat16* d_w_taps = nullptr;  // taps-in-N layout [9 * 16][cin_pad64] (3x3 layers with cout_pad == 16 only)
     CUtensorMap w_map_taps;
 };
@@ -160,7 +159,7 @@ class Engine {
                          cudaStream_t stream);
     void drop_plans();  // frees the active and the cached plans (an option that changes the op graph was flipped)
     int launches_per_forward() const;
-    // categories: 0 preprocess, 1 stem, 2 conv (tcgen05), 3 pool, 4 eSE, 5 relu, 6 decode, 7 nms
+    // categories: 0 preprocess, 1 stem, 2 conv (wgmma), 3 pool, 4 eSE, 5 relu, 6 decode, 7 nms
     void get_profile(double* ms, double* flops, double* bytes, int32_t* launches);
     int get_op_times(float* ms, int32_t* cats, double* flops, int max_ops);
 
@@ -179,15 +178,15 @@ class Engine {
 
     dd3d_model_desc desc;
     int device = 0;
-    int num_sms = 148;
+    int num_sms = 132;
     int fp16 = 0;  // desc.act_dtype == DD3D_ACT_FP16: 16-bit storage of activations / weights is fp16 instead of bf16
     bool finalized = false;
     int opt_do_postprocess = 1;
     int opt_profile = 0;
     int opt_workspace_reuse = 1;  // 0: bump allocation, every op output keeps its own memory (stage-level tests / debugging)
     int opt_ese_pool = 0;  // 1: a VoVNet stage's last eSE scale pass also writes the next stage's max-pooled input; 0 (default):
-                           // separate pool kernel -- measured: the fused pass is ~10 % SLOWER (profiles/r02l_*: 1.53 vs 0.75 + 0.56 ms)
-    int opt_stem_mma = 1;  // 1: VoVNet stem_1 on the register-fragment kernel (stem_mma.cu); 0: tcgen05 im2col kernel (stem_tc.cu)
+                           // separate pool kernel (the fused pass re-reads each pooling window's inputs 2.25 times)
+    int opt_stem_mma = 1;  // 1: VoVNet stem_1 on the register-fragment kernel (stem_mma.cu); 0: wgmma im2col kernel (stem_tc.cu)
     int opt_sparse_box3d = 2;  // box3d predictor at the final candidates only (b3d_sparse.cu): 0 never (dense maps), 1 always, 2 auto (by head size)
     int opt_dla_front = 1;  // 1: DLA-34 base_layer + level0 + level1 (+ pool) as ONE kernel (dla_front.cu); 0: layer by layer
     int opt_workspace_fill = -1;  // >= 0: byte the whole arena is filled with at dd3d_plan (poison test)

@@ -326,8 +326,8 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
 // ---------------------------------------------------------------------------------------------- multi-CTA path
 // batched_nms never lets boxes of different classes suppress each other (detectron2 batched_nms -> torchvision: per-class
 // coordinate offsets), so the greedy scan is independent per (image, class) -- but one class can hold most of an image's
-// candidates (the DLA-34 bench batch: 616 of 623 in one class), and the n^2 / 2 IoUs of a 600-box class on ONE SM cost
-// 205 us (ncu, profiles/r02i_launches_dla34.csv): the NMS was 9 % of the DLA-34 step.  Four launches:
+// candidates (the DLA-34 bench batch: 616 of 623 in one class), and the n^2 / 2 IoUs of a 600-box class would run on
+// ONE SM.  Four launches:
 //   nms_sort_kernel  (32 x B CTAs)       : rank sort of the image's candidates by score_3d; publish order / class and a
 //                                          CLASS-MAJOR copy (boxes + sorted position, score order inside a class, 64-aligned)
 //   nms_mask_kernel  (64 x B CTAs)       : IoU bit matrix of every class segment, 64 x 64 boxes per step, on all SMs

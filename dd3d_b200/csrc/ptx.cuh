@@ -1,5 +1,5 @@
-// Inline-PTX wrappers for the sm_100a features the DD3D kernels use: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld) and proxy fences.  sm_100a only -- there is no fallback path.
+// Inline-PTX wrappers for the sm_90a features the DD3D kernels use: mbarrier, TMA (cp.async.bulk.tensor), wgmma operand
+// descriptors and proxy fences.  sm_90a only -- there is no fallback path.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -22,6 +22,17 @@ __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint4 v) {
 }
 __device__ __forceinline__ void st_shared_f32(uint32_t addr, float v) {
     asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_f2(uint32_t addr, float2 v) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
+}
+__device__ __forceinline__ float2 ld_shared_f2(uint32_t addr) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+    return v;
 }
 __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
     uint4 v;
@@ -56,16 +67,24 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded wait: a protocol bug must trap (error return to the host), never hang the GPU box.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag) {
-    uint32_t spins = 0;
-    while (!mbar_try_wait(bar, parity)) {
-        if (++spins > (1u << 26)) {
-            printf("dd3d: mbarrier wait timeout tag=%d block=%d thread=%d parity=%u\n", tag, blockIdx.x, threadIdx.x,
-                   parity);
-            __trap();
-        }
-    }
+// Bounded wait: a protocol bug must trap (error return to the host), never hang the GPU.  ONE asm block, so the compiler sees
+// neither a branch nor a call: a C++ polling loop before a wgmma is a divergent path to ptxas, and a diagnostic printf is a
+// function call -- either makes it serialize the wgmma pipeline of the whole kernel.  Traps after 2^26 polls.  The labels are
+// local to the braces, so the block can be inlined any number of times.
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .u32 n;\n\t"
+        "mov.u32 n, 0;\n\t"
+        "WAIT:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra.uni DONE;\n\t"
+        "add.u32 n, n, 1;\n\t"
+        "setp.lt.u32 p, n, 67108864;\n\t"
+        "@p bra.uni WAIT;\n\t"
+        "trap;\n\t"
+        "DONE:\n\t}" ::"r"(smem_u32(bar)),
+        "r"(parity)
+        : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -117,163 +136,15 @@ __device__ __forceinline__ void tma_store_wait_read() {
 }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// tcgen05.commit: arrives (count 1) on `bar` once all previously issued MMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 inputs, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// ---------------------------------------------------------------- CTA pair (cta_group::2, cluster of 2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync() {  // all threads of both CTAs
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same smem location in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa(const void* smem, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(smem)), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA loads of a CTA pair: data lands in THIS CTA's smem, the transaction bytes are reported to the mbarrier at
-// `bar_cluster_addr`, which may live in the peer (leader) CTA.
-__device__ __forceinline__ void tma2_load_2d(void* smem, const void* map, uint32_t bar_cluster_addr, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-        "[%2];" ::"r"(smem_u32(smem)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void* smem, const void* map, uint32_t bar_cluster_addr, int c0, int c1,
-                                             int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], "
-        "[%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(smem)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tma2_load_5d(void* smem, const void* map, uint32_t bar_cluster_addr, int c0, int c1,
-                                             int c2, int c3, int c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], "
-        "[%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(smem_u32(smem)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_dst, uint32_t ncols) {  // one warp in EACH CTA of the pair
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// commit of the pair's MMAs: arrives on the barrier at the same smem offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit2(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(cta_mask)
-        : "memory");
-}
-// M = 256 over the CTA pair: each CTA supplies its 128 rows of A and half of the N rows of B; issued by the leader only
-__device__ __forceinline__ void umma2_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// K-major, 128-byte-swizzled operand tile: rows of 128 B (64 bf16), 8-row groups 1024 B apart.
-// Field layout = cute::UMMA::SmemDescriptor (start>>4 @0, LBO>>4 @16, SBO>>4 @32, version=1 @46, layout @61).
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>(1) << 16;            // LBO (unused for swizzled K-major; canonical value 1)
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;    // SBO: 8 rows * 128 B
-    d |= static_cast<uint64_t>(1) << 46;            // descriptor version (Blackwell)
-    d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
-    return d;
-}
-// kind::f16 instruction descriptor: D=f32 (bits 4-5 = 1), A / B format (bits 7-9 / 10-12: 0 = fp16, 1 = bf16), both
-// K-major, M=m, N=n.
-__host__ __device__ inline uint32_t make_idesc_f16(int m, int n, int fp16) {
-    const uint32_t fmt = fp16 ? 0u : 1u;
-    return (1u << 4) | (fmt << 7) | (fmt << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-           (static_cast<uint32_t>(m >> 4) << 24);
-}
-__host__ __device__ inline uint32_t make_idesc_bf16(int m, int n) { return make_idesc_f16(m, n, 0); }
-
-// TMEM -> registers: each lane of the warp reads its own TMEM lane (row), 32 / 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// Same, and makes every later use of v[] data-dependent on the wait (the registers are in/out operands of the asm), so the
-// compiler cannot schedule arithmetic on the loaded values above it.
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&v)[32]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]),
-                   "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]), "+r"(v[16]),
-                   "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]), "+r"(v[24]),
-                   "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-                 :
-                 : "memory");
+// ---------------------------------------------------------------- wgmma operand descriptors
+// K-major, 128-byte-swizzled operand tile: rows of 128 B (64 bf16), 8-row groups `sbo` bytes apart (1024 for a dense tile).
+// Field layout of the sm_90 matrix descriptor: start >> 4 @0, LBO >> 4 @16 (unused for swizzled K-major; canonical 1),
+// SBO >> 4 @32, layout @62 (1 = 128B swizzle).  The swizzle is a function of the absolute shared-memory address (TMA writes
+// the same pattern into 1024-byte-aligned slots), so a view may start at any 128-byte row of a tile and advancing the start
+// by 32 bytes steps K by 16.
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t sbo = 1024) {
+    return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF) | (static_cast<uint64_t>(1) << 16) |
+           (static_cast<uint64_t>(sbo >> 4) << 32) | (static_cast<uint64_t>(1) << 62);
 }
 
 }  // namespace ptx

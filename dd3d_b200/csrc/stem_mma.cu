@@ -2,10 +2,9 @@
 // as a register-fragment kernel.
 //
 // The layer is a pure streaming problem: 0.39 GB of normalised input in, 1.57 GB of 64-channel output out per 32-image batch
-// (0.30 ms at the HBM roof) around 75 GFLOP.  The tcgen05 form (stem_tc.cu) builds a K-major im2col tile in shared memory
-// per 128 pixels (thread-gathered, 9 predicated 8-byte loads + swizzled stores per pixel, then UMMA, then a TMEM round trip)
-// and ran at 1.09 ms = 1.8 TB/s.  Here a CTA copies the 17 x 66 input patch of an 8 x 32 output tile with cp.async (double
-// buffered), and every warp feeds mma.sync.m16n8k16 straight from it: one K step per kernel row, its 16 k slots = 4
+// around 75 GFLOP.  The wgmma form (stem_tc.cu) builds a K-major im2col tile in shared memory per 128 pixels
+// (thread-gathered, 9 predicated 8-byte loads + swizzled stores per pixel, then wgmma).  Here a CTA copies the 17 x 66
+// input patch of an 8 x 32 output tile with cp.async (double buffered), and every warp feeds mma.sync.m16n8k16 straight from it: one K step per kernel row, its 16 k slots = 4
 // consecutive input pixels x 4 channels (4th pixel / 4th channel carry zero weights), so lane t's fragment registers are ONE
 // 8-byte shared-memory load of input pixel 2x - 1 + t.  The 64 x 48 weight fragments stay in registers for the whole kernel.
 // Output channels are PERMUTED across the n-tiles (column j of n-tile nt = channel 16 (j / 2) + 2 nt + (j % 2)) so that the
@@ -40,7 +39,6 @@ struct StemParams {
     const float* sb;          // scale[64] | bias[64]
     __nv_bfloat16* out;       // [B][Ho][Wo][out_pitch]
     int B, H, W, Ho, Wo, out_pitch, tiles_x, tiles_y;
-    int wide_store;  // out is 32-byte aligned and out_pitch a multiple of 16 channels: 256-bit stores
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -175,15 +173,8 @@ __global__ void __launch_bounds__(kThreads, 2) stem_s2_mma_kernel(const StemPara
                 if (gy < p.Ho && gx < p.Wo) {
                     const uint32_t* o = h ? o_hi : o_lo;
                     __nv_bfloat16* dst = p.out + (static_cast<size_t>(b * p.Ho + gy) * p.Wo + gx) * p.out_pitch + 16 * t;
-                    if (p.wide_store) {
-                        // one 256-bit store per (pixel, lane): a whole 32-byte sector at once instead of two half-sector writes
-                        asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst), "r"(o[0]), "r"(o[1]), "r"(o[2]),
-                                     "r"(o[3]), "r"(o[4]), "r"(o[5]), "r"(o[6]), "r"(o[7])
-                                     : "memory");
-                    } else {
-                        reinterpret_cast<uint4*>(dst)[0] = make_uint4(o[0], o[1], o[2], o[3]);
-                        reinterpret_cast<uint4*>(dst)[1] = make_uint4(o[4], o[5], o[6], o[7]);
-                    }
+                    reinterpret_cast<uint4*>(dst)[0] = make_uint4(o[0], o[1], o[2], o[3]);
+                    reinterpret_cast<uint4*>(dst)[1] = make_uint4(o[4], o[5], o[6], o[7]);
                 }
             }
         }
@@ -202,7 +193,6 @@ cudaError_t launch_stem_s2_mma(const __nv_bfloat16* in4, const __nv_bfloat16* w,
     p.in = in4; p.w = w; p.sb = sb; p.out = out;
     p.B = B; p.H = H; p.W = W; p.Ho = (H + 1) / 2; p.Wo = (W + 1) / 2;
     p.out_pitch = out_pitch;
-    p.wide_store = (reinterpret_cast<uintptr_t>(out) % 32 == 0 && out_pitch % 16 == 0) ? 1 : 0;
     p.tiles_x = (p.Wo + TW - 1) / TW;
     p.tiles_y = (p.Ho + TH - 1) / TH;
     static uint64_t attr_devices[2] = {0, 0};

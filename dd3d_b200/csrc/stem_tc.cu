@@ -1,11 +1,12 @@
-// Stem convolutions (Cin = 3) on tcgen05 tensor cores.
+// Stem convolutions (Cin = 3) on Hopper tensor cores (wgmma).
 //
 // Replaces DLA `base_layer` (7x7 s1, 3->16, reference dla.py:271-280) and VoVNet `stem_1` (3x3 s2, 3->64,
 // vovnet.py:302) + FrozenBN + ReLU.  Cin=3 is too thin for TMA-fed implicit GEMM (a pixel is 8 bytes), so the CTA
 // builds the im2col tile itself: thread m gathers the KSxKS neighbourhood of output pixel m from the normalised
 // bf16 [B][H][W][4] image (4th channel = 0) and writes it as one K-major, 128B-swizzled operand row
-// (k = (ky*KS + kx)*4 + c), then ONE elected thread issues the UMMAs (M=128 pixels, N=Cout, K padded to 16) and the
-// same 128 threads run the epilogue from TMEM.  Several CTAs per SM overlap gather / MMA / epilogue of different tiles.
+// (k = (ky*KS + kx)*4 + c), then the warpgroup issues the wgmmas (two M = 64 halves of the 128 pixels, N = Cout, K padded
+// to 16) and runs the epilogue from its accumulator registers.  Several CTAs per SM overlap gather / MMA / epilogue of
+// different tiles.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -17,53 +18,34 @@
 #include "device_once.cuh"
 #include "ptx.cuh"
 #include "small_kernels.cuh"
+#include "wgmma.cuh"
 
 namespace dd3d {
 
 namespace {
 
 constexpr int kTileH = 8, kTileW = 16;  // 128 output pixels
+constexpr int kStemThreads = 128;       // one warpgroup
 
-__device__ __forceinline__ bool elect_one_stem() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-        "elect.sync rx|px, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, px;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-
-template <int KS, int STRIDE, int COUT>
-__global__ void __launch_bounds__(160) stem_tc_kernel(const __nv_bfloat16* __restrict__ in, const __nv_bfloat16* __restrict__ w,
-                                                      const float* __restrict__ scale, const float* __restrict__ bias,
-                                                      __nv_bfloat16* __restrict__ out, int B, int H, int W, int Ho, int Wo,
-                                                      int out_pitch, int tiles_x, int tiles_y, int fp16) {
+template <int KS, int STRIDE, int COUT, bool F16>
+__global__ void __launch_bounds__(kStemThreads) stem_tc_kernel(const __nv_bfloat16* __restrict__ in, const __nv_bfloat16* __restrict__ w,
+                                                               const float* __restrict__ scale, const float* __restrict__ bias,
+                                                               __nv_bfloat16* __restrict__ out, int B, int H, int W, int Ho, int Wo,
+                                                               int out_pitch, int tiles_x, int tiles_y) {
     constexpr int PAD = (KS - 1) / 2;
     constexpr int K = KS * KS * 4;            // 36 / 196
     constexpr int KB = (K + 63) / 64;         // 64-element k-blocks: 1 / 4
-    constexpr int KSTEPS = (K + 15) / 16;     // UMMA K=16 steps: 3 / 13
+    constexpr int KSTEPS = (K + 15) / 16;     // wgmma K=16 steps: 3 / 13
     constexpr int CHUNKS = (KS * KS + 1) / 2; // 16-byte chunks (2 taps each) per row that carry data
-    constexpr int TMEM_COLS = COUT < 32 ? 32 : COUT;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sA = smem;                     // [KB][128 rows][128 B]
     uint8_t* sB = smem + KB * 16384;        // [KB][COUT rows][128 B]
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_slot;
-    __shared__ __align__(16) float s_scale[COUT];  // folded BN, read as broadcast LDS.128 in the epilogue (128 scalar LDG
-    __shared__ __align__(16) float s_bias[COUT];   // per thread and tile before)
+    __shared__ __align__(16) float s_scale[COUT];  // folded BN, read as broadcast LDS in the epilogue
+    __shared__ __align__(16) float s_bias[COUT];
     const uint32_t sA_u32 = ptx::smem_u32(sA);     // explicit STS: the integer-aligned pointer would compile to generic ST.E
     const int tid = threadIdx.x;
-    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-    if (tid == 0) {
-        ptx::mbar_init(&bar, 1);
-        ptx::fence_barrier_init();
-    }
-    if (warp == 4) {
-        ptx::tmem_alloc(&tmem_slot, TMEM_COLS);
-        ptx::tmem_relinquish();
-    }
+    const int warp = tid >> 5, lane = tid & 31;
     // weights -> swizzled smem (global layout [COUT][KB*64] bf16, K contiguous)
     for (int i = tid; i < COUT * KB * 8; i += blockDim.x) {
         const int n = i / (KB * 8), q = i - n * (KB * 8);
@@ -71,34 +53,28 @@ __global__ void __launch_bounds__(160) stem_tc_kernel(const __nv_bfloat16* __res
         const uint4 v = __ldg(reinterpret_cast<const uint4*>(w + static_cast<size_t>(n) * KB * 64) + q);
         *reinterpret_cast<uint4*>(sB + kb * COUT * 128 + n * 128 + ((c ^ (n & 7)) << 4)) = v;
     }
-    if (tid < 128) {  // zero the K padding of the operand rows once (chunks >= CHUNKS never change)
-        for (int q = CHUNKS; q < KB * 8; ++q)
-            ptx::st_shared_v4(sA_u32 + (q >> 3) * 16384 + tid * 128 + (((q & 7) ^ (tid & 7)) << 4), make_uint4(0, 0, 0, 0));
-    }
+    // zero the K padding of the operand rows once (chunks >= CHUNKS never change)
+    for (int q = CHUNKS; q < KB * 8; ++q)
+        ptx::st_shared_v4(sA_u32 + (q >> 3) * 16384 + tid * 128 + (((q & 7) ^ (tid & 7)) << 4), make_uint4(0, 0, 0, 0));
     for (int i = tid; i < COUT; i += blockDim.x) {
         s_scale[i] = __ldg(scale + i);
         s_bias[i] = __ldg(bias + i);
     }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem = tmem_slot;
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-    const uint32_t idesc = ptx::make_idesc_f16(128, COUT, fp16);
-    constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);
-    const uint32_t a_lo = (ptx::smem_u32(sA) >> 4) | (1u << 16);
-    const uint32_t b_lo = (ptx::smem_u32(sB) >> 4) | (1u << 16);
+    const uint64_t desc_hi = ptx::make_sw128_desc(0) & ~0x3FFFull;
+    const uint32_t a_lo = ptx::smem_u32(sA) >> 4;
+    const uint32_t b_lo = ptx::smem_u32(sB) >> 4;
     const int total = B * tiles_x * tiles_y;
-    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
         const int b = tile / (tiles_x * tiles_y);
         const int r = tile - b * tiles_x * tiles_y;
         const int ty = r / tiles_x, tx = r - ty * tiles_x;
-        const int oy = ty * kTileH + (tid >> 4), ox = tx * kTileW + (tid & 15);  // valid for tid < 128
-        if (tid < 128) {
+        {
             // ---- im2col gather: one operand row per thread
+            const int oy = ty * kTileH + (tid >> 4), ox = tx * kTileW + (tid & 15);
             const int iy0 = oy * STRIDE - PAD, ix0 = ox * STRIDE - PAD;
             const __nv_bfloat16* img = in + static_cast<size_t>(b) * H * W * 4;
             // fully unrolled: all KS*KS predicated 8-byte loads are issued before the first use (memory-level
@@ -124,67 +100,43 @@ __global__ void __launch_bounds__(160) stem_tc_kernel(const __nv_bfloat16* __res
             ptx::fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
         }
         __syncthreads();
-        if (warp == 4) {
-            ptx::tc_fence_after();
-            if (elect_one_stem()) {
+        // ---- two M = 64 halves of the tile, N = COUT
+        float acc[2][COUT / 2];
+        wg::fence();
 #pragma unroll
-                for (int s = 0; s < KSTEPS; ++s) {
-                    const int kb = s >> 2, k = s & 3;
-                    const uint64_t adesc = (static_cast<uint64_t>(kDescHi) << 32) | (a_lo + kb * (16384 >> 4) + 2 * k);
-                    const uint64_t bdesc = (static_cast<uint64_t>(kDescHi) << 32) | (b_lo + kb * ((COUT * 128) >> 4) + 2 * k);
-                    ptx::umma_bf16(tmem, adesc, bdesc, idesc, s > 0 ? 1u : 0u);
-                }
-                ptx::umma_commit(&bar);
+        for (int m = 0; m < 2; ++m) {
+#pragma unroll
+            for (int s = 0; s < KSTEPS; ++s) {
+                const int kb = s >> 2, k = s & 3;
+                const uint64_t adesc = desc_hi | (a_lo + kb * (16384 >> 4) + m * (64 * 128 >> 4) + 2 * k);
+                const uint64_t bdesc = desc_hi | (b_lo + kb * ((COUT * 128) >> 4) + 2 * k);
+                wg::wgmma<COUT, F16>(acc[m], adesc, bdesc, s > 0 ? 1u : 0u);
             }
-            __syncwarp();
-        } else {
-            // ---- epilogue: TMEM -> scale/bias/ReLU -> bf16 -> global (thread m = pixel m)
-            ptx::mbar_wait(&bar, phase, 9);
-            ptx::tc_fence_after();
-            const uint32_t t_addr = tmem + (static_cast<uint32_t>(warp * 32) << 16);
-            const bool ok = (oy < Ho) && (ox < Wo);
-            __nv_bfloat16* dst = out + (static_cast<size_t>(b * Ho + oy) * Wo + ox) * out_pitch;
+        }
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs(acc[0]);
+        wg::fence_regs(acc[1]);
+        // ---- epilogue: scale/bias/ReLU -> bf16 -> global.  d[4j + 2h + e] = (row 16 warp + lane/4 + 8h, col 8j + 2(lane%4) + e)
 #pragma unroll
-            for (int c0 = 0; c0 < COUT; c0 += 32) {
-                uint32_t v[32];
-                if (COUT - c0 >= 32) {
-                    ptx::tmem_ld32(t_addr + c0, v);
-                } else {
-                    ptx::tmem_ld16(t_addr + c0, v);
-                }
-                ptx::tmem_ld_wait();
-                constexpr int cols = (COUT >= 32) ? 32 : 16;
-                if (ok) {
+        for (int m = 0; m < 2; ++m) {
 #pragma unroll
-                    for (int i = 0; i < cols; i += 8) {
-                        uint32_t o[4];
+            for (int h = 0; h < 2; ++h) {
+                const int pix = 64 * m + 16 * warp + (lane >> 2) + 8 * h;
+                const int oy = ty * kTileH + (pix >> 4), ox = tx * kTileW + (pix & 15);
+                if (oy < Ho && ox < Wo) {
+                    __nv_bfloat16* dst = out + (static_cast<size_t>(b * Ho + oy) * Wo + ox) * out_pitch + 2 * (lane & 3);
 #pragma unroll
-                        const float4 sc0 = *reinterpret_cast<const float4*>(s_scale + c0 + i);
-                        const float4 sc1 = *reinterpret_cast<const float4*>(s_scale + c0 + i + 4);
-                        const float4 bi0 = *reinterpret_cast<const float4*>(s_bias + c0 + i);
-                        const float4 bi1 = *reinterpret_cast<const float4*>(s_bias + c0 + i + 4);
-                        const float scv[8] = {sc0.x, sc0.y, sc0.z, sc0.w, sc1.x, sc1.y, sc1.z, sc1.w};
-                        const float biv[8] = {bi0.x, bi0.y, bi0.z, bi0.w, bi1.x, bi1.y, bi1.z, bi1.w};
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const float y0 = fmaxf(fmaf(__uint_as_float(v[i + 2 * j]), scv[2 * j], biv[2 * j]), 0.f);
-                            const float y1 = fmaxf(fmaf(__uint_as_float(v[i + 2 * j + 1]), scv[2 * j + 1], biv[2 * j + 1]), 0.f);
-                            o[j] = pack2_act(y0, y1, fp16);
-                        }
-                        *reinterpret_cast<uint4*>(dst + c0 + i) = make_uint4(o[0], o[1], o[2], o[3]);
+                    for (int j = 0; j < COUT / 8; ++j) {
+                        const int col = 8 * j + 2 * (lane & 3);
+                        const float y0 = fmaxf(fmaf(acc[m][4 * j + 2 * h], s_scale[col], s_bias[col]), 0.f);
+                        const float y1 = fmaxf(fmaf(acc[m][4 * j + 2 * h + 1], s_scale[col + 1], s_bias[col + 1]), 0.f);
+                        *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2_act(y0, y1, F16 ? 1 : 0);
                     }
                 }
             }
-            ptx::tc_fence_before();
         }
-        phase ^= 1;
-        __syncthreads();  // TMEM drained and operand tile consumed before the next tile overwrites them
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 4) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem, TMEM_COLS);
+        __syncthreads();  // operand tile consumed before the next tile overwrites it
     }
 }
 
@@ -199,7 +151,9 @@ cudaError_t launch_one(const __nv_bfloat16* in, const __nv_bfloat16* w, const fl
     const int smem = KB * 16384 + KB * COUT * 128 + 1024;
     static uint64_t attr_devices = 0;  // per template instantiation, per device
     if (first_use_on_device(&attr_devices)) {
-        cudaError_t e = cudaFuncSetAttribute(stem_tc_kernel<KS, STRIDE, COUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        cudaError_t e = cudaFuncSetAttribute(stem_tc_kernel<KS, STRIDE, COUT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(stem_tc_kernel<KS, STRIDE, COUT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return e;
     }
     const int ctas_per_sm = std::max(1, std::min(4, (200 * 1024) / smem));
@@ -207,7 +161,7 @@ cudaError_t launch_one(const __nv_bfloat16* in, const __nv_bfloat16* w, const fl
     const int grid = std::min(total, num_sms * ctas_per_sm);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(160);
+    cfg.blockDim = dim3(kStemThreads);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
@@ -215,8 +169,10 @@ cudaError_t launch_one(const __nv_bfloat16* in, const __nv_bfloat16* w, const fl
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, stem_tc_kernel<KS, STRIDE, COUT>, in, w, scale, bias, out, B, H, W, Ho, Wo, out_pitch,
-                              tiles_x, tiles_y, fp16);
+    return fp16 ? cudaLaunchKernelEx(&cfg, stem_tc_kernel<KS, STRIDE, COUT, true>, in, w, scale, bias, out, B, H, W, Ho, Wo,
+                                     out_pitch, tiles_x, tiles_y)
+                : cudaLaunchKernelEx(&cfg, stem_tc_kernel<KS, STRIDE, COUT, false>, in, w, scale, bias, out, B, H, W, Ho, Wo,
+                                     out_pitch, tiles_x, tiles_y);
 }
 
 }  // namespace

@@ -4,7 +4,7 @@ Same constructor and call contract as ``tridet.modeling.dd3d.core.DD3D`` (core.p
 ``DD3DB200(cfg)``, ``.to(device)``, ``load_state_dict(reference_state_dict)``,
 ``forward(batched_inputs: list[dict]) -> list[{"instances": Instances}]`` with the attributes callers toggle
 (``postprocess_in_inference``, ``do_nms``, ``only_box2d``, ``num_classes``, ``device``,
-``backbone.size_divisibility``).  All arithmetic runs in libdd3d_b200.so (hand-written sm_100a kernels) through the
+``backbone.size_divisibility``).  All arithmetic runs in libdd3d_b200.so (hand-written sm_90a kernels for the H100) through the
 C ABI in include/dd3d_b200.h; torch is used for device memory and streams only.  No CPU fallback exists.
 """
 import ctypes as C
@@ -110,7 +110,7 @@ class DD3DB200(nn.Module):
         if self._state is None:
             raise RuntimeError("DD3DB200: load_state_dict() must be called before forward()")
         if self._device.type != "cuda":
-            raise RuntimeError("DD3DB200 runs on CUDA sm_100a only (model.to('cuda')); there is no CPU path")
+            raise RuntimeError("DD3DB200 runs on CUDA sm_90a (H100) only (model.to('cuda')); there is no CPU path")
         L = _lib.load()
         # pixel mean/std travel in the state_dict like in the reference (core.py:54-55)
         for i in range(3):

@@ -1,5 +1,5 @@
 /*
- * dd3d_b200 -- C ABI of the B200-native DD3D inference path.
+ * dd3d_b200 -- C ABI of the H100-native (sm_90a) DD3D inference path.
  *
  * Drop-in boundary for ONE reference call: the eval-mode DD3D.forward()
  *   /root/reference/tridet/modeling/dd3d/core.py:64-164
@@ -166,8 +166,6 @@ int dd3d_overflow_flags(dd3d_handle h, dd3d_stream stream, int32_t* h_flags);
  * the poison test of tests/test_determinism_gpu.py: results must not depend on what the arena held). */
 int dd3d_set_option(dd3d_handle h, const char* name, int value);
 /* Process-wide kernel-selection policy for plans / operator calls made afterwards (tests, A/B measurements):
- * "cta2" = 0 single-CTA conv kernel everywhere, 1 CTA pairs (tcgen05.mma.cta_group::2) wherever legal, 2 auto (default:
- * pairs for block_n >= 160 and >= 296 tiles), -1 back to the DD3D_CONV_CTA2 environment setting.
  * "op_fp16" = 1: the dd3d_op_* entry points below treat their 16-bit buffers as fp16 (default 0: bf16).
  * "nms_class_parallel" = 0: one CTA per image does the whole NMS instead of the multi-CTA path (rank sort, IoU bit matrix on
  * all SMs, one scan CTA per (class, image), finish; default 1; same kept set and order).
@@ -182,7 +180,7 @@ int dd3d_launches_per_forward(dd3d_handle h);
 
 /* Per-category device time of the LAST dd3d_forward issued with option "profile" = 1 (CUDA events recorded on the
  * launch stream around every op), with the algorithmic FLOPs / HBM bytes and launch counts of one forward.
- * Categories (arrays of 8): 0 preprocess, 1 stem conv, 2 tcgen05 implicit-GEMM conv, 3 max-pool, 4 eSE, 5 relu,
+ * Categories (arrays of 8): 0 preprocess, 1 stem conv, 2 wgmma implicit-GEMM conv, 3 max-pool, 4 eSE, 5 relu,
  * 6 decode, 7 NMS. */
 int dd3d_get_profile(dd3d_handle h, double* h_ms, double* h_flops, double* h_bytes, int32_t* h_launches);
 /* Same events, per op in launch order (entry 0 = preprocess, then every engine op, then decode, NMS): device ms,
@@ -246,7 +244,7 @@ int dd3d_num_ops(dd3d_handle h);
 /* dd3d_op_stem_conv: Cin=3 stem conv on tensor cores; d_in4 = bf16 [B][H][W][4] (dd3d_op_preprocess output), d_w =
  * bf16 [cout][kpad] with k = (ky*ksize + kx)*4 + c, kpad = ksize*ksize*4 rounded up to 64; (ksize, stride, cout) in
  * {(7,1,16), (3,2,64)}. */
-/* NHWC bf16 conv via the tcgen05 implicit-GEMM kernel.  d_w: bf16 [cout_pad][ksize*ksize][cin_pad64];
+/* NHWC bf16 conv via the wgmma implicit-GEMM kernel.  d_w: bf16 [cout_pad][ksize*ksize][cin_pad64];
  * d_scale/d_bias: fp32 [cout_pad]; d_residual (optional) NHWC bf16 with res_pitch channels, res_up2: residual is
  * the 2x coarser map; out: bf16 (out_f32 == 0, pitch out_pitch) or fp32. */
 int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout, int ksize,

@@ -16,7 +16,7 @@ the reference's OWN modules executed in the build container under oracle/ref_sta
 runs produced (tests/golden/*.npz, written by oracle/gen_golden.py).  The third-party pieces themselves remain
 "parity unpinned" upstream (no pinned versions in the reference's Dockerfile) -- see DESIGN.md.
 
-``emulate="bf16" | "fp16"`` (``emulate_bf16=True``) reproduces the B200 engine's storage precision: conv weights
+``emulate="bf16" | "fp16"`` (``emulate_bf16=True``) reproduces the CUDA engine's storage precision: conv weights
 and every stored activation are rounded to that 16-bit type at the points where the engine stores it (after each conv
 epilogue, after eSE scaling, after preprocessing); accumulation, BN affine, predictors' outputs, decode and NMS stay
 fp32.  ``threads=1`` makes that emulation reproducible across processes (VERDICT r1 weak #4).

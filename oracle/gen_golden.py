@@ -185,9 +185,77 @@ def gen_dd3d_goldens(names, out_dir):
         np.savez_compressed(os.path.join(out_dir, f"golden_{arch}.npz"), **blob)
 
 
+def inventory_digest(shapes):
+    """SHA-256 over the sorted (parameter name, shape) pairs of a state_dict."""
+    import hashlib
+    text = "\n".join(f"{k}:{','.join(str(int(d)) for d in shapes[k])}" for k in sorted(shapes))
+    return hashlib.sha256(text.encode()).hexdigest()
+
+
+def gen_live_reference_goldens(out_dir):
+    """reference_live.npz / reference_live.json: what the comparisons of the CPU tests read from the reference itself --
+    its composed experiment configs, its parameter inventories and its forward on the seeded 128x256 case (default heads,
+    the decode flags and the head configurations of tests/test_cpu_oracle.py), its BEV NMS / sample aggregation on the
+    seeded cases of tests/test_bev_nms.py / tests/test_nuscenes.py and its intrinsics rescale."""
+    import json
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from hydra_lite import compose_experiment
+    from test_config_vs_reference import EXPERIMENTS
+    from test_cpu_oracle import FLAG_CASES, HEAD_CASES, apply_flags, apply_head_flags, case_key
+    from test_bev_nms import _random_case
+    from test_nuscenes import aggregate_case
+    ref_standin.install()
+    meta = {"configs": {e: compose_experiment(os.path.join(ref_standin.REFERENCE_ROOT, "configs"), e) for e, _ in EXPERIMENTS},
+            "inventory": {}}
+    blob = {}
+
+    def forward_case(key, cfg):
+        model = ref_standin.build_reference_model(cfg).eval()
+        meta["inventory"][key] = inventory_digest({k: tuple(v.shape) for k, v in model.state_dict().items()})
+        model.load_state_dict(make_state_dict(cfg))
+        with torch.no_grad():
+            inst = model(make_inputs(1, 128, 256, 721.5, seed_base=7))[0]["instances"]
+        blob.update({f"{key}/boxes": inst.pred_boxes.tensor.numpy(), f"{key}/scores": inst.scores.numpy(),
+                     f"{key}/classes": inst.pred_classes.numpy(), f"{key}/levels": inst.fpn_levels.numpy(),
+                     f"{key}/locations": inst.locations.numpy()})
+        if inst.has("pred_boxes3d"):
+            b3 = inst.pred_boxes3d
+            blob.update({f"{key}/scores_3d": inst.scores_3d.numpy(), f"{key}/quat": b3.quat.numpy(),
+                         f"{key}/depth": b3.depth.reshape(-1).numpy(), f"{key}/size": b3.size.numpy(),
+                         f"{key}/tvec": b3.tvec.numpy()})
+        print("live reference case", key, "detections", len(inst))
+
+    for arch in ("dla34", "v2_99"):
+        forward_case(arch, get_cfg(arch, CASES[arch][0]))
+    for flags in FLAG_CASES:
+        cfg = apply_flags(get_cfg("dla34", "kitti_3d"), flags)
+        cfg.DD3D.FCOS2D.INFERENCE.PRE_NMS_THRESH = 0.03
+        forward_case(case_key("flags", flags), cfg)
+    for flags in HEAD_CASES:
+        cfg = apply_head_flags(get_cfg("dla34", "kitti_3d"), flags)
+        cfg.DD3D.FCOS2D.INFERENCE.PRE_NMS_THRESH = 0.03
+        forward_case(case_key("head", flags), cfg)
+    for c in range(4):
+        det, pq, pt = _random_case(7 + c, 40 + 5 * c)
+        blob[f"bev{c}/keep"] = reference_bev_keep(det, pq, pt, 0.3)[0].numpy()
+    dets, gids, poses = aggregate_case(3)
+    for i, (keep, _, _) in enumerate(reference_sample_aggregate(dets, gids, poses, 0.3, 200)):
+        blob[f"aggregate/keep{i}"] = keep.numpy()
+    from tridet.data.augmentations.resize_transform import ResizeTransform
+    K = np.float32([[1266.4, 0, 816.3], [0, 1266.4, 491.5], [0, 0, 1]])
+    for c, ((h, w), (nh, nw)) in enumerate([((900, 1600), (896, 1593)), ((375, 1242), (384, 1272))]):
+        blob[f"intrinsics{c}"] = ResizeTransform(h, w, nh, nw).apply_intrinsics(K)
+    np.savez_compressed(os.path.join(out_dir, "reference_live.npz"), **blob)
+    with open(os.path.join(out_dir, "reference_live.json"), "w") as f:
+        json.dump(meta, f, sort_keys=True, separators=(",", ":"))
+
+
 def main():
     out_dir = os.path.join(ROOT, "tests", "golden")
     os.makedirs(out_dir, exist_ok=True)
+    if "--live" in sys.argv:  # only the fixtures of the former live-reference comparisons
+        gen_live_reference_goldens(out_dir)
+        return
     if "--full" in sys.argv:  # only the BASELINE-shape cases (a V2-99 900x1600 reference forward takes ~10 s here)
         gen_dd3d_goldens(list(FULL_CASES), out_dir)
         return
@@ -291,6 +359,7 @@ def main():
              depth_in=depth.numpy(), size_in=size.numpy(), loc=loc.numpy(), canon=canon.numpy(), quat=b3.quat.numpy(),
              proj_ctr=b3.proj_ctr.numpy(), depth=b3.depth.numpy(), size=b3.size.numpy(), tvec=b3.tvec.numpy())
     print("KAT quat", b3.quat.numpy(), "tvec", b3.tvec.numpy())
+    gen_live_reference_goldens(out_dir)
 
 
 if __name__ == "__main__":

@@ -6,12 +6,11 @@ import pytest
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, os.path.abspath(ROOT))
 
-REFERENCE_ROOT = "/root/reference"
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA sm_100a device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA sm_90a (H100) device")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -27,7 +26,3 @@ def pytest_collection_modifyitems(config, items):
         if "gpu" in item.keywords:
             item.add_marker(skip)
 
-
-@pytest.fixture(scope="session")
-def have_reference():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "tridet"))

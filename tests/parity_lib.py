@@ -1,5 +1,5 @@
-"""Measured end-to-end parity of the B200 engine against the CPU oracle (shared by tests/test_parity_full_gpu.py, which
-asserts thresholds, and tools/parity_report.py, which writes the measured numbers to profiles/parity_r02.json).
+"""Measured end-to-end parity of the CUDA engine against the CPU oracle (shared by tests/test_parity_full_gpu.py, which
+asserts thresholds, and tools/parity_report.py, which writes the measured numbers as JSON).
 
 For one seeded case (oracle/gen_golden.py: small ragged cases and the BASELINE.json shapes 1 x 384x1280 DLA-34 /
 1 x 900x1600 V2-99) and one storage type (bf16 / fp16) it measures, all through the C ABI:
@@ -192,7 +192,7 @@ def measure_case(name, dtype, emu_threads=1, want_fp32=True):
     B = len(inputs)
     rep = dict(case=name, dtype=dtype, images=B)
     # sparse vs dense predictor: same detections in the same order; the 3-D fields differ only by the fp32 summation order
-    # of the two tensor paths (mma.sync vs tcgen05) over K = 2304
+    # of the two tensor paths (mma.sync vs wgmma) over K = 2304
     sv = dict(same_keys_and_order=True, n=0, max_err={f: 0.0 for f in FIELDS})
     for b in range(B):
         d_, s_ = dets_from_instances(out[b]["instances"]), sparse_dets[b]

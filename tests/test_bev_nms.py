@@ -100,14 +100,13 @@ def test_bev_oracle_matches_golden():
         np.testing.assert_allclose(B.boxes3d_to_rotated_boxes(q, t, det["size"]).numpy(), g[f"rot{c}"], rtol=1e-4, atol=1e-4)
 
 
-def test_bev_oracle_vs_live_reference(have_reference):
-    if not have_reference:
-        pytest.skip("/root/reference not present: covered by tests/golden/bev_nms.npz")
-    from oracle.gen_golden import reference_bev_keep
+def test_bev_oracle_vs_live_reference():
+    """The reference's own BEV NMS keep lists on four more seeded cases (tests/golden/reference_live.npz)."""
+    g = np.load(os.path.join(GOLDEN_DIR, "reference_live.npz"))
     for c in range(4):
         det, pq, pt = _random_case(7 + c, 40 + 5 * c)
-        keep_ref, _ = reference_bev_keep(det, pq, pt, 0.3)
-        assert torch.equal(B.bev_nms_image(det, pq, pt, 0.3), keep_ref)
+        keep_ref = torch.as_tensor(g[f"bev{c}/keep"])
+        assert torch.equal(B.bev_nms_image(det, pq, pt, 0.3), keep_ref.to(torch.long))
 
 
 # ------------------------------------------------------------------------------------------------ GPU

@@ -1,5 +1,6 @@
 """CPU suite (-m "not gpu"): pins the oracle against the reference's golden vectors / the reference itself, checks
 the host logic and that the C-ABI library loads and exports every declared symbol."""
+import json
 import os
 import re
 
@@ -7,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN_DIR, REFERENCE_ROOT
+from conftest import GOLDEN_DIR
 from dd3d_b200.arch import param_specs
 from dd3d_b200.config import get_cfg
 from dd3d_b200.synthetic import make_inputs, make_state_dict
@@ -101,31 +102,35 @@ def test_bf16_emulation_stays_close_to_fp32():
         assert (x["score3d"][ia] - y["score3d"][ib]).abs().max() < 0.05
 
 
-# ------------------------------------------------------------------------------------------------ vs live reference
+# ------------------------------------------------------------------------------------------------ vs the reference's forward
+# tests/golden/reference_live.{npz,json} (oracle/gen_golden.py --live): the reference's parameter inventory (SHA-256 of its
+# sorted (name, shape) pairs) and its fp32 forward on the seeded 128x256 case, per configuration.
+def _live(key):
+    with open(os.path.join(GOLDEN_DIR, "reference_live.json")) as f:
+        digest = json.load(f)["inventory"][key]
+    g = np.load(os.path.join(GOLDEN_DIR, "reference_live.npz"))
+    return digest, {k.split("/", 1)[1]: torch.as_tensor(g[k]) for k in g.files if k.startswith(key + "/")}
+
+
+def _check_inventory(cfg, digest):
+    from oracle.gen_golden import inventory_digest
+    assert inventory_digest({k: shape for k, (shape, _) in param_specs(cfg).items()}) == digest, "parameter inventory differs"
+
+
 @pytest.mark.parametrize("arch", ["dla34", "v2_99"])
-def test_inventory_and_oracle_vs_live_reference(arch, have_reference):
-    if not have_reference:
-        pytest.skip("/root/reference not present (GPU box): covered by the committed golden fixtures")
-    from oracle import ref_standin
+def test_inventory_and_oracle_vs_live_reference(arch):
     cfg = get_cfg(arch, CASES[arch][0])
-    model = ref_standin.build_reference_model(cfg).eval()
-    ref_sd = model.state_dict()
-    specs = param_specs(cfg)
-    assert set(ref_sd.keys()) == set(specs.keys())
-    for k, (shape, _) in specs.items():
-        assert tuple(ref_sd[k].shape) == tuple(shape), k
+    digest, ref = _live(arch)
+    _check_inventory(cfg, digest)
     sd = make_state_dict(cfg)
-    model.load_state_dict(sd)
     inputs = make_inputs(1, 128, 256, 721.5, seed_base=7)
-    with torch.no_grad():
-        ref = model(inputs)[0]["instances"]
     out = DD3DOracle(cfg, sd).forward(inputs)[0]
-    assert len(ref) == out["box2d"].shape[0]
-    if len(ref):
-        assert (ref.pred_boxes.tensor - out["box2d"]).abs().max() < 1e-3
-        assert (ref.scores_3d - out["score3d"]).abs().max() < 1e-5
-        assert quat_dist(ref.pred_boxes3d.quat, out["quat"]).max() < 1e-4
-        assert (ref.pred_boxes3d.tvec - out["tvec"]).abs().max() < 1e-3
+    assert ref["boxes"].shape[0] == out["box2d"].shape[0]
+    if ref["boxes"].shape[0]:
+        assert (ref["boxes"] - out["box2d"]).abs().max() < 1e-3
+        assert (ref["scores_3d"] - out["score3d"]).abs().max() < 1e-5
+        assert quat_dist(ref["quat"], out["quat"]).max() < 1e-4
+        assert (ref["tvec"] - out["tvec"]).abs().max() < 1e-3
 
 
 FLAG_CASES = [
@@ -135,6 +140,11 @@ FLAG_CASES = [
     dict(SCALE_DEPTH_BY_FOCAL_LENGTHS=False),
     dict(FEATURE_LOCATIONS_OFFSET="half", PREDICT_DISTANCE=True, PREDICT_ALLOCENTRIC_ROT=False),
 ]
+
+
+def case_key(kind, flags):
+    """Name of a case in tests/golden/reference_live.npz."""
+    return kind + ":" + "+".join(f"{k}={v}" for k, v in flags.items())
 
 
 def apply_flags(cfg, flags):
@@ -147,28 +157,22 @@ def apply_flags(cfg, flags):
 
 
 @pytest.mark.parametrize("flags", FLAG_CASES, ids=lambda f: "+".join(f))
-def test_oracle_decode_flags_vs_live_reference(flags, have_reference):
+def test_oracle_decode_flags_vs_live_reference(flags):
     """The non-default decode switches the reference reads (core.py:38, fcos3d.py:36-47,306-312): feature-location offset
     "half", PREDICT_DISTANCE, egocentric quaternions, no focal-length depth scaling -- oracle == the reference's forward."""
-    if not have_reference:
-        pytest.skip("/root/reference not present (GPU box)")
-    from oracle import ref_standin
     cfg = apply_flags(get_cfg("dla34", "kitti_3d"), flags)
     cfg.DD3D.FCOS2D.INFERENCE.PRE_NMS_THRESH = 0.03
-    model = ref_standin.build_reference_model(cfg).eval()
+    _, ref = _live(case_key("flags", flags))
     sd = make_state_dict(cfg)
-    model.load_state_dict(sd)
     inputs = make_inputs(1, 128, 256, 721.5, seed_base=7)
-    with torch.no_grad():
-        ref = model(inputs)[0]["instances"]
     out = DD3DOracle(cfg, sd).forward(inputs)[0]
-    assert len(ref) == out["box2d"].shape[0] > 5
-    assert (ref.pred_boxes.tensor - out["box2d"]).abs().max() < 1e-3
-    assert (ref.locations - out["loc"]).abs().max() == 0
-    assert (ref.scores_3d - out["score3d"]).abs().max() < 1e-5
-    assert quat_dist(ref.pred_boxes3d.quat, out["quat"]).max() < 1e-4
-    assert (ref.pred_boxes3d.depth.reshape(-1) - out["depth"]).abs().max() < 1e-3
-    assert (ref.pred_boxes3d.tvec - out["tvec"]).abs().max() < 1e-3
+    assert ref["boxes"].shape[0] == out["box2d"].shape[0] > 5
+    assert (ref["boxes"] - out["box2d"]).abs().max() < 1e-3
+    assert (ref["locations"] - out["loc"]).abs().max() == 0
+    assert (ref["scores_3d"] - out["score3d"]).abs().max() < 1e-5
+    assert quat_dist(ref["quat"], out["quat"]).max() < 1e-4
+    assert (ref["depth"] - out["depth"]).abs().max() < 1e-3
+    assert (ref["tvec"] - out["tvec"]).abs().max() < 1e-3
 
 
 HEAD_CASES = [  # head configurations no shipped experiment uses (VERDICT r1 missing #2)
@@ -199,39 +203,29 @@ def apply_head_flags(cfg, flags):
 
 
 @pytest.mark.parametrize("flags", HEAD_CASES, ids=lambda f: "+".join(f))
-def test_oracle_head_configs_vs_live_reference(flags, have_reference):
+def test_oracle_head_configs_vs_live_reference(flags):
     """THRESH_WITH_CTR False (fcos2d.py:280-290), USE_SCALE False (fcos2d.py:100-108,145-152; fcos3d.py:116,128-139,175-180),
     CLASS_AGNOSTIC_BOX3D (fcos3d.py:103,333-352), PER_LEVEL_PREDICTORS (fcos3d.py:104,166), BOX3D_ON False (core.py:34-40,
     117-125): the parameter inventory equals the reference's state_dict and the oracle equals the reference's forward."""
-    if not have_reference:
-        pytest.skip("/root/reference not present (GPU box)")
-    from oracle import ref_standin
     cfg = apply_head_flags(get_cfg("dla34", "kitti_3d"), flags)
     cfg.DD3D.FCOS2D.INFERENCE.PRE_NMS_THRESH = 0.03
-    model = ref_standin.build_reference_model(cfg).eval()
-    specs = param_specs(cfg)
-    ref_sd = model.state_dict()
-    assert set(ref_sd.keys()) == set(specs.keys()), set(ref_sd.keys()) ^ set(specs.keys())
-    for k, (shape, _) in specs.items():
-        assert tuple(ref_sd[k].shape) == tuple(shape), k
+    digest, ref = _live(case_key("head", flags))
+    _check_inventory(cfg, digest)
     sd = make_state_dict(cfg)
-    model.load_state_dict(sd)
     inputs = make_inputs(1, 128, 256, 721.5, seed_base=7)
-    with torch.no_grad():
-        ref = model(inputs)[0]["instances"]
     out = DD3DOracle(cfg, sd).forward(inputs)[0]
-    assert len(ref) == out["box2d"].shape[0] > 5
-    assert (ref.pred_boxes.tensor - out["box2d"]).abs().max() < 1e-3
-    assert (ref.scores - out["score"]).abs().max() < 1e-5
-    assert torch.equal(ref.pred_classes, out["cls"]) and torch.equal(ref.fpn_levels, out["level"])
+    assert ref["boxes"].shape[0] == out["box2d"].shape[0] > 5
+    assert (ref["boxes"] - out["box2d"]).abs().max() < 1e-3
+    assert (ref["scores"] - out["score"]).abs().max() < 1e-5
+    assert torch.equal(ref["classes"], out["cls"]) and torch.equal(ref["levels"], out["level"])
     if cfg.MODEL.BOX3D_ON:
-        assert (ref.scores_3d - out["score3d"]).abs().max() < 1e-5
-        assert quat_dist(ref.pred_boxes3d.quat, out["quat"]).max() < 1e-4
-        assert (ref.pred_boxes3d.depth.reshape(-1) - out["depth"]).abs().max() < 1e-3
-        assert ((ref.pred_boxes3d.size - out["size"]).abs() / out["size"].abs().clamp(min=1e-3)).max() < 1e-4
-        assert (ref.pred_boxes3d.tvec - out["tvec"]).abs().max() < 1e-3
+        assert (ref["scores_3d"] - out["score3d"]).abs().max() < 1e-5
+        assert quat_dist(ref["quat"], out["quat"]).max() < 1e-4
+        assert (ref["depth"] - out["depth"]).abs().max() < 1e-3
+        assert ((ref["size"] - out["size"]).abs() / out["size"].abs().clamp(min=1e-3)).max() < 1e-4
+        assert (ref["tvec"] - out["tvec"]).abs().max() < 1e-3
     else:
-        assert not ref.has("pred_boxes3d") and not ref.has("scores_3d")
+        assert "scores_3d" not in ref and "quat" not in ref
 
 
 # ------------------------------------------------------------------------------------------------ host logic / ABI

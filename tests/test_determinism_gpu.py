@@ -5,7 +5,7 @@
  * processes: two fresh processes (one of them with programmatic dependent launch disabled) produce identical hashes of
    every stage (tools/determinism_probe.py).
 compute-sanitizer's initcheck cannot replace the poison test: it does not track global memory written by TMA stores
-(cp.async.bulk.tensor), so it reports every read of a conv output as uninitialised (profiles/r02_determinism.md)."""
+(cp.async.bulk.tensor), so it reports every read of a conv output as uninitialised."""
 import ctypes as C
 import json
 import os

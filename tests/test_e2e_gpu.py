@@ -1,6 +1,6 @@
-"""End-to-end parity (-m gpu): DD3DB200.forward (C ABI -> sm_100a kernels) vs the CPU oracle on identical inputs.
+"""End-to-end parity (-m gpu): DD3DB200.forward (C ABI -> sm_90a kernels) vs the CPU oracle on identical inputs.
 
-Tolerances (see DESIGN.md "Numerics"; thresholds = the measured values of profiles/parity_r02.json x ~2): the engine
+Tolerances (see DESIGN.md "Numerics"; thresholds = the measured values of tools/parity_report.py x ~2): the engine
 stores activations in bf16, so it is compared
   (a) with the oracle run in bf16-storage emulation on ONE thread (same rounding points; differences come only from fp32
       accumulation order -> isolated 1-ulp bf16 flips): relative L2 error of every FPN / head map <= 1e-2 / 1.5e-2 (measured
@@ -323,7 +323,7 @@ def test_conv_n_split_is_bit_identical(arch):
 
 
 def test_v2_99_stem_mma_matches_stem_tc():
-    """VoVNet stem_1 on the register-fragment kernel (csrc/stem_mma.cu, default) against the tcgen05 im2col kernel
+    """VoVNet stem_1 on the register-fragment kernel (csrc/stem_mma.cu, default) against the wgmma im2col kernel
     (csrc/stem_tc.cu, engine option "stem_mma" = 0) inside the engine: same FPN maps up to isolated 1-ulp flips of the stem's
     16-bit outputs (different fp32 summation order), amplified like any other rounding by the random-weight network."""
     cfg, sd, model = _model("v2_99")

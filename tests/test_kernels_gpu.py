@@ -275,7 +275,7 @@ def test_dla_front_fused(B, H, W, out_pitch, pool_pitch, act):
     d = (out[..., :32].float() - a2.float()).abs()
     tol = (2.0**-10 if act == "fp16" else 2.0**-7) * a2.float().abs() + (3e-3 if act == "fp16" else 2e-2)
     assert not (d > tol).any(), f"fused vs layer-by-layer: max diff {float(d.max()):.4f}"
-    # accumulation order differs (mma.sync vs tcgen05), so equality is not exact, but nearly all elements agree bit for bit
+    # accumulation order differs (mma.sync vs wgmma), so equality is not exact, but nearly all elements agree bit for bit
     assert float((d == 0).float().mean()) > 0.9
 
 
@@ -538,39 +538,6 @@ def test_conv_taps_in_n_matches_per_tap_kernel(cin, cout, H, W, B, f32, act):
     else:
         _check_bf16(outs[0], ref, "taps-in-N 16-bit output")
         assert (a != b).float().mean().item() < 2e-3  # isolated 1-ulp storage flips only
-
-
-@pytest.mark.parametrize("cin,cout,k,stride,H,W,B,relu,res", CONV_CASES)
-def test_conv_cta_pair_bitwise_equals_single_cta(cin, cout, k, stride, H, W, B, relu, res):
-    """The CTA-pair kernel (tcgen05.mma.cta_group::2, M = 256, half weight tile per CTA) accumulates every output in the
-    same K order as the single-CTA kernel: outputs must be bit-identical, including odd tile counts (padding tile),
-    ragged maps, channel tails, stride 2 and residuals."""
-    from dd3d_b200 import lib
-    L = lib.load()
-    g = torch.Generator().manual_seed(cin * 131 + cout + k + H)
-    x = _rand_act(B, H, W, cin, seed=cin + H)
-    w = torch.randn(cout, cin, k, k, generator=g) / (cin * k * k)**0.5
-    scale = 0.5 + torch.rand(cout, generator=g)
-    bias = torch.randn(cout, generator=g) * 0.5
-    Ho, Wo = H // stride, W // stride
-    residual = None
-    if res == 1:
-        residual = _rand_act(B, Ho, Wo, cout, seed=5)
-    elif res == 2:
-        residual = _rand_act(B, Ho // 2, Wo // 2, cout, seed=6)
-    outs = []
-    try:
-        for mode in (0, 1):
-            assert L.dd3d_set_conv_policy(b"cta2", mode) == 0
-            outs.append(gpu_ops.conv2d(x, w, scale, bias, stride, relu, residual, res == 2))
-            if cout <= 112:  # fp32 predictor path as well
-                outs.append(gpu_ops.conv2d(x, w, scale, bias, stride, False, None, False, out_f32=True))
-    finally:
-        L.dd3d_set_conv_policy(b"cta2", -1)
-    n = len(outs) // 2
-    for a, b in zip(outs[:n], outs[n:]):
-        assert torch.equal(a.view(torch.int16) if a.dtype == torch.bfloat16 else a.view(torch.int32),
-                           b.view(torch.int16) if b.dtype == torch.bfloat16 else b.view(torch.int32))
 
 
 @pytest.mark.parametrize("cin,cout,H,W,B,res", [(64, 64, 192, 320, 4, 0), (64, 64, 45, 77, 2, 1), (48, 64, 33, 40, 1, 0), (64, 32, 64, 64, 3, 0)])

@@ -1,6 +1,6 @@
-"""Static checks on the built library and the kernel sources (CPU only; cuobjdump cross-reads the sm_100a SASS):
+"""Static checks on the built library and the kernel sources (CPU only; cuobjdump cross-reads the sm_90a SASS):
 
-  * the GEMM-shaped kernels are tcgen05 kernels (UTCHMMA + TMA + TMEM loads in their SASS) and contain no legacy HMMA;
+  * the GEMM-shaped kernels are wgmma kernels (HGMMA in their SASS, operands staged by TMA) and contain no legacy HMMA;
   * the legacy tensor path (HMMA, mma.sync) appears ONLY in the three register-fragment kernels that use it on purpose
     (DESIGN.md 3: dla_front, stem_s2_mma, b3d_sparse);
   * the programmatic-dependent-launch rule of csrc/pdl.cuh: every kernel launched through launch_pdl() starts with
@@ -8,6 +8,7 @@
     attribute only inside a PdlScope;
   * the double-buffer rule of the cp.async kernels: a prefetch is issued only after the barrier that retires the readers of
     the buffer it overwrites (stem_mma had it the other way round once; the race showed only at full size)."""
+import glob
 import os
 import re
 import shutil
@@ -44,23 +45,35 @@ def test_tensor_core_paths_in_the_sass():
     def has(ops, prefix):
         return any(o.startswith(prefix) for o in ops)
     tc = {n: o for n, o in kernels.items() if re.search(r"conv_igemm_kernel|conv_taps_kernel|stem_tc_kernel", n)}
-    assert len(tc) >= 7  # 4 conv_igemm variants + taps + 2 stems
+    assert len(tc) >= 8  # 4 conv_igemm variants (generic / halo x bf16 / fp16) + 2 taps + 2 stems
     for n, ops in tc.items():
-        assert has(ops, "UTCHMMA"), f"{n}: no tcgen05.mma"
-        assert has(ops, "LDTM"), f"{n}: no tcgen05.ld"
-        assert not has(ops, "HMMA"), f"{n}: legacy mma.sync in a tcgen05 kernel"
+        assert has(ops, "HGMMA"), f"{n}: no wgmma"
+        assert not has(ops, "HMMA"), f"{n}: legacy mma.sync in a wgmma kernel"
     for n, ops in kernels.items():
         if re.search(r"conv_igemm_kernel|conv_taps_kernel", n):
             assert has(ops, "UTMALDG"), f"{n}: operands are not staged by TMA"
-    pairs = [o for n, o in kernels.items() if "conv_igemm_kernelILb" in n and n.split("conv_igemm_kernelILb")[1][3:5] == "b1"]
-    assert pairs and all(has(o, "UTCHMMA.2CTA") for o in pairs), "CTA-pair variants must issue cta_group::2 MMAs"
+        if re.search(r"conv_igemm_kernel", n):
+            assert has(ops, "UTMASTG"), f"{n}: outputs are not stored by TMA"
     legacy = {n for n, ops in kernels.items() if has(ops, "HMMA")}
     assert legacy, "the register-fragment kernels are missing"
     for n in legacy:
         assert re.search(r"dla_front_kernel|stem_s2_mma_kernel|b3d_sparse_kernel", n), f"unexpected mma.sync kernel: {n}"
     stem = [o for n, o in kernels.items() if "stem_s2_mma_kernel" in n]
-    assert stem and all(has(o, "STG.E.ENL2.256") for o in stem), "stem_mma: 256-bit stores expected"
+    assert stem and all(has(o, "STG.E.128") for o in stem), "stem_mma: 128-bit stores expected"
 
+
+
+def test_wgmma_pipelines_are_not_serialized():
+    """ptxas reports C7510 / C7520 when it serializes a kernel's wgmma pipeline (a call, or control flow it cannot prove
+    warpgroup-uniform, between issue and wait): the build's ptxas logs must carry neither."""
+    logs = sorted(glob.glob(os.path.join(ROOT, "dd3d_b200", "_lib", "obj", "*.ptxas.log")))
+    if not logs:
+        pytest.skip("the build's ptxas logs are not available")
+    bad = []
+    for path in logs:
+        with open(path) as f:
+            bad += [f"{os.path.basename(path)}: {line.strip()[:160]}" for line in f if re.search(r"\(C75(10|20)\)", line)]
+    assert not bad, "\n".join(bad)
 
 def _src(name):
     with open(os.path.join(CSRC, name)) as f:

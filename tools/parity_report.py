@@ -1,4 +1,4 @@
-"""Writes profiles/parity_r02.json: MEASURED end-to-end parity of the engine against the CPU oracle for every golden case
+"""Writes a JSON report (--out, default parity.json in the working directory): MEASURED end-to-end parity of the engine against the CPU oracle for every golden case
 (small ragged cases + the BASELINE.json shapes) and both storage types.  GPU box only; the numbers the thresholds of
 tests/test_parity_full_gpu.py / tests/test_e2e_gpu.py are derived from.
 
@@ -19,7 +19,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--cases", default="dla34,v2_99,dla34_full,v2_99_full")
     ap.add_argument("--dtypes", default="bf16,fp16")
-    ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "parity_r02.json"))
+    ap.add_argument("--out", default="parity.json")
     a = ap.parse_args()
     import torch
     from parity_lib import measure_case
