@@ -538,6 +538,25 @@ int dd3d_op_sample_aggregate(dd3d_det* d_dets, int32_t* d_counts, const float* d
                        nullptr);
 }
 
+int64_t dd3d_op_group_bev_nms_scratch_bytes(int B, int cap, int max_group_images) {
+    if (B < 1 || B > 256 || cap < 1 || cap > 1024 || max_group_images < 1 || max_group_images > 16) return DD3D_ERR_INVALID;
+    return static_cast<int64_t>(group_bev_nms_scratch_bytes(B, cap, max_group_images));
+}
+
+int dd3d_op_group_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_view_K, int num_views, const float* d_poses,
+                          int pose_mode, const int32_t* d_group, int num_groups, int max_group_images, float* d_global,
+                          void* d_scratch, int32_t* d_flags, int B, int cap, float iou_thresh, int max_dets,
+                          dd3d_stream stream) {
+    if (!d_dets || !d_counts || !d_view_K || !d_group || !d_scratch || !d_flags || num_views < 1 || B < 1 || B > 256 ||
+        cap < 1 || cap > 1024 || num_groups < 1 || num_groups > B || max_group_images < 1 || max_group_images > 16 ||
+        (pose_mode != DD3D_POSE_GLOBAL && pose_mode != DD3D_POSE_CAMERA) || (pose_mode == DD3D_POSE_GLOBAL && !d_poses))
+        return DD3D_ERR_INVALID;
+    return cuda_status(launch_group_bev_nms(reinterpret_cast<Det*>(d_dets), d_counts, d_view_K, num_views, d_poses,
+                                            pose_mode, d_group, num_groups, max_group_images, d_global, d_scratch,
+                                            d_flags, B, cap, iou_thresh, max_dets, static_cast<cudaStream_t>(stream)),
+                       nullptr);
+}
+
 int64_t dd3d_op_detect_scratch_bytes(int B, int pre_nms_topk) {
     return static_cast<int64_t>(decode_scratch_bytes(B, pre_nms_topk)) + DD3D_MAX_CLASSES * 3 * 4 + 512 +
            static_cast<int64_t>(nms_scratch_bytes(B, pre_nms_topk, DD3D_MAX_CLASSES));

@@ -125,4 +125,13 @@ cudaError_t launch_sample_aggregate(Det* dets, int32_t* counts, const float* K, 
                                     int num_groups, float* global, void* scratch, int32_t* flags, int B, int cap,
                                     float thr, int max_dets, cudaStream_t stream);
 
+// Grouped rotated BEV NMS for large sets (bev_nms_group.cu): B <= 256 images of cap <= 1024 slots, groups of
+// <= max_group_images <= 16 images; view_K [B][num_views][9] indexed by Det::level; pose_mode 0: global (poses [B][7]),
+// 1: camera (CAMERA_TO_VEHICLE_ROTATION); global (or nullptr): [B][cap][10]; max_dets <= 0: no cap.
+size_t group_bev_nms_scratch_bytes(int B, int cap, int max_group_images);
+cudaError_t launch_group_bev_nms(Det* dets, int32_t* counts, const float* view_K, int num_views, const float* poses,
+                                 int pose_mode, const int32_t* group, int num_groups, int max_group_images, float* global,
+                                 void* scratch, int32_t* flags, int B, int cap, float thr, int max_dets,
+                                 cudaStream_t stream);
+
 }  // namespace dd3d

@@ -14,6 +14,7 @@ NUM_LEVELS = 5
 ARCH_DLA34, ARCH_V2_99 = 0, 1
 IMG_U8, IMG_F32 = 0, 1
 ACT_BF16, ACT_FP16 = 0, 1
+POSE_GLOBAL, POSE_CAMERA = 0, 1
 DET_WORDS = 24  # sizeof(dd3d_det) / 4
 
 
@@ -106,6 +107,8 @@ SIGNATURES = {
     "dd3d_op_resize_preprocess": (_I, [_P, _I, _I, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P]),
     "dd3d_op_sample_aggregate_scratch_bytes": (_I64, [_I, _I]),
     "dd3d_op_sample_aggregate": (_I, [_P, _P, _P, _P, _P, _I, _P, _P, _P, _I, _I, C.c_float, _I, _P]),
+    "dd3d_op_group_bev_nms_scratch_bytes": (_I64, [_I, _I, _I]),
+    "dd3d_op_group_bev_nms": (_I, [_P, _P, _P, _I, _P, _I, _P, _I, _I, _P, _P, _P, _I, _I, C.c_float, _I, _P]),
     "dd3d_op_detect_scratch_bytes": (_I64, [_I, _I]),
     "dd3d_op_detect": (_I, [C.POINTER(ModelDesc), _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P),
                             C.POINTER(_P), C.POINTER(_P), _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -166,7 +166,8 @@ class DD3DB200(nn.Module):
         if flags:
             names = {1: "more candidates tied at the k-th pre-NMS score than the boundary buffer holds",
                      2: "more detections than out_cap slots", 4: "more than 256 boxes entered the BEV NMS of one image",
-                     8: "sample aggregation capacity exceeded"}
+                     8: "sample aggregation capacity exceeded", 16: "more merged TTA detections than slots",
+                     32: "grouped BEV NMS capacity exceeded"}
             raise RuntimeError("DD3DB200: detection capacity exceeded (" +
                                "; ".join(v for k, v in names.items() if flags & k) + f"; flags={int(flags)})")
 

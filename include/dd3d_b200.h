@@ -313,6 +313,27 @@ int64_t dd3d_op_sample_aggregate_scratch_bytes(int B, int cap);
 int dd3d_op_sample_aggregate(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsics, const float* d_poses,
                              const int32_t* d_group, int num_groups, float* d_global, void* d_scratch, int32_t* d_flags,
                              int B, int cap, float iou_thresh, int max_dets, dd3d_stream stream);
+/* Grouped rotated BEV NMS for large detection sets (csrc/bev_nms_group.cu): the BEV steps of NuscenesDD3D test-time
+ * augmentation (nuscenes_dd3d_tta.py), whose merged sets exceed the limits of the two entry points above.  In place on
+ * d_dets [B][cap] / d_counts [B] (B <= 256, cap <= 1024): one class-aware rotated NMS (scores_3d descending, ties by image
+ * then slot) per group of images (d_group [B], 0..num_groups-1, at most max_group_images <= 16 images per group), then --
+ * max_dets > 0 -- only
+ * the max_dets best survivors of the WHOLE call stay (keep[:max_num_dets_per_sample] of postprocessing.py:92-93); survivors
+ * keep their order.  Each box's translation is inv(K) (proj_ctr, 1) * depth with K = d_view_K[b][level][9] (num_views = 1:
+ * one K per image; the TTA merge stores the view index in `level`).  pose_mode DD3D_POSE_GLOBAL: boxes go to the global
+ * frame through d_poses [B][7] (sample_bev_nms, postprocessing.py:22-55); DD3D_POSE_CAMERA: bev_nms with its default
+ * pose_cam_global = CAMERA_TO_VEHICLE_ROTATION (tridet/layers/bev_nms.py:99-133), d_poses unused.  d_global (or NULL):
+ * [B][cap][10] receives quat (w,x,y,z), tvec, size of every survivor in that frame, compacted like d_dets.  d_scratch:
+ * dd3d_op_group_bev_nms_scratch_bytes(B, cap, max_group_images) bytes, any content (about
+ * B * cap^2 * max_group_images / 8 bytes: the IoU bit matrix).  Arguments out of range return DD3D_ERR_INVALID before any
+ * launch; d_flags bit 5 (32) is set when a count exceeds cap, a group holds more than max_group_images images, or a group
+ * index, class (>= 64) or view index is out of range. */
+enum dd3d_pose_mode { DD3D_POSE_GLOBAL = 0, DD3D_POSE_CAMERA = 1 };
+int64_t dd3d_op_group_bev_nms_scratch_bytes(int B, int cap, int max_group_images);
+int dd3d_op_group_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_view_K, int num_views, const float* d_poses,
+                          int pose_mode, const int32_t* d_group, int num_groups, int max_group_images, float* d_global,
+                          void* d_scratch, int32_t* d_flags, int B, int cap, float iou_thresh, int max_dets,
+                          dd3d_stream stream);
 /* decode + NMS on caller-provided head maps (layout documented in csrc/detect.cuh). */
 int64_t dd3d_op_detect_scratch_bytes(int B, int pre_nms_topk);
 int dd3d_op_detect(const dd3d_model_desc* h_desc, int B, const int32_t* h_level_hw /*[5][2]*/,
