@@ -133,6 +133,10 @@ int dd3d_set_conv_policy(const char* name, int value) {
         conv_set_n_split(value);
         return DD3D_OK;
     }
+    if (!strcmp(name, "pair_tile")) {
+        conv_set_pair(value);
+        return DD3D_OK;
+    }
     if (!strcmp(name, "op_fp16")) {
         g_op_fp16 = value ? 1 : 0;
         return DD3D_OK;
@@ -255,6 +259,24 @@ int dd3d_get_op_times(dd3d_handle h, float* h_ms, int32_t* h_cats, double* h_flo
     return st == DD3D_OK ? n : st;
 }
 
+int dd3d_get_conv_info(dd3d_handle h, int32_t* h_info, int max_ops) {
+    if (!h_info || max_ops < 1) return DD3D_ERR_INVALID;
+    int n = 0;
+    int st = guarded(h, [&](Engine& e) {
+        if (!e.plan.valid) throw EngineError(DD3D_ERR_STATE, "no plan");
+        for (const Op& op : e.plan.ops) {
+            if (n == max_ops) break;
+            int32_t* r = h_info + 8 * n++;
+            for (int i = 0; i < 8; ++i) r[i] = 0;
+            if (op.type != Op::CONV) continue;
+            const ConvParams& p = op.conv;
+            const int v[8] = {1, p.taps, p.stride, p.cin, p.block_n * p.n_blocks, p.halo ? 1 : 0, p.pair, p.block_n};
+            for (int i = 0; i < 8; ++i) r[i] = v[i];
+        }
+    });
+    return st == DD3D_OK ? n : st;
+}
+
 int dd3d_get_tensor(dd3d_handle h, const char* name, void** d_ptr, int32_t dims[6]) {
     return guarded(h, [&](Engine& e) {
         if (!e.plan.valid) throw EngineError(DD3D_ERR_STATE, "no plan");
@@ -372,6 +394,7 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
     }
     p.taps_n = conv_taps_eligible(taps, stride, cout_pad, 1, &Ho, &Wo) ? 1 : 0;
     if (!out_f32) g.out16 = d_out;
+    conv_select_pair(&p, cout_pad, device_sms());
     conv_finalize_params(&p);
     void* d_w_taps = nullptr;
     if (p.taps_n) {
@@ -386,7 +409,7 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
             cudaFree(d_w_taps);
             return DD3D_ERR_CUDA;
         }
-    } else if (!make_weight_map(&p.w_map, d_w, taps * kchunks * kBlockK, cout_pad, block_n, g_op_fp16)) {
+    } else if (!make_weight_map(&p.w_map, d_w, taps * kchunks * kBlockK, cout_pad, p.block_n, g_op_fp16)) {
         fprintf(stderr, "dd3d_op_conv2d: %s\n", conv_last_error());
         return DD3D_ERR_CUDA;
     }

@@ -335,45 +335,84 @@ int conv_tiles_per_image(int H, int W) {
     return ((H + th - 1) / th) * ((W + tw - 1) / tw);
 }
 
+// M units per image of a segment: tiles, or tile pairs with the pair tile
+static int conv_units_per_image(const ConvParams& p, const ConvSeg& g) {
+    const int tiles = ((g.W + g.tw - 1) / g.tw) * ((g.H + g.th - 1) / g.th);
+    return p.pair ? (tiles + 1) / 2 : tiles;
+}
+
+// Dynamic shared memory of everything but the B ring: staging tiles, alignment slack, barriers, (scale, bias) vectors and
+// the A patches (pair tile: two staging tiles per consumer warpgroup, two patches per A stage).
+static int conv_fixed_smem(const ConvParams& p) {
+    return (p.pair ? 4 : 2) * kStagingBytes + 1024 /*alignment slack*/ + kBarBytes + kSbBytes +
+           p.a_stages * (p.pair ? 2 : 1) * kHaloABytes;
+}
+
 void conv_finalize_params(ConvParams* p) {
-    int tile = 0;
+    int unit = 0;
     for (int s = 0; s < p->nseg; ++s) {
         ConvSeg& g = p->seg[s];
         g.tw_shift = 0;
         while ((1 << g.tw_shift) < g.tw) ++g.tw_shift;
         g.tiles_x = (g.W + g.tw - 1) / g.tw;
         g.tiles_y = (g.H + g.th - 1) / g.th;
-        g.tile_begin = tile;
-        g.inv_per_img = 1.0f / static_cast<float>(g.tiles_x * g.tiles_y);
+        g.tile_begin = unit;
+        const int per_img = conv_units_per_image(*p, g);
+        g.inv_per_img = 1.0f / static_cast<float>(per_img);
         g.inv_tiles_x = 1.0f / static_cast<float>(g.tiles_x);
-        tile += g.tiles_x * g.tiles_y * p->B;
+        unit += per_img * p->B;
     }
     p->inv_n_blocks = 1.0f / static_cast<float>(p->n_blocks);
-    p->total_work = tile * p->n_blocks;
+    p->total_work = unit * p->n_blocks;
     const int stage_bytes = (p->halo ? 0 : kABytes) + p->block_n * 128;
-    const int base = 2 * kStagingBytes + 1024 /*alignment slack*/ + kBarBytes + kSbBytes;
-    p->a_stages = p->halo ? kHaloAStages : 0;
+    p->a_stages = p->pair ? kPairAStages : p->halo ? kHaloAStages : 0;
     p->wstat = 0;
     // Weight-stationary: a 3x3 layer whose whole weight tensor is a few k-blocks (64 -> 64: 9 x 8 KiB; DLA-34 level2, VoVNet
     // stem_2) would re-stream it through the B ring for every 128-pixel tile -- barely one tile of lookahead against a TMA
     // round trip.  The tensor stays resident instead and the freed barriers / shared memory go to deeper A-patch prefetch.
-    if (p->halo && !p->taps_n && p->n_blocks == 1 && conv_wstat_enabled()) {
+    // (Never with the pair tile: 128 output channels x 9 taps of even one k-block do not fit next to the patches.)
+    if (p->halo && !p->taps_n && !p->pair && p->n_blocks == 1 && conv_wstat_enabled()) {
         const int resident = p->taps * p->kchunks * stage_bytes;
         for (int a = kMaxAStages; a >= kHaloAStages; --a) {
-            if (base + resident + a * kHaloABytes <= kSmemBudget) {
+            p->a_stages = a;
+            if (conv_fixed_smem(*p) + resident <= kSmemBudget) {
                 p->wstat = 1;
-                p->a_stages = a;
                 break;
             }
         }
+        if (!p->wstat) p->a_stages = kHaloAStages;
     }
-    const int fixed = base + p->a_stages * kHaloABytes;
-    int stages = (kSmemBudget - fixed) / stage_bytes;
+    int stages = (kSmemBudget - conv_fixed_smem(*p)) / stage_bytes;
     p->num_stages = p->wstat ? 2 : std::max(2, std::min(kMaxStages, stages));
 }
 
 static int g_n_split = -1;
 static int g_wstat = -1;
+static int g_pair = -1;
+
+void conv_set_pair(int mode) { g_pair = (mode == 0 || mode == 1) ? mode : -1; }
+
+bool conv_select_pair(ConvParams* p, int cout_pad, int num_sms) {
+    int mode = g_pair;
+    if (mode < 0) {
+        const char* e = getenv("DD3D_CONV_PAIR");
+        mode = (e && atoi(e) == 0) ? 0 : -1;
+    }
+    if (mode == 0 || !p->halo || p->taps_n || p->out_mode != 0 || cout_pad % 128 != 0) return false;
+    p->pair = 1;
+    if (mode < 0) {
+        // fill rule: below one work item per SM the 128-pixel tile (and the N-split) keeps more SMs busy
+        long pairs = 0;
+        for (int s = 0; s < p->nseg; ++s) pairs += static_cast<long>(p->B) * conv_units_per_image(*p, p->seg[s]);
+        if (pairs * (cout_pad / 128) < num_sms) {
+            p->pair = 0;
+            return false;
+        }
+    }
+    p->block_n = 128;
+    p->n_blocks = cout_pad / 128;
+    return true;
+}
 
 bool conv_wstat_enabled() {
     if (g_wstat < 0) {
@@ -395,9 +434,12 @@ void conv_set_n_split(int mode) { g_n_split = (mode == 0 || mode == 1) ? mode : 
 
 cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
     const int stage_bytes = (p.halo ? 0 : kABytes) + p.block_n * 128;
-    const int smem_bytes = (p.wstat ? p.taps * p.kchunks : p.num_stages) * stage_bytes + 2 * kStagingBytes + 1024 + kBarBytes +
-                           kSbBytes + p.a_stages * kHaloABytes;
+    const int smem_bytes = (p.wstat ? p.taps * p.kchunks : p.num_stages) * stage_bytes + conv_fixed_smem(p);
     ConvKernel kernel = nullptr;
+    if (p.pair) {
+        if (!p.halo || p.block_n != 128 || p.out_mode != 0) return cudaErrorInvalidValue;
+        kernel = conv_kernel_pair(p.fp16 != 0);
+    }
     for (auto group : {conv_kernel_n16_64, conv_kernel_n80_128, conv_kernel_n144_192, conv_kernel_n208_256}) {
         if (kernel == nullptr) kernel = group(p.halo != 0, p.fp16 != 0, p.block_n);
     }
@@ -415,6 +457,10 @@ cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
                     if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
                 }
             }
+        }
+        for (bool fp16 : {false, true}) {
+            if (e == cudaSuccess)
+                e = cudaFuncSetAttribute(conv_kernel_pair(fp16), cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
         }
         for (auto fn : {conv_taps_kernel<false>, conv_taps_kernel<true>}) {
             if (e == cudaSuccess) e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kTapsSmem);

@@ -57,7 +57,8 @@ struct ConvParams {
     int taps_n;       // 1: taps-in-N variant for 3x3 stride-1 convs with <= 16 output channels (conv_taps_kernel)
     int fp16;         // 16-bit storage type of activations and weights: 0 bf16, 1 fp16 (act16.cuh)
     int wstat;        // 1: weight-stationary halo variant -- all taps * kchunks weight blocks resident in shared memory
-    int a_stages;     // halo variants: A patches in flight (3, or up to 5 with wstat)
+    int a_stages;     // halo variants: A patches in flight (3, or up to 5 with wstat; 2 pairs of patches with pair)
+    int pair;         // 1: pair-tile halo variant -- work item = two 16x8 tiles x one 128-channel n-block (conv_select_pair)
 };
 static_assert(sizeof(ConvParams) <= 4096, "kernel parameter space");
 
@@ -88,6 +89,12 @@ bool conv_wstat_enabled();       // weight-stationary halo layers: on by default
 void conv_set_wstat(int mode);   // 0 off, 1 on, -1 environment / default
 bool conv_n_split_enabled();
 void conv_set_n_split(int mode);  // 0 off, 1 on, -1 environment / default (on)
+// Pair tile for halo layers whose cout_pad is a multiple of 128 (out_mode 0, not taps-in-N): when selected, sets p->pair,
+// block_n = 128 and n_blocks = cout_pad / 128 (the caller then needs a weight map with 128-row boxes) and returns true.
+// Needs the halo tiling of every segment set.  Default rule: also (tile pairs x n-blocks) >= num_sms, so small launches keep
+// the 128-pixel tile and the N-split.  conv_set_pair / DD3D_CONV_PAIR=0: 0 off, 1 on wherever eligible, -1 default.
+bool conv_select_pair(ConvParams* p, int cout_pad, int num_sms);
+void conv_set_pair(int mode);
 // Fills num_stages / total_work / tile bookkeeping from the already-set fields.
 void conv_finalize_params(ConvParams* p);
 cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream);

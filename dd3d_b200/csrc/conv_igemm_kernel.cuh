@@ -27,9 +27,17 @@
 //                for the predictor heads).  The producers keep prefetching the next tile's operands during the epilogue.
 // Launched with programmatic dependent launch: the prologue overlaps the previous kernel's tail.
 //
-// The kernel is templated on (halo variant, fp16 storage, wgmma N = block_n); conv_igemm_n*.cu instantiate it, one group of
-// N values per translation unit so that the build compiles them in parallel; conv_igemm.cu holds the host side and the
-// taps-in-N kernel.
+// Pair tile (PAIR, halo only, block_n = 128): the work item is TWO 16x8 halo tiles (tiles 2i, 2i + 1 of one image in
+// row-major tile order) x one 128-channel n-block, so every weight tile fetched from L2 feeds 256 output pixels instead of
+// 128 -- half the weight bytes per MAC of the 128 x 256 tile, for about 39 % less L2->SM traffic.  Warpgroup 1 + w owns
+// sub-tile w (its own [18][10][64ch] patch) and issues two m64n128k16 wgmmas per K step, one per 64-row half, on the same B
+// descriptor; it stores its sub-tile itself (own staging buffers, named barrier and store leader).  An odd per-image tile
+// count leaves the last pair's second sub-tile outside the image: its rows are never stored and read no residual.  The K
+// order per output element is unchanged, so results are bit-identical to the 128 x 256 tile.
+//
+// The kernel is templated on (halo variant, fp16 storage, wgmma N = block_n, pair tile); conv_igemm_n*.cu instantiate it, one
+// group of N values per translation unit so that the build compiles them in parallel; conv_igemm.cu holds the host side and
+// the taps-in-N kernel.
 #pragma once
 #include "conv_igemm.cuh"
 
@@ -54,6 +62,7 @@ constexpr int kHaloPW = kHaloTw + 2, kHaloPH = kHaloTh + 2;
 constexpr int kHaloABytes = (kHaloPW * kHaloPH * 128 + 1023) / 1024 * 1024;  // 23552
 constexpr int kHaloAStages = 3;   // default number of A patches in flight
 constexpr int kMaxAStages = 5;    // weight-stationary layers (ConvParams::wstat) spend the freed B ring on deeper A prefetch
+constexpr int kPairAStages = 2;   // pair tile: one patch pair feeds 9 k-blocks, so two pairs in flight suffice
 constexpr int kBarBytes = 512;
 constexpr int kSbBytes = 2 * 256 * 4;  // staged (scale, bias) vectors of the current (segment, n-block)
 constexpr int kConsumerWarps = 8, kEpiThreads = kConsumerWarps * 32;
@@ -71,8 +80,9 @@ __device__ __forceinline__ int fast_div(int x, int d, float inv_d) {
     return q;
 }
 
-// work item = (M-tile, n-block), n-block fastest
-__device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int work) {
+// work item = (M-tile, n-block), n-block fastest.  PAIR: the M unit is a pair of tiles, `sub` selects tile 2i + sub.
+template <bool PAIR = false>
+__device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int work, int sub = 0) {
     TileCoord t;
     int mt = work;
     t.n_blk = 0;
@@ -89,8 +99,10 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int work) 
     const ConvSeg& g = p.seg[s];
     int local = mt - g.tile_begin;
     int per_img = g.tiles_x * g.tiles_y;
+    if (PAIR) per_img = (per_img + 1) >> 1;
     t.img = fast_div(local, per_img, g.inv_per_img);
     int r = local - t.img * per_img;
+    if (PAIR) r = 2 * r + sub;
     int ty = fast_div(r, g.tiles_x, g.inv_tiles_x);
     int tx = r - ty * g.tiles_x;
     t.y0 = ty * g.th;
@@ -142,21 +154,40 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[L], uint64_t adesc, uint
     wg::commit();
 }
 
+// Pair tile: the same k-block for both 64-row halves of the warpgroup's sub-tile (one B descriptor, two A descriptors).
+template <int N, bool F16, int L>
+__device__ __forceinline__ void mma_kblock2(float (&acc0)[L], float (&acc1)[L], uint64_t adesc0, uint64_t adesc1,
+                                            uint64_t bdesc, bool first) {
+    wg::fence();
+#pragma unroll
+    for (int k = 0; k < kBlockK / 16; ++k) {
+        const uint32_t scale_d = (first && k == 0) ? 0u : 1u;
+        wg::wgmma<N, F16>(acc0, adesc0 + 2 * k, bdesc + 2 * k, scale_d);
+        wg::wgmma<N, F16>(acc1, adesc1 + 2 * k, bdesc + 2 * k, scale_d);
+    }
+    wg::commit();
+}
+
 // BN = block_n, the wgmma N: a compile-time parameter, so the accumulators are exactly BN / 2 registers per consumer thread
-template <bool HALO, bool F16, int BN>
+// and 64-row half (PAIR: two halves per warpgroup)
+template <bool HALO, bool F16, int BN, bool PAIR = false>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
+    static_assert(!PAIR || (HALO && BN == 128), "the pair tile is a halo variant with block_n 128");
+    constexpr int MH = PAIR ? 2 : 1;                                   // 64-row halves per consumer warpgroup
+    constexpr int kASlot = PAIR ? 2 * kHaloABytes : kHaloABytes;       // one A stage: the patch of every sub-tile
     extern __shared__ uint8_t smem_raw[];
     // 128B-swizzled tiles need 1024-byte alignment
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    // generic: num_stages x [A 16 KiB | B block_n*128].  halo: num_stages x [B block_n*128], then a_stages x [A patch 23 KiB]
+    // generic: num_stages x [A 16 KiB | B block_n*128].  halo: num_stages x [B block_n*128], then a_stages x [A patch 23 KiB
+    // (PAIR: two patches)], then the staging tiles (PAIR: two per consumer warpgroup)
     const int stage_bytes = (HALO ? 0 : kABytes) + BN * 128;
     // weight-stationary (HALO, one n-block, cin <= 64): ALL k-blocks of the weight tensor stay resident in the B region
     // (loaded once per CTA) instead of cycling through the stage ring for every tile
-    const bool wstat = HALO && p.wstat != 0;
+    const bool wstat = HALO && !PAIR && p.wstat != 0;
     const int a_stages = HALO ? p.a_stages : 0;
     uint8_t* halo_a = smem + (wstat ? p.taps * p.kchunks : p.num_stages) * stage_bytes;
-    uint8_t* staging = halo_a + a_stages * kHaloABytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 2 * kStagingBytes);
+    uint8_t* staging = halo_a + a_stages * kASlot;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 2 * MH * kStagingBytes);
     uint64_t* full_bar = bars;                     // [kMaxStages]
     uint64_t* empty_bar = bars + kMaxStages;       // [kMaxStages]
     uint64_t* afull_bar = bars + 2 * kMaxStages;   // [kMaxAStages]
@@ -212,7 +243,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             __syncwarp();
         }
         for (int work = w_first; work < w_total && !wstat; work += w_step) {
-            const TileCoord t = decode_tile(p, work);
+            const TileCoord t = decode_tile<PAIR>(p, work);
             const ConvSeg& g = p.seg[t.seg];
             if (HALO) {
                 for (int kc = 0; kc < p.kchunks; ++kc) {
@@ -285,17 +316,22 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
         } else {
             // ------------------------------------------------------------ warp 2: halo A-patch producer: one box
             // [18][10][64 ch] (180 rows of 128 B, 128B-swizzled, zero-filled outside the image) per 64-channel block
+            // (PAIR: one per sub-tile, both on one barrier)
             int as = 0;
             uint32_t aphase = 0;
             for (int work = w_first; work < w_total; work += w_step) {
-                const TileCoord t = decode_tile(p, work);
+                const TileCoord t = decode_tile<PAIR>(p, work);
+                const TileCoord t1 = PAIR ? decode_tile<PAIR>(p, work, 1) : t;
                 const ConvSeg& g = p.seg[t.seg];
                 for (int kc = 0; kc < p.kchunks; ++kc) {
                     ptx::mbar_wait(&aempty_bar[as], aphase ^ 1);
                     if (elect_one()) {
-                        ptx::mbar_expect_tx(&afull_bar[as], kHaloPW * kHaloPH * 128);
-                        ptx::tma_load_4d(halo_a + as * kHaloABytes, &g.in_map[0], &afull_bar[as], kc * kBlockK, t.x0 - 1,
+                        ptx::mbar_expect_tx(&afull_bar[as], MH * kHaloPW * kHaloPH * 128);
+                        ptx::tma_load_4d(halo_a + as * kASlot, &g.in_map[0], &afull_bar[as], kc * kBlockK, t.x0 - 1,
                                          t.y0 - 1, t.img);
+                        if (PAIR)
+                            ptx::tma_load_4d(halo_a + as * kASlot + kHaloABytes, &g.in_map[0], &afull_bar[as], kc * kBlockK,
+                                             t1.x0 - 1, t1.y0 - 1, t1.img);
                     }
                     __syncwarp();
                     if (++as == a_stages) {
@@ -307,21 +343,28 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
         }
     } else if (warp >= 4) {
         // ---------------------------------------------------------------- consumer warpgroups 1, 2
-        const int wgi = (warp >> 2) - 1;                                 // rows 64 * wgi ..
+        const int wgi = (warp >> 2) - 1;                                 // rows 64 * wgi .. (PAIR: sub-tile wgi)
         const int et = static_cast<int>(threadIdx.x) - 128;              // 0 .. kEpiThreads - 1
         const int wl = (et >> 5) & 3;
-        const bool store_leader = (et == 0);
+        // PAIR: each warpgroup stages and stores its own sub-tile, synchronised on its own named barrier
+        const bool store_leader = PAIR ? (et & 127) == 0 : (et == 0);
+        const uint32_t epi_bar = PAIR ? 2 + wgi : 1;
+        const uint32_t epi_threads = PAIR ? 128 : kEpiThreads;
+        const int out_mode = PAIR ? 0 : p.out_mode;
         const uint64_t desc_hi = ptx::make_sw128_desc(0, HALO ? kHaloPW * 128 : 1024) & ~0x3FFFull;
         const uint64_t bdesc_hi = ptx::make_sw128_desc(0, 1024) & ~0x3FFFull;
         const uint32_t smem_lo = ptx::smem_u32(smem) >> 4;
         const uint32_t halo_lo = ptx::smem_u32(halo_a) >> 4;
         const uint32_t stage_units = static_cast<uint32_t>(stage_bytes) >> 4;
-        // the rows of this thread's two accumulator row-halves within the 128-pixel tile
-        int row[2];
-        row[0] = 64 * wgi + 16 * wl + (lane >> 2);
-        row[1] = row[0] + 8;
+        // the rows of this thread's accumulator row-halves within the 128-pixel tile (2 per 64-row half)
+        int row[2 * MH];
+#pragma unroll
+        for (int m = 0; m < MH; ++m) {
+            row[2 * m] = 64 * (PAIR ? m : wgi) + 16 * wl + (lane >> 2);
+            row[2 * m + 1] = row[2 * m] + 8;
+        }
         const int qc = 2 * (lane & 3);  // first of this thread's two columns in every 8-column group
-        float acc[BN / 2];
+        float acc[MH][BN / 2];
         int stage = 0;
         uint32_t phase = 0;
         int as = 0;
@@ -330,7 +373,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
         int sb_key = -1;  // (segment, n-block) whose folded-BN vectors are staged in s_scale / s_bias
         if (wstat) ptx::mbar_wait(wfull_bar, 0);
         for (int work = w_first; work < w_total; work += w_step) {
-            const TileCoord t = decode_tile(p, work);
+            const TileCoord t = decode_tile<PAIR>(p, work, PAIR ? wgi : 0);
             const ConvSeg& g = p.seg[t.seg];
             // ---- main loop: one commit group per k-block; the slot (and halo patch) of group i is released after
             // group i + 1 has been issued and group i has retired (wait_group 1)
@@ -346,14 +389,20 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             if (HALO) {
                 for (int kc = 0; kc < p.kchunks; ++kc) {
                     ptx::mbar_wait(&afull_bar[as], aphase);
-                    const uint32_t a_lo = halo_lo + static_cast<uint32_t>(as) * (kHaloABytes >> 4) + wgi * 8 * kHaloPW * 8;
+                    // rows 64 * wgi.. of the tile's patch; PAIR: row 0 of sub-tile wgi's patch (rows 64.. are 8 patch rows on)
+                    const uint32_t a_lo = halo_lo + static_cast<uint32_t>(as) * (kASlot >> 4) +
+                                          (PAIR ? wgi * (kHaloABytes >> 4) : wgi * 8 * kHaloPW * 8);
                     for (int tap = 0; tap < 9; ++tap) {
                         if (!wstat) ptx::mbar_wait(&full_bar[stage], phase);
                         const int r = tap / 3, s = tap - 3 * r;
                         const uint32_t a_tap = a_lo + (r * kHaloPW + s) * 8;  // whole pixels: 128 B = 8 x 16 B
                         const uint32_t b_lo =
                             smem_lo + static_cast<uint32_t>(wstat ? tap * p.kchunks + kc : stage) * stage_units;
-                        mma_kblock<BN, F16>(acc, desc_hi | a_tap, bdesc_hi | b_lo, (kc | tap) == 0);
+                        if constexpr (PAIR)
+                            mma_kblock2<BN, F16>(acc[0], acc[MH - 1], desc_hi | a_tap, desc_hi | (a_tap + 8 * kHaloPW * 8),
+                                                 bdesc_hi | b_lo, (kc | tap) == 0);
+                        else
+                            mma_kblock<BN, F16>(acc[0], desc_hi | a_tap, bdesc_hi | b_lo, (kc | tap) == 0);
                         wg::wait<1>();
                         release();
                         rel_stage = wstat ? -1 : stage;
@@ -373,7 +422,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                     ptx::mbar_wait(&full_bar[stage], phase);
                     const uint32_t a_lo = smem_lo + static_cast<uint32_t>(stage) * stage_units + wgi * (64 * 128 / 16);
                     const uint32_t b_lo = smem_lo + static_cast<uint32_t>(stage) * stage_units + (kABytes >> 4);
-                    mma_kblock<BN, F16>(acc, desc_hi | a_lo, bdesc_hi | b_lo, kb == 0);
+                    mma_kblock<BN, F16>(acc[0], desc_hi | a_lo, bdesc_hi | b_lo, kb == 0);
                     wg::wait<1>();
                     release();
                     rel_stage = stage;
@@ -385,15 +434,16 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             }
             wg::wait<0>();
             release();
-            wg::fence_regs(acc);
-
-            // ---- epilogue of this warpgroup's 64 rows
-            const int n_base = t.n_blk * BN;
-            bool in_img[2];
-            const __nv_bfloat16* res_ptr[2];
-            float* f32_ptr[2];
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
+            for (int m = 0; m < MH; ++m) wg::fence_regs(acc[m]);
+
+            // ---- epilogue of this warpgroup's 64 rows (PAIR: of its 128-row sub-tile)
+            const int n_base = t.n_blk * BN;
+            bool in_img[2 * MH];
+            const __nv_bfloat16* res_ptr[2 * MH];
+            float* f32_ptr[2 * MH];
+#pragma unroll
+            for (int h = 0; h < 2 * MH; ++h) {
                 const int ly = row[h] >> g.tw_shift;
                 const int lx = row[h] - (ly << g.tw_shift);
                 const int oy = t.y0 + ly, ox = t.x0 + lx;
@@ -406,7 +456,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                         g.residual + (static_cast<size_t>(t.img * g.res_H + ry) * g.res_W + rx) * g.res_pitch + n_base + qc;
                 }
                 f32_ptr[h] = nullptr;
-                if (p.out_mode == 1 && in_img[h])
+                if (out_mode == 1 && in_img[h])
                     f32_ptr[h] = g.out_f32 + (static_cast<size_t>(t.img * g.H + oy) * g.W + ox) * g.out_pitch + n_base + qc;
             }
             // per-channel (scale, bias) of this (segment, n-block) in shared memory: broadcast LDS instead of LDG with their
@@ -426,12 +476,13 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
 #pragma unroll
             for (int c = 0; c < (BN + 63) / 64; ++c) {
                 const int c0 = 64 * c;
-                uint8_t* stag = staging + sbuf * kStagingBytes;
-                const uint32_t stag_u32 = staging_u32 + sbuf * kStagingBytes;
-                if (p.out_mode == 0) {
+                const int sb = PAIR ? 2 * wgi + sbuf : sbuf;
+                uint8_t* stag = staging + sb * kStagingBytes;
+                const uint32_t stag_u32 = staging_u32 + sb * kStagingBytes;
+                if (out_mode == 0) {
                     // the TMA store that last read this staging buffer must have drained
                     if (store_leader) ptx::tma_store_wait_read<1>();
-                    ptx::named_bar_sync(1, kEpiThreads);
+                    ptx::named_bar_sync(epi_bar, epi_threads);
                 }
 #pragma unroll
                 for (int jj = 0; jj < 8; ++jj) {
@@ -441,9 +492,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                     const float2 sc = ptx::ld_shared_f2(s_scale_u32 + col * 4);
                     const float2 bi = ptx::ld_shared_f2(s_bias_u32 + col * 4);
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        float y0 = fmaf(acc[4 * j + 2 * h], sc.x, bi.x);
-                        float y1 = fmaf(acc[4 * j + 2 * h + 1], sc.y, bi.y);
+                    for (int h = 0; h < 2 * MH; ++h) {
+                        float y0 = fmaf(acc[h >> 1][4 * j + 2 * (h & 1)], sc.x, bi.x);
+                        float y1 = fmaf(acc[h >> 1][4 * j + 2 * (h & 1) + 1], sc.y, bi.y);
                         if (has_res) {
                             const uint32_t rv =
                                 res_ptr[h] != nullptr ? __ldg(reinterpret_cast<const unsigned int*>(res_ptr[h] + 8 * j)) : 0u;
@@ -451,7 +502,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                             y0 += f.x;
                             y1 += f.y;
                         }
-                        if (p.out_mode == 0) {
+                        if (out_mode == 0) {
                             const int r = row[h];
                             ptx::st_shared_u32(stag_u32 + r * 128 + ((jj ^ (r & 7)) << 4) + qc * 2,
                                                pack2_relu<F16>(y0, y1, p.relu != 0));
@@ -469,14 +520,14 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                         }
                     }
                 }
-                if (p.out_mode == 0) {
+                if (out_mode == 0) {
                     ptx::fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the TMA engine
-                    ptx::named_bar_sync(1, kEpiThreads);
+                    ptx::named_bar_sync(epi_bar, epi_threads);
                     if (store_leader) {
                         ptx::tma_store_4d(&g.out_map, stag, n_base + c0, t.x0, t.y0, t.img);
                         ptx::tma_store_commit();
                     }
-                    if (g.pool_partial != nullptr && et < 128) {
+                    if (!PAIR && g.pool_partial != nullptr && et < 128) {
                         // eSE global-average-pool, fused: per-tile channel sums of the 16-bit tile just staged (exactly the
                         // values the reference pools, vovnet.py:181).  Thread e covers channels 8*(e&7).. of rows
                         // (e>>3) + 16*i; the 4 row-groups of a warp are shuffle-reduced; one fp32 partial per
@@ -542,6 +593,7 @@ using ConvKernel = void (*)(ConvParams);
     }
 ConvKernel conv_kernel_n16_64(bool halo, bool fp16, int block_n);
 ConvKernel conv_kernel_n80_128(bool halo, bool fp16, int block_n);
+ConvKernel conv_kernel_pair(bool fp16);  // the pair-tile halo kernel (block_n 128), in conv_igemm_n80_128.cu
 ConvKernel conv_kernel_n144_192(bool halo, bool fp16, int block_n);
 ConvKernel conv_kernel_n208_256(bool halo, bool fp16, int block_n);
 

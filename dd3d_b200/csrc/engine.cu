@@ -362,8 +362,11 @@ struct Builder {
         // Under-filled launches (DLA-34 level5 at B = 8: 30 M-tiles x 2 N-blocks on 132 SMs; p6 / p7): split N until the grid
         // covers the machine.  Each CTA's serial MMA chain shrinks with N while the
         // A tiles it re-reads are tiny; K order per output element is unchanged, so results are bit-identical.
+        // Filled halo layers with 128-multiple widths (FCOS towers, FPN outputs, VoVNet stage 2) run the 256 x 128 pair tile:
+        // half the weight traffic per MAC, same K order -> bit-identical.
+        const bool pair = conv_select_pair(&p, L.cout_pad, E->num_sms);
         bool n_split = false;
-        if (!p.taps_n && conv_n_split_enabled()) {
+        if (!p.taps_n && !pair && conv_n_split_enabled()) {
             int tiles = 0;
             for (int s = 0; s < p.nseg; ++s)
                 tiles += B * ((p.seg[s].H + p.seg[s].th - 1) / p.seg[s].th) * ((p.seg[s].W + p.seg[s].tw - 1) / p.seg[s].tw);
@@ -376,7 +379,7 @@ struct Builder {
             }
         }
         conv_finalize_params(&p);
-        if (n_split) {
+        if (n_split || pair) {
             if (!make_weight_map(&p.w_map, L.d_w, L.ktot, L.cout_pad, p.block_n, E->fp16))
                 fail(DD3D_ERR_CUDA, conv_last_error());
         } else {

@@ -173,7 +173,11 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value);
  * "wstat" = 0: 3x3 layers whose whole weight tensor fits in shared memory next to the activation patches (64 -> 64 channels)
  * stream it per tile like every other layer instead of keeping it resident (default 1; bit-identical results either way).
  * "n_split" = 0: conv launches with fewer work items than half the SMs keep their N tile instead of splitting it (default 1;
- * bit-identical results either way). */
+ * bit-identical results either way).
+ * "pair_tile": 3x3 stride-1 (halo) layers whose padded output channels are a multiple of 128 run a 256-pixel x 128-channel
+ * tile (two 16x8 tiles share each weight tile: half the weight traffic per MAC).  -1 (default): when the launch has at least
+ * one (tile pair, 128-channel block) per SM, otherwise the 128-pixel tile and the N-split keep the machine filled; 1: wherever
+ * eligible; 0 (or environment DD3D_CONV_PAIR=0): never.  Bit-identical results either way. */
 int dd3d_set_conv_policy(const char* name, int value);
 /* Number of kernel launches one dd3d_forward enqueues (for the bench's gpu_launches claim). */
 int dd3d_launches_per_forward(dd3d_handle h);
@@ -186,6 +190,10 @@ int dd3d_get_profile(dd3d_handle h, double* h_ms, double* h_flops, double* h_byt
 /* Same events, per op in launch order (entry 0 = preprocess, then every engine op, then decode, NMS): device ms,
  * category and algorithmic FLOPs.  Returns the number of entries written (<= max_ops). */
 int dd3d_get_op_times(dd3d_handle h, float* h_ms, int32_t* h_cats, double* h_flops, int max_ops);
+/* Kernel choice of every engine op of the current plan, in launch order (entry i = entry i + 1 of dd3d_get_op_times): 8
+ * int32 per op = {is implicit-GEMM conv, taps, stride, cin, padded cout, halo variant, pair tile, block_n}, all 0 for other
+ * ops.  Returns the number of ops written (<= max_ops). */
+int dd3d_get_conv_info(dd3d_handle h, int32_t* h_info, int max_ops);
 
 /* ---- GPU input pipeline (SURVEY.md 8f row 3) ------------------------------------------------------------------
  * Replaces the per-image CPU work of DefaultDatasetMapper.__call__ at test time
