@@ -1,8 +1,8 @@
-"""Parameter inventory of the two shipped DD3D configurations, keyed by the reference's state_dict names.
+"""Parameter inventory of the DD3D configurations (DLA-34 and every VoVNetV2-eSE variant), keyed by the reference's state_dict names.
 
 The names/shapes follow what ``DD3D(cfg).state_dict()`` yields in the reference
-(tridet/modeling/dd3d/core.py:19-55; DLA-34 tridet/modeling/feature_extractor/dla.py:250-361; V2-99-eSE
-tridet/modeling/feature_extractor/vovnet.py:79-87,276-336; FPN + top blocks dla.py:537-561, vovnet.py:411-454;
+(tridet/modeling/dd3d/core.py:19-55; DLA-34 tridet/modeling/feature_extractor/dla.py:250-361; VoVNetV2-eSE
+tridet/modeling/feature_extractor/vovnet.py:19-143,188-336; FPN + top blocks dla.py:537-561, vovnet.py:411-454;
 heads fcos2d.py:55-108, fcos3d.py:81-139).  tests/test_cpu_oracle.py::test_inventory_and_oracle_vs_live_reference checks this inventory against the
 reference's own state_dict when /root/reference is present.
 """
@@ -65,27 +65,59 @@ V99_STAGE_CONV_CH = [128, 160, 192, 224]
 V99_STAGE_OUT_CH = [256, 512, 768, 1024]
 V99_BLOCKS = [1, 3, 9, 3]
 
+# The reference's VoVNet _STAGE_SPECS (vovnet.py:19-97), by arch key: (FE.BACKBONE.NAME, stem, stage_conv_ch, stage_out_ch,
+# layer_per_block, block_per_stage, dw).  The engine has its own copy (csrc/engine.cu kVovSpecs); tests/test_vovnet_family.py
+# pins both against the reference.
+VOVNET_SPECS = {
+    "v2_19_slim_dw": ("V-19-slim-dw-eSE", (64, 64, 64), (64, 80, 96, 112), (112, 256, 384, 512), 3, (1, 1, 1, 1), True),
+    "v2_19_dw": ("V-19-dw-eSE", (64, 64, 64), (128, 160, 192, 224), (256, 512, 768, 1024), 3, (1, 1, 1, 1), True),
+    "v2_19_slim": ("V-19-slim-eSE", (64, 64, 128), (64, 80, 96, 112), (112, 256, 384, 512), 3, (1, 1, 1, 1), False),
+    "v2_19": ("V-19-eSE", (64, 64, 128), (128, 160, 192, 224), (256, 512, 768, 1024), 3, (1, 1, 1, 1), False),
+    "v2_39": ("V-39-eSE", (64, 64, 128), (128, 160, 192, 224), (256, 512, 768, 1024), 5, (1, 1, 2, 2), False),
+    "v2_57": ("V-57-eSE", (64, 64, 128), (128, 160, 192, 224), (256, 512, 768, 1024), 5, (1, 1, 4, 3), False),
+    "v2_99": ("V-99-eSE", (64, 64, 128), tuple(V99_STAGE_CONV_CH), tuple(V99_STAGE_OUT_CH), 5, tuple(V99_BLOCKS), False),
+}
+VOVNET_KEYS = {spec[0]: key for key, spec in VOVNET_SPECS.items()}  # FE.BACKBONE.NAME -> arch key
+ARCH_KEYS = ("dla34", ) + tuple(VOVNET_SPECS)
 
-def _v2_99(specs):
+
+def _vov_conv3x3(specs, n, cout, cin, dw):
+    """conv3x3 (vovnet.py:124-143) or dw_conv3x3 (vovnet.py:100-121; the reference builds it only with cin == cout)."""
+    if dw:
+        specs[f"{n}/dw_conv3x3.weight"] = ((cout, 1, 3, 3), "conv:dw")
+        _conv(specs, f"{n}/pw_conv1x1", cout, cin, 1)
+        _bn(specs, f"{n}/pw_norm", cout)
+    else:
+        _conv(specs, f"{n}/conv", cout, cin, 3)
+        _bn(specs, f"{n}/norm", cout)
+
+
+def _vovnet(specs, arch):
     p = "backbone.bottom_up"
-    for name, cout, cin in (("stem_1", 64, 3), ("stem_2", 64, 64), ("stem_3", 128, 64)):
-        _conv(specs, f"{p}.stem.{name}/conv", cout, cin, 3)
-        _bn(specs, f"{p}.stem.{name}/norm", cout)
-    in_ch = 128
-    for si, (sc, oc, nb) in enumerate(zip(V99_STAGE_CONV_CH, V99_STAGE_OUT_CH, V99_BLOCKS), start=2):
+    _, stem, stage_ch, out_ch, nl, blocks, dw = VOVNET_SPECS[arch]
+    _conv(specs, f"{p}.stem.stem_1/conv", stem[0], 3, 3)
+    _bn(specs, f"{p}.stem.stem_1/norm", stem[0])
+    _vov_conv3x3(specs, f"{p}.stem.stem_2", stem[1], stem[0], dw)
+    _vov_conv3x3(specs, f"{p}.stem.stem_3", stem[2], stem[1], dw)
+    in_ch = stem[2]
+    for si, (sc, oc, nb) in enumerate(zip(stage_ch, out_ch, blocks), start=2):
         for b in range(nb):
             name = f"OSA{si}_{b + 1}"
             q = f"{p}.stage{si}.{name}"
             cin = in_ch
-            for i in range(5):
-                _conv(specs, f"{q}.layers.{i}.{name}_{i}/conv", sc, cin, 3)
-                _bn(specs, f"{q}.layers.{i}.{name}_{i}/norm", sc)
+            if dw and in_ch != sc:  # conv_reduction (vovnet.py:200-205)
+                r = f"{q}.conv_reduction.{name}_reduction_0"
+                _conv(specs, f"{r}/conv", sc, in_ch, 1)
+                _bn(specs, f"{r}/norm", sc)
                 cin = sc
-            _conv(specs, f"{q}.concat.{name}_concat/conv", oc, in_ch + 5 * sc, 1)
+            for i in range(nl):
+                _vov_conv3x3(specs, f"{q}.layers.{i}.{name}_{i}", sc, cin, dw)
+                cin = sc
+            _conv(specs, f"{q}.concat.{name}_concat/conv", oc, in_ch + nl * sc, 1)
             _bn(specs, f"{q}.concat.{name}_concat/norm", oc)
             _conv(specs, f"{q}.ese.fc", oc, oc, 1, bias=True, role="ese")
             in_ch = oc
-    return {"stage2": 256, "stage3": 512, "stage4": 768, "stage5": 1024}
+    return {f"stage{si}": oc for si, oc in enumerate(out_ch, start=2)}
 
 
 def param_specs(cfg):
@@ -98,7 +130,7 @@ def param_specs(cfg):
         feats = _dla34(specs)
         stages = {"level3": 3, "level4": 4, "level5": 5}
     else:
-        feats = _v2_99(specs)
+        feats = _vovnet(specs, arch)
         stages = {"stage2": 2, "stage3": 3, "stage4": 4, "stage5": 5}
     for name, ch in feats.items():
         st = stages[name]
@@ -162,11 +194,15 @@ def is_nuscenes_arch(cfg):
 
 
 def arch_of(cfg):
+    """Arch key of FE.BUILDER + FE.BACKBONE.NAME: "dla34" or a key of VOVNET_SPECS."""
     b = cfg.FE.BUILDER
     if b == "build_fcos_dla_fpn_backbone_p67":
+        name = cfg.FE.BACKBONE.NAME
+        if name != "DLA-34":  # dla.py builds DLA-46-C, DLA-60, ... too: Bottleneck / BottleneckX blocks the engine lacks
+            raise NotImplementedError(f"DLA variant {name!r} is not supported: only DLA-34 is built by the engine")
         return "dla34"
     if b == "build_fcos_vovnet_fpn_backbone_p6":
-        return "v2_99"
+        return VOVNET_KEYS[cfg.FE.BACKBONE.NAME]  # KeyError for an unknown name, like _STAGE_SPECS[cfg.NAME]
     raise KeyError("No object named '{}' found in 'BACKBONE' registry!".format(b))
 
 

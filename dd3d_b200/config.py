@@ -9,6 +9,8 @@ eval-mode BN in FCOS2D, NMS_THRESH 0.75).
 """
 import copy
 
+from .arch import VOVNET_SPECS
+
 
 class CfgNode(dict):
     """dict with attribute access, like the OmegaConf/yacs nodes the reference uses."""
@@ -81,10 +83,16 @@ _FEATURE_EXTRACTORS = {
         BACKBONE=dict(NAME="V-99-eSE", OUT_FEATURES=["stage2", "stage3", "stage4", "stage5"], NORM="FrozenBN"),
     ),
 }
+# the other VoVNets of vovnet.py:_STAGE_SPECS: same builder and FPN, FE.BACKBONE.NAME picks the variant
+for _key, _spec in VOVNET_SPECS.items():
+    if _key not in _FEATURE_EXTRACTORS:
+        _FEATURE_EXTRACTORS[_key] = copy.deepcopy(_FEATURE_EXTRACTORS["v2_99"])
+        _FEATURE_EXTRACTORS[_key]["BACKBONE"]["NAME"] = _spec[0]
 
 
 def get_cfg(backbone="dla34", dataset="kitti_3d", nms_thresh=0.75, meta_arch="DD3D", act_dtype="bf16"):
-    """backbone in {"dla34", "v2_99"}; dataset in {"kitti_3d", "nuscenes"} (head constants only); meta_arch in
+    """backbone: "dla34" or a VoVNet key of dd3d_b200.arch.VOVNET_SPECS ("v2_19_slim_dw", "v2_19_dw", "v2_19_slim", "v2_19",
+    "v2_39", "v2_57", "v2_99"), which sets FE.BACKBONE.NAME; dataset in {"kitti_3d", "nuscenes"} (head constants only); meta_arch in
     {"DD3D", "NuscenesDD3D"} (configs/experiments/dd3d_nusc_{dla34,v99}.yaml:9,30-36)."""
     ds = _DATASETS[dataset]
     fe = copy.deepcopy(_FEATURE_EXTRACTORS[backbone])

@@ -344,8 +344,8 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
     const int kchunks = (cin + kBlockK - 1) / kBlockK;
     const int taps = ksize * ksize;
     const int cout_pad = (cout + 15) / 16 * 16;
-    const int block_n = cout_pad > 256 ? 256 : cout_pad;
-    if (cout_pad % block_n) return DD3D_ERR_INVALID;
+    const int block_n = conv_block_n(cout_pad);
+    if (block_n == 0) return DD3D_ERR_INVALID;
     if (!out_f32 && cout % 16) return DD3D_ERR_INVALID;
     p.nseg = 1;
     p.B = B;
@@ -445,6 +445,15 @@ int dd3d_op_stem_s2_mma(const void* d_in4, const void* d_w, const float* d_sb, v
     return cuda_status(launch_stem_s2_mma(static_cast<const __nv_bfloat16*>(d_in4), static_cast<const __nv_bfloat16*>(d_w), d_sb,
                                           static_cast<__nv_bfloat16*>(d_out), out_pitch, B, H, W, device_sms(),
                                           static_cast<cudaStream_t>(stream), g_op_fp16),
+                       nullptr);
+}
+
+int dd3d_op_dwconv3x3(const void* d_in, int B, int H, int W, int C, int in_pitch, const void* d_w, int stride, void* d_out,
+                      int out_pitch, dd3d_stream stream) {
+    if (!d_in || !d_w || !d_out) return DD3D_ERR_INVALID;
+    return cuda_status(launch_dwconv3x3(static_cast<const __nv_bfloat16*>(d_in), B, H, W, C, in_pitch,
+                                        static_cast<const __nv_bfloat16*>(d_w), stride, static_cast<__nv_bfloat16*>(d_out),
+                                        out_pitch, static_cast<cudaStream_t>(stream), g_op_fp16),
                        nullptr);
 }
 

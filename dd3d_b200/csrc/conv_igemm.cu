@@ -392,6 +392,14 @@ static int g_pair = -1;
 
 void conv_set_pair(int mode) { g_pair = (mode == 0 || mode == 1) ? mode : -1; }
 
+int conv_block_n(int cout_pad) {
+    if (cout_pad <= 256) return cout_pad;
+    if (cout_pad % 256 == 0) return 256;
+    for (int n = 192; n >= 64; n -= 64)
+        if (cout_pad % n == 0) return n;
+    return 0;
+}
+
 bool conv_select_pair(ConvParams* p, int cout_pad, int num_sms) {
     int mode = g_pair;
     if (mode < 0) {

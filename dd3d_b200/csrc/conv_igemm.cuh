@@ -95,6 +95,10 @@ void conv_set_n_split(int mode);  // 0 off, 1 on, -1 environment / default (on)
 // the 128-pixel tile and the N-split.  conv_set_pair / DD3D_CONV_PAIR=0: 0 off, 1 on wherever eligible, -1 default.
 bool conv_select_pair(ConvParams* p, int cout_pad, int num_sms);
 void conv_set_pair(int mode);
+// N tile of a layer with cout_pad output channels: cout_pad itself up to 256, 256 for multiples of 256, otherwise the
+// largest multiple of 64 that is <= 256 and divides cout_pad (384 -> 192: every 64-channel store box stays inside its
+// n-block).  0: no such tile (the width is refused).
+int conv_block_n(int cout_pad);
 // Fills num_stages / total_work / tile bookkeeping from the already-set fields.
 void conv_finalize_params(ConvParams* p);
 cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream);

@@ -1,8 +1,8 @@
-// DD3D inference engine: weight folding/packing, static graph for DLA-34 / VoVNetV2-99 + FPN + FCOS2D/3D heads,
-// workspace planning and the forward launch sequence.  Reference structure being reproduced:
+// DD3D inference engine: weight folding/packing, static graph for DLA-34 / every VoVNetV2-eSE variant + FPN + FCOS2D/3D
+// heads, workspace planning and the forward launch sequence.  Reference structure being reproduced:
 //   DD3D.forward                      tridet/modeling/dd3d/core.py:64-164
 //   DLA-34                            tridet/modeling/feature_extractor/dla.py:24-62,146-247,250-361
-//   VoVNetV2-99-eSE                   tridet/modeling/feature_extractor/vovnet.py:79-87,173-273,276-367
+//   VoVNetV2-{19-slim-dw,19-dw,19-slim,19,39,57,99}-eSE   tridet/modeling/feature_extractor/vovnet.py:19-143,173-273,276-367
 //   FPN + LastLevelP6P7 / LastLevelP6 detectron2 (SURVEY.md Appendix A), dla.py:537-561, vovnet.py:411-454
 //   FCOS2DHead / FCOS3DHead           fcos2d.py:30-156, fcos3d.py:55-188 (+ normalization.py Scale/Offset/ModuleListDial)
 // Design notes (DESIGN.md): NHWC bf16 activations; BN folded to fp32 (scale, bias) applied in the conv epilogue;
@@ -37,7 +37,7 @@ void cuda_check(cudaError_t e, const char* what) {
 // ================================================================================================ Engine basics
 
 Engine::Engine(const dd3d_model_desc& d) : desc(d) {
-    if (d.arch != DD3D_ARCH_DLA34 && d.arch != DD3D_ARCH_V2_99) fail(DD3D_ERR_INVALID, "unknown arch");
+    if (d.arch != DD3D_ARCH_DLA34 && vovnet_spec(d.arch) == nullptr) fail(DD3D_ERR_INVALID, "unknown arch");
     if (d.num_classes < 1 || d.num_classes > DD3D_MAX_CLASSES) fail(DD3D_ERR_INVALID, "num_classes out of range");
     if (d.pre_nms_topk < 1 || d.pre_nms_topk * kLevels > 8192) fail(DD3D_ERR_INVALID, "pre_nms_topk out of range");
     if (d.out_cap < 1) fail(DD3D_ERR_INVALID, "out_cap must be positive");
@@ -122,12 +122,8 @@ const ConvLayer& Engine::conv_layer(const std::string& key, const std::vector<st
     }
     L.cout = cout;
     L.cout_pad = round_up(cout, 16);
-    if (L.cout_pad > 256) {
-        if (L.cout_pad % 256) fail(DD3D_ERR_INVALID, "cout > 256 must be a multiple of 256: " + key);
-        L.block_n = 256;
-    } else {
-        L.block_n = L.cout_pad;
-    }
+    L.block_n = conv_block_n(L.cout_pad);  // 384 (slim VoVNet stage 4) -> 192
+    if (L.block_n == 0) fail(DD3D_ERR_INVALID, "cout > 256 needs a multiple of 64 <= 256 that divides it: " + key);
     L.n_blocks = L.cout_pad / L.block_n;
     std::vector<uint16_t> packed(static_cast<size_t>(L.cout_pad) * L.ktot, 0);
     int co0 = 0;
@@ -156,6 +152,23 @@ const ConvLayer& Engine::conv_layer(const std::string& key, const std::vector<st
         if (!make_weight_map_taps(&L.w_map_taps, L.d_w_taps, cin_pad, fp16)) fail(DD3D_ERR_CUDA, conv_last_error());
     }
     return convs.emplace(key, L).first->second;
+}
+
+// Depthwise 3x3 weights [C][1][3][3] -> 16-bit [9][C] (tap-major: one 16-byte load per 8 channels and tap, dwconv.cu).
+const DwLayer& Engine::dw_layer(const std::string& wname, int C) {
+    auto it = dws.find(wname);
+    if (it != dws.end()) return it->second;
+    const HostTensor& w = weight(wname + ".weight");
+    if (w.shape.size() != 4 || w.shape[0] != C || w.shape[1] != 1 || w.shape[2] != 3 || w.shape[3] != 3 || C % 8)
+        fail(DD3D_ERR_INVALID, "bad depthwise conv weight shape: " + wname);
+    std::vector<uint16_t> packed(static_cast<size_t>(9) * C);
+    for (int c = 0; c < C; ++c)
+        for (int t = 0; t < 9; ++t) packed[static_cast<size_t>(t) * C + c] = host_f32_to_act(w.data[static_cast<size_t>(c) * 9 + t], fp16);
+    DwLayer L;
+    L.C = C;
+    L.d_w = static_cast<__nv_bfloat16*>(dev_alloc(packed.size() * 2));
+    cuda_check(cudaMemcpy(L.d_w, packed.data(), packed.size() * 2, cudaMemcpyHostToDevice), "upload depthwise weights");
+    return dws.emplace(wname, L).first->second;
 }
 
 // (scale, bias) of `conv (+bias) -> BN` for channels [0, cout); identity on the padding channels.
@@ -214,6 +227,25 @@ const Epilogue& Engine::bn_epilogue(const std::string& key, const std::string& b
 }
 
 // ================================================================================================ graph builder
+
+// The reference's VoVNet _STAGE_SPECS (vovnet.py:19-97).  eSE is applied in every module whatever the "eSE" flag says
+// (_OSA_module, vovnet.py:216,233), so the flag is not carried.  dd3d_b200/arch.py keeps the copy param_specs needs.
+static const VovSpec kVovSpecs[] = {
+    // arch                     stem            stage_conv_ch          stage_out_ch            layers blocks        dw
+    {DD3D_ARCH_V2_19_SLIM_DW, {64, 64, 64}, {64, 80, 96, 112}, {112, 256, 384, 512}, 3, {1, 1, 1, 1}, true},
+    {DD3D_ARCH_V2_19_DW, {64, 64, 64}, {128, 160, 192, 224}, {256, 512, 768, 1024}, 3, {1, 1, 1, 1}, true},
+    {DD3D_ARCH_V2_19_SLIM, {64, 64, 128}, {64, 80, 96, 112}, {112, 256, 384, 512}, 3, {1, 1, 1, 1}, false},
+    {DD3D_ARCH_V2_19, {64, 64, 128}, {128, 160, 192, 224}, {256, 512, 768, 1024}, 3, {1, 1, 1, 1}, false},
+    {DD3D_ARCH_V2_39, {64, 64, 128}, {128, 160, 192, 224}, {256, 512, 768, 1024}, 5, {1, 1, 2, 2}, false},
+    {DD3D_ARCH_V2_57, {64, 64, 128}, {128, 160, 192, 224}, {256, 512, 768, 1024}, 5, {1, 1, 4, 3}, false},
+    {DD3D_ARCH_V2_99, {64, 64, 128}, {128, 160, 192, 224}, {256, 512, 768, 1024}, 5, {1, 3, 9, 3}, false},
+};
+
+const VovSpec* vovnet_spec(int arch) {
+    for (const VovSpec& s : kVovSpecs)
+        if (s.arch == arch) return &s;
+    return nullptr;
+}
 
 struct Builder {
     Engine* E;
@@ -555,21 +587,57 @@ struct Builder {
         P->ops.push_back(op);
     }
 
-    // ---- VoVNetV2-99-eSE ----------------------------------------------------------------------------------
-    void build_v2_99(View input, std::vector<View>* feats) {
+    // ---- VoVNetV2-eSE (every entry of the reference's _STAGE_SPECS) ----------------------------------------------
+    // depthwise 3x3 (groups = C, no bias / norm / activation)
+    void dwconv(const std::string& wname, View in, View out, int stride) {
+        const DwLayer& L = E->dw_layer(wname, in.C);
+        touch(in);
+        touch(out);
+        ++op_idx;
+        if (dry) return;
+        if (out.C != in.C || out.H != dwconv3x3_out_size(in.H, stride) || out.W != dwconv3x3_out_size(in.W, stride))
+            fail(DD3D_ERR_INVALID, "depthwise conv output view mismatch: " + wname);
+        Op op;
+        op.type = Op::DW;
+        op.in = in;
+        op.out = out;
+        op.stride = stride;
+        op.dw = &L;
+        op.outs[0] = out;
+        op.nouts = 1;
+        const double out_px = static_cast<double>(B) * out.H * out.W, in_px = static_cast<double>(B) * in.H * in.W;
+        op.flops = 2.0 * out_px * L.C * 9;
+        op.bytes = (in_px + out_px) * L.C * 2;
+        P->ops.push_back(op);
+    }
+
+    // 3x3 conv -> norm -> ReLU (conv3x3, vovnet.py:124-143), or for the -dw variants depthwise 3x3 -> pointwise 1x1 ->
+    // pw_norm -> ReLU (dw_conv3x3, vovnet.py:100-121) through a depthwise output buffer
+    void vov_conv3x3(const std::string& n, View in, View out, int stride, bool dw) {
+        if (!dw) {
+            conv1(n + "/conv", n + "/norm", false, in, out, 3, stride, true);
+            return;
+        }
+        View t = alloc(out.H, out.W, in.C);
+        dwconv(n + "/dw_conv3x3", in, t, stride);
+        conv1(n + "/pw_conv1x1", n + "/pw_norm", false, t, out, 1, 1, true);
+    }
+
+    void build_vovnet(const VovSpec& S, View input, std::vector<View>* feats) {
         const std::string p = "backbone.bottom_up";
         const int H = input.H, W = input.W;
-        static const int stage_ch[4] = {128, 160, 192, 224};
-        static const int out_ch[4] = {256, 512, 768, 1024};
-        static const int blocks[4] = {1, 3, 9, 3};
-        View s1 = alloc(H / 2, W / 2, 64);
+        const int* stage_ch = S.stage_ch;
+        const int* out_ch = S.out_ch;
+        const int* blocks = S.blocks;
+        const int nl = S.layers;
+        View s1 = alloc(H / 2, W / 2, S.stem[0]);
         stem(p + ".stem.stem_1/conv", p + ".stem.stem_1/norm", input, s1, 3, 2);
-        View s2 = alloc(H / 2, W / 2, 64);
-        conv1(p + ".stem.stem_2/conv", p + ".stem.stem_2/norm", false, s1, s2, 3, 1, true);
+        View s2 = alloc(H / 2, W / 2, S.stem[1]);
+        vov_conv3x3(p + ".stem.stem_2", s1, s2, 1, S.dw);
         int h = H / 4, w = W / 4;
-        int in_ch = 128;
-        View cat = alloc(h, w, in_ch + 5 * stage_ch[0]);
-        conv1(p + ".stem.stem_3/conv", p + ".stem.stem_3/norm", false, s2, slice(cat, 0, in_ch), 3, 2, true);
+        int in_ch = S.stem[2];
+        View cat = alloc(h, w, in_ch + nl * stage_ch[0]);
+        vov_conv3x3(p + ".stem.stem_3", s2, slice(cat, 0, in_ch), 2, S.dw);
         View stage_out;
         View pooled_cat;  // next stage's concat buffer when its pooled slice was produced by the previous stage's eSE pass
         for (int si = 0; si < 4; ++si) {
@@ -579,7 +647,7 @@ struct Builder {
                 if (pooled_cat.ptr != nullptr || pooled_cat.buf >= 0) {
                     cat = pooled_cat;  // the previous stage's last eSE pass already wrote the pooled map (ese_scale_pool_kernel)
                 } else {
-                    cat = alloc(hp, wp, in_ch + 5 * sc);
+                    cat = alloc(hp, wp, in_ch + nl * sc);
                     maxpool(stage_out, slice(cat, 0, in_ch), 3);
                 }
                 h = hp;
@@ -592,10 +660,17 @@ struct Builder {
                 View x = slice(cat, 0, in_ch);
                 int c0 = in_ch;
                 View prev = x;
-                for (int i = 0; i < 5; ++i) {
+                if (S.dw && in_ch != sc) {
+                    // conv_reduction (vovnet.py:200-205,221-222): feeds layer 0 only; the concat keeps the unreduced input
+                    View r = alloc(h, w, sc);
+                    const std::string rn = q + ".conv_reduction." + name + "_reduction_0";
+                    conv1(rn + "/conv", rn + "/norm", false, x, r, 1, 1, true);
+                    prev = r;
+                }
+                for (int i = 0; i < nl; ++i) {
                     const std::string ln = q + ".layers." + std::to_string(i) + "." + name + "_" + std::to_string(i);
                     View o = slice(cat, c0, sc);
-                    conv1(ln + "/conv", ln + "/norm", false, prev, o, 3, 1, true);
+                    vov_conv3x3(ln, prev, o, 1, S.dw);
                     prev = o;
                     c0 += sc;
                 }
@@ -611,11 +686,11 @@ struct Builder {
                     dst = alloc(h, w, oc);
                     if (si < 3 && E->opt_ese_pool && h >= 3 && w >= 3) {
                         // the eSE scale pass of a stage's last module also writes the next stage's 3x3 / s2 pooled input
-                        pooled_next = alloc((h - 3 + 1) / 2 + 1, (w - 3 + 1) / 2 + 1, oc + 5 * stage_ch[si + 1]);
+                        pooled_next = alloc((h - 3 + 1) / 2 + 1, (w - 3 + 1) / 2 + 1, oc + nl * stage_ch[si + 1]);
                         pooled = slice(pooled_next, 0, oc);
                     }
                 } else {
-                    next_cat = alloc(h, w, oc + 5 * sc);
+                    next_cat = alloc(h, w, oc + nl * sc);
                     dst = slice(next_cat, 0, oc);
                 }
                 ese(q + ".ese.fc", xt, b > 0 ? &x : nullptr, dst, pooled.buf >= 0 ? &pooled : nullptr);
@@ -1092,7 +1167,7 @@ size_t Engine::build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry) 
             bld.build_dla34(input, &feats);
             bld.build_fpn(feats, 3, &fpn);
         } else {
-            bld.build_v2_99(input, &feats);
+            bld.build_vovnet(*vovnet_spec(desc.arch), input, &feats);
             bld.build_fpn(feats, 2, &fpn);
         }
         if (static_cast<int>(fpn.size()) != kLevels) fail(DD3D_ERR_STATE, "internal: expected 5 FPN levels");
@@ -1386,8 +1461,13 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
                                             op.identity.pitch, P.B, op.in.H, op.in.W, num_sms, stream, fp16),
                            "dla front");
                 break;
+            case Op::DW:
+                cuda_check(launch_dwconv3x3(op.in.ptr, P.B, op.in.H, op.in.W, op.in.C, op.in.pitch, op.dw->d_w, op.stride,
+                                            op.out.ptr, op.out.pitch, stream, fp16),
+                           "depthwise conv");
+                break;
         }
-        mark((op.type == Op::STEM || op.type == Op::FRONT) ? 1 : op.type == Op::CONV ? 2 : op.type == Op::POOL ? 3 : op.type == Op::ESE ? 4 : 5);
+        mark((op.type == Op::STEM || op.type == Op::FRONT || op.type == Op::DW) ? 1 : op.type == Op::CONV ? 2 : op.type == Op::POOL ? 3 : op.type == Op::ESE ? 4 : 5);
     }
     DecodeParams dp = P.decode;
     dp.K = d_K;
@@ -1465,6 +1545,7 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
                 bytes[5] += in_px * op.in.C * 4;
                 break;
             case Op::FRONT:
+            case Op::DW:  // special-purpose conv kernels are counted with the stems, so category 2 stays wgmma-only
                 launches[1] += 1;
                 flops[1] += op.flops;
                 bytes[1] += op.bytes;

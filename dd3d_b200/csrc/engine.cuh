@@ -71,9 +71,25 @@ struct EseLayer {
     float* d_b;
     int C;
 };
+struct DwLayer {  // depthwise 3x3 weights, 16-bit [9][C]
+    __nv_bfloat16* d_w;
+    int C;
+};
+
+// One VoVNet variant (reference _STAGE_SPECS, vovnet.py:19-97); the table is in engine.cu
+struct VovSpec {
+    int arch;  // dd3d_arch
+    int stem[3];
+    int stage_ch[4];
+    int out_ch[4];
+    int layers;  // layer_per_block
+    int blocks[4];
+    bool dw;  // depthwise 3x3 layers (and stem_2 / stem_3) with 1x1 conv_reduction where in_ch != stage_ch
+};
+const VovSpec* vovnet_spec(int arch);  // nullptr: not a VoVNet arch
 
 struct Op {
-    enum Type { CONV, STEM, POOL, ESE, RELU, FRONT } type;
+    enum Type { CONV, STEM, POOL, ESE, RELU, FRONT, DW } type;
     ConvParams conv;
     View in, out, identity;
     View outs[kMaxSeg];  // bf16 output views (CONV: one per segment; others: outs[0] == out), for dd3d_get_tensor "op<i>"
@@ -83,6 +99,7 @@ struct Op {
     const StemLayer* stem = nullptr;
     const EseLayer* ese = nullptr;
     const FrontLayer* front = nullptr;  // FRONT: in = input, out = level1 output, identity = its 2x2 max-pool
+    const DwLayer* dw = nullptr;        // DW: depthwise 3x3 of `in` into `out` with `stride`
     float* f0 = nullptr;
     float* f1 = nullptr;
     float* f2 = nullptr;
@@ -159,7 +176,7 @@ class Engine {
                          cudaStream_t stream);
     void drop_plans();  // frees the active and the cached plans (an option that changes the op graph was flipped)
     int launches_per_forward() const;
-    // categories: 0 preprocess, 1 stem, 2 conv (wgmma), 3 pool, 4 eSE, 5 relu, 6 decode, 7 nms
+    // categories: 0 preprocess, 1 stem and depthwise conv, 2 conv (wgmma), 3 pool, 4 eSE, 5 relu, 6 decode, 7 nms
     void get_profile(double* ms, double* flops, double* bytes, int32_t* launches);
     int get_op_times(float* ms, int32_t* cats, double* flops, int max_ops);
 
@@ -175,6 +192,7 @@ class Engine {
     const StemLayer& stem_layer(const std::string& wname, const std::string& bn, int ksize, int stride);
     const EseLayer& ese_layer(const std::string& fc, int C);
     const FrontLayer& front_layer(const std::string& prefix);
+    const DwLayer& dw_layer(const std::string& wname, int C);
 
     dd3d_model_desc desc;
     int device = 0;
@@ -200,6 +218,7 @@ class Engine {
     std::map<std::string, StemLayer> stems;
     std::map<std::string, EseLayer> eses;
     std::map<std::string, FrontLayer> fronts;
+    std::map<std::string, DwLayer> dws;
     std::vector<void*> device_allocs;
     float* d_canon = nullptr;
     Plan plan;

@@ -50,6 +50,12 @@ cudaError_t launch_ese_fused(const __nv_bfloat16* x, int x_pitch, const float* t
                              cudaStream_t stream, int fp16 = 0, __nv_bfloat16* pool = nullptr, int pool_pitch = 0, int H = 0,
                              int W = 0);  // pool != null: also writes the 3x3 / s2 ceil-mode max-pool of `out` (H * W == HW)
 
+// Depthwise 3x3 conv, padding 1, stride 1 or 2 (dwconv.cu): in / out NHWC 16-bit with channel pitches, w 16-bit [9][C]
+// (tap = r * 3 + s); fp32 accumulation in tap order, no bias / norm / activation.  C, both pitches multiples of 8.
+int dwconv3x3_out_size(int n, int stride);
+cudaError_t launch_dwconv3x3(const __nv_bfloat16* in, int B, int H, int W, int C, int in_pitch, const __nv_bfloat16* w,
+                             int stride, __nv_bfloat16* out, int out_pitch, cudaStream_t stream, int fp16 = 0);
+
 cudaError_t launch_relu(const __nv_bfloat16* x, __nv_bfloat16* out, size_t n_elems, int num_sms, cudaStream_t stream);
 
 }  // namespace dd3d

@@ -12,6 +12,9 @@ LIB_PATH = os.path.join(_HERE, "_lib", "libdd3d_b200.so")
 MAX_CLASSES = 16
 NUM_LEVELS = 5
 ARCH_DLA34, ARCH_V2_99 = 0, 1
+# dd3d_arch of every arch key (dd3d_b200.arch.ARCH_KEYS)
+ARCH_IDS = {"dla34": ARCH_DLA34, "v2_99": ARCH_V2_99, "v2_19_slim_dw": 2, "v2_19_dw": 3, "v2_19_slim": 4, "v2_19": 5,
+            "v2_39": 6, "v2_57": 7}
 IMG_U8, IMG_F32 = 0, 1
 ACT_BF16, ACT_FP16 = 0, 1
 POSE_GLOBAL, POSE_CAMERA = 0, 1
@@ -93,6 +96,7 @@ SIGNATURES = {
     "dd3d_op_dla_front": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_s2_mma": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_conv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "dd3d_op_dwconv3x3": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _I, _P]),
     "dd3d_op_preprocess": (_I, [_P, _I, _P, _P, _I, _I, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
     "dd3d_op_maxpool": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "dd3d_op_ese": (_I, [_P, _I, _P, _P, _P, _I, _P, _I, _P, _I, _I, _I, _P]),
@@ -139,7 +143,7 @@ def desc_from_cfg(cfg, out_cap=None):
     """dd3d_model_desc from the reference-style cfg tree (the fields DD3D.__init__ reads, core.py:20-55)."""
     from .arch import arch_of
     d = ModelDesc()
-    d.arch = ARCH_DLA34 if arch_of(cfg) == "dla34" else ARCH_V2_99
+    d.arch = ARCH_IDS[arch_of(cfg)]
     d.num_classes = cfg.DD3D.NUM_CLASSES
     for i in range(3):
         d.pixel_mean[i] = cfg.MODEL.PIXEL_MEAN[i]

@@ -52,7 +52,7 @@ def make_state_dict(cfg, seed=0, gains=None):
         role = kind.split(":")[1] if ":" in kind else ""
         layer = name.rsplit(".", 1)[0]
         if base == "conv":
-            fan_in = shape[1] * shape[2] * shape[3]
+            fan_in = shape[1] * shape[2] * shape[3]  # role "dw" (depthwise [C, 1, 3, 3]): fan-in 9
             gain = gains.get(layer, 1.0)
             if role == "cls_logits":
                 gain = gains.get(layer, 1.0)

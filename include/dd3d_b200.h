@@ -35,7 +35,19 @@ enum dd3d_status {
     DD3D_ERR_MISSING = -4   /* a weight the architecture needs was never loaded */
 };
 
-enum dd3d_arch { DD3D_ARCH_DLA34 = 0, DD3D_ARCH_V2_99 = 1 };
+/* FE.BUILDER build_fcos_dla_fpn_backbone_p67 with FE.BACKBONE.NAME "DLA-34", or build_fcos_vovnet_fpn_backbone_p6 with the
+ * VoVNet named by FE.BACKBONE.NAME (vovnet.py:19-97): "V-99-eSE" (1), "V-19-slim-dw-eSE", "V-19-dw-eSE", "V-19-slim-eSE",
+ * "V-19-eSE", "V-39-eSE", "V-57-eSE" (2..7).  Every VoVNet has FPN levels p2..p6 and a size divisibility of 64. */
+enum dd3d_arch {
+    DD3D_ARCH_DLA34 = 0,
+    DD3D_ARCH_V2_99 = 1,
+    DD3D_ARCH_V2_19_SLIM_DW = 2,
+    DD3D_ARCH_V2_19_DW = 3,
+    DD3D_ARCH_V2_19_SLIM = 4,
+    DD3D_ARCH_V2_19 = 5,
+    DD3D_ARCH_V2_39 = 6,
+    DD3D_ARCH_V2_57 = 7
+};
 enum dd3d_image_dtype { DD3D_IMG_U8 = 0, DD3D_IMG_F32 = 1 };
 /* 16-bit storage type of activations and conv weights (accumulation, BN affine, head maps, decode and NMS are fp32
  * either way).  bf16 is the default; fp16 is the reference's mixed-precision type (amp.autocast, scripts/train.py:121;
@@ -48,7 +60,7 @@ enum dd3d_act_dtype { DD3D_ACT_BF16 = 0, DD3D_ACT_FP16 = 1 };
 /* Mirrors the cfg values DD3D.__init__ / FCOS2DInference / FCOS3DInference read
  * (core.py:20-55, fcos2d.py:242-249, fcos3d.py:302-313; defaults configs/models/dd3d.yaml). */
 typedef struct dd3d_model_desc {
-    int32_t arch;        /* dd3d_arch: FE.BUILDER build_fcos_dla_fpn_backbone_p67 / build_fcos_vovnet_fpn_backbone_p6 */
+    int32_t arch;        /* dd3d_arch: FE.BUILDER + FE.BACKBONE.NAME */
     int32_t num_classes; /* DD3D.NUM_CLASSES (<= DD3D_MAX_CLASSES) */
     float pixel_mean[3]; /* MODEL.PIXEL_MEAN (BGR) */
     float pixel_std[3];  /* MODEL.PIXEL_STD */
@@ -184,8 +196,8 @@ int dd3d_launches_per_forward(dd3d_handle h);
 
 /* Per-category device time of the LAST dd3d_forward issued with option "profile" = 1 (CUDA events recorded on the
  * launch stream around every op), with the algorithmic FLOPs / HBM bytes and launch counts of one forward.
- * Categories (arrays of 8): 0 preprocess, 1 stem conv, 2 wgmma implicit-GEMM conv, 3 max-pool, 4 eSE, 5 relu,
- * 6 decode, 7 NMS. */
+ * Categories (arrays of 8): 0 preprocess, 1 special-purpose conv kernels (stem convs, the fused DLA-34 front end and the
+ * depthwise 3x3 convs of the VoVNet -dw variants), 2 wgmma implicit-GEMM conv, 3 max-pool, 4 eSE, 5 relu, 6 decode, 7 NMS. */
 int dd3d_get_profile(dd3d_handle h, double* h_ms, double* h_flops, double* h_bytes, int32_t* h_launches);
 /* Same events, per op in launch order (entry 0 = preprocess, then every engine op, then decode, NMS): device ms,
  * category and algorithmic FLOPs.  Returns the number of entries written (<= max_ops). */
@@ -273,6 +285,12 @@ int dd3d_op_dla_front(const void* d_in4, const void* d_w0, const void* d_w1, con
  * c = 3 zero), d_sb = fp32 scale[64] | bias[64], d_out = [B][ceil(H/2)][ceil(W/2)][out_pitch]. */
 int dd3d_op_stem_s2_mma(const void* d_in4, const void* d_w, const float* d_sb, void* d_out, int out_pitch, int B, int H, int W,
                         dd3d_stream stream);
+/* dd3d_op_dwconv3x3: depthwise 3x3 conv (groups = C, padding 1, no bias; vovnet.py:100-121 dw_conv3x3) on the kernel the
+ * engine runs for the VoVNet -dw variants (csrc/dwconv.cu).  d_in = [B][H][W][in_pitch], d_w = 16-bit [9][C] (tap = ky * 3
+ * + kx), d_out = [B][(H-1)/stride+1][(W-1)/stride+1][out_pitch]; stride 1 or 2; C and both pitches multiples of 8, all three
+ * pointers 16-byte aligned.  fp32 accumulation in tap order, one rounding to the 16-bit type at the store. */
+int dd3d_op_dwconv3x3(const void* d_in, int B, int H, int W, int C, int in_pitch, const void* d_w, int stride, void* d_out,
+                      int out_pitch, dd3d_stream stream);
 int dd3d_op_preprocess(const void* d_images, int img_dtype, const int32_t* d_sizes2, void* d_out4, int B, int Hs, int Ws,
                        int Hp, int Wp, const float* h_mean, const float* h_std, dd3d_stream stream);
 int dd3d_op_maxpool(const void* d_in, void* d_out, int B, int H, int W, int C, int in_pitch, int out_pitch, int ksize,
