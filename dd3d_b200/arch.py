@@ -8,7 +8,8 @@ reference's own state_dict when /root/reference is present.
 """
 from collections import OrderedDict
 
-# kind tags: "conv" (weight, fan-in init), "bias", "bn_w", "bn_b", "bn_mean", "bn_var", "nbt", "scalar", "buffer"
+# kind tags: "conv" (weight, fan-in init), "bias", "bn_w", "bn_b", "bn_mean", "bn_var", "nbt", "gn_w", "gn_b", "scalar",
+# "buffer"
 
 
 def _conv(specs, name, cout, cin, k, bias=False, role="relu"):
@@ -24,6 +25,18 @@ def _bn(specs, name, c, frozen=True):
     specs[name + ".running_var"] = ((c, ), "bn_var")
     if not frozen:
         specs[name + ".num_batches_tracked"] = ((), "nbt")
+
+
+def _norm(specs, name, c, norm):
+    """get_norm(norm, c) as `name` (ref_standin.get_norm / detectron2): BatchNorm2d ("BN", "SyncBN") has
+    num_batches_tracked, FrozenBatchNorm2d does not, GroupNorm(32, c) has an affine only; "" adds nothing.  Any other
+    string raises KeyError like get_norm's dict lookup."""
+    kind = {"BN": "bn", "SyncBN": "bn", "FrozenBN": "frozen", "GN": "gn", "": None}[norm]
+    if kind == "gn":
+        specs[name + ".weight"] = ((c, ), "gn_w")
+        specs[name + ".bias"] = ((c, ), "gn_b")
+    elif kind is not None:
+        _bn(specs, name, c, frozen=kind == "frozen")
 
 
 def _conv_bn(specs, name, cout, cin, k, role="relu"):
@@ -132,10 +145,12 @@ def param_specs(cfg):
     else:
         feats = _vovnet(specs, arch)
         stages = {"stage2": 2, "stage3": 3, "stage4": 4, "stage5": 5}
+    fpn_norm = cfg.FE.FPN.NORM  # detectron2 FPN: bias only without a norm; one norm per conv
     for name, ch in feats.items():
         st = stages[name]
-        _conv_bn(specs, f"backbone.fpn_lateral{st}", 256, ch, 1, role="linear")
-        _conv_bn(specs, f"backbone.fpn_output{st}", 256, 256, 3, role="linear")
+        for conv, cin, k in ((f"backbone.fpn_lateral{st}", ch, 1), (f"backbone.fpn_output{st}", 256, 3)):
+            _conv(specs, conv, 256, cin, k, bias=fpn_norm == "", role="linear")
+            _norm(specs, conv + ".norm", 256, fpn_norm)
     _conv(specs, "backbone.top_block.p6", 256, 256, 3, bias=True, role="linear")
     if arch == "dla34":
         _conv(specs, "backbone.top_block.p7", 256, 256, 3, bias=True, role="linear")
@@ -144,14 +159,20 @@ def param_specs(cfg):
     L = 5
     f2, f3 = cfg.DD3D.FCOS2D, cfg.DD3D.FCOS3D
     box3d_on = bool(cfg.MODEL.BOX3D_ON)  # core.py:34-40: no FCOS3D head at all when off
-    towers = [("fcos2d_head.cls_tower", False), ("fcos2d_head.box2d_tower", False)]
+    # fcos2d.py:46-91, fcos3d.py:75-112: NUM_*_CONVS x Conv2d(bias = no norm, norm); BN / FrozenBN one per level
+    # (ModuleListDial), any other norm one shared by the levels
+    towers = [("fcos2d_head.cls_tower", f2.NUM_CLS_CONVS, f2.NORM), ("fcos2d_head.box2d_tower", f2.NUM_BOX_CONVS, f2.NORM)]
     if box3d_on:
-        towers.append(("fcos3d_head.box3d_tower", True))
-    for tower, frozen in towers:
-        for i in range(4):
-            _conv(specs, f"{tower}.{i}", 256, 256, 3)
-            for l in range(L):
-                _bn(specs, f"{tower}.{i}.norm.{l}", 256, frozen=frozen)
+        towers.append(("fcos3d_head.box3d_tower", f3.NUM_CONVS, f3.NORM))
+    for tower, depth, norm in towers:
+        _norm({}, "", 256, norm)  # KeyError for an unknown NORM even at depth 0
+        for i in range(depth):
+            _conv(specs, f"{tower}.{i}", 256, 256, 3, bias=norm == "")
+            if norm in ("BN", "FrozenBN"):
+                for l in range(L):
+                    _norm(specs, f"{tower}.{i}.norm.{l}", 256, norm)
+            else:
+                _norm(specs, f"{tower}.{i}.norm", 256, norm)
     _conv(specs, "fcos2d_head.cls_logits", C, 256, 3, bias=True, role="cls_logits")
     _conv(specs, "fcos2d_head.box2d_reg", 4, 256, 3, bias=True, role="box2d_reg")
     _conv(specs, "fcos2d_head.centerness", 1, 256, 3, bias=True, role="centerness")

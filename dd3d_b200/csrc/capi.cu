@@ -77,6 +77,11 @@ const char* dd3d_last_error(dd3d_handle h) { return h ? h->err.c_str() : g_creat
 
 int dd3d_size_divisibility(dd3d_handle h) { return (h && h->eng) ? h->eng->size_divisibility() : DD3D_ERR_INVALID; }
 
+int dd3d_set_layout(dd3d_handle h, const dd3d_layout_desc* layout) {
+    if (layout == nullptr) return DD3D_ERR_INVALID;
+    return guarded(h, [&](Engine& e) { e.set_layout(*layout); });
+}
+
 int dd3d_load_weight(dd3d_handle h, const char* name, const float* data, const int64_t* shape, int ndim) {
     if (name == nullptr || data == nullptr || (ndim > 0 && shape == nullptr) || ndim < 0 || ndim > 8)
         return DD3D_ERR_INVALID;
@@ -455,6 +460,42 @@ int dd3d_op_dwconv3x3(const void* d_in, int B, int H, int W, int C, int in_pitch
                                         static_cast<const __nv_bfloat16*>(d_w), stride, static_cast<__nv_bfloat16*>(d_out),
                                         out_pitch, static_cast<cudaStream_t>(stream), g_op_fp16),
                        nullptr);
+}
+
+int64_t dd3d_op_group_norm_scratch_bytes(int B, int H, int W) {
+    if (B < 1 || H < 1 || W < 1) return DD3D_ERR_INVALID;
+    return static_cast<int64_t>(group_norm_scratch_bytes(B, H, W));
+}
+
+int dd3d_op_group_norm(const void* d_in, int B, int H, int W, int in_pitch, const float* d_gamma, const float* d_beta, int relu,
+                       const void* d_residual, int res_pitch, int avg, void* d_out, int out_pitch, void* d_scratch,
+                       dd3d_stream stream) {
+    if (!d_in || !d_out || (d_gamma == nullptr) != (d_beta == nullptr) || (d_gamma && !d_scratch)) return DD3D_ERR_INVALID;
+    if (B < 1 || H < 1 || W < 1) return DD3D_ERR_INVALID;
+    GroupNormParams p;
+    p.nseg = 1;
+    p.B = B;
+    p.gamma = d_gamma;
+    p.beta = d_beta;
+    p.relu = relu ? 1 : 0;
+    p.avg = avg ? 1 : 0;
+    p.fp16 = g_op_fp16;
+    GroupNormSeg& g = p.seg[0];
+    g.in = static_cast<const __nv_bfloat16*>(d_in);
+    g.out = static_cast<__nv_bfloat16*>(d_out);
+    g.H = H;
+    g.W = W;
+    g.in_pitch = in_pitch;
+    g.out_pitch = out_pitch;
+    if (d_residual) {
+        g.res = static_cast<const __nv_bfloat16*>(d_residual);
+        g.res_pitch = res_pitch;
+        g.res_H = (H + 1) / 2;
+        g.res_W = (W + 1) / 2;
+    }
+    g.part = static_cast<float2*>(d_scratch);
+    const cudaError_t e = launch_group_norm(p, static_cast<cudaStream_t>(stream));
+    return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
 }
 
 int dd3d_op_preprocess(const void* d_images, int img_dtype, const int32_t* d_sizes2, void* d_out4, int B, int Hs, int Ws,

@@ -171,6 +171,28 @@ const DwLayer& Engine::dw_layer(const std::string& wname, int C) {
     return dws.emplace(wname, L).first->second;
 }
 
+void Engine::set_layout(const dd3d_layout_desc& l) {
+    if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_layout after finalize");
+    for (int n : {l.fcos2d_norm, l.fcos3d_norm, l.fpn_norm})
+        if (n < DD3D_NORM_BN_PER_LEVEL || n > DD3D_NORM_NONE) fail(DD3D_ERR_INVALID, "unknown dd3d_norm value");
+    for (int d : {l.num_cls_convs, l.num_box2d_convs, l.num_box3d_convs})
+        if (d < 0 || d > 16) fail(DD3D_ERR_INVALID, "tower depth outside 0..16");
+    if (l.fpn_fuse_avg != 0 && l.fpn_fuse_avg != 1) fail(DD3D_ERR_INVALID, "fpn_fuse_avg must be 0 or 1");
+    layout = l;
+}
+
+// GroupNorm(32, C) affine of `<prefix>.weight` / `<prefix>.bias`, uploaded as fp32 vectors (cached like the epilogues)
+const Epilogue& Engine::gn_affine(const std::string& prefix) {
+    const std::string key = "gn|" + prefix;
+    auto it = epis.find(key);
+    if (it != epis.end()) return it->second;
+    const HostTensor& g = weight(prefix + ".weight");
+    const HostTensor& b = weight(prefix + ".bias");
+    if (g.data.size() != static_cast<size_t>(kGnChannels) || b.data.size() != static_cast<size_t>(kGnChannels))
+        fail(DD3D_ERR_INVALID, "bad GroupNorm shape: " + prefix);
+    return epilogue(key, g.data, b.data, nullptr);
+}
+
 // (scale, bias) of `conv (+bias) -> BN` for channels [0, cout); identity on the padding channels.
 void Engine::bn_fold(const std::string& bn_prefix, const std::string& conv_bias_name, int cout, std::vector<float>* scale,
                      std::vector<float>* bias) const {
@@ -441,6 +463,50 @@ struct Builder {
             segs[0].res_up2 = res_up2;
         }
         conv(L, stride, relu, segs, false);
+    }
+
+    // GroupNorm (affine != nullptr) or the add / scale alone, in place on every map of `x`: + nearest-2x(res[s]) when
+    // res is given, * 0.5 when avg, ReLU when relu (group_norm.cu).  Statistics scratch in the persistent region.
+    void group_norm(const std::vector<View>& x, const Epilogue* affine, bool relu, const View* res, bool avg) {
+        std::vector<float*> part(x.size(), nullptr);
+        for (size_t s = 0; s < x.size(); ++s) {
+            touch(x[s]);
+            if (res) touch(res[s]);
+            if (affine) part[s] = alloc_f32(group_norm_scratch_bytes(B, x[s].H, x[s].W) / 4);
+        }
+        ++op_idx;
+        if (dry) return;
+        Op op;
+        op.type = Op::GN;
+        GroupNormParams& p = op.gn;
+        p.nseg = static_cast<int>(x.size());
+        p.B = B;
+        p.gamma = affine ? affine->d_scale : nullptr;
+        p.beta = affine ? affine->d_bias : nullptr;
+        p.relu = relu ? 1 : 0;
+        p.avg = avg ? 1 : 0;
+        p.fp16 = E->fp16;
+        for (size_t s = 0; s < x.size(); ++s) {
+            if (x[s].C != kGnChannels) fail(DD3D_ERR_INVALID, "GroupNorm needs 256 channels");
+            GroupNormSeg& g = p.seg[s];
+            g.in = x[s].ptr;
+            g.out = x[s].ptr;
+            g.H = x[s].H;
+            g.W = x[s].W;
+            g.in_pitch = g.out_pitch = x[s].pitch;
+            if (res) {
+                g.res = res[s].ptr;
+                g.res_pitch = res[s].pitch;
+                g.res_H = res[s].H;
+                g.res_W = res[s].W;
+            }
+            g.part = reinterpret_cast<float2*>(part[s]);
+            op.outs[s] = x[s];
+            const double px = static_cast<double>(B) * x[s].H * x[s].W * kGnChannels * 2;
+            op.bytes += px * (affine ? 3 : 2) + (res ? px / 4 : 0.0);  // stats read, apply read + write, residual read
+        }
+        op.nouts = p.nseg;
+        P->ops.push_back(op);
     }
 
     void maxpool(View in, View out, int ksize) {
@@ -749,23 +815,35 @@ struct Builder {
     void build_fpn(const std::vector<View>& feats, int first_stage, std::vector<View>* outs) {
         const std::string p = "backbone";
         const int n = static_cast<int>(feats.size());
+        // FE.FPN.NORM: BN (folded into the conv epilogue), "" (biased convs) or GN (identity epilogue, then a GN op);
+        // FUSE_TYPE avg halves lateral + top-down.  The add follows the norm (detectron2 FPN.forward), so with GN or avg it
+        // moves from the lateral conv's epilogue into the GN apply pass.
+        const int norm = E->layout.fpn_norm;
+        const bool gn = norm == DD3D_NORM_GN, bn = norm == DD3D_NORM_BN_SHARED || norm == DD3D_NORM_BN_PER_LEVEL;
+        const bool avg = E->layout.fpn_fuse_avg != 0;
+        auto conv_norm = [&](const std::string& name, View in, View out, int ksize, const View* res) {
+            conv1(name, bn ? name + ".norm" : "", norm == DD3D_NORM_NONE, in, out, ksize, 1, false, res, res != nullptr);
+        };
         std::vector<View> res(n);
         View prev;
         for (int i = n - 1; i >= 0; --i) {
             const std::string st = std::to_string(first_stage + i);
+            const std::string lname = p + ".fpn_lateral" + st, oname = p + ".fpn_output" + st;
             const View& c = feats[i];
             View lat = alloc(c.H, c.W, 256);
-            if (i == n - 1) {
-                conv1(p + ".fpn_lateral" + st, p + ".fpn_lateral" + st + ".norm", false, c, lat, 1, 1, false);
+            if (i == n - 1 || gn || avg) {
+                conv_norm(lname, c, lat, 1, nullptr);
+                const bool add = i != n - 1;
+                if (gn || add) group_norm({lat}, gn ? &E->gn_affine(lname + ".norm") : nullptr, false, add ? &prev : nullptr, add && avg);
             } else {
                 // lateral + nearest-2x(prev): the un-smoothed `prev` is what propagates downwards
-                conv1(p + ".fpn_lateral" + st, p + ".fpn_lateral" + st + ".norm", false, c, lat, 1, 1, false, &prev,
-                      true);
+                conv_norm(lname, c, lat, 1, &prev);
             }
             prev = lat;
             res[i] = alloc(c.H, c.W, 256);
             persist(res[i]);
-            conv1(p + ".fpn_output" + st, p + ".fpn_output" + st + ".norm", false, lat, res[i], 3, 1, false);
+            conv_norm(oname, lat, res[i], 3, nullptr);
+            if (gn) group_norm({res[i]}, &E->gn_affine(oname + ".norm"), false, nullptr, false);
         }
         *outs = res;
         const View& p5 = res[n - 1];
@@ -784,22 +862,33 @@ struct Builder {
     }
 
     // ---- heads ------------------------------------------------------------------------------------------------
-    void tower(const std::string& tp, const std::vector<View>& feats, std::vector<View>* out) {
+    // `depth` x (3x3 conv -> norm -> ReLU) over every level in one launch per layer (fcos2d.py:55-91, fcos3d.py:81-112).
+    // norm: per-level BN (ModuleListDial, folded per segment), shared BN (one folded epilogue), none (conv bias), or GN
+    // (identity epilogue, then one GN op over the levels).  Depth 0: the FPN outputs themselves.
+    void tower(const std::string& tp, int depth, int norm, const std::vector<View>& feats, std::vector<View>* out) {
         std::vector<View> cur = feats;
         std::vector<View> buf[2];
-        for (int k = 0; k < 2; ++k)
+        for (int k = 0; k < std::min(depth, 2); ++k)
             for (auto& f : feats) buf[k].push_back(alloc(f.H, f.W, 256));
-        for (int i = 0; i < 4; ++i) {
+        for (int i = 0; i < depth; ++i) {
             const std::string wn = tp + "." + std::to_string(i);
             const ConvLayer& L = E->conv_layer(wn, {wn}, 256, 3);
             std::vector<SegSpec> segs(feats.size());
             for (size_t l = 0; l < feats.size(); ++l) {
-                const std::string bn = wn + ".norm." + std::to_string(l);  // ModuleListDial: level l -> norm l
                 segs[l].in = cur[l];
                 segs[l].out = buf[i & 1][l];
-                segs[l].epi = &E->bn_epilogue(wn + "|" + bn, bn, "", 256);
+                if (norm == DD3D_NORM_BN_PER_LEVEL) {
+                    const std::string bn = wn + ".norm." + std::to_string(l);  // ModuleListDial: level l -> norm l
+                    segs[l].epi = &E->bn_epilogue(wn + "|" + bn, bn, "", 256);
+                } else if (norm == DD3D_NORM_BN_SHARED) {
+                    segs[l].epi = &E->bn_epilogue(wn + "|" + wn + ".norm", wn + ".norm", "", 256);
+                } else {  // none: conv bias; GN: raw conv output, normalised by the GN op below
+                    segs[l].epi = &E->bn_epilogue(wn + "|", "", norm == DD3D_NORM_NONE ? wn + ".bias" : "", 256);
+                }
             }
-            conv(L, 1, true, segs, false);
+            const bool gn = norm == DD3D_NORM_GN;
+            conv(L, 1, !gn, segs, false);
+            if (gn) group_norm(buf[i & 1], &E->gn_affine(wn + ".norm"), true, nullptr, false);
             cur = buf[i & 1];
         }
         *out = cur;
@@ -842,7 +931,7 @@ struct Builder {
         // cls_logits (fcos2d.py:96,142): bias only, shared across levels.  NuscenesDD3D adds attr_logits (3) and
         // relu(speed) (1) on the same tower output (nuscenes_dd3d.py:311-312,380-383): fused as extra GEMM columns
         // [cls C | attr 3 | speed 1] of the one predictor conv (still N = 16 for the 10 nuScenes classes).
-        tower("fcos2d_head.cls_tower", feats, &cls_t);
+        tower("fcos2d_head.cls_tower", E->layout.num_cls_convs, E->layout.fcos2d_norm, feats, &cls_t);
         {
             std::vector<std::string> names = {"fcos2d_head.cls_logits"};
             if (nusc) {
@@ -876,7 +965,7 @@ struct Builder {
             conv(Lc, 1, false, segs, true);
         }
         // [box2d_reg (4) | centerness (1)] on the box2d tower: relu(scale_l * (conv + b)) / conv + b (fcos2d.py:143-152)
-        tower("fcos2d_head.box2d_tower", feats, &box_t);
+        tower("fcos2d_head.box2d_tower", E->layout.num_box2d_convs, E->layout.fcos2d_norm, feats, &box_t);
         {
             const ConvLayer& Lb = E->conv_layer("fcos2d_head.box2d_reg+centerness",
                                                 {"fcos2d_head.box2d_reg", "fcos2d_head.centerness"}, 256, 3);
@@ -909,7 +998,7 @@ struct Builder {
         // [quat 4C | ctr 2C | depth C | size 3C | conf C] on the box3d tower with the per-level Scale/Offset folded
         // (fcos3d.py:166-180; PER_LEVEL_PREDICTORS False -> predictor index 0)
         if (!box3d_on) return;  // MODEL.BOX3D_ON = False (core.py:34-40): 2-D detector only
-        tower("fcos3d_head.box3d_tower", feats, &b3d_t);
+        tower("fcos3d_head.box3d_tower", E->layout.num_box3d_convs, E->layout.fcos3d_norm, feats, &b3d_t);
         // [quat 4C | ctr 2C | depth C | size 3C | conf C] on the box3d tower with the per-level Scale/Offset folded
         // (fcos3d.py:166-180).  PER_LEVEL_PREDICTORS False (shipped): predictor index 0 for every level, one launch over the
         // five levels; True: level l uses predictor l, one launch per level.
@@ -1335,7 +1424,7 @@ void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodePar
 
 int Engine::launches_per_forward() const {
     int n = 1 /*preprocess*/ + 6 /*decode: clear, 2 dense passes, 2 selects, final*/ + (plan.sparse_b3d ? 1 : 0) + ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) /*nms: sort, IoU bit matrix, scan, finish*/;
-    for (const Op& op : plan.ops) n += (op.type == Op::ESE) ? 3 : 1;
+    for (const Op& op : plan.ops) n += (op.type == Op::ESE) ? 3 : (op.type == Op::GN && op.gn.gamma != nullptr) ? 2 : 1;
     return n;
 }
 
@@ -1466,6 +1555,9 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
                                             op.out.ptr, op.out.pitch, stream, fp16),
                            "depthwise conv");
                 break;
+            case Op::GN:
+                cuda_check(launch_group_norm(op.gn, stream), "group norm");
+                break;
         }
         mark((op.type == Op::STEM || op.type == Op::FRONT || op.type == Op::DW) ? 1 : op.type == Op::CONV ? 2 : op.type == Op::POOL ? 3 : op.type == Op::ESE ? 4 : 5);
     }
@@ -1543,6 +1635,10 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
             case Op::RELU:
                 launches[5] += 1;
                 bytes[5] += in_px * op.in.C * 4;
+                break;
+            case Op::GN:  // statistics + apply (one launch without the affine)
+                launches[5] += op.gn.gamma != nullptr ? 2 : 1;
+                bytes[5] += op.bytes;
                 break;
             case Op::FRONT:
             case Op::DW:  // special-purpose conv kernels are counted with the stems, so category 2 stays wgmma-only

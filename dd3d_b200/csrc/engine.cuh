@@ -11,6 +11,7 @@
 #include "conv_igemm.cuh"
 #include "b3d_sparse.cuh"
 #include "detect.cuh"
+#include "group_norm.cuh"
 #include "resize.cuh"
 #include "small_kernels.cuh"
 
@@ -89,8 +90,9 @@ struct VovSpec {
 const VovSpec* vovnet_spec(int arch);  // nullptr: not a VoVNet arch
 
 struct Op {
-    enum Type { CONV, STEM, POOL, ESE, RELU, FRONT, DW } type;
+    enum Type { CONV, STEM, POOL, ESE, RELU, FRONT, DW, GN } type;
     ConvParams conv;
+    GroupNormParams gn;  // GN: GroupNorm (or, without gamma, the FPN avg fuse) in place on outs[0..nouts)
     View in, out, identity;
     View outs[kMaxSeg];  // bf16 output views (CONV: one per segment; others: outs[0] == out), for dd3d_get_tensor "op<i>"
     int nouts = 0;
@@ -176,7 +178,7 @@ class Engine {
                          cudaStream_t stream);
     void drop_plans();  // frees the active and the cached plans (an option that changes the op graph was flipped)
     int launches_per_forward() const;
-    // categories: 0 preprocess, 1 stem and depthwise conv, 2 conv (wgmma), 3 pool, 4 eSE, 5 relu, 6 decode, 7 nms
+    // categories: 0 preprocess, 1 stem and depthwise conv, 2 conv (wgmma), 3 pool, 4 eSE, 5 relu and GroupNorm, 6 decode, 7 nms
     void get_profile(double* ms, double* flops, double* bytes, int32_t* launches);
     int get_op_times(float* ms, int32_t* cats, double* flops, int max_ops);
 
@@ -193,8 +195,12 @@ class Engine {
     const EseLayer& ese_layer(const std::string& fc, int C);
     const FrontLayer& front_layer(const std::string& prefix);
     const DwLayer& dw_layer(const std::string& wname, int C);
+    const Epilogue& gn_affine(const std::string& prefix);  // GroupNorm weight / bias as d_scale / d_bias
+    void set_layout(const dd3d_layout_desc& l);
 
     dd3d_model_desc desc;
+    // FPN / head layout (dd3d_set_layout); the default is the shipped one
+    dd3d_layout_desc layout = {DD3D_NORM_BN_PER_LEVEL, DD3D_NORM_BN_PER_LEVEL, DD3D_NORM_BN_SHARED, 4, 4, 4, 0};
     int device = 0;
     int num_sms = 132;
     int fp16 = 0;  // desc.act_dtype == DD3D_ACT_FP16: 16-bit storage of activations / weights is fp16 instead of bf16

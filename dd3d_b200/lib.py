@@ -18,6 +18,11 @@ ARCH_IDS = {"dla34": ARCH_DLA34, "v2_99": ARCH_V2_99, "v2_19_slim_dw": 2, "v2_19
 IMG_U8, IMG_F32 = 0, 1
 ACT_BF16, ACT_FP16 = 0, 1
 POSE_GLOBAL, POSE_CAMERA = 0, 1
+NORM_BN_PER_LEVEL, NORM_BN_SHARED, NORM_GN, NORM_NONE = 0, 1, 2, 3  # dd3d_norm
+# NORM value -> dd3d_norm (get_norm's table: any other string raises KeyError like its dict lookup).  In a head tower BN /
+# FrozenBN are per level (ModuleListDial, fcos2d.py:73-80); the FPN's norms are one per conv, so every BN is "shared" there.
+HEAD_NORMS = {"BN": NORM_BN_PER_LEVEL, "FrozenBN": NORM_BN_PER_LEVEL, "SyncBN": NORM_BN_SHARED, "GN": NORM_GN, "": NORM_NONE}
+FPN_NORMS = {"BN": NORM_BN_SHARED, "FrozenBN": NORM_BN_SHARED, "SyncBN": NORM_BN_SHARED, "GN": NORM_GN, "": NORM_NONE}
 DET_WORDS = 24  # sizeof(dd3d_det) / 4
 
 
@@ -52,6 +57,19 @@ class ModelDesc(C.Structure):
     ]
 
 
+class LayoutDesc(C.Structure):
+    """dd3d_layout_desc: the FPN / head structure switches (dd3d_set_layout)."""
+    _fields_ = [
+        ("fcos2d_norm", C.c_int32),
+        ("fcos3d_norm", C.c_int32),
+        ("fpn_norm", C.c_int32),
+        ("num_cls_convs", C.c_int32),
+        ("num_box2d_convs", C.c_int32),
+        ("num_box3d_convs", C.c_int32),
+        ("fpn_fuse_avg", C.c_int32),
+    ]
+
+
 class TtaView(C.Structure):
     """dd3d_tta_view."""
     _fields_ = [("flip", C.c_int32), ("view_w", C.c_float), ("inv_sx", C.c_float * 2), ("inv_sy", C.c_float * 2),
@@ -65,6 +83,7 @@ SIGNATURES = {
     "dd3d_destroy": (None, [_P]),
     "dd3d_last_error": (C.c_char_p, [_P]),
     "dd3d_size_divisibility": (_I, [_P]),
+    "dd3d_set_layout": (_I, [_P, C.POINTER(LayoutDesc)]),
     "dd3d_load_weight": (_I, [_P, C.c_char_p, _P, C.POINTER(_I64), _I]),
     "dd3d_finalize": (_I, [_P]),
     "dd3d_workspace_bytes": (_I64, [_P, _I, _I, _I]),
@@ -97,6 +116,8 @@ SIGNATURES = {
     "dd3d_op_stem_s2_mma": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_conv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "dd3d_op_dwconv3x3": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _I, _P]),
+    "dd3d_op_group_norm_scratch_bytes": (_I64, [_I, _I, _I]),
+    "dd3d_op_group_norm": (_I, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _I, _P, _P]),
     "dd3d_op_preprocess": (_I, [_P, _I, _P, _P, _I, _I, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
     "dd3d_op_maxpool": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "dd3d_op_ese": (_I, [_P, _I, _P, _P, _P, _I, _P, _I, _P, _I, _I, _I, _P]),
@@ -177,6 +198,23 @@ def desc_from_cfg(cfg, out_cap=None):
     from .arch import is_nuscenes_arch
     d.nuscenes_heads = int(is_nuscenes_arch(cfg))
     d.act_dtype = act_dtype_of(cfg)
+    return d
+
+
+def layout_from_cfg(cfg):
+    """dd3d_layout_desc from the cfg keys the reference builds the FPN and the heads from (fcos2d.py:46-91,
+    fcos3d.py:75-112, detectron2 FPN norm / fuse_type).  Unknown NORM strings raise KeyError, like get_norm."""
+    f2, f3, fpn = cfg.DD3D.FCOS2D, cfg.DD3D.FCOS3D, cfg.FE.FPN
+    d = LayoutDesc()
+    d.fcos2d_norm = HEAD_NORMS[f2.NORM]
+    d.fcos3d_norm = HEAD_NORMS[f3.NORM]
+    d.fpn_norm = FPN_NORMS[fpn.NORM]
+    d.num_cls_convs = int(f2.NUM_CLS_CONVS)
+    d.num_box2d_convs = int(f2.NUM_BOX_CONVS)
+    d.num_box3d_convs = int(f3.NUM_CONVS)
+    if fpn.FUSE_TYPE not in ("sum", "avg"):  # FPN.__init__: assert fuse_type in {"avg", "sum"}
+        raise ValueError(f"FE.FPN.FUSE_TYPE must be 'sum' or 'avg', got {fpn.FUSE_TYPE!r}")
+    d.fpn_fuse_avg = int(fpn.FUSE_TYPE == "avg")
     return d
 
 

@@ -41,6 +41,9 @@ class DD3DB200(nn.Module):
         self._state = None  # reference-keyed fp32 CPU tensors
         self._device = torch.device("cpu")
         self._desc = _lib.desc_from_cfg(cfg)
+        self._layout = _lib.layout_from_cfg(cfg)
+        if cfg.DD3D.FCOS2D.USE_DEFORMABLE or (cfg.MODEL.BOX3D_ON and cfg.DD3D.FCOS3D.USE_DEFORMABLE):
+            raise ValueError("Not supported yet.")  # fcos2d.py:51-52, fcos3d.py:77-78
         self._handle = None
         self._plan_key = None
         self._host_bufs = None
@@ -120,6 +123,7 @@ class DD3DB200(nn.Module):
         handle = C.c_void_p()
         with torch.cuda.device(self._device):
             _lib.check(L.dd3d_create(C.byref(self._desc), C.byref(handle)))
+            _lib.check(L.dd3d_set_layout(handle, C.byref(self._layout)), handle)
             for name, t in self._state.items():
                 if not t.is_floating_point():
                     continue

@@ -74,11 +74,11 @@ def make_state_dict(cfg, seed=0, gains=None):
                 sd[name] = torch.randn(shape, generator=g)
             else:  # top_block p6/p7
                 sd[name] = 0.1 * torch.randn(shape, generator=g)
-        elif base == "bn_w":
+        elif base in ("bn_w", "gn_w"):
             sd[name] = 0.7 + 0.6 * torch.rand(shape, generator=g)
             if layer in gains and len(gains[layer]) > 2:  # per-level output equalisation (see calibrate_synthetic)
                 sd[name] = sd[name] * gains[layer][2]
-        elif base == "bn_b":
+        elif base in ("bn_b", "gn_b"):
             sd[name] = 0.1 * torch.randn(shape, generator=g)
             if layer in gains and len(gains[layer]) > 2:
                 sd[name] = sd[name] * gains[layer][2]

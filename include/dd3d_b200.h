@@ -91,6 +91,25 @@ typedef struct dd3d_model_desc {
     int32_t box3d_on;             /* MODEL.BOX3D_ON: 0 = 2-D detector only (core.py:34-40; NMS keyed on `scores`, :117-125) */
 } dd3d_model_desc;
 
+/* Normalisation after a head-tower or FPN conv (get_norm in fcos2d.py:73-91, fcos3d.py:82-100, detectron2 FPN):
+ * "BN" / "FrozenBN" in a head tower give one BN per FPN level (ModuleListDial, keys <conv>.norm.<level>); "SyncBN" gives one
+ * BN shared by the levels (<conv>.norm); "GN" GroupNorm(32, 256) (<conv>.norm.weight / .bias); "" no norm, the conv has a
+ * bias.  The FPN has no per-level case: its BN / FrozenBN / SyncBN is DD3D_NORM_BN_SHARED (DD3D_NORM_BN_PER_LEVEL is
+ * accepted as the same). */
+enum dd3d_norm { DD3D_NORM_BN_PER_LEVEL = 0, DD3D_NORM_BN_SHARED = 1, DD3D_NORM_GN = 2, DD3D_NORM_NONE = 3 };
+
+/* Structural switches of the FPN and the FCOS heads (defaults = the shipped layout, in brackets).  A separate struct so
+ * that dd3d_model_desc keeps its size: an engine that never receives one builds the default layout. */
+typedef struct dd3d_layout_desc {
+    int32_t fcos2d_norm;      /* dd3d_norm of the cls / box2d towers: DD3D.FCOS2D.NORM [BN per level] */
+    int32_t fcos3d_norm;      /* dd3d_norm of the box3d tower: DD3D.FCOS3D.NORM [BN per level] */
+    int32_t fpn_norm;         /* dd3d_norm of the FPN lateral / output convs: FE.FPN.NORM [BN shared] */
+    int32_t num_cls_convs;    /* DD3D.FCOS2D.NUM_CLS_CONVS, 0..16 [4]; 0: the predictors read the FPN outputs */
+    int32_t num_box2d_convs;  /* DD3D.FCOS2D.NUM_BOX_CONVS, 0..16 [4] */
+    int32_t num_box3d_convs;  /* DD3D.FCOS3D.NUM_CONVS, 0..16 [4] */
+    int32_t fpn_fuse_avg;     /* FE.FPN.FUSE_TYPE == "avg": (lateral + top-down) / 2 [0 = "sum"] */
+} dd3d_layout_desc;
+
 /* One detection = the fields the reference returns in Instances (fcos2d.py:331-335,263; fcos3d.py:398-399). */
 typedef struct dd3d_det {
     float box[4];      /* pred_boxes (x1, y1, x2, y2) */
@@ -126,6 +145,9 @@ int dd3d_create(const dd3d_model_desc* h_desc, dd3d_handle* out);
 void dd3d_destroy(dd3d_handle h);
 const char* dd3d_last_error(dd3d_handle h); /* h may be NULL: error of the last failed dd3d_create */
 int dd3d_size_divisibility(dd3d_handle h);  /* backbone.size_divisibility: 128 (DLA p67) / 64 (V2-99 p6) */
+/* Sets the FPN / head layout (dd3d_layout_desc) before dd3d_finalize (DD3D_ERR_STATE afterwards).  An unknown dd3d_norm value,
+ * a depth outside 0..16 or fpn_fuse_avg other than 0 / 1 returns DD3D_ERR_INVALID and leaves the layout unchanged. */
+int dd3d_set_layout(dd3d_handle h, const dd3d_layout_desc* h_layout);
 
 /* ---- weights: one call per tensor of the reference state_dict (Checkpointer.load, scripts/train.py:52) ----- */
 /* h_data: host fp32, contiguous, `ndim` dims in h_shape.  Unknown names are ignored (return DD3D_OK, e.g.
@@ -197,7 +219,8 @@ int dd3d_launches_per_forward(dd3d_handle h);
 /* Per-category device time of the LAST dd3d_forward issued with option "profile" = 1 (CUDA events recorded on the
  * launch stream around every op), with the algorithmic FLOPs / HBM bytes and launch counts of one forward.
  * Categories (arrays of 8): 0 preprocess, 1 special-purpose conv kernels (stem convs, the fused DLA-34 front end and the
- * depthwise 3x3 convs of the VoVNet -dw variants), 2 wgmma implicit-GEMM conv, 3 max-pool, 4 eSE, 5 relu, 6 decode, 7 NMS. */
+ * depthwise 3x3 convs of the VoVNet -dw variants), 2 wgmma implicit-GEMM conv, 3 max-pool, 4 eSE, 5 relu and GroupNorm (the
+ * elementwise passes over a map), 6 decode, 7 NMS. */
 int dd3d_get_profile(dd3d_handle h, double* h_ms, double* h_flops, double* h_bytes, int32_t* h_launches);
 /* Same events, per op in launch order (entry 0 = preprocess, then every engine op, then decode, NMS): device ms,
  * category and algorithmic FLOPs.  Returns the number of entries written (<= max_ops). */
@@ -291,6 +314,17 @@ int dd3d_op_stem_s2_mma(const void* d_in4, const void* d_w, const float* d_sb, v
  * pointers 16-byte aligned.  fp32 accumulation in tap order, one rounding to the 16-bit type at the store. */
 int dd3d_op_dwconv3x3(const void* d_in, int B, int H, int W, int C, int in_pitch, const void* d_w, int stride, void* d_out,
                       int out_pitch, dd3d_stream stream);
+/* dd3d_op_group_norm: GroupNorm(32, 256) on the kernels the engine runs for NORM "GN" (csrc/group_norm.cu): statistics over
+ * each image's whole H x W map (biased variance, eps 1e-5, fp32 chunk statistics combined in a fixed order), then
+ * y = x * gamma_c * rstd_g + (beta_c - mean_g * gamma_c * rstd_g), then + nearest-2x(d_residual) when d_residual is not NULL
+ * (the coarser map [B][(H+1)/2 or H/2][(W+1)/2 or W/2][res_pitch]), then * 0.5 when avg, then ReLU when relu; one rounding to
+ * the 16-bit type at the store.  d_in / d_out = [B][H][W][pitch] with 256 channels, d_out may equal d_in.  d_gamma == NULL
+ * (d_beta too): add / scale only, no statistics.  d_scratch: dd3d_op_group_norm_scratch_bytes(B, H, W) bytes, any content.
+ * Pitches multiples of 8 and >= 256, every pointer 16-byte aligned. */
+int64_t dd3d_op_group_norm_scratch_bytes(int B, int H, int W);
+int dd3d_op_group_norm(const void* d_in, int B, int H, int W, int in_pitch, const float* d_gamma, const float* d_beta, int relu,
+                       const void* d_residual, int res_pitch, int avg, void* d_out, int out_pitch, void* d_scratch,
+                       dd3d_stream stream);
 int dd3d_op_preprocess(const void* d_images, int img_dtype, const int32_t* d_sizes2, void* d_out4, int B, int Hs, int Ws,
                        int Hp, int Wp, const float* h_mean, const float* h_std, dd3d_stream stream);
 int dd3d_op_maxpool(const void* d_in, void* d_out, int B, int H, int W, int C, int in_pitch, int out_pitch, int ksize,
