@@ -226,6 +226,10 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value) {
             const int v = value < 0 ? 0 : (value > 2 ? 2 : value);
             if (e.opt_sparse_box3d != v) e.drop_plans();
             e.opt_sparse_box3d = v;
+        } else if (n == "sparse_tower") {  // 2 (default): auto by head size; 1: with every sparse predictor; 0: dense tower
+            const int v = value < 0 ? 0 : (value > 2 ? 2 : value);
+            if (e.opt_sparse_tower != v) e.drop_plans();
+            e.opt_sparse_tower = v;
         } else if (n == "dla_front") {  // 1 (default): fused DLA-34 front end (dla_front.cu); 0: layer by layer
             if (e.opt_dla_front != (value ? 1 : 0)) e.drop_plans();
             e.opt_dla_front = value ? 1 : 0;

@@ -444,9 +444,10 @@ cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
     const int stage_bytes = (p.halo ? 0 : kABytes) + p.block_n * 128;
     const int smem_bytes = (p.wstat ? p.taps * p.kchunks : p.num_stages) * stage_bytes + conv_fixed_smem(p);
     ConvKernel kernel = nullptr;
+    if (p.tile_list != nullptr && (!p.pair || p.tile_count == nullptr)) return cudaErrorInvalidValue;  // list mode: pair tile only
     if (p.pair) {
         if (!p.halo || p.block_n != 128 || p.out_mode != 0) return cudaErrorInvalidValue;
-        kernel = conv_kernel_pair(p.fp16 != 0);
+        kernel = conv_kernel_pair(p.fp16 != 0, p.tile_list != nullptr);
     }
     for (auto group : {conv_kernel_n16_64, conv_kernel_n80_128, conv_kernel_n144_192, conv_kernel_n208_256}) {
         if (kernel == nullptr) kernel = group(p.halo != 0, p.fp16 != 0, p.block_n);
@@ -467,8 +468,11 @@ cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
             }
         }
         for (bool fp16 : {false, true}) {
-            if (e == cudaSuccess)
-                e = cudaFuncSetAttribute(conv_kernel_pair(fp16), cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
+            for (bool list : {false, true}) {
+                if (e == cudaSuccess)
+                    e = cudaFuncSetAttribute(conv_kernel_pair(fp16, list), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             kSmemBudget);
+            }
         }
         for (auto fn : {conv_taps_kernel<false>, conv_taps_kernel<true>}) {
             if (e == cudaSuccess) e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kTapsSmem);

@@ -59,7 +59,13 @@ struct ConvParams {
     int wstat;        // 1: weight-stationary halo variant -- all taps * kchunks weight blocks resident in shared memory
     int a_stages;     // halo variants: A patches in flight (3, or up to 5 with wstat; 2 pairs of patches with pair)
     int pair;         // 1: pair-tile halo variant -- work item = two 16x8 tiles x one 128-channel n-block (conv_select_pair)
+    // Work-list mode (nullptr: every tile of every segment).  The M units are the entries of tile_list (pair tile: entries
+    // 2i, 2i + 1 form unit i and must lie in one segment), each (seg << 29) | (img << 16) | (row-major tile of the image);
+    // *tile_count entries, read on the device after griddepcontrol.wait.  total_work then only sizes the grid.
+    const uint32_t* tile_list;
+    const int32_t* tile_count;
 };
+constexpr int kTileListMaxImages = 1 << 13, kTileListMaxTiles = 1 << 16;  // field widths of a tile_list entry
 static_assert(sizeof(ConvParams) <= 4096, "kernel parameter space");
 
 // Host helpers (conv_igemm.cu)

@@ -35,7 +35,11 @@
 // count leaves the last pair's second sub-tile outside the image: its rows are never stored and read no residual.  The K
 // order per output element is unchanged, so results are bit-identical to the 128 x 256 tile.
 //
-// The kernel is templated on (halo variant, fp16 storage, wgmma N = block_n, pair tile); conv_igemm_n*.cu instantiate it, one
+// Work-list mode (LIST, pair tile only): the M units come from ConvParams::tile_list, whose length the kernel reads from the
+// device after griddepcontrol.wait, so a launch can cover a tile set an earlier kernel chose (the sparse box3d tower, engine.cu)
+// without a host round trip; the grid stays persistent.  Everything else, K order included, is the dense pair tile's.
+//
+// The kernel is templated on (halo variant, fp16 storage, wgmma N = block_n, pair tile, work list); conv_igemm_n*.cu instantiate it, one
 // group of N values per translation unit so that the build compiles them in parallel; conv_igemm.cu holds the host side and
 // the taps-in-N kernel.
 #pragma once
@@ -81,7 +85,8 @@ __device__ __forceinline__ int fast_div(int x, int d, float inv_d) {
 }
 
 // work item = (M-tile, n-block), n-block fastest.  PAIR: the M unit is a pair of tiles, `sub` selects tile 2i + sub.
-template <bool PAIR = false>
+// Called by whole warps (the list entry is broadcast from lane 0, so the coordinates stay provably warp-uniform).
+template <bool PAIR = false, bool LIST = false>
 __device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int work, int sub = 0) {
     TileCoord t;
     int mt = work;
@@ -90,19 +95,28 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int work, 
         mt = fast_div(work, p.n_blocks, p.inv_n_blocks);
         t.n_blk = work - mt * p.n_blocks;
     }
-    int s = 0;
+    int r;
+    if (LIST) {
+        const uint32_t e = __shfl_sync(0xffffffffu, __ldg(p.tile_list + (PAIR ? 2 * mt + sub : mt)), 0);
+        t.seg = static_cast<int>(e >> 29);
+        t.img = static_cast<int>((e >> 16) & (kTileListMaxImages - 1));
+        r = static_cast<int>(e & (kTileListMaxTiles - 1));
+    } else {
+        int s = 0;
 #pragma unroll
-    for (int i = 1; i < kMaxSeg; ++i) {
-        if (i < p.nseg && mt >= p.seg[i].tile_begin) s = i;
+        for (int i = 1; i < kMaxSeg; ++i) {
+            if (i < p.nseg && mt >= p.seg[i].tile_begin) s = i;
+        }
+        t.seg = s;
+        const ConvSeg& g = p.seg[s];
+        int local = mt - g.tile_begin;
+        int per_img = g.tiles_x * g.tiles_y;
+        if (PAIR) per_img = (per_img + 1) >> 1;
+        t.img = fast_div(local, per_img, g.inv_per_img);
+        r = local - t.img * per_img;
+        if (PAIR) r = 2 * r + sub;
     }
-    t.seg = s;
-    const ConvSeg& g = p.seg[s];
-    int local = mt - g.tile_begin;
-    int per_img = g.tiles_x * g.tiles_y;
-    if (PAIR) per_img = (per_img + 1) >> 1;
-    t.img = fast_div(local, per_img, g.inv_per_img);
-    int r = local - t.img * per_img;
-    if (PAIR) r = 2 * r + sub;
+    const ConvSeg& g = p.seg[t.seg];
     int ty = fast_div(r, g.tiles_x, g.inv_tiles_x);
     int tx = r - ty * g.tiles_x;
     t.y0 = ty * g.th;
@@ -170,9 +184,10 @@ __device__ __forceinline__ void mma_kblock2(float (&acc0)[L], float (&acc1)[L], 
 
 // BN = block_n, the wgmma N: a compile-time parameter, so the accumulators are exactly BN / 2 registers per consumer thread
 // and 64-row half (PAIR: two halves per warpgroup)
-template <bool HALO, bool F16, int BN, bool PAIR = false>
+template <bool HALO, bool F16, int BN, bool PAIR = false, bool LIST = false>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __grid_constant__ ConvParams p) {
     static_assert(!PAIR || (HALO && BN == 128), "the pair tile is a halo variant with block_n 128");
+    static_assert(!LIST || PAIR, "work-list mode is instantiated for the pair tile only");
     constexpr int MH = PAIR ? 2 : 1;                                   // 64-row halves per consumer warpgroup
     constexpr int kASlot = PAIR ? 2 * kHaloABytes : kHaloABytes;       // one A stage: the patch of every sub-tile
     extern __shared__ uint8_t smem_raw[];
@@ -226,7 +241,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
     const int kblocks = p.taps * p.kchunks;
-    const int w_first = static_cast<int>(blockIdx.x), w_step = static_cast<int>(gridDim.x), w_total = p.total_work;
+    const int w_first = static_cast<int>(blockIdx.x), w_step = static_cast<int>(gridDim.x);
+    int w_total = p.total_work;
+    if (LIST) {  // work-list mode: the list was written by an earlier kernel of the stream
+        const int units = PAIR ? (__ldg(p.tile_count) >> 1) : __ldg(p.tile_count);
+        w_total = __shfl_sync(0xffffffffu, units, 0) * p.n_blocks;
+    }
 
     if (warp == 0) {
         // ---------------------------------------------------------------- warp 0: activation (A) producer in the
@@ -243,7 +263,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             __syncwarp();
         }
         for (int work = w_first; work < w_total && !wstat; work += w_step) {
-            const TileCoord t = decode_tile<PAIR>(p, work);
+            const TileCoord t = decode_tile<PAIR, LIST>(p, work);
             const ConvSeg& g = p.seg[t.seg];
             if (HALO) {
                 for (int kc = 0; kc < p.kchunks; ++kc) {
@@ -320,8 +340,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             int as = 0;
             uint32_t aphase = 0;
             for (int work = w_first; work < w_total; work += w_step) {
-                const TileCoord t = decode_tile<PAIR>(p, work);
-                const TileCoord t1 = PAIR ? decode_tile<PAIR>(p, work, 1) : t;
+                const TileCoord t = decode_tile<PAIR, LIST>(p, work);
+                const TileCoord t1 = PAIR ? decode_tile<PAIR, LIST>(p, work, 1) : t;
                 const ConvSeg& g = p.seg[t.seg];
                 for (int kc = 0; kc < p.kchunks; ++kc) {
                     ptx::mbar_wait(&aempty_bar[as], aphase ^ 1);
@@ -373,7 +393,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
         int sb_key = -1;  // (segment, n-block) whose folded-BN vectors are staged in s_scale / s_bias
         if (wstat) ptx::mbar_wait(wfull_bar, 0);
         for (int work = w_first; work < w_total; work += w_step) {
-            const TileCoord t = decode_tile<PAIR>(p, work, PAIR ? wgi : 0);
+            const TileCoord t = decode_tile<PAIR, LIST>(p, work, PAIR ? wgi : 0);
             const ConvSeg& g = p.seg[t.seg];
             // ---- main loop: one commit group per k-block; the slot (and halo patch) of group i is released after
             // group i + 1 has been issued and group i has retired (wait_group 1)
@@ -593,7 +613,7 @@ using ConvKernel = void (*)(ConvParams);
     }
 ConvKernel conv_kernel_n16_64(bool halo, bool fp16, int block_n);
 ConvKernel conv_kernel_n80_128(bool halo, bool fp16, int block_n);
-ConvKernel conv_kernel_pair(bool fp16);  // the pair-tile halo kernel (block_n 128), in conv_igemm_n80_128.cu
+ConvKernel conv_kernel_pair(bool fp16, bool list);  // the pair-tile halo kernel (block_n 128), in conv_igemm_n80_128.cu
 ConvKernel conv_kernel_n144_192(bool halo, bool fp16, int block_n);
 ConvKernel conv_kernel_n208_256(bool halo, bool fp16, int block_n);
 

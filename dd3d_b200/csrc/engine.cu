@@ -53,6 +53,7 @@ Engine::Engine(const dd3d_model_desc& d) : desc(d) {
     num_sms = prop.multiProcessorCount;
     if (const char* e = getenv("DD3D_DLA_FRONT")) opt_dla_front = atoi(e) ? 1 : 0;  // A/B runs of bench.py; default 1
     if (const char* e = getenv("DD3D_SPARSE_BOX3D")) opt_sparse_box3d = std::max(0, std::min(2, atoi(e)));
+    if (const char* e = getenv("DD3D_SPARSE_TOWER")) opt_sparse_tower = std::max(0, std::min(2, atoi(e)));
     if (const char* e = getenv("DD3D_STEM_MMA")) opt_stem_mma = atoi(e) ? 1 : 0;
     if (const char* e = getenv("DD3D_ESE_POOL")) opt_ese_pool = atoi(e) ? 1 : 0;
 }
@@ -894,6 +895,63 @@ struct Builder {
         *out = cur;
     }
 
+    // Tile lists of the sparse box3d tower (TowerTilesParams): the tiling conv() gives the tower layers, and the staging, list
+    // and count areas in the persistent region.  false: the shapes exceed the list entry fields, the tower stays dense.
+    bool tower_tile_lists(const std::vector<View>& feats, int depth) {
+        TowerTilesParams& tt = P->tower_tiles;
+        memset(&tt, 0, sizeof(tt));
+        const int L = static_cast<int>(feats.size());
+        int hs[kMaxSeg], ws[kMaxSeg];
+        for (int l = 0; l < L; ++l) {
+            hs[l] = feats[l].H;
+            ws[l] = feats[l].W;
+        }
+        const bool halo = conv_prefer_halo(9, 1, 256, L, hs, ws);
+        for (int l = 0; l < L; ++l) {
+            TowerTilesLevel& v = tt.lvl[l];
+            v.H = hs[l];
+            v.W = ws[l];
+            if (halo) {
+                v.th = kHaloTh;
+                v.tw = kHaloTw;
+            } else {
+                choose_tile(v.H, v.W, &v.th, &v.tw);
+            }
+            v.tiles_x = (v.W + v.tw - 1) / v.tw;
+            v.tiles_y = (v.H + v.th - 1) / v.th;
+            const int T = v.tiles_x * v.tiles_y;
+            v.stage_begin = tt.cap;
+            tt.cap += B * (T + (T & 1));
+            tt.max_tiles = std::max(tt.max_tiles, T);
+        }
+        if (B > kTileListMaxImages || tt.max_tiles >= kTileListMaxTiles || tower_tiles_smem_bytes(tt.max_tiles) > 48 * 1024)
+            return false;
+        // the work-list mode is built for the pair tile, which every filled 256-channel halo layer selects (conv() below)
+        ConvParams cp;
+        memset(&cp, 0, sizeof(cp));
+        cp.nseg = L;
+        cp.B = B;
+        cp.halo = halo ? conv_halo_mode() : 0;
+        for (int l = 0; l < L; ++l) {
+            cp.seg[l].H = hs[l];
+            cp.seg[l].W = ws[l];
+            cp.seg[l].th = tt.lvl[l].th;
+            cp.seg[l].tw = tt.lvl[l].tw;
+        }
+        if (!conv_select_pair(&cp, 256, E->num_sms)) return false;
+        tt.B = B;
+        tt.depth = depth;
+        const size_t list_bytes = static_cast<size_t>(depth) * tt.cap * 4, bl_bytes = static_cast<size_t>(depth) * L * B * 4;
+        tt.stage = static_cast<uint32_t*>(alloc_bytes(list_bytes));
+        tt.list = static_cast<uint32_t*>(alloc_bytes(list_bytes));
+        tt.bl_count = static_cast<int32_t*>(alloc_bytes(bl_bytes));
+        tt.bl_pixels = static_cast<int32_t*>(alloc_bytes(bl_bytes));
+        tt.count = static_cast<int32_t*>(alloc_bytes(static_cast<size_t>(depth) * 4));
+        tt.pixels = static_cast<long long*>(alloc_bytes(static_cast<size_t>(depth) * 8));
+        tt.ticket = static_cast<uint32_t*>(alloc_bytes(4));
+        return true;
+    }
+
     void build_heads(const std::vector<View>& feats) {
         const int C = E->desc.num_classes;
         const int L = static_cast<int>(feats.size());
@@ -998,7 +1056,29 @@ struct Builder {
         // [quat 4C | ctr 2C | depth C | size 3C | conf C] on the box3d tower with the per-level Scale/Offset folded
         // (fcos3d.py:166-180; PER_LEVEL_PREDICTORS False -> predictor index 0)
         if (!box3d_on) return;  // MODEL.BOX3D_ON = False (core.py:34-40): 2-D detector only
-        tower("fcos3d_head.box3d_tower", E->layout.num_box3d_convs, E->layout.fcos3d_norm, feats, &b3d_t);
+        // sparse box3d tower: the sparse predictor reads the tower output only around the final candidates, so the tower runs
+        // after the threshold / top-k half of the decode on the tiles tower_tiles_kernel lists (GN needs whole-map statistics).
+        // It is the last part of the op list, so its buffers keep the lifetimes of the dense order: the decode between the
+        // two parts touches only the persistent region.
+        const int d3 = E->layout.num_box3d_convs;
+        const bool sparse_tower = sparse3 && d3 > 0 && E->layout.fcos3d_norm != DD3D_NORM_GN &&
+                                  (E->opt_sparse_tower == 1 || (E->opt_sparse_tower == 2 && head_px >= 50000)) &&
+                                  tower_tile_lists(feats, d3);
+        P->tower_begin = sparse_tower ? static_cast<int>(P->ops.size()) : -1;
+        tower("fcos3d_head.box3d_tower", d3, E->layout.fcos3d_norm, feats, &b3d_t);
+        if (sparse_tower && !dry) {
+            const TowerTilesParams& tt = P->tower_tiles;
+            for (int j = 0; j < d3; ++j) {
+                Op& op = P->ops[P->tower_begin + j];
+                ConvParams& c = op.conv;
+                if (op.type != Op::CONV || c.nseg != L || !c.pair) fail(DD3D_ERR_STATE, "internal: sparse box3d tower layout");
+                for (int l = 0; l < L; ++l)
+                    if (c.seg[l].th != tt.lvl[l].th || c.seg[l].tw != tt.lvl[l].tw)
+                        fail(DD3D_ERR_STATE, "internal: sparse box3d tower tiling");
+                c.tile_list = tt.list + static_cast<size_t>(j) * tt.cap;
+                c.tile_count = tt.count + j;
+            }
+        }
         // [quat 4C | ctr 2C | depth C | size 3C | conf C] on the box3d tower with the per-level Scale/Offset folded
         // (fcos3d.py:166-180).  PER_LEVEL_PREDICTORS False (shipped): predictor index 0 for every level, one launch over the
         // five levels; True: level l uses predictor l, one launch per level.
@@ -1380,6 +1460,16 @@ void Engine::make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes) {
         plan.b3d_sparse.fin = dp.fin;
         plan.b3d_sparse.cand_count = dp.cand_count;
     }
+    if (plan.tower_begin >= 0) {
+        TowerTilesParams& tt = plan.tower_tiles;
+        tt.fin = dp.fin;
+        tt.cand_count = dp.cand_count;
+        tt.C = desc.num_classes;
+        tt.topk = desc.pre_nms_topk;
+        // the kernel's completion ticket starts at zero; each launch leaves it at zero
+        cuda_check(cudaMemset(tt.ticket, 0, 4), "cudaMemset(tower tile ticket)");
+        cuda_check(cudaDeviceSynchronize(), "cudaDeviceSynchronize");
+    }
     fill_nms_params(&plan.nms, desc, dp, B);
     plan.nms.scratch = plan.nms_scratch;
 }
@@ -1423,7 +1513,8 @@ void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodePar
 }
 
 int Engine::launches_per_forward() const {
-    int n = 1 /*preprocess*/ + 6 /*decode: clear, 2 dense passes, 2 selects, final*/ + (plan.sparse_b3d ? 1 : 0) + ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) /*nms: sort, IoU bit matrix, scan, finish*/;
+    int n = 1 /*preprocess*/ + 6 /*decode: clear, 2 dense passes, 2 selects, final*/ + (plan.sparse_b3d ? 1 : 0) +
+            (plan.tower_begin >= 0 ? 1 : 0) /*tower tile lists*/ + ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) /*nms: sort, IoU bit matrix, scan, finish*/;
     for (const Op& op : plan.ops) n += (op.type == Op::ESE) ? 3 : (op.type == Op::GN && op.gn.gamma != nullptr) ? 2 : 1;
     return n;
 }
@@ -1482,17 +1573,20 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
     const bool raw = raw_pending;
     raw_pending = false;
     size_t ev_i = 0;
-    auto mark = [&](int cat) {  // opt_profile: CUDA events on the launch stream around every op
+    auto mark = [&](int cat, int op = -1) {  // opt_profile: CUDA events on the launch stream around every op
         if (!opt_profile) return;
         if (ev_i >= prof_ev.size()) {
             cudaEvent_t e;
             cuda_check(cudaEventCreate(&e), "cudaEventCreate");
             prof_ev.push_back(e);
             prof_cat.push_back(cat);
+            prof_op.push_back(op);
         }
         prof_cat[ev_i] = cat;
+        prof_op[ev_i] = op;
         cuda_check(cudaEventRecord(prof_ev[ev_i++], stream), "cudaEventRecord");
     };
+    plan.ran = true;
     mark(-1);
     // sizes (h, w, out_h, out_w) -> the (h, w) pairs the preprocess kernel reads are its first two columns
     if (raw) {
@@ -1508,7 +1602,15 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
     mark(0);
     // from here on every launch follows one of our kernels: the small kernels may use programmatic dependent launch (pdl.cuh)
     PdlScope pdl_scope;
+    DecodeParams dp = P.decode;
+    dp.K = d_K;
     for (const Op& op : P.ops) {
+        const int oi = static_cast<int>(&op - P.ops.data());
+        if (oi == P.tower_begin) {  // sparse box3d tower: the final candidates first, then the tiles they need
+            cuda_check(launch_decode_select(dp, stream), "decode (threshold + top-k)");
+            cuda_check(launch_tower_tiles(P.tower_tiles, stream), "box3d tower tile lists");
+            mark(6);
+        }
         switch (op.type) {
             case Op::CONV:
                 cuda_check(launch_conv(op.conv, num_sms, stream), "conv");
@@ -1559,12 +1661,11 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
                 cuda_check(launch_group_norm(op.gn, stream), "group norm");
                 break;
         }
-        mark((op.type == Op::STEM || op.type == Op::FRONT || op.type == Op::DW) ? 1 : op.type == Op::CONV ? 2 : op.type == Op::POOL ? 3 : op.type == Op::ESE ? 4 : 5);
+        mark((op.type == Op::STEM || op.type == Op::FRONT || op.type == Op::DW) ? 1 : op.type == Op::CONV ? 2 : op.type == Op::POOL ? 3 : op.type == Op::ESE ? 4 : 5,
+             oi);
     }
-    DecodeParams dp = P.decode;
-    dp.K = d_K;
     if (P.sparse_b3d) {
-        cuda_check(launch_decode_select(dp, stream), "decode (threshold + top-k)");
+        if (P.tower_begin < 0) cuda_check(launch_decode_select(dp, stream), "decode (threshold + top-k)");
         cuda_check(launch_b3d_sparse(P.b3d_sparse, stream), "sparse box3d predictor");
         cuda_check(launch_decode_final(dp, stream), "decode (boxes)");
     } else {
@@ -1582,16 +1683,39 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
     if (opt_profile) prof_used = ev_i;
 }
 
-// per-op device time of the last profiled forward: entry 0 = preprocess, then plan.ops in order, then decode, nms
+// Algorithmic FLOPs per plan op.  The sparse box3d tower convs count the in-map pixels of the tiles the last forward ran,
+// read back from the device (call after that forward has completed).
+std::vector<double> Engine::op_flops() {
+    std::vector<double> f(plan.ops.size());
+    for (size_t i = 0; i < f.size(); ++i) f[i] = plan.ops[i].flops;
+    if (plan.tower_begin >= 0) {
+        const int d = plan.tower_tiles.depth;
+        std::vector<long long> px(d, 0);
+        if (plan.ran && prof_used >= 2)  // the callers have synchronised the last profiled forward
+            cuda_check(cudaMemcpy(px.data(), plan.tower_tiles.pixels, d * sizeof(long long), cudaMemcpyDeviceToHost),
+                       "D2H tower tile pixels");
+        for (int j = 0; j < d; ++j) {
+            const ConvParams& c = plan.ops[plan.tower_begin + j].conv;
+            double dense_px = 0.0;
+            for (int s = 0; s < c.nseg; ++s) dense_px += static_cast<double>(c.B) * c.seg[s].H * c.seg[s].W;
+            f[plan.tower_begin + j] *= static_cast<double>(px[j]) / dense_px;
+        }
+    }
+    return f;
+}
+
+// per-op device time of the last profiled forward: entry 0 = preprocess, then plan.ops in order (with the sparse box3d
+// tower, the threshold / top-k and the tile lists before the tower convs), then decode, nms
 int Engine::get_op_times(float* ms, int32_t* cats, double* flops, int max_ops) {
     if (!plan.valid) fail(DD3D_ERR_STATE, "no plan");
     if (prof_used < 2) return 0;
     cuda_check(cudaEventSynchronize(prof_ev[prof_used - 1]), "cudaEventSynchronize");
+    const std::vector<double> f = op_flops();
     int n = 0;
     for (size_t i = 1; i < prof_used && n < max_ops; ++i, ++n) {
         cuda_check(cudaEventElapsedTime(&ms[n], prof_ev[i - 1], prof_ev[i]), "cudaEventElapsedTime");
         cats[n] = prof_cat[i];
-        flops[n] = (i >= 2 && i - 2 < plan.ops.size()) ? plan.ops[i - 2].flops : 0.0;
+        flops[n] = (prof_op[i] >= 0 && prof_op[i] < static_cast<int>(f.size())) ? f[prof_op[i]] : 0.0;
     }
     return n;
 }
@@ -1609,6 +1733,7 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
     }
     const Plan& P = plan;
     const double C = desc.num_classes;
+    const std::vector<double> f = op_flops();
     launches[0] = 1;
     bytes[0] = static_cast<double>(P.B) * 3 * P.Hs * P.Ws + static_cast<double>(P.B) * P.Hp * P.Wp * 8;
     for (const Op& op : P.ops) {
@@ -1621,7 +1746,7 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
                 break;
             case Op::CONV:
                 launches[2] += 1;
-                flops[2] += op.flops;
+                flops[2] += f[&op - P.ops.data()];
                 break;
             case Op::POOL:
                 launches[3] += 1;
@@ -1648,7 +1773,7 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
                 break;
         }
     }
-    launches[6] = 6 + (P.sparse_b3d ? 1 : 0);
+    launches[6] = 6 + (P.sparse_b3d ? 1 : 0) + (P.tower_begin >= 0 ? 1 : 0);
     launches[7] = (desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1;
     for (int l = 0; l < kLevels; ++l)  // two dense passes over the fp32 logits + centerness
         bytes[6] += 2.0 * P.B * P.lvl_h[l] * P.lvl_w[l] * (C + 1) * 4;

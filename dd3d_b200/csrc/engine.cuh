@@ -144,6 +144,12 @@ struct Plan {
     bool sparse_b3d = false;
     float* b3d_rows = nullptr;  // [B][L][topk][b3d_pitch]
     B3dSparseParams b3d_sparse;
+    // sparse box3d tower: ops [tower_begin, ops.size()) are the box3d tower convs.  They run after the threshold / top-k half
+    // of the decode, in work-list mode on the tiles tower_tiles_kernel lists; every other pixel of their outputs keeps stale
+    // workspace contents and is read by nothing.  -1: dense tower.
+    int tower_begin = -1;
+    TowerTilesParams tower_tiles;
+    bool ran = false;  // a forward has run on this plan (the tile counts on the device are valid)
 };
 
 void fill_decode_params(DecodeParams* dp, const dd3d_model_desc& desc, int B, int cls_pitch, int b3d_pitch,
@@ -212,10 +218,13 @@ class Engine {
                            // separate pool kernel (the fused pass re-reads each pooling window's inputs 2.25 times)
     int opt_stem_mma = 1;  // 1: VoVNet stem_1 on the register-fragment kernel (stem_mma.cu); 0: wgmma im2col kernel (stem_tc.cu)
     int opt_sparse_box3d = 2;  // box3d predictor at the final candidates only (b3d_sparse.cu): 0 never (dense maps), 1 always, 2 auto (by head size)
+    int opt_sparse_tower = 2;  // box3d tower on the tiles the sparse predictor reads (tower_tiles.cu): 0 never, 1 whenever the
+                               // sparse predictor runs and the tower norm is not GN, 2 auto (as 1, for heads of >= 50 000 pixels)
     int opt_dla_front = 1;  // 1: DLA-34 base_layer + level0 + level1 (+ pool) as ONE kernel (dla_front.cu); 0: layer by layer
     int opt_workspace_fill = -1;  // >= 0: byte the whole arena is filled with at dd3d_plan (poison test)
     std::vector<cudaEvent_t> prof_ev;
     std::vector<int> prof_cat;
+    std::vector<int> prof_op;  // plan op that ends at event i, or -1
     size_t prof_used = 0;
     std::string err;
     std::map<std::string, HostTensor> weights;
@@ -252,6 +261,7 @@ class Engine {
     size_t build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry);
     void release_plan();
     static void free_plan(Plan* P);
+    std::vector<double> op_flops();
 };
 
 }  // namespace dd3d

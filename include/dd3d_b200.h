@@ -193,7 +193,10 @@ int dd3d_overflow_flags(dd3d_handle h, dd3d_stream stream, int32_t* h_flags);
  * two kernels, kept as a tested alternative; changing it drops the plans), "stem_mma" (default 1: VoVNet stem_1 runs on csrc/stem_mma.cu, 0: on csrc/stem_tc.cu), "sparse_box3d" (2 = auto, the default: the fused FCOS3D predictor conv is evaluated only at the pixels that survive the 2-D
  * threshold and per-level top-k, between the two halves of the decode, when the head maps of one image hold >= 50 000 pixels (a per-image rule: batch-independent results) -- the dense
  * "b3d<l>" maps of dd3d_get_tensor then do not exist; 1: always; 0: never (dense fp32 maps, for stage-level tests); changing
- * it drops the engine's plans), "dla_front" (default 1: DLA-34 base_layer + level0 + level1 + pool run as one kernel; 0: layer by layer; flipping it
+ * it drops the engine's plans), "sparse_tower" (2 = auto, the default: with the sparse predictor, a non-GN box3d tower on
+ * pair-tile convs and >= 50 000 head pixels per image, the tower runs after the threshold / top-k on the conv tiles the
+ * predictor's reads need -- bit-identical detections, the "op<i>" outputs of the tower hold stale values elsewhere; 1: whenever
+ * the sparse predictor runs and the tower qualifies; 0: dense tower; changing it drops the engine's plans), "dla_front" (default 1: DLA-34 base_layer + level0 + level1 + pool run as one kernel; 0: layer by layer; flipping it
  * drops the engine's plans), "workspace_reuse" (default 1: activation buffers with disjoint lifetimes share workspace memory --
  * after a forward only "input", "p0".."p4" and the head maps of dd3d_get_tensor are intact; 0: every op output keeps its own
  * memory, for stage-level tests; applies to plans made afterwards), and "workspace_fill" (0..255: dd3d_plan fills the whole workspace with that byte first, -1 = off;
