@@ -430,6 +430,82 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
     return st;
 }
 
+int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
+                         const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch, const uint32_t* d_tiles,
+                         const int32_t* d_count, dd3d_stream stream) {
+    if (!d_in || !d_w || !d_scale || !d_bias || !d_out || !d_tiles || !d_count) return DD3D_ERR_INVALID;
+    if (B < 1 || B > kTileListMaxImages || H < 1 || W < 1 || cin < 1 || in_pitch < cin || cout < 128 || cout % 128 ||
+        out_pitch < cout)
+        return DD3D_ERR_INVALID;
+    ConvParams p;
+    memset(&p, 0, sizeof(p));
+    const int kchunks = (cin + kBlockK - 1) / kBlockK;
+    p.nseg = 1;
+    p.B = B;
+    p.taps = 9;
+    p.stride = 1;
+    p.kchunks = kchunks;
+    p.cin = cin;
+    p.relu = relu;
+    p.fp16 = g_op_fp16;
+    // the pair tile in work-list mode, whatever the pair / halo policies choose for dd3d_op_conv2d
+    p.halo = conv_halo_mode();
+    p.pair = 1;
+    p.block_n = 128;
+    p.n_blocks = cout / 128;
+    p.tile_list = d_tiles;
+    p.tile_count = d_count;
+    ConvSeg& g = p.seg[0];
+    g.H = H;
+    g.W = W;
+    g.th = kHaloTh;
+    g.tw = kHaloTw;
+    if (((H + kHaloTh - 1) / kHaloTh) * ((W + kHaloTw - 1) / kHaloTw) >= kTileListMaxTiles) return DD3D_ERR_INVALID;
+    if (!make_act_map_halo(&g.in_map[0], d_in, B, H, W, cin, in_pitch, g_op_fp16) ||
+        !make_act_map(&g.out_map, d_out, B, H, W, cout, out_pitch, g.th, g.tw, g_op_fp16) ||
+        !make_weight_map(&p.w_map, d_w, 9 * kchunks * kBlockK, cout, p.block_n, g_op_fp16)) {
+        fprintf(stderr, "dd3d_op_conv2d_tiles: %s\n", conv_last_error());
+        return DD3D_ERR_CUDA;
+    }
+    g.scale = d_scale;
+    g.bias = d_bias;
+    g.out_pitch = out_pitch;
+    conv_finalize_params(&p);
+    const cudaError_t e = launch_conv(p, device_sms(), static_cast<cudaStream_t>(stream));
+    return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
+}
+
+int dd3d_op_b3d_sparse(const void* const* d_in, const int32_t* h_level_hw, const int32_t* h_pitch, const void* const* d_w,
+                       const float* const* d_scale, const float* const* d_bias, const void* d_fin, const int32_t* d_counts,
+                       int B, int C, int topk, int n_pad, float* d_rows, int out_pitch, dd3d_stream stream) {
+    if (!d_in || !h_level_hw || !h_pitch || !d_w || !d_scale || !d_bias || !d_fin || !d_counts || !d_rows) return DD3D_ERR_INVALID;
+    if (B < 1 || C < 1 || topk < 1) return DD3D_ERR_INVALID;
+    B3dSparseParams p;
+    memset(&p, 0, sizeof(p));
+    for (int l = 0; l < kLevels; ++l) {
+        B3dSparseLevel& v = p.lvl[l];
+        v.in = static_cast<const __nv_bfloat16*>(d_in[l]);
+        v.w = static_cast<const __nv_bfloat16*>(d_w[l]);
+        v.scale = d_scale[l];
+        v.bias = d_bias[l];
+        v.H = h_level_hw[2 * l];
+        v.W = h_level_hw[2 * l + 1];
+        v.pitch = h_pitch[l];
+        if (!v.scale || !v.bias || v.H < 1 || v.W < 1 || v.pitch < 256) return DD3D_ERR_INVALID;
+    }
+    p.fin = static_cast<const uint2*>(d_fin);
+    p.cand_count = d_counts;
+    p.rows = d_rows;
+    p.B = B;
+    p.C = C;
+    p.topk = topk;
+    p.n_pad = n_pad;
+    p.out_pitch = out_pitch;
+    p.fp16 = g_op_fp16;
+    const cudaError_t e = launch_b3d_sparse(p, static_cast<cudaStream_t>(stream));
+    return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
+}
+
 int dd3d_op_stem_conv(const void* d_in4, const void* d_w, const float* d_scale, const float* d_bias, void* d_out, int B,
                       int H, int W, int ksize, int stride, int cout, int out_pitch, dd3d_stream stream) {
     return cuda_status(launch_stem_tc(static_cast<const __nv_bfloat16*>(d_in4), static_cast<const __nv_bfloat16*>(d_w),

@@ -112,6 +112,9 @@ SIGNATURES = {
     "dd3d_get_conv_info": (_I, [_P, C.POINTER(C.c_int32), _I]),
     "dd3d_get_tensor": (_I, [_P, C.c_char_p, C.POINTER(_P), C.POINTER(C.c_int32 * 6)]),
     "dd3d_op_conv2d": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _I, _I, _P]),
+    "dd3d_op_conv2d_tiles": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _I, _P, _I, _P, _P, _P]),
+    "dd3d_op_b3d_sparse": (_I, [C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P),
+                                C.POINTER(_P), _P, _P, _I, _I, _I, _I, _P, _I, _P]),
     "dd3d_op_dla_front": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_s2_mma": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_conv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),

@@ -296,6 +296,25 @@ int dd3d_num_ops(dd3d_handle h);
 int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout, int ksize,
                    int stride, const float* d_scale, const float* d_bias, int relu, const void* d_residual,
                    int res_pitch, int res_up2, void* d_out, int out_pitch, int out_f32, dd3d_stream stream);
+/* dd3d_op_conv2d_tiles: dd3d_op_conv2d (3x3, stride 1, 16-bit output, cout a multiple of 128, no residual) on the pair-tile
+ * kernel in work-list mode, the form the engine runs the sparse box3d tower in: only the 16x8 output tiles listed in d_tiles
+ * are computed, every other output pixel is left untouched.  d_tiles: device uint32 entries (img << 16) | tile, tile = the
+ * row-major index of a 16x8 tile of one image (the tile count of an image, ceil(H/16) * ceil(W/8), names the out-of-image
+ * tile, which writes nothing); consecutive entries 2i, 2i + 1 form one work item.  d_count: device int32, the number of
+ * entries (even), read by the kernel. */
+int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
+                         const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch, const uint32_t* d_tiles,
+                         const int32_t* d_count, dd3d_stream stream);
+/* dd3d_op_b3d_sparse: the sparse FCOS3D box3d predictor (csrc/b3d_sparse.cu) on caller buffers: for every (image b, level l)
+ * and slot s < min(d_counts[b * 5 + l], topk), row (b * 5 + l) * topk + s of d_rows (fp32, out_pitch floats per row) receives
+ * the 3x3 conv of level l's tower output at the candidate's pixel, channels 0 .. n_pad-1, times d_scale[l] plus d_bias[l]
+ * (fp32).  Other rows are not written.  d_in[l]: 16-bit NHWC [B][H_l][W_l][h_pitch[l]] with 256 channels (h_level_hw = [5][2]
+ * (H, W)); d_w[l]: 16-bit [n_pad][9][256] (dd3d_op_conv2d layout); d_fin: device [B][5][topk] uint32 pairs (any, pixel * C +
+ * class); n_pad a multiple of 8, at most 112. */
+int dd3d_op_b3d_sparse(const void* const* d_in /*[5]*/, const int32_t* h_level_hw, const int32_t* h_pitch /*[5]*/,
+                       const void* const* d_w /*[5]*/, const float* const* d_scale /*[5]*/, const float* const* d_bias /*[5]*/,
+                       const void* d_fin, const int32_t* d_counts, int B, int C, int topk, int n_pad, float* d_rows,
+                       int out_pitch, dd3d_stream stream);
 int dd3d_op_stem_conv(const void* d_in4, const void* d_w, const float* d_scale, const float* d_bias, void* d_out,
                       int B, int H, int W, int ksize, int stride, int cout, int out_pitch, dd3d_stream stream);
 /* dd3d_op_dla_front: the fused DLA-34 front end (csrc/dla_front.cu; reference dla.py:271-283,346-350 base_layer -> level0
