@@ -34,15 +34,30 @@ cudaError_t launch_b3d_sparse(const B3dSparseParams& p, cudaStream_t stream);
 // (Chebyshev), clipped to the map.  tower_tiles_kernel lists, per layer, the conv tiles that meet that set; the tower convs
 // then run the pair tile in work-list mode (ConvParams::tile_list) on exactly those tiles; every (image, level) list is
 // padded to an even length with an out-of-image tile, so that a pair never spans two levels.
+//
+// Sparse box2d tower: the decode reads the [box2d_reg | centerness] map only at the pixels of P, where some class passes the
+// class-only threshold (class_passes, detect.cuh), and the predictor is a 3x3 conv of the last tower layer.  So list `depth`
+// - 1 (the predictor's) holds the tiles that meet P, and tower layer i the tiles within depth - 1 - i of it.  Its seeds come
+// from a pixel-parallel marking pass over the cls maps (launch_tower_mark), which lowers the tile distances in `dist`.
+//
+// List i holds the tiles at distance <= reach - i from a seed: reach = depth for the box3d tower (its predictor reads 3x3
+// neighbourhoods of the candidates), depth - 1 for the box2d tower and its predictor.
 struct TowerTilesLevel {
     int H, W, th, tw, tiles_x, tiles_y;
     int stage_begin;  // first entry of this level's (image-major) per-image regions in a layer's staging / list area
+    const float* cls;  // mark pass: cls map [B][H*W][cls_pitch] of the level
+    int mark_begin;    // mark pass: first block (of grid.x) of this level
 };
+constexpr int kTowerTileFar = 0x3F3F3F3F;  // tile distance "no seed near": the 0x3F byte pattern (cudaMemset)
 struct TowerTilesParams {
     TowerTilesLevel lvl[kLevels];
-    const uint2* fin;           // DecodeParams::fin
+    const uint2* fin;           // seeds: DecodeParams::fin (nullptr: the distances of the mark pass in `dist`)
     const int32_t* cand_count;  // [B][L]
-    int B, C, topk, depth;
+    int32_t* dist;              // mark pass: [cap] tile distances, (level, image) regions at the offsets of a layer's list;
+                                // kTowerTileFar between launches (tower_tiles_kernel reads and resets them)
+    int B, C, topk, depth, reach;
+    int cls_pitch, mark_blocks;  // mark pass
+    float thresh;                // mark pass: PRE_NMS_THRESH
     int cap;        // entries per layer: sum over levels of B * (tiles per image, rounded up to even)
     int max_tiles;  // largest tiles per image of a level (shared memory)
     uint32_t* stage;     // [depth][cap] per-(image, level) lists at fixed offsets
@@ -54,6 +69,8 @@ struct TowerTilesParams {
     uint32_t* ticket;    // zero between launches; the last CTA to finish compacts and resets it
 };
 size_t tower_tiles_smem_bytes(int max_tiles);
+constexpr int kTowerMarkThreads = 256;  // mark pass: head pixels per block (TowerTilesLevel::mark_begin)
+cudaError_t launch_tower_mark(const TowerTilesParams& p, cudaStream_t stream);  // needs p.dist; then launch_tower_tiles
 cudaError_t launch_tower_tiles(const TowerTilesParams& p, cudaStream_t stream);
 
 }  // namespace dd3d

@@ -230,6 +230,10 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value) {
             const int v = value < 0 ? 0 : (value > 2 ? 2 : value);
             if (e.opt_sparse_tower != v) e.drop_plans();
             e.opt_sparse_tower = v;
+        } else if (n == "sparse_box2d_tower") {  // 2 (default): auto with the sparse predictor; 1: whenever eligible; 0: dense
+            const int v = value < 0 ? 0 : (value > 2 ? 2 : value);
+            if (e.opt_sparse_box2d_tower != v) e.drop_plans();
+            e.opt_sparse_box2d_tower = v;
         } else if (n == "dla_front") {  // 1 (default): fused DLA-34 front end (dla_front.cu); 0: layer by layer
             if (e.opt_dla_front != (value ? 1 : 0)) e.drop_plans();
             e.opt_dla_front = value ? 1 : 0;
@@ -322,6 +326,9 @@ int dd3d_get_tensor(dd3d_handle h, const char* name, void** d_ptr, int32_t dims[
             memcpy(dims, d, sizeof(d));
         } else if (n.rfind("box", 0) == 0) {
             const int l = level(3);
+            if (P.box2d_begin >= 0)
+                throw EngineError(DD3D_ERR_INVALID, "the box2d map is computed only around the pixels that pass the threshold "
+                                                    "with option sparse_box2d_tower: " + n);
             *d_ptr = P.box_map[l];
             const int32_t d[6] = {P.B, P.lvl_h[l], P.lvl_w[l], 5, 16, 4};
             memcpy(dims, d, sizeof(d));
@@ -341,6 +348,22 @@ int dd3d_get_tensor(dd3d_handle h, const char* name, void** d_ptr, int32_t dims[
 }
 
 // ------------------------------------------------------------------------------------------------ operators
+
+// Repacks the 3x3 weights [16][9][cin_pad] into the taps-in-N layout [9 * 16][cin_pad] in a new device buffer *d_w_taps
+// (the caller frees it after the launch has run; operator entry points only, not a hot path) and encodes its tensor map.
+static bool taps_weights(const void* d_w, int cin_pad, CUtensorMap* map, void** d_w_taps, cudaStream_t stream) {
+    if (cudaMalloc(d_w_taps, static_cast<size_t>(kTapsN) * cin_pad * 2) != cudaSuccess) return false;
+    for (int t = 0; t < 9; ++t)
+        cudaMemcpy2DAsync(static_cast<uint8_t*>(*d_w_taps) + static_cast<size_t>(t) * 16 * cin_pad * 2, cin_pad * 2,
+                          static_cast<const uint8_t*>(d_w) + static_cast<size_t>(t) * cin_pad * 2, 9 * cin_pad * 2,
+                          cin_pad * 2, 16, cudaMemcpyDeviceToDevice, stream);
+    if (!make_weight_map_taps(map, *d_w_taps, cin_pad, g_op_fp16)) {
+        cudaStreamSynchronize(stream);
+        cudaFree(*d_w_taps);
+        return false;
+    }
+    return true;
+}
 
 int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout, int ksize,
                    int stride, const float* d_scale, const float* d_bias, int relu, const void* d_residual,
@@ -407,17 +430,7 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
     conv_finalize_params(&p);
     void* d_w_taps = nullptr;
     if (p.taps_n) {
-        // repack [16][9][cin_pad] -> taps-in-N [9 * 16][cin_pad] on the device (operator entry point: not a hot path)
-        const int cin_pad = kchunks * kBlockK;
-        if (cudaMalloc(&d_w_taps, static_cast<size_t>(kTapsN) * cin_pad * 2) != cudaSuccess) return DD3D_ERR_CUDA;
-        for (int t = 0; t < 9; ++t)
-            cudaMemcpy2DAsync(static_cast<uint8_t*>(d_w_taps) + static_cast<size_t>(t) * 16 * cin_pad * 2, cin_pad * 2,
-                              static_cast<const uint8_t*>(d_w) + static_cast<size_t>(t) * cin_pad * 2, 9 * cin_pad * 2,
-                              cin_pad * 2, 16, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream));
-        if (!make_weight_map_taps(&p.w_map, d_w_taps, cin_pad, g_op_fp16)) {
-            cudaFree(d_w_taps);
-            return DD3D_ERR_CUDA;
-        }
+        if (!taps_weights(d_w, kchunks * kBlockK, &p.w_map, &d_w_taps, static_cast<cudaStream_t>(stream))) return DD3D_ERR_CUDA;
     } else if (!make_weight_map(&p.w_map, d_w, taps * kchunks * kBlockK, cout_pad, p.block_n, g_op_fp16)) {
         fprintf(stderr, "dd3d_op_conv2d: %s\n", conv_last_error());
         return DD3D_ERR_CUDA;
@@ -472,6 +485,58 @@ int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_
     g.out_pitch = out_pitch;
     conv_finalize_params(&p);
     const cudaError_t e = launch_conv(p, device_sms(), static_cast<cudaStream_t>(stream));
+    return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
+}
+
+int dd3d_op_conv2d_taps_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
+                              const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch, int out_f32,
+                              const uint32_t* d_tiles, const int32_t* d_count, dd3d_stream stream) {
+    if (!d_in || !d_w || !d_scale || !d_bias || !d_out || !d_tiles || !d_count) return DD3D_ERR_INVALID;
+    if (B < 1 || B > kTileListMaxImages || H < 1 || W < 1 || cin < 1 || in_pitch < cin || cout < 1 || cout > 16 ||
+        out_pitch < 16 || (out_f32 ? out_pitch % 4 : out_pitch % 8))
+        return DD3D_ERR_INVALID;
+    if (((H + kHaloTh - 1) / kHaloTh) * ((W + kHaloTw - 1) / kHaloTw) >= kTileListMaxTiles) return DD3D_ERR_INVALID;
+    ConvParams p;
+    memset(&p, 0, sizeof(p));
+    const int kchunks = (cin + kBlockK - 1) / kBlockK;
+    p.nseg = 1;
+    p.B = B;
+    p.taps = 9;
+    p.stride = 1;
+    p.kchunks = kchunks;
+    p.cin = cin;
+    p.n_blocks = 1;
+    p.block_n = 16;
+    p.relu = relu;
+    p.out_mode = out_f32 ? 1 : 0;
+    p.fp16 = g_op_fp16;
+    // the taps-in-N kernel in work-list mode, whatever the taps / halo policies choose for dd3d_op_conv2d
+    p.halo = conv_halo_mode();
+    p.taps_n = 1;
+    p.tile_list = d_tiles;
+    p.tile_count = d_count;
+    ConvSeg& g = p.seg[0];
+    g.H = H;
+    g.W = W;
+    g.th = kHaloTh;
+    g.tw = kHaloTw;
+    if (!make_act_map_halo(&g.in_map[0], d_in, B, H, W, cin, in_pitch, g_op_fp16)) {
+        fprintf(stderr, "dd3d_op_conv2d_taps_tiles: %s\n", conv_last_error());
+        return DD3D_ERR_CUDA;
+    }
+    g.scale = d_scale;
+    g.bias = d_bias;
+    g.out_pitch = out_pitch;
+    if (out_f32)
+        g.out_f32 = static_cast<float*>(d_out);
+    else
+        g.out16 = d_out;
+    conv_finalize_params(&p);
+    void* d_w_taps = nullptr;
+    if (!taps_weights(d_w, kchunks * kBlockK, &p.w_map, &d_w_taps, static_cast<cudaStream_t>(stream))) return DD3D_ERR_CUDA;
+    const cudaError_t e = launch_conv(p, device_sms(), static_cast<cudaStream_t>(stream));
+    cudaStreamSynchronize(static_cast<cudaStream_t>(stream));
+    cudaFree(d_w_taps);
     return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
 }
 

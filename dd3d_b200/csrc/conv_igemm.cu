@@ -30,7 +30,9 @@ constexpr int kTapsPBytes = (kTapsPRows * kTapsPStride * 4 + 1023) / 1024 * 1024
 constexpr int kTapsSmem = kTapsStages * (kHaloABytes + kTapsBBytes) + kTapsPBytes + kBarBytes + 1024;
 constexpr int kTapsConsumerWarps = 12;
 
-template <bool F16>
+// LIST: work-list mode (ConvParams::tile_list, one entry per tile) -- the sparse box2d tower's predictor.  The out-of-image
+// padding tile of a list loads zeros and stores nothing (the oy < H && ox < W guard).
+template <bool F16, bool LIST = false>
 __global__ void __launch_bounds__(kTapsThreads, 1) conv_taps_kernel(const __grid_constant__ ConvParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -58,13 +60,16 @@ __global__ void __launch_bounds__(kTapsThreads, 1) conv_taps_kernel(const __grid
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-    const int w_first = static_cast<int>(blockIdx.x), w_step = static_cast<int>(gridDim.x), w_total = p.total_work;
+    const int w_first = static_cast<int>(blockIdx.x), w_step = static_cast<int>(gridDim.x);
+    // work-list mode: the list was written by an earlier kernel of the stream (n_blocks is 1).  The count is re-read (an L1
+    // hit) at every step rather than held: the consumers have no register to spare.
+    auto w_total = [&]() { return LIST ? __shfl_sync(0xffffffffu, __ldg(p.tile_count), 0) : p.total_work; };
     if (warp == 0) {
         // ------------------------------------------------------------ TMA producer: halo patch + weight tile per 64-ch block
         int stage = 0;
         uint32_t phase = 0;
-        for (int work = w_first; work < w_total; work += w_step) {
-            const TileCoord t = decode_tile(p, work);
+        for (int work = w_first; work < w_total(); work += w_step) {
+            const TileCoord t = decode_tile<false, LIST>(p, work);
             const ConvSeg& g = p.seg[t.seg];
             for (int kc = 0; kc < p.kchunks; ++kc) {
                 ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -92,8 +97,8 @@ __global__ void __launch_bounds__(kTapsThreads, 1) conv_taps_kernel(const __grid
         float acc[kTapsN / 2];
         int stage = 0;
         uint32_t phase = 0;
-        for (int work = w_first; work < w_total; work += w_step) {
-            const TileCoord t = decode_tile(p, work);
+        for (int work = w_first; work < w_total(); work += w_step) {
+            const TileCoord t = decode_tile<false, LIST>(p, work);
             const ConvSeg& g = p.seg[t.seg];
             for (int kc = 0; kc < p.kchunks; ++kc) {
                 ptx::mbar_wait(&full_bar[stage], phase);
@@ -444,10 +449,11 @@ cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
     const int stage_bytes = (p.halo ? 0 : kABytes) + p.block_n * 128;
     const int smem_bytes = (p.wstat ? p.taps * p.kchunks : p.num_stages) * stage_bytes + conv_fixed_smem(p);
     ConvKernel kernel = nullptr;
-    if (p.tile_list != nullptr && (!p.pair || p.tile_count == nullptr)) return cudaErrorInvalidValue;  // list mode: pair tile only
+    const bool list = p.tile_list != nullptr;  // list mode: pair tile or taps-in-N
+    if (list && ((!p.pair && !p.taps_n) || p.tile_count == nullptr)) return cudaErrorInvalidValue;
     if (p.pair) {
         if (!p.halo || p.block_n != 128 || p.out_mode != 0) return cudaErrorInvalidValue;
-        kernel = conv_kernel_pair(p.fp16 != 0, p.tile_list != nullptr);
+        kernel = conv_kernel_pair(p.fp16 != 0, list);
     }
     for (auto group : {conv_kernel_n16_64, conv_kernel_n80_128, conv_kernel_n144_192, conv_kernel_n208_256}) {
         if (kernel == nullptr) kernel = group(p.halo != 0, p.fp16 != 0, p.block_n);
@@ -474,7 +480,8 @@ cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
                                              kSmemBudget);
             }
         }
-        for (auto fn : {conv_taps_kernel<false>, conv_taps_kernel<true>}) {
+        for (auto fn : {conv_taps_kernel<false>, conv_taps_kernel<true>, conv_taps_kernel<false, true>,
+                        conv_taps_kernel<true, true>}) {
             if (e == cudaSuccess) e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kTapsSmem);
         }
         if (e != cudaSuccess) return e;
@@ -496,8 +503,12 @@ cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = use_pdl ? 1 : 0;
-    if (p.taps_n)
+    if (p.taps_n) {
+        if (list)
+            return p.fp16 ? cudaLaunchKernelEx(&cfg, conv_taps_kernel<true, true>, p)
+                          : cudaLaunchKernelEx(&cfg, conv_taps_kernel<false, true>, p);
         return p.fp16 ? cudaLaunchKernelEx(&cfg, conv_taps_kernel<true>, p) : cudaLaunchKernelEx(&cfg, conv_taps_kernel<false>, p);
+    }
     return cudaLaunchKernelEx(&cfg, kernel, p);
 }
 

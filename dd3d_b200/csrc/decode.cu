@@ -24,8 +24,6 @@ namespace {
 constexpr int kDenseThreads = 256;
 constexpr float kEps = 1e-7f;
 
-__device__ __forceinline__ float sigmoidf(float x) { return 1.0f / (1.0f + expf(-x)); }
-
 __device__ __forceinline__ int find_level(const DecodeParams& p, int blk) {
     int l = 0;
 #pragma unroll
@@ -55,10 +53,11 @@ __global__ void __launch_bounds__(kDenseThreads) dense_kernel(const __grid_const
     }
     int T = 0;
     if (MODE == 1) T = p.sel[bl * 4 + 0];
-    if (pix < hw) {
-        const size_t gp = static_cast<size_t>(b) * hw + pix;
+    const size_t gp = static_cast<size_t>(b) * hw + pix;
+    const float* lg = L.cls + gp * p.cls_pitch;
+    // no class passing alone: no score passes either (class_passes), and the box map row may not have been computed
+    if (pix < hw && class_passes(lg, p.C, p.thresh)) {
         const float ctr = sigmoidf(__ldg(L.box + gp * 16 + 4));
-        const float* lg = L.cls + gp * p.cls_pitch;
         for (int c0 = 0; c0 < p.C; c0 += 4) {
             const float4 v = __ldg(reinterpret_cast<const float4*>(lg + c0));
             const float vv[4] = {v.x, v.y, v.z, v.w};

@@ -30,6 +30,23 @@ struct Det {
 };
 static_assert(sizeof(Det) == 96, "Det must be 24 words");
 
+__device__ __forceinline__ float sigmoidf(float x) { return 1.0f / (1.0f + expf(-x)); }
+
+// The class-only threshold: some class column c < C of a pixel's logits (a 16-byte aligned cls map row) has
+// sigmoid(logit) > thresh.  The decode reads a pixel's box2d map row only when this holds: with THRESH_WITH_CTR the
+// thresholded score is RN(sigmoid(cls) * sigmoid(ctr)) <= sigmoid(cls), since sigmoid(ctr) <= 1 (or NaN) and rounding is
+// monotone.  So the sparse box2d tower (tower_tiles.cu) seeds its tile lists with the pixels this returns true for.
+__device__ __forceinline__ bool class_passes(const float* logits, int C, float thresh) {
+    bool any = false;
+    for (int c0 = 0; c0 < C; c0 += 4) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(logits + c0));
+        const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) any |= c0 + j < C && sigmoidf(vv[j]) > thresh;
+    }
+    return any;
+}
+
 struct DecodeLevel {
     const float* cls;  // [B][H*W][cls_pitch]   logits
     const float* box;  // [B][H*W][16]          0..3 = relu(scale*reg) (l,t,r,b), 4 = centerness logit

@@ -54,6 +54,7 @@ Engine::Engine(const dd3d_model_desc& d) : desc(d) {
     if (const char* e = getenv("DD3D_DLA_FRONT")) opt_dla_front = atoi(e) ? 1 : 0;  // A/B runs of bench.py; default 1
     if (const char* e = getenv("DD3D_SPARSE_BOX3D")) opt_sparse_box3d = std::max(0, std::min(2, atoi(e)));
     if (const char* e = getenv("DD3D_SPARSE_TOWER")) opt_sparse_tower = std::max(0, std::min(2, atoi(e)));
+    if (const char* e = getenv("DD3D_SPARSE_BOX2D_TOWER")) opt_sparse_box2d_tower = std::max(0, std::min(2, atoi(e)));
     if (const char* e = getenv("DD3D_STEM_MMA")) opt_stem_mma = atoi(e) ? 1 : 0;
     if (const char* e = getenv("DD3D_ESE_POOL")) opt_ese_pool = atoi(e) ? 1 : 0;
 }
@@ -895,10 +896,10 @@ struct Builder {
         *out = cur;
     }
 
-    // Tile lists of the sparse box3d tower (TowerTilesParams): the tiling conv() gives the tower layers, and the staging, list
-    // and count areas in the persistent region.  false: the shapes exceed the list entry fields, the tower stays dense.
-    bool tower_tile_lists(const std::vector<View>& feats, int depth) {
-        TowerTilesParams& tt = P->tower_tiles;
+    // Tile lists of a sparse tower (TowerTilesParams): `depth` lists, list i at distance <= reach - i; the tiling conv() gives
+    // the tower layers, and the staging, list and count areas in the persistent region.  false: the shapes exceed the list
+    // entry fields or the layers do not run the pair tile, the tower stays dense.
+    bool tower_tile_lists(TowerTilesParams& tt, const std::vector<View>& feats, int depth, int reach) {
         memset(&tt, 0, sizeof(tt));
         const int L = static_cast<int>(feats.size());
         int hs[kMaxSeg], ws[kMaxSeg];
@@ -941,6 +942,7 @@ struct Builder {
         if (!conv_select_pair(&cp, 256, E->num_sms)) return false;
         tt.B = B;
         tt.depth = depth;
+        tt.reach = reach;
         const size_t list_bytes = static_cast<size_t>(depth) * tt.cap * 4, bl_bytes = static_cast<size_t>(depth) * L * B * 4;
         tt.stage = static_cast<uint32_t*>(alloc_bytes(list_bytes));
         tt.list = static_cast<uint32_t*>(alloc_bytes(list_bytes));
@@ -950,6 +952,22 @@ struct Builder {
         tt.pixels = static_cast<long long*>(alloc_bytes(static_cast<size_t>(depth) * 8));
         tt.ticket = static_cast<uint32_t*>(alloc_bytes(4));
         return true;
+    }
+
+    // Points plan ops [begin, begin + tt.depth) -- tower convs on the pair tile, then (box2d) the taps-in-N predictor -- at
+    // their tile lists.
+    void use_tile_lists(int begin, const TowerTilesParams& tt, int L, const char* what) {
+        for (int j = 0; j < tt.depth; ++j) {
+            Op& op = P->ops[begin + j];
+            ConvParams& c = op.conv;
+            if (op.type != Op::CONV || c.nseg != L || !(c.pair || c.taps_n))
+                fail(DD3D_ERR_STATE, std::string("internal: sparse ") + what + " layout");
+            for (int l = 0; l < L; ++l)
+                if (c.seg[l].th != tt.lvl[l].th || c.seg[l].tw != tt.lvl[l].tw)
+                    fail(DD3D_ERR_STATE, std::string("internal: sparse ") + what + " tiling");
+            c.tile_list = tt.list + static_cast<size_t>(j) * tt.cap;
+            c.tile_count = tt.count + j;
+        }
     }
 
     void build_heads(const std::vector<View>& feats) {
@@ -1022,8 +1040,33 @@ struct Builder {
             }
             conv(Lc, 1, false, segs, true);
         }
+        // sparse box2d tower: the decode reads the box map only at the pixels where some class passes the threshold alone
+        // (class_passes, detect.cuh), which the cls map above decides.  So the tower runs on the tiles within d2 - i of them
+        // and the taps-in-N predictor on the tiles that meet them, listed right before the tower (GN needs whole-map
+        // statistics).  Auto follows the sparse box3d predictor, which the stage-level tests switch off to read dense maps.
+        const int d2 = E->layout.num_box2d_convs;
+        int hs[kMaxSeg], ws[kMaxSeg];
+        for (int l = 0; l < L; ++l) {
+            hs[l] = feats[l].H;
+            ws[l] = feats[l].W;
+        }
+        const bool sparse_box2d =
+            d2 > 0 && E->layout.fcos2d_norm != DD3D_NORM_GN &&
+            (E->opt_sparse_box2d_tower == 1 || (E->opt_sparse_box2d_tower == 2 && sparse3 && head_px >= 50000)) &&
+            conv_taps_eligible(9, 1, 16, L, hs, ws) && tower_tile_lists(P->box2d_tiles, feats, d2 + 1, d2);
+        P->box2d_begin = sparse_box2d ? static_cast<int>(P->ops.size()) : -1;
+        if (sparse_box2d) {
+            TowerTilesParams& tt = P->box2d_tiles;
+            tt.dist = static_cast<int32_t*>(alloc_bytes(static_cast<size_t>(tt.cap) * 4));
+            tt.cls_pitch = cls_pitch;
+            for (int l = 0; l < L; ++l) {
+                tt.lvl[l].cls = P->cls_map[l];
+                tt.lvl[l].mark_begin = tt.mark_blocks;
+                tt.mark_blocks += (feats[l].H * feats[l].W + kTowerMarkThreads - 1) / kTowerMarkThreads;
+            }
+        }
         // [box2d_reg (4) | centerness (1)] on the box2d tower: relu(scale_l * (conv + b)) / conv + b (fcos2d.py:143-152)
-        tower("fcos2d_head.box2d_tower", E->layout.num_box2d_convs, E->layout.fcos2d_norm, feats, &box_t);
+        tower("fcos2d_head.box2d_tower", d2, E->layout.fcos2d_norm, feats, &box_t);
         {
             const ConvLayer& Lb = E->conv_layer("fcos2d_head.box2d_reg+centerness",
                                                 {"fcos2d_head.box2d_reg", "fcos2d_head.centerness"}, 256, 3);
@@ -1053,6 +1096,7 @@ struct Builder {
             }
             conv(Lb, 1, false, segs, true);
         }
+        if (sparse_box2d && !dry) use_tile_lists(P->box2d_begin, P->box2d_tiles, L, "box2d tower");
         // [quat 4C | ctr 2C | depth C | size 3C | conf C] on the box3d tower with the per-level Scale/Offset folded
         // (fcos3d.py:166-180; PER_LEVEL_PREDICTORS False -> predictor index 0)
         if (!box3d_on) return;  // MODEL.BOX3D_ON = False (core.py:34-40): 2-D detector only
@@ -1063,22 +1107,10 @@ struct Builder {
         const int d3 = E->layout.num_box3d_convs;
         const bool sparse_tower = sparse3 && d3 > 0 && E->layout.fcos3d_norm != DD3D_NORM_GN &&
                                   (E->opt_sparse_tower == 1 || (E->opt_sparse_tower == 2 && head_px >= 50000)) &&
-                                  tower_tile_lists(feats, d3);
+                                  tower_tile_lists(P->tower_tiles, feats, d3, d3);
         P->tower_begin = sparse_tower ? static_cast<int>(P->ops.size()) : -1;
         tower("fcos3d_head.box3d_tower", d3, E->layout.fcos3d_norm, feats, &b3d_t);
-        if (sparse_tower && !dry) {
-            const TowerTilesParams& tt = P->tower_tiles;
-            for (int j = 0; j < d3; ++j) {
-                Op& op = P->ops[P->tower_begin + j];
-                ConvParams& c = op.conv;
-                if (op.type != Op::CONV || c.nseg != L || !c.pair) fail(DD3D_ERR_STATE, "internal: sparse box3d tower layout");
-                for (int l = 0; l < L; ++l)
-                    if (c.seg[l].th != tt.lvl[l].th || c.seg[l].tw != tt.lvl[l].tw)
-                        fail(DD3D_ERR_STATE, "internal: sparse box3d tower tiling");
-                c.tile_list = tt.list + static_cast<size_t>(j) * tt.cap;
-                c.tile_count = tt.count + j;
-            }
-        }
+        if (sparse_tower && !dry) use_tile_lists(P->tower_begin, P->tower_tiles, L, "box3d tower");
         // [quat 4C | ctr 2C | depth C | size 3C | conf C] on the box3d tower with the per-level Scale/Offset folded
         // (fcos3d.py:166-180).  PER_LEVEL_PREDICTORS False (shipped): predictor index 0 for every level, one launch over the
         // five levels; True: level l uses predictor l, one launch per level.
@@ -1470,6 +1502,15 @@ void Engine::make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes) {
         cuda_check(cudaMemset(tt.ticket, 0, 4), "cudaMemset(tower tile ticket)");
         cuda_check(cudaDeviceSynchronize(), "cudaDeviceSynchronize");
     }
+    if (plan.box2d_begin >= 0) {
+        TowerTilesParams& tt = plan.box2d_tiles;
+        tt.C = desc.num_classes;
+        tt.thresh = dp.thresh;  // the decode's own threshold value: class_passes must agree bit for bit
+        // the ticket and the tile distances start as each launch leaves them
+        cuda_check(cudaMemset(tt.ticket, 0, 4), "cudaMemset(box2d tile ticket)");
+        cuda_check(cudaMemset(tt.dist, kTowerTileFar & 0xFF, static_cast<size_t>(tt.cap) * 4), "cudaMemset(box2d tile distances)");
+        cuda_check(cudaDeviceSynchronize(), "cudaDeviceSynchronize");
+    }
     fill_nms_params(&plan.nms, desc, dp, B);
     plan.nms.scratch = plan.nms_scratch;
 }
@@ -1514,7 +1555,7 @@ void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodePar
 
 int Engine::launches_per_forward() const {
     int n = 1 /*preprocess*/ + 6 /*decode: clear, 2 dense passes, 2 selects, final*/ + (plan.sparse_b3d ? 1 : 0) +
-            (plan.tower_begin >= 0 ? 1 : 0) /*tower tile lists*/ + ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) /*nms: sort, IoU bit matrix, scan, finish*/;
+            (plan.tower_begin >= 0 ? 1 : 0) /*tower tile lists*/ + (plan.box2d_begin >= 0 ? 2 : 0) /*box2d mark + lists*/ + ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) /*nms: sort, IoU bit matrix, scan, finish*/;
     for (const Op& op : plan.ops) n += (op.type == Op::ESE) ? 3 : (op.type == Op::GN && op.gn.gamma != nullptr) ? 2 : 1;
     return n;
 }
@@ -1606,6 +1647,11 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
     dp.K = d_K;
     for (const Op& op : P.ops) {
         const int oi = static_cast<int>(&op - P.ops.data());
+        if (oi == P.box2d_begin) {  // sparse box2d tower: the pixels of the cls maps that pass the threshold, then the tiles
+            cuda_check(launch_tower_mark(P.box2d_tiles, stream), "box2d tower seeds");
+            cuda_check(launch_tower_tiles(P.box2d_tiles, stream), "box2d tower tile lists");
+            mark(6);
+        }
         if (oi == P.tower_begin) {  // sparse box3d tower: the final candidates first, then the tiles they need
             cuda_check(launch_decode_select(dp, stream), "decode (threshold + top-k)");
             cuda_check(launch_tower_tiles(P.tower_tiles, stream), "box3d tower tile lists");
@@ -1683,24 +1729,26 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
     if (opt_profile) prof_used = ev_i;
 }
 
-// Algorithmic FLOPs per plan op.  The sparse box3d tower convs count the in-map pixels of the tiles the last forward ran,
+// Algorithmic FLOPs per plan op.  The convs of the sparse towers count the in-map pixels of the tiles the last forward ran,
 // read back from the device (call after that forward has completed).
 std::vector<double> Engine::op_flops() {
     std::vector<double> f(plan.ops.size());
     for (size_t i = 0; i < f.size(); ++i) f[i] = plan.ops[i].flops;
-    if (plan.tower_begin >= 0) {
-        const int d = plan.tower_tiles.depth;
+    auto listed = [&](int begin, const TowerTilesParams& tt, const char* what) {
+        if (begin < 0) return;
+        const int d = tt.depth;
         std::vector<long long> px(d, 0);
         if (plan.ran && prof_used >= 2)  // the callers have synchronised the last profiled forward
-            cuda_check(cudaMemcpy(px.data(), plan.tower_tiles.pixels, d * sizeof(long long), cudaMemcpyDeviceToHost),
-                       "D2H tower tile pixels");
+            cuda_check(cudaMemcpy(px.data(), tt.pixels, d * sizeof(long long), cudaMemcpyDeviceToHost), what);
         for (int j = 0; j < d; ++j) {
-            const ConvParams& c = plan.ops[plan.tower_begin + j].conv;
+            const ConvParams& c = plan.ops[begin + j].conv;
             double dense_px = 0.0;
             for (int s = 0; s < c.nseg; ++s) dense_px += static_cast<double>(c.B) * c.seg[s].H * c.seg[s].W;
-            f[plan.tower_begin + j] *= static_cast<double>(px[j]) / dense_px;
+            f[begin + j] *= static_cast<double>(px[j]) / dense_px;
         }
-    }
+    };
+    listed(plan.box2d_begin, plan.box2d_tiles, "D2H box2d tile pixels");
+    listed(plan.tower_begin, plan.tower_tiles, "D2H tower tile pixels");
     return f;
 }
 
@@ -1773,7 +1821,7 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
                 break;
         }
     }
-    launches[6] = 6 + (P.sparse_b3d ? 1 : 0) + (P.tower_begin >= 0 ? 1 : 0);
+    launches[6] = 6 + (P.sparse_b3d ? 1 : 0) + (P.tower_begin >= 0 ? 1 : 0) + (P.box2d_begin >= 0 ? 2 : 0);
     launches[7] = (desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1;
     for (int l = 0; l < kLevels; ++l)  // two dense passes over the fp32 logits + centerness
         bytes[6] += 2.0 * P.B * P.lvl_h[l] * P.lvl_w[l] * (C + 1) * 4;

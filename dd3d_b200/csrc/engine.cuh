@@ -149,6 +149,11 @@ struct Plan {
     // workspace contents and is read by nothing.  -1: dense tower.
     int tower_begin = -1;
     TowerTilesParams tower_tiles;
+    // sparse box2d tower: ops [box2d_begin, box2d_begin + depth) are the box2d tower convs and its predictor (depth = tower
+    // convs + 1), in work-list mode on the tiles the class-only threshold needs (box2d_tiles, seeded by tower_mark_kernel
+    // right before them); the box map holds stale workspace contents outside those tiles.  -1: dense.
+    int box2d_begin = -1;
+    TowerTilesParams box2d_tiles;
     bool ran = false;  // a forward has run on this plan (the tile counts on the device are valid)
 };
 
@@ -220,6 +225,10 @@ class Engine {
     int opt_sparse_box3d = 2;  // box3d predictor at the final candidates only (b3d_sparse.cu): 0 never (dense maps), 1 always, 2 auto (by head size)
     int opt_sparse_tower = 2;  // box3d tower on the tiles the sparse predictor reads (tower_tiles.cu): 0 never, 1 whenever the
                                // sparse predictor runs and the tower norm is not GN, 2 auto (as 1, for heads of >= 50 000 pixels)
+    int opt_sparse_box2d_tower = 2;  // box2d tower + predictor on the tiles around the pixels whose class score passes the
+                                     // threshold (tower_tiles.cu): 0 never, 1 whenever the tower norm is not GN and the tower
+                                     // convs use the pair tile, 2 auto (as 1, with the sparse box3d predictor and heads of
+                                     // >= 50 000 pixels)
     int opt_dla_front = 1;  // 1: DLA-34 base_layer + level0 + level1 (+ pool) as ONE kernel (dla_front.cu); 0: layer by layer
     int opt_workspace_fill = -1;  // >= 0: byte the whole arena is filled with at dd3d_plan (poison test)
     std::vector<cudaEvent_t> prof_ev;

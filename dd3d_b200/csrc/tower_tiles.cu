@@ -1,11 +1,13 @@
-// Tile lists of the sparse box3d tower (TowerTilesParams, b3d_sparse.cuh).
+// Tile lists of the sparse box3d and box2d towers (TowerTilesParams, b3d_sparse.cuh).
 //
-// One CTA per (level, image).  Every final candidate of the decode's `fin` list lowers, by a shared-memory atomicMin (order
-// free, so deterministic), the Chebyshev distance of the conv tiles around it: the distance from the candidate pixel to the
-// part of the tile inside the map.  Tower layer i of `depth` is needed at the candidates dilated by depth - i pixels, so its
-// list holds the tiles with distance <= depth - i, in row-major order, written to the (level, image) region of the staging
-// area.  The last CTA to finish (atomic ticket, no waiting) concatenates the regions level-major, then image -- a fixed order,
-// so the lists and the conv schedule do not depend on timing -- writes the counts and resets the ticket.
+// One CTA per (level, image).  Every seed pixel lowers, by an atomicMin (order free, so deterministic), the Chebyshev
+// distance of the conv tiles around it: the distance from the seed pixel to the part of the tile inside the map.  The box3d
+// tower's seeds are the final candidates of the decode's `fin` list, read by the CTA itself into shared memory; the box2d
+// tower's are the pixels of P, marked by tower_mark_kernel (one thread per head pixel) in the global `dist` array, which the
+// CTA copies and resets.  List i holds the tiles with distance <= reach - i, in row-major order, written to the (level,
+// image) region of the staging area.  The last CTA to finish (atomic ticket, no waiting) concatenates the regions
+// level-major, then image -- a fixed order, so the lists and the conv schedule do not depend on timing -- writes the counts
+// and resets the ticket.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -47,6 +49,44 @@ __device__ __forceinline__ uint32_t tile_entry(int l, int b, int tile) {
     return (static_cast<uint32_t>(l) << 29) | (static_cast<uint32_t>(b) << 16) | static_cast<uint32_t>(tile);
 }
 
+// seed pixel (py, px): lower the distance of every tile within `reach` of it (dist: shared or global, [tiles_y][tiles_x])
+__device__ __forceinline__ void seed_tiles(int* dist, const TowerTilesLevel& L, int py, int px, int reach) {
+    const int ty0 = max(py - reach, 0) / L.th, ty1 = min(py + reach, L.H - 1) / L.th;
+    const int tx0 = max(px - reach, 0) / L.tw, tx1 = min(px + reach, L.W - 1) / L.tw;
+    for (int ty = ty0; ty <= ty1; ++ty) {
+        const int y0 = ty * L.th, y1 = min(y0 + L.th, L.H) - 1;
+        const int dy = py < y0 ? y0 - py : (py > y1 ? py - y1 : 0);
+        for (int tx = tx0; tx <= tx1; ++tx) {
+            const int x0 = tx * L.tw, x1 = min(x0 + L.tw, L.W) - 1;
+            const int dx = px < x0 ? x0 - px : (px > x1 ? px - x1 : 0);
+            atomicMin(&dist[ty * L.tiles_x + tx], max(dy, dx));
+        }
+    }
+}
+
+// (level, image) region of a layer's staging / list area, and of `dist`
+__device__ __forceinline__ size_t region(const TowerTilesLevel& L, int b) {
+    const int T = L.tiles_x * L.tiles_y;
+    return L.stage_begin + static_cast<size_t>(b) * (T + (T & 1));
+}
+
+// One thread per head pixel, the grid of the decode's dense passes: the pixels of P seed the tiles around them.
+constexpr int kMarkThreads = kTowerMarkThreads;
+__global__ void __launch_bounds__(kMarkThreads) tower_mark_kernel(const __grid_constant__ TowerTilesParams p) {
+    DD3D_PDL_PROLOGUE();
+    int l = 0;
+#pragma unroll
+    for (int i = 1; i < kLevels; ++i)
+        if (static_cast<int>(blockIdx.x) >= p.lvl[i].mark_begin) l = i;
+    const TowerTilesLevel& L = p.lvl[l];
+    const int b = blockIdx.y;
+    const int pix = (static_cast<int>(blockIdx.x) - L.mark_begin) * kMarkThreads + static_cast<int>(threadIdx.x);
+    const int hw = L.H * L.W;
+    if (pix >= hw || !class_passes(L.cls + (static_cast<size_t>(b) * hw + pix) * p.cls_pitch, p.C, p.thresh)) return;
+    const int py = pix / L.W;
+    seed_tiles(p.dist + region(L, b), L, py, pix - py * L.W, p.reach);
+}
+
 __global__ void __launch_bounds__(kThreads) tower_tiles_kernel(const TowerTilesParams p) {
     DD3D_PDL_PROLOGUE();
     extern __shared__ int s_dist[];  // [max_tiles]
@@ -60,34 +100,32 @@ __global__ void __launch_bounds__(kThreads) tower_tiles_kernel(const TowerTilesP
     const TowerTilesLevel& L = p.lvl[l];
     const int T = L.tiles_x * L.tiles_y;
     const int D = p.depth;
-    for (int t = threadIdx.x; t < T; t += kThreads) s_dist[t] = 1 << 30;
-    __syncthreads();
-    const int bl = b * kLevels + l;  // fin / cand_count order
-    const int n = min(p.cand_count[bl], p.topk);
-    for (int c = threadIdx.x; c < n; c += kThreads) {
-        const int pix = static_cast<int>(p.fin[static_cast<size_t>(bl) * p.topk + c].y / static_cast<uint32_t>(p.C));
-        const int py = pix / L.W, px = pix - py * L.W;
-        const int ty0 = max(py - D, 0) / L.th, ty1 = min(py + D, L.H - 1) / L.th;
-        const int tx0 = max(px - D, 0) / L.tw, tx1 = min(px + D, L.W - 1) / L.tw;
-        for (int ty = ty0; ty <= ty1; ++ty) {
-            const int y0 = ty * L.th, y1 = min(y0 + L.th, L.H) - 1;
-            const int dy = py < y0 ? y0 - py : (py > y1 ? py - y1 : 0);
-            for (int tx = tx0; tx <= tx1; ++tx) {
-                const int x0 = tx * L.tw, x1 = min(x0 + L.tw, L.W) - 1;
-                const int dx = px < x0 ? x0 - px : (px > x1 ? px - x1 : 0);
-                atomicMin(&s_dist[ty * L.tiles_x + tx], max(dy, dx));
-            }
+    if (p.fin != nullptr) {
+        for (int t = threadIdx.x; t < T; t += kThreads) s_dist[t] = kTowerTileFar;
+        __syncthreads();
+        const int bl = b * kLevels + l;  // fin / cand_count order
+        const int n = min(p.cand_count[bl], p.topk);
+        for (int c = threadIdx.x; c < n; c += kThreads) {
+            const int pix = static_cast<int>(p.fin[static_cast<size_t>(bl) * p.topk + c].y / static_cast<uint32_t>(p.C));
+            const int py = pix / L.W;
+            seed_tiles(s_dist, L, py, pix - py * L.W, p.reach);
+        }
+    } else {
+        int* dist = p.dist + region(L, b);
+        for (int t = threadIdx.x; t < T; t += kThreads) {
+            s_dist[t] = __ldcg(dist + t);
+            dist[t] = kTowerTileFar;  // ready for the next forward's mark pass
         }
     }
     __syncthreads();
 
-    uint32_t* stage = p.stage + L.stage_begin + static_cast<size_t>(b) * (T + (T & 1));
+    uint32_t* stage = p.stage + region(L, b);
     for (int i = 0; i < D; ++i) {
         if (threadIdx.x == 0) s_pix = 0;
         int written = 0;
         for (int base = 0; base < T; base += kThreads) {
             const int t = base + threadIdx.x;
-            const bool on = t < T && s_dist[t] <= D - i;
+            const bool on = t < T && s_dist[t] <= p.reach - i;
             int total;
             const int at = written + block_exclusive_scan(on ? 1 : 0, s_warp, &total);
             if (on) {
@@ -165,8 +203,16 @@ __global__ void __launch_bounds__(kThreads) tower_tiles_kernel(const TowerTilesP
 
 size_t tower_tiles_smem_bytes(int max_tiles) { return static_cast<size_t>(max_tiles) * 4; }
 
+cudaError_t launch_tower_mark(const TowerTilesParams& p, cudaStream_t stream) {
+    if (p.dist == nullptr || p.fin != nullptr || p.B < 1 || p.C < 1 || p.cls_pitch < p.C || p.cls_pitch % 4 ||
+        p.mark_blocks < 1 || p.reach < 0)
+        return cudaErrorInvalidValue;
+    return launch_pdl(tower_mark_kernel, dim3(p.mark_blocks, p.B), dim3(kMarkThreads), 0, stream, p);
+}
+
 cudaError_t launch_tower_tiles(const TowerTilesParams& p, cudaStream_t stream) {
-    if (p.depth < 1 || p.B < 1 || p.B > kTileListMaxImages || p.topk < 1 || p.C < 1 || p.max_tiles >= kTileListMaxTiles ||
+    if (p.depth < 1 || p.reach < p.depth - 1 || p.B < 1 || p.B > kTileListMaxImages || p.C < 1 ||
+        (p.fin != nullptr ? p.topk < 1 : p.dist == nullptr) || p.max_tiles >= kTileListMaxTiles ||
         tower_tiles_smem_bytes(p.max_tiles) > 48 * 1024)
         return cudaErrorInvalidValue;
     return launch_pdl(tower_tiles_kernel, dim3(kLevels * p.B), dim3(kThreads), tower_tiles_smem_bytes(p.max_tiles), stream, p);

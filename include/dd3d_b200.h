@@ -196,7 +196,13 @@ int dd3d_overflow_flags(dd3d_handle h, dd3d_stream stream, int32_t* h_flags);
  * it drops the engine's plans), "sparse_tower" (2 = auto, the default: with the sparse predictor, a non-GN box3d tower on
  * pair-tile convs and >= 50 000 head pixels per image, the tower runs after the threshold / top-k on the conv tiles the
  * predictor's reads need -- bit-identical detections, the "op<i>" outputs of the tower hold stale values elsewhere; 1: whenever
- * the sparse predictor runs and the tower qualifies; 0: dense tower; changing it drops the engine's plans), "dla_front" (default 1: DLA-34 base_layer + level0 + level1 + pool run as one kernel; 0: layer by layer; flipping it
+ * the sparse predictor runs and the tower qualifies; 0: dense tower; changing it drops the engine's plans),
+ * "sparse_box2d_tower" (2 = auto, the default: with the sparse box3d predictor, a non-GN FCOS2D head whose box2d tower runs
+ * on pair-tile convs and >= 50 000 head pixels per image, the box2d tower and its [box2d_reg | centerness] predictor run
+ * only on the conv tiles around the pixels where some class score passes PRE_NMS_THRESH -- bit-identical detections;
+ * "box0".."box4" of dd3d_get_tensor then refuse (the map is stale elsewhere) and the "op<i>" outputs of that tower hold
+ * stale values; 1: whenever the head qualifies; 0: dense; environment DD3D_SPARSE_BOX2D_TOWER; changing it drops the
+ * engine's plans), "dla_front" (default 1: DLA-34 base_layer + level0 + level1 + pool run as one kernel; 0: layer by layer; flipping it
  * drops the engine's plans), "workspace_reuse" (default 1: activation buffers with disjoint lifetimes share workspace memory --
  * after a forward only "input", "p0".."p4" and the head maps of dd3d_get_tensor are intact; 0: every op output keeps its own
  * memory, for stage-level tests; applies to plans made afterwards), and "workspace_fill" (0..255: dd3d_plan fills the whole workspace with that byte first, -1 = off;
@@ -305,6 +311,14 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
 int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
                          const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch, const uint32_t* d_tiles,
                          const int32_t* d_count, dd3d_stream stream);
+/* dd3d_op_conv2d_taps_tiles: the 3x3 stride-1 conv of dd3d_op_conv2d with cout <= 16 on the taps-in-N kernel in work-list
+ * mode, the form the engine runs the sparse box2d tower's predictor in: only the 16x8 output tiles listed in d_tiles are
+ * computed (entries as in dd3d_op_conv2d_tiles, one work item each, the out-of-image tile writes nothing), every other output
+ * pixel is left untouched.  d_scale / d_bias: fp32 [16]; out: fp32 (out_f32, out_pitch a multiple of 4) or 16-bit (a
+ * multiple of 8), 16 channels written per pixel.  d_count: device int32, the number of entries, read by the kernel. */
+int dd3d_op_conv2d_taps_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
+                              const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch, int out_f32,
+                              const uint32_t* d_tiles, const int32_t* d_count, dd3d_stream stream);
 /* dd3d_op_b3d_sparse: the sparse FCOS3D box3d predictor (csrc/b3d_sparse.cu) on caller buffers: for every (image b, level l)
  * and slot s < min(d_counts[b * 5 + l], topk), row (b * 5 + l) * topk + s of d_rows (fp32, out_pitch floats per row) receives
  * the 3x3 conv of level l's tower output at the candidate's pixel, channels 0 .. n_pad-1, times d_scale[l] plus d_bias[l]
