@@ -18,7 +18,7 @@ def _conv(specs, name, cout, cin, k, bias=False, role="relu"):
         specs[name + ".bias"] = ((cout, ), "bias:" + role)
 
 
-def _bn(specs, name, c, frozen=True):
+def _bn(specs, name, c, frozen):
     specs[name + ".weight"] = ((c, ), "bn_w")
     specs[name + ".bias"] = ((c, ), "bn_b")
     specs[name + ".running_mean"] = ((c, ), "bn_mean")
@@ -32,6 +32,8 @@ def _norm(specs, name, c, norm):
     num_batches_tracked, FrozenBatchNorm2d does not, GroupNorm(32, c) has an affine only; "" adds nothing.  Any other
     string raises KeyError like get_norm's dict lookup."""
     kind = {"BN": "bn", "SyncBN": "bn", "FrozenBN": "frozen", "GN": "gn", "": None}[norm]
+    if kind == "gn" and c % 32:  # nn.GroupNorm(32, c)
+        raise ValueError(f"num_channels ({c}) must be divisible by num_groups (32)")
     if kind == "gn":
         specs[name + ".weight"] = ((c, ), "gn_w")
         specs[name + ".bias"] = ((c, ), "gn_b")
@@ -39,38 +41,39 @@ def _norm(specs, name, c, norm):
         _bn(specs, name, c, frozen=kind == "frozen")
 
 
-def _conv_bn(specs, name, cout, cin, k, role="relu"):
-    _conv(specs, name, cout, cin, k, role=role)
-    _bn(specs, name + ".norm", cout)
+def _conv_bn(specs, name, cout, cin, k, role="relu", norm="FrozenBN"):
+    """DLA-34 Conv2d(bias=norm == "") -> get_norm(norm) (dla.py:33,44,154,230,277,337)."""
+    _conv(specs, name, cout, cin, k, bias=norm == "", role=role)
+    _norm(specs, name + ".norm", cout, norm)
 
 
-def _dla_tree(specs, p, levels, in_ch, out_ch, level_root, root_dim=0):
+def _dla_tree(specs, p, levels, in_ch, out_ch, level_root, root_dim=0, norm="FrozenBN"):
     if root_dim == 0:
         root_dim = 2 * out_ch
     if level_root:
         root_dim += in_ch
     if levels == 1:
         for t, cin in (("tree1", in_ch), ("tree2", out_ch)):
-            _conv_bn(specs, f"{p}.{t}.conv1", out_ch, cin, 3)
-            _conv_bn(specs, f"{p}.{t}.conv2", out_ch, out_ch, 3, role="linear")
-        _conv_bn(specs, f"{p}.root.conv", out_ch, root_dim, 1)
+            _conv_bn(specs, f"{p}.{t}.conv1", out_ch, cin, 3, norm=norm)
+            _conv_bn(specs, f"{p}.{t}.conv2", out_ch, out_ch, 3, role="linear", norm=norm)
+        _conv_bn(specs, f"{p}.root.conv", out_ch, root_dim, 1, norm=norm)
         if in_ch != out_ch:
-            _conv_bn(specs, f"{p}.project", out_ch, in_ch, 1, role="linear")
+            _conv_bn(specs, f"{p}.project", out_ch, in_ch, 1, role="linear", norm=norm)
     else:
-        _dla_tree(specs, p + ".tree1", levels - 1, in_ch, out_ch, False)
-        _dla_tree(specs, p + ".tree2", levels - 1, out_ch, out_ch, False, root_dim=root_dim + out_ch)
+        _dla_tree(specs, p + ".tree1", levels - 1, in_ch, out_ch, False, norm=norm)
+        _dla_tree(specs, p + ".tree2", levels - 1, out_ch, out_ch, False, root_dim=root_dim + out_ch, norm=norm)
 
 
-def _dla34(specs):
+def _dla34(specs, norm):
     p = "backbone.bottom_up"
     ch = [16, 32, 64, 128, 256, 512]
     levels = [1, 1, 1, 2, 2, 1]
-    _conv_bn(specs, p + ".base_layer", ch[0], 3, 7)
-    _conv_bn(specs, p + ".level0.0", ch[0], ch[0], 3)
-    _conv_bn(specs, p + ".level1.0", ch[1], ch[0], 3)
-    _dla_tree(specs, p + ".level2", levels[2], ch[1], ch[2], False)
+    _conv_bn(specs, p + ".base_layer", ch[0], 3, 7, norm=norm)
+    _conv_bn(specs, p + ".level0.0", ch[0], ch[0], 3, norm=norm)
+    _conv_bn(specs, p + ".level1.0", ch[1], ch[0], 3, norm=norm)
+    _dla_tree(specs, p + ".level2", levels[2], ch[1], ch[2], False, norm=norm)
     for lvl in (3, 4, 5):
-        _dla_tree(specs, p + f".level{lvl}", levels[lvl], ch[lvl - 1], ch[lvl], True)
+        _dla_tree(specs, p + f".level{lvl}", levels[lvl], ch[lvl - 1], ch[lvl], True, norm=norm)
     return {"level3": 128, "level4": 256, "level5": 512}
 
 
@@ -94,24 +97,25 @@ VOVNET_KEYS = {spec[0]: key for key, spec in VOVNET_SPECS.items()}  # FE.BACKBON
 ARCH_KEYS = ("dla34", ) + tuple(VOVNET_SPECS)
 
 
-def _vov_conv3x3(specs, n, cout, cin, dw):
+def _vov_conv3x3(specs, n, cout, cin, dw, norm):
     """conv3x3 (vovnet.py:124-143) or dw_conv3x3 (vovnet.py:100-121; the reference builds it only with cin == cout)."""
     if dw:
         specs[f"{n}/dw_conv3x3.weight"] = ((cout, 1, 3, 3), "conv:dw")
         _conv(specs, f"{n}/pw_conv1x1", cout, cin, 1)
-        _bn(specs, f"{n}/pw_norm", cout)
+        _norm(specs, f"{n}/pw_norm", cout, norm)
     else:
         _conv(specs, f"{n}/conv", cout, cin, 3)
-        _bn(specs, f"{n}/norm", cout)
+        _norm(specs, f"{n}/norm", cout, norm)
 
 
-def _vovnet(specs, arch):
+def _vovnet(specs, arch, norm):
+    """The VoVNet convs never have a bias; every one is followed by get_norm(norm) (vovnet.py:100-159,286-287)."""
     p = "backbone.bottom_up"
     _, stem, stage_ch, out_ch, nl, blocks, dw = VOVNET_SPECS[arch]
     _conv(specs, f"{p}.stem.stem_1/conv", stem[0], 3, 3)
-    _bn(specs, f"{p}.stem.stem_1/norm", stem[0])
-    _vov_conv3x3(specs, f"{p}.stem.stem_2", stem[1], stem[0], dw)
-    _vov_conv3x3(specs, f"{p}.stem.stem_3", stem[2], stem[1], dw)
+    _norm(specs, f"{p}.stem.stem_1/norm", stem[0], norm)
+    _vov_conv3x3(specs, f"{p}.stem.stem_2", stem[1], stem[0], dw, norm)
+    _vov_conv3x3(specs, f"{p}.stem.stem_3", stem[2], stem[1], dw, norm)
     in_ch = stem[2]
     for si, (sc, oc, nb) in enumerate(zip(stage_ch, out_ch, blocks), start=2):
         for b in range(nb):
@@ -121,13 +125,13 @@ def _vovnet(specs, arch):
             if dw and in_ch != sc:  # conv_reduction (vovnet.py:200-205)
                 r = f"{q}.conv_reduction.{name}_reduction_0"
                 _conv(specs, f"{r}/conv", sc, in_ch, 1)
-                _bn(specs, f"{r}/norm", sc)
+                _norm(specs, f"{r}/norm", sc, norm)
                 cin = sc
             for i in range(nl):
-                _vov_conv3x3(specs, f"{q}.layers.{i}.{name}_{i}", sc, cin, dw)
+                _vov_conv3x3(specs, f"{q}.layers.{i}.{name}_{i}", sc, cin, dw, norm)
                 cin = sc
             _conv(specs, f"{q}.concat.{name}_concat/conv", oc, in_ch + nl * sc, 1)
-            _bn(specs, f"{q}.concat.{name}_concat/norm", oc)
+            _norm(specs, f"{q}.concat.{name}_concat/norm", oc, norm)
             _conv(specs, f"{q}.ese.fc", oc, oc, 1, bias=True, role="ese")
             in_ch = oc
     return {f"stage{si}": oc for si, oc in enumerate(out_ch, start=2)}
@@ -139,11 +143,12 @@ def param_specs(cfg):
     specs["pixel_mean"] = ((3, 1, 1), "buffer")
     specs["pixel_std"] = ((3, 1, 1), "buffer")
     arch = arch_of(cfg)
+    norm = backbone_norm(cfg)
     if arch == "dla34":
-        feats = _dla34(specs)
+        feats = _dla34(specs, norm)
         stages = {"level3": 3, "level4": 4, "level5": 5}
     else:
-        feats = _vovnet(specs, arch)
+        feats = _vovnet(specs, arch, norm)
         stages = {"stage2": 2, "stage3": 3, "stage4": 4, "stage5": 5}
     fpn_norm = cfg.FE.FPN.NORM  # detectron2 FPN: bias only without a norm; one norm per conv
     for name, ch in feats.items():
@@ -225,6 +230,19 @@ def arch_of(cfg):
     if b == "build_fcos_vovnet_fpn_backbone_p6":
         return VOVNET_KEYS[cfg.FE.BACKBONE.NAME]  # KeyError for an unknown name, like _STAGE_SPECS[cfg.NAME]
     raise KeyError("No object named '{}' found in 'BACKBONE' registry!".format(b))
+
+
+def backbone_norm(cfg):
+    """FE.BACKBONE.NORM, with the errors the reference raises for the combinations it cannot build or run: an unknown string
+    (KeyError, get_norm's lookup), GN on channel counts that 32 does not divide (ValueError from nn.GroupNorm: DLA-34's 16, the
+    slim VoVNets' 112; raised by _norm while the inventory is built) and a VoVNet without a norm.  The reference raises the
+    last one only at its first forward, where nn.Sequential calls the None norm (vovnet.py:119,139,159); the mirror raises it
+    at construction."""
+    norm = cfg.FE.BACKBONE.NORM
+    _norm({}, "", 32, norm)  # KeyError for an unknown NORM
+    if norm == "" and arch_of(cfg) != "dla34":
+        raise TypeError("'NoneType' object is not callable")
+    return norm
 
 
 def level_strides(cfg):

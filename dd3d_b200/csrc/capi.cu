@@ -82,6 +82,10 @@ int dd3d_set_layout(dd3d_handle h, const dd3d_layout_desc* layout) {
     return guarded(h, [&](Engine& e) { e.set_layout(*layout); });
 }
 
+int dd3d_set_backbone_norm(dd3d_handle h, int32_t norm) {
+    return guarded(h, [&](Engine& e) { e.set_backbone_norm(norm); });
+}
+
 int dd3d_load_weight(dd3d_handle h, const char* name, const float* data, const int64_t* shape, int ndim) {
     if (name == nullptr || data == nullptr || (ndim > 0 && shape == nullptr) || ndim < 0 || ndim > 8)
         return DD3D_ERR_INVALID;
@@ -638,6 +642,31 @@ int dd3d_op_group_norm(const void* d_in, int B, int H, int W, int in_pitch, cons
         g.res_H = (H + 1) / 2;
         g.res_W = (W + 1) / 2;
     }
+    g.part = static_cast<float2*>(d_scratch);
+    const cudaError_t e = launch_group_norm(p, static_cast<cudaStream_t>(stream));
+    return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
+}
+
+int dd3d_op_group_norm_c(const void* d_in, int B, int H, int W, int C, int in_c0, int in_pitch, const float* d_gamma,
+                         const float* d_beta, int relu, void* d_out, int out_c0, int out_pitch, void* d_scratch, dd3d_stream stream) {
+    if (!d_in || !d_out || !d_gamma || !d_beta || !d_scratch) return DD3D_ERR_INVALID;
+    if (B < 1 || H < 1 || W < 1 || in_c0 < 0 || out_c0 < 0 || in_c0 % 8 || out_c0 % 8) return DD3D_ERR_INVALID;
+    if (in_c0 + C > in_pitch || out_c0 + C > out_pitch) return DD3D_ERR_INVALID;
+    GroupNormParams p;
+    p.nseg = 1;
+    p.B = B;
+    p.C = C;
+    p.gamma = d_gamma;
+    p.beta = d_beta;
+    p.relu = relu ? 1 : 0;
+    p.fp16 = g_op_fp16;
+    GroupNormSeg& g = p.seg[0];
+    g.in = static_cast<const __nv_bfloat16*>(d_in) + in_c0;
+    g.out = static_cast<__nv_bfloat16*>(d_out) + out_c0;
+    g.H = H;
+    g.W = W;
+    g.in_pitch = in_pitch;
+    g.out_pitch = out_pitch;
     g.part = static_cast<float2*>(d_scratch);
     const cudaError_t e = launch_group_norm(p, static_cast<cudaStream_t>(stream));
     return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);

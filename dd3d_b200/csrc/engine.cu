@@ -183,14 +183,31 @@ void Engine::set_layout(const dd3d_layout_desc& l) {
     layout = l;
 }
 
+void Engine::set_backbone_norm(int norm) {
+    if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_backbone_norm after finalize");
+    if (norm < DD3D_NORM_BN_PER_LEVEL || norm > DD3D_NORM_NONE) fail(DD3D_ERR_INVALID, "unknown dd3d_norm value");
+    const bool dla = desc.arch == DD3D_ARCH_DLA34;
+    // DLA-34's 16-channel convs cannot take GroupNorm(32, C); a VoVNet without a norm fails in the reference's forward
+    if (dla && norm == DD3D_NORM_GN) fail(DD3D_ERR_INVALID, "DLA-34 has no GroupNorm backbone (16 channels)");
+    if (!dla && norm == DD3D_NORM_NONE) fail(DD3D_ERR_INVALID, "a VoVNet backbone needs a norm");
+    if (!dla && norm == DD3D_NORM_GN) {  // GroupNorm(32, C) of every stem, OSA, concat and reduction conv
+        const VovSpec& S = *vovnet_spec(desc.arch);
+        bool ok = true;
+        for (int i = 0; i < 4; ++i) ok = ok && group_norm_channels_ok(S.stage_ch[i]) && group_norm_channels_ok(S.out_ch[i]);
+        for (int i = 0; i < 3; ++i) ok = ok && group_norm_channels_ok(S.stem[i]);
+        if (!ok) fail(DD3D_ERR_INVALID, "GroupNorm(32, C) needs channel counts 32 divides (slim VoVNets have 112)");
+    }
+    backbone_norm = norm;
+}
+
 // GroupNorm(32, C) affine of `<prefix>.weight` / `<prefix>.bias`, uploaded as fp32 vectors (cached like the epilogues)
-const Epilogue& Engine::gn_affine(const std::string& prefix) {
+const Epilogue& Engine::gn_affine(const std::string& prefix, int C) {
     const std::string key = "gn|" + prefix;
     auto it = epis.find(key);
     if (it != epis.end()) return it->second;
     const HostTensor& g = weight(prefix + ".weight");
     const HostTensor& b = weight(prefix + ".bias");
-    if (g.data.size() != static_cast<size_t>(kGnChannels) || b.data.size() != static_cast<size_t>(kGnChannels))
+    if (g.data.size() != static_cast<size_t>(C) || b.data.size() != static_cast<size_t>(C))
         fail(DD3D_ERR_INVALID, "bad GroupNorm shape: " + prefix);
     return epilogue(key, g.data, b.data, nullptr);
 }
@@ -488,8 +505,9 @@ struct Builder {
         p.relu = relu ? 1 : 0;
         p.avg = avg ? 1 : 0;
         p.fp16 = E->fp16;
+        p.C = x[0].C;
         for (size_t s = 0; s < x.size(); ++s) {
-            if (x[s].C != kGnChannels) fail(DD3D_ERR_INVALID, "GroupNorm needs 256 channels");
+            if (x[s].C != p.C || !group_norm_channels_ok(p.C)) fail(DD3D_ERR_INVALID, "GroupNorm channel count");
             GroupNormSeg& g = p.seg[s];
             g.in = x[s].ptr;
             g.out = x[s].ptr;
@@ -504,7 +522,7 @@ struct Builder {
             }
             g.part = reinterpret_cast<float2*>(part[s]);
             op.outs[s] = x[s];
-            const double px = static_cast<double>(B) * x[s].H * x[s].W * kGnChannels * 2;
+            const double px = static_cast<double>(B) * x[s].H * x[s].W * p.C * 2;
             op.bytes += px * (affine ? 3 : 2) + (res ? px / 4 : 0.0);  // stats read, apply read + write, residual read
         }
         op.nouts = p.nseg;
@@ -540,12 +558,22 @@ struct Builder {
     }
 
     // ---- DLA-34 -------------------------------------------------------------------------------------------
+    // DLA-34 conv -> norm: the folded BN, or with FE.BACKBONE.NORM "" the conv's own bias (Conv2d(bias=norm == ""), dla.py:33,44,
+    // 154,230,277,337).  Returns the (BN prefix, bias name) pair bn_fold takes.
+    std::pair<std::string, std::string> dla_norm(const std::string& conv) const {
+        if (E->backbone_norm == DD3D_NORM_NONE) return {"", conv + ".bias"};
+        return {conv + ".norm", ""};
+    }
+    void dla_conv(const std::string& name, View in, View out, int ksize, int stride, bool relu, const View* res = nullptr) {
+        const auto nb = dla_norm(name);
+        conv1(name, nb.first, !nb.second.empty(), in, out, ksize, stride, relu, res);
+    }
     // BasicBlock (dla.py:24-62): conv1 -> BN -> ReLU -> conv2 -> BN -> (+residual) -> ReLU
     void dla_block(const std::string& p, View x, int stride, View residual, View dst) {
         const int Ho = x.H / stride, Wo = x.W / stride;
         View t = alloc(Ho, Wo, dst.C);
-        conv1(p + ".conv1", p + ".conv1.norm", false, x, t, 3, stride, true);
-        conv1(p + ".conv2", p + ".conv2.norm", false, t, dst, 3, 1, true, &residual);
+        dla_conv(p + ".conv1", x, t, 3, stride, true);
+        dla_conv(p + ".conv2", t, dst, 3, 1, true, &residual);
     }
     // Tree with levels == 1 (dla.py:170-247): `rc` is the Root's concat buffer, laid out [x2 | x1 | children...]
     // with the children already in place; `bottom` is the (pooled) input the optional `project` acts on.
@@ -553,13 +581,13 @@ struct Builder {
         View residual = bottom;
         if (in_ch != out_ch) {
             residual = alloc(bottom.H, bottom.W, out_ch);
-            conv1(p + ".project", p + ".project.norm", false, bottom, residual, 1, 1, false);
+            dla_conv(p + ".project", bottom, residual, 1, 1, false);
         }
         View x1 = slice(rc, out_ch, out_ch);
         View x2 = slice(rc, 0, out_ch);
         dla_block(p + ".tree1", x, stride, residual, x1);
         dla_block(p + ".tree2", x1, 1, x1, x2);
-        conv1(p + ".root.conv", p + ".root.conv.norm", false, rc, dst, 1, 1, true);  // Root: cat -> 1x1 -> BN -> ReLU
+        dla_conv(p + ".root.conv", rc, dst, 1, 1, true);  // Root: cat -> 1x1 -> BN -> ReLU
     }
     // Tree with levels == 2 and level_root (level3 / level4, dla.py:309-314)
     View dla_tree2(const std::string& p, View x, int in_ch, int out_ch) {
@@ -581,11 +609,12 @@ struct Builder {
         // both forms of the front end are packed at finalize (host weights are dropped afterwards), so that the
         // "dla_front" option can be flipped on a finalized engine
         const FrontLayer& F = E->front_layer(p);
-        E->stem_layer(p + ".base_layer", p + ".base_layer.norm", 7, 1);
+        const auto n0 = dla_norm(p + ".base_layer"), n1 = dla_norm(p + ".level0.0"), n2 = dla_norm(p + ".level1.0");
+        E->stem_layer(p + ".base_layer", n0.first, n0.second, 7, 1);
         E->conv_layer(p + ".level0.0", {p + ".level0.0"}, 16, 3);
-        E->bn_epilogue(p + ".level0.0|" + p + ".level0.0.norm", p + ".level0.0.norm", "", 16);
+        E->bn_epilogue(p + ".level0.0|" + n1.first, n1.first, n1.second, 16);
         E->conv_layer(p + ".level1.0", {p + ".level1.0"}, 16, 3);
-        E->bn_epilogue(p + ".level1.0|" + p + ".level1.0.norm", p + ".level1.0.norm", "", 32);
+        E->bn_epilogue(p + ".level1.0|" + n2.first, n2.first, n2.second, 32);
         View a2, bottom;
         if (E->opt_dla_front && H % 4 == 0 && W % 4 == 0) {
             // base_layer -> level0 -> level1 -> 2x2 max-pool in one kernel (dla_front.cu); the two full-resolution
@@ -595,11 +624,11 @@ struct Builder {
             front(F, input, a2, bottom);
         } else {
             View a0 = alloc(H, W, 16);
-            stem(p + ".base_layer", p + ".base_layer.norm", input, a0, 7, 1);
+            stem(p + ".base_layer", n0.first, n0.second, input, a0, 7, 1);
             View a1 = alloc(H, W, 16);
-            conv1(p + ".level0.0", p + ".level0.0.norm", false, a0, a1, 3, 1, true);
+            dla_conv(p + ".level0.0", a0, a1, 3, 1, true);
             a2 = alloc(H / 2, W / 2, 32);
-            conv1(p + ".level1.0", p + ".level1.0.norm", false, a1, a2, 3, 2, true);
+            dla_conv(p + ".level1.0", a1, a2, 3, 2, true);
             bottom = alloc(H / 4, W / 4, 32);
             maxpool(a2, bottom, 2);
         }
@@ -638,8 +667,9 @@ struct Builder {
         P->ops.push_back(op);
     }
 
-    void stem(const std::string& wname, const std::string& bn, View in4, View out, int ksize, int stride) {
-        const StemLayer& S = E->stem_layer(wname, bn, ksize, stride);
+    void stem(const std::string& wname, const std::string& bn, const std::string& bias, View in4, View out, int ksize, int stride,
+              bool relu = true) {
+        const StemLayer& S = E->stem_layer(wname, bn, bias, ksize, stride, relu);
         touch(out);
         ++op_idx;
         if (dry) return;
@@ -683,12 +713,23 @@ struct Builder {
     // pw_norm -> ReLU (dw_conv3x3, vovnet.py:100-121) through a depthwise output buffer
     void vov_conv3x3(const std::string& n, View in, View out, int stride, bool dw) {
         if (!dw) {
-            conv1(n + "/conv", n + "/norm", false, in, out, 3, stride, true);
+            vov_conv_norm(n + "/conv", n + "/norm", in, out, 3, stride);
             return;
         }
         View t = alloc(out.H, out.W, in.C);
         dwconv(n + "/dw_conv3x3", in, t, stride);
-        conv1(n + "/pw_conv1x1", n + "/pw_norm", false, t, out, 1, 1, true);
+        vov_conv_norm(n + "/pw_conv1x1", n + "/pw_norm", t, out, 1, 1);
+    }
+    // VoVNet conv -> norm -> ReLU (get_norm(cfg.NORM), vovnet.py:119,139,159): the BN folded into the conv epilogue, or for GN
+    // the raw conv output stored (a channel slice of the concat buffer for the OSA layers), then GroupNorm + ReLU in place on
+    // it.  One GN op per conv: every VoVNet conv reads the previous one's normalised output, so none can share a launch.
+    void vov_conv_norm(const std::string& conv, const std::string& norm, View in, View out, int ksize, int stride) {
+        if (E->backbone_norm != DD3D_NORM_GN) {
+            conv1(conv, norm, false, in, out, ksize, stride, true);
+            return;
+        }
+        conv1(conv, "", false, in, out, ksize, stride, false);
+        group_norm({out}, &E->gn_affine(norm, out.C), true, nullptr, false);
     }
 
     void build_vovnet(const VovSpec& S, View input, std::vector<View>* feats) {
@@ -699,7 +740,12 @@ struct Builder {
         const int* blocks = S.blocks;
         const int nl = S.layers;
         View s1 = alloc(H / 2, W / 2, S.stem[0]);
-        stem(p + ".stem.stem_1/conv", p + ".stem.stem_1/norm", input, s1, 3, 2);
+        if (E->backbone_norm == DD3D_NORM_GN) {
+            stem(p + ".stem.stem_1/conv", "", "", input, s1, 3, 2, false);
+            group_norm({s1}, &E->gn_affine(p + ".stem.stem_1/norm", s1.C), true, nullptr, false);
+        } else {
+            stem(p + ".stem.stem_1/conv", p + ".stem.stem_1/norm", "", input, s1, 3, 2);
+        }
         View s2 = alloc(H / 2, W / 2, S.stem[1]);
         vov_conv3x3(p + ".stem.stem_2", s1, s2, 1, S.dw);
         int h = H / 4, w = W / 4;
@@ -732,7 +778,7 @@ struct Builder {
                     // conv_reduction (vovnet.py:200-205,221-222): feeds layer 0 only; the concat keeps the unreduced input
                     View r = alloc(h, w, sc);
                     const std::string rn = q + ".conv_reduction." + name + "_reduction_0";
-                    conv1(rn + "/conv", rn + "/norm", false, x, r, 1, 1, true);
+                    vov_conv_norm(rn + "/conv", rn + "/norm", x, r, 1, 1);
                     prev = r;
                 }
                 for (int i = 0; i < nl; ++i) {
@@ -743,9 +789,8 @@ struct Builder {
                     c0 += sc;
                 }
                 View xt = alloc(h, w, oc);
-                conv1(q + ".concat." + name + "_concat/conv", q + ".concat." + name + "_concat/norm", false, cat, xt, 1,
-                      1, true);
-                // eSE (always applied, vovnet.py:216,233) then identity add for non-first blocks (:235-236)
+                vov_conv_norm(q + ".concat." + name + "_concat/conv", q + ".concat." + name + "_concat/norm", cat, xt, 1, 1);
+                // eSE (always applied, vovnet.py:216,233) then identity add for non-first blocks (:235-236), after the norm
                 View dst;
                 View next_cat;
                 const bool last = (b == blocks[si] - 1);
@@ -776,10 +821,12 @@ struct Builder {
 
     void ese(const std::string& fc, View xt, const View* identity, View dst, const View* pooled = nullptr) {
         const EseLayer& L = E->ese_layer(fc, xt.C);
-        // The concat conv (the op just emitted) writes per-tile channel sums from its epilogue: [B][T][C], T = 4 * tiles
+        // The concat conv (the op just emitted) writes per-tile channel sums from its epilogue: [B][T][C], T = 4 * tiles.
+        // Behind a GroupNorm the eSE pools the normalised map itself (launch_ese): [B][ese_nsplit(HW)][C] partial sums.
+        const bool fused = E->backbone_norm != DD3D_NORM_GN;
         const int T = 4 * conv_tiles_per_image(xt.H, xt.W);
-        float* tile_partial = alloc_f32(static_cast<size_t>(B) * T * xt.C);
-        float* sums = alloc_f32(static_cast<size_t>(B) * xt.C);
+        float* tile_partial = fused ? alloc_f32(static_cast<size_t>(B) * T * xt.C) : nullptr;
+        float* sums = alloc_f32(static_cast<size_t>(B) * (fused ? 1 : ese_nsplit(xt.H * xt.W)) * xt.C);
         float* gate = alloc_f32(static_cast<size_t>(B) * xt.C);
         touch(xt);
         if (identity) touch(*identity);
@@ -787,12 +834,14 @@ struct Builder {
         if (pooled) touch(*pooled);
         ++op_idx;
         if (dry) return;
-        Op& cv = P->ops.back();
-        if (cv.type != Op::CONV || cv.conv.nseg != 1 || cv.conv.halo || cv.conv.out_mode != 0 ||
-            4 * cv.conv.seg[0].tiles_x * cv.conv.seg[0].tiles_y != T)
-            fail(DD3D_ERR_STATE, "internal: eSE must follow its concat conv");
-        cv.conv.seg[0].pool_partial = tile_partial;
-        cv.conv.seg[0].pool_pitch = xt.C;
+        if (fused) {
+            Op& cv = P->ops.back();
+            if (cv.type != Op::CONV || cv.conv.nseg != 1 || cv.conv.halo || cv.conv.out_mode != 0 ||
+                4 * cv.conv.seg[0].tiles_x * cv.conv.seg[0].tiles_y != T)
+                fail(DD3D_ERR_STATE, "internal: eSE must follow its concat conv");
+            cv.conv.seg[0].pool_partial = tile_partial;
+            cv.conv.seg[0].pool_pitch = xt.C;
+        }
         Op op;
         op.type = Op::ESE;
         op.in = xt;
@@ -1192,7 +1241,8 @@ struct Builder {
 
 // ------------------------------------------------------------------------------------------------ misc layers
 
-const StemLayer& Engine::stem_layer(const std::string& wname, const std::string& bn, int ksize, int stride) {
+const StemLayer& Engine::stem_layer(const std::string& wname, const std::string& bn, const std::string& conv_bias_name, int ksize,
+                                    int stride, bool relu) {
     auto it = stems.find(wname);
     if (it != stems.end()) return it->second;
     const HostTensor& w = weight(wname + ".weight");
@@ -1202,6 +1252,7 @@ const StemLayer& Engine::stem_layer(const std::string& wname, const std::string&
     S.ksize = ksize;
     S.stride = stride;
     S.cout = static_cast<int>(w.shape[0]);
+    S.relu = relu;
     // tensor-core stem layout: bf16 [cout][kpad], k = (ky*ksize + kx)*4 + c, zero padded (4th channel and K tail)
     const int kpad = stem_tc_kpad(ksize);
     std::vector<uint16_t> packed(static_cast<size_t>(S.cout) * kpad, 0);
@@ -1212,7 +1263,7 @@ const StemLayer& Engine::stem_layer(const std::string& wname, const std::string&
                     host_f32_to_act(w.data[(static_cast<size_t>(co) * 3 + c) * ksize * ksize + t], fp16);
     S.d_w = static_cast<__nv_bfloat16*>(dev_alloc(packed.size() * 2));
     cuda_check(cudaMemcpy(S.d_w, packed.data(), packed.size() * 2, cudaMemcpyHostToDevice), "upload stem weights");
-    S.epi = bn_epilogue(wname + "|" + bn, bn, "", S.cout);
+    S.epi = bn_epilogue(wname + "|" + bn, bn, conv_bias_name, S.cout);
     if (ksize == 3 && stride == 2 && S.cout == 64) {
         std::vector<uint16_t> pm(64 * 3 * 4 * 4, 0);
         for (int co = 0; co < 64; ++co)
@@ -1223,7 +1274,7 @@ const StemLayer& Engine::stem_layer(const std::string& wname, const std::string&
         S.d_w_mma = static_cast<__nv_bfloat16*>(dev_alloc(pm.size() * 2));
         cuda_check(cudaMemcpy(S.d_w_mma, pm.data(), pm.size() * 2, cudaMemcpyHostToDevice), "upload stem weights (mma)");
         std::vector<float> sc, bi;
-        bn_fold(bn, "", 64, &sc, &bi);
+        bn_fold(bn, conv_bias_name, 64, &sc, &bi);
         sc.insert(sc.end(), bi.begin(), bi.end());
         S.d_sb_mma = upload_f32(sc);
     }
@@ -1259,9 +1310,10 @@ const FrontLayer& Engine::front_layer(const std::string& prefix) {
         cuda_check(cudaMemcpy(d, v.data(), v.size() * 2, cudaMemcpyHostToDevice), "upload DLA front weights");
         return d;
     };
-    auto sb = [&](const std::string& bn, int cout) {
+    auto sb = [&](const std::string& conv, int cout) {  // folded BN, or the conv bias with FE.BACKBONE.NORM ""
+        const bool none = backbone_norm == DD3D_NORM_NONE;
         std::vector<float> s, b;
-        bn_fold(bn, "", cout, &s, &b);
+        bn_fold(none ? "" : conv + ".norm", none ? conv + ".bias" : "", cout, &s, &b);
         s.insert(s.end(), b.begin(), b.end());
         return upload_f32(s);
     };
@@ -1269,9 +1321,9 @@ const FrontLayer& Engine::front_layer(const std::string& prefix) {
     F.d_w0 = up16(p0);
     F.d_w1 = up16(p1);
     F.d_w2 = up16(p2);
-    F.d_sb0 = sb(prefix + ".base_layer.norm", 16);
-    F.d_sb1 = sb(prefix + ".level0.0.norm", 16);
-    F.d_sb2 = sb(prefix + ".level1.0.norm", 32);
+    F.d_sb0 = sb(prefix + ".base_layer", 16);
+    F.d_sb1 = sb(prefix + ".level0.0", 16);
+    F.d_sb2 = sb(prefix + ".level1.0", 32);
     return fronts.emplace(prefix, F).first->second;
 }
 
@@ -1664,13 +1716,13 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
             case Op::STEM:
                 if (op.stem->d_w_mma != nullptr && opt_stem_mma) {
                     cuda_check(launch_stem_s2_mma(op.in.ptr, op.stem->d_w_mma, op.stem->d_sb_mma, op.out.ptr, op.out.pitch, P.B,
-                                                  op.in.H, op.in.W, num_sms, stream, fp16),
+                                                  op.in.H, op.in.W, num_sms, stream, fp16, op.stem->relu ? 1 : 0),
                                "stem conv (mma)");
                     break;
                 }
                 cuda_check(launch_stem_tc(op.in.ptr, op.stem->d_w, op.stem->epi.d_scale, op.stem->epi.d_bias, op.out.ptr,
                                           P.B, op.in.H, op.in.W, op.ksize, op.stride, op.stem->cout, op.out.pitch, num_sms,
-                                          stream, fp16),
+                                          stream, fp16, op.stem->relu ? 1 : 0),
                            "stem conv");
                 break;
             case Op::POOL:
@@ -1679,6 +1731,15 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
                            "maxpool");
                 break;
             case Op::ESE:
+                if (op.f2 == nullptr) {  // behind a GroupNorm: pool pass over the normalised map -> fc -> scale
+                    cuda_check(launch_ese(op.in.ptr, op.in.pitch, op.ese->d_w, op.ese->d_b,
+                                          op.has_identity ? op.identity.ptr : nullptr, op.has_identity ? op.identity.pitch : 0,
+                                          op.out.ptr, op.out.pitch, op.f0, op.f1, P.B, op.in.H * op.in.W, op.in.C, num_sms,
+                                          stream, fp16, op.nouts == 2 ? op.outs[1].ptr : nullptr,
+                                          op.nouts == 2 ? op.outs[1].pitch : 0, op.in.H, op.in.W),
+                               "eSE");
+                    break;
+                }
                 cuda_check(launch_ese_fused(op.in.ptr, op.in.pitch, op.f2, op.ksize, op.ese->d_w, op.ese->d_b,
                                             op.has_identity ? op.identity.ptr : nullptr,
                                             op.has_identity ? op.identity.pitch : 0, op.out.ptr, op.out.pitch, op.f0, op.f1,
@@ -1802,7 +1863,8 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
                 break;
             case Op::ESE:
                 launches[4] += 3;
-                bytes[4] += in_px * op.in.C * 2 * (op.has_identity ? 3 : 2);  // pooling is fused into the concat conv
+                // pooling is fused into the concat conv, or behind a GroupNorm one more pass over the map
+                bytes[4] += in_px * op.in.C * 2 * ((op.has_identity ? 3 : 2) + (op.f2 == nullptr ? 1 : 0));
                 if (op.nouts == 2) bytes[4] += static_cast<double>(P.B) * op.outs[1].H * op.outs[1].W * op.in.C * 2;
                 break;
             case Op::RELU:

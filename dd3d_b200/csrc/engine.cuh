@@ -62,6 +62,7 @@ struct StemLayer {
     Epilogue epi;
     __nv_bfloat16* d_w_mma = nullptr;  // 3x3 stride-2 64-channel stem (VoVNet stem_1): [64][3][4][4] for stem_mma.cu
     float* d_sb_mma = nullptr;         // scale[64] | bias[64]
+    bool relu = true;                  // false: raw output (VoVNet stem_1 in front of its GroupNorm)
 };
 struct FrontLayer {  // DLA-34 base_layer + level0 + level1 packed for dla_front.cu
     __nv_bfloat16 *d_w0, *d_w1, *d_w2;
@@ -202,16 +203,21 @@ class Engine {
                              const std::vector<float>* lo);
     const Epilogue& bn_epilogue(const std::string& key, const std::string& bn_prefix, const std::string& conv_bias_name,
                                 int cout);
-    const StemLayer& stem_layer(const std::string& wname, const std::string& bn, int ksize, int stride);
+    const StemLayer& stem_layer(const std::string& wname, const std::string& bn, const std::string& conv_bias_name, int ksize,
+                                int stride, bool relu = true);
     const EseLayer& ese_layer(const std::string& fc, int C);
     const FrontLayer& front_layer(const std::string& prefix);
     const DwLayer& dw_layer(const std::string& wname, int C);
-    const Epilogue& gn_affine(const std::string& prefix);  // GroupNorm weight / bias as d_scale / d_bias
+    const Epilogue& gn_affine(const std::string& prefix, int C = kGnChannels);  // GroupNorm weight / bias as d_scale / d_bias
     void set_layout(const dd3d_layout_desc& l);
+    void set_backbone_norm(int norm);
 
     dd3d_model_desc desc;
     // FPN / head layout (dd3d_set_layout); the default is the shipped one
     dd3d_layout_desc layout = {DD3D_NORM_BN_PER_LEVEL, DD3D_NORM_BN_PER_LEVEL, DD3D_NORM_BN_SHARED, 4, 4, 4, 0};
+    // FE.BACKBONE.NORM (dd3d_set_backbone_norm): BN folded into the conv epilogues (default), DD3D_NORM_NONE (DLA-34: conv bias)
+    // or DD3D_NORM_GN (VoVNet: raw conv outputs, each normalised by a GroupNorm op)
+    int backbone_norm = DD3D_NORM_BN_SHARED;
     int device = 0;
     int num_sms = 132;
     int fp16 = 0;  // desc.act_dtype == DD3D_ACT_FP16: 16-bit storage of activations / weights is fp16 instead of bf16

@@ -1,18 +1,23 @@
-// GroupNorm(32, 256) on NHWC 16-bit views with a channel pitch (FCOS heads / FPN with NORM "GN": fcos2d.py:73-91,
-// fcos3d.py:82-100 get_norm("GN") = nn.GroupNorm(32, 256); detectron2 FPN with norm "GN").  Group g holds channels
-// [8g, 8g + 8): exactly one 16-byte vector per pixel, so warp lane g owns group g and a warp reads one 512-byte pixel.
+// GroupNorm(32, C) on NHWC 16-bit views with a channel pitch, C = 32 * cpg for cpg in {2, 4, 5, 6, 7, 8, 16, 24, 32}:
+// the FCOS heads / FPN with NORM "GN" (fcos2d.py:73-91, fcos3d.py:82-100 get_norm("GN") = nn.GroupNorm(32, 256); detectron2
+// FPN with norm "GN") and the VoVNet backbone with FE.BACKBONE.NORM "GN" (vovnet.py:119,139,159: 64 .. 1024 channels).
+// Thread t of a CTA owns the 16-byte vector v = t % (C / 8) of every pixel it visits (channels [8v, 8v + 8)) and visits the
+// pixels r, r + R, ... of its chunk, r = t / (C / 8), R = 256 / (C / 8).  For 256 channels (cpg 8) that is lane = group,
+// warp = pixel row: one warp reads one 512-byte pixel.  With cpg 5, 6 or 7 a vector holds the ends of two or three groups;
+// each thread then keeps one (count, mean, M2) per group it touches (a slot), fixed by v.
 //
-// Two kernels, one launch each for up to kMaxSeg maps (the five FPN levels of a tower layer):
-//   group_norm_stats_kernel  one CTA per (segment, image, chunk of kGnChunk pixels): per-lane running (count, mean, M2) with
-//                            Chan's update per pixel, then the 8 warps combined in warp order -> scratch (mean, M2) per
-//                            (chunk, group).  No E[x^2] - E[x]^2: a V2-99 p2 group holds 768k values around a non-zero mean.
+// Two kernels, one launch each for up to kMaxSeg maps of the same channel count (the five FPN levels of a tower layer):
+//   group_norm_stats_kernel  one CTA per (segment, image, chunk of kGnChunk pixels): per-thread running (count, mean, M2) per
+//                            slot with Chan's update per pixel, then per group the threads' slots combined in (row, vector)
+//                            order -> scratch (mean, M2) per (chunk, group).  No E[x^2] - E[x]^2: a V2-99 p2 group holds 768k
+//                            values around a non-zero mean.
 //   group_norm_apply_kernel  same grid; every CTA first combines the chunks of its (segment, image) in a fixed order
 //                            (warp w takes chunks w, w + 8, ...; then warps 0..7), then y = x * s_c + b_c with
 //                            s_c = gamma_c * rstd_g, b_c = beta_c - mean_g * s_c, + nearest-2x(residual), * 0.5 (FUSE_TYPE avg),
 //                            ReLU; one rounding at the store.  In place is allowed (each pixel is read before it is written
 //                            by the same thread).  gamma == nullptr: no statistics, s = 1, b = 0 (the avg fuse of a BN FPN).
-// The chunking depends on the map shape only, and every sum runs in a fixed order: bit-identical across launches and
-// processes; the scratch is fully written by the stats kernel before the apply kernel reads it.
+// The chunking depends on the map shape only, and every sum runs in a fixed order: bit-identical across launches, processes
+// and batch sizes; the scratch is fully written by the stats kernel before the apply kernel reads it.
 #include "act16.cuh"
 #include "group_norm.cuh"
 #include "pdl.cuh"
@@ -40,6 +45,22 @@ __device__ __forceinline__ void chan(float& n, float& mean, float& m2, float nb,
     n = nn;
 }
 
+// Thread layout of one channel count (see the file comment)
+template <int CPG>
+struct GnShape {
+    static constexpr int C = 32 * CPG;
+    static constexpr int kVec = C / 8;                   // 16-byte vectors per pixel
+    static constexpr int kRows = kGnThreads / kVec;      // pixels per CTA step
+    static constexpr int slots_of(int v) { return (8 * v + 7) / CPG - 8 * v / CPG + 1; }
+    static constexpr int max_slots() {
+        int m = 1;
+        for (int v = 0; v < kVec; ++v) m = slots_of(v) > m ? slots_of(v) : m;
+        return m;
+    }
+    static constexpr int kSlots = max_slots();           // groups one vector can touch: 1 (cpg % 8 == 0) .. 4 (cpg 2)
+    static_assert(C % 8 == 0 && kRows >= 1, "GroupNorm channel count");
+};
+
 // segment, image and chunk of CTA `cta`
 __device__ __forceinline__ int locate(const GroupNormParams& p, int cta, int* b, int* chunk) {
     int s = 0;
@@ -52,40 +73,97 @@ __device__ __forceinline__ int locate(const GroupNormParams& p, int cta, int* b,
     return s;
 }
 
+template <int CPG>
 __global__ void __launch_bounds__(kGnThreads) group_norm_stats_kernel(const GroupNormParams p) {
     DD3D_PDL_PROLOGUE();
-    __shared__ float sh[kGnWarps][32][3];
+    using S = GnShape<CPG>;
+    constexpr int K = S::kSlots;
+    __shared__ float sh[S::kRows * S::kVec][K][3];
     int b, chunk;
     const int s = locate(p, blockIdx.x, &b, &chunk);
     const GroupNormSeg& g = p.seg[s];
     const int HW = g.H * g.W;
     const int p0 = chunk * kGnChunk, p1 = min(HW, p0 + kGnChunk);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const __nv_bfloat16* img = g.in + static_cast<size_t>(b) * HW * g.in_pitch + lane * 8;
-    float n = 0.f, mean = 0.f, m2 = 0.f;
-#pragma unroll 4
-    for (int px = p0 + warp; px < p1; px += kGnWarps) {
-        float x[8];
-        unpack8(*reinterpret_cast<const uint4*>(img + static_cast<size_t>(px) * g.in_pitch), p.fp16, x);
-        const float mb = (((x[0] + x[1]) + (x[2] + x[3])) + ((x[4] + x[5]) + (x[6] + x[7]))) * 0.125f;
-        float m2b = 0.f;
+    const int v = threadIdx.x % S::kVec, r = threadIdx.x / S::kVec;
+    const __nv_bfloat16* img = g.in + static_cast<size_t>(b) * HW * g.in_pitch + v * 8;
+    float n[K], mean[K], m2[K];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) m2b = fmaf(x[j] - mb, x[j] - mb, m2b);
-        chan(n, mean, m2, 8.f, mb, m2b);
+    for (int j = 0; j < K; ++j) n[j] = mean[j] = m2[j] = 0.f;
+    if (r < S::kRows) {
+        if constexpr (K == 1) {
+#pragma unroll 4
+            for (int px = p0 + r; px < p1; px += S::kRows) {
+                float x[8];
+                unpack8(*reinterpret_cast<const uint4*>(img + static_cast<size_t>(px) * g.in_pitch), p.fp16, x);
+                const float mb = (((x[0] + x[1]) + (x[2] + x[3])) + ((x[4] + x[5]) + (x[6] + x[7]))) * 0.125f;
+                float m2b = 0.f;
+#pragma unroll
+                for (int k = 0; k < 8; ++k) m2b = fmaf(x[k] - mb, x[k] - mb, m2b);
+                chan(n[0], mean[0], m2[0], 8.f, mb, m2b);
+            }
+        } else {
+            // channel k of the vector belongs to slot sl[k] = group - first group of the vector; cnt[j] channels per slot
+            const int g0 = 8 * v / CPG;
+            int sl[8];
+            float cnt[K], inv[K];
+#pragma unroll
+            for (int j = 0; j < K; ++j) cnt[j] = 0.f;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                sl[k] = (8 * v + k) / CPG - g0;
+#pragma unroll
+                for (int j = 0; j < K; ++j) cnt[j] += sl[k] == j ? 1.f : 0.f;
+            }
+#pragma unroll
+            for (int j = 0; j < K; ++j) inv[j] = cnt[j] > 0.f ? 1.f / cnt[j] : 0.f;
+#pragma unroll 1
+            for (int px = p0 + r; px < p1; px += S::kRows) {
+                float x[8];
+                unpack8(*reinterpret_cast<const uint4*>(img + static_cast<size_t>(px) * g.in_pitch), p.fp16, x);
+#pragma unroll
+                for (int j = 0; j < K; ++j) {
+                    if (cnt[j] == 0.f) continue;
+                    float sum = 0.f;
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) sum += sl[k] == j ? x[k] : 0.f;
+                    const float mb = sum * inv[j];
+                    float m2b = 0.f;
+#pragma unroll
+                    for (int k = 0; k < 8; ++k)
+                        if (sl[k] == j) m2b = fmaf(x[k] - mb, x[k] - mb, m2b);
+                    chan(n[j], mean[j], m2[j], cnt[j], mb, m2b);
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < K; ++j) {
+            sh[threadIdx.x][j][0] = n[j];
+            sh[threadIdx.x][j][1] = mean[j];
+            sh[threadIdx.x][j][2] = m2[j];
+        }
     }
-    sh[warp][lane][0] = n;
-    sh[warp][lane][1] = mean;
-    sh[warp][lane][2] = m2;
     __syncthreads();
-    if (warp == 0) {
-        for (int w = 1; w < kGnWarps; ++w) chan(n, mean, m2, sh[w][lane][0], sh[w][lane][1], sh[w][lane][2]);
-        float2* out = g.part + (static_cast<size_t>(b) * g.nchunks + chunk) * 32 + lane;
-        *out = make_float2(mean, m2);
+    if (threadIdx.x < 32) {
+        // group gi: the slots of the vectors [v0, v1] that hold its channels, rows in order, then vectors in order
+        const int gi = threadIdx.x;
+        const int v0 = gi * CPG / 8, v1 = (gi * CPG + CPG - 1) / 8;
+        const int j0 = gi - 8 * v0 / CPG;
+        float an = sh[v0][j0][0], am = sh[v0][j0][1], a2 = sh[v0][j0][2];
+        for (int rr = 0; rr < S::kRows; ++rr)
+            for (int vv = v0; vv <= v1; ++vv) {
+                if (rr == 0 && vv == v0) continue;
+                const int t = rr * S::kVec + vv, j = gi - 8 * vv / CPG;
+                chan(an, am, a2, sh[t][j][0], sh[t][j][1], sh[t][j][2]);
+            }
+        float2* out = g.part + (static_cast<size_t>(b) * g.nchunks + chunk) * 32 + gi;
+        *out = make_float2(am, a2);
     }
 }
 
+template <int CPG>
 __global__ void __launch_bounds__(kGnThreads) group_norm_apply_kernel(const GroupNormParams p) {
     DD3D_PDL_PROLOGUE();
+    using S = GnShape<CPG>;
     __shared__ float sh[kGnWarps][32][3];
     __shared__ float stat[32][2];  // (mean, rstd) per group
     int b, chunk;
@@ -93,13 +171,14 @@ __global__ void __launch_bounds__(kGnThreads) group_norm_apply_kernel(const Grou
     const GroupNormSeg& g = p.seg[s];
     const int HW = g.H * g.W;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int v = threadIdx.x % S::kVec, r = threadIdx.x / S::kVec;
     float sc[8], bi[8];
     if (p.gamma != nullptr) {
         float n = 0.f, mean = 0.f, m2 = 0.f;
         const float2* part = g.part + static_cast<size_t>(b) * g.nchunks * 32 + lane;
         for (int c = warp; c < g.nchunks; c += kGnWarps) {
-            const float2 v = part[static_cast<size_t>(c) * 32];
-            chan(n, mean, m2, 8.f * static_cast<float>(min(kGnChunk, HW - c * kGnChunk)), v.x, v.y);
+            const float2 pv = part[static_cast<size_t>(c) * 32];
+            chan(n, mean, m2, static_cast<float>(CPG) * static_cast<float>(min(kGnChunk, HW - c * kGnChunk)), pv.x, pv.y);
         }
         sh[warp][lane][0] = n;
         sh[warp][lane][1] = mean;
@@ -111,45 +190,46 @@ __global__ void __launch_bounds__(kGnThreads) group_norm_apply_kernel(const Grou
             stat[lane][1] = 1.0f / sqrtf(m2 / n + 1e-5f);  // biased variance, eps = 1e-5 (nn.GroupNorm)
         }
         __syncthreads();
-        const float mu = stat[lane][0], rstd = stat[lane][1];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            sc[j] = p.gamma[lane * 8 + j] * rstd;
-            bi[j] = p.beta[lane * 8 + j] - mu * sc[j];
+        for (int k = 0; k < 8; ++k) {
+            const int c = v * 8 + k, gi = c / CPG;
+            sc[k] = p.gamma[c] * stat[gi][1];
+            bi[k] = p.beta[c] - stat[gi][0] * sc[k];
         }
     } else {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            sc[j] = 1.f;
-            bi[j] = 0.f;
+        for (int k = 0; k < 8; ++k) {
+            sc[k] = 1.f;
+            bi[k] = 0.f;
         }
     }
+    if (r >= S::kRows) return;
     const int p0 = chunk * kGnChunk, p1 = min(HW, p0 + kGnChunk);
-    const __nv_bfloat16* src = g.in + static_cast<size_t>(b) * HW * g.in_pitch + lane * 8;
-    __nv_bfloat16* dst = g.out + static_cast<size_t>(b) * HW * g.out_pitch + lane * 8;
+    const __nv_bfloat16* src = g.in + static_cast<size_t>(b) * HW * g.in_pitch + v * 8;
+    __nv_bfloat16* dst = g.out + static_cast<size_t>(b) * HW * g.out_pitch + v * 8;
     const __nv_bfloat16* res =
-        g.res != nullptr ? g.res + static_cast<size_t>(b) * g.res_H * g.res_W * g.res_pitch + lane * 8 : nullptr;
+        g.res != nullptr ? g.res + static_cast<size_t>(b) * g.res_H * g.res_W * g.res_pitch + v * 8 : nullptr;
 #pragma unroll 4
-    for (int px = p0 + warp; px < p1; px += kGnWarps) {
+    for (int px = p0 + r; px < p1; px += S::kRows) {
         float x[8];
         unpack8(*reinterpret_cast<const uint4*>(src + static_cast<size_t>(px) * g.in_pitch), p.fp16, x);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) x[j] = fmaf(x[j], sc[j], bi[j]);
+        for (int k = 0; k < 8; ++k) x[k] = fmaf(x[k], sc[k], bi[k]);
         if (res != nullptr) {
             const int y = px / g.W, xx = px - y * g.W;
-            float r[8];
+            float rv[8];
             unpack8(*reinterpret_cast<const uint4*>(res + (static_cast<size_t>(y >> 1) * g.res_W + (xx >> 1)) * g.res_pitch),
-                    p.fp16, r);
+                    p.fp16, rv);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) x[j] += r[j];
+            for (int k = 0; k < 8; ++k) x[k] += rv[k];
         }
         if (p.avg) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) x[j] *= 0.5f;
+            for (int k = 0; k < 8; ++k) x[k] *= 0.5f;
         }
         if (p.relu) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) x[j] = fmaxf(x[j], 0.f);
+            for (int k = 0; k < 8; ++k) x[k] = fmaxf(x[k], 0.f);
         }
         uint4 o;
         o.x = pack2_act(x[0], x[1], p.fp16);
@@ -160,9 +240,25 @@ __global__ void __launch_bounds__(kGnThreads) group_norm_apply_kernel(const Grou
     }
 }
 
+template <int CPG>
+cudaError_t launch_cpg(const GroupNormParams& p, unsigned ctas, cudaStream_t stream) {
+    if (p.gamma != nullptr) {
+        const cudaError_t e = launch_pdl(group_norm_stats_kernel<CPG>, dim3(ctas), dim3(kGnThreads), 0, stream, p);
+        if (e != cudaSuccess) return e;
+    }
+    return launch_pdl(group_norm_apply_kernel<CPG>, dim3(ctas), dim3(kGnThreads), 0, stream, p);
+}
+
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
 
 }  // namespace
+
+bool group_norm_channels_ok(int C) {
+    switch (C) {
+        case 64: case 128: case 160: case 192: case 224: case 256: case 512: case 768: case 1024: return true;
+        default: return false;
+    }
+}
 
 int group_norm_chunks(int H, int W) { return (H * W + kGnChunk - 1) / kGnChunk; }
 
@@ -171,7 +267,7 @@ size_t group_norm_scratch_bytes(int B, int H, int W) {
 }
 
 cudaError_t launch_group_norm(GroupNormParams p, cudaStream_t stream) {
-    if (p.nseg < 1 || p.nseg > kMaxSeg || p.B < 1) return cudaErrorInvalidValue;
+    if (p.nseg < 1 || p.nseg > kMaxSeg || p.B < 1 || !group_norm_channels_ok(p.C)) return cudaErrorInvalidValue;
     if ((p.gamma == nullptr) != (p.beta == nullptr)) return cudaErrorInvalidValue;
     if (p.gamma == nullptr && p.avg == 0 && p.relu == 0) {
         bool any_res = false;
@@ -182,10 +278,10 @@ cudaError_t launch_group_norm(GroupNormParams p, cudaStream_t stream) {
     for (int s = 0; s < p.nseg; ++s) {
         GroupNormSeg& g = p.seg[s];
         if (g.H < 1 || g.W < 1 || !g.in || !g.out) return cudaErrorInvalidValue;
-        if (g.in_pitch < kGnChannels || g.out_pitch < kGnChannels || g.in_pitch % 8 || g.out_pitch % 8) return cudaErrorInvalidValue;
+        if (g.in_pitch < p.C || g.out_pitch < p.C || g.in_pitch % 8 || g.out_pitch % 8) return cudaErrorInvalidValue;
         if (!aligned16(g.in) || !aligned16(g.out)) return cudaErrorInvalidValue;
         if (g.res != nullptr) {
-            if (g.res_pitch < kGnChannels || g.res_pitch % 8 || !aligned16(g.res)) return cudaErrorInvalidValue;
+            if (g.res_pitch < p.C || g.res_pitch % 8 || !aligned16(g.res)) return cudaErrorInvalidValue;
             if (g.res_H != (g.H + 1) / 2 && g.res_H != g.H / 2) return cudaErrorInvalidValue;
             if (g.res_W != (g.W + 1) / 2 && g.res_W != g.W / 2) return cudaErrorInvalidValue;
             if (g.res_H * 2 < g.H || g.res_W * 2 < g.W) return cudaErrorInvalidValue;  // every output pixel has a source
@@ -197,11 +293,18 @@ cudaError_t launch_group_norm(GroupNormParams p, cudaStream_t stream) {
         ctas += static_cast<long>(p.B) * g.nchunks;
     }
     if (ctas > 0x7fffffffL) return cudaErrorInvalidValue;
-    if (p.gamma != nullptr) {
-        const cudaError_t e = launch_pdl(group_norm_stats_kernel, dim3(static_cast<unsigned>(ctas)), dim3(kGnThreads), 0, stream, p);
-        if (e != cudaSuccess) return e;
+    const unsigned n = static_cast<unsigned>(ctas);
+    switch (p.C / 32) {
+        case 2: return launch_cpg<2>(p, n, stream);
+        case 4: return launch_cpg<4>(p, n, stream);
+        case 5: return launch_cpg<5>(p, n, stream);
+        case 6: return launch_cpg<6>(p, n, stream);
+        case 7: return launch_cpg<7>(p, n, stream);
+        case 8: return launch_cpg<8>(p, n, stream);
+        case 16: return launch_cpg<16>(p, n, stream);
+        case 24: return launch_cpg<24>(p, n, stream);
+        default: return launch_cpg<32>(p, n, stream);
     }
-    return launch_pdl(group_norm_apply_kernel, dim3(static_cast<unsigned>(ctas)), dim3(kGnThreads), 0, stream, p);
 }
 
 }  // namespace dd3d

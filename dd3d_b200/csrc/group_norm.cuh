@@ -1,4 +1,5 @@
-// GroupNorm(32, 256) of the FCOS towers and the FPN (group_norm.cu): statistics + apply over up to kMaxSeg maps per launch.
+// GroupNorm(32, C) of the FCOS towers, the FPN and the VoVNet backbone (group_norm.cu): statistics + apply over up to kMaxSeg
+// maps of C channels per launch.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -8,11 +9,11 @@
 
 namespace dd3d {
 
-constexpr int kGnChannels = 256;  // 32 groups of 8 channels
+constexpr int kGnChannels = 256;  // heads and FPN: 32 groups of 8 channels
 constexpr int kGnChunk = 1024;    // pixels per statistics chunk (a function of the shape only: deterministic)
 
 struct GroupNormSeg {
-    const __nv_bfloat16* in = nullptr;   // [B][H][W][in_pitch], channels [0, 256)
+    const __nv_bfloat16* in = nullptr;   // [B][H][W][in_pitch], channels [0, C)
     __nv_bfloat16* out = nullptr;        // [B][H][W][out_pitch]; may equal `in`
     const __nv_bfloat16* res = nullptr;  // optional [B][res_H][res_W][res_pitch]: added as nearest-2x after the norm
     int H = 0, W = 0, in_pitch = 0, out_pitch = 0, res_pitch = 0, res_H = 0, res_W = 0;
@@ -23,11 +24,14 @@ struct GroupNormSeg {
 struct GroupNormParams {
     GroupNormSeg seg[kMaxSeg];
     int nseg = 0, B = 0;
-    const float* gamma = nullptr;  // fp32 [256]; nullptr: no normalisation (s = 1, b = 0)
+    const float* gamma = nullptr;  // fp32 [C]; nullptr: no normalisation (s = 1, b = 0)
     const float* beta = nullptr;
     int relu = 0, avg = 0, fp16 = 0;
+    int C = kGnChannels;  // channels per pixel of every segment: group_norm_channels_ok(C)
 };
 
+// C = 32 * cpg with cpg in {2, 4, 5, 6, 7, 8, 16, 24, 32}: the channel counts of the GN heads, FPN and VoVNet backbones
+bool group_norm_channels_ok(int C);
 int group_norm_chunks(int H, int W);
 size_t group_norm_scratch_bytes(int B, int H, int W);
 // One launch of the statistics kernel (skipped when gamma == nullptr) and one of the apply kernel over every segment.

@@ -14,11 +14,12 @@ cudaError_t launch_preprocess(const void* src, int src_is_u8, const int* d_sizes
                               cudaStream_t stream, int fp16 = 0);
 
 // Stem conv (Cin = 3) on tensor cores (stem_tc.cu).  in: bf16 [B][H][W][4]; w: bf16 [cout][stem_tc_kpad(ksize)] with
-// k = (ky*ksize + kx)*4 + c (zero padded); out NHWC bf16 with `out_pitch` channels per pixel.
+// k = (ky*ksize + kx)*4 + c (zero padded); out NHWC bf16 with `out_pitch` channels per pixel.  relu = 0: no ReLU after the
+// folded affine (the raw conv output of a GroupNorm backbone); the same for launch_stem_s2_mma.
 int stem_tc_kpad(int ksize);
 cudaError_t launch_stem_tc(const __nv_bfloat16* in, const __nv_bfloat16* w, const float* scale, const float* bias,
                            __nv_bfloat16* out, int B, int H, int W, int ksize, int stride, int cout, int out_pitch,
-                           int num_sms, cudaStream_t stream, int fp16 = 0);
+                           int num_sms, cudaStream_t stream, int fp16 = 0, int relu = 1);
 
 // DLA-34 front end fused (dla_front.cu): base_layer 7x7 -> level0 3x3 -> level1 3x3/s2 (+ 2x2 max-pool of the result), conv +
 // BN + ReLU each, intermediates in shared memory.  in4: [B][H][W][4]; w0 [16][7][8][4], w1 [16][9][16], w2 [32][9][16] 16-bit;
@@ -31,7 +32,8 @@ cudaError_t launch_dla_front(const __nv_bfloat16* in4, const __nv_bfloat16* w0, 
 // VoVNet stem_1 (3x3 stride 2, 3 -> 64) on register fragments (stem_mma.cu).  w: 16-bit [64][3][4][4] (cout, ky, kx, c; kx = 3
 // and c = 3 zero); sb: fp32 scale[64] | bias[64]; out: [B][ceil(H/2)][ceil(W/2)][out_pitch].
 cudaError_t launch_stem_s2_mma(const __nv_bfloat16* in4, const __nv_bfloat16* w, const float* sb, __nv_bfloat16* out,
-                               int out_pitch, int B, int H, int W, int num_sms, cudaStream_t stream, int fp16 = 0);
+                               int out_pitch, int B, int H, int W, int num_sms, cudaStream_t stream, int fp16 = 0,
+                               int relu = 1);
 
 cudaError_t launch_maxpool(const __nv_bfloat16* in, __nv_bfloat16* out, int B, int H, int W, int C, int in_pitch,
                            int Ho, int Wo, int out_pitch, int ksize, int num_sms, cudaStream_t stream, int fp16 = 0);

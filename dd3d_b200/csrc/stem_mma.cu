@@ -39,6 +39,7 @@ struct StemParams {
     const float* sb;          // scale[64] | bias[64]
     __nv_bfloat16* out;       // [B][Ho][Wo][out_pitch]
     int B, H, W, Ho, Wo, out_pitch, tiles_x, tiles_y;
+    int relu;  // 0: no ReLU (the raw output of a GroupNorm backbone)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -94,6 +95,11 @@ __device__ __forceinline__ void load_input(const StemParams& p, int tile, uint32
             cp_async8(dst + (y * IW + x) * 8, row + (ok ? gx * 4 : 0), ok ? 8u : 0u);
         }
     }
+}
+
+template <bool FP16>
+__device__ __forceinline__ uint32_t pack2_stem(int relu, float a, float b) {
+    return relu ? pack2_relu<FP16>(a, b) : pack2_act(a, b, FP16 ? 1 : 0);
 }
 
 template <bool FP16>
@@ -155,16 +161,16 @@ __global__ void __launch_bounds__(kThreads, 2) stem_s2_mma_kernel(const StemPara
 #pragma unroll
                 for (int nt = 0; nt < 8; ++nt) mma16816<FP16>(acc[nt], lo.x, hi.x, lo.y, hi.y, wb[ky][nt].x, wb[ky][nt].y);
             }
-            // BN + ReLU + rounding in registers: this lane's columns are channels 16 t .. 16 t + 15 of rows g and g + 8
+            // BN + ReLU (p.relu) + rounding in registers: this lane's columns are channels 16 t .. 16 t + 15 of rows g and g + 8
             uint32_t o_lo[8], o_hi[8];
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 const float4 sc = __ldg(reinterpret_cast<const float4*>(p.sb + 16 * t) + q);
                 const float4 bi = __ldg(reinterpret_cast<const float4*>(p.sb + 64 + 16 * t) + q);
-                o_lo[2 * q] = pack2_relu<FP16>(fmaf(acc[2 * q][0], sc.x, bi.x), fmaf(acc[2 * q][1], sc.y, bi.y));
-                o_hi[2 * q] = pack2_relu<FP16>(fmaf(acc[2 * q][2], sc.x, bi.x), fmaf(acc[2 * q][3], sc.y, bi.y));
-                o_lo[2 * q + 1] = pack2_relu<FP16>(fmaf(acc[2 * q + 1][0], sc.z, bi.z), fmaf(acc[2 * q + 1][1], sc.w, bi.w));
-                o_hi[2 * q + 1] = pack2_relu<FP16>(fmaf(acc[2 * q + 1][2], sc.z, bi.z), fmaf(acc[2 * q + 1][3], sc.w, bi.w));
+                o_lo[2 * q] = pack2_stem<FP16>(p.relu, fmaf(acc[2 * q][0], sc.x, bi.x), fmaf(acc[2 * q][1], sc.y, bi.y));
+                o_hi[2 * q] = pack2_stem<FP16>(p.relu, fmaf(acc[2 * q][2], sc.x, bi.x), fmaf(acc[2 * q][3], sc.y, bi.y));
+                o_lo[2 * q + 1] = pack2_stem<FP16>(p.relu, fmaf(acc[2 * q + 1][0], sc.z, bi.z), fmaf(acc[2 * q + 1][1], sc.w, bi.w));
+                o_hi[2 * q + 1] = pack2_stem<FP16>(p.relu, fmaf(acc[2 * q + 1][2], sc.z, bi.z), fmaf(acc[2 * q + 1][3], sc.w, bi.w));
             }
             const int gy = oy0 + oy;
 #pragma unroll
@@ -187,12 +193,13 @@ __global__ void __launch_bounds__(kThreads, 2) stem_s2_mma_kernel(const StemPara
 // in4: [B][H][W][4]; w: 16-bit [64][3][4][4] (cout, ky, kx, c; kx = 3 and c = 3 zero); sb: fp32 scale[64] | bias[64];
 // out: [B][ceil(H/2)][ceil(W/2)][out_pitch].
 cudaError_t launch_stem_s2_mma(const __nv_bfloat16* in4, const __nv_bfloat16* w, const float* sb, __nv_bfloat16* out,
-                               int out_pitch, int B, int H, int W, int num_sms, cudaStream_t stream, int fp16) {
+                               int out_pitch, int B, int H, int W, int num_sms, cudaStream_t stream, int fp16, int relu) {
     if (out_pitch % 8 || B < 1 || H < 1 || W < 1) return cudaErrorInvalidValue;
     StemParams p;
     p.in = in4; p.w = w; p.sb = sb; p.out = out;
     p.B = B; p.H = H; p.W = W; p.Ho = (H + 1) / 2; p.Wo = (W + 1) / 2;
     p.out_pitch = out_pitch;
+    p.relu = relu ? 1 : 0;
     p.tiles_x = (p.Wo + TW - 1) / TW;
     p.tiles_y = (p.Ho + TH - 1) / TH;
     static uint64_t attr_devices[2] = {0, 0};

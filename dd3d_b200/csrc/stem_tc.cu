@@ -31,7 +31,7 @@ template <int KS, int STRIDE, int COUT, bool F16>
 __global__ void __launch_bounds__(kStemThreads) stem_tc_kernel(const __nv_bfloat16* __restrict__ in, const __nv_bfloat16* __restrict__ w,
                                                                const float* __restrict__ scale, const float* __restrict__ bias,
                                                                __nv_bfloat16* __restrict__ out, int B, int H, int W, int Ho, int Wo,
-                                                               int out_pitch, int tiles_x, int tiles_y) {
+                                                               int out_pitch, int tiles_x, int tiles_y, int relu) {
     constexpr int PAD = (KS - 1) / 2;
     constexpr int K = KS * KS * 4;            // 36 / 196
     constexpr int KB = (K + 63) / 64;         // 64-element k-blocks: 1 / 4
@@ -129,8 +129,12 @@ __global__ void __launch_bounds__(kStemThreads) stem_tc_kernel(const __nv_bfloat
 #pragma unroll
                     for (int j = 0; j < COUT / 8; ++j) {
                         const int col = 8 * j + 2 * (lane & 3);
-                        const float y0 = fmaxf(fmaf(acc[m][4 * j + 2 * h], s_scale[col], s_bias[col]), 0.f);
-                        const float y1 = fmaxf(fmaf(acc[m][4 * j + 2 * h + 1], s_scale[col + 1], s_bias[col + 1]), 0.f);
+                        float y0 = fmaf(acc[m][4 * j + 2 * h], s_scale[col], s_bias[col]);
+                        float y1 = fmaf(acc[m][4 * j + 2 * h + 1], s_scale[col + 1], s_bias[col + 1]);
+                        if (relu) {  // 0: the raw output a GroupNorm normalises
+                            y0 = fmaxf(y0, 0.f);
+                            y1 = fmaxf(y1, 0.f);
+                        }
                         *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2_act(y0, y1, F16 ? 1 : 0);
                     }
                 }
@@ -143,7 +147,7 @@ __global__ void __launch_bounds__(kStemThreads) stem_tc_kernel(const __nv_bfloat
 template <int KS, int STRIDE, int COUT>
 cudaError_t launch_one(const __nv_bfloat16* in, const __nv_bfloat16* w, const float* scale, const float* bias,
                        __nv_bfloat16* out, int B, int H, int W, int out_pitch, int num_sms, cudaStream_t stream,
-                       int fp16) {
+                       int fp16, int relu) {
     constexpr int PAD = (KS - 1) / 2;
     constexpr int KB = (KS * KS * 4 + 63) / 64;
     const int Ho = (H + 2 * PAD - KS) / STRIDE + 1, Wo = (W + 2 * PAD - KS) / STRIDE + 1;
@@ -170,9 +174,9 @@ cudaError_t launch_one(const __nv_bfloat16* in, const __nv_bfloat16* w, const fl
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     return fp16 ? cudaLaunchKernelEx(&cfg, stem_tc_kernel<KS, STRIDE, COUT, true>, in, w, scale, bias, out, B, H, W, Ho, Wo,
-                                     out_pitch, tiles_x, tiles_y)
+                                     out_pitch, tiles_x, tiles_y, relu)
                 : cudaLaunchKernelEx(&cfg, stem_tc_kernel<KS, STRIDE, COUT, false>, in, w, scale, bias, out, B, H, W, Ho, Wo,
-                                     out_pitch, tiles_x, tiles_y);
+                                     out_pitch, tiles_x, tiles_y, relu);
 }
 
 }  // namespace
@@ -182,11 +186,11 @@ int stem_tc_kpad(int ksize) { return (ksize * ksize * 4 + 63) / 64 * 64; }
 // in: bf16 [B][H][W][4]; w: bf16 [cout][stem_tc_kpad(ksize)] with k = (ky*ksize + kx)*4 + c; out: NHWC bf16.
 cudaError_t launch_stem_tc(const __nv_bfloat16* in, const __nv_bfloat16* w, const float* scale, const float* bias,
                            __nv_bfloat16* out, int B, int H, int W, int ksize, int stride, int cout, int out_pitch,
-                           int num_sms, cudaStream_t stream, int fp16) {
+                           int num_sms, cudaStream_t stream, int fp16, int relu) {
     if (ksize == 7 && stride == 1 && cout == 16)
-        return launch_one<7, 1, 16>(in, w, scale, bias, out, B, H, W, out_pitch, num_sms, stream, fp16);
+        return launch_one<7, 1, 16>(in, w, scale, bias, out, B, H, W, out_pitch, num_sms, stream, fp16, relu);
     if (ksize == 3 && stride == 2 && cout == 64)
-        return launch_one<3, 2, 64>(in, w, scale, bias, out, B, H, W, out_pitch, num_sms, stream, fp16);
+        return launch_one<3, 2, 64>(in, w, scale, bias, out, B, H, W, out_pitch, num_sms, stream, fp16, relu);
     return cudaErrorInvalidValue;
 }
 

@@ -23,6 +23,8 @@ NORM_BN_PER_LEVEL, NORM_BN_SHARED, NORM_GN, NORM_NONE = 0, 1, 2, 3  # dd3d_norm
 # FrozenBN are per level (ModuleListDial, fcos2d.py:73-80); the FPN's norms are one per conv, so every BN is "shared" there.
 HEAD_NORMS = {"BN": NORM_BN_PER_LEVEL, "FrozenBN": NORM_BN_PER_LEVEL, "SyncBN": NORM_BN_SHARED, "GN": NORM_GN, "": NORM_NONE}
 FPN_NORMS = {"BN": NORM_BN_SHARED, "FrozenBN": NORM_BN_SHARED, "SyncBN": NORM_BN_SHARED, "GN": NORM_GN, "": NORM_NONE}
+# FE.BACKBONE.NORM -> dd3d_norm of dd3d_set_backbone_norm (eval BatchNorm2d and FrozenBatchNorm2d fold alike)
+BACKBONE_NORMS = {"BN": NORM_BN_SHARED, "FrozenBN": NORM_BN_SHARED, "SyncBN": NORM_BN_SHARED, "GN": NORM_GN, "": NORM_NONE}
 DET_WORDS = 24  # sizeof(dd3d_det) / 4
 
 
@@ -84,6 +86,7 @@ SIGNATURES = {
     "dd3d_last_error": (C.c_char_p, [_P]),
     "dd3d_size_divisibility": (_I, [_P]),
     "dd3d_set_layout": (_I, [_P, C.POINTER(LayoutDesc)]),
+    "dd3d_set_backbone_norm": (_I, [_P, C.c_int32]),
     "dd3d_load_weight": (_I, [_P, C.c_char_p, _P, C.POINTER(_I64), _I]),
     "dd3d_finalize": (_I, [_P]),
     "dd3d_workspace_bytes": (_I64, [_P, _I, _I, _I]),
@@ -122,6 +125,7 @@ SIGNATURES = {
     "dd3d_op_dwconv3x3": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _I, _P]),
     "dd3d_op_group_norm_scratch_bytes": (_I64, [_I, _I, _I]),
     "dd3d_op_group_norm": (_I, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _I, _P, _P]),
+    "dd3d_op_group_norm_c": (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _P]),
     "dd3d_op_preprocess": (_I, [_P, _I, _P, _P, _I, _I, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
     "dd3d_op_maxpool": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "dd3d_op_ese": (_I, [_P, _I, _P, _P, _P, _I, _P, _I, _P, _I, _I, _I, _P]),

@@ -44,6 +44,8 @@ class DD3DB200(nn.Module):
         self._layout = _lib.layout_from_cfg(cfg)
         if cfg.DD3D.FCOS2D.USE_DEFORMABLE or (cfg.MODEL.BOX3D_ON and cfg.DD3D.FCOS3D.USE_DEFORMABLE):
             raise ValueError("Not supported yet.")  # fcos2d.py:51-52, fcos3d.py:77-78
+        # param_specs raised the reference's errors for the FE.BACKBONE.NORM values it cannot build
+        self._backbone_norm = _lib.BACKBONE_NORMS[cfg.FE.BACKBONE.NORM]
         self._handle = None
         self._plan_key = None
         self._host_bufs = None
@@ -124,6 +126,7 @@ class DD3DB200(nn.Module):
         with torch.cuda.device(self._device):
             _lib.check(L.dd3d_create(C.byref(self._desc), C.byref(handle)))
             _lib.check(L.dd3d_set_layout(handle, C.byref(self._layout)), handle)
+            _lib.check(L.dd3d_set_backbone_norm(handle, self._backbone_norm), handle)
             for name, t in self._state.items():
                 if not t.is_floating_point():
                     continue

@@ -148,6 +148,12 @@ int dd3d_size_divisibility(dd3d_handle h);  /* backbone.size_divisibility: 128 (
 /* Sets the FPN / head layout (dd3d_layout_desc) before dd3d_finalize (DD3D_ERR_STATE afterwards).  An unknown dd3d_norm value,
  * a depth outside 0..16 or fpn_fuse_avg other than 0 / 1 returns DD3D_ERR_INVALID and leaves the layout unchanged. */
 int dd3d_set_layout(dd3d_handle h, const dd3d_layout_desc* h_layout);
+/* Sets the backbone's norm (FE.BACKBONE.NORM) before dd3d_finalize (DD3D_ERR_STATE afterwards), as a dd3d_norm:
+ * DD3D_NORM_BN_SHARED or DD3D_NORM_BN_PER_LEVEL (the default, for "FrozenBN", "BN" and "SyncBN", which compute the same thing in
+ * eval: the BN is folded into each conv) or DD3D_NORM_NONE (DLA-34 only: "", every backbone conv has a bias and no norm).
+ * DD3D_NORM_GN and, for a VoVNet, DD3D_NORM_NONE return DD3D_ERR_INVALID and leave the backbone unchanged.  An engine that
+ * never receives the call builds the BN backbone. */
+int dd3d_set_backbone_norm(dd3d_handle h, int32_t dd3d_norm);
 
 /* ---- weights: one call per tensor of the reference state_dict (Checkpointer.load, scripts/train.py:52) ----- */
 /* h_data: host fp32, contiguous, `ndim` dims in h_shape.  Unknown names are ignored (return DD3D_OK, e.g.
@@ -361,6 +367,14 @@ int64_t dd3d_op_group_norm_scratch_bytes(int B, int H, int W);
 int dd3d_op_group_norm(const void* d_in, int B, int H, int W, int in_pitch, const float* d_gamma, const float* d_beta, int relu,
                        const void* d_residual, int res_pitch, int avg, void* d_out, int out_pitch, void* d_scratch,
                        dd3d_stream stream);
+/* dd3d_op_group_norm_c: GroupNorm(32, C) for C = 32 * cpg, cpg in {2, 4, 5, 6, 7, 8, 16, 24, 32} (64 .. 1024 channels), same
+ * kernels and arithmetic as dd3d_op_group_norm (for C = 256 bit-identical to it), then ReLU when relu; one rounding at the store.
+ * Reads channels [in_c0, in_c0 + C) of d_in = [B][H][W][in_pitch] and writes channels [out_c0, out_c0 + C) of
+ * d_out = [B][H][W][out_pitch]: channel slices of concat buffers; in place when d_out == d_in and out_c0 == in_c0.  d_gamma,
+ * d_beta: fp32 [C].  d_scratch: dd3d_op_group_norm_scratch_bytes(B, H, W) bytes, any content.  Offsets and pitches multiples
+ * of 8, d_in / d_out 16-byte aligned. */
+int dd3d_op_group_norm_c(const void* d_in, int B, int H, int W, int C, int in_c0, int in_pitch, const float* d_gamma,
+                         const float* d_beta, int relu, void* d_out, int out_c0, int out_pitch, void* d_scratch, dd3d_stream stream);
 int dd3d_op_preprocess(const void* d_images, int img_dtype, const int32_t* d_sizes2, void* d_out4, int B, int Hs, int Ws,
                        int Hp, int Wp, const float* h_mean, const float* h_std, dd3d_stream stream);
 int dd3d_op_maxpool(const void* d_in, void* d_out, int B, int H, int W, int C, int in_pitch, int out_pitch, int ksize,
