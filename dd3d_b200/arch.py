@@ -1,7 +1,7 @@
-"""Parameter inventory of the DD3D configurations (DLA-34 and every VoVNetV2-eSE variant), keyed by the reference's state_dict names.
+"""Parameter inventory of the DD3D configurations (DLA-34, the DLA-X networks and every VoVNetV2-eSE variant), keyed by the reference's state_dict names.
 
 The names/shapes follow what ``DD3D(cfg).state_dict()`` yields in the reference
-(tridet/modeling/dd3d/core.py:19-55; DLA-34 tridet/modeling/feature_extractor/dla.py:250-361; VoVNetV2-eSE
+(tridet/modeling/dd3d/core.py:19-55; DLA tridet/modeling/feature_extractor/dla.py:24-441; VoVNetV2-eSE
 tridet/modeling/feature_extractor/vovnet.py:19-143,188-336; FPN + top blocks dla.py:537-561, vovnet.py:411-454;
 heads fcos2d.py:55-108, fcos3d.py:81-139).  tests/test_cpu_oracle.py::test_inventory_and_oracle_vs_live_reference checks this inventory against the
 reference's own state_dict when /root/reference is present.
@@ -47,34 +47,62 @@ def _conv_bn(specs, name, cout, cin, k, role="relu", norm="FrozenBN"):
     _norm(specs, name + ".norm", cout, norm)
 
 
-def _dla_tree(specs, p, levels, in_ch, out_ch, level_root, root_dim=0, norm="FrozenBN"):
+# The reference's DLA_NAME_TO_BUILDER networks the engine builds (dla.py:358-441), by arch key: (FE.BACKBONE.NAME, levels,
+# channels, BottleneckX blocks, residual_root, cardinality).  DLA-X-102-64 is dla102x2, which sets BottleneckX.cardinality = 64
+# (dla.py:411).  The engine has its own copy (csrc/engine.cu kDlaSpecs); tests/test_dla_x.py pins both against the reference.
+DLA_SPECS = {
+    "dla34": ("DLA-34", (1, 1, 1, 2, 2, 1), (16, 32, 64, 128, 256, 512), False, False, 0),
+    "dla_x_46_c": ("DLA-X-46-C", (1, 1, 1, 2, 2, 1), (16, 32, 64, 64, 128, 256), True, False, 32),
+    "dla_x_60_c": ("DLA-X-60-C", (1, 1, 1, 2, 3, 1), (16, 32, 64, 64, 128, 256), True, False, 32),
+    "dla_x_60": ("DLA-X-60", (1, 1, 1, 2, 3, 1), (16, 32, 128, 256, 512, 1024), True, False, 32),
+    "dla_x_102": ("DLA-X-102", (1, 1, 1, 3, 4, 1), (16, 32, 128, 256, 512, 1024), True, True, 32),
+    "dla_x_102_64": ("DLA-X-102-64", (1, 1, 1, 3, 4, 1), (16, 32, 128, 256, 512, 1024), True, True, 64),
+}
+DLA_KEYS = {spec[0]: key for key, spec in DLA_SPECS.items()}  # FE.BACKBONE.NAME -> arch key
+
+
+def _dla_block(specs, p, cin, cout, norm, cardinality):
+    """BasicBlock (dla.py:24-62), or BottleneckX (dla.py:104-143) when cardinality > 0: 1x1 -> grouped 3x3 -> 1x1 with
+    bottleneck width cout * cardinality / 32 and conv2.weight (width, width / cardinality, 3, 3)."""
+    if not cardinality:
+        _conv_bn(specs, f"{p}.conv1", cout, cin, 3, norm=norm)
+        _conv_bn(specs, f"{p}.conv2", cout, cout, 3, role="linear", norm=norm)
+        return
+    width = cout * cardinality // 32
+    _conv_bn(specs, f"{p}.conv1", width, cin, 1, norm=norm)
+    _conv_bn(specs, f"{p}.conv2", width, width // cardinality, 3, norm=norm)
+    _conv_bn(specs, f"{p}.conv3", cout, width, 1, role="linear", norm=norm)
+
+
+def _dla_tree(specs, p, levels, in_ch, out_ch, level_root, root_dim=0, norm="FrozenBN", cardinality=0):
+    """Tree (dla.py:170-247) in module registration order: tree1, tree2, root, project (only where tree1 is a block)."""
     if root_dim == 0:
         root_dim = 2 * out_ch
     if level_root:
         root_dim += in_ch
     if levels == 1:
-        for t, cin in (("tree1", in_ch), ("tree2", out_ch)):
-            _conv_bn(specs, f"{p}.{t}.conv1", out_ch, cin, 3, norm=norm)
-            _conv_bn(specs, f"{p}.{t}.conv2", out_ch, out_ch, 3, role="linear", norm=norm)
+        _dla_block(specs, f"{p}.tree1", in_ch, out_ch, norm, cardinality)
+        _dla_block(specs, f"{p}.tree2", out_ch, out_ch, norm, cardinality)
         _conv_bn(specs, f"{p}.root.conv", out_ch, root_dim, 1, norm=norm)
         if in_ch != out_ch:
             _conv_bn(specs, f"{p}.project", out_ch, in_ch, 1, role="linear", norm=norm)
     else:
-        _dla_tree(specs, p + ".tree1", levels - 1, in_ch, out_ch, False, norm=norm)
-        _dla_tree(specs, p + ".tree2", levels - 1, out_ch, out_ch, False, root_dim=root_dim + out_ch, norm=norm)
+        _dla_tree(specs, p + ".tree1", levels - 1, in_ch, out_ch, False, norm=norm, cardinality=cardinality)
+        _dla_tree(specs, p + ".tree2", levels - 1, out_ch, out_ch, False, root_dim=root_dim + out_ch, norm=norm,
+                  cardinality=cardinality)
 
 
-def _dla34(specs, norm):
+def _dla(specs, arch, norm):
     p = "backbone.bottom_up"
-    ch = [16, 32, 64, 128, 256, 512]
-    levels = [1, 1, 1, 2, 2, 1]
+    _, levels, ch, bottleneck_x, _, cardinality = DLA_SPECS[arch]
+    card = cardinality if bottleneck_x else 0
     _conv_bn(specs, p + ".base_layer", ch[0], 3, 7, norm=norm)
     _conv_bn(specs, p + ".level0.0", ch[0], ch[0], 3, norm=norm)
     _conv_bn(specs, p + ".level1.0", ch[1], ch[0], 3, norm=norm)
-    _dla_tree(specs, p + ".level2", levels[2], ch[1], ch[2], False, norm=norm)
+    _dla_tree(specs, p + ".level2", levels[2], ch[1], ch[2], False, norm=norm, cardinality=card)
     for lvl in (3, 4, 5):
-        _dla_tree(specs, p + f".level{lvl}", levels[lvl], ch[lvl - 1], ch[lvl], True, norm=norm)
-    return {"level3": 128, "level4": 256, "level5": 512}
+        _dla_tree(specs, p + f".level{lvl}", levels[lvl], ch[lvl - 1], ch[lvl], True, norm=norm, cardinality=card)
+    return {"level3": ch[3], "level4": ch[4], "level5": ch[5]}
 
 
 V99_STAGE_CONV_CH = [128, 160, 192, 224]
@@ -94,7 +122,7 @@ VOVNET_SPECS = {
     "v2_99": ("V-99-eSE", (64, 64, 128), tuple(V99_STAGE_CONV_CH), tuple(V99_STAGE_OUT_CH), 5, tuple(V99_BLOCKS), False),
 }
 VOVNET_KEYS = {spec[0]: key for key, spec in VOVNET_SPECS.items()}  # FE.BACKBONE.NAME -> arch key
-ARCH_KEYS = ("dla34", ) + tuple(VOVNET_SPECS)
+ARCH_KEYS = ("dla34", ) + tuple(VOVNET_SPECS) + tuple(k for k in DLA_SPECS if k != "dla34")
 
 
 def _vov_conv3x3(specs, n, cout, cin, dw, norm):
@@ -144,8 +172,8 @@ def param_specs(cfg):
     specs["pixel_std"] = ((3, 1, 1), "buffer")
     arch = arch_of(cfg)
     norm = backbone_norm(cfg)
-    if arch == "dla34":
-        feats = _dla34(specs, norm)
+    if arch in DLA_SPECS:
+        feats = _dla(specs, arch, norm)
         stages = {"level3": 3, "level4": 4, "level5": 5}
     else:
         feats = _vovnet(specs, arch, norm)
@@ -157,7 +185,7 @@ def param_specs(cfg):
             _conv(specs, conv, 256, cin, k, bias=fpn_norm == "", role="linear")
             _norm(specs, conv + ".norm", 256, fpn_norm)
     _conv(specs, "backbone.top_block.p6", 256, 256, 3, bias=True, role="linear")
-    if arch == "dla34":
+    if arch in DLA_SPECS:
         _conv(specs, "backbone.top_block.p7", 256, 256, 3, bias=True, role="linear")
 
     C = cfg.DD3D.NUM_CLASSES
@@ -220,13 +248,14 @@ def is_nuscenes_arch(cfg):
 
 
 def arch_of(cfg):
-    """Arch key of FE.BUILDER + FE.BACKBONE.NAME: "dla34" or a key of VOVNET_SPECS."""
+    """Arch key of FE.BUILDER + FE.BACKBONE.NAME: a key of DLA_SPECS or of VOVNET_SPECS."""
     b = cfg.FE.BUILDER
     if b == "build_fcos_dla_fpn_backbone_p67":
         name = cfg.FE.BACKBONE.NAME
-        if name != "DLA-34":  # dla.py builds DLA-46-C, DLA-60, ... too: Bottleneck / BottleneckX blocks the engine lacks
-            raise NotImplementedError(f"DLA variant {name!r} is not supported: only DLA-34 is built by the engine")
-        return "dla34"
+        if name not in DLA_KEYS:  # dla.py also builds DLA-46-C, DLA-60, DLA-102, DLA-169: plain Bottleneck blocks
+            raise NotImplementedError(f"DLA variant {name!r} is not supported: the engine builds "
+                                      + ", ".join(DLA_KEYS))
+        return DLA_KEYS[name]
     if b == "build_fcos_vovnet_fpn_backbone_p6":
         return VOVNET_KEYS[cfg.FE.BACKBONE.NAME]  # KeyError for an unknown name, like _STAGE_SPECS[cfg.NAME]
     raise KeyError("No object named '{}' found in 'BACKBONE' registry!".format(b))
@@ -240,14 +269,14 @@ def backbone_norm(cfg):
     at construction."""
     norm = cfg.FE.BACKBONE.NORM
     _norm({}, "", 32, norm)  # KeyError for an unknown NORM
-    if norm == "" and arch_of(cfg) != "dla34":
+    if norm == "" and arch_of(cfg) not in DLA_SPECS:
         raise TypeError("'NoneType' object is not callable")
     return norm
 
 
 def level_strides(cfg):
-    return [8, 16, 32, 64, 128] if arch_of(cfg) == "dla34" else [4, 8, 16, 32, 64]
+    return [8, 16, 32, 64, 128] if arch_of(cfg) in DLA_SPECS else [4, 8, 16, 32, 64]
 
 
 def size_divisibility(cfg):
-    return 128 if arch_of(cfg) == "dla34" else 64
+    return 128 if arch_of(cfg) in DLA_SPECS else 64

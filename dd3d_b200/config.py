@@ -9,7 +9,7 @@ eval-mode BN in FCOS2D, NMS_THRESH 0.75).
 """
 import copy
 
-from .arch import VOVNET_SPECS
+from .arch import DLA_SPECS, VOVNET_SPECS
 
 
 class CfgNode(dict):
@@ -88,11 +88,17 @@ for _key, _spec in VOVNET_SPECS.items():
     if _key not in _FEATURE_EXTRACTORS:
         _FEATURE_EXTRACTORS[_key] = copy.deepcopy(_FEATURE_EXTRACTORS["v2_99"])
         _FEATURE_EXTRACTORS[_key]["BACKBONE"]["NAME"] = _spec[0]
+# the DLA-X networks of dla.py:DLA_NAME_TO_BUILDER: DLA-34's builder, FPN and outputs, FE.BACKBONE.NAME picks the network
+for _key, _spec in DLA_SPECS.items():
+    if _key not in _FEATURE_EXTRACTORS:
+        _FEATURE_EXTRACTORS[_key] = copy.deepcopy(_FEATURE_EXTRACTORS["dla34"])
+        _FEATURE_EXTRACTORS[_key]["BACKBONE"]["NAME"] = _spec[0]
 
 
 def get_cfg(backbone="dla34", dataset="kitti_3d", nms_thresh=0.75, meta_arch="DD3D", act_dtype="bf16"):
-    """backbone: "dla34" or a VoVNet key of dd3d_b200.arch.VOVNET_SPECS ("v2_19_slim_dw", "v2_19_dw", "v2_19_slim", "v2_19",
-    "v2_39", "v2_57", "v2_99"), which sets FE.BACKBONE.NAME; dataset in {"kitti_3d", "nuscenes"} (head constants only); meta_arch in
+    """backbone: a DLA key of dd3d_b200.arch.DLA_SPECS ("dla34", "dla_x_46_c", "dla_x_60_c", "dla_x_60", "dla_x_102",
+    "dla_x_102_64") or a VoVNet key of VOVNET_SPECS ("v2_19_slim_dw", "v2_19_dw", "v2_19_slim", "v2_19", "v2_39", "v2_57",
+    "v2_99"), which sets FE.BACKBONE.NAME; dataset in {"kitti_3d", "nuscenes"} (head constants only); meta_arch in
     {"DD3D", "NuscenesDD3D"} (configs/experiments/dd3d_nusc_{dla34,v99}.yaml:9,30-36)."""
     ds = _DATASETS[dataset]
     fe = copy.deepcopy(_FEATURE_EXTRACTORS[backbone])
@@ -160,7 +166,7 @@ def get_cfg(backbone="dla34", dataset="kitti_3d", nms_thresh=0.75, meta_arch="DD
         B200=dict(ACT_DTYPE=act_dtype),
         # test-time augmentation: configs/experiments/dd3d_kitti_{dla34,v99}.yaml:47-53, dd3d_nusc_v99.yaml:57-63
         # IMS_PER_BATCH: dd3d_kitti_*.yaml 80, dd3d_nusc_dla34.yaml 96, dd3d_nusc_v99.yaml 192
-        TEST=dict(IMS_PER_BATCH=80 if dataset == "kitti_3d" else (96 if backbone == "dla34" else 192),
+        TEST=dict(IMS_PER_BATCH=80 if dataset == "kitti_3d" else (96 if backbone in DLA_SPECS else 192),
                   AUG=dict(ENABLED=True,
                            MIN_SIZES=[320, 384, 448, 512, 576] if dataset == "kitti_3d" else [640, 768, 896, 1024, 1152],
                            MAX_SIZE=100000, FLIP=True)),

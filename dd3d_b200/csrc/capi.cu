@@ -287,7 +287,7 @@ int dd3d_get_conv_info(dd3d_handle h, int32_t* h_info, int max_ops) {
             for (int i = 0; i < 8; ++i) r[i] = 0;
             if (op.type != Op::CONV) continue;
             const ConvParams& p = op.conv;
-            const int v[8] = {1, p.taps, p.stride, p.cin, p.block_n * p.n_blocks, p.halo ? 1 : 0, p.pair, p.block_n};
+            const int v[8] = {p.grouped ? 2 : 1, p.taps, p.stride, p.cin, p.block_n * p.n_blocks, p.halo ? 1 : 0, p.pair, p.block_n};
             for (int i = 0; i < 8; ++i) r[i] = v[i];
         }
     });
@@ -445,6 +445,58 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
         cudaFree(d_w_taps);
     }
     return st;
+}
+
+int dd3d_op_conv2d_grouped(const void* d_in, int B, int H, int W, int C, int in_pitch, const void* d_w, int groups,
+                           int stride, const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch,
+                           dd3d_stream stream) {
+    if (!d_in || !d_w || !d_scale || !d_bias || !d_out) return DD3D_ERR_INVALID;
+    if (B < 1 || H < 1 || W < 1 || C < kBlockK || C % kBlockK || groups < 1 || C % groups || kBlockK % (C / groups) ||
+        in_pitch < C || out_pitch < C || (in_pitch | out_pitch) & 7)
+        return DD3D_ERR_INVALID;
+    if ((stride != 1 && stride != 2) || (stride == 2 && ((H | W) & 1))) return DD3D_ERR_INVALID;
+    ConvParams p;
+    memset(&p, 0, sizeof(p));
+    p.nseg = 1;
+    p.B = B;
+    p.taps = 9;
+    p.stride = stride;
+    p.kchunks = 1;
+    p.cin = C;
+    p.block_n = kBlockK;
+    p.n_blocks = C / kBlockK;
+    p.relu = relu;
+    p.fp16 = g_op_fp16;
+    p.grouped = 1;
+    ConvSeg& g = p.seg[0];
+    const int Ho = H / stride, Wo = W / stride;
+    g.H = Ho;
+    g.W = Wo;
+    choose_tile(Ho, Wo, &g.th, &g.tw);
+    bool ok = true;
+    p.halo = conv_prefer_halo(9, stride, kBlockK, 1, &Ho, &Wo) ? conv_halo_mode() : 0;
+    if (p.halo) {
+        g.th = kHaloTh;
+        g.tw = kHaloTw;
+        ok = make_act_map_halo(&g.in_map[0], d_in, B, H, W, C, in_pitch, g_op_fp16);
+    } else if (stride == 1) {
+        ok = make_act_map(&g.in_map[0], d_in, B, H, W, C, in_pitch, g.th, g.tw, g_op_fp16);
+    } else {
+        ok = make_act_map_s2(&g.in_map[0], d_in, 0, B, H, W, C, in_pitch, g.th, g.tw, g_op_fp16) &&
+             make_act_map_s2(&g.in_map[1], d_in, 1, B, H, W, C, in_pitch, g.th, g.tw, g_op_fp16);
+    }
+    ok = ok && make_act_map(&g.out_map, d_out, B, Ho, Wo, C, out_pitch, g.th, g.tw, g_op_fp16) &&
+         make_weight_map(&p.w_map, d_w, 9 * kBlockK, C, kBlockK, g_op_fp16);
+    if (!ok) {
+        fprintf(stderr, "dd3d_op_conv2d_grouped: %s\n", conv_last_error());
+        return DD3D_ERR_CUDA;
+    }
+    g.scale = d_scale;
+    g.bias = d_bias;
+    g.out16 = d_out;
+    g.out_pitch = out_pitch;
+    conv_finalize_params(&p);
+    return cuda_status(launch_conv(p, device_sms(), static_cast<cudaStream_t>(stream)), nullptr);
 }
 
 int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,

@@ -451,6 +451,8 @@ cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
     ConvKernel kernel = nullptr;
     const bool list = p.tile_list != nullptr;  // list mode: pair tile or taps-in-N
     if (list && ((!p.pair && !p.taps_n) || p.tile_count == nullptr)) return cudaErrorInvalidValue;
+    if (p.grouped && (p.block_n != kBlockK || p.kchunks != 1 || p.pair || p.taps_n || (p.wstat && p.n_blocks != 1)))
+        return cudaErrorInvalidValue;  // block-diagonal mode: one 64-channel k-block per 64-channel n-block
     if (p.pair) {
         if (!p.halo || p.block_n != 128 || p.out_mode != 0) return cudaErrorInvalidValue;
         kernel = conv_kernel_pair(p.fp16 != 0, list);

@@ -59,6 +59,10 @@ struct ConvParams {
     int wstat;        // 1: weight-stationary halo variant -- all taps * kchunks weight blocks resident in shared memory
     int a_stages;     // halo variants: A patches in flight (3, or up to 5 with wstat; 2 pairs of patches with pair)
     int pair;         // 1: pair-tile halo variant -- work item = two 16x8 tiles x one 128-channel n-block (conv_select_pair)
+    // 1: block-diagonal grouped 3x3 (ResNeXt conv2 with channels per group dividing 64): block_n 64, kchunks 1, and the A
+    // operand of n-block j is input channels [64 j, 64 j + 64) -- the only channels its 64 output channels read.  Weights
+    // [cout][9][64] hold each row's group at its position in the 64-channel block and zeros elsewhere (exact zeros).
+    int grouped;
     // Work-list mode (nullptr: every tile of every segment).  The M units are the entries of tile_list (pair tile: entries
     // 2i, 2i + 1 form unit i and must lie in one segment), each (seg << 29) | (img << 16) | (row-major tile of the image);
     // *tile_count entries, read on the device after griddepcontrol.wait.  total_work then only sizes the grid.

@@ -283,6 +283,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                 }
                 continue;
             }
+            const int a_c0 = p.grouped ? t.n_blk * kBlockK : 0;  // block-diagonal: n-block j reads channels 64 j..
             for (int tap = 0; tap < p.taps; ++tap) {
                 const int r = (p.taps == 9) ? tap / 3 : 1;
                 const int s = (p.taps == 9) ? tap - 3 * (tap / 3) : 1;
@@ -292,7 +293,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                         uint8_t* a_dst = smem + stage * stage_bytes;
                         ptx::mbar_expect_tx(&full_bar[stage], kABytes);  // the weight tile is armed + issued by warp 2
                         if (p.stride == 1) {
-                            ptx::tma_load_4d(a_dst, &g.in_map[0], &full_bar[stage], kc * kBlockK, t.x0 + s - 1,
+                            ptx::tma_load_4d(a_dst, &g.in_map[0], &full_bar[stage], a_c0 + kc * kBlockK, t.x0 + s - 1,
                                              t.y0 + r - 1, t.img);
                         } else {
                             // stride 2: input (2*oy + r - 1, 2*ox + s - 1) in the parity-split view [B][H/2][2][W/2][wp*C..]
@@ -300,7 +301,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                             const int dw = (s == 0) ? -1 : 0;
                             const int hp = (r == 1) ? 0 : 1;
                             const int dh = (r == 0) ? -1 : 0;
-                            ptx::tma_load_5d(a_dst, &g.in_map[wp], &full_bar[stage], kc * kBlockK, t.x0 + dw, hp,
+                            ptx::tma_load_5d(a_dst, &g.in_map[wp], &full_bar[stage], a_c0 + kc * kBlockK, t.x0 + dw, hp,
                                              t.y0 + dh, t.img);
                         }
                     }
@@ -343,11 +344,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                 const TileCoord t = decode_tile<PAIR, LIST>(p, work);
                 const TileCoord t1 = PAIR ? decode_tile<PAIR, LIST>(p, work, 1) : t;
                 const ConvSeg& g = p.seg[t.seg];
+                const int a_c0 = p.grouped ? t.n_blk * kBlockK : 0;  // block-diagonal: n-block j reads channels 64 j..
                 for (int kc = 0; kc < p.kchunks; ++kc) {
                     ptx::mbar_wait(&aempty_bar[as], aphase ^ 1);
                     if (elect_one()) {
                         ptx::mbar_expect_tx(&afull_bar[as], MH * kHaloPW * kHaloPH * 128);
-                        ptx::tma_load_4d(halo_a + as * kASlot, &g.in_map[0], &afull_bar[as], kc * kBlockK, t.x0 - 1,
+                        ptx::tma_load_4d(halo_a + as * kASlot, &g.in_map[0], &afull_bar[as], a_c0 + kc * kBlockK, t.x0 - 1,
                                          t.y0 - 1, t.img);
                         if (PAIR)
                             ptx::tma_load_4d(halo_a + as * kASlot + kHaloABytes, &g.in_map[0], &afull_bar[as], kc * kBlockK,

@@ -1,7 +1,7 @@
-// DD3D inference engine: weight folding/packing, static graph for DLA-34 / every VoVNetV2-eSE variant + FPN + FCOS2D/3D
+// DD3D inference engine: weight folding/packing, static graph for DLA-34 and DLA-X / every VoVNetV2-eSE variant + FPN + FCOS2D/3D
 // heads, workspace planning and the forward launch sequence.  Reference structure being reproduced:
 //   DD3D.forward                      tridet/modeling/dd3d/core.py:64-164
-//   DLA-34                            tridet/modeling/feature_extractor/dla.py:24-62,146-247,250-361
+//   DLA-34, DLA-X-{46-C,60-C,60,102,102-64}  tridet/modeling/feature_extractor/dla.py:24-62,104-247,250-441
 //   VoVNetV2-{19-slim-dw,19-dw,19-slim,19,39,57,99}-eSE   tridet/modeling/feature_extractor/vovnet.py:19-143,173-273,276-367
 //   FPN + LastLevelP6P7 / LastLevelP6 detectron2 (SURVEY.md Appendix A), dla.py:537-561, vovnet.py:411-454
 //   FCOS2DHead / FCOS3DHead           fcos2d.py:30-156, fcos3d.py:55-188 (+ normalization.py Scale/Offset/ModuleListDial)
@@ -37,7 +37,7 @@ void cuda_check(cudaError_t e, const char* what) {
 // ================================================================================================ Engine basics
 
 Engine::Engine(const dd3d_model_desc& d) : desc(d) {
-    if (d.arch != DD3D_ARCH_DLA34 && vovnet_spec(d.arch) == nullptr) fail(DD3D_ERR_INVALID, "unknown arch");
+    if (dla_spec(d.arch) == nullptr && vovnet_spec(d.arch) == nullptr) fail(DD3D_ERR_INVALID, "unknown arch");
     if (d.num_classes < 1 || d.num_classes > DD3D_MAX_CLASSES) fail(DD3D_ERR_INVALID, "num_classes out of range");
     if (d.pre_nms_topk < 1 || d.pre_nms_topk * kLevels > 8192) fail(DD3D_ERR_INVALID, "pre_nms_topk out of range");
     if (d.out_cap < 1) fail(DD3D_ERR_INVALID, "out_cap must be positive");
@@ -173,6 +173,42 @@ const DwLayer& Engine::dw_layer(const std::string& wname, int C) {
     return dws.emplace(wname, L).first->second;
 }
 
+// Grouped 3x3 weights [C][C / groups][3][3] (groups dividing C, channels per group dividing 64) -> 16-bit [C][9][64] for the
+// block-diagonal mode of the implicit-GEMM kernel: row co holds its group's input channels at their position inside the
+// 64-channel block of co, zeros elsewhere.
+const ConvLayer& Engine::grouped_conv_layer(const std::string& wname, int C, int groups) {
+    auto it = convs.find(wname);
+    if (it != convs.end()) return it->second;
+    const HostTensor& w = weight(wname + ".weight");
+    const int cpg = groups > 0 ? C / groups : 0;
+    if (groups < 1 || C % groups || C % kBlockK || cpg < 1 || kBlockK % cpg || w.shape.size() != 4 || w.shape[0] != C ||
+        w.shape[1] != cpg || w.shape[2] != 3 || w.shape[3] != 3)
+        fail(DD3D_ERR_INVALID, "bad grouped conv weight shape: " + wname);
+    ConvLayer L;
+    L.cin = C;
+    L.cout = C;
+    L.cout_pad = C;
+    L.ksize = 3;
+    L.taps = 9;
+    L.kchunks = 1;
+    L.ktot = 9 * kBlockK;
+    L.block_n = kBlockK;
+    L.n_blocks = C / kBlockK;
+    L.groups = groups;
+    std::vector<uint16_t> packed(static_cast<size_t>(C) * L.ktot, 0);
+    for (int co = 0; co < C; ++co) {
+        const int ci0 = (co / cpg) * cpg % kBlockK;  // the group's first input channel inside co's 64-channel block
+        for (int ci = 0; ci < cpg; ++ci)
+            for (int t = 0; t < 9; ++t)
+                packed[(static_cast<size_t>(co) * 9 + t) * kBlockK + ci0 + ci] =
+                    host_f32_to_act(w.data[(static_cast<size_t>(co) * cpg + ci) * 9 + t], fp16);
+    }
+    L.d_w = static_cast<__nv_bfloat16*>(dev_alloc(packed.size() * 2));
+    cuda_check(cudaMemcpy(L.d_w, packed.data(), packed.size() * 2, cudaMemcpyHostToDevice), "upload grouped conv weights");
+    if (!make_weight_map(&L.w_map, L.d_w, L.ktot, L.cout_pad, L.block_n, fp16)) fail(DD3D_ERR_CUDA, conv_last_error());
+    return convs.emplace(wname, L).first->second;
+}
+
 void Engine::set_layout(const dd3d_layout_desc& l) {
     if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_layout after finalize");
     for (int n : {l.fcos2d_norm, l.fcos3d_norm, l.fpn_norm})
@@ -186,9 +222,9 @@ void Engine::set_layout(const dd3d_layout_desc& l) {
 void Engine::set_backbone_norm(int norm) {
     if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_backbone_norm after finalize");
     if (norm < DD3D_NORM_BN_PER_LEVEL || norm > DD3D_NORM_NONE) fail(DD3D_ERR_INVALID, "unknown dd3d_norm value");
-    const bool dla = desc.arch == DD3D_ARCH_DLA34;
-    // DLA-34's 16-channel convs cannot take GroupNorm(32, C); a VoVNet without a norm fails in the reference's forward
-    if (dla && norm == DD3D_NORM_GN) fail(DD3D_ERR_INVALID, "DLA-34 has no GroupNorm backbone (16 channels)");
+    const bool dla = dla_spec(desc.arch) != nullptr;
+    // the 16-channel base_layer of every DLA cannot take GroupNorm(32, C); a VoVNet without a norm fails in the reference's forward
+    if (dla && norm == DD3D_NORM_GN) fail(DD3D_ERR_INVALID, "a DLA has no GroupNorm backbone (16 channels)");
     if (!dla && norm == DD3D_NORM_NONE) fail(DD3D_ERR_INVALID, "a VoVNet backbone needs a norm");
     if (!dla && norm == DD3D_NORM_GN) {  // GroupNorm(32, C) of every stem, OSA, concat and reduction conv
         const VovSpec& S = *vovnet_spec(desc.arch);
@@ -288,6 +324,24 @@ const VovSpec* vovnet_spec(int arch) {
     return nullptr;
 }
 
+// The DLA networks of the reference's DLA_NAME_TO_BUILDER (dla.py:358-441) that the engine builds.  DLA-X-102-64 is
+// dla102x2, which sets BottleneckX.cardinality = 64 (dla.py:411).  dd3d_b200/arch.py keeps the copy param_specs needs.
+static const DlaSpec kDlaSpecs[] = {
+    // arch                    levels                channels                          bottleneck_x root_res  cardinality
+    {DD3D_ARCH_DLA34, {1, 1, 1, 2, 2, 1}, {16, 32, 64, 128, 256, 512}, false, false, 0},
+    {DD3D_ARCH_DLA_X_46_C, {1, 1, 1, 2, 2, 1}, {16, 32, 64, 64, 128, 256}, true, false, 32},
+    {DD3D_ARCH_DLA_X_60_C, {1, 1, 1, 2, 3, 1}, {16, 32, 64, 64, 128, 256}, true, false, 32},
+    {DD3D_ARCH_DLA_X_60, {1, 1, 1, 2, 3, 1}, {16, 32, 128, 256, 512, 1024}, true, false, 32},
+    {DD3D_ARCH_DLA_X_102, {1, 1, 1, 3, 4, 1}, {16, 32, 128, 256, 512, 1024}, true, true, 32},
+    {DD3D_ARCH_DLA_X_102_64, {1, 1, 1, 3, 4, 1}, {16, 32, 128, 256, 512, 1024}, true, true, 64},
+};
+
+const DlaSpec* dla_spec(int arch) {
+    for (const DlaSpec& s : kDlaSpecs)
+        if (s.arch == arch) return &s;
+    return nullptr;
+}
+
 struct Builder {
     Engine* E;
     Plan* P;
@@ -374,6 +428,7 @@ struct Builder {
         p.relu = relu ? 1 : 0;
         p.out_mode = f32_out ? 1 : 0;
         p.fp16 = E->fp16;
+        p.grouped = L.groups > 1 ? 1 : 0;
         {
             int hs[kMaxSeg], ws[kMaxSeg];
             for (int s = 0; s < p.nseg; ++s) {
@@ -437,9 +492,11 @@ struct Builder {
         // A tiles it re-reads are tiny; K order per output element is unchanged, so results are bit-identical.
         // Filled halo layers with 128-multiple widths (FCOS towers, FPN outputs, VoVNet stage 2) run the 256 x 128 pair tile:
         // half the weight traffic per MAC, same K order -> bit-identical.
-        const bool pair = conv_select_pair(&p, L.cout_pad, E->num_sms);
+        // Grouped layers (block-diagonal mode) keep block_n 64, one k-block per n-block: no pair tile, no N-split (the weight-
+        // stationary variant still applies to a single n-block, conv_finalize_params)
+        const bool pair = !p.grouped && conv_select_pair(&p, L.cout_pad, E->num_sms);
         bool n_split = false;
-        if (!p.taps_n && !pair && conv_n_split_enabled()) {
+        if (!p.taps_n && !pair && !p.grouped && conv_n_split_enabled()) {
             int tiles = 0;
             for (int s = 0; s < p.nseg; ++s)
                 tiles += B * ((p.seg[s].H + p.seg[s].th - 1) / p.seg[s].th) * ((p.seg[s].W + p.seg[s].tw - 1) / p.seg[s].tw);
@@ -459,7 +516,7 @@ struct Builder {
             p.w_map = p.taps_n ? L.w_map_taps : L.w_map;
         }
         for (int s = 0; s < p.nseg; ++s)
-            op.flops += 2.0 * B * p.seg[s].H * p.seg[s].W * static_cast<double>(L.cout) * L.cin * L.taps;
+            op.flops += 2.0 * B * p.seg[s].H * p.seg[s].W * static_cast<double>(L.cout) * (L.cin / L.groups) * L.taps;  // useful MACs
         if (!f32_out) {
             op.nouts = p.nseg;
             for (int s = 0; s < p.nseg; ++s) op.outs[s] = segs[s].out;
@@ -557,8 +614,8 @@ struct Builder {
         P->ops.push_back(op);
     }
 
-    // ---- DLA-34 -------------------------------------------------------------------------------------------
-    // DLA-34 conv -> norm: the folded BN, or with FE.BACKBONE.NORM "" the conv's own bias (Conv2d(bias=norm == ""), dla.py:33,44,
+    // ---- DLA (DLA-34 and the DLA-X networks of kDlaSpecs) ---------------------------------------------------------
+    // DLA conv -> norm: the folded BN, or with FE.BACKBONE.NORM "" the conv's own bias (Conv2d(bias=norm == ""), dla.py:33,44,
     // 154,230,277,337).  Returns the (BN prefix, bias name) pair bn_fold takes.
     std::pair<std::string, std::string> dla_norm(const std::string& conv) const {
         if (E->backbone_norm == DD3D_NORM_NONE) return {"", conv + ".bias"};
@@ -575,9 +632,54 @@ struct Builder {
         dla_conv(p + ".conv1", x, t, 3, stride, true);
         dla_conv(p + ".conv2", t, dst, 3, 1, true, &residual);
     }
-    // Tree with levels == 1 (dla.py:170-247): `rc` is the Root's concat buffer, laid out [x2 | x1 | children...]
-    // with the children already in place; `bottom` is the (pooled) input the optional `project` acts on.
-    void dla_tree1(const std::string& p, View x, int in_ch, int out_ch, int stride, View rc, View bottom, View dst) {
+    // BottleneckX (dla.py:104-143): 1x1 -> BN -> ReLU -> grouped 3x3 (stride) -> BN -> ReLU -> 1x1 -> BN -> (+residual) -> ReLU;
+    // bottleneck width planes * cardinality / 32
+    void dla_block_x(const std::string& p, View x, int stride, View residual, View dst, int cardinality) {
+        const int width = dst.C * cardinality / 32;
+        View t1 = alloc(x.H, x.W, width);
+        dla_conv(p + ".conv1", x, t1, 1, 1, true);
+        View t2 = alloc(x.H / stride, x.W / stride, width);
+        const auto nb = dla_norm(p + ".conv2");
+        const ConvLayer& L = E->grouped_conv_layer(p + ".conv2", width, cardinality);
+        const Epilogue& e = E->bn_epilogue(p + ".conv2|" + nb.first, nb.first, nb.second, width);
+        std::vector<SegSpec> segs(1);
+        segs[0].in = t1;
+        segs[0].out = t2;
+        segs[0].epi = &e;
+        conv(L, stride, true, segs, false);
+        dla_conv(p + ".conv3", t2, dst, 1, 1, true, &residual);
+    }
+    // Tree (dla.py:170-247) of `levels` levels, output into *dst (a new buffer when dst is null, allocated where DLA-34's
+    // hand-written builder allocated it, so that its ops and workspace plan are unchanged).  `rc` is the Root concat of the
+    // levels-1 tree at the end of this tree's tree2 chain, laid out [x2 | x1 | bottom (level_root) | x1 of each enclosing
+    // tree, outermost first]; `child` is the channel of this tree's first child slot in it.  `pooled`: x max-pooled by
+    // `stride` when the caller has it already (every nested tree1 pools the same tensor as its parent, dla.py:235).
+    View dla_tree(const std::string& p, View x, int levels, int in_ch, int out_ch, int stride, bool level_root, View rc,
+                  int child, const View* pooled, const View* dst) {
+        const DlaSpec& S = *dla_spec(E->desc.arch);
+        const int Ho = x.H / stride, Wo = x.W / stride;
+        View bottom = x;
+        if (level_root) {
+            if (pooled != nullptr || stride != 2) fail(DD3D_ERR_INVALID, "DLA level_root tree without its own pool: " + p);
+            bottom = slice(rc, child, in_ch);
+            maxpool(x, bottom, 2);
+            child += in_ch;
+        } else if (stride > 1) {
+            if (pooled != nullptr) {
+                bottom = *pooled;
+            } else {
+                bottom = alloc(Ho, Wo, in_ch);
+                maxpool(x, bottom, stride);
+            }
+        }
+        if (levels > 1) {
+            View t1 = slice(rc, child, out_ch);
+            View rc1 = alloc(Ho, Wo, levels * out_ch);  // tree1's own chain: [x2 | x1 | one x1 per level below]
+            dla_tree(p + ".tree1", x, levels - 1, in_ch, out_ch, stride, false, rc1, 2 * out_ch, stride > 1 ? &bottom : nullptr,
+                     &t1);
+            return dla_tree(p + ".tree2", t1, levels - 1, out_ch, out_ch, 1, false, rc, child + out_ch, nullptr, dst);
+        }
+        View out = dst != nullptr ? *dst : alloc(Ho, Wo, out_ch);
         View residual = bottom;
         if (in_ch != out_ch) {
             residual = alloc(bottom.H, bottom.W, out_ch);
@@ -585,29 +687,30 @@ struct Builder {
         }
         View x1 = slice(rc, out_ch, out_ch);
         View x2 = slice(rc, 0, out_ch);
-        dla_block(p + ".tree1", x, stride, residual, x1);
-        dla_block(p + ".tree2", x1, 1, x1, x2);
-        dla_conv(p + ".root.conv", rc, dst, 1, 1, true);  // Root: cat -> 1x1 -> BN -> ReLU
-    }
-    // Tree with levels == 2 and level_root (level3 / level4, dla.py:309-314)
-    View dla_tree2(const std::string& p, View x, int in_ch, int out_ch) {
-        const int Ho = x.H / 2, Wo = x.W / 2;
-        View rc2 = alloc(Ho, Wo, 3 * out_ch + in_ch);  // [x2 | x1 | bottom | tree1-out]   (dla.py:235-245)
-        View bottom = slice(rc2, 2 * out_ch, in_ch);
-        View t1_out = slice(rc2, 2 * out_ch + in_ch, out_ch);
-        maxpool(x, bottom, 2);  // outer and inner Tree pool the same tensor (dla.py:235) -> computed once
-        View rc1 = alloc(Ho, Wo, 2 * out_ch);
-        dla_tree1(p + ".tree1", x, in_ch, out_ch, 2, rc1, bottom, t1_out);
-        View out = alloc(Ho, Wo, out_ch);
-        dla_tree1(p + ".tree2", t1_out, out_ch, out_ch, 1, rc2, t1_out, out);
+        if (S.bottleneck_x) {
+            dla_block_x(p + ".tree1", x, stride, residual, x1, S.cardinality);
+            dla_block_x(p + ".tree2", x1, 1, x1, x2, S.cardinality);
+        } else {
+            dla_block(p + ".tree1", x, stride, residual, x1);
+            dla_block(p + ".tree2", x1, 1, x1, x2);
+        }
+        // Root: cat -> 1x1 -> BN (-> + x2 with residual_root) -> ReLU; x2 is the concat's first slice
+        dla_conv(p + ".root.conv", rc, out, 1, 1, true, S.root_residual ? &x2 : nullptr);
         return out;
     }
+    // DLA level 2..5: Tree(levels, channels[l-1] -> channels[l], stride 2, level_root = l > 2) with its root concat
+    View dla_level(const std::string& p, View x, int levels, int in_ch, int out_ch, bool level_root, const View* pooled) {
+        View rc = alloc(x.H / 2, x.W / 2, (levels + 1) * out_ch + (level_root ? in_ch : 0));
+        return dla_tree(p, x, levels, in_ch, out_ch, 2, level_root, rc, 2 * out_ch, pooled, nullptr);
+    }
 
-    void build_dla34(View input, std::vector<View>* feats) {
+    void build_dla(View input, std::vector<View>* feats) {
+        const DlaSpec& S = *dla_spec(E->desc.arch);
         const std::string p = "backbone.bottom_up";
         const int H = input.H, W = input.W;
         // both forms of the front end are packed at finalize (host weights are dropped afterwards), so that the
-        // "dla_front" option can be flipped on a finalized engine
+        // "dla_front" option can be flipped on a finalized engine.  base_layer / level0 / level1 have DLA-34's shapes in
+        // every variant (channels 16, 16, 32).
         const FrontLayer& F = E->front_layer(p);
         const auto n0 = dla_norm(p + ".base_layer"), n1 = dla_norm(p + ".level0.0"), n2 = dla_norm(p + ".level1.0");
         E->stem_layer(p + ".base_layer", n0.first, n0.second, 7, 1);
@@ -632,19 +735,13 @@ struct Builder {
             bottom = alloc(H / 4, W / 4, 32);
             maxpool(a2, bottom, 2);
         }
-        // level2: Tree(levels=1, 32->64, stride 2)
-        View rc = alloc(H / 4, W / 4, 128);
-        View l2 = alloc(H / 4, W / 4, 64);
-        dla_tree1(p + ".level2", a2, 32, 64, 2, rc, bottom, l2);
-        View l3 = dla_tree2(p + ".level3", l2, 64, 128);
-        View l4 = dla_tree2(p + ".level4", l3, 128, 256);
-        // level5: Tree(levels=1, 256->512, stride 2, level_root) -> root input [x2 | x1 | bottom]
-        View rc5 = alloc(H / 32, W / 32, 1280);
-        View bottom5 = slice(rc5, 1024, 256);
-        maxpool(l4, bottom5, 2);
-        View l5 = alloc(H / 32, W / 32, 512);
-        dla_tree1(p + ".level5", l4, 256, 512, 2, rc5, bottom5, l5);
-        feats->assign({l3, l4, l5});
+        const int* ch = S.channels;
+        View x = dla_level(p + ".level2", a2, S.levels[2], ch[1], ch[2], false, &bottom);
+        feats->clear();
+        for (int l = 3; l <= 5; ++l) {
+            x = dla_level(p + ".level" + std::to_string(l), x, S.levels[l], ch[l - 1], ch[l], true, nullptr);
+            feats->push_back(x);
+        }
     }
 
     void front(const FrontLayer& F, View in4, View out, View pooled) {
@@ -902,7 +999,7 @@ struct Builder {
         persist(p6);
         conv1(p + ".top_block.p6", "", true, p5, p6, 3, 2, false);
         outs->push_back(p6);
-        if (E->desc.arch == DD3D_ARCH_DLA34) {
+        if (dla_spec(E->desc.arch) != nullptr) {  // LastLevelP6P7
             View r6 = alloc(p6.H, p6.W, 256);
             relu(p6, r6);
             View p7 = alloc(p6.H / 2, p6.W / 2, 256);
@@ -1343,7 +1440,7 @@ const EseLayer& Engine::ese_layer(const std::string& fc, int C) {
 
 // ================================================================================================ plan / forward
 
-int Engine::size_divisibility() const { return desc.arch == DD3D_ARCH_DLA34 ? 128 : 64; }
+int Engine::size_divisibility() const { return dla_spec(desc.arch) != nullptr ? 128 : 64; }
 
 // Offsets for the activation buffers: largest first, each at the lowest address where it does not collide (in address
 // AND lifetime) with an already placed one -- the greedy interval packing of static memory planners.  Without reuse
@@ -1416,8 +1513,8 @@ size_t Engine::build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry) 
         bld.off += round_up_sz(static_cast<size_t>(B) * Hp * Wp * 4 * 2, 1024);
         P->input = input;
         std::vector<View> feats, fpn;
-        if (desc.arch == DD3D_ARCH_DLA34) {
-            bld.build_dla34(input, &feats);
+        if (dla_spec(desc.arch) != nullptr) {
+            bld.build_dla(input, &feats);
             bld.build_fpn(feats, 3, &fpn);
         } else {
             bld.build_vovnet(*vovnet_spec(desc.arch), input, &feats);
@@ -1527,7 +1624,7 @@ void Engine::make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes) {
     memset(&dp, 0, sizeof(dp));
     static const int strides_dla[5] = {8, 16, 32, 64, 128};
     static const int strides_vov[5] = {4, 8, 16, 32, 64};
-    const int* strides = desc.arch == DD3D_ARCH_DLA34 ? strides_dla : strides_vov;
+    const int* strides = dla_spec(desc.arch) != nullptr ? strides_dla : strides_vov;
     for (int l = 0; l < kLevels; ++l) {
         dp.lvl[l].cls = plan.cls_map[l];
         dp.lvl[l].box = plan.box_map[l];

@@ -46,6 +46,7 @@ struct ArenaBuf {
 
 struct ConvLayer {
     int cin, cout, ksize, taps, kchunks, ktot, cout_pad, block_n, n_blocks;
+    int groups = 1;  // > 1: grouped 3x3 packed block-diagonally for ConvParams::grouped (Engine::grouped_conv_layer)
     __nv_bfloat16* d_w;
     CUtensorMap w_map;
     __nv_bfloat16* d_w_taps = nullptr;  // taps-in-N layout [9 * 16][cin_pad64] (3x3 layers with cout_pad == 16 only)
@@ -89,6 +90,17 @@ struct VovSpec {
     bool dw;  // depthwise 3x3 layers (and stem_2 / stem_3) with 1x1 conv_reduction where in_ch != stage_ch
 };
 const VovSpec* vovnet_spec(int arch);  // nullptr: not a VoVNet arch
+
+// One DLA network the engine builds (reference DLA_NAME_TO_BUILDER, dla.py:358-441); the table is in engine.cu
+struct DlaSpec {
+    int arch;  // dd3d_arch
+    int levels[6];
+    int channels[6];
+    bool bottleneck_x;   // BottleneckX blocks (dla.py:104-143) instead of BasicBlock (dla.py:24-62)
+    bool root_residual;  // Root adds its first child before the ReLU (dla.py:160-167)
+    int cardinality;     // BottleneckX groups; its bottleneck width is planes * cardinality / 32
+};
+const DlaSpec* dla_spec(int arch);  // nullptr: not a DLA arch
 
 struct Op {
     enum Type { CONV, STEM, POOL, ESE, RELU, FRONT, DW, GN } type;
@@ -208,6 +220,7 @@ class Engine {
     const EseLayer& ese_layer(const std::string& fc, int C);
     const FrontLayer& front_layer(const std::string& prefix);
     const DwLayer& dw_layer(const std::string& wname, int C);
+    const ConvLayer& grouped_conv_layer(const std::string& wname, int C, int groups);  // (C, C / groups, 3, 3) weights
     const Epilogue& gn_affine(const std::string& prefix, int C = kGnChannels);  // GroupNorm weight / bias as d_scale / d_bias
     void set_layout(const dd3d_layout_desc& l);
     void set_backbone_norm(int norm);

@@ -14,7 +14,7 @@ NUM_LEVELS = 5
 ARCH_DLA34, ARCH_V2_99 = 0, 1
 # dd3d_arch of every arch key (dd3d_b200.arch.ARCH_KEYS)
 ARCH_IDS = {"dla34": ARCH_DLA34, "v2_99": ARCH_V2_99, "v2_19_slim_dw": 2, "v2_19_dw": 3, "v2_19_slim": 4, "v2_19": 5,
-            "v2_39": 6, "v2_57": 7}
+            "v2_39": 6, "v2_57": 7, "dla_x_46_c": 8, "dla_x_60_c": 9, "dla_x_60": 10, "dla_x_102": 11, "dla_x_102_64": 12}
 IMG_U8, IMG_F32 = 0, 1
 ACT_BF16, ACT_FP16 = 0, 1
 POSE_GLOBAL, POSE_CAMERA = 0, 1
@@ -115,6 +115,7 @@ SIGNATURES = {
     "dd3d_get_conv_info": (_I, [_P, C.POINTER(C.c_int32), _I]),
     "dd3d_get_tensor": (_I, [_P, C.c_char_p, C.POINTER(_P), C.POINTER(C.c_int32 * 6)]),
     "dd3d_op_conv2d": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _I, _I, _P]),
+    "dd3d_op_conv2d_grouped": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _I, _P, _P, _I, _P, _I, _P]),
     "dd3d_op_conv2d_tiles": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _I, _P, _I, _P, _P, _P]),
     "dd3d_op_conv2d_taps_tiles": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _I, _P, _I, _I, _P, _P, _P]),
     "dd3d_op_b3d_sparse": (_I, [C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P),

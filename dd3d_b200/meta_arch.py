@@ -467,11 +467,12 @@ class DD3DB200(nn.Module):
 
     def get_conv_info(self, max_ops=1024):
         """Per engine op of the current plan, in launch order: None, or the conv's dict(taps, stride, cin, cout_pad, halo,
-        pair, block_n) (dd3d_get_conv_info)."""
+        pair, block_n, grouped) (dd3d_get_conv_info; grouped: the block-diagonal mode of a grouped 3x3)."""
         info = (C.c_int32 * (8 * max_ops))()
         n = _lib.check(_lib.load().dd3d_get_conv_info(self._handle, info, max_ops), self._handle)
         keys = ("taps", "stride", "cin", "cout_pad", "halo", "pair", "block_n")
-        return [dict(zip(keys, info[8 * i + 1:8 * i + 8])) if info[8 * i] else None for i in range(n)]
+        return [dict(zip(keys, info[8 * i + 1:8 * i + 8]), grouped=info[8 * i] == 2) if info[8 * i] else None
+                for i in range(n)]
 
     def launches_per_forward(self):
         return _lib.load().dd3d_launches_per_forward(self._handle)

@@ -37,7 +37,9 @@ enum dd3d_status {
 
 /* FE.BUILDER build_fcos_dla_fpn_backbone_p67 with FE.BACKBONE.NAME "DLA-34", or build_fcos_vovnet_fpn_backbone_p6 with the
  * VoVNet named by FE.BACKBONE.NAME (vovnet.py:19-97): "V-99-eSE" (1), "V-19-slim-dw-eSE", "V-19-dw-eSE", "V-19-slim-eSE",
- * "V-19-eSE", "V-39-eSE", "V-57-eSE" (2..7).  Every VoVNet has FPN levels p2..p6 and a size divisibility of 64. */
+ * "V-19-eSE", "V-39-eSE", "V-57-eSE" (2..7).  Every VoVNet has FPN levels p2..p6 and a size divisibility of 64.  The DLA
+ * builder also takes "DLA-X-46-C", "DLA-X-60-C", "DLA-X-60", "DLA-X-102", "DLA-X-102-64" (8..12); every DLA has FPN levels
+ * p3..p7 and a size divisibility of 128. */
 enum dd3d_arch {
     DD3D_ARCH_DLA34 = 0,
     DD3D_ARCH_V2_99 = 1,
@@ -46,7 +48,13 @@ enum dd3d_arch {
     DD3D_ARCH_V2_19_SLIM = 4,
     DD3D_ARCH_V2_19 = 5,
     DD3D_ARCH_V2_39 = 6,
-    DD3D_ARCH_V2_57 = 7
+    DD3D_ARCH_V2_57 = 7,
+    /* DLA-X (ResNeXt-style BottleneckX blocks with a grouped 3x3; dla.py:104-143,370-415) */
+    DD3D_ARCH_DLA_X_46_C = 8,
+    DD3D_ARCH_DLA_X_60_C = 9,
+    DD3D_ARCH_DLA_X_60 = 10,
+    DD3D_ARCH_DLA_X_102 = 11,
+    DD3D_ARCH_DLA_X_102_64 = 12
 };
 enum dd3d_image_dtype { DD3D_IMG_U8 = 0, DD3D_IMG_F32 = 1 };
 /* 16-bit storage type of activations and conv weights (accumulation, BN affine, head maps, decode and NMS are fp32
@@ -241,8 +249,8 @@ int dd3d_get_profile(dd3d_handle h, double* h_ms, double* h_flops, double* h_byt
  * category and algorithmic FLOPs.  Returns the number of entries written (<= max_ops). */
 int dd3d_get_op_times(dd3d_handle h, float* h_ms, int32_t* h_cats, double* h_flops, int max_ops);
 /* Kernel choice of every engine op of the current plan, in launch order (entry i = entry i + 1 of dd3d_get_op_times): 8
- * int32 per op = {is implicit-GEMM conv, taps, stride, cin, padded cout, halo variant, pair tile, block_n}, all 0 for other
- * ops.  Returns the number of ops written (<= max_ops). */
+ * int32 per op = {implicit-GEMM conv: 1 dense, 2 grouped block-diagonal mode; taps, stride, cin, padded cout, halo variant,
+ * pair tile, block_n}, all 0 for other ops.  Returns the number of ops written (<= max_ops). */
 int dd3d_get_conv_info(dd3d_handle h, int32_t* h_info, int max_ops);
 
 /* ---- GPU input pipeline (SURVEY.md 8f row 3) ------------------------------------------------------------------
@@ -308,6 +316,16 @@ int dd3d_num_ops(dd3d_handle h);
 int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout, int ksize,
                    int stride, const float* d_scale, const float* d_bias, int relu, const void* d_residual,
                    int res_pitch, int res_up2, void* d_out, int out_pitch, int out_f32, dd3d_stream stream);
+/* dd3d_op_conv2d_grouped: grouped 3x3 conv (padding 1, C input = C output channels, `groups` groups of cpg = C / groups
+ * channels; the BottleneckX conv2 of dla.py:113-124) -> scale / bias -> ReLU when relu -> 16-bit NHWC, on the block-diagonal
+ * mode of the implicit-GEMM kernel: one launch, 64 output channels per n-block, each reading only its own 64 input channels.
+ * Needs C a multiple of 64 and cpg dividing 64 (cpg 2..32 for groups 32 / 64).  d_in / d_out: first channel of the input /
+ * output slice, pitches in channels (multiples of 8); stride 1 or 2 (even H, W).  d_w: 16-bit [C][9][64], tap = ky * 3 + kx:
+ * row co holds w[co][i][ky][kx] at column (co / cpg) * cpg % 64 + i and zeros in every other column.  d_scale / d_bias:
+ * fp32 [C].  Channels outside the output slice are not written. */
+int dd3d_op_conv2d_grouped(const void* d_in, int B, int H, int W, int C, int in_pitch, const void* d_w, int groups,
+                           int stride, const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch,
+                           dd3d_stream stream);
 /* dd3d_op_conv2d_tiles: dd3d_op_conv2d (3x3, stride 1, 16-bit output, cout a multiple of 128, no residual) on the pair-tile
  * kernel in work-list mode, the form the engine runs the sparse box3d tower in: only the 16x8 output tiles listed in d_tiles
  * are computed, every other output pixel is left untouched.  d_tiles: device uint32 entries (img << 16) | tile, tile = the
