@@ -861,13 +861,14 @@ int64_t dd3d_op_detect_scratch_bytes(int B, int pre_nms_topk) {
            static_cast<int64_t>(nms_scratch_bytes(B, pre_nms_topk, DD3D_MAX_CLASSES));
 }
 
-int dd3d_op_detect(const dd3d_model_desc* desc, int B, const int32_t* h_level_hw, const int32_t* h_strides,
-                   const float* const* d_cls, const float* const* d_box, const float* const* d_b3d, int cls_pitch,
-                   int b3d_pitch, const float* d_intrinsics, const int32_t* d_sizes, void* d_scratch, dd3d_det* d_pre_nms,
-                   int32_t* d_pre_counts, dd3d_det* d_out, int32_t* d_counts, dd3d_stream stream_) {
+int dd3d_op_detect_flags(const dd3d_model_desc* desc, int B, const int32_t* h_level_hw, const int32_t* h_strides,
+                         const float* const* d_cls, const float* const* d_box, const float* const* d_b3d, int cls_pitch,
+                         int b3d_pitch, const float* d_intrinsics, const int32_t* d_sizes, void* d_scratch,
+                         dd3d_det* d_pre_nms, int32_t* d_pre_counts, dd3d_det* d_out, int32_t* d_counts, int32_t* d_flags,
+                         dd3d_stream stream_) {
     if (!desc || !h_level_hw || !h_strides || !d_cls || !d_box || !d_b3d || !d_scratch || !d_out || !d_counts)
         return DD3D_ERR_INVALID;
-    if (desc->pre_nms_topk < 1 || desc->pre_nms_topk * kLevels > 8192) return DD3D_ERR_INVALID;
+    if (desc->pre_nms_topk < 1 || desc->pre_nms_topk > kMaxPreNmsTopk) return DD3D_ERR_INVALID;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     DecodeParams dp;
     memset(&dp, 0, sizeof(dp));
@@ -903,7 +904,17 @@ int dd3d_op_detect(const dd3d_model_desc* desc, int B, const int32_t* h_level_hw
     np.sizes = d_sizes;
     np.out = reinterpret_cast<Det*>(d_out);
     np.out_count = d_counts;
-    return cuda_status(launch_nms(np, stream), nullptr);
+    c = launch_nms(np, stream);
+    if (c == cudaSuccess && d_flags) c = cudaMemcpyAsync(d_flags, dp.flags, 4, cudaMemcpyDeviceToDevice, stream);
+    return cuda_status(c, nullptr);
+}
+
+int dd3d_op_detect(const dd3d_model_desc* desc, int B, const int32_t* h_level_hw, const int32_t* h_strides,
+                   const float* const* d_cls, const float* const* d_box, const float* const* d_b3d, int cls_pitch,
+                   int b3d_pitch, const float* d_intrinsics, const int32_t* d_sizes, void* d_scratch, dd3d_det* d_pre_nms,
+                   int32_t* d_pre_counts, dd3d_det* d_out, int32_t* d_counts, dd3d_stream stream) {
+    return dd3d_op_detect_flags(desc, B, h_level_hw, h_strides, d_cls, d_box, d_b3d, cls_pitch, b3d_pitch, d_intrinsics,
+                                d_sizes, d_scratch, d_pre_nms, d_pre_counts, d_out, d_counts, nullptr, stream);
 }
 
 }  // extern "C"

@@ -8,8 +8,10 @@
 //   1. score_hist   : s = sigmoid(logit) * sigmoid(ctr);  s > thresh  -> histogram of the float bits of s
 //   2. select       : per (image, level) find the histogram bin T holding the k-th largest score
 //   3. compact      : candidates in bins > T are certainly in the top-k ("sure"); bin == T goes to "boundary"
-//   4. finalize     : exact rank inside the boundary bin (score desc, index asc), then one thread per survivor
-//                     gathers its 4 + 11 regression values and decodes the 2-D box and the 3-D box.
+//   4. finalize     : exact rank inside the boundary bin (score desc, index asc) -- from the boundary buffer, or, when more
+//                     than kBoundaryCap candidates share that bin, by re-reading the level (select_overflow) -- then one
+//                     thread per survivor gathers its 4 + 11 regression values and decodes the 2-D box and the 3-D box.
+// The result is exactly the first PRE_NMS_TOPK candidates in (score desc, index asc) order, for every input.
 // Set semantics match `topk(sorted=False)` (fcos2d.py:312-313); order is fixed later by the NMS sort.
 #include "detect.cuh"
 #include "pdl.cuh"
@@ -32,8 +34,36 @@ __device__ __forceinline__ int find_level(const DecodeParams& p, int blk) {
     return l;
 }
 
+// key of a score above the threshold: its float bits relative to the threshold's; bin = key >> hist_shift.  Every ranked
+// score is <= 1.0f (a product of two sigmoids), so the bin stays below kHistBins (decode_finalize_params picks the shift).
+__device__ __forceinline__ uint32_t score_key(const DecodeParams& p, float s) { return __float_as_uint(s) - p.thresh_bits; }
+
 __device__ __forceinline__ int score_bin(const DecodeParams& p, float s) {
-    return static_cast<int>((__float_as_uint(s) - p.thresh_bits) >> p.hist_shift);
+    return static_cast<int>(score_key(p, s) >> p.hist_shift);
+}
+
+// Calls f(class, s) for every class of pixel `pix` (< H * W) of image b at level L whose thresholded score passes, in class
+// order; s = sigmoid(cls) * sigmoid(ctr) is the ranked score.  Pixels where no class passes alone are skipped before the
+// centerness is read (class_passes): under the sparse box2d tower their box map rows hold stale workspace.
+template <class F>
+__device__ __forceinline__ void for_each_candidate(const DecodeParams& p, const DecodeLevel& L, int b, int pix, F&& f) {
+    const size_t gp = static_cast<size_t>(b) * (L.H * L.W) + pix;
+    const float* lg = L.cls + gp * p.cls_pitch;
+    if (!class_passes(lg, p.C, p.thresh)) return;
+    const float ctr = sigmoidf(__ldg(L.box + gp * 16 + 4));
+    for (int c0 = 0; c0 < p.C; c0 += 4) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(lg + c0));
+        const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int c = c0 + j;
+            if (c < p.C) {
+                const float cs = sigmoidf(vv[j]);
+                const float s = cs * ctr;
+                if ((p.thresh_with_ctr ? s : cs) > p.thresh) f(c, s);
+            }
+        }
+    }
 }
 
 // mode 0: histogram, mode 1: compaction
@@ -53,38 +83,22 @@ __global__ void __launch_bounds__(kDenseThreads) dense_kernel(const __grid_const
     }
     int T = 0;
     if (MODE == 1) T = p.sel[bl * 4 + 0];
-    const size_t gp = static_cast<size_t>(b) * hw + pix;
-    const float* lg = L.cls + gp * p.cls_pitch;
-    // no class passing alone: no score passes either (class_passes), and the box map row may not have been computed
-    if (pix < hw && class_passes(lg, p.C, p.thresh)) {
-        const float ctr = sigmoidf(__ldg(L.box + gp * 16 + 4));
-        for (int c0 = 0; c0 < p.C; c0 += 4) {
-            const float4 v = __ldg(reinterpret_cast<const float4*>(lg + c0));
-            const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int c = c0 + j;
-                if (c < p.C) {
-                    const float cs = sigmoidf(vv[j]);
-                    const float s = cs * ctr;
-                    if ((p.thresh_with_ctr ? s : cs) > p.thresh) {
-                        const int bin = min(score_bin(p, s), kHistBins - 1);
-                        if (MODE == 0) {
-                            atomicAdd(&shist[bin], 1u);
-                        } else {
-                            const uint2 rec = make_uint2(__float_as_uint(s), static_cast<uint32_t>(pix * p.C + c));
-                            if (bin > T) {
-                                const int slot = atomicAdd(&p.counters[bl * 2 + 0], 1);
-                                if (slot < p.topk) p.sure[static_cast<size_t>(bl) * p.topk + slot] = rec;
-                            } else if (bin == T) {
-                                const int slot = atomicAdd(&p.counters[bl * 2 + 1], 1);
-                                if (slot < kBoundaryCap) p.boundary[static_cast<size_t>(bl) * kBoundaryCap + slot] = rec;
-                            }
-                        }
-                    }
+    if (pix < hw) {
+        for_each_candidate(p, L, b, pix, [&](int c, float s) {
+            const int bin = min(score_bin(p, s), kHistBins - 1);
+            if (MODE == 0) {
+                atomicAdd(&shist[bin], 1u);
+            } else {
+                const uint2 rec = make_uint2(__float_as_uint(s), static_cast<uint32_t>(pix * p.C + c));
+                if (bin > T) {
+                    const int slot = atomicAdd(&p.counters[bl * 2 + 0], 1);
+                    if (slot < p.topk) p.sure[static_cast<size_t>(bl) * p.topk + slot] = rec;
+                } else if (bin == T) {
+                    const int slot = atomicAdd(&p.counters[bl * 2 + 1], 1);
+                    if (slot < kBoundaryCap) p.boundary[static_cast<size_t>(bl) * kBoundaryCap + slot] = rec;
                 }
             }
-        }
+        });
     }
     if (MODE == 0) {
         __syncthreads();
@@ -329,9 +343,114 @@ __device__ void decode_one(const DecodeParams& p, const DecodeLevel& L, int b, i
     *out = d;
 }
 
+constexpr int kSelectThreads = 256;
+
+// Exclusive prefix sum over the CTA (kSelectThreads threads, all of them call it); *total = the sum of all v.
+__device__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* s_warp /* [kSelectThreads / 32 + 1] */, uint32_t* total) {
+    constexpr int kWarps = kSelectThreads / 32;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t acc = 0;
+        for (int w = 0; w < kWarps; ++w) {
+            const uint32_t t = s_warp[w];
+            s_warp[w] = acc;
+            acc += t;
+        }
+        s_warp[kWarps] = acc;
+    }
+    __syncthreads();
+    const uint32_t r = s_warp[warp] + incl - v;
+    *total = s_warp[kWarps];
+    __syncthreads();  // s_warp is reused by the next call
+    return r;
+}
+
+// Bin T of (image b, level l) holds more candidates than the boundary buffer (scores clustered in one bin, or tied): the CTA
+// ranks it by re-reading the level instead.  Histogram passes over the next bits of the key (11 per pass: two passes for the
+// widest bins, 2^19 ulps) narrow bin T down to the one score value V of the k-th candidate; a last pass takes every
+// candidate of bin T above V (out[0, n_above), pixel order) and the first `need_v` ties at V in index order
+// (out[n_above, need), by a CTA scan per 256-pixel chunk, which visits the (pixel, class) pairs in index order).
+// Same set as the boundary ranking (score desc, index asc); off the common path, which never has more than kBoundaryCap.
+__device__ void select_overflow(const DecodeParams& p, int b, int l, uint32_t T, int need, uint2* out) {
+    __shared__ uint32_t h[kHistBins];
+    __shared__ uint32_t s_warp[kSelectThreads / 32 + 1];
+    __shared__ uint32_t s_prefix;
+    __shared__ int s_need;
+    const DecodeLevel& L = p.lvl[l];
+    const int hw = L.H * L.W;
+    const int need_total = need;
+    uint32_t prefix = T;  // key >> shift of the candidates still in play
+    for (int shift = p.hist_shift; shift > 0;) {
+        const int bits = min(shift, 11), nshift = shift - bits;
+        const uint32_t nbins = 1u << bits;
+        for (uint32_t i = threadIdx.x; i < nbins; i += blockDim.x) h[i] = 0;
+        __syncthreads();
+        for (int pix = threadIdx.x; pix < hw; pix += blockDim.x) {
+            for_each_candidate(p, L, b, pix, [&](int, float s) {
+                const uint32_t key = score_key(p, s);
+                if ((key >> shift) == prefix) atomicAdd(&h[(key >> nshift) & (nbins - 1)], 1u);
+            });
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t cum = 0;
+            int bin = static_cast<int>(nbins) - 1;
+            for (; bin > 0; --bin) {
+                if (cum + h[bin] >= static_cast<uint32_t>(need)) break;
+                cum += h[bin];
+            }
+            s_prefix = (prefix << bits) | static_cast<uint32_t>(bin);
+            s_need = need - static_cast<int>(cum);
+        }
+        __syncthreads();
+        prefix = s_prefix;
+        need = s_need;
+        shift = nshift;
+    }
+    const uint32_t vkey = prefix;  // the k-th candidate's key; `need` ties at it are still taken
+    const int n_above = need_total - need;
+    uint32_t base_above = 0, base_tie = 0;
+    for (int p0 = 0; p0 < hw; p0 += blockDim.x) {
+        const int pix = p0 + threadIdx.x;
+        uint32_t cnt = 0;  // (candidates above V << 16) | ties at V, of this pixel: <= 16 each, < 2^16 per chunk
+        if (pix < hw) {
+            for_each_candidate(p, L, b, pix, [&](int, float s) {
+                const uint32_t key = score_key(p, s);
+                if ((key >> p.hist_shift) == T) cnt += key > vkey ? (1u << 16) : key == vkey ? 1u : 0u;
+            });
+        }
+        uint32_t total;
+        const uint32_t excl = block_exclusive_scan(cnt, s_warp, &total);
+        if (cnt) {
+            uint32_t a = base_above + (excl >> 16), t = base_tie + (excl & 0xffffu);
+            for_each_candidate(p, L, b, pix, [&](int c, float s) {
+                const uint32_t key = score_key(p, s);
+                if ((key >> p.hist_shift) != T) return;
+                const uint2 rec = make_uint2(__float_as_uint(s), static_cast<uint32_t>(pix * p.C + c));
+                if (key > vkey) {
+                    out[a++] = rec;
+                } else if (key == vkey) {
+                    if (t < static_cast<uint32_t>(need)) out[n_above + t] = rec;
+                    ++t;
+                }
+            });
+        }
+        base_above += total >> 16;
+        base_tie += total & 0xffffu;
+    }
+}
+
 // One block per (level, image): the final candidate list.  Candidates in histogram bins above the k-th score's bin are in
 // ("sure"); inside that bin the exact rank (score desc, index asc) decides.  fin[slot] = (score bits, index).
-__global__ void __launch_bounds__(256) select_final_kernel(const __grid_constant__ DecodeParams p) {
+__global__ void __launch_bounds__(kSelectThreads) select_final_kernel(const __grid_constant__ DecodeParams p) {
     DD3D_PDL_PROLOGUE();
     const int l = blockIdx.x, b = blockIdx.y;
     const int bl = b * kLevels + l;
@@ -339,16 +458,16 @@ __global__ void __launch_bounds__(256) select_final_kernel(const __grid_constant
     const int n_sure = min(p.counters[bl * 2 + 0], p.topk);
     const int nb_raw = p.counters[bl * 2 + 1];
     const int nb = min(nb_raw, kBoundaryCap);
-    const int need = sel[0] < 0 ? 0 : min(sel[2], nb);
-    if (threadIdx.x == 0) {
-        if (nb_raw > kBoundaryCap) atomicOr(p.flags, 1);
-        p.cand_count[bl] = n_sure + need;
-    }
+    const bool overflow = sel[0] >= 0 && nb_raw > kBoundaryCap;
+    const int need = sel[0] < 0 ? 0 : overflow ? sel[2] : min(sel[2], nb);
+    if (threadIdx.x == 0) p.cand_count[bl] = n_sure + need;
     const uint2* sure = p.sure + static_cast<size_t>(bl) * p.topk;
     const uint2* bnd = p.boundary + static_cast<size_t>(bl) * kBoundaryCap;
     uint2* fin = p.fin + static_cast<size_t>(bl) * p.topk;
     for (int i = threadIdx.x; i < n_sure; i += blockDim.x) fin[i] = sure[i];
-    if (need > 0) {
+    if (overflow) {
+        select_overflow(p, b, l, static_cast<uint32_t>(sel[0]), need, fin + n_sure);
+    } else if (need > 0) {
         for (int i = threadIdx.x; i < nb; i += blockDim.x) {
             const uint2 me = bnd[i];
             int rank = 0;
@@ -460,7 +579,7 @@ cudaError_t launch_decode_select(const DecodeParams& p, cudaStream_t stream) {
     if (e == cudaSuccess) e = launch_pdl(dense_kernel<0>, dgrid, dim3(kDenseThreads), 0, stream, p);
     if (e == cudaSuccess) e = launch_pdl(select_kernel, dim3(kLevels, p.B), dim3(256), 0, stream, p);
     if (e == cudaSuccess) e = launch_pdl(dense_kernel<1>, dgrid, dim3(kDenseThreads), 0, stream, p);
-    if (e == cudaSuccess) e = launch_pdl(select_final_kernel, dim3(kLevels, p.B), dim3(256), 0, stream, p);
+    if (e == cudaSuccess) e = launch_pdl(select_final_kernel, dim3(kLevels, p.B), dim3(kSelectThreads), 0, stream, p);
     return e;
 }
 

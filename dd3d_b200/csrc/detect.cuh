@@ -9,7 +9,22 @@ namespace dd3d {
 constexpr int kLevels = 5;
 constexpr int kNumAttributes = 3;  // MAX_NUM_ATTRIBUTES, tridet/data/datasets/nuscenes/build.py:77
 constexpr int kHistBins = 2048;
-constexpr int kBoundaryCap = 4096;  // candidates sharing the histogram bin of the k-th score (per image x level)
+
+// Dynamic shared memory of the NMS's one-CTA working set (nms_kernel, nms_finish_kernel; csrc/nms.cu) for `cap` =
+// kLevels * PRE_NMS_TOPK candidates: 8192-entry sort keys and payloads + per-candidate box, lists, class and flag.
+constexpr int kNmsSortCap = 8192;
+constexpr size_t nms_smem_bytes(int cap) { return static_cast<size_t>(kNmsSortCap) * 10 + static_cast<size_t>(cap) * 26; }
+// The largest PRE_NMS_TOPK whose working set fits the 227 KiB a block may opt into on sm_90, 1 KiB left for the kernels'
+// static shared memory: 1150.  A larger value is refused (DD3D_ERR_INVALID) before any launch.
+constexpr int max_pre_nms_topk() {
+    int t = kNmsSortCap / kLevels;
+    while (nms_smem_bytes(kLevels * t) + 1024 > 227 * 1024) --t;
+    return t;
+}
+constexpr int kMaxPreNmsTopk = max_pre_nms_topk();
+static_assert(kMaxPreNmsTopk == 1150, "PRE_NMS_TOPK limit (documented in include/dd3d_b200.h)");
+constexpr int kBoundaryCap = 4096;  // candidates sharing the histogram bin of the k-th score (per image x level) that the
+                                    // boundary buffer ranks; a fuller bin is ranked by re-reading the level (decode.cu)
 
 // One decoded detection, 24 x 4 bytes.  Also the element type of the C-ABI output buffer (dd3d_det in the header).
 struct Det {
@@ -82,7 +97,7 @@ struct DecodeParams {
     uint2* boundary;      // [B][L][kBoundaryCap]
     Det* cand;            // [B][L*topk]           decoded candidates
     int32_t* cand_count;  // [B][L]
-    int32_t* flags;       // [1] bit0: boundary overflow
+    int32_t* flags;       // [1] overflow word (the decode sets no bit; NMS: bit1)
     uint2* fin;           // [B][L][topk] final candidates (score bits, index): slot order of `cand`
     // sparse 3-D head: the box3d predictor is evaluated only at the final candidates (b3d_sparse.cu); row of candidate `slot`
     // of (image b, level l) = b3d_rows + ((b * L + l) * topk + slot) * b3d_pitch, same channel layout as a dense map pixel

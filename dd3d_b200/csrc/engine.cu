@@ -39,7 +39,7 @@ void cuda_check(cudaError_t e, const char* what) {
 Engine::Engine(const dd3d_model_desc& d) : desc(d) {
     if (dla_spec(d.arch) == nullptr && vovnet_spec(d.arch) == nullptr) fail(DD3D_ERR_INVALID, "unknown arch");
     if (d.num_classes < 1 || d.num_classes > DD3D_MAX_CLASSES) fail(DD3D_ERR_INVALID, "num_classes out of range");
-    if (d.pre_nms_topk < 1 || d.pre_nms_topk * kLevels > 8192) fail(DD3D_ERR_INVALID, "pre_nms_topk out of range");
+    if (d.pre_nms_topk < 1 || d.pre_nms_topk > kMaxPreNmsTopk) fail(DD3D_ERR_INVALID, "pre_nms_topk out of range");
     if (d.out_cap < 1) fail(DD3D_ERR_INVALID, "out_cap must be positive");
     if (d.act_dtype != DD3D_ACT_BF16 && d.act_dtype != DD3D_ACT_FP16) fail(DD3D_ERR_INVALID, "unknown act_dtype");
     fp16 = d.act_dtype == DD3D_ACT_FP16 ? 1 : 0;

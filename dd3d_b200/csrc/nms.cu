@@ -21,7 +21,7 @@ namespace dd3d {
 namespace {
 
 constexpr int kNmsThreads = 1024;
-constexpr int kMaxCand = 8192;  // bitonic sort capacity (>= L * topk)
+constexpr int kMaxCand = kNmsSortCap;  // bitonic sort capacity (>= L * topk)
 
 __device__ __forceinline__ float iou_tv(const float4 a, const float4 b) {
     const float area_a = __fmul_rn(__fsub_rn(a.z, a.x), __fsub_rn(a.w, a.y));
@@ -626,9 +626,8 @@ size_t nms_scratch_bytes(int B, int topk, int num_classes) {
 
 cudaError_t launch_nms(const NmsParams& p, cudaStream_t stream) {
     const int cap = kLevels * p.topk;
-    if (cap > kMaxCand || p.B <= 0) return cudaErrorInvalidValue;
-    const size_t smem = static_cast<size_t>(kMaxCand) * 8 + static_cast<size_t>(cap) * 16 +
-                        static_cast<size_t>(cap) * 8 + static_cast<size_t>(kMaxCand) * 2 + static_cast<size_t>(cap) * 2;
+    if (p.topk > kMaxPreNmsTopk || p.B <= 0) return cudaErrorInvalidValue;
+    const size_t smem = nms_smem_bytes(cap);  // key 8 + val 2 per sort entry; box 16 + list 4 + list2 4 + cls 1 + flag 1
     const size_t smem_sort = static_cast<size_t>(cap) * (8 + 2 + 1) + 16;
     static size_t attr_smem_dev[64] = {};  // per device; the limit is 227 KiB minus the static shared memory: ask for what we use
     size_t& attr_smem = attr_smem_dev[current_device_or_zero()];

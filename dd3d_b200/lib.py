@@ -147,6 +147,8 @@ SIGNATURES = {
     "dd3d_op_detect_scratch_bytes": (_I64, [_I, _I]),
     "dd3d_op_detect": (_I, [C.POINTER(ModelDesc), _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P),
                             C.POINTER(_P), C.POINTER(_P), _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "dd3d_op_detect_flags": (_I, [C.POINTER(ModelDesc), _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P),
+                                  C.POINTER(_P), C.POINTER(_P), _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
 }
 
 _lib = None

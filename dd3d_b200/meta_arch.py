@@ -171,8 +171,7 @@ class DD3DB200(nn.Module):
         reference's (which has no capacity limits) -- fail loudly instead of returning truncated detections."""
         self.last_overflow_flags = int(flags)
         if flags:
-            names = {1: "more candidates tied at the k-th pre-NMS score than the boundary buffer holds",
-                     2: "more detections than out_cap slots", 4: "more than 256 boxes entered the BEV NMS of one image",
+            names = {2: "more detections than out_cap slots", 4: "more than 256 boxes entered the BEV NMS of one image",
                      8: "sample aggregation capacity exceeded", 16: "more merged TTA detections than slots",
                      32: "grouped BEV NMS capacity exceeded"}
             raise RuntimeError("DD3DB200: detection capacity exceeded (" +

@@ -74,7 +74,7 @@ typedef struct dd3d_model_desc {
     float pixel_std[3];  /* MODEL.PIXEL_STD */
     int32_t feature_locations_offset_half; /* DD3D.FEATURE_LOCATIONS_OFFSET == "half" */
     float pre_nms_thresh;   /* FCOS2D.INFERENCE.PRE_NMS_THRESH (applied to sigmoid(cls)*sigmoid(ctr)) */
-    int32_t pre_nms_topk;   /* PRE_NMS_TOPK (<= 1638 so that 5 levels fit the NMS sort) */
+    int32_t pre_nms_topk;   /* PRE_NMS_TOPK (<= 1150: 5 levels of candidates fit the NMS's shared memory) */
     int32_t post_nms_topk;  /* POST_NMS_TOPK */
     float nms_thresh;       /* NMS_THRESH (<= 0 disables suppression) */
     int32_t do_nms;         /* DD3D.INFERENCE.DO_NMS */
@@ -197,8 +197,8 @@ int dd3d_forward_host(dd3d_handle h, const void* h_images, int img_dtype, const 
 int dd3d_submit_host(dd3d_handle h, int slot, const void* h_images, int img_dtype, const float* h_intrinsics,
                      const int32_t* h_sizes, dd3d_det* h_out, int32_t* h_counts, dd3d_stream stream);
 int dd3d_wait_host(dd3d_handle h, int slot);
-/* bit 0: more candidates tied at the k-th pre-NMS score than the boundary buffer holds; bit 1: more than
- * out_cap detections survived.  Reads a device word (synchronises `stream`). */
+/* bit 0: unused (the pre-NMS top-k is exact for every input and sets no bit); bit 1: more than out_cap detections
+ * survived.  Reads a device word (synchronises `stream`). */
 int dd3d_overflow_flags(dd3d_handle h, dd3d_stream stream, int32_t* h_flags);
 /* Runtime switches the reference's callers toggle on the meta-arch: "do_postprocess" (postprocess_in_inference,
  * scripts/train.py:206-209, test_time_augmentation.py:107), "do_nms" (core.py:134), "profile" (see
@@ -469,6 +469,13 @@ int dd3d_op_detect(const dd3d_model_desc* h_desc, int B, const int32_t* h_level_
                    const float* const* d_b3d, int cls_pitch, int b3d_pitch, const float* d_intrinsics,
                    const int32_t* d_sizes, void* d_scratch, dd3d_det* d_pre_nms /* [B][5*topk] or NULL */,
                    int32_t* d_pre_counts /* [B][5] or NULL */, dd3d_det* d_out, int32_t* d_counts, dd3d_stream stream);
+/* Same, and d_flags (or NULL) receives one int32 word on `stream`: the overflow flags of this call (bits as
+ * dd3d_overflow_flags). */
+int dd3d_op_detect_flags(const dd3d_model_desc* h_desc, int B, const int32_t* h_level_hw /*[5][2]*/,
+                         const int32_t* h_strides /*[5]*/, const float* const* d_cls /*[5]*/, const float* const* d_box,
+                         const float* const* d_b3d, int cls_pitch, int b3d_pitch, const float* d_intrinsics,
+                         const int32_t* d_sizes, void* d_scratch, dd3d_det* d_pre_nms, int32_t* d_pre_counts,
+                         dd3d_det* d_out, int32_t* d_counts, int32_t* d_flags /* or NULL */, dd3d_stream stream);
 
 #ifdef __cplusplus
 }

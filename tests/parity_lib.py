@@ -34,8 +34,8 @@ def rel_l2(a, b):
 
 
 def run_detect(desc, cls, box, b3d, K, sizes, level_hw, strides, topk):
-    """dd3d_op_detect on device head maps (lists of 5 cuda tensors, engine layout); returns pre-NMS candidates and
-    final detections on the host."""
+    """dd3d_op_detect_flags on device head maps (lists of 5 cuda tensors, engine layout); returns pre-NMS candidates and
+    final detections on the host.  The overflow word must stay 0."""
     L = lib.load()
     B = K.shape[0]
     arr = lambda ts: (C.c_void_p * 5)(*[t.data_ptr() for t in ts])  # noqa: E731
@@ -45,14 +45,16 @@ def run_detect(desc, cls, box, b3d, K, sizes, level_hw, strides, topk):
     pre_n = torch.zeros(B, 5, dtype=torch.int32, device="cuda")
     out = torch.zeros(B, desc.out_cap, 24, dtype=torch.float32, device="cuda")
     cnt = torch.zeros(B, dtype=torch.int32, device="cuda")
+    flags = torch.full((1,), -1, dtype=torch.int32, device="cuda")
     hw = (C.c_int32 * 10)(*[v for q in level_hw for v in q])
     st = (C.c_int32 * 5)(*strides)
     Kd, sd = K.reshape(B, 9).contiguous().cuda(), sizes.cuda()
-    r = L.dd3d_op_detect(C.byref(desc), B, hw, st, arr(cls), arr(box), arr(b3d), cls[0].shape[-1], b3d[0].shape[-1],
-                         p(Kd), p(sd), p(scratch), p(pre), p(pre_n), p(out), p(cnt),
-                         C.c_void_p(torch.cuda.current_stream().cuda_stream))
+    r = L.dd3d_op_detect_flags(C.byref(desc), B, hw, st, arr(cls), arr(box), arr(b3d), cls[0].shape[-1],
+                               b3d[0].shape[-1], p(Kd), p(sd), p(scratch), p(pre), p(pre_n), p(out), p(cnt), p(flags),
+                               C.c_void_p(torch.cuda.current_stream().cuda_stream))
     assert r == 0
     torch.cuda.synchronize()
+    assert int(flags) == 0, f"overflow flags {int(flags)}"
     return pre.cpu(), pre_n.cpu(), out.cpu(), cnt.cpu()
 
 

@@ -363,14 +363,16 @@ def _run_detect(desc, maps, K, sizes, level_hw, strides, topk):
     pre_n = torch.zeros(B, 5, dtype=torch.int32, device="cuda")
     out = torch.zeros(B, desc.out_cap, 24, dtype=torch.float32, device="cuda")
     cnt = torch.zeros(B, dtype=torch.int32, device="cuda")
+    flags = torch.full((1,), -1, dtype=torch.int32, device="cuda")
     hw = (C.c_int32 * 10)(*[v for p in level_hw for v in p])
     st = (C.c_int32 * 5)(*strides)
     Kd, sd = K.reshape(B, 9).contiguous().cuda(), sizes.cuda()
-    r = L.dd3d_op_detect(C.byref(desc), B, hw, st, arr(cls), arr(box), arr(b3d), cls[0].shape[-1], b3d[0].shape[-1],
-                         gpu_ops._p(Kd), gpu_ops._p(sd), gpu_ops._p(scratch), gpu_ops._p(pre), gpu_ops._p(pre_n),
-                         gpu_ops._p(out), gpu_ops._p(cnt), gpu_ops._stream())
+    r = L.dd3d_op_detect_flags(C.byref(desc), B, hw, st, arr(cls), arr(box), arr(b3d), cls[0].shape[-1],
+                               b3d[0].shape[-1], gpu_ops._p(Kd), gpu_ops._p(sd), gpu_ops._p(scratch), gpu_ops._p(pre),
+                               gpu_ops._p(pre_n), gpu_ops._p(out), gpu_ops._p(cnt), gpu_ops._p(flags), gpu_ops._stream())
     assert r == 0
     torch.cuda.synchronize()
+    assert int(flags) == 0, f"overflow flags {int(flags)}"
     return pre.cpu(), pre_n.cpu(), out.cpu(), cnt.cpu()
 
 
