@@ -1,5 +1,5 @@
-// Rotated-box geometry shared by the BEV NMS kernels (bev_nms.cu, bev_nms_group.cu): detectron2's rotated IoU
-// (box_iou_rotated_utils.h), pytorch3d's quaternion <-> matrix conversions and the decoded box -> global frame -> BEV
+// Rotated-box geometry shared by the BEV NMS kernels (bev_nms.cu, bev_nms_group.cu): the rotated IoU of detectron2's
+// box_iou_rotated_utils.h, pytorch3d's quaternion <-> matrix conversions and the decoded box -> global frame -> BEV
 // top-surface rectangle of postprocessing.py / boxes3d.py / bev_nms.py.  Internal linkage: every translation unit that
 // includes it gets its own copy, so the kernels inline them as before.
 #pragma once
@@ -14,116 +14,66 @@ namespace {
 struct P2 {
     float x, y;
 };
-__device__ __forceinline__ float cross2(P2 a, P2 b) { return a.x * b.y - a.y * b.x; }
-__device__ __forceinline__ float dot2(P2 a, P2 b) { return a.x * b.x + a.y * b.y; }
-__device__ __forceinline__ P2 sub2(P2 a, P2 b) { return {a.x - b.x, a.y - b.y}; }
 
-// detectron2 box_iou_rotated_utils.h: get_rotated_vertices
-__device__ void rect_vertices(float x, float y, float w, float h, float a, P2* p) {
-    const float th = a * 0.01745329251994329577f;
-    const float c = cosf(th) * 0.5f, s = sinf(th) * 0.5f;
-    p[0] = {x + s * h + c * w, y + c * h - s * w};
-    p[1] = {x - s * h + c * w, y - c * h - s * w};
-    p[2] = {2.f * x - p[0].x, 2.f * y - p[0].y};
-    p[3] = {2.f * x - p[1].x, 2.f * y - p[1].y};
+constexpr int kClipMax = 20;  // Sutherland-Hodgman output bound from a quadrilateral: 4 -> 6 -> 9 -> 13 -> 19 vertices
+
+// One Sutherland-Hodgman step against the axis-aligned half-plane sgn * (axis ? y : x) <= lim.  A crossing point is put
+// exactly on the line, and it lies between the two vertices of its edge, so a vertex that rounding places on the wrong
+// side of a line it (nearly) lies on moves the area by no more than that rounding: parallel and collinear edges need no
+// special case.  Returns the output count (<= n + n / 2: one extra vertex per outside -> inside transition).
+__device__ int clip_half_plane(const P2* in, int n, P2* out, int axis, float sgn, float lim) {
+    int m = 0;
+    if (n == 0) return 0;
+    P2 prev = in[n - 1];
+    float dp = lim - sgn * (axis ? prev.y : prev.x);
+    for (int i = 0; i < n; ++i) {
+        const P2 cur = in[i];
+        const float dc = lim - sgn * (axis ? cur.y : cur.x);
+        if ((dc >= 0.f) != (dp >= 0.f)) {
+            const float t = dp / (dp - dc);  // in [0, 1]: dp and dc have opposite signs
+            const float o = axis ? prev.x + t * (cur.x - prev.x) : prev.y + t * (cur.y - prev.y);
+            out[m++] = axis ? P2{o, sgn * lim} : P2{sgn * lim, o};
+        }
+        if (dc >= 0.f) out[m++] = cur;
+        prev = cur;
+        dp = dc;
+    }
+    return m;
 }
 
-// get_intersection_points: edge x edge intersections + vertices of one rectangle inside the other (<= 24 points)
-__device__ int intersection_points(const P2* p1, const P2* p2, P2* out) {
-    P2 v1[4], v2[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        v1[i] = sub2(p1[(i + 1) & 3], p1[i]);
-        v2[i] = sub2(p2[(i + 1) & 3], p2[i]);
-    }
-    int n = 0;
-    for (int i = 0; i < 4; ++i)
-        for (int j = 0; j < 4; ++j) {
-            const float det = cross2(v2[j], v1[i]);
-            if (fabsf(det) <= 1e-14f) continue;
-            const P2 v12 = sub2(p2[j], p1[i]);
-            const float t1 = cross2(v2[j], v12) / det, t2 = cross2(v1[i], v12) / det;
-            if (t1 >= 0.f && t1 <= 1.f && t2 >= 0.f && t2 <= 1.f) out[n++] = {p1[i].x + v1[i].x * t1, p1[i].y + v1[i].y * t1};
-        }
-    {
-        const P2 AB = v2[0], DA = v2[3];
-        const float ABdotAB = dot2(AB, AB), ADdotAD = dot2(DA, DA);
-        for (int i = 0; i < 4; ++i) {
-            const P2 AP = sub2(p1[i], p2[0]);
-            const float APdotAB = dot2(AP, AB), APdotAD = -dot2(AP, DA);
-            if (APdotAB >= 0.f && APdotAD >= 0.f && APdotAB <= ABdotAB && APdotAD <= ADdotAD) out[n++] = p1[i];
-        }
-    }
-    {
-        const P2 AB = v1[0], DA = v1[3];
-        const float ABdotAB = dot2(AB, AB), ADdotAD = dot2(DA, DA);
-        for (int i = 0; i < 4; ++i) {
-            const P2 AP = sub2(p2[i], p1[0]);
-            const float APdotAB = dot2(AP, AB), APdotAD = -dot2(AP, DA);
-            if (APdotAB >= 0.f && APdotAD >= 0.f && APdotAB <= ABdotAB && APdotAD <= ADdotAD) out[n++] = p2[i];
-        }
-    }
-    return n;
-}
-
-// convex_hull_graham (shift_to_zero = true) followed by polygon_area
-__device__ float hull_area(P2* q, int n) {
-    int t = 0;
-    for (int i = 1; i < n; ++i)
-        if (q[i].y < q[t].y || (q[i].y == q[t].y && q[i].x < q[t].x)) t = i;
-    const P2 start = q[t];
-    for (int i = 0; i < n; ++i) q[i] = sub2(q[i], start);
-    {
-        const P2 tmp = q[0];
-        q[0] = q[t];
-        q[t] = tmp;
-    }
-    float dist[24];
-    for (int i = 0; i < n; ++i) dist[i] = dot2(q[i], q[i]);
-    // insertion sort of q[1..n) by polar angle around q[0] (ties: nearer first), as detectron2's CUDA path
-    for (int i = 2; i < n; ++i) {
-        const P2 qi = q[i];
-        const float di = dist[i];
-        int j = i - 1;
-        while (j >= 1) {
-            const float tmp = cross2(qi, q[j]);  // qi before q[j] ?
-            const bool before = (fabsf(tmp) < 1e-6f) ? (di < dist[j]) : (tmp > 0.f);
-            if (!before) break;
-            q[j + 1] = q[j];
-            dist[j + 1] = dist[j];
-            --j;
-        }
-        q[j + 1] = qi;
-        dist[j + 1] = di;
-    }
-    int k = 1;
-    while (k < n && dist[k] <= 1e-8f) ++k;
-    if (k == n) return 0.f;
-    P2 hull[24];
-    hull[0] = q[0];
-    hull[1] = q[k];
-    int m = 2;
-    for (int i = k + 1; i < n; ++i) {
-        while (m > 1 && cross2(sub2(q[i], hull[m - 2]), sub2(hull[m - 1], hull[m - 2])) >= 0.f) --m;
-        hull[m++] = q[i];
-    }
-    if (m <= 2) return 0.f;
-    float area = 0.f;
-    for (int i = 1; i < m - 1; ++i) area += fabsf(cross2(sub2(hull[i], hull[0]), sub2(hull[i + 1], hull[0])));
-    return area * 0.5f;
-}
-
-// single_box_iou_rotated; boxes are (cx, cy, w, h, angle_deg)
+// Rotated IoU of two BEV rectangles (cx, cy, w, h, angle_deg): the quantity detectron2's single_box_iou_rotated
+// (box_iou_rotated_utils.h) defines -- corners centre +- (w/2) (cos, -sin) +- (h/2) (sin, cos), zero below 1e-14 m^2 of
+// area -- computed by clipping b2 against b1 in b1's own frame, where b1 is the axis-aligned [-w1/2, w1/2] x [-h1/2, h1/2]
+// and b2 is turned by the angle difference alone.  So boxes of one yaw stay exactly axis-aligned and rectangles that
+// share an edge, are nested or are the same box written another way (angle + 180, w <-> h with angle + 90) come out
+// within float32 rounding of their float64 IoU; detectron2's float32 edge-intersection test (|det| <= 1e-14 on metre
+// scale edges) and its contracted hull test do not.  sincospif is exact at multiples of 90 degrees.
 __device__ float rotated_iou(const float* b1, const float* b2) {
     const float a1 = b1[2] * b1[3], a2 = b2[2] * b2[3];
     if (a1 < 1e-14f || a2 < 1e-14f) return 0.f;
-    const float sx = (b1[0] + b2[0]) * 0.5f, sy = (b1[1] + b2[1]) * 0.5f;  // shift centres for precision
-    P2 p1[4], p2[4], pts[24];
-    rect_vertices(b1[0] - sx, b1[1] - sy, b1[2], b1[3], b1[4], p1);
-    rect_vertices(b2[0] - sx, b2[1] - sy, b2[2], b2[3], b2[4], p2);
-    const int n = intersection_points(p1, p2, pts);
+    float s1, c1, s, c;
+    sincospif(b1[4] / 180.f, &s1, &c1);
+    sincospif((b2[4] - b1[4]) / 180.f, &s, &c);
+    const float dx = b2[0] - b1[0], dy = b2[1] - b1[1];
+    const float X = dx * c1 - dy * s1, Y = dx * s1 + dy * c1;  // b2's centre on b1's width / length axes
+    const float hw = 0.5f * b2[2], hh = 0.5f * b2[3];
+    const float ux = c * hw, uy = -s * hw, vx = s * hh, vy = c * hh;
+    P2 buf[2][kClipMax];
+    buf[0][0] = {X + ux + vx, Y + uy + vy};
+    buf[0][1] = {X + ux - vx, Y + uy - vy};
+    buf[0][2] = {X - ux - vx, Y - uy - vy};
+    buf[0][3] = {X - ux + vx, Y - uy + vy};
+    const float lx = 0.5f * b1[2], ly = 0.5f * b1[3];
+    int n = clip_half_plane(buf[0], 4, buf[1], 0, 1.f, lx);
+    n = clip_half_plane(buf[1], n, buf[0], 0, -1.f, lx);
+    n = clip_half_plane(buf[0], n, buf[1], 1, 1.f, ly);
+    n = clip_half_plane(buf[1], n, buf[0], 1, -1.f, ly);
     if (n <= 2) return 0.f;
-    const float inter = hull_area(pts, n);
+    const P2* q = buf[0];
+    float area2 = 0.f;
+    for (int i = 1; i + 1 < n; ++i)
+        area2 += (q[i].x - q[0].x) * (q[i + 1].y - q[0].y) - (q[i].y - q[0].y) * (q[i + 1].x - q[0].x);
+    const float inter = fminf(0.5f * fabsf(area2), fminf(a1, a2));
     return inter / (a1 + a2 - inter);
 }
 

@@ -305,7 +305,19 @@ __global__ void __launch_bounds__(kBevThreads) bev_nms_kernel(const BevParams p)
     if (threadIdx.x == 0) p.counts[b] = s_total;
 }
 
+// One thread per pair: the rotated IoU every BEV kernel thresholds, exposed so tests can hold it to a float64 reference.
+__global__ void __launch_bounds__(kBevThreads) rotated_iou_kernel(const float* a, const float* b, int n, float* out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = rotated_iou(a + static_cast<size_t>(i) * 5, b + static_cast<size_t>(i) * 5);
+}
+
 }  // namespace
+
+cudaError_t launch_rotated_iou(const float* a, const float* b, int n, float* out, cudaStream_t stream) {
+    if (n < 1) return cudaSuccess;
+    rotated_iou_kernel<<<(n + kBevThreads - 1) / kBevThreads, kBevThreads, 0, stream>>>(a, b, n, out);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_bev_nms(Det* dets, int32_t* counts, const float* K, const float* poses, const int32_t* sizes,
                            int32_t* flags, int B, int cap, float thr, int do_postprocess, cudaStream_t stream) {

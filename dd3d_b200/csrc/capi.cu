@@ -781,6 +781,11 @@ int dd3d_op_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsi
                        nullptr);
 }
 
+int dd3d_op_rotated_iou(const float* d_a, const float* d_b, int n, float* d_out, dd3d_stream stream) {
+    if (!d_a || !d_b || !d_out || n < 0) return DD3D_ERR_INVALID;
+    return cuda_status(launch_rotated_iou(d_a, d_b, n, d_out, static_cast<cudaStream_t>(stream)), nullptr);
+}
+
 static_assert(sizeof(dd3d_tta_view) == sizeof(TtaView), "dd3d_tta_view must mirror TtaView");
 
 int dd3d_op_tta_merged_cap(int num_views, int cap) { return tta_merged_cap(num_views, cap); }

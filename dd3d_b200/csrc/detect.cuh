@@ -132,6 +132,8 @@ void nms_set_class_parallel(int mode);  // 0 single-CTA kernel, 1 multi-CTA path
 // BEV rotated NMS on the (already 2-D-NMSed, score-sorted) detections, in place; poses: [B][7] (w,x,y,z, tx,ty,tz).
 cudaError_t launch_bev_nms(Det* dets, int32_t* counts, const float* K, const float* poses, const int32_t* sizes,
                            int32_t* flags, int B, int cap, float thr, int do_postprocess, cudaStream_t stream);
+// out[i] = rotated IoU of rectangles a[i], b[i] ((cx, cy, w, h, angle_deg) rows), the function the BEV kernels threshold.
+cudaError_t launch_rotated_iou(const float* a, const float* b, int n, float* out, cudaStream_t stream);
 
 // Test-time-augmentation merge (tta.cu): the views' detections back to the original image + one merged NMS.
 constexpr int kTtaMaxViews = 16;

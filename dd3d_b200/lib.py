@@ -133,6 +133,7 @@ SIGNATURES = {
     "dd3d_op_ese_pool": (_I, [_P, _I, _P, _P, _P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_ese_scratch_bytes": (_I64, [_I, _I, _I]),
     "dd3d_op_bev_nms": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, C.c_float, _I, _P]),
+    "dd3d_op_rotated_iou": (_I, [_P, _P, _I, _P, _P]),
     "dd3d_resize_shape": (_I, [_I, _I, _I, _I, _P, _P]),
     "dd3d_forward_raw": (_I, [_P, _P, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
     "dd3d_forward_resized": (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),

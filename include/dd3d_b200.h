@@ -413,6 +413,10 @@ int dd3d_op_ese_pool(const void* d_x, int x_pitch, const float* d_fc_w, const fl
 int dd3d_op_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsics, const float* d_poses,
                     const int32_t* d_sizes, int32_t* d_flags, int B, int cap, float iou_thresh, int do_postprocess,
                     dd3d_stream stream);
+/* d_out[i] = rotated IoU of the BEV rectangles d_a[i] and d_b[i] (rows of 5 floats: cx, cy, w, h, angle in degrees;
+ * detectron2's single_box_iou_rotated), one thread per pair: the function the three BEV NMS kernels threshold, exposed
+ * for tests. */
+int dd3d_op_rotated_iou(const float* d_a, const float* d_b, int n, float* d_out, dd3d_stream stream);
 /* resize (+ optional horizontal flip, h_flip [B] or NULL) + normalise + pad + NHWC4 bf16 of raw HWC uint8 images (the
  * first kernel of dd3d_forward_raw / dd3d_forward_resized). */
 int dd3d_op_resize_preprocess(const uint8_t* d_raw, int raw_h, int raw_w, const int32_t* h_raw_sizes,

@@ -6,49 +6,9 @@ import numpy as np
 import pytest
 import torch
 
+from bev_geom_cases import clip_area as _clip, rect_poly as _rect_poly  # independent Sutherland-Hodgman clipper
 from conftest import GOLDEN_DIR
 from oracle import bev_nms_oracle as B
-
-
-# ------------------------------------------------------------------------------------------------ independent clipper
-def _rect_poly(box):
-    return [(x, y) for x, y in B._vertices(tuple(float(v) for v in box))]
-
-
-def _clip(subject, clip):
-    """Sutherland-Hodgman clipping of convex polygons (independent of the Graham-scan formulation under test)."""
-    def area2(p):
-        return sum(p[i][0] * p[(i + 1) % len(p)][1] - p[(i + 1) % len(p)][0] * p[i][1] for i in range(len(p)))
-    if area2(clip) < 0:
-        clip = clip[::-1]
-    out = subject
-    for i in range(len(clip)):
-        a, b = clip[i], clip[(i + 1) % len(clip)]
-        inp, out = out, []
-        if not inp:
-            break
-
-        def inside(p):
-            return (b[0] - a[0]) * (p[1] - a[1]) - (b[1] - a[1]) * (p[0] - a[0]) >= 0
-
-        def inter(p, q):
-            d1 = (b[0] - a[0]) * (p[1] - a[1]) - (b[1] - a[1]) * (p[0] - a[0])
-            d2 = (b[0] - a[0]) * (q[1] - a[1]) - (b[1] - a[1]) * (q[0] - a[0])
-            t = d1 / (d1 - d2)
-            return (p[0] + t * (q[0] - p[0]), p[1] + t * (q[1] - p[1]))
-        s = inp[-1]
-        for e in inp:
-            if inside(e):
-                if not inside(s):
-                    out.append(inter(s, e))
-                out.append(e)
-            elif inside(s):
-                out.append(inter(s, e))
-            s = e
-    if len(out) < 3:
-        return 0.0
-    return abs(sum(out[i][0] * out[(i + 1) % len(out)][1] - out[(i + 1) % len(out)][0] * out[i][1]
-                   for i in range(len(out)))) / 2.0
 
 
 def test_rotated_iou_closed_forms():
