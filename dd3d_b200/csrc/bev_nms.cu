@@ -13,7 +13,7 @@ namespace dd3d {
 
 namespace {
 
-constexpr int kBevMax = 256;
+constexpr int kBevMax = kBevNmsMax;
 constexpr int kBevThreads = 128;
 
 // ------------------------------------------------------------------------------------------------------------------

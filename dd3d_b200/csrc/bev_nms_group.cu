@@ -1,7 +1,12 @@
 // Grouped rotated BEV NMS for large detection sets, spread over the whole GPU.
 //
-// Serves the two BEV steps of test-time augmentation for NuscenesDD3D (nuscenes_dd3d_tta.py), whose inputs are too large
-// for the one-CTA kernels of bev_nms.cu (256 boxes per image, 768 per sample group):
+// Serves the BEV steps whose inputs are too large for the one-CTA kernels of bev_nms.cu (256 boxes per image, 768 per
+// sample group):
+//   * image mode -- the DO_BEV_NMS step of DD3D.forward (core.py:137-151) on up to 5 * PRE_NMS_TOPK boxes per image:
+//     nuscenes_sample_aggregate with one group per image, the image's own pose and K, no cap, then (optionally)
+//     detector_postprocess on the survivors (core.py:153-160).  Runs as the last op of Engine::forward when DO_NMS is off
+//     or POST_NMS_TOPK is outside 1..256 (bev_nms_path);
+// and the two BEV steps of test-time augmentation for NuscenesDD3D (nuscenes_dd3d_tta.py):
 //   * camera mode -- bev_nms(merged_instances.pred_boxes3d, ...) on the merged set of one image (<= kTtaMergedMax boxes),
 //     with the default pose_cam_global = CAMERA_TO_VEHICLE_ROTATION (tridet/layers/bev_nms.py:99-133);
 //   * global mode -- nuscenes_sample_aggregate over the images of the call (postprocessing.py:22-108): boxes to the global
@@ -17,8 +22,11 @@
 //   mask     all SMs      one warp per row of a class segment: rotated-IoU bit matrix in global scratch
 //   scan     1 CTA per (group, class)   greedy pass, 64 rows at a time; survivors publish their score
 //   select   1 CTA        radix select of the max_dets-th survivor key of the call (only when the cap binds)
-//   compact  1 CTA/image  order-preserving compaction of dets / global rows, new counts
+//   compact  1 CTA/image  order-preserving compaction of dets / global rows (image mode: after detector_postprocess),
+//                         new counts
 // Every output is written from scratch each call and no step depends on CTA scheduling order: bit-deterministic.
+#include <algorithm>
+
 #include "bev_geom.cuh"
 #include "device_once.cuh"
 #include "pdl.cuh"
@@ -27,18 +35,20 @@ namespace dd3d {
 
 namespace {
 
-constexpr int kGbMaxB = 256;          // images per call
-constexpr int kGbMaxCap = 1024;       // detection slots per image (kTtaMergedMax)
+constexpr int kGbMaxB = 256;          // images per launch (image mode: per chunk of the batch)
+constexpr int kGbMaxCap = kLevels * kMaxPreNmsTopk;  // detection slots per image (image mode with DO_NMS off)
 constexpr int kGbGroupImages = 16;    // images per group (the caller's max_group_images is at most this)
 constexpr int kGbMaxCls = 64;         // class ids 0..63
-constexpr int kGbSortMax = kGbGroupImages * kGbMaxCap;  // boxes per group
+constexpr int kGbSortMax = kGbGroupImages * kTtaMergedMax;  // boxes per group: max_group_images * cap <= this
 constexpr int kGbMaxWords = kGbSortMax / 64;
 constexpr int kGbSortThreads = 1024;
 constexpr int kGbThreads = 256;
 constexpr int kGbPrepThreads = 128;
+constexpr int kGbCompactThreads = 1024;
 constexpr int kGbFlag = 32;           // capacity exceeded (a count above cap, more than max_group_images images in a
                                       // group, group, class or view index out of range)
-static_assert(kGbMaxCap <= 1024, "compaction runs one thread per slot");
+constexpr int kGbImageFlag = 64;      // the same in image mode
+static_assert(kGbMaxCap <= kGbSortMax, "one image fits one group");
 static_assert(kGbSortMax <= 65536, "the sort key holds the concatenation index in 16 bits");
 
 struct GbParams {
@@ -46,9 +56,11 @@ struct GbParams {
     int32_t* counts;       // [B]
     const float* view_K;   // [B][num_views][9] intrinsics each detection's translation is computed with
     const float* poses;    // [B][7] global camera pose (w, x, y, z, tx, ty, tz); global mode only
-    const int32_t* group;  // [B]
+    const int32_t* group;  // [B], or nullptr: image b is group b
+    const int32_t* sizes;  // [B][4] (h, w, out_h, out_w): detector_postprocess on the survivors, or nullptr
     float* global;         // [B][cap][10] quat (w, x, y, z), tvec, size in the pose's frame, or nullptr
     int32_t* flags;
+    int flag_bit;          // kGbFlag or kGbImageFlag
     int B, cap, num_views, pose_mode, num_groups, max_group_images, max_dets;
     float thr;
     // scratch
@@ -106,6 +118,8 @@ GbScratch gb_layout(int B, int cap, int max_group_images) {
 // pose_cam_global = CAMERA_TO_VEHICLE_ROTATION (bev_nms.py:27-32): x_vehicle = z_cam, y_vehicle = -x_cam, z_vehicle = -y_cam
 __constant__ float kCamToVehicle[9] = {0.f, 0.f, 1.f, -1.f, 0.f, 0.f, 0.f, -1.f, 0.f};
 
+__device__ __forceinline__ int group_of(const GbParams& p, int b) { return p.group ? p.group[b] : b; }
+
 __global__ void __launch_bounds__(32) gbev_layout_kernel(const GbParams p) {
     DD3D_PDL_PROLOGUE();
     __shared__ int s_n[kGbMaxB], s_imgs[kGbMaxB], s_local[kGbMaxB], s_base[kGbMaxB];
@@ -113,7 +127,7 @@ __global__ void __launch_bounds__(32) gbev_layout_kernel(const GbParams p) {
     for (int g = 0; g < p.num_groups; ++g) s_n[g] = s_imgs[g] = 0;
     int bad = 0;
     for (int b = 0; b < p.B; ++b) {
-        const int g = p.group[b];
+        const int g = group_of(p, b);
         p.img_n[b] = 0;
         s_local[b] = 0;
         if (g < 0 || g >= p.num_groups || s_imgs[g] == p.max_group_images) {
@@ -139,10 +153,10 @@ __global__ void __launch_bounds__(32) gbev_layout_kernel(const GbParams p) {
     }
     *p.total = base;
     for (int b = 0; b < p.B; ++b) {
-        const int g = p.group[b];
+        const int g = group_of(p, b);
         p.img_pos[b] = (g >= 0 && g < p.num_groups) ? s_base[g] + s_local[b] : 0;
     }
-    if (bad) atomicOr(p.flags, kGbFlag);
+    if (bad) atomicOr(p.flags, p.flag_bit);
 }
 
 __global__ void __launch_bounds__(kGbPrepThreads) gbev_prep_kernel(const GbParams p) {
@@ -155,7 +169,7 @@ __global__ void __launch_bounds__(kGbPrepThreads) gbev_prep_kernel(const GbParam
     const Det& D = p.dets[flat];
     int view = p.num_views > 1 ? D.level : 0;
     if (view < 0 || view >= p.num_views) {
-        atomicOr(p.flags, kGbFlag);
+        atomicOr(p.flags, p.flag_bit);
         view = 0;
     }
     float iK[9], Rw[9], R[9], t[3], rect[5];
@@ -183,10 +197,10 @@ __global__ void __launch_bounds__(kGbPrepThreads) gbev_prep_kernel(const GbParam
     }
     int cls = D.cls;
     if (cls < 0 || cls >= kGbMaxCls) {
-        atomicOr(p.flags, kGbFlag);
+        atomicOr(p.flags, p.flag_bit);
         cls = min(max(cls, 0), kGbMaxCls - 1);
     }
-    const int local = concat - p.grp[p.group[b] * 3];
+    const int local = concat - p.grp[group_of(p, b) * 3];
     // class major; descending scores_3d (non-negative floats order like their bit patterns); concatenation index
     p.key[concat] = (static_cast<unsigned long long>(cls) << 48) |
                     (static_cast<unsigned long long>(~__float_as_uint(D.score3d)) << 16) | static_cast<unsigned>(local);
@@ -338,9 +352,11 @@ __global__ void __launch_bounds__(kGbSortThreads) gbev_select_kernel(const GbPar
     const size_t N = static_cast<size_t>(p.B) * p.cap;
     if (threadIdx.x == 0) s_total = 0;
     __syncthreads();
-    int part = 0;
-    for (size_t i = threadIdx.x; i < N; i += blockDim.x) part += p.keep_score[i] >= 0.f;
-    atomicAdd(&s_total, part);
+    if (p.max_dets > 0) {
+        int part = 0;
+        for (size_t i = threadIdx.x; i < N; i += blockDim.x) part += p.keep_score[i] >= 0.f;
+        atomicAdd(&s_total, part);
+    }
     __syncthreads();
     if (p.max_dets <= 0 || s_total <= p.max_dets) {
         if (threadIdx.x == 0) {
@@ -385,78 +401,72 @@ __global__ void __launch_bounds__(kGbSortThreads) gbev_select_kernel(const GbPar
     }
 }
 
-__global__ void __launch_bounds__(kGbMaxCap) gbev_compact_kernel(const GbParams p) {
+// One CTA per image, kGbCompactThreads slots at a time: every write of a chunk lands at or before its own slot, after
+// the chunk's reads, so the compaction runs in place.
+__global__ void __launch_bounds__(kGbCompactThreads) gbev_compact_kernel(const GbParams p) {
     DD3D_PDL_PROLOGUE();
-    __shared__ int s_warp[kGbMaxCap / 32];
-    const int b = blockIdx.x, s = threadIdx.x, lane = s & 31, warp = s >> 5;
-    const size_t flat = static_cast<size_t>(b) * p.cap + s;
+    __shared__ int s_warp[kGbCompactThreads / 32];
+    const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const bool capped = p.sel[1] != 0ull;
     const unsigned long long last = p.sel[0];
-    bool keep = false;
-    Det d;
-    float gl[10];
-    if (s < p.cap) {
-        const float sc = p.keep_score[flat];
-        keep = sc >= 0.f && (!capped || survivor_key(sc, flat) <= last);
+    // detector_postprocess (core.py:153-160): scale to the output size, clip, drop empty boxes
+    float sxs = 1.f, sys = 1.f, out_w = 0.f, out_h = 0.f;
+    if (p.sizes) {
+        const int32_t* sz = p.sizes + b * 4;
+        out_h = static_cast<float>(sz[2]);
+        out_w = static_cast<float>(sz[3]);
+        sxs = out_w / static_cast<float>(sz[1]);
+        sys = out_h / static_cast<float>(sz[0]);
+    }
+    int base = 0;  // survivors of the earlier chunks
+    for (int s0 = 0; s0 < p.cap; s0 += blockDim.x) {
+        const int s = s0 + threadIdx.x;
+        const size_t flat = static_cast<size_t>(b) * p.cap + s;
+        bool keep = false;
+        Det d;
+        float gl[10];
+        if (s < p.cap) {
+            const float sc = p.keep_score[flat];
+            keep = sc >= 0.f && (!capped || survivor_key(sc, flat) <= last);
+            if (keep) {
+                d = p.dets[flat];
+                if (p.sizes) {
+                    d.box[0] = fminf(fmaxf(d.box[0] * sxs, 0.f), out_w);
+                    d.box[2] = fminf(fmaxf(d.box[2] * sxs, 0.f), out_w);
+                    d.box[1] = fminf(fmaxf(d.box[1] * sys, 0.f), out_h);
+                    d.box[3] = fminf(fmaxf(d.box[3] * sys, 0.f), out_h);
+                    keep = (d.box[2] - d.box[0]) > 0.f && (d.box[3] - d.box[1]) > 0.f;
+                }
+                if (keep && p.global)
+#pragma unroll
+                    for (int e = 0; e < 10; ++e) gl[e] = p.global[flat * 10 + e];
+            }
+        }
+        const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) s_warp[warp] = __popc(ballot);
+        __syncthreads();  // every read of this chunk's slots happened above
+        int off = base, total = base;
+        for (int w = 0; w < static_cast<int>(blockDim.x) / 32; ++w) {
+            if (w < warp) off += s_warp[w];
+            total += s_warp[w];
+        }
         if (keep) {
-            d = p.dets[flat];
+            const size_t to = static_cast<size_t>(b) * p.cap + off + __popc(ballot & ((1u << lane) - 1u));
+            p.dets[to] = d;
             if (p.global)
 #pragma unroll
-                for (int e = 0; e < 10; ++e) gl[e] = p.global[flat * 10 + e];
+                for (int e = 0; e < 10; ++e) p.global[to * 10 + e] = gl[e];
         }
+        base = total;
+        __syncthreads();  // s_warp is rewritten by the next chunk
     }
-    const unsigned ballot = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) s_warp[warp] = __popc(ballot);
-    __syncthreads();  // every read of this image's slots happened above
-    int off = 0;
-    for (int w = 0; w < warp; ++w) off += s_warp[w];
-    if (keep) {
-        const size_t to = static_cast<size_t>(b) * p.cap + off + __popc(ballot & ((1u << lane) - 1u));
-        p.dets[to] = d;
-        if (p.global)
-#pragma unroll
-            for (int e = 0; e < 10; ++e) p.global[to * 10 + e] = gl[e];
-    }
-    if (s == 0) {
-        int total = 0;
-        for (int w = 0; w < static_cast<int>(blockDim.x) / 32; ++w) total += s_warp[w];
-        p.counts[b] = total;
-    }
+    if (threadIdx.x == 0) p.counts[b] = base;
 }
 
-}  // namespace
-
-size_t group_bev_nms_scratch_bytes(int B, int cap, int max_group_images) {
-    if (B < 1 || cap < 1 || max_group_images < 1) return 0;
-    return gb_layout(B, cap, max_group_images).bytes;
-}
-
-cudaError_t launch_group_bev_nms(Det* dets, int32_t* counts, const float* view_K, int num_views, const float* poses,
-                                 int pose_mode, const int32_t* group, int num_groups, int max_group_images, float* global,
-                                 void* scratch, int32_t* flags, int B, int cap, float thr, int max_dets,
-                                 cudaStream_t stream) {
-    if (B < 1 || B > kGbMaxB || cap < 1 || cap > kGbMaxCap || num_groups < 1 || num_groups > B || num_views < 1 ||
-        max_group_images < 1 || max_group_images > kGbGroupImages ||
-        (pose_mode != 0 && pose_mode != 1) || (pose_mode == 0 && poses == nullptr))
-        return cudaErrorInvalidValue;
-    const GbScratch L = gb_layout(B, cap, max_group_images);
+// Fills the scratch pointers of p (for p.B images, groups of at most max_group_images) and enqueues the seven kernels.
+cudaError_t gb_launch(GbParams p, void* scratch, cudaStream_t stream) {
+    const GbScratch L = gb_layout(p.B, p.cap, p.max_group_images);
     uint8_t* s = static_cast<uint8_t*>(scratch);
-    GbParams p;
-    p.dets = dets;
-    p.counts = counts;
-    p.view_K = view_K;
-    p.poses = poses;
-    p.group = group;
-    p.global = global;
-    p.flags = flags;
-    p.B = B;
-    p.cap = cap;
-    p.num_views = num_views;
-    p.pose_mode = pose_mode;
-    p.num_groups = num_groups;
-    p.max_group_images = max_group_images;
-    p.max_dets = max_dets;
-    p.thr = thr;
     p.img_n = reinterpret_cast<int32_t*>(s + L.img_n);
     p.img_pos = reinterpret_cast<int32_t*>(s + L.img_pos);
     p.grp = reinterpret_cast<int32_t*>(s + L.grp);
@@ -480,17 +490,90 @@ cudaError_t launch_group_bev_nms(Det* dets, int32_t* counts, const float* view_K
     }
     int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int B = p.B, cap = p.cap;
     cudaError_t e = launch_pdl(gbev_layout_kernel, dim3(1), dim3(32), 0, stream, p);
     if (e == cudaSuccess)
         e = launch_pdl(gbev_prep_kernel, dim3((cap + kGbPrepThreads - 1) / kGbPrepThreads, B), dim3(kGbPrepThreads), 0,
                        stream, p);
-    if (e == cudaSuccess) e = launch_pdl(gbev_sort_kernel, dim3(num_groups), dim3(kGbSortThreads), sort_smem, stream, p);
+    if (e == cudaSuccess) e = launch_pdl(gbev_sort_kernel, dim3(p.num_groups), dim3(kGbSortThreads), sort_smem, stream, p);
     if (e == cudaSuccess) e = launch_pdl(gbev_mask_kernel, dim3(sms * 8), dim3(kGbThreads), 0, stream, p);
-    if (e == cudaSuccess) e = launch_pdl(gbev_scan_kernel, dim3(num_groups, kGbMaxCls), dim3(kGbThreads), 0, stream, p);
+    if (e == cudaSuccess) e = launch_pdl(gbev_scan_kernel, dim3(p.num_groups, kGbMaxCls), dim3(kGbThreads), 0, stream, p);
     if (e == cudaSuccess) e = launch_pdl(gbev_select_kernel, dim3(1), dim3(kGbSortThreads), 0, stream, p);
     if (e == cudaSuccess)
-        e = launch_pdl(gbev_compact_kernel, dim3(B), dim3((cap + 31) / 32 * 32), 0, stream, p);
+        e = launch_pdl(gbev_compact_kernel, dim3(B), dim3(std::min(kGbCompactThreads, (cap + 31) / 32 * 32)), 0, stream, p);
     return e;
 }
+
+}  // namespace
+
+size_t group_bev_nms_scratch_bytes(int B, int cap, int max_group_images) {
+    if (B < 1 || cap < 1 || max_group_images < 1) return 0;
+    return gb_layout(B, cap, max_group_images).bytes;
+}
+
+cudaError_t launch_group_bev_nms(Det* dets, int32_t* counts, const float* view_K, int num_views, const float* poses,
+                                 int pose_mode, const int32_t* group, int num_groups, int max_group_images, float* global,
+                                 void* scratch, int32_t* flags, int B, int cap, float thr, int max_dets,
+                                 cudaStream_t stream) {
+    if (B < 1 || B > kGbMaxB || cap < 1 || cap > kGbMaxCap || num_groups < 1 || num_groups > B || num_views < 1 ||
+        max_group_images < 1 || max_group_images > kGbGroupImages || max_group_images * cap > kGbSortMax ||
+        (pose_mode != 0 && pose_mode != 1) || (pose_mode == 0 && poses == nullptr) || group == nullptr)
+        return cudaErrorInvalidValue;
+    GbParams p{};
+    p.dets = dets;
+    p.counts = counts;
+    p.view_K = view_K;
+    p.poses = poses;
+    p.group = group;
+    p.sizes = nullptr;
+    p.global = global;
+    p.flags = flags;
+    p.flag_bit = kGbFlag;
+    p.B = B;
+    p.cap = cap;
+    p.num_views = num_views;
+    p.pose_mode = pose_mode;
+    p.num_groups = num_groups;
+    p.max_group_images = max_group_images;
+    p.max_dets = max_dets;
+    p.thr = thr;
+    return gb_launch(p, scratch, stream);
+}
+
+size_t image_bev_nms_scratch_bytes(int B, int cap) {
+    if (B < 1 || cap < 1) return 0;
+    return gb_layout(std::min(B, kGbMaxB), cap, 1).bytes;
+}
+
+cudaError_t launch_image_bev_nms(Det* dets, int32_t* counts, const float* K, const float* poses, const int32_t* sizes,
+                                 void* scratch, int32_t* flags, int B, int cap, float thr, cudaStream_t stream) {
+    if (B < 1 || cap < 1 || cap > kGbMaxCap || poses == nullptr) return cudaErrorInvalidValue;
+    cudaError_t e = cudaSuccess;
+    for (int b0 = 0; b0 < B && e == cudaSuccess; b0 += kGbMaxB) {  // chunks of kGbMaxB images share the scratch in order
+        const int n = std::min(kGbMaxB, B - b0);
+        GbParams p{};
+        p.dets = dets + static_cast<size_t>(b0) * cap;
+        p.counts = counts + b0;
+        p.view_K = K + static_cast<size_t>(b0) * 9;
+        p.poses = poses + static_cast<size_t>(b0) * 7;
+        p.group = nullptr;
+        p.sizes = sizes ? sizes + static_cast<size_t>(b0) * 4 : nullptr;
+        p.global = nullptr;
+        p.flags = flags;
+        p.flag_bit = kGbImageFlag;
+        p.B = n;
+        p.cap = cap;
+        p.num_views = 1;  // the image's own K: Det::level is the FPN level here, not a view index
+        p.pose_mode = 0;
+        p.num_groups = n;
+        p.max_group_images = 1;
+        p.max_dets = 0;
+        p.thr = thr;
+        e = gb_launch(p, scratch, stream);
+    }
+    return e;
+}
+
+int image_bev_nms_launches(int B) { return 7 * ((B + kGbMaxB - 1) / kGbMaxB); }
 
 }  // namespace dd3d

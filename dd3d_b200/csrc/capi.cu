@@ -110,7 +110,7 @@ int dd3d_forward(dd3d_handle h, const void* d_images, int img_dtype, const float
                  dd3d_det* d_out, int32_t* d_counts, dd3d_stream stream) {
     if (!d_images || !d_intrinsics || !d_sizes || !d_out || !d_counts) return DD3D_ERR_INVALID;
     return guarded(h, [&](Engine& e) {
-        e.forward(d_images, img_dtype, d_intrinsics, d_sizes, reinterpret_cast<Det*>(d_out), d_counts,
+        e.forward(d_images, img_dtype, d_intrinsics, d_sizes, reinterpret_cast<Det*>(d_out), d_counts, e.user_poses,
                   static_cast<cudaStream_t>(stream));
     });
 }
@@ -216,6 +216,8 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value) {
                 throw EngineError(DD3D_ERR_INVALID, "do_nms = 0 needs out_cap >= 5 * pre_nms_topk (" +
                                                         std::to_string(kLevels * e.desc.pre_nms_topk) + "), engine has " +
                                                         std::to_string(e.desc.out_cap) + ": recreate the engine");
+            const int bev = e.bev_mode();
+            if (bev && bev_nms_path(value ? 1 : 0, e.desc.post_nms_topk) != bev) e.drop_plans();  // BEV kernel changes
             e.desc.do_nms = value ? 1 : 0;
         } else if (n == "profile") {
             e.opt_profile = value ? 1 : 0;
@@ -247,6 +249,24 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value) {
             throw EngineError(DD3D_ERR_INVALID, "unknown option: " + n);
         }
     });
+}
+
+int dd3d_set_bev_nms(dd3d_handle h, int enable, float iou_thresh) {
+    return guarded(h, [&](Engine& e) { e.set_bev_nms(enable, iou_thresh); });
+}
+
+int dd3d_set_poses(dd3d_handle h, const float* d_poses) {
+    return guarded(h, [&](Engine& e) { e.user_poses = d_poses; });
+}
+
+int dd3d_set_host_poses(dd3d_handle h, int slot, const float* h_poses) {
+    if (!h_poses) return DD3D_ERR_INVALID;
+    return guarded(h, [&](Engine& e) { e.set_host_poses(slot, h_poses); });
+}
+
+int dd3d_bev_nms_path(const dd3d_model_desc* h_desc) {
+    if (!h_desc) return DD3D_ERR_INVALID;
+    return bev_nms_path(h_desc->do_nms, h_desc->post_nms_topk);
 }
 
 int dd3d_num_ops(dd3d_handle h) {
@@ -778,6 +798,23 @@ int dd3d_op_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsi
         return DD3D_ERR_INVALID;
     return cuda_status(launch_bev_nms(reinterpret_cast<Det*>(d_dets), d_counts, d_intrinsics, d_poses, d_sizes, d_flags, B,
                                       cap, iou_thresh, do_postprocess, static_cast<cudaStream_t>(stream)),
+                       nullptr);
+}
+
+int64_t dd3d_op_bev_nms_large_scratch_bytes(int B, int cap) {
+    if (B < 1 || cap < 1 || cap > kLevels * kMaxPreNmsTopk) return DD3D_ERR_INVALID;
+    return static_cast<int64_t>(image_bev_nms_scratch_bytes(B, cap));
+}
+
+int dd3d_op_bev_nms_large(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsics, const float* d_poses,
+                          const int32_t* d_sizes, void* d_scratch, int32_t* d_flags, int B, int cap, float iou_thresh,
+                          int do_postprocess, dd3d_stream stream) {
+    if (!d_dets || !d_counts || !d_intrinsics || !d_poses || (do_postprocess && !d_sizes) || !d_scratch || !d_flags ||
+        B < 1 || cap < 1 || cap > kLevels * kMaxPreNmsTopk)
+        return DD3D_ERR_INVALID;
+    return cuda_status(launch_image_bev_nms(reinterpret_cast<Det*>(d_dets), d_counts, d_intrinsics, d_poses,
+                                            do_postprocess ? d_sizes : nullptr, d_scratch, d_flags, B, cap, iou_thresh,
+                                            static_cast<cudaStream_t>(stream)),
                        nullptr);
 }
 

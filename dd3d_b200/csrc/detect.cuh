@@ -129,6 +129,15 @@ cudaError_t launch_decode_final(const DecodeParams& p, cudaStream_t stream);
 cudaError_t launch_nms(const NmsParams& p, cudaStream_t stream);
 size_t nms_scratch_bytes(int B, int topk, int num_classes);
 void nms_set_class_parallel(int mode);  // 0 single-CTA kernel, 1 multi-CTA path (sort / IoU bit matrix / scan / finish), -1 environment / default (1)
+// BEV rotated NMS of DD3D.forward (DO_BEV_NMS, core.py:137-151).  The one-CTA kernel (launch_bev_nms) holds kBevNmsMax
+// boxes per image and relies on them arriving sorted by scores_3d: the output of the 2-D NMS with 0 < POST_NMS_TOPK <=
+// kBevNmsMax.  Every other configuration -- DO_NMS off (all 5 * PRE_NMS_TOPK candidates, level-major) or POST_NMS_TOPK
+// outside 1..kBevNmsMax (every 2-D NMS survivor) -- takes the multi-CTA path (launch_image_bev_nms), which sorts itself.
+constexpr int kBevNmsMax = 256;
+constexpr int kBevPathOneCta = 1, kBevPathMultiCta = 2;
+inline int bev_nms_path(int do_nms, int post_nms_topk) {
+    return (do_nms && post_nms_topk > 0 && post_nms_topk <= kBevNmsMax) ? kBevPathOneCta : kBevPathMultiCta;
+}
 // BEV rotated NMS on the (already 2-D-NMSed, score-sorted) detections, in place; poses: [B][7] (w,x,y,z, tx,ty,tz).
 cudaError_t launch_bev_nms(Det* dets, int32_t* counts, const float* K, const float* poses, const int32_t* sizes,
                            int32_t* flags, int B, int cap, float thr, int do_postprocess, cudaStream_t stream);
@@ -162,6 +171,13 @@ cudaError_t launch_sample_aggregate(Det* dets, int32_t* counts, const float* K, 
 // Grouped rotated BEV NMS for large sets (bev_nms_group.cu): B <= 256 images of cap <= 1024 slots, groups of
 // <= max_group_images <= 16 images; view_K [B][num_views][9] indexed by Det::level; pose_mode 0: global (poses [B][7]),
 // 1: camera (CAMERA_TO_VEHICLE_ROTATION); global (or nullptr): [B][cap][10]; max_dets <= 0: no cap.
+// Image mode of the same kernels: the per-image BEV NMS of DD3D.forward on up to kLevels * kMaxPreNmsTopk unsorted boxes
+// per image (each image its own group, its own K [B][9] and pose [B][7], no cap); then detector_postprocess when sizes
+// ([B][4]) is not null.  Any B (chunks of 256 images share the scratch); flags bit 6 (64): a count above cap.
+size_t image_bev_nms_scratch_bytes(int B, int cap);
+cudaError_t launch_image_bev_nms(Det* dets, int32_t* counts, const float* K, const float* poses, const int32_t* sizes,
+                                 void* scratch, int32_t* flags, int B, int cap, float thr, cudaStream_t stream);
+int image_bev_nms_launches(int B);
 size_t group_bev_nms_scratch_bytes(int B, int cap, int max_group_images);
 cudaError_t launch_group_bev_nms(Det* dets, int32_t* counts, const float* view_K, int num_views, const float* poses,
                                  int pose_mode, const int32_t* group, int num_groups, int max_group_images, float* global,

@@ -1532,6 +1532,9 @@ size_t Engine::build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry) 
         P->d_counts = static_cast<int32_t*>(bld.alloc_bytes(static_cast<size_t>(B) * 4));
         P->d_images = bld.alloc_bytes(static_cast<size_t>(B) * 3 * Hs * Ws * 4);
         P->d_canon = nullptr;
+        P->bev = bev_mode();
+        if (P->bev) P->d_poses = static_cast<float*>(bld.alloc_bytes(static_cast<size_t>(B) * 7 * 4));
+        if (P->bev == kBevPathMultiCta) P->bev_scratch = bld.alloc_bytes(image_bev_nms_scratch_bytes(B, desc.out_cap));
         if (tracing) {
             arena_bytes = plan_arena(bufs, opt_workspace_reuse != 0);
             total = arena_bytes + bld.off;
@@ -1702,8 +1705,32 @@ void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodePar
     np->num_classes = desc.num_classes;
 }
 
+int Engine::bev_mode() const { return opt_bev_nms ? bev_nms_path(desc.do_nms, desc.post_nms_topk) : 0; }
+
+// kernel launches of the BEV NMS op of a plan
+static int bev_launches(const Plan& P) {
+    return P.bev == kBevPathOneCta ? 1 : P.bev == kBevPathMultiCta ? image_bev_nms_launches(P.B) : 0;
+}
+
+void Engine::set_bev_nms(int enable, float thr) {
+    if (enable && !desc.box3d_on) fail(DD3D_ERR_INVALID, "the BEV NMS needs the 3-D head (box3d_on)");
+    if (!(thr == thr)) fail(DD3D_ERR_INVALID, "BEV NMS IoU threshold is NaN");
+    const int after = enable ? bev_nms_path(desc.do_nms, desc.post_nms_topk) : 0;
+    // the op list and the workspace change: plans are rebuilt at the next dd3d_plan (throws, changing nothing, while a
+    // dd3d_submit_host is pending)
+    if (after != bev_mode()) drop_plans();
+    opt_bev_nms = enable ? 1 : 0;
+    bev_nms_thresh = thr;
+}
+
+void Engine::set_host_poses(int slot, const float* h_poses) {
+    if (!plan.valid) fail(DD3D_ERR_STATE, "set_host_poses before plan");
+    if (slot < 0 || slot > 1) fail(DD3D_ERR_INVALID, "slot must be 0 or 1");
+    host_poses[slot].assign(h_poses, h_poses + static_cast<size_t>(plan.B) * 7);
+}
+
 int Engine::launches_per_forward() const {
-    int n = 1 /*preprocess*/ + 6 /*decode: clear, 2 dense passes, 2 selects, final*/ + (plan.sparse_b3d ? 1 : 0) +
+    int n = bev_launches(plan) + 1 /*preprocess*/ + 6 /*decode: clear, 2 dense passes, 2 selects, final*/ + (plan.sparse_b3d ? 1 : 0) +
             (plan.tower_begin >= 0 ? 1 : 0) /*tower tile lists*/ + (plan.box2d_begin >= 0 ? 2 : 0) /*box2d mark + lists*/ + ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) /*nms: sort, IoU bit matrix, scan, finish*/;
     for (const Op& op : plan.ops) n += (op.type == Op::ESE) ? 3 : (op.type == Op::GN && op.gn.gamma != nullptr) ? 2 : 1;
     return n;
@@ -1753,13 +1780,17 @@ void Engine::forward_resized(const uint8_t* d_raw, int raw_h, int raw_w, const i
                "H2D sizes");
     raw_pending = true;
     raw_args = {d_raw, raw_h, raw_w, h_raw_sizes, h_new_sizes, h_flip};
-    forward(nullptr, DD3D_IMG_U8, P.d_K, P.d_sizes, d_out, d_counts, stream);
+    forward(nullptr, DD3D_IMG_U8, P.d_K, P.d_sizes, d_out, d_counts, user_poses, stream);
 }
 
 void Engine::forward(const void* d_images, int img_dtype, const float* d_K, const int32_t* d_sizes, Det* d_out,
-                     int32_t* d_counts, cudaStream_t stream) {
+                     int32_t* d_counts, const float* d_poses, cudaStream_t stream) {
     if (!plan.valid) fail(DD3D_ERR_STATE, "forward before plan");
     const Plan& P = plan;
+    if (P.bev && d_poses == nullptr) {
+        raw_pending = false;
+        fail(DD3D_ERR_STATE, "BEV NMS is on: the forward needs the poses (dd3d_set_poses / dd3d_set_host_poses)");
+    }
     const bool raw = raw_pending;
     raw_pending = false;
     size_t ev_i = 0;
@@ -1877,12 +1908,20 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
     }
     mark(6);
     NmsParams np = P.nms;
-    np.do_postprocess = opt_do_postprocess;
+    np.do_postprocess = P.bev ? 0 : opt_do_postprocess;  // with BEV NMS detector_postprocess follows it (core.py:137-160)
     np.do_nms = desc.do_nms;
     np.sizes = d_sizes;
     np.out = d_out;
     np.out_count = d_counts;
     cuda_check(launch_nms(np, stream), "nms");
+    if (P.bev == kBevPathOneCta)
+        cuda_check(launch_bev_nms(d_out, d_counts, d_K, d_poses, d_sizes, P.decode.flags, P.B, desc.out_cap, bev_nms_thresh,
+                                  opt_do_postprocess, stream),
+                   "bev nms");
+    else if (P.bev == kBevPathMultiCta)
+        cuda_check(launch_image_bev_nms(d_out, d_counts, d_K, d_poses, opt_do_postprocess ? d_sizes : nullptr, P.bev_scratch,
+                                        P.decode.flags, P.B, desc.out_cap, bev_nms_thresh, stream),
+                   "bev nms (multi-CTA)");
     mark(7);
     if (opt_profile) prof_used = ev_i;
 }
@@ -1981,7 +2020,7 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
         }
     }
     launches[6] = 6 + (P.sparse_b3d ? 1 : 0) + (P.tower_begin >= 0 ? 1 : 0) + (P.box2d_begin >= 0 ? 2 : 0);
-    launches[7] = (desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1;
+    launches[7] = ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) + bev_launches(P);
     for (int l = 0; l < kLevels; ++l)  // two dense passes over the fp32 logits + centerness
         bytes[6] += 2.0 * P.B * P.lvl_h[l] * P.lvl_w[l] * (C + 1) * 4;
 }
@@ -1995,7 +2034,12 @@ void Engine::forward_host(const void* h_images, int img_dtype, const float* h_K,
     cuda_check(cudaMemcpyAsync(P.d_K, h_K, static_cast<size_t>(P.B) * 36, cudaMemcpyHostToDevice, stream), "H2D K");
     cuda_check(cudaMemcpyAsync(P.d_sizes, h_sizes, static_cast<size_t>(P.B) * 16, cudaMemcpyHostToDevice, stream),
                "H2D sizes");
-    forward(P.d_images, img_dtype, P.d_K, P.d_sizes, P.d_out, P.d_counts, stream);
+    if (P.bev) {
+        if (host_poses[0].size() != static_cast<size_t>(P.B) * 7) fail(DD3D_ERR_STATE, "BEV NMS is on: dd3d_set_host_poses(0, ...) first");
+        cuda_check(cudaMemcpyAsync(P.d_poses, host_poses[0].data(), host_poses[0].size() * 4, cudaMemcpyHostToDevice, stream),
+                   "H2D poses");
+    }
+    forward(P.d_images, img_dtype, P.d_K, P.d_sizes, P.d_out, P.d_counts, P.d_poses, stream);
     cuda_check(cudaMemcpyAsync(h_out, P.d_out, static_cast<size_t>(P.B) * desc.out_cap * sizeof(Det),
                                cudaMemcpyDeviceToHost, stream),
                "D2H dets");
@@ -2025,27 +2069,35 @@ void Engine::submit_host(int slot, const void* h_images, int img_dtype, const fl
     if (slot == 1 && P.slot1 == nullptr) {
         const size_t a = 1024;
         auto up = [&](size_t n) { return (n + a - 1) / a * a; };
-        const size_t total = up(img_cap) + up(P.B * 36) + up(P.B * 16) + up(out_bytes) + up(P.B * 4);
+        const size_t total = up(img_cap) + up(P.B * 36) + up(P.B * 16) + up(out_bytes) + up(P.B * 4) + (P.bev ? up(P.B * 28) : 0);
         cuda_check(cudaMalloc(&P.slot1, total), "cudaMalloc(slot 1 staging)");
         uint8_t* q = static_cast<uint8_t*>(P.slot1);
         P.s1_images = q; q += up(img_cap);
         P.s1_K = reinterpret_cast<float*>(q); q += up(P.B * 36);
         P.s1_sizes = reinterpret_cast<int32_t*>(q); q += up(P.B * 16);
         P.s1_out = reinterpret_cast<Det*>(q); q += up(out_bytes);
-        P.s1_counts = reinterpret_cast<int32_t*>(q);
+        P.s1_counts = reinterpret_cast<int32_t*>(q); q += up(P.B * 4);
+        if (P.bev) P.s1_poses = reinterpret_cast<float*>(q);
     }
     void* d_img = slot ? P.s1_images : P.d_images;
     float* d_K = slot ? P.s1_K : P.d_K;
     int32_t* d_sz = slot ? P.s1_sizes : P.d_sizes;
     Det* d_out = slot ? P.s1_out : P.d_out;
     int32_t* d_cnt = slot ? P.s1_counts : P.d_counts;
+    float* d_poses = slot ? P.s1_poses : P.d_poses;
+    if (P.bev && host_poses[slot].size() != static_cast<size_t>(P.B) * 7)
+        fail(DD3D_ERR_STATE, "BEV NMS is on: dd3d_set_host_poses(slot, ...) first");
     const size_t img_bytes = static_cast<size_t>(P.B) * 3 * P.Hs * P.Ws * (img_dtype == DD3D_IMG_U8 ? 1 : 4);
     cuda_check(cudaMemcpyAsync(d_img, h_images, img_bytes, cudaMemcpyHostToDevice, copy_stream), "H2D images");
     cuda_check(cudaMemcpyAsync(d_K, h_K, static_cast<size_t>(P.B) * 36, cudaMemcpyHostToDevice, copy_stream), "H2D K");
     cuda_check(cudaMemcpyAsync(d_sz, h_sizes, static_cast<size_t>(P.B) * 16, cudaMemcpyHostToDevice, copy_stream), "H2D sizes");
+    if (P.bev)  // pageable source: staged before the call returns, so the next dd3d_set_host_poses may overwrite it
+        cuda_check(cudaMemcpyAsync(d_poses, host_poses[slot].data(), host_poses[slot].size() * 4, cudaMemcpyHostToDevice,
+                                   copy_stream),
+                   "H2D poses");
     cuda_check(cudaEventRecord(h2d_done[slot], copy_stream), "cudaEventRecord");
     cuda_check(cudaStreamWaitEvent(stream, h2d_done[slot], 0), "cudaStreamWaitEvent");
-    forward(d_img, img_dtype, d_K, d_sz, d_out, d_cnt, stream);
+    forward(d_img, img_dtype, d_K, d_sz, d_out, d_cnt, d_poses, stream);
     cuda_check(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, stream), "D2H dets");
     cuda_check(cudaMemcpyAsync(h_counts, d_cnt, static_cast<size_t>(P.B) * 4, cudaMemcpyDeviceToHost, stream), "D2H counts");
     cuda_check(cudaEventRecord(all_done[slot], stream), "cudaEventRecord");

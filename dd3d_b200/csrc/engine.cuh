@@ -134,6 +134,7 @@ struct Plan {
     int32_t* s1_sizes = nullptr;
     Det* s1_out = nullptr;
     int32_t* s1_counts = nullptr;
+    float* s1_poses = nullptr;  // BEV NMS on: slot 1's copy of the host poses
     View input;
     View fpn[kLevels];
     float* cls_map[kLevels] = {};
@@ -152,6 +153,10 @@ struct Plan {
     const float* d_canon = nullptr;
     DecodeParams decode;
     NmsParams nms;
+    // BEV NMS as the last op of the forward (dd3d_set_bev_nms): 0 off, else bev_nms_path() of the config at plan time
+    int bev = 0;
+    float* d_poses = nullptr;      // [B][7] staging of the host poses (host paths, slot 0)
+    void* bev_scratch = nullptr;   // image_bev_nms_scratch_bytes(B, out_cap) (multi-CTA path only)
     // sparse FCOS3D predictor (b3d_sparse.cu): the fused box3d conv runs only at the final 2-D candidates, between the two
     // halves of the decode; the dense fp32 maps b3d_map[] then do not exist
     bool sparse_b3d = false;
@@ -183,8 +188,9 @@ class Engine {
     int size_divisibility() const;
     size_t workspace_bytes(int B, int Hs, int Ws);
     void make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes);
+    // d_poses: [B][7] poses the BEV NMS reads (unused when it is off)
     void forward(const void* d_images, int img_dtype, const float* d_K, const int32_t* d_sizes, Det* d_out,
-                 int32_t* d_counts, cudaStream_t stream);
+                 int32_t* d_counts, const float* d_poses, cudaStream_t stream);
     void forward_host(const void* h_images, int img_dtype, const float* h_K, const int32_t* h_sizes, Det* h_out,
                       int32_t* h_counts, cudaStream_t stream);
     // double-buffered host path: H2D of one slot on a private copy stream while the other slot computes
@@ -202,6 +208,11 @@ class Engine {
                          cudaStream_t stream);
     void drop_plans();  // frees the active and the cached plans (an option that changes the op graph was flipped)
     int launches_per_forward() const;
+    // BEV NMS (DO_BEV_NMS): on / off and its IoU threshold; the poses of dd3d_forward / dd3d_forward_raw (device) and of
+    // the host paths (copied per slot)
+    void set_bev_nms(int enable, float thr);
+    int bev_mode() const;  // 0 off, else the bev_nms_path() the current options select
+    void set_host_poses(int slot, const float* h_poses);
     // categories: 0 preprocess, 1 stem and depthwise conv, 2 conv (wgmma), 3 pool, 4 eSE, 5 relu and GroupNorm, 6 decode, 7 nms
     void get_profile(double* ms, double* flops, double* bytes, int32_t* launches);
     int get_op_times(float* ms, int32_t* cats, double* flops, int max_ops);
@@ -250,6 +261,10 @@ class Engine {
                                      // >= 50 000 pixels)
     int opt_dla_front = 1;  // 1: DLA-34 base_layer + level0 + level1 (+ pool) as ONE kernel (dla_front.cu); 0: layer by layer
     int opt_workspace_fill = -1;  // >= 0: byte the whole arena is filled with at dd3d_plan (poison test)
+    int opt_bev_nms = 0;
+    float bev_nms_thresh = 0.f;
+    const float* user_poses = nullptr;   // dd3d_set_poses
+    std::vector<float> host_poses[2];    // dd3d_set_host_poses, per slot
     std::vector<cudaEvent_t> prof_ev;
     std::vector<int> prof_cat;
     std::vector<int> prof_op;  // plan op that ends at event i, or -1

@@ -99,6 +99,10 @@ SIGNATURES = {
     "dd3d_overflow_flags": (_I, [_P, _P, C.POINTER(C.c_int32)]),
     "dd3d_set_option": (_I, [_P, C.c_char_p, _I]),
     "dd3d_copy_flags": (_I, [_P, _P, _P]),
+    "dd3d_set_bev_nms": (_I, [_P, _I, C.c_float]),
+    "dd3d_set_poses": (_I, [_P, _P]),
+    "dd3d_set_host_poses": (_I, [_P, _I, _P]),
+    "dd3d_bev_nms_path": (_I, [C.POINTER(ModelDesc)]),
     "dd3d_packed_bytes": (_I64, [_I, _I]),
     "dd3d_comm_unique_id": (_I, [_P]),
     "dd3d_comm_create": (_I, [_P, _I, _I, C.POINTER(_P)]),
@@ -133,6 +137,8 @@ SIGNATURES = {
     "dd3d_op_ese_pool": (_I, [_P, _I, _P, _P, _P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_ese_scratch_bytes": (_I64, [_I, _I, _I]),
     "dd3d_op_bev_nms": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, C.c_float, _I, _P]),
+    "dd3d_op_bev_nms_large_scratch_bytes": (_I64, [_I, _I]),
+    "dd3d_op_bev_nms_large": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, C.c_float, _I, _P]),
     "dd3d_op_rotated_iou": (_I, [_P, _P, _I, _P, _P]),
     "dd3d_resize_shape": (_I, [_I, _I, _I, _I, _P, _P]),
     "dd3d_forward_raw": (_I, [_P, _P, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P]),

@@ -139,24 +139,24 @@ class DD3DB200(nn.Module):
 
     def _plan(self, B, Hs, Ws):
         key = (B, Hs, Ws)
-        if self._plan_key != key:
-            L = _lib.load()
-            handle = self._engine()  # raises (no CPU path / weights not loaded) before any CUDA call
+        L = _lib.load()
+        handle = self._engine()  # raises (no CPU path / weights not loaded) before any CUDA call
+        # a switch that changes the op graph (do_bev_nms, or do_nms under it) makes the engine drop its plans
+        if self._plan_key != key or L.dd3d_num_ops(handle) < 0:
             with torch.cuda.device(self._device):
                 _lib.check(L.dd3d_plan(handle, B, Hs, Ws, None, 0), self._handle)
             self._plan_key = key
             self._host_bufs = None
 
     def _sync_options(self, postprocess_in_forward):
-        """Pushes the attributes callers toggle at run time (postprocess_in_inference, do_nms: scripts/train.py:206-209,
-        core.py:134) to the engine.  Without NMS (or without a post-NMS top-k) up to 5 * PRE_NMS_TOPK detections per image
-        survive: an engine planned with the small NMS-sized output buffer is rebuilt with the large one instead of silently
-        truncating (the reference never truncates)."""
+        """Pushes the attributes callers toggle at run time (postprocess_in_inference, do_nms, do_bev_nms:
+        scripts/train.py:206-209, core.py:134-137) to the engine.  Without NMS (or without a post-NMS top-k) up to
+        5 * PRE_NMS_TOPK detections per image survive: an engine planned with the small NMS-sized output buffer is rebuilt
+        with the large one instead of silently truncating (the reference never truncates).  With do_bev_nms the engine
+        runs the BEV NMS as its last op, then detector_postprocess (core.py:137-160)."""
         inf = self.cfg.DD3D.FCOS2D.INFERENCE
         if self.do_bev_nms and self.only_box2d:
             self.do_bev_nms = False  # core.py:137: the BEV NMS needs the 3-D boxes
-        if self.do_bev_nms and not self.do_nms:
-            raise NotImplementedError("DO_BEV_NMS without DO_NMS: the BEV kernel expects the score-sorted output of the 2-D NMS")
         need = 5 * inf.PRE_NMS_TOPK if (not self.do_nms or inf.POST_NMS_TOPK <= 0) else 0
         if need > self._desc.out_cap:
             self._release()
@@ -165,6 +165,7 @@ class DD3DB200(nn.Module):
         h = self._engine()
         _lib.check(L.dd3d_set_option(h, b"do_postprocess", int(postprocess_in_forward)), h)
         _lib.check(L.dd3d_set_option(h, b"do_nms", int(self.do_nms)), h)
+        _lib.check(L.dd3d_set_bev_nms(h, int(self.do_bev_nms), float(self.bev_nms_iou_thresh)), h)
 
     def _check_flags(self, flags):
         """Overflow word of the last forward (folded into the counts D2H): any set bit means the output differs from the
@@ -173,7 +174,7 @@ class DD3DB200(nn.Module):
         if flags:
             names = {2: "more detections than out_cap slots", 4: "more than 256 boxes entered the BEV NMS of one image",
                      8: "sample aggregation capacity exceeded", 16: "more merged TTA detections than slots",
-                     32: "grouped BEV NMS capacity exceeded"}
+                     32: "grouped BEV NMS capacity exceeded", 64: "more than out_cap boxes entered the BEV NMS of one image"}
             raise RuntimeError("DD3DB200: detection capacity exceeded (" +
                                "; ".join(v for k, v in names.items() if flags & k) + f"; flags={int(flags)})")
 
@@ -273,8 +274,6 @@ class DD3DB200(nn.Module):
 
     def _forward_device_raw(self, raw_inputs):
         device = self._device
-        if self.do_bev_nms:
-            raise NotImplementedError("forward_raw with DO_BEV_NMS: run the mapper-style forward()")
         L = _lib.load()
         imgs = [torch.as_tensor(x["image_hwc"]) for x in raw_inputs]
         if not all(im.dtype == torch.uint8 and im.dim() == 3 and im.shape[2] == 3 for im in imgs):
@@ -304,6 +303,7 @@ class DD3DB200(nn.Module):
         cap = self._desc.out_cap
         K = torch.empty((B, 9), dtype=torch.float32)
         with torch.cuda.device(device):
+            d_poses = self._set_device_poses(raw_inputs)
             d_raw = raw.to(device, non_blocking=True)
             out = torch.empty((B, cap, _lib.DET_WORDS), dtype=torch.float32, device=device)
             counts = torch.zeros((B + 1, ), dtype=torch.int32, device=device)  # [B] counts + overflow word
@@ -316,13 +316,26 @@ class DD3DB200(nn.Module):
             _lib.check(L.dd3d_copy_flags(self._handle, C.c_void_p(counts[B:].data_ptr()), C.c_void_p(stream)), self._handle)
             d_K = K.to(device, non_blocking=True)
         sizes = torch.cat([new_sizes, raw_sizes if self.postprocess_in_inference else new_sizes], 1)
-        return dict(out=out, counts=counts, K=K, sizes=sizes, d_K=d_K, B=B, cap=cap, stream=stream)
+        return dict(out=out, counts=counts, K=K, sizes=sizes, d_K=d_K, B=B, cap=cap, stream=stream, d_poses=d_poses)
+
+    def _set_device_poses(self, batched_inputs):
+        """With do_bev_nms: the [B][7] poses on the device, handed to the engine for the next forward (kept alive by the
+        caller until that forward is enqueued)."""
+        if not self.do_bev_nms:
+            return None
+        d_poses = self._gather_poses(batched_inputs).to(self._device, non_blocking=True)
+        _lib.check(_lib.load().dd3d_set_poses(self._handle, C.c_void_p(d_poses.data_ptr())), self._handle)
+        return d_poses
+
+    def _set_host_poses(self, batched_inputs, slot):
+        if self.do_bev_nms:
+            poses = self._gather_poses(batched_inputs).contiguous()
+            _lib.check(_lib.load().dd3d_set_host_poses(self._handle, int(slot), C.c_void_p(poses.data_ptr())), self._handle)
 
     def _forward_device(self, batched_inputs):
         device = self._device
         batch, K, sizes, shape, is_u8 = self._gather_inputs(batched_inputs, device)
-        # with BEV NMS the rescale/clip happens after it (core.py:137-160): the BEV kernel applies it then
-        self._sync_options(self.postprocess_in_inference and not self.do_bev_nms)
+        self._sync_options(self.postprocess_in_inference)
         self._plan(*shape)
         L = _lib.load()
         B = shape[0]
@@ -331,6 +344,7 @@ class DD3DB200(nn.Module):
             d_batch = batch.to(device, non_blocking=True)
             d_K = K.to(device, non_blocking=True)
             d_sizes = sizes.to(device, non_blocking=True)
+            d_poses = self._set_device_poses(batched_inputs)
             out = torch.empty((B, cap, _lib.DET_WORDS), dtype=torch.float32, device=device)
             counts = torch.zeros((B + 1, ), dtype=torch.int32, device=device)  # [B] counts + overflow word
             stream = torch.cuda.current_stream(device).cuda_stream
@@ -339,16 +353,7 @@ class DD3DB200(nn.Module):
                                C.c_void_p(d_K.data_ptr()), C.c_void_p(d_sizes.data_ptr()), C.c_void_p(out.data_ptr()),
                                C.c_void_p(counts.data_ptr()), C.c_void_p(stream)), self._handle)
             _lib.check(L.dd3d_copy_flags(self._handle, C.c_void_p(counts[B:].data_ptr()), C.c_void_p(stream)), self._handle)
-            if self.do_bev_nms:
-                d_poses = self._gather_poses(batched_inputs).to(device, non_blocking=True)
-                self._bev_flags = torch.zeros(1, dtype=torch.int32, device=device)
-                _lib.check(
-                    L.dd3d_op_bev_nms(C.c_void_p(out.data_ptr()), C.c_void_p(counts.data_ptr()), C.c_void_p(d_K.data_ptr()),
-                                      C.c_void_p(d_poses.data_ptr()), C.c_void_p(d_sizes.data_ptr()),
-                                      C.c_void_p(self._bev_flags.data_ptr()), B, cap, float(self.bev_nms_iou_thresh),
-                                      int(self.postprocess_in_inference), C.c_void_p(stream)), self._handle)
-                counts[B:] |= self._bev_flags  # bit 2 rides in the same overflow word
-        return dict(out=out, counts=counts, K=K, sizes=sizes, d_K=d_K, B=B, cap=cap, stream=stream)
+        return dict(out=out, counts=counts, K=K, sizes=sizes, d_K=d_K, B=B, cap=cap, stream=stream, d_poses=d_poses)
 
     def __call__(self, batched_inputs):
         return self.forward(batched_inputs)
@@ -356,8 +361,6 @@ class DD3DB200(nn.Module):
     @torch.no_grad()
     def forward_host(self, batched_inputs):
         """End-to-end path through HOST buffers: pinned staging -> dd3d_forward_host (H2D, kernels, D2H, sync)."""
-        if self.do_bev_nms:  # the BEV NMS runs on the device buffers: device forward, then the results to the host
-            return [{"instances": o["instances"].to("cpu")} for o in self.forward(batched_inputs)]
         batch, K, sizes, shape, is_u8 = self._gather_inputs(batched_inputs, self._device)
         self._sync_options(self.postprocess_in_inference)
         self._plan(*shape)
@@ -374,6 +377,7 @@ class DD3DB200(nn.Module):
         hb["img"].copy_(batch)
         hb["K"].copy_(K)
         hb["sizes"].copy_(sizes)
+        self._set_host_poses(batched_inputs, 0)
         with torch.cuda.device(self._device):
             stream = torch.cuda.current_stream(self._device).cuda_stream
             _lib.check(
@@ -389,9 +393,6 @@ class DD3DB200(nn.Module):
         """Double-buffered host path (dd3d_submit_host): enqueues H2D -> kernels -> D2H for `slot` (0 / 1) and returns;
         ``wait_host(slot)`` returns the results.  Submitting the next batch to the other slot before waiting overlaps
         its H2D with the current batch's kernels.  All batches of a pipeline must share one plan shape."""
-        if self.do_bev_nms:
-            raise NotImplementedError("submit_host with DO_BEV_NMS: use forward() / forward_host() (the BEV NMS kernel runs on "
-                                      "the device buffers before the D2H)")
         batch, K, sizes, shape, is_u8 = self._gather_inputs(batched_inputs, self._device)
         self._sync_options(self.postprocess_in_inference)
         self._plan(*shape)
@@ -410,6 +411,7 @@ class DD3DB200(nn.Module):
         hb["K"].copy_(K)
         hb["sizes"].copy_(sizes)
         hb["ctx"] = (K, sizes)
+        self._set_host_poses(batched_inputs, slot)
         with torch.cuda.device(self._device):
             stream = torch.cuda.current_stream(self._device).cuda_stream
             _lib.check(
@@ -480,10 +482,7 @@ class DD3DB200(nn.Module):
         flags = C.c_int32(0)
         stream = torch.cuda.current_stream(self._device).cuda_stream
         _lib.check(_lib.load().dd3d_overflow_flags(self._handle, C.c_void_p(stream), C.byref(flags)), self._handle)
-        f = flags.value
-        if getattr(self, "_bev_flags", None) is not None:
-            f |= int(self._bev_flags.item())
-        return f
+        return flags.value
 
 
 def group_indices(sample_tokens, num_images_per_sample):

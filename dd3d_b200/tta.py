@@ -99,6 +99,8 @@ class _DeviceTTA(nn.Module):
         counts = torch.empty((A, ), dtype=torch.int32, device=device)
         if bev:  # the model's own forward runs the per-image BEV NMS on every view (core.py:137-151, x["pose"])
             pose = model._gather_poses([x]).to(device, non_blocking=True)
+        # that BEV NMS runs below, after each chunk of views, with the views' intrinsics: not as the engine's last op
+        _lib.check(L.dd3d_set_bev_nms(model._engine(), 0, float(model.bev_nms_iou_thresh)), model._handle)
         # chunks of `batch_size` views, each padded to the chunk's largest view like ImageList.from_tensors does for
         # one model(inputs) call (test_time_augmentation.py:118-133)
         for a0 in range(0, A, self.batch_size):

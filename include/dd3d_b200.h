@@ -198,7 +198,8 @@ int dd3d_submit_host(dd3d_handle h, int slot, const void* h_images, int img_dtyp
                      const int32_t* h_sizes, dd3d_det* h_out, int32_t* h_counts, dd3d_stream stream);
 int dd3d_wait_host(dd3d_handle h, int slot);
 /* bit 0: unused (the pre-NMS top-k is exact for every input and sets no bit); bit 1: more than out_cap detections
- * survived.  Reads a device word (synchronises `stream`). */
+ * survived; with the BEV NMS on (dd3d_set_bev_nms), bit 2: more than 256 boxes reached the one-CTA BEV kernel of an
+ * image, bit 6: a count above out_cap reached the multi-CTA one.  Reads a device word (synchronises `stream`). */
 int dd3d_overflow_flags(dd3d_handle h, dd3d_stream stream, int32_t* h_flags);
 /* Runtime switches the reference's callers toggle on the meta-arch: "do_postprocess" (postprocess_in_inference,
  * scripts/train.py:206-209, test_time_augmentation.py:107), "do_nms" (core.py:134), "profile" (see
@@ -222,6 +223,27 @@ int dd3d_overflow_flags(dd3d_handle h, dd3d_stream stream, int32_t* h_flags);
  * memory, for stage-level tests; applies to plans made afterwards), and "workspace_fill" (0..255: dd3d_plan fills the whole workspace with that byte first, -1 = off;
  * the poison test of tests/test_determinism_gpu.py: results must not depend on what the arena held). */
 int dd3d_set_option(dd3d_handle h, const char* name, int value);
+
+/* ---- BEV NMS (DD3D.INFERENCE.DO_BEV_NMS, core.py:137-151) as the last op of every forward ----------------------------
+ * dd3d_set_bev_nms(h, 1, thr): every following dd3d_forward / dd3d_forward_host / dd3d_submit_host / dd3d_forward_raw
+ * ends with the reference's per-image BEV NMS (boxes to the global frame through the image's pose, class-aware rotated
+ * NMS on scores_3d with IoU threshold BEV_NMS_IOU_THRESH; survivors keep their order), and option "do_postprocess" then
+ * applies detector_postprocess after it instead of inside the 2-D NMS (core.py:153-160).  Needs box3d_on.  The kernel is
+ * chosen from the config (dd3d_bev_nms_path); turning the BEV NMS on or off, or a "do_nms" change that switches the
+ * kernel, drops the engine's plans (call dd3d_plan again).  With it off the op list, the launches and the workspace are
+ * those of an engine that never had it.
+ * Poses: [B][7] sensor->global pose of each image (quaternion w, x, y, z + translation; input["pose"] /
+ * input["extrinsics"]).  dd3d_set_poses: a DEVICE buffer read by every following dd3d_forward / dd3d_forward_raw (kept
+ * until replaced; it must stay valid while those forwards run).  dd3d_set_host_poses: a HOST array of the current plan's
+ * B images, copied at the call, for dd3d_forward_host (slot 0) and dd3d_submit_host (slot 0 / 1).  A forward with the BEV
+ * NMS on and no poses returns DD3D_ERR_STATE. */
+int dd3d_set_bev_nms(dd3d_handle h, int enable, float iou_thresh);
+int dd3d_set_poses(dd3d_handle h, const float* d_poses);
+int dd3d_set_host_poses(dd3d_handle h, int slot, const float* h_poses);
+/* The BEV NMS kernel a config runs (no device needed): 1 = the one-CTA kernel of dd3d_op_bev_nms (do_nms and
+ * 0 < post_nms_topk <= 256: at most 256 score-sorted boxes per image), 2 = the multi-CTA kernels of dd3d_op_bev_nms_large
+ * (every other config: up to 5 * pre_nms_topk unsorted boxes per image). */
+int dd3d_bev_nms_path(const dd3d_model_desc* h_desc);
 /* Process-wide kernel-selection policy for plans / operator calls made afterwards (tests, A/B measurements):
  * "op_fp16" = 1: the dd3d_op_* entry points below treat their 16-bit buffers as fp16 (default 0: bf16).
  * "nms_class_parallel" = 0: one CTA per image does the whole NMS instead of the multi-CTA path (rank sort, IoU bit matrix on
@@ -409,10 +431,20 @@ int dd3d_op_ese_pool(const void* d_x, int x_pitch, const float* d_fc_w, const fl
  * tridet/layers/bev_nms.py:51-133 -> detectron2 batched_nms_rotated), in place on the detections a dd3d_forward run
  * with option "do_postprocess" = 0 produced: d_dets [B][cap], d_counts [B].  d_poses: [B][7] sensor->global pose of
  * each image (quaternion w,x,y,z + translation; input["pose"] / input["extrinsics"]).  Applies detector_postprocess
- * afterwards when do_postprocess != 0.  d_flags: one int32 word, bit 2 set if an image had more than 256 boxes. */
+ * afterwards when do_postprocess != 0.  d_flags: one int32 word, bit 2 set if an image had more than 256 boxes.  The input
+ * must be sorted by scores_3d (the 2-D NMS output); dd3d_op_bev_nms_large takes any order and size. */
 int dd3d_op_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsics, const float* d_poses,
                     const int32_t* d_sizes, int32_t* d_flags, int B, int cap, float iou_thresh, int do_postprocess,
                     dd3d_stream stream);
+/* dd3d_op_bev_nms_large: the same BEV NMS on the multi-CTA kernels of csrc/bev_nms_group.cu for up to 5 * 1150 boxes per
+ * image in any order (cap <= 5750): per image a sort by (class, scores_3d descending, slot), the rotated-IoU bit matrix on
+ * all SMs, one greedy scan per (image, class), then an order-preserving compaction (with detector_postprocess when
+ * do_postprocess != 0).  d_scratch: dd3d_op_bev_nms_large_scratch_bytes(B, cap) bytes, any content (about
+ * min(B, 256) * cap^2 / 8 bytes: the IoU bit matrix).  d_flags bit 6 (64): a count above cap. */
+int64_t dd3d_op_bev_nms_large_scratch_bytes(int B, int cap);
+int dd3d_op_bev_nms_large(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsics, const float* d_poses,
+                          const int32_t* d_sizes, void* d_scratch, int32_t* d_flags, int B, int cap, float iou_thresh,
+                          int do_postprocess, dd3d_stream stream);
 /* d_out[i] = rotated IoU of the BEV rectangles d_a[i] and d_b[i] (rows of 5 floats: cx, cy, w, h, angle in degrees;
  * detectron2's single_box_iou_rotated), one thread per pair: the function the three BEV NMS kernels threshold, exposed
  * for tests. */
