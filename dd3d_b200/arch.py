@@ -179,14 +179,15 @@ def param_specs(cfg):
         feats = _vovnet(specs, arch, norm)
         stages = {"stage2": 2, "stage3": 3, "stage4": 4, "stage5": 5}
     fpn_norm = cfg.FE.FPN.NORM  # detectron2 FPN: bias only without a norm; one norm per conv
+    F = fpn_channels(cfg)  # the FPN's width is every head's width too (fcos2d.py:43-45, fcos3d.py:70-72)
     for name, ch in feats.items():
         st = stages[name]
-        for conv, cin, k in ((f"backbone.fpn_lateral{st}", ch, 1), (f"backbone.fpn_output{st}", 256, 3)):
-            _conv(specs, conv, 256, cin, k, bias=fpn_norm == "", role="linear")
-            _norm(specs, conv + ".norm", 256, fpn_norm)
-    _conv(specs, "backbone.top_block.p6", 256, 256, 3, bias=True, role="linear")
+        for conv, cin, k in ((f"backbone.fpn_lateral{st}", ch, 1), (f"backbone.fpn_output{st}", F, 3)):
+            _conv(specs, conv, F, cin, k, bias=fpn_norm == "", role="linear")
+            _norm(specs, conv + ".norm", F, fpn_norm)
+    _conv(specs, "backbone.top_block.p6", F, F, 3, bias=True, role="linear")
     if arch in DLA_SPECS:
-        _conv(specs, "backbone.top_block.p7", 256, 256, 3, bias=True, role="linear")
+        _conv(specs, "backbone.top_block.p7", F, F, 3, bias=True, role="linear")
 
     C = cfg.DD3D.NUM_CLASSES
     L = 5
@@ -198,17 +199,17 @@ def param_specs(cfg):
     if box3d_on:
         towers.append(("fcos3d_head.box3d_tower", f3.NUM_CONVS, f3.NORM))
     for tower, depth, norm in towers:
-        _norm({}, "", 256, norm)  # KeyError for an unknown NORM even at depth 0
+        _norm({}, "", 32, norm)  # KeyError for an unknown NORM even at depth 0
         for i in range(depth):
-            _conv(specs, f"{tower}.{i}", 256, 256, 3, bias=norm == "")
+            _conv(specs, f"{tower}.{i}", F, F, 3, bias=norm == "")
             if norm in ("BN", "FrozenBN"):
                 for l in range(L):
-                    _norm(specs, f"{tower}.{i}.norm.{l}", 256, norm)
+                    _norm(specs, f"{tower}.{i}.norm.{l}", F, norm)
             else:
-                _norm(specs, f"{tower}.{i}.norm", 256, norm)
-    _conv(specs, "fcos2d_head.cls_logits", C, 256, 3, bias=True, role="cls_logits")
-    _conv(specs, "fcos2d_head.box2d_reg", 4, 256, 3, bias=True, role="box2d_reg")
-    _conv(specs, "fcos2d_head.centerness", 1, 256, 3, bias=True, role="centerness")
+                _norm(specs, f"{tower}.{i}.norm", F, norm)
+    _conv(specs, "fcos2d_head.cls_logits", C, F, 3, bias=True, role="cls_logits")
+    _conv(specs, "fcos2d_head.box2d_reg", 4, F, 3, bias=True, role="box2d_reg")
+    _conv(specs, "fcos2d_head.centerness", 1, F, 3, bias=True, role="centerness")
     if f2.USE_SCALE:  # fcos2d.py:100-108
         for l in range(L):
             specs[f"fcos2d_head.scales_box2d_reg.{l}.scale"] = ((1, ), "scalar:box2d")
@@ -221,7 +222,7 @@ def param_specs(cfg):
                                        ("depth", 1, "depth", not f3.USE_SCALE),  # fcos3d.py:116
                                        ("size", 3, "size", True), ("conf", 1, "conf", True)):
             for li in range(NL):
-                _conv(specs, f"fcos3d_head.box3d_{name}.{li}", mult * C3, 256, 3, bias=bias, role=role)
+                _conv(specs, f"fcos3d_head.box3d_{name}.{li}", mult * C3, F, 3, bias=bias, role=role)
         if f3.USE_SCALE:  # fcos3d.py:128-139
             for l in range(L):
                 specs[f"fcos3d_head.scales_proj_ctr.{l}.scale"] = ((1, ), "scalar:ctr")
@@ -230,12 +231,31 @@ def param_specs(cfg):
                 specs[f"fcos3d_head.scales_depth.{l}.scale"] = ((1, ), "scalar:depth")
                 specs[f"fcos3d_head.offsets_depth.{l}.bias"] = ((1, ), "scalar:depth_offset")
     if is_nuscenes_arch(cfg):  # nuscenes_dd3d.py:311-312 (appended last: the synthetic generator stream of the rest is unchanged)
-        _conv(specs, "attr_logits", MAX_NUM_ATTRIBUTES, 256, 3, bias=True, role="attr")
-        _conv(specs, "speed", 1, 256, 3, bias=True, role="speed")
+        _conv(specs, "attr_logits", MAX_NUM_ATTRIBUTES, F, 3, bias=True, role="attr")
+        _conv(specs, "speed", 1, F, 3, bias=True, role="speed")
     return specs
 
 
 MAX_NUM_ATTRIBUTES = 3  # tridet/data/datasets/nuscenes/build.py:77
+
+# FE.FPN.OUT_CHANNELS the engine builds (dd3d_set_fpn_channels): every multiple of 64 from 64 to 512
+FPN_WIDTHS = tuple(range(64, 513, 64))
+
+
+def fpn_channels(cfg):
+    """FE.FPN.OUT_CHANNELS (configs/feature_extractors/d2_fpn.yaml:5; the reference's FPN builders read it, dla.py:546-557,
+    vovnet.py:438-450): the width of the FPN laterals, outputs and top block and of every FCOS head conv."""
+    return int(cfg.FE.FPN.OUT_CHANNELS)
+
+
+def check_fpn_channels(cfg):
+    """NotImplementedError for an FPN width the reference builds and the engine does not.  Call it after param_specs, which
+    raises the reference's own errors first (GN on a width that 32 does not divide: nn.GroupNorm's ValueError)."""
+    c = fpn_channels(cfg)
+    if c not in FPN_WIDTHS:
+        raise NotImplementedError(f"FE.FPN.OUT_CHANNELS = {c} is not supported: the engine builds "
+                                  + ", ".join(str(w) for w in FPN_WIDTHS))
+    return c
 
 
 def is_nuscenes_arch(cfg):

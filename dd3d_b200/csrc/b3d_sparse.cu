@@ -5,12 +5,13 @@
 // 2-D candidates).  Dense, the layer is 0.53 TFLOP of a V2-99 step (32 x 127 875 pixels x 2304 x 110); the
 // bench batch keeps ~1 100 candidates per image: 115 x fewer rows.
 //
-// Gathered GEMM: row = one final candidate (image b, level l, slot) of decode.cu's `fin` list, K = 9 taps x 256 channels read
-// straight from the NHWC tower output at the candidate's 3x3 neighbourhood (zeros outside the map), N = the fused predictor's
+// Gathered GEMM: row = one final candidate (image b, level l, slot) of decode.cu's `fin` list, K = 9 taps x cin channels (the
+// FPN width FE.FPN.OUT_CHANNELS: a multiple of 64, 256 by default) read straight from the NHWC tower output at the candidate's 3x3 neighbourhood (zeros outside the map), N = the fused predictor's
 // output channels.  One CTA = 128 rows of one (image, level); warp = 16 rows x all N in registers (mma.sync m16n8k16, fp32
 // accumulate -- the rows are gathered per lane with 16-byte loads, which is exactly the fragment layout once K is permuted
-// identically on both operands; the work is ~20 GFLOP per step, the tensor path is not the limit).  The weight tile of a
-// 64-channel block is staged in shared memory by cp.async (double buffered) and shared by the 8 warps.
+// identically on both operands; the work is ~20 GFLOP per step, the tensor path is not the limit).  The K loop runs over
+// 9 x cin / 64 blocks in (tap, 64-channel block) order, so every width sums in the same order as the 256-wide layer.  The
+// weight tile of a 64-channel block is staged in shared memory by cp.async (double buffered) and shared by the 8 warps.
 // Output: fp32 rows [(b * L + l) * topk + slot][pitch] in the channel layout of a dense map pixel; decode_final_kernel reads
 // them through DecodeParams::b3d_rows.
 #include <cuda_bf16.h>
@@ -26,8 +27,7 @@ namespace dd3d {
 namespace {
 
 constexpr int kRowsPerCta = 128, kThreads = 256;
-constexpr int kCin = 256, kChunk = 64;  // channels per shared-memory weight block
-constexpr int kChunks = 9 * (kCin / kChunk);
+constexpr int kChunk = 64;  // channels per shared-memory weight block
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
@@ -56,18 +56,20 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
 
-// weight block (tap, kc) of predictor `w` -> smem [n_pad rows][128 B], 16-byte chunk q of row n stored at q ^ ((n & 1) << 2)
+// weight block `chunk` = (tap, kc) of predictor `w` ([n_pad][9][cin]) -> smem [n_pad rows][128 B], 16-byte chunk q of row n stored at q ^ ((n & 1) << 2)
 // (the two rows a quarter-warp reads with one LDS.128 then sit in different halves of the 128-byte line: conflict-free)
-__device__ __forceinline__ void stage_weights(const __nv_bfloat16* w, int n_pad, int chunk, uint32_t dst) {
-    const int tap = chunk >> 2, kc = chunk & 3;
-    const __nv_bfloat16* src = w + tap * kCin + kc * kChunk;
+__device__ __forceinline__ void stage_weights(const __nv_bfloat16* w, int n_pad, int kcs, int chunk, uint32_t dst) {
+    const int cin = kcs * kChunk, tap = chunk / kcs, kc = chunk - tap * kcs;
+    const __nv_bfloat16* src = w + tap * cin + kc * kChunk;
     for (int i = threadIdx.x; i < n_pad * 8; i += kThreads) {
         const int n = i >> 3, q = i & 7;
-        cp_async16(dst + n * 128 + ((q ^ ((n & 1) << 2)) << 4), src + static_cast<size_t>(n) * (9 * kCin) + q * 8);
+        cp_async16(dst + n * 128 + ((q ^ ((n & 1) << 2)) << 4), src + static_cast<size_t>(n) * (9 * cin) + q * 8);
     }
 }
 
-template <int NT, bool FP16>
+// KCS: 64-channel blocks per tap (cin / 64) as a compile-time constant (4: the default 256-wide FPN), or 0 to read it from
+// p.cin at run time (every other width; the runtime division costs 16 registers)
+template <int NT, bool FP16, int KCS>
 __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel(const B3dSparseParams p) {
     DD3D_PDL_PROLOGUE();
     extern __shared__ __align__(16) uint8_t smem[];
@@ -78,6 +80,7 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel(const B3dSparsePar
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
     const int nt_real = p.n_pad >> 3;
+    const int kcs = KCS > 0 ? KCS : p.cin / kChunk, chunks = 9 * kcs;
     const uint32_t s_w = smem_u32(smem);
     const uint32_t buf_bytes = static_cast<uint32_t>(p.n_pad) * 128;
     const B3dSparseLevel& L = p.lvl[l];
@@ -97,7 +100,7 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel(const B3dSparsePar
         base[h] = L.in + (static_cast<size_t>(b * L.H + py[h]) * L.W + px[h]) * L.pitch + 8 * t;
     }
     auto load_a = [&](int chunk, uint4 (&a)[2][2]) {  // [group of 32 channels][row half]
-        const int tap = chunk >> 2, kc = chunk & 3;
+        const int tap = chunk / kcs, kc = chunk - tap * kcs;
         const int dy = tap / 3 - 1, dx = tap % 3 - 1;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -116,12 +119,12 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel(const B3dSparsePar
         for (int j = 0; j < 4; ++j) acc[nt][j] = 0.f;
 
     uint4 a_cur[2][2], a_nxt[2][2];
-    stage_weights(L.w, p.n_pad, 0, s_w);
+    stage_weights(L.w, p.n_pad, kcs, 0, s_w);
     asm volatile("cp.async.commit_group;" ::: "memory");
     load_a(0, a_cur);
-    for (int c = 0; c < kChunks; ++c) {
-        if (c + 1 < kChunks) {
-            stage_weights(L.w, p.n_pad, c + 1, s_w + ((c + 1) & 1) * buf_bytes);
+    for (int c = 0; c < chunks; ++c) {
+        if (c + 1 < chunks) {
+            stage_weights(L.w, p.n_pad, kcs, c + 1, s_w + ((c + 1) & 1) * buf_bytes);
             load_a(c + 1, a_nxt);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
@@ -171,12 +174,17 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel(const B3dSparsePar
     }
 }
 
-template <int NT>
+template <int NT, int KCS>
 cudaError_t launch_nt(const B3dSparseParams& p, cudaStream_t stream) {
     const int smem = 2 * p.n_pad * 128;
     dim3 grid((p.topk + kRowsPerCta - 1) / kRowsPerCta, kLevels, p.B);
-    if (p.fp16) return launch_pdl(b3d_sparse_kernel<NT, true>, grid, dim3(kThreads), smem, stream, p);
-    return launch_pdl(b3d_sparse_kernel<NT, false>, grid, dim3(kThreads), smem, stream, p);
+    if (p.fp16) return launch_pdl(b3d_sparse_kernel<NT, true, KCS>, grid, dim3(kThreads), smem, stream, p);
+    return launch_pdl(b3d_sparse_kernel<NT, false, KCS>, grid, dim3(kThreads), smem, stream, p);
+}
+
+template <int NT>
+cudaError_t launch_cin(const B3dSparseParams& p, cudaStream_t stream) {
+    return p.cin == 256 ? launch_nt<NT, 4>(p, stream) : launch_nt<NT, 0>(p, stream);
 }
 
 }  // namespace
@@ -184,10 +192,12 @@ cudaError_t launch_nt(const B3dSparseParams& p, cudaStream_t stream) {
 cudaError_t launch_b3d_sparse(const B3dSparseParams& p, cudaStream_t stream) {
     if (p.n_pad < 8 || p.n_pad % 8 || p.n_pad > kB3dSparseMaxN || p.out_pitch < p.n_pad || p.out_pitch % 2 || p.B < 1 || p.topk < 1)
         return cudaErrorInvalidValue;
+    if (p.cin < kChunk || p.cin % kChunk || p.cin > kB3dSparseMaxCin) return cudaErrorInvalidValue;
     for (int l = 0; l < kLevels; ++l)
-        if (p.lvl[l].pitch % 8 || p.lvl[l].in == nullptr || p.lvl[l].w == nullptr) return cudaErrorInvalidValue;
-    if (p.n_pad <= 64) return launch_nt<8>(p, stream);    // C3 <= 5 (KITTI: 5 classes -> 55 -> 64), class-agnostic (11 -> 16)
-    return launch_nt<14>(p, stream);                       // nuScenes: 10 classes -> 110 -> 112
+        if (p.lvl[l].pitch % 8 || p.lvl[l].pitch < p.cin || p.lvl[l].in == nullptr || p.lvl[l].w == nullptr)
+            return cudaErrorInvalidValue;
+    if (p.n_pad <= 64) return launch_cin<8>(p, stream);   // C3 <= 5 (KITTI: 5 classes -> 55 -> 64), class-agnostic (11 -> 16)
+    return launch_cin<14>(p, stream);                      // nuScenes: 10 classes -> 110 -> 112
 }
 
 }  // namespace dd3d

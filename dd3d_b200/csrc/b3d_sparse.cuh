@@ -9,8 +9,8 @@
 namespace dd3d {
 
 struct B3dSparseLevel {
-    const __nv_bfloat16* in;  // box3d tower output of the level, NHWC 16-bit [B][H][W][pitch], 256 channels
-    const __nv_bfloat16* w;   // fused predictor weights [n_pad][9][256] (engine conv_layer layout; per level when PER_LEVEL_PREDICTORS)
+    const __nv_bfloat16* in;  // box3d tower output of the level, NHWC 16-bit [B][H][W][pitch], cin channels
+    const __nv_bfloat16* w;   // fused predictor weights [n_pad][9][cin] (engine conv_layer layout; per level when PER_LEVEL_PREDICTORS)
     const float* scale;       // [n_pad] per-level epilogue (Scale folded)
     const float* bias;        // [n_pad] conv bias * scale (+ depth Offset)
     int H, W, pitch;
@@ -22,11 +22,13 @@ struct B3dSparseParams {
     const int32_t* cand_count;  // [B][L]
     float* rows;                // [B][L][topk][out_pitch] fp32, channel layout of a dense map pixel
     int B, C, topk, n_pad, out_pitch, fp16;
+    int cin;  // tower width (FE.FPN.OUT_CHANNELS): a multiple of 64 in [64, kB3dSparseMaxCin]
 };
 
 // widest fused predictor the kernel is instantiated for (14 n-tiles of 8: the 10 nuScenes classes); the engine keeps the dense
 // predictor for models with more 3-D output channels
 constexpr int kB3dSparseMaxN = 112;
+constexpr int kB3dSparseMaxCin = 512;  // widest FPN the engine builds
 cudaError_t launch_b3d_sparse(const B3dSparseParams& p, cudaStream_t stream);
 
 // Sparse box3d tower (tower_tiles.cu): the sparse predictor reads the tower output only in the 3x3 neighbourhoods of the

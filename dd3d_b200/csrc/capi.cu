@@ -86,6 +86,10 @@ int dd3d_set_backbone_norm(dd3d_handle h, int32_t norm) {
     return guarded(h, [&](Engine& e) { e.set_backbone_norm(norm); });
 }
 
+int dd3d_set_fpn_channels(dd3d_handle h, int32_t channels) {
+    return guarded(h, [&](Engine& e) { e.set_fpn_channels(channels); });
+}
+
 int dd3d_load_weight(dd3d_handle h, const char* name, const float* data, const int64_t* shape, int ndim) {
     if (name == nullptr || data == nullptr || (ndim > 0 && shape == nullptr) || ndim < 0 || ndim > 8)
         return DD3D_ERR_INVALID;
@@ -616,11 +620,11 @@ int dd3d_op_conv2d_taps_tiles(const void* d_in, int B, int H, int W, int cin, in
     return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
 }
 
-int dd3d_op_b3d_sparse(const void* const* d_in, const int32_t* h_level_hw, const int32_t* h_pitch, const void* const* d_w,
-                       const float* const* d_scale, const float* const* d_bias, const void* d_fin, const int32_t* d_counts,
-                       int B, int C, int topk, int n_pad, float* d_rows, int out_pitch, dd3d_stream stream) {
+int dd3d_op_b3d_sparse_c(const void* const* d_in, const int32_t* h_level_hw, const int32_t* h_pitch, const void* const* d_w,
+                         const float* const* d_scale, const float* const* d_bias, const void* d_fin, const int32_t* d_counts,
+                         int B, int C, int topk, int n_pad, float* d_rows, int out_pitch, int cin, dd3d_stream stream) {
     if (!d_in || !h_level_hw || !h_pitch || !d_w || !d_scale || !d_bias || !d_fin || !d_counts || !d_rows) return DD3D_ERR_INVALID;
-    if (B < 1 || C < 1 || topk < 1) return DD3D_ERR_INVALID;
+    if (B < 1 || C < 1 || topk < 1 || cin < 1) return DD3D_ERR_INVALID;
     B3dSparseParams p;
     memset(&p, 0, sizeof(p));
     for (int l = 0; l < kLevels; ++l) {
@@ -632,7 +636,7 @@ int dd3d_op_b3d_sparse(const void* const* d_in, const int32_t* h_level_hw, const
         v.H = h_level_hw[2 * l];
         v.W = h_level_hw[2 * l + 1];
         v.pitch = h_pitch[l];
-        if (!v.scale || !v.bias || v.H < 1 || v.W < 1 || v.pitch < 256) return DD3D_ERR_INVALID;
+        if (!v.scale || !v.bias || v.H < 1 || v.W < 1 || v.pitch < cin) return DD3D_ERR_INVALID;
     }
     p.fin = static_cast<const uint2*>(d_fin);
     p.cand_count = d_counts;
@@ -643,8 +647,16 @@ int dd3d_op_b3d_sparse(const void* const* d_in, const int32_t* h_level_hw, const
     p.n_pad = n_pad;
     p.out_pitch = out_pitch;
     p.fp16 = g_op_fp16;
+    p.cin = cin;
     const cudaError_t e = launch_b3d_sparse(p, static_cast<cudaStream_t>(stream));
     return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
+}
+
+int dd3d_op_b3d_sparse(const void* const* d_in, const int32_t* h_level_hw, const int32_t* h_pitch, const void* const* d_w,
+                       const float* const* d_scale, const float* const* d_bias, const void* d_fin, const int32_t* d_counts,
+                       int B, int C, int topk, int n_pad, float* d_rows, int out_pitch, dd3d_stream stream) {
+    return dd3d_op_b3d_sparse_c(d_in, h_level_hw, h_pitch, d_w, d_scale, d_bias, d_fin, d_counts, B, C, topk, n_pad, d_rows,
+                                out_pitch, 256, stream);
 }
 
 int dd3d_op_stem_conv(const void* d_in4, const void* d_w, const float* d_scale, const float* d_bias, void* d_out, int B,

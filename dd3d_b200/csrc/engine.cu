@@ -236,6 +236,12 @@ void Engine::set_backbone_norm(int norm) {
     backbone_norm = norm;
 }
 
+void Engine::set_fpn_channels(int C) {
+    if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_fpn_channels after finalize");
+    if (C < 64 || C > 512 || C % 64) fail(DD3D_ERR_INVALID, "FPN width must be a multiple of 64 in [64, 512]");
+    fpn_channels = C;
+}
+
 // GroupNorm(32, C) affine of `<prefix>.weight` / `<prefix>.bias`, uploaded as fp32 vectors (cached like the epilogues)
 const Epilogue& Engine::gn_affine(const std::string& prefix, int C) {
     const std::string key = "gn|" + prefix;
@@ -969,6 +975,7 @@ struct Builder {
         const int norm = E->layout.fpn_norm;
         const bool gn = norm == DD3D_NORM_GN, bn = norm == DD3D_NORM_BN_SHARED || norm == DD3D_NORM_BN_PER_LEVEL;
         const bool avg = E->layout.fpn_fuse_avg != 0;
+        const int width = E->fpn_channels;  // FE.FPN.OUT_CHANNELS: laterals, outputs, P6 / P7
         auto conv_norm = [&](const std::string& name, View in, View out, int ksize, const View* res) {
             conv1(name, bn ? name + ".norm" : "", norm == DD3D_NORM_NONE, in, out, ksize, 1, false, res, res != nullptr);
         };
@@ -978,31 +985,31 @@ struct Builder {
             const std::string st = std::to_string(first_stage + i);
             const std::string lname = p + ".fpn_lateral" + st, oname = p + ".fpn_output" + st;
             const View& c = feats[i];
-            View lat = alloc(c.H, c.W, 256);
+            View lat = alloc(c.H, c.W, width);
             if (i == n - 1 || gn || avg) {
                 conv_norm(lname, c, lat, 1, nullptr);
                 const bool add = i != n - 1;
-                if (gn || add) group_norm({lat}, gn ? &E->gn_affine(lname + ".norm") : nullptr, false, add ? &prev : nullptr, add && avg);
+                if (gn || add) group_norm({lat}, gn ? &E->gn_affine(lname + ".norm", width) : nullptr, false, add ? &prev : nullptr, add && avg);
             } else {
                 // lateral + nearest-2x(prev): the un-smoothed `prev` is what propagates downwards
                 conv_norm(lname, c, lat, 1, &prev);
             }
             prev = lat;
-            res[i] = alloc(c.H, c.W, 256);
+            res[i] = alloc(c.H, c.W, width);
             persist(res[i]);
             conv_norm(oname, lat, res[i], 3, nullptr);
-            if (gn) group_norm({res[i]}, &E->gn_affine(oname + ".norm"), false, nullptr, false);
+            if (gn) group_norm({res[i]}, &E->gn_affine(oname + ".norm", width), false, nullptr, false);
         }
         *outs = res;
         const View& p5 = res[n - 1];
-        View p6 = alloc(p5.H / 2, p5.W / 2, 256);
+        View p6 = alloc(p5.H / 2, p5.W / 2, width);
         persist(p6);
         conv1(p + ".top_block.p6", "", true, p5, p6, 3, 2, false);
         outs->push_back(p6);
         if (dla_spec(E->desc.arch) != nullptr) {  // LastLevelP6P7
-            View r6 = alloc(p6.H, p6.W, 256);
+            View r6 = alloc(p6.H, p6.W, width);
             relu(p6, r6);
-            View p7 = alloc(p6.H / 2, p6.W / 2, 256);
+            View p7 = alloc(p6.H / 2, p6.W / 2, width);
             persist(p7);
             conv1(p + ".top_block.p7", "", true, r6, p7, 3, 2, false);
             outs->push_back(p7);
@@ -1012,31 +1019,33 @@ struct Builder {
     // ---- heads ------------------------------------------------------------------------------------------------
     // `depth` x (3x3 conv -> norm -> ReLU) over every level in one launch per layer (fcos2d.py:55-91, fcos3d.py:81-112).
     // norm: per-level BN (ModuleListDial, folded per segment), shared BN (one folded epilogue), none (conv bias), or GN
-    // (identity epilogue, then one GN op over the levels).  Depth 0: the FPN outputs themselves.
+    // (identity epilogue, then one GN op over the levels).  Depth 0: the FPN outputs themselves.  Every layer is as wide as the
+    // FPN (FE.FPN.OUT_CHANNELS; the reference's heads take their width from the backbone's output shape).
     void tower(const std::string& tp, int depth, int norm, const std::vector<View>& feats, std::vector<View>* out) {
+        const int width = E->fpn_channels;
         std::vector<View> cur = feats;
         std::vector<View> buf[2];
         for (int k = 0; k < std::min(depth, 2); ++k)
-            for (auto& f : feats) buf[k].push_back(alloc(f.H, f.W, 256));
+            for (auto& f : feats) buf[k].push_back(alloc(f.H, f.W, width));
         for (int i = 0; i < depth; ++i) {
             const std::string wn = tp + "." + std::to_string(i);
-            const ConvLayer& L = E->conv_layer(wn, {wn}, 256, 3);
+            const ConvLayer& L = E->conv_layer(wn, {wn}, width, 3);
             std::vector<SegSpec> segs(feats.size());
             for (size_t l = 0; l < feats.size(); ++l) {
                 segs[l].in = cur[l];
                 segs[l].out = buf[i & 1][l];
                 if (norm == DD3D_NORM_BN_PER_LEVEL) {
                     const std::string bn = wn + ".norm." + std::to_string(l);  // ModuleListDial: level l -> norm l
-                    segs[l].epi = &E->bn_epilogue(wn + "|" + bn, bn, "", 256);
+                    segs[l].epi = &E->bn_epilogue(wn + "|" + bn, bn, "", width);
                 } else if (norm == DD3D_NORM_BN_SHARED) {
-                    segs[l].epi = &E->bn_epilogue(wn + "|" + wn + ".norm", wn + ".norm", "", 256);
+                    segs[l].epi = &E->bn_epilogue(wn + "|" + wn + ".norm", wn + ".norm", "", width);
                 } else {  // none: conv bias; GN: raw conv output, normalised by the GN op below
-                    segs[l].epi = &E->bn_epilogue(wn + "|", "", norm == DD3D_NORM_NONE ? wn + ".bias" : "", 256);
+                    segs[l].epi = &E->bn_epilogue(wn + "|", "", norm == DD3D_NORM_NONE ? wn + ".bias" : "", width);
                 }
             }
             const bool gn = norm == DD3D_NORM_GN;
             conv(L, 1, !gn, segs, false);
-            if (gn) group_norm(buf[i & 1], &E->gn_affine(wn + ".norm"), true, nullptr, false);
+            if (gn) group_norm(buf[i & 1], &E->gn_affine(wn + ".norm", width), true, nullptr, false);
             cur = buf[i & 1];
         }
         *out = cur;
@@ -1044,7 +1053,8 @@ struct Builder {
 
     // Tile lists of a sparse tower (TowerTilesParams): `depth` lists, list i at distance <= reach - i; the tiling conv() gives
     // the tower layers, and the staging, list and count areas in the persistent region.  false: the shapes exceed the list
-    // entry fields or the layers do not run the pair tile, the tower stays dense.
+    // entry fields or the layers do not run the pair tile, the tower stays dense.  The pair tile needs a width that 128 divides,
+    // so at FPN widths 64, 192, 320 and 448 the sparse box2d / box3d towers always fall back to the dense tower.
     bool tower_tile_lists(TowerTilesParams& tt, const std::vector<View>& feats, int depth, int reach) {
         memset(&tt, 0, sizeof(tt));
         const int L = static_cast<int>(feats.size());
@@ -1053,7 +1063,8 @@ struct Builder {
             hs[l] = feats[l].H;
             ws[l] = feats[l].W;
         }
-        const bool halo = conv_prefer_halo(9, 1, 256, L, hs, ws);
+        const int width = E->fpn_channels;
+        const bool halo = conv_prefer_halo(9, 1, width, L, hs, ws);
         for (int l = 0; l < L; ++l) {
             TowerTilesLevel& v = tt.lvl[l];
             v.H = hs[l];
@@ -1073,7 +1084,7 @@ struct Builder {
         }
         if (B > kTileListMaxImages || tt.max_tiles >= kTileListMaxTiles || tower_tiles_smem_bytes(tt.max_tiles) > 48 * 1024)
             return false;
-        // the work-list mode is built for the pair tile, which every filled 256-channel halo layer selects (conv() below)
+        // the work-list mode is built for the pair tile, which every filled halo layer of a 128-multiple width selects (conv())
         ConvParams cp;
         memset(&cp, 0, sizeof(cp));
         cp.nseg = L;
@@ -1085,7 +1096,7 @@ struct Builder {
             cp.seg[l].th = tt.lvl[l].th;
             cp.seg[l].tw = tt.lvl[l].tw;
         }
-        if (!conv_select_pair(&cp, 256, E->num_sms)) return false;
+        if (!conv_select_pair(&cp, width, E->num_sms)) return false;
         tt.B = B;
         tt.depth = depth;
         tt.reach = reach;
@@ -1119,6 +1130,7 @@ struct Builder {
     void build_heads(const std::vector<View>& feats) {
         const int C = E->desc.num_classes;
         const int L = static_cast<int>(feats.size());
+        const int width = E->fpn_channels;  // input channels of every predictor
         const bool nusc = E->desc.nuscenes_heads != 0;
         // head switches no shipped experiment changes (dd3d_model_desc): class-agnostic 3-D channels, per-level predictors,
         // no Scale / Offset layers, no 3-D head at all
@@ -1161,7 +1173,7 @@ struct Builder {
                 names.push_back("speed");
             }
             const ConvLayer& Lc = E->conv_layer(nusc ? "fcos2d_head.cls_logits+attr+speed" : "fcos2d_head.cls_logits",
-                                                names, 256, 3);
+                                                names, width, 3);
             const std::string ekey = "fcos2d_head.cls_logits|";
             if (E->epis.find(ekey) == E->epis.end()) {
                 std::vector<float> sc, bi, lo;
@@ -1215,7 +1227,7 @@ struct Builder {
         tower("fcos2d_head.box2d_tower", d2, E->layout.fcos2d_norm, feats, &box_t);
         {
             const ConvLayer& Lb = E->conv_layer("fcos2d_head.box2d_reg+centerness",
-                                                {"fcos2d_head.box2d_reg", "fcos2d_head.centerness"}, 256, 3);
+                                                {"fcos2d_head.box2d_reg", "fcos2d_head.centerness"}, width, 3);
             std::vector<SegSpec> segs(L);
             for (int l = 0; l < L; ++l) {
                 const std::string key = "fcos2d_head.box@" + std::to_string(l);
@@ -1266,7 +1278,7 @@ struct Builder {
                 return E->conv_layer("fcos3d_head.box3d_all." + i,
                                      {"fcos3d_head.box3d_quat." + i, "fcos3d_head.box3d_ctr." + i, "fcos3d_head.box3d_depth." + i,
                                       "fcos3d_head.box3d_size." + i, "fcos3d_head.box3d_conf." + i},
-                                     256, 3);
+                                     width, 3);
             };
             std::vector<SegSpec> segs(L);
             for (int l = 0; l < L; ++l) {
@@ -1314,7 +1326,7 @@ struct Builder {
                     sp.lvl[l].w = Lw.d_w;
                     sp.lvl[l].scale = segs[l].epi->d_scale;
                     sp.lvl[l].bias = segs[l].epi->d_bias;
-                    if (Lw.cout_pad != b3d_pitch || Lw.cin != 256) fail(DD3D_ERR_INVALID, "box3d predictor shape");
+                    if (Lw.cout_pad != b3d_pitch || Lw.cin != width) fail(DD3D_ERR_INVALID, "box3d predictor shape");
                 }
                 ++op_idx;
                 sp.rows = P->b3d_rows;
@@ -1324,6 +1336,7 @@ struct Builder {
                 sp.n_pad = b3d_pitch;
                 sp.out_pitch = b3d_pitch;
                 sp.fp16 = E->fp16;
+                sp.cin = width;
             } else if (!per_level) {
                 conv(layer_for(0), 1, false, segs, true);
             } else {

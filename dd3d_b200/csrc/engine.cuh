@@ -235,6 +235,7 @@ class Engine {
     const Epilogue& gn_affine(const std::string& prefix, int C = kGnChannels);  // GroupNorm weight / bias as d_scale / d_bias
     void set_layout(const dd3d_layout_desc& l);
     void set_backbone_norm(int norm);
+    void set_fpn_channels(int C);
 
     dd3d_model_desc desc;
     // FPN / head layout (dd3d_set_layout); the default is the shipped one
@@ -242,6 +243,9 @@ class Engine {
     // FE.BACKBONE.NORM (dd3d_set_backbone_norm): BN folded into the conv epilogues (default), DD3D_NORM_NONE (DLA-34: conv bias)
     // or DD3D_NORM_GN (VoVNet: raw conv outputs, each normalised by a GroupNorm op)
     int backbone_norm = DD3D_NORM_BN_SHARED;
+    // FE.FPN.OUT_CHANNELS (dd3d_set_fpn_channels): width of the FPN outputs, the head towers and the predictors' input; a
+    // multiple of 64 in [64, 512]
+    int fpn_channels = 256;
     int device = 0;
     int num_sms = 132;
     int fp16 = 0;  // desc.act_dtype == DD3D_ACT_FP16: 16-bit storage of activations / weights is fp16 instead of bf16

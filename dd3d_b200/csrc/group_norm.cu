@@ -1,10 +1,13 @@
-// GroupNorm(32, C) on NHWC 16-bit views with a channel pitch, C = 32 * cpg for cpg in {2, 4, 5, 6, 7, 8, 16, 24, 32}:
-// the FCOS heads / FPN with NORM "GN" (fcos2d.py:73-91, fcos3d.py:82-100 get_norm("GN") = nn.GroupNorm(32, 256); detectron2
-// FPN with norm "GN") and the VoVNet backbone with FE.BACKBONE.NORM "GN" (vovnet.py:119,139,159: 64 .. 1024 channels).
+// GroupNorm(32, C) on NHWC 16-bit views with a channel pitch, C = 32 * cpg for cpg in {2, 4, 5, 6, 7, 8, 10, 12, 14, 16, 24,
+// 32}: the FCOS heads / FPN with NORM "GN" (fcos2d.py:73-91, fcos3d.py:82-100 get_norm("GN") = nn.GroupNorm(32, C) at every
+// FE.FPN.OUT_CHANNELS from 64 to 512; detectron2 FPN with norm "GN") and the VoVNet backbone with FE.BACKBONE.NORM "GN"
+// (vovnet.py:119,139,159: 64 .. 1024 channels).
 // Thread t of a CTA owns the 16-byte vector v = t % (C / 8) of every pixel it visits (channels [8v, 8v + 8)) and visits the
-// pixels r, r + R, ... of its chunk, r = t / (C / 8), R = 256 / (C / 8).  For 256 channels (cpg 8) that is lane = group,
-// warp = pixel row: one warp reads one 512-byte pixel.  With cpg 5, 6 or 7 a vector holds the ends of two or three groups;
-// each thread then keeps one (count, mean, M2) per group it touches (a slot), fixed by v.
+// pixels r, r + R, ... of its chunk, r = t / (C / 8), R = floor(256 / (C / 8)).  For 256 channels (cpg 8) that is lane = group,
+// warp = pixel row: one warp reads one 512-byte pixel.  Where C / 8 does not divide 256 (cpg 5, 6, 7, 10, 12, 14: 20 .. 56
+// vectors per pixel) the last 256 - R * C / 8 threads (4 .. 32) own no (vector, row) and only take part in the barriers; the
+// mapping is still a function of C alone.  With cpg 5, 6, 7, 10, 12 or 14 a vector holds the ends of two (cpg 5: up to
+// three) groups; each thread then keeps one (count, mean, M2) per group it touches (a slot), fixed by v.
 //
 // Two kernels, one launch each for up to kMaxSeg maps of the same channel count (the five FPN levels of a tower layer):
 //   group_norm_stats_kernel  one CTA per (segment, image, chunk of kGnChunk pixels): per-thread running (count, mean, M2) per
@@ -107,13 +110,12 @@ __global__ void __launch_bounds__(kGnThreads) group_norm_stats_kernel(const Grou
             int sl[8];
             float cnt[K], inv[K];
 #pragma unroll
-            for (int j = 0; j < K; ++j) cnt[j] = 0.f;
+            for (int k = 0; k < 8; ++k) sl[k] = (8 * v + k) / CPG - g0;
+            // channels of group g0 + j inside [8v, 8v + 8), in closed form (a per-channel count left a local-memory array in
+            // the cpg 14 instantiation)
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                sl[k] = (8 * v + k) / CPG - g0;
-#pragma unroll
-                for (int j = 0; j < K; ++j) cnt[j] += sl[k] == j ? 1.f : 0.f;
-            }
+            for (int j = 0; j < K; ++j)
+                cnt[j] = static_cast<float>(max(0, min(8 * v + 8, (g0 + j + 1) * CPG) - max(8 * v, (g0 + j) * CPG)));
 #pragma unroll
             for (int j = 0; j < K; ++j) inv[j] = cnt[j] > 0.f ? 1.f / cnt[j] : 0.f;
 #pragma unroll 1
@@ -255,7 +257,8 @@ bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 
 
 bool group_norm_channels_ok(int C) {
     switch (C) {
-        case 64: case 128: case 160: case 192: case 224: case 256: case 512: case 768: case 1024: return true;
+        case 64: case 128: case 160: case 192: case 224: case 256: case 320: case 384: case 448: case 512: case 768: case 1024:
+            return true;
         default: return false;
     }
 }
@@ -301,6 +304,9 @@ cudaError_t launch_group_norm(GroupNormParams p, cudaStream_t stream) {
         case 6: return launch_cpg<6>(p, n, stream);
         case 7: return launch_cpg<7>(p, n, stream);
         case 8: return launch_cpg<8>(p, n, stream);
+        case 10: return launch_cpg<10>(p, n, stream);
+        case 12: return launch_cpg<12>(p, n, stream);
+        case 14: return launch_cpg<14>(p, n, stream);
         case 16: return launch_cpg<16>(p, n, stream);
         case 24: return launch_cpg<24>(p, n, stream);
         default: return launch_cpg<32>(p, n, stream);

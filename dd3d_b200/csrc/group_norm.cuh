@@ -9,7 +9,7 @@
 
 namespace dd3d {
 
-constexpr int kGnChannels = 256;  // heads and FPN: 32 groups of 8 channels
+constexpr int kGnChannels = 256;  // heads and FPN at the default FE.FPN.OUT_CHANNELS: 32 groups of 8 channels
 constexpr int kGnChunk = 1024;    // pixels per statistics chunk (a function of the shape only: deterministic)
 
 struct GroupNormSeg {
@@ -30,7 +30,8 @@ struct GroupNormParams {
     int C = kGnChannels;  // channels per pixel of every segment: group_norm_channels_ok(C)
 };
 
-// C = 32 * cpg with cpg in {2, 4, 5, 6, 7, 8, 16, 24, 32}: the channel counts of the GN heads, FPN and VoVNet backbones
+// C = 32 * cpg with cpg in {2, 4, 5, 6, 7, 8, 10, 12, 14, 16, 24, 32}: the channel counts of the GN heads and FPN (every
+// multiple of 64 up to 512) and of the VoVNet backbones
 bool group_norm_channels_ok(int C);
 int group_norm_chunks(int H, int W);
 size_t group_norm_scratch_bytes(int B, int H, int W);

@@ -87,6 +87,7 @@ SIGNATURES = {
     "dd3d_size_divisibility": (_I, [_P]),
     "dd3d_set_layout": (_I, [_P, C.POINTER(LayoutDesc)]),
     "dd3d_set_backbone_norm": (_I, [_P, C.c_int32]),
+    "dd3d_set_fpn_channels": (_I, [_P, C.c_int32]),
     "dd3d_load_weight": (_I, [_P, C.c_char_p, _P, C.POINTER(_I64), _I]),
     "dd3d_finalize": (_I, [_P]),
     "dd3d_workspace_bytes": (_I64, [_P, _I, _I, _I]),
@@ -124,6 +125,8 @@ SIGNATURES = {
     "dd3d_op_conv2d_taps_tiles": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _I, _P, _I, _I, _P, _P, _P]),
     "dd3d_op_b3d_sparse": (_I, [C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P),
                                 C.POINTER(_P), _P, _P, _I, _I, _I, _I, _P, _I, _P]),
+    "dd3d_op_b3d_sparse_c": (_I, [C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P),
+                                  C.POINTER(_P), _P, _P, _I, _I, _I, _I, _P, _I, _I, _P]),
     "dd3d_op_dla_front": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_s2_mma": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_conv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),

@@ -14,7 +14,7 @@ import torch
 from torch import nn
 
 from . import lib as _lib
-from .arch import arch_of, is_nuscenes_arch, param_specs, size_divisibility
+from .arch import arch_of, check_fpn_channels, is_nuscenes_arch, param_specs, size_divisibility
 from .structures import Boxes, Boxes3D, GenericBoxes3D, Instances
 
 try:  # register next to the reference's DD3D when detectron2 is present (scripts/train.py:48 build_model)
@@ -37,7 +37,8 @@ class DD3DB200(nn.Module):
         self.do_bev_nms = cfg.DD3D.INFERENCE.DO_BEV_NMS
         self.bev_nms_iou_thresh = cfg.DD3D.INFERENCE.BEV_NMS_IOU_THRESH
         self.backbone = SimpleNamespace(size_divisibility=size_divisibility(cfg))
-        self._specs = param_specs(cfg)
+        self._specs = param_specs(cfg)  # the reference's own errors first (nn.GroupNorm's ValueError for GN widths)
+        self._fpn_channels = check_fpn_channels(cfg)  # FE.FPN.OUT_CHANNELS: a multiple of 64 in [64, 512]
         self._state = None  # reference-keyed fp32 CPU tensors
         self._device = torch.device("cpu")
         self._desc = _lib.desc_from_cfg(cfg)
@@ -127,6 +128,7 @@ class DD3DB200(nn.Module):
             _lib.check(L.dd3d_create(C.byref(self._desc), C.byref(handle)))
             _lib.check(L.dd3d_set_layout(handle, C.byref(self._layout)), handle)
             _lib.check(L.dd3d_set_backbone_norm(handle, self._backbone_norm), handle)
+            _lib.check(L.dd3d_set_fpn_channels(handle, self._fpn_channels), handle)
             for name, t in self._state.items():
                 if not t.is_floating_point():
                     continue

@@ -101,8 +101,8 @@ typedef struct dd3d_model_desc {
 
 /* Normalisation after a head-tower or FPN conv (get_norm in fcos2d.py:73-91, fcos3d.py:82-100, detectron2 FPN):
  * "BN" / "FrozenBN" in a head tower give one BN per FPN level (ModuleListDial, keys <conv>.norm.<level>); "SyncBN" gives one
- * BN shared by the levels (<conv>.norm); "GN" GroupNorm(32, 256) (<conv>.norm.weight / .bias); "" no norm, the conv has a
- * bias.  The FPN has no per-level case: its BN / FrozenBN / SyncBN is DD3D_NORM_BN_SHARED (DD3D_NORM_BN_PER_LEVEL is
+ * BN shared by the levels (<conv>.norm); "GN" GroupNorm(32, C) at the FPN width C (<conv>.norm.weight / .bias); "" no norm,
+ * the conv has a bias.  The FPN has no per-level case: its BN / FrozenBN / SyncBN is DD3D_NORM_BN_SHARED (DD3D_NORM_BN_PER_LEVEL is
  * accepted as the same). */
 enum dd3d_norm { DD3D_NORM_BN_PER_LEVEL = 0, DD3D_NORM_BN_SHARED = 1, DD3D_NORM_GN = 2, DD3D_NORM_NONE = 3 };
 
@@ -162,6 +162,12 @@ int dd3d_set_layout(dd3d_handle h, const dd3d_layout_desc* h_layout);
  * DD3D_NORM_GN and, for a VoVNet, DD3D_NORM_NONE return DD3D_ERR_INVALID and leave the backbone unchanged.  An engine that
  * never receives the call builds the BN backbone. */
 int dd3d_set_backbone_norm(dd3d_handle h, int32_t dd3d_norm);
+/* Sets the FPN width (FE.FPN.OUT_CHANNELS) before dd3d_finalize (DD3D_ERR_STATE afterwards): the channels of the FPN laterals,
+ * outputs and P6 / P7, of every head-tower conv and of the predictors' input (the reference's heads take their width from the
+ * backbone's output shape).  Every multiple of 64 from 64 to 512; anything else returns DD3D_ERR_INVALID and leaves the width
+ * unchanged.  An engine that never receives the call builds 256.  The sparse box2d / box3d towers need the pair tile, which
+ * only widths that 128 divides run: at 64, 192, 320 and 448 those towers are dense (the sparse box3d predictor still runs). */
+int dd3d_set_fpn_channels(dd3d_handle h, int32_t channels);
 
 /* ---- weights: one call per tensor of the reference state_dict (Checkpointer.load, scripts/train.py:52) ----- */
 /* h_data: host fp32, contiguous, `ndim` dims in h_shape.  Unknown names are ignored (return DD3D_OK, e.g.
@@ -375,6 +381,13 @@ int dd3d_op_b3d_sparse(const void* const* d_in /*[5]*/, const int32_t* h_level_h
                        const void* const* d_w /*[5]*/, const float* const* d_scale /*[5]*/, const float* const* d_bias /*[5]*/,
                        const void* d_fin, const int32_t* d_counts, int B, int C, int topk, int n_pad, float* d_rows,
                        int out_pitch, dd3d_stream stream);
+/* dd3d_op_b3d_sparse_c: dd3d_op_b3d_sparse with `cin` tower channels instead of 256 (FE.FPN.OUT_CHANNELS): d_in[l] has cin
+ * channels (h_pitch[l] >= cin), d_w[l] is 16-bit [n_pad][9][cin].  cin a multiple of 64 from 64 to 512.  With cin = 256 it is
+ * dd3d_op_b3d_sparse. */
+int dd3d_op_b3d_sparse_c(const void* const* d_in /*[5]*/, const int32_t* h_level_hw, const int32_t* h_pitch /*[5]*/,
+                         const void* const* d_w /*[5]*/, const float* const* d_scale /*[5]*/, const float* const* d_bias /*[5]*/,
+                         const void* d_fin, const int32_t* d_counts, int B, int C, int topk, int n_pad, float* d_rows,
+                         int out_pitch, int cin, dd3d_stream stream);
 int dd3d_op_stem_conv(const void* d_in4, const void* d_w, const float* d_scale, const float* d_bias, void* d_out,
                       int B, int H, int W, int ksize, int stride, int cout, int out_pitch, dd3d_stream stream);
 /* dd3d_op_dla_front: the fused DLA-34 front end (csrc/dla_front.cu; reference dla.py:271-283,346-350 base_layer -> level0
@@ -407,9 +420,9 @@ int64_t dd3d_op_group_norm_scratch_bytes(int B, int H, int W);
 int dd3d_op_group_norm(const void* d_in, int B, int H, int W, int in_pitch, const float* d_gamma, const float* d_beta, int relu,
                        const void* d_residual, int res_pitch, int avg, void* d_out, int out_pitch, void* d_scratch,
                        dd3d_stream stream);
-/* dd3d_op_group_norm_c: GroupNorm(32, C) for C = 32 * cpg, cpg in {2, 4, 5, 6, 7, 8, 16, 24, 32} (64 .. 1024 channels), same
- * kernels and arithmetic as dd3d_op_group_norm (for C = 256 bit-identical to it), then ReLU when relu; one rounding at the store.
- * Reads channels [in_c0, in_c0 + C) of d_in = [B][H][W][in_pitch] and writes channels [out_c0, out_c0 + C) of
+/* dd3d_op_group_norm_c: GroupNorm(32, C) for C = 32 * cpg, cpg in {2, 4, 5, 6, 7, 8, 10, 12, 14, 16, 24, 32} (64 .. 1024
+ * channels), same kernels and arithmetic as dd3d_op_group_norm (for C = 256 bit-identical to it), then ReLU when relu; one
+ * rounding at the store.  Reads channels [in_c0, in_c0 + C) of d_in = [B][H][W][in_pitch] and writes channels [out_c0, out_c0 + C) of
  * d_out = [B][H][W][out_pitch]: channel slices of concat buffers; in place when d_out == d_in and out_c0 == in_c0.  d_gamma,
  * d_beta: fp32 [C].  d_scratch: dd3d_op_group_norm_scratch_bytes(B, H, W) bytes, any content.  Offsets and pitches multiples
  * of 8, d_in / d_out 16-byte aligned. */
