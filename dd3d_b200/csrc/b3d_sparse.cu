@@ -19,6 +19,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "b3d_mma.cuh"
 #include "b3d_sparse.cuh"
 #include "pdl.cuh"
 
@@ -27,43 +28,21 @@ namespace dd3d {
 namespace {
 
 constexpr int kRowsPerCta = 128, kThreads = 256;
-constexpr int kChunk = 64;  // channels per shared-memory weight block
+using b3d_mma::kChunk;  // channels per shared-memory weight block
+using b3d_mma::smem_u32;
+using b3d_mma::weight_slot;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-template <bool FP16>
-__device__ __forceinline__ void mma16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                         uint32_t b1) {
-    if (FP16) {
-        asm volatile(
-            "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-            : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-    } else {
-        asm volatile(
-            "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-            : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-    }
-}
-
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-    uint4 v;
-    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-    return v;
-}
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
 
-// weight block `chunk` = (tap, kc) of predictor `w` ([n_pad][9][cin]) -> smem [n_pad rows][128 B], 16-byte chunk q of row n stored at q ^ ((n & 1) << 2)
-// (the two rows a quarter-warp reads with one LDS.128 then sit in different halves of the 128-byte line: conflict-free)
+// weight block `chunk` = (tap, kc) of predictor `w` ([n_pad][9][cin]) -> smem [n_pad rows][128 B] (b3d_mma::weight_slot)
 __device__ __forceinline__ void stage_weights(const __nv_bfloat16* w, int n_pad, int kcs, int chunk, uint32_t dst) {
     const int cin = kcs * kChunk, tap = chunk / kcs, kc = chunk - tap * kcs;
     const __nv_bfloat16* src = w + tap * cin + kc * kChunk;
     for (int i = threadIdx.x; i < n_pad * 8; i += kThreads) {
         const int n = i >> 3, q = i & 7;
-        cp_async16(dst + n * 128 + ((q ^ ((n & 1) << 2)) << 4), src + static_cast<size_t>(n) * (9 * cin) + q * 8);
+        cp_async16(dst + weight_slot(n, q), src + static_cast<size_t>(n) * (9 * cin) + q * 8);
     }
 }
 
@@ -100,16 +79,7 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel(const B3dSparsePar
         base[h] = L.in + (static_cast<size_t>(b * L.H + py[h]) * L.W + px[h]) * L.pitch + 8 * t;
     }
     auto load_a = [&](int chunk, uint4 (&a)[2][2]) {  // [group of 32 channels][row half]
-        const int tap = chunk / kcs, kc = chunk - tap * kcs;
-        const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const bool ok = valid[h] && (py[h] + dy) >= 0 && (py[h] + dy) < L.H && (px[h] + dx) >= 0 && (px[h] + dx) < L.W;
-            const __nv_bfloat16* src = base[h] + (static_cast<ptrdiff_t>(dy) * L.W + dx) * L.pitch + kc * kChunk;
-#pragma unroll
-            for (int G = 0; G < 2; ++G)
-                a[G][h] = ok ? __ldg(reinterpret_cast<const uint4*>(src + G * 32)) : make_uint4(0u, 0u, 0u, 0u);
-        }
+        b3d_mma::load_a(base, py, px, valid, L.H, L.W, L.pitch, kcs, chunk, a);
     };
 
     float acc[NT][4];
@@ -133,19 +103,9 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel(const B3dSparsePar
         const uint32_t wb = s_w + (c & 1) * buf_bytes;
 #pragma unroll
         for (int G = 0; G < 2; ++G) {
-            // lane t holds channels 8t .. 8t+7 of the 32-channel group for rows g / g+8 (a_cur) and, per n-tile, of weight row
-            // nt*8 + g: two K = 16 steps whose k slots {2t, 2t+1 | 2t+8, 2t+9} are register pairs (x, y) and (z, w) of those
-            // 16-byte loads -- the same channel permutation on both operands, so the products pair up correctly
-            const uint4 lo = a_cur[G][0], hi = a_cur[G][1];
 #pragma unroll
-            for (int nt = 0; nt < NT; ++nt) {
-                if (nt < nt_real) {
-                    const int n = nt * 8 + g;
-                    const uint4 w = lds128(wb + n * 128 + ((((G << 2) | t) ^ ((n & 1) << 2)) << 4));
-                    mma16816<FP16>(acc[nt], lo.x, hi.x, lo.y, hi.y, w.x, w.y);
-                    mma16816<FP16>(acc[nt], lo.z, hi.z, lo.w, hi.w, w.z, w.w);
-                }
-            }
+            for (int nt = 0; nt < NT; ++nt)
+                if (nt < nt_real) b3d_mma::mma_group<FP16>(acc[nt], a_cur[G][0], a_cur[G][1], wb, nt * 8 + g, G, t);
         }
         __syncthreads();  // every warp is done with buffer c & 1 before block c + 2 is staged into it
 #pragma unroll

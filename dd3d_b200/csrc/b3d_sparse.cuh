@@ -31,6 +31,27 @@ constexpr int kB3dSparseMaxN = 112;
 constexpr int kB3dSparseMaxCin = 512;  // widest FPN the engine builds
 cudaError_t launch_b3d_sparse(const B3dSparseParams& p, cudaStream_t stream);
 
+// Class-gathered sparse FCOS3D predictor (b3d_gather.cu), for class-specific heads wider than kB3dSparseMaxN: the decode reads
+// only the 11 channels {q * C + c} of a candidate's own class c (fcos3d.py:333-352), so each candidate gets exactly those,
+// computed with the same per-channel arithmetic as b3d_sparse_kernel.  lvl[].w is the whole fused predictor [>= 11 C][9][cin],
+// lvl[].scale / bias its [11 C] epilogue.  Output rows [B][L][topk][kB3dGatherPitch] fp32: channel q of the candidate's class
+// at column q (the layout of a class-agnostic map pixel); columns 11..15 are not written.
+constexpr int kB3dGatherPitch = 16;
+constexpr int kB3dGatherMaxC = 128;  // DD3D_MAX_NUM_CLASSES
+struct B3dGatherParams {
+    B3dSparseLevel lvl[kLevels];
+    const uint2* fin;           // [B][L][topk] (score bits, pixel * C + class): DecodeParams::fin
+    const int32_t* cand_count;  // [B][L]
+    float* rows;                // [B][L][topk][kB3dGatherPitch]
+    int32_t* order;             // scratch [B][L][topk]: the slots of each (image, level), grouped by class
+    int2* seg;                  // scratch [B][L][C]: (first entry in `order`, count) of each class
+    int B, C, topk, fp16, cin;
+};
+size_t b3d_gather_scratch_bytes(int B, int C, int topk);
+void b3d_gather_bind_scratch(B3dGatherParams* p, void* scratch);
+constexpr int kB3dGatherLaunches = 2;  // class grouping + predictor
+cudaError_t launch_b3d_gather(const B3dGatherParams& p, cudaStream_t stream);
+
 // Sparse box3d tower (tower_tiles.cu): the sparse predictor reads the tower output only in the 3x3 neighbourhoods of the
 // final candidates, so tower layer i of `depth` (0-based) is needed only at the candidates dilated by depth - i pixels
 // (Chebyshev), clipped to the map.  tower_tiles_kernel lists, per layer, the conv tiles that meet that set; the tower convs

@@ -38,7 +38,9 @@ namespace {
 constexpr int kGbMaxB = 256;          // images per launch (image mode: per chunk of the batch)
 constexpr int kGbMaxCap = kLevels * kMaxPreNmsTopk;  // detection slots per image (image mode with DO_NMS off)
 constexpr int kGbGroupImages = 16;    // images per group (the caller's max_group_images is at most this)
-constexpr int kGbMaxCls = 64;         // class ids 0..63
+constexpr int kGbMaxCls = 128;        // class ids 0..127 (DD3D_MAX_NUM_CLASSES)
+// class segments per group: 64 for models of up to 64 classes (the table and the scan grid they always had), else 128
+inline int gb_class_bound(int num_classes) { return num_classes <= 64 ? 64 : kGbMaxCls; }
 constexpr int kGbSortMax = kGbGroupImages * kTtaMergedMax;  // boxes per group: max_group_images * cap <= this
 constexpr int kGbMaxWords = kGbSortMax / 64;
 constexpr int kGbSortThreads = 1024;
@@ -62,6 +64,7 @@ struct GbParams {
     int32_t* flags;
     int flag_bit;          // kGbFlag or kGbImageFlag
     int B, cap, num_views, pose_mode, num_groups, max_group_images, max_dets;
+    int num_cls;           // class segments per group (gb_class_bound): class ids 0..num_cls-1
     float thr;
     // scratch
     int32_t* img_n;              // [B] boxes of image b that enter the NMS
@@ -74,7 +77,7 @@ struct GbParams {
     float* srect;                // [N][5] by sorted position
     int32_t* ssrc;               // [N] by sorted position
     int4* row;                   // [N] by sorted position: segment start, segment size, first mask word, row in segment
-    int4* seg;                   // [num_groups][kGbMaxCls] start, size, first mask word of each class segment
+    int4* seg;                   // [num_groups][num_cls] start, size, first mask word of each class segment
     unsigned long long* mask;    // rows of the class segments, ceil(size / 64) words each
     float* keep_score;           // [B][cap] scores_3d of the NMS survivors, -1 elsewhere
     unsigned long long* sel;     // [2] key of the max_dets-th survivor, capped
@@ -86,7 +89,7 @@ struct GbScratch {
 
 size_t align256(size_t x) { return (x + 255) / 256 * 256; }
 
-GbScratch gb_layout(int B, int cap, int max_group_images) {
+GbScratch gb_layout(int B, int cap, int max_group_images, int num_cls) {
     const size_t N = static_cast<size_t>(B) * cap;
     // a group of n boxes needs at most n * ceil(n / 64) mask words (sum over its class segments), n <= max_group_images * cap
     const size_t words = N * ((static_cast<size_t>(max_group_images) * cap + 63) / 64);
@@ -107,7 +110,7 @@ GbScratch gb_layout(int B, int cap, int max_group_images) {
     s.srect = take(N * 5 * 4);
     s.ssrc = take(N * 4);
     s.row = take(N * 16);
-    s.seg = take(static_cast<size_t>(B) * kGbMaxCls * 16);
+    s.seg = take(static_cast<size_t>(B) * num_cls * 16);
     s.mask = take(words * 8);
     s.keep_score = take(N * 4);
     s.sel = take(16);
@@ -196,9 +199,9 @@ __global__ void __launch_bounds__(kGbPrepThreads) gbev_prep_kernel(const GbParam
         go[7] = D.size[0]; go[8] = D.size[1]; go[9] = D.size[2];
     }
     int cls = D.cls;
-    if (cls < 0 || cls >= kGbMaxCls) {
+    if (cls < 0 || cls >= p.num_cls) {
         atomicOr(p.flags, p.flag_bit);
-        cls = min(max(cls, 0), kGbMaxCls - 1);
+        cls = min(max(cls, 0), p.num_cls - 1);
     }
     const int local = concat - p.grp[group_of(p, b) * 3];
     // class major; descending scores_3d (non-negative floats order like their bit patterns); concatenation index
@@ -216,7 +219,7 @@ __global__ void __launch_bounds__(kGbSortThreads) gbev_sort_kernel(const GbParam
     const int base = p.grp[g * 3 + 0], n = p.grp[g * 3 + 1], mbase = p.grp[g * 3 + 2];
     int n2 = 1;
     while (n2 < n) n2 <<= 1;
-    for (int c = threadIdx.x; c < kGbMaxCls; c += blockDim.x) s_cnt[c] = 0;
+    for (int c = threadIdx.x; c < p.num_cls; c += blockDim.x) s_cnt[c] = 0;
     for (int i = threadIdx.x; i < n2; i += blockDim.x) keys[i] = i < n ? p.key[base + i] : ~0ull;
     __syncthreads();
     for (int i = threadIdx.x; i < n; i += blockDim.x) atomicAdd(&s_cnt[static_cast<int>(keys[i] >> 48)], 1);
@@ -237,11 +240,11 @@ __global__ void __launch_bounds__(kGbSortThreads) gbev_sort_kernel(const GbParam
     __syncthreads();
     if (threadIdx.x == 0) {
         int start = 0, moff = mbase;
-        for (int c = 0; c < kGbMaxCls; ++c) {
+        for (int c = 0; c < p.num_cls; ++c) {
             const int m = s_cnt[c];
             s_start[c] = start;
             s_moff[c] = moff;
-            p.seg[g * kGbMaxCls + c] = make_int4(base + start, m, moff, 0);
+            p.seg[g * p.num_cls + c] = make_int4(base + start, m, moff, 0);
             start += m;
             moff += m * ((m + 63) / 64);
         }
@@ -303,7 +306,7 @@ __global__ void __launch_bounds__(kGbThreads) gbev_scan_kernel(const GbParams p)
     __shared__ unsigned long long removed[kGbMaxWords];
     __shared__ unsigned long long diag[64];
     __shared__ unsigned long long s_kept;
-    const int4 sg = p.seg[blockIdx.x * kGbMaxCls + blockIdx.y];
+    const int4 sg = p.seg[blockIdx.x * p.num_cls + blockIdx.y];
     const int start = sg.x, n = sg.y;
     if (n == 0) return;
     const int W = (n + 63) / 64;
@@ -465,7 +468,7 @@ __global__ void __launch_bounds__(kGbCompactThreads) gbev_compact_kernel(const G
 
 // Fills the scratch pointers of p (for p.B images, groups of at most max_group_images) and enqueues the seven kernels.
 cudaError_t gb_launch(GbParams p, void* scratch, cudaStream_t stream) {
-    const GbScratch L = gb_layout(p.B, p.cap, p.max_group_images);
+    const GbScratch L = gb_layout(p.B, p.cap, p.max_group_images, p.num_cls);
     uint8_t* s = static_cast<uint8_t*>(scratch);
     p.img_n = reinterpret_cast<int32_t*>(s + L.img_n);
     p.img_pos = reinterpret_cast<int32_t*>(s + L.img_pos);
@@ -497,7 +500,7 @@ cudaError_t gb_launch(GbParams p, void* scratch, cudaStream_t stream) {
                        stream, p);
     if (e == cudaSuccess) e = launch_pdl(gbev_sort_kernel, dim3(p.num_groups), dim3(kGbSortThreads), sort_smem, stream, p);
     if (e == cudaSuccess) e = launch_pdl(gbev_mask_kernel, dim3(sms * 8), dim3(kGbThreads), 0, stream, p);
-    if (e == cudaSuccess) e = launch_pdl(gbev_scan_kernel, dim3(p.num_groups, kGbMaxCls), dim3(kGbThreads), 0, stream, p);
+    if (e == cudaSuccess) e = launch_pdl(gbev_scan_kernel, dim3(p.num_groups, p.num_cls), dim3(kGbThreads), 0, stream, p);
     if (e == cudaSuccess) e = launch_pdl(gbev_select_kernel, dim3(1), dim3(kGbSortThreads), 0, stream, p);
     if (e == cudaSuccess)
         e = launch_pdl(gbev_compact_kernel, dim3(B), dim3(std::min(kGbCompactThreads, (cap + 31) / 32 * 32)), 0, stream, p);
@@ -508,7 +511,7 @@ cudaError_t gb_launch(GbParams p, void* scratch, cudaStream_t stream) {
 
 size_t group_bev_nms_scratch_bytes(int B, int cap, int max_group_images) {
     if (B < 1 || cap < 1 || max_group_images < 1) return 0;
-    return gb_layout(B, cap, max_group_images).bytes;
+    return gb_layout(B, cap, max_group_images, kGbMaxCls).bytes;
 }
 
 cudaError_t launch_group_bev_nms(Det* dets, int32_t* counts, const float* view_K, int num_views, const float* poses,
@@ -536,18 +539,21 @@ cudaError_t launch_group_bev_nms(Det* dets, int32_t* counts, const float* view_K
     p.num_groups = num_groups;
     p.max_group_images = max_group_images;
     p.max_dets = max_dets;
+    p.num_cls = kGbMaxCls;  // the operator takes any class id of DD3D_MAX_NUM_CLASSES
     p.thr = thr;
     return gb_launch(p, scratch, stream);
 }
 
-size_t image_bev_nms_scratch_bytes(int B, int cap) {
-    if (B < 1 || cap < 1) return 0;
-    return gb_layout(std::min(B, kGbMaxB), cap, 1).bytes;
+size_t image_bev_nms_scratch_bytes(int B, int cap, int num_classes) {
+    if (B < 1 || cap < 1 || num_classes < 1 || num_classes > kGbMaxCls) return 0;
+    return gb_layout(std::min(B, kGbMaxB), cap, 1, gb_class_bound(num_classes)).bytes;
 }
 
 cudaError_t launch_image_bev_nms(Det* dets, int32_t* counts, const float* K, const float* poses, const int32_t* sizes,
-                                 void* scratch, int32_t* flags, int B, int cap, float thr, cudaStream_t stream) {
-    if (B < 1 || cap < 1 || cap > kGbMaxCap || poses == nullptr) return cudaErrorInvalidValue;
+                                 void* scratch, int32_t* flags, int B, int cap, float thr, int num_classes,
+                                 cudaStream_t stream) {
+    if (B < 1 || cap < 1 || cap > kGbMaxCap || poses == nullptr || num_classes < 1 || num_classes > kGbMaxCls)
+        return cudaErrorInvalidValue;
     cudaError_t e = cudaSuccess;
     for (int b0 = 0; b0 < B && e == cudaSuccess; b0 += kGbMaxB) {  // chunks of kGbMaxB images share the scratch in order
         const int n = std::min(kGbMaxB, B - b0);
@@ -568,6 +574,7 @@ cudaError_t launch_image_bev_nms(Det* dets, int32_t* counts, const float* K, con
         p.num_groups = n;
         p.max_group_images = 1;
         p.max_dets = 0;
+        p.num_cls = gb_class_bound(num_classes);
         p.thr = thr;
         e = gb_launch(p, scratch, stream);
     }

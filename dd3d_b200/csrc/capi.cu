@@ -90,6 +90,11 @@ int dd3d_set_fpn_channels(dd3d_handle h, int32_t channels) {
     return guarded(h, [&](Engine& e) { e.set_fpn_channels(channels); });
 }
 
+int dd3d_set_canonical_sizes(dd3d_handle h, int32_t num_classes, const float* h_sizes) {
+    if (h_sizes == nullptr) return DD3D_ERR_INVALID;
+    return guarded(h, [&](Engine& e) { e.set_canonical_sizes(num_classes, h_sizes); });
+}
+
 int dd3d_load_weight(dd3d_handle h, const char* name, const float* data, const int64_t* shape, int ndim) {
     if (name == nullptr || data == nullptr || (ndim > 0 && shape == nullptr) || ndim < 0 || ndim > 8)
         return DD3D_ERR_INVALID;
@@ -652,6 +657,43 @@ int dd3d_op_b3d_sparse_c(const void* const* d_in, const int32_t* h_level_hw, con
     return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
 }
 
+int64_t dd3d_op_b3d_gather_scratch_bytes(int B, int C, int topk) {
+    if (B < 1 || C < 1 || C > kB3dGatherMaxC || topk < 1) return DD3D_ERR_INVALID;
+    return static_cast<int64_t>(b3d_gather_scratch_bytes(B, C, topk));
+}
+
+int dd3d_op_b3d_gather(const void* const* d_in, const int32_t* h_level_hw, const int32_t* h_pitch, const void* const* d_w,
+                       const float* const* d_scale, const float* const* d_bias, const void* d_fin, const int32_t* d_counts,
+                       int B, int C, int topk, int cin, float* d_rows, void* d_scratch, dd3d_stream stream) {
+    if (!d_in || !h_level_hw || !h_pitch || !d_w || !d_scale || !d_bias || !d_fin || !d_counts || !d_rows || !d_scratch)
+        return DD3D_ERR_INVALID;
+    if (B < 1 || C < 1 || C > kB3dGatherMaxC || topk < 1 || cin < 1) return DD3D_ERR_INVALID;
+    B3dGatherParams p;
+    memset(&p, 0, sizeof(p));
+    for (int l = 0; l < kLevels; ++l) {
+        B3dSparseLevel& v = p.lvl[l];
+        v.in = static_cast<const __nv_bfloat16*>(d_in[l]);
+        v.w = static_cast<const __nv_bfloat16*>(d_w[l]);
+        v.scale = d_scale[l];
+        v.bias = d_bias[l];
+        v.H = h_level_hw[2 * l];
+        v.W = h_level_hw[2 * l + 1];
+        v.pitch = h_pitch[l];
+        if (!v.scale || !v.bias || v.H < 1 || v.W < 1 || v.pitch < cin) return DD3D_ERR_INVALID;
+    }
+    p.fin = static_cast<const uint2*>(d_fin);
+    p.cand_count = d_counts;
+    p.rows = d_rows;
+    p.B = B;
+    p.C = C;
+    p.topk = topk;
+    p.fp16 = g_op_fp16;
+    p.cin = cin;
+    b3d_gather_bind_scratch(&p, d_scratch);
+    const cudaError_t e = launch_b3d_gather(p, static_cast<cudaStream_t>(stream));
+    return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
+}
+
 int dd3d_op_b3d_sparse(const void* const* d_in, const int32_t* h_level_hw, const int32_t* h_pitch, const void* const* d_w,
                        const float* const* d_scale, const float* const* d_bias, const void* d_fin, const int32_t* d_counts,
                        int B, int C, int topk, int n_pad, float* d_rows, int out_pitch, dd3d_stream stream) {
@@ -815,7 +857,7 @@ int dd3d_op_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsi
 
 int64_t dd3d_op_bev_nms_large_scratch_bytes(int B, int cap) {
     if (B < 1 || cap < 1 || cap > kLevels * kMaxPreNmsTopk) return DD3D_ERR_INVALID;
-    return static_cast<int64_t>(image_bev_nms_scratch_bytes(B, cap));
+    return static_cast<int64_t>(image_bev_nms_scratch_bytes(B, cap, DD3D_MAX_NUM_CLASSES));
 }
 
 int dd3d_op_bev_nms_large(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsics, const float* d_poses,
@@ -826,7 +868,7 @@ int dd3d_op_bev_nms_large(dd3d_det* d_dets, int32_t* d_counts, const float* d_in
         return DD3D_ERR_INVALID;
     return cuda_status(launch_image_bev_nms(reinterpret_cast<Det*>(d_dets), d_counts, d_intrinsics, d_poses,
                                             do_postprocess ? d_sizes : nullptr, d_scratch, d_flags, B, cap, iou_thresh,
-                                            static_cast<cudaStream_t>(stream)),
+                                            DD3D_MAX_NUM_CLASSES, static_cast<cudaStream_t>(stream)),
                        nullptr);
 }
 
@@ -915,14 +957,25 @@ int64_t dd3d_op_detect_scratch_bytes(int B, int pre_nms_topk) {
            static_cast<int64_t>(nms_scratch_bytes(B, pre_nms_topk, DD3D_MAX_CLASSES));
 }
 
-int dd3d_op_detect_flags(const dd3d_model_desc* desc, int B, const int32_t* h_level_hw, const int32_t* h_strides,
-                         const float* const* d_cls, const float* const* d_box, const float* const* d_b3d, int cls_pitch,
-                         int b3d_pitch, const float* d_intrinsics, const int32_t* d_sizes, void* d_scratch,
-                         dd3d_det* d_pre_nms, int32_t* d_pre_counts, dd3d_det* d_out, int32_t* d_counts, int32_t* d_flags,
-                         dd3d_stream stream_) {
+// scratch of dd3d_op_detect_c: decode | canonical sizes (256-byte aligned, [C][3] fp32) | NMS.  At C <= 16 this is the layout
+// dd3d_op_detect_scratch_bytes has always sized: the sizes take one 256-byte block.
+int64_t dd3d_op_detect_c_scratch_bytes(int B, int pre_nms_topk, int num_classes) {
+    if (B < 1 || pre_nms_topk < 1 || num_classes < 1 || num_classes > DD3D_MAX_NUM_CLASSES) return DD3D_ERR_INVALID;
+    const int64_t canon = (num_classes * 3 * 4 + 255) / 256 * 256;
+    return static_cast<int64_t>(decode_scratch_bytes(B, pre_nms_topk)) + 255 + canon + 256 +
+           static_cast<int64_t>(nms_scratch_bytes(B, pre_nms_topk, num_classes));
+}
+
+int dd3d_op_detect_c(const dd3d_model_desc* desc, const float* h_canon, int B, const int32_t* h_level_hw, const int32_t* h_strides,
+                     const float* const* d_cls, const float* const* d_box, const float* const* d_b3d, int cls_pitch,
+                     int b3d_pitch, const float* d_intrinsics, const int32_t* d_sizes, void* d_scratch,
+                     dd3d_det* d_pre_nms, int32_t* d_pre_counts, dd3d_det* d_out, int32_t* d_counts, int32_t* d_flags,
+                     dd3d_stream stream_) {
     if (!desc || !h_level_hw || !h_strides || !d_cls || !d_box || !d_b3d || !d_scratch || !d_out || !d_counts)
         return DD3D_ERR_INVALID;
     if (desc->pre_nms_topk < 1 || desc->pre_nms_topk > kMaxPreNmsTopk) return DD3D_ERR_INVALID;
+    const int C = desc->num_classes;
+    if (C < 1 || C > DD3D_MAX_NUM_CLASSES || (h_canon == nullptr && C > DD3D_MAX_CLASSES)) return DD3D_ERR_INVALID;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     DecodeParams dp;
     memset(&dp, 0, sizeof(dp));
@@ -937,8 +990,9 @@ int dd3d_op_detect_flags(const dd3d_model_desc* desc, int B, const int32_t* h_le
     // canonical sizes live at the tail of the caller's scratch
     const size_t dec_bytes = decode_scratch_bytes(B, desc->pre_nms_topk);
     float* d_canon = reinterpret_cast<float*>(static_cast<uint8_t*>(d_scratch) + (dec_bytes + 255) / 256 * 256);
-    cudaError_t c = cudaMemcpyAsync(d_canon, desc->canonical_box3d_sizes, DD3D_MAX_CLASSES * 3 * 4,
-                                    cudaMemcpyHostToDevice, stream);
+    cudaError_t c = h_canon ? cudaMemcpyAsync(d_canon, h_canon, static_cast<size_t>(C) * 3 * 4, cudaMemcpyHostToDevice, stream)
+                            : cudaMemcpyAsync(d_canon, desc->canonical_box3d_sizes, DD3D_MAX_CLASSES * 3 * 4,
+                                              cudaMemcpyHostToDevice, stream);
     if (c != cudaSuccess) return DD3D_ERR_CUDA;
     fill_decode_params(&dp, *desc, B, cls_pitch, b3d_pitch, d_canon);
     decode_bind_scratch(&dp, d_scratch);
@@ -954,13 +1008,25 @@ int dd3d_op_detect_flags(const dd3d_model_desc* desc, int B, const int32_t* h_le
     }
     NmsParams np;
     fill_nms_params(&np, *desc, dp, B);
-    np.scratch = reinterpret_cast<uint8_t*>(d_canon) + 256;  // behind the canonical sizes (192 B) at the tail of d_scratch
+    // behind the canonical sizes at the tail of d_scratch (one 256-byte block at C <= 16)
+    np.scratch = reinterpret_cast<uint8_t*>(d_canon) + (static_cast<size_t>(C) * 3 * 4 + 255) / 256 * 256;
     np.sizes = d_sizes;
     np.out = reinterpret_cast<Det*>(d_out);
     np.out_count = d_counts;
     c = launch_nms(np, stream);
     if (c == cudaSuccess && d_flags) c = cudaMemcpyAsync(d_flags, dp.flags, 4, cudaMemcpyDeviceToDevice, stream);
     return cuda_status(c, nullptr);
+}
+
+int dd3d_op_detect_flags(const dd3d_model_desc* desc, int B, const int32_t* h_level_hw, const int32_t* h_strides,
+                         const float* const* d_cls, const float* const* d_box, const float* const* d_b3d, int cls_pitch,
+                         int b3d_pitch, const float* d_intrinsics, const int32_t* d_sizes, void* d_scratch,
+                         dd3d_det* d_pre_nms, int32_t* d_pre_counts, dd3d_det* d_out, int32_t* d_counts, int32_t* d_flags,
+                         dd3d_stream stream) {
+    // its scratch (dd3d_op_detect_scratch_bytes) holds the NMS of DD3D_MAX_CLASSES classes
+    if (desc && desc->num_classes > DD3D_MAX_CLASSES) return DD3D_ERR_INVALID;
+    return dd3d_op_detect_c(desc, nullptr, B, h_level_hw, h_strides, d_cls, d_box, d_b3d, cls_pitch, b3d_pitch, d_intrinsics,
+                            d_sizes, d_scratch, d_pre_nms, d_pre_counts, d_out, d_counts, d_flags, stream);
 }
 
 int dd3d_op_detect(const dd3d_model_desc* desc, int B, const int32_t* h_level_hw, const int32_t* h_strides,

@@ -275,8 +275,10 @@ __device__ void decode_one(const DecodeParams& p, const DecodeLevel& L, int b, i
         *out = d;
         return;
     }
-    const int C = p.C3;  // channel = component * C3 + class (class 0 when class agnostic; fcos3d.py:333-352)
-    const float* g = g3d + (p.C3 == 1 ? 0 : c);
+    // channel = component * C3 + class (class 0 when class agnostic; fcos3d.py:333-352); the class-gathered rows hold the
+    // candidate's own class only
+    const int C = p.b3d_by_class ? 1 : p.C3;
+    const float* g = g3d + (C == 1 ? 0 : c);
     float q[4] = {__ldg(g), __ldg(g + C), __ldg(g + 2 * C), __ldg(g + 3 * C)};
     const float cx = __ldg(g + 4 * C), cy = __ldg(g + 5 * C);
     float depth = __ldg(g + 6 * C);
@@ -420,7 +422,7 @@ __device__ void select_overflow(const DecodeParams& p, int b, int l, uint32_t T,
     uint32_t base_above = 0, base_tie = 0;
     for (int p0 = 0; p0 < hw; p0 += blockDim.x) {
         const int pix = p0 + threadIdx.x;
-        uint32_t cnt = 0;  // (candidates above V << 16) | ties at V, of this pixel: <= 16 each, < 2^16 per chunk
+        uint32_t cnt = 0;  // (candidates above V << 16) | ties at V, of this pixel: <= C <= 128 each, < 2^16 per chunk
         if (pix < hw) {
             for_each_candidate(p, L, b, pix, [&](int, float s) {
                 const uint32_t key = score_key(p, s);
@@ -496,6 +498,7 @@ __global__ void __launch_bounds__(kFinalThreads) decode_final_kernel(const __gri
         const uint2 me = fin[i];
         const float* g3d = nullptr;
         if (p.box3d_on) {
+            // b3d_pitch is the row pitch of either sparse predictor (kB3dGatherPitch for the class-gathered one)
             g3d = p.b3d_rows != nullptr ? p.b3d_rows + (static_cast<size_t>(bl) * p.topk + i) * p.b3d_pitch
                                         : L.b3d + (static_cast<size_t>(b) * hw + me.y / p.C) * p.b3d_pitch;
         }

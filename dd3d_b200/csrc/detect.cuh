@@ -102,6 +102,9 @@ struct DecodeParams {
     // sparse 3-D head: the box3d predictor is evaluated only at the final candidates (b3d_sparse.cu); row of candidate `slot`
     // of (image b, level l) = b3d_rows + ((b * L + l) * topk + slot) * b3d_pitch, same channel layout as a dense map pixel
     const float* b3d_rows;  // nullptr: dense maps (lvl[].b3d)
+    // 1: b3d_rows come from the class-gathered predictor (b3d_gather.cu): channel q of the candidate's own class at column q,
+    // read as if C3 were 1
+    int b3d_by_class;
 };
 
 struct NmsParams {
@@ -173,10 +176,13 @@ cudaError_t launch_sample_aggregate(Det* dets, int32_t* counts, const float* K, 
 // 1: camera (CAMERA_TO_VEHICLE_ROTATION); global (or nullptr): [B][cap][10]; max_dets <= 0: no cap.
 // Image mode of the same kernels: the per-image BEV NMS of DD3D.forward on up to kLevels * kMaxPreNmsTopk unsorted boxes
 // per image (each image its own group, its own K [B][9] and pose [B][7], no cap); then detector_postprocess when sizes
-// ([B][4]) is not null.  Any B (chunks of 256 images share the scratch); flags bit 6 (64): a count above cap.
-size_t image_bev_nms_scratch_bytes(int B, int cap);
+// ([B][4]) is not null.  Any B (chunks of 256 images share the scratch); flags bit 6 (64): a count above cap.  num_classes
+// (1..128) sizes the per-group class table and the scan grid: 64 class segments up to 64 classes, 128 above.
+// The grouped mode (launch_group_bev_nms) always has 128 class segments: class ids 0..127.
+size_t image_bev_nms_scratch_bytes(int B, int cap, int num_classes);
 cudaError_t launch_image_bev_nms(Det* dets, int32_t* counts, const float* K, const float* poses, const int32_t* sizes,
-                                 void* scratch, int32_t* flags, int B, int cap, float thr, cudaStream_t stream);
+                                 void* scratch, int32_t* flags, int B, int cap, float thr, int num_classes,
+                                 cudaStream_t stream);
 int image_bev_nms_launches(int B);
 size_t group_bev_nms_scratch_bytes(int B, int cap, int max_group_images);
 cudaError_t launch_group_bev_nms(Det* dets, int32_t* counts, const float* view_K, int num_views, const float* poses,

@@ -25,6 +25,12 @@ namespace {
 
 inline int round_up(int v, int a) { return (v + a - 1) / a * a; }
 inline size_t round_up_sz(size_t v, size_t a) { return (v + a - 1) / a * a; }
+// Output channels a conv layer (and its epilogue vectors) is padded to: a multiple of 16, or of 64 when no N-block width of the
+// conv kernel divides that (wide class-specific heads: 11 x 26 = 286 -> 320)
+inline int cout_padded(int cout) {
+    const int p = round_up(cout, 16);
+    return conv_block_n(p) != 0 ? p : round_up(cout, 64);
+}
 
 [[noreturn]] void fail(int status, const std::string& msg) { throw EngineError(status, msg); }
 
@@ -38,7 +44,7 @@ void cuda_check(cudaError_t e, const char* what) {
 
 Engine::Engine(const dd3d_model_desc& d) : desc(d) {
     if (dla_spec(d.arch) == nullptr && vovnet_spec(d.arch) == nullptr) fail(DD3D_ERR_INVALID, "unknown arch");
-    if (d.num_classes < 1 || d.num_classes > DD3D_MAX_CLASSES) fail(DD3D_ERR_INVALID, "num_classes out of range");
+    if (d.num_classes < 1 || d.num_classes > DD3D_MAX_NUM_CLASSES) fail(DD3D_ERR_INVALID, "num_classes out of range");
     if (d.pre_nms_topk < 1 || d.pre_nms_topk > kMaxPreNmsTopk) fail(DD3D_ERR_INVALID, "pre_nms_topk out of range");
     if (d.out_cap < 1) fail(DD3D_ERR_INVALID, "out_cap must be positive");
     if (d.act_dtype != DD3D_ACT_BF16 && d.act_dtype != DD3D_ACT_FP16) fail(DD3D_ERR_INVALID, "unknown act_dtype");
@@ -123,7 +129,7 @@ const ConvLayer& Engine::conv_layer(const std::string& key, const std::vector<st
         cout += static_cast<int>(w.shape[0]);
     }
     L.cout = cout;
-    L.cout_pad = round_up(cout, 16);
+    L.cout_pad = cout_padded(cout);
     L.block_n = conv_block_n(L.cout_pad);  // 384 (slim VoVNet stage 4) -> 192
     if (L.block_n == 0) fail(DD3D_ERR_INVALID, "cout > 256 needs a multiple of 64 <= 256 that divides it: " + key);
     L.n_blocks = L.cout_pad / L.block_n;
@@ -242,6 +248,13 @@ void Engine::set_fpn_channels(int C) {
     fpn_channels = C;
 }
 
+void Engine::set_canonical_sizes(int num_classes, const float* sizes) {
+    if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_canonical_sizes after finalize");
+    if (num_classes != desc.num_classes || sizes == nullptr)
+        fail(DD3D_ERR_INVALID, "dd3d_set_canonical_sizes needs num_classes (" + std::to_string(desc.num_classes) + ") rows");
+    canonical_sizes.assign(sizes, sizes + static_cast<size_t>(num_classes) * 3);
+}
+
 // GroupNorm(32, C) affine of `<prefix>.weight` / `<prefix>.bias`, uploaded as fp32 vectors (cached like the epilogues)
 const Epilogue& Engine::gn_affine(const std::string& prefix, int C) {
     const std::string key = "gn|" + prefix;
@@ -284,7 +297,7 @@ const Epilogue& Engine::epilogue(const std::string& key, const std::vector<float
                                  const std::vector<float>* lo) {
     auto it = epis.find(key);
     if (it != epis.end()) return it->second;
-    const int n_pad = round_up(static_cast<int>(scale.size()), 16);
+    const int n_pad = cout_padded(static_cast<int>(scale.size()));
     std::vector<float> s(n_pad, 1.0f), b(n_pad, 0.0f);
     std::copy(scale.begin(), scale.end(), s.begin());
     std::copy(bias.begin(), bias.end(), b.begin());
@@ -1137,7 +1150,7 @@ struct Builder {
         const bool use_scale2 = E->desc.fcos2d_use_scale != 0, use_scale3 = E->desc.fcos3d_use_scale != 0;
         const bool per_level = E->desc.per_level_predictors != 0, box3d_on = E->desc.box3d_on != 0;
         const int C3 = E->desc.class_agnostic_box3d ? 1 : C;
-        const int cls_pitch = round_up(C + (nusc ? kNumAttributes + 1 : 0), 16), b3d_pitch = round_up(11 * C3, 16);
+        const int cls_pitch = round_up(C + (nusc ? kNumAttributes + 1 : 0), 16), b3d_pitch = cout_padded(11 * C3);
         // sparse box3d predictor: forced (1), off (0) or auto (2, default).  The dense launch costs time in proportion to the
         // head pixels, the gathered one a near-constant latency-bound K loop, so large heads go sparse.  The rule looks at
         // the head pixels of ONE image, not of the batch, so that an image gives bit-identical detections whatever batch it
@@ -1145,10 +1158,17 @@ struct Builder {
         // batch size, 384x1280 DLA-34 = 10 230 -> dense.
         size_t head_px = 0;
         for (int l = 0; l < L; ++l) head_px += static_cast<size_t>(feats[l].H) * feats[l].W;
-        const bool sparse3 = box3d_on && b3d_pitch <= kB3dSparseMaxN &&
+        // Class-specific heads wider than the sparse kernel's registers (C3 > 10) take the class-gathered predictor
+        // (b3d_gather.cu) under the same rule; C3 11..16 keep the dense predictor, as before that kernel existed.
+        const bool gather3 = box3d_on && C3 > DD3D_MAX_CLASSES;
+        const bool sparse3 = box3d_on && (b3d_pitch <= kB3dSparseMaxN || gather3) &&
                              (E->opt_sparse_box3d == 1 || (E->opt_sparse_box3d == 2 && head_px >= 50000));
+        const int rows_pitch = gather3 ? kB3dGatherPitch : b3d_pitch;
         P->sparse_b3d = sparse3;
-        P->b3d_rows = sparse3 ? alloc_f32(static_cast<size_t>(B) * kLevels * E->desc.pre_nms_topk * b3d_pitch) : nullptr;
+        P->gather_b3d = sparse3 && gather3;
+        P->b3d_rows = sparse3 ? alloc_f32(static_cast<size_t>(B) * kLevels * E->desc.pre_nms_topk * rows_pitch) : nullptr;
+        P->b3d_gather_scratch =
+            P->gather_b3d ? alloc_bytes(b3d_gather_scratch_bytes(B, C, E->desc.pre_nms_topk)) : nullptr;
         P->cls_pitch = cls_pitch;
         P->b3d_pitch = b3d_pitch;
         // each tower is followed at once by its predictor, so that its ping-pong buffers die before the next tower starts
@@ -1311,7 +1331,31 @@ struct Builder {
                 segs[l].out_f32 = P->b3d_map[l];
                 segs[l].out_pitch = b3d_pitch;
             }
-            if (sparse3) {
+            if (sparse3 && gather3) {
+                // as below, on the class-gathered kernel: 11 channels per candidate, those of its own class
+                B3dGatherParams& gp = P->b3d_gather;
+                memset(&gp, 0, sizeof(gp));
+                for (int l = 0; l < L; ++l) {
+                    const ConvLayer& Lw = layer_for(per_level ? l : 0);
+                    touch(b3d_t[l]);
+                    gp.lvl[l].in = b3d_t[l].ptr;
+                    gp.lvl[l].H = b3d_t[l].H;
+                    gp.lvl[l].W = b3d_t[l].W;
+                    gp.lvl[l].pitch = b3d_t[l].pitch;
+                    gp.lvl[l].w = Lw.d_w;
+                    gp.lvl[l].scale = segs[l].epi->d_scale;
+                    gp.lvl[l].bias = segs[l].epi->d_bias;
+                    if (Lw.cout < 11 * C || Lw.cin != width) fail(DD3D_ERR_INVALID, "box3d predictor shape");
+                }
+                ++op_idx;
+                gp.rows = P->b3d_rows;
+                gp.B = B;
+                gp.C = C;
+                gp.topk = E->desc.pre_nms_topk;
+                gp.fp16 = E->fp16;
+                gp.cin = width;
+                if (!dry) b3d_gather_bind_scratch(&gp, P->b3d_gather_scratch);
+            } else if (sparse3) {
                 // no dense launch: the predictor runs on the final candidates, after the threshold / top-k half of the decode
                 // (Engine::forward).  The tower outputs must outlive every op: a phantom op index keeps them in the arena.
                 B3dSparseParams& sp = P->b3d_sparse;
@@ -1547,7 +1591,7 @@ size_t Engine::build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry) 
         P->d_canon = nullptr;
         P->bev = bev_mode();
         if (P->bev) P->d_poses = static_cast<float*>(bld.alloc_bytes(static_cast<size_t>(B) * 7 * 4));
-        if (P->bev == kBevPathMultiCta) P->bev_scratch = bld.alloc_bytes(image_bev_nms_scratch_bytes(B, desc.out_cap));
+        if (P->bev == kBevPathMultiCta) P->bev_scratch = bld.alloc_bytes(image_bev_nms_scratch_bytes(B, desc.out_cap, desc.num_classes));
         if (tracing) {
             arena_bytes = plan_arena(bufs, opt_workspace_reuse != 0);
             total = arena_bytes + bld.off;
@@ -1562,8 +1606,12 @@ void Engine::finalize() {
     // dry graph walk with the smallest legal shape: creates (packs + uploads) every layer and names the first
     // missing tensor, without needing a workspace.
     Plan tmp;
+    if (canonical_sizes.empty() && desc.num_classes > DD3D_MAX_CLASSES && desc.box3d_on)
+        fail(DD3D_ERR_STATE, "num_classes " + std::to_string(desc.num_classes) + " > " + std::to_string(DD3D_MAX_CLASSES) +
+                                 " needs dd3d_set_canonical_sizes before dd3d_finalize");
     build(&tmp, 1, size_divisibility(), size_divisibility(), nullptr, true);
     std::vector<float> canon(desc.canonical_box3d_sizes, desc.canonical_box3d_sizes + DD3D_MAX_CLASSES * 3);
+    if (!canonical_sizes.empty()) canon = canonical_sizes;
     d_canon = upload_f32(canon);
     finalized = true;
     weights.clear();  // host copies are no longer needed
@@ -1652,7 +1700,13 @@ void Engine::make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes) {
     fill_decode_params(&dp, desc, B, plan.cls_pitch, plan.b3d_pitch, d_canon);
     decode_bind_scratch(&dp, plan.detect_scratch);
     decode_finalize_params(&dp);
-    if (plan.sparse_b3d) {
+    if (plan.gather_b3d) {
+        dp.b3d_rows = plan.b3d_rows;
+        dp.b3d_pitch = kB3dGatherPitch;
+        dp.b3d_by_class = 1;
+        plan.b3d_gather.fin = dp.fin;
+        plan.b3d_gather.cand_count = dp.cand_count;
+    } else if (plan.sparse_b3d) {
         dp.b3d_rows = plan.b3d_rows;
         plan.b3d_sparse.fin = dp.fin;
         plan.b3d_sparse.cand_count = dp.cand_count;
@@ -1743,7 +1797,7 @@ void Engine::set_host_poses(int slot, const float* h_poses) {
 }
 
 int Engine::launches_per_forward() const {
-    int n = bev_launches(plan) + 1 /*preprocess*/ + 6 /*decode: clear, 2 dense passes, 2 selects, final*/ + (plan.sparse_b3d ? 1 : 0) +
+    int n = bev_launches(plan) + 1 /*preprocess*/ + 6 /*decode: clear, 2 dense passes, 2 selects, final*/ + (plan.gather_b3d ? kB3dGatherLaunches : plan.sparse_b3d ? 1 : 0) +
             (plan.tower_begin >= 0 ? 1 : 0) /*tower tile lists*/ + (plan.box2d_begin >= 0 ? 2 : 0) /*box2d mark + lists*/ + ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) /*nms: sort, IoU bit matrix, scan, finish*/;
     for (const Op& op : plan.ops) n += (op.type == Op::ESE) ? 3 : (op.type == Op::GN && op.gn.gamma != nullptr) ? 2 : 1;
     return n;
@@ -1914,7 +1968,10 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
     }
     if (P.sparse_b3d) {
         if (P.tower_begin < 0) cuda_check(launch_decode_select(dp, stream), "decode (threshold + top-k)");
-        cuda_check(launch_b3d_sparse(P.b3d_sparse, stream), "sparse box3d predictor");
+        if (P.gather_b3d)
+            cuda_check(launch_b3d_gather(P.b3d_gather, stream), "class-gathered box3d predictor");
+        else
+            cuda_check(launch_b3d_sparse(P.b3d_sparse, stream), "sparse box3d predictor");
         cuda_check(launch_decode_final(dp, stream), "decode (boxes)");
     } else {
         cuda_check(launch_decode(dp, stream), "decode");
@@ -1933,7 +1990,7 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
                    "bev nms");
     else if (P.bev == kBevPathMultiCta)
         cuda_check(launch_image_bev_nms(d_out, d_counts, d_K, d_poses, opt_do_postprocess ? d_sizes : nullptr, P.bev_scratch,
-                                        P.decode.flags, P.B, desc.out_cap, bev_nms_thresh, stream),
+                                        P.decode.flags, P.B, desc.out_cap, bev_nms_thresh, desc.num_classes, stream),
                    "bev nms (multi-CTA)");
     mark(7);
     if (opt_profile) prof_used = ev_i;
@@ -2032,7 +2089,7 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
                 break;
         }
     }
-    launches[6] = 6 + (P.sparse_b3d ? 1 : 0) + (P.tower_begin >= 0 ? 1 : 0) + (P.box2d_begin >= 0 ? 2 : 0);
+    launches[6] = 6 + (P.gather_b3d ? kB3dGatherLaunches : P.sparse_b3d ? 1 : 0) + (P.tower_begin >= 0 ? 1 : 0) + (P.box2d_begin >= 0 ? 2 : 0);
     launches[7] = ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) + bev_launches(P);
     for (int l = 0; l < kLevels; ++l)  // two dense passes over the fp32 logits + centerness
         bytes[6] += 2.0 * P.B * P.lvl_h[l] * P.lvl_w[l] * (C + 1) * 4;

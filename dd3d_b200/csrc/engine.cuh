@@ -156,12 +156,17 @@ struct Plan {
     // BEV NMS as the last op of the forward (dd3d_set_bev_nms): 0 off, else bev_nms_path() of the config at plan time
     int bev = 0;
     float* d_poses = nullptr;      // [B][7] staging of the host poses (host paths, slot 0)
-    void* bev_scratch = nullptr;   // image_bev_nms_scratch_bytes(B, out_cap) (multi-CTA path only)
+    void* bev_scratch = nullptr;   // image_bev_nms_scratch_bytes(B, out_cap, num_classes) (multi-CTA path only)
     // sparse FCOS3D predictor (b3d_sparse.cu): the fused box3d conv runs only at the final 2-D candidates, between the two
     // halves of the decode; the dense fp32 maps b3d_map[] then do not exist
     bool sparse_b3d = false;
     float* b3d_rows = nullptr;  // [B][L][topk][b3d_pitch]
     B3dSparseParams b3d_sparse;
+    // class-gathered sparse predictor (b3d_gather.cu), for class-specific heads whose 11 C outputs exceed kB3dSparseMaxN: rows
+    // [B][L][topk][kB3dGatherPitch] in b3d_rows, same place in the forward as the sparse predictor (sparse_b3d is also set)
+    bool gather_b3d = false;
+    B3dGatherParams b3d_gather;
+    void* b3d_gather_scratch = nullptr;  // b3d_gather_scratch_bytes(B, C, topk): the class grouping
     // sparse box3d tower: ops [tower_begin, ops.size()) are the box3d tower convs.  They run after the threshold / top-k half
     // of the decode, in work-list mode on the tiles tower_tiles_kernel lists; every other pixel of their outputs keeps stale
     // workspace contents and is read by nothing.  -1: dense tower.
@@ -236,8 +241,11 @@ class Engine {
     void set_layout(const dd3d_layout_desc& l);
     void set_backbone_norm(int norm);
     void set_fpn_channels(int C);
+    void set_canonical_sizes(int num_classes, const float* sizes);
 
     dd3d_model_desc desc;
+    // FCOS3D.CANONICAL_BOX3D_SIZES rows 0..num_classes-1 (dd3d_set_canonical_sizes); empty: the desc's rows (num_classes <= 16)
+    std::vector<float> canonical_sizes;
     // FPN / head layout (dd3d_set_layout); the default is the shipped one
     dd3d_layout_desc layout = {DD3D_NORM_BN_PER_LEVEL, DD3D_NORM_BN_PER_LEVEL, DD3D_NORM_BN_SHARED, 4, 4, 4, 0};
     // FE.BACKBONE.NORM (dd3d_set_backbone_norm): BN folded into the conv epilogues (default), DD3D_NORM_NONE (DLA-34: conv bias)

@@ -9,7 +9,8 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_lib", "libdd3d_b200.so")
 
-MAX_CLASSES = 16
+MAX_CLASSES = 16        # DD3D_MAX_CLASSES: canonical-size rows of ModelDesc
+MAX_NUM_CLASSES = 128   # DD3D_MAX_NUM_CLASSES: largest DD3D.NUM_CLASSES (rows past 16 go through dd3d_set_canonical_sizes)
 NUM_LEVELS = 5
 ARCH_DLA34, ARCH_V2_99 = 0, 1
 # dd3d_arch of every arch key (dd3d_b200.arch.ARCH_KEYS)
@@ -88,6 +89,7 @@ SIGNATURES = {
     "dd3d_set_layout": (_I, [_P, C.POINTER(LayoutDesc)]),
     "dd3d_set_backbone_norm": (_I, [_P, C.c_int32]),
     "dd3d_set_fpn_channels": (_I, [_P, C.c_int32]),
+    "dd3d_set_canonical_sizes": (_I, [_P, C.c_int32, C.POINTER(C.c_float)]),
     "dd3d_load_weight": (_I, [_P, C.c_char_p, _P, C.POINTER(_I64), _I]),
     "dd3d_finalize": (_I, [_P]),
     "dd3d_workspace_bytes": (_I64, [_P, _I, _I, _I]),
@@ -127,6 +129,9 @@ SIGNATURES = {
                                 C.POINTER(_P), _P, _P, _I, _I, _I, _I, _P, _I, _P]),
     "dd3d_op_b3d_sparse_c": (_I, [C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P),
                                   C.POINTER(_P), _P, _P, _I, _I, _I, _I, _P, _I, _I, _P]),
+    "dd3d_op_b3d_gather_scratch_bytes": (_I64, [_I, _I, _I]),
+    "dd3d_op_b3d_gather": (_I, [C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P),
+                                C.POINTER(_P), _P, _P, _I, _I, _I, _I, _P, _P, _P]),
     "dd3d_op_dla_front": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_s2_mma": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_conv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
@@ -159,6 +164,9 @@ SIGNATURES = {
                             C.POINTER(_P), C.POINTER(_P), _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
     "dd3d_op_detect_flags": (_I, [C.POINTER(ModelDesc), _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P),
                                   C.POINTER(_P), C.POINTER(_P), _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "dd3d_op_detect_c_scratch_bytes": (_I64, [_I, _I, _I]),
+    "dd3d_op_detect_c": (_I, [C.POINTER(ModelDesc), C.POINTER(C.c_float), _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                              C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
 }
 
 _lib = None
@@ -220,6 +228,15 @@ def desc_from_cfg(cfg, out_cap=None):
     d.nuscenes_heads = int(is_nuscenes_arch(cfg))
     d.act_dtype = act_dtype_of(cfg)
     return d
+
+
+def canonical_sizes_from_cfg(cfg):
+    """FCOS3D.CANONICAL_BOX3D_SIZES rows 0..NUM_CLASSES-1 as the flat fp32 array of dd3d_set_canonical_sizes.  Fewer rows than
+    classes raise IndexError (the reference indexes the table by predicted class, fcos3d.py:378)."""
+    n, sizes = int(cfg.DD3D.NUM_CLASSES), cfg.DD3D.FCOS3D.CANONICAL_BOX3D_SIZES
+    if len(sizes) < n:
+        raise IndexError(f"FCOS3D.CANONICAL_BOX3D_SIZES has {len(sizes)} rows for DD3D.NUM_CLASSES = {n}")
+    return (C.c_float * (3 * n))(*[float(sizes[c][k]) for c in range(n) for k in range(3)])
 
 
 def layout_from_cfg(cfg):

@@ -39,6 +39,14 @@ class DD3DB200(nn.Module):
         self.backbone = SimpleNamespace(size_divisibility=size_divisibility(cfg))
         self._specs = param_specs(cfg)  # the reference's own errors first (nn.GroupNorm's ValueError for GN widths)
         self._fpn_channels = check_fpn_channels(cfg)  # FE.FPN.OUT_CHANNELS: a multiple of 64 in [64, 512]
+        if not 1 <= self.num_classes <= _lib.MAX_NUM_CLASSES:
+            raise NotImplementedError(f"DD3D.NUM_CLASSES = {self.num_classes} is not supported: the engine builds 1 to "
+                                      f"{_lib.MAX_NUM_CLASSES} classes")
+        # above 16 classes the sizes travel through dd3d_set_canonical_sizes; missing rows raise IndexError here, where the
+        # reference raises it at the first forward that predicts such a class (fcos3d.py:378)
+        self._canon = None
+        if cfg.MODEL.BOX3D_ON and self.num_classes > _lib.MAX_CLASSES:
+            self._canon = _lib.canonical_sizes_from_cfg(cfg)
         self._state = None  # reference-keyed fp32 CPU tensors
         self._device = torch.device("cpu")
         self._desc = _lib.desc_from_cfg(cfg)
@@ -129,6 +137,8 @@ class DD3DB200(nn.Module):
             _lib.check(L.dd3d_set_layout(handle, C.byref(self._layout)), handle)
             _lib.check(L.dd3d_set_backbone_norm(handle, self._backbone_norm), handle)
             _lib.check(L.dd3d_set_fpn_channels(handle, self._fpn_channels), handle)
+            if self._canon is not None:
+                _lib.check(L.dd3d_set_canonical_sizes(handle, self.num_classes, self._canon), handle)
             for name, t in self._state.items():
                 if not t.is_floating_point():
                     continue

@@ -62,14 +62,15 @@ enum dd3d_image_dtype { DD3D_IMG_U8 = 0, DD3D_IMG_F32 = 1 };
  * BASELINE.json configs[4]) -- 3 more mantissa bits, range +-65504. */
 enum dd3d_act_dtype { DD3D_ACT_BF16 = 0, DD3D_ACT_FP16 = 1 };
 
-#define DD3D_MAX_CLASSES 16
+#define DD3D_MAX_CLASSES 16      /* rows of dd3d_model_desc.canonical_box3d_sizes */
+#define DD3D_MAX_NUM_CLASSES 128 /* largest DD3D.NUM_CLASSES: above DD3D_MAX_CLASSES the sizes come from dd3d_set_canonical_sizes */
 #define DD3D_NUM_LEVELS 5
 
 /* Mirrors the cfg values DD3D.__init__ / FCOS2DInference / FCOS3DInference read
  * (core.py:20-55, fcos2d.py:242-249, fcos3d.py:302-313; defaults configs/models/dd3d.yaml). */
 typedef struct dd3d_model_desc {
     int32_t arch;        /* dd3d_arch: FE.BUILDER + FE.BACKBONE.NAME */
-    int32_t num_classes; /* DD3D.NUM_CLASSES (<= DD3D_MAX_CLASSES) */
+    int32_t num_classes; /* DD3D.NUM_CLASSES, 1..DD3D_MAX_NUM_CLASSES */
     float pixel_mean[3]; /* MODEL.PIXEL_MEAN (BGR) */
     float pixel_std[3];  /* MODEL.PIXEL_STD */
     int32_t feature_locations_offset_half; /* DD3D.FEATURE_LOCATIONS_OFFSET == "half" */
@@ -83,7 +84,8 @@ typedef struct dd3d_model_desc {
     float scale_depth_by_focal_lengths_factor;
     int32_t predict_allocentric_rot;        /* FCOS3D.PREDICT_ALLOCENTRIC_ROT */
     int32_t predict_distance;               /* FCOS3D.PREDICT_DISTANCE */
-    float canonical_box3d_sizes[DD3D_MAX_CLASSES * 3]; /* FCOS3D.CANONICAL_BOX3D_SIZES rows 0..num_classes-1 (W,L,H) */
+    float canonical_box3d_sizes[DD3D_MAX_CLASSES * 3]; /* FCOS3D.CANONICAL_BOX3D_SIZES rows 0..num_classes-1 (W,L,H); rows
+                                                        * 0..15 only: more classes pass theirs to dd3d_set_canonical_sizes */
     int32_t out_cap;        /* detection slots per image in the output buffer (>= post_nms_topk; ties may exceed it) */
     int32_t nuscenes_heads; /* MODEL.META_ARCHITECTURE == NuscenesDD3D: attr_logits (3) + speed (1, relu) predictor convs
                              * on the cls tower (nuscenes_dd3d.py:311-312,380-383) */
@@ -168,6 +170,12 @@ int dd3d_set_backbone_norm(dd3d_handle h, int32_t dd3d_norm);
  * unchanged.  An engine that never receives the call builds 256.  The sparse box2d / box3d towers need the pair tile, which
  * only widths that 128 divides run: at 64, 192, 320 and 448 those towers are dense (the sparse box3d predictor still runs). */
 int dd3d_set_fpn_channels(dd3d_handle h, int32_t channels);
+/* Sets FCOS3D.CANONICAL_BOX3D_SIZES, h_sizes = [num_classes][3] (W, L, H), before dd3d_finalize (DD3D_ERR_STATE afterwards);
+ * num_classes must equal the desc's (DD3D_ERR_INVALID otherwise).  Required when num_classes > DD3D_MAX_CLASSES and box3d_on
+ * (dd3d_finalize fails with DD3D_ERR_STATE without it); at 16 classes or fewer the desc's rows are used unless this call
+ * replaces them.  Class-specific heads above 16 classes run the box3d predictor at the final candidates only, 11 channels
+ * each, on the class-gathered kernel (csrc/b3d_gather.cu) under the "sparse_box3d" rule of dd3d_set_option. */
+int dd3d_set_canonical_sizes(dd3d_handle h, int32_t num_classes, const float* h_sizes);
 
 /* ---- weights: one call per tensor of the reference state_dict (Checkpointer.load, scripts/train.py:52) ----- */
 /* h_data: host fp32, contiguous, `ndim` dims in h_shape.  Unknown names are ignored (return DD3D_OK, e.g.
@@ -388,6 +396,18 @@ int dd3d_op_b3d_sparse_c(const void* const* d_in /*[5]*/, const int32_t* h_level
                          const void* const* d_w /*[5]*/, const float* const* d_scale /*[5]*/, const float* const* d_bias /*[5]*/,
                          const void* d_fin, const int32_t* d_counts, int B, int C, int topk, int n_pad, float* d_rows,
                          int out_pitch, int cin, dd3d_stream stream);
+/* dd3d_op_b3d_gather: the class-gathered sparse box3d predictor (csrc/b3d_gather.cu) on caller buffers: for every (image b,
+ * level l) and slot s < min(d_counts[b * 5 + l], topk) with class c = d_fin entry % C, row (b * 5 + l) * topk + s of d_rows
+ * (fp32, 16 floats per row) receives at column q < 11 channel q * C + c of the 3x3 conv of level l's tower output at the
+ * candidate's pixel, times d_scale[l][q * C + c] plus d_bias[l][q * C + c]: the values dd3d_op_b3d_sparse_c writes to those
+ * columns, bit for bit.  Columns 11..15 and other rows are not written.  d_in / h_level_hw / h_pitch / d_fin / cin as for
+ * dd3d_op_b3d_sparse_c; d_w[l]: 16-bit [>= 11 * C][9][cin]; C 1..128.  d_scratch: dd3d_op_b3d_gather_scratch_bytes(B, C, topk)
+ * bytes, any content. */
+int64_t dd3d_op_b3d_gather_scratch_bytes(int B, int C, int topk);
+int dd3d_op_b3d_gather(const void* const* d_in /*[5]*/, const int32_t* h_level_hw, const int32_t* h_pitch /*[5]*/,
+                       const void* const* d_w /*[5]*/, const float* const* d_scale /*[5]*/, const float* const* d_bias /*[5]*/,
+                       const void* d_fin, const int32_t* d_counts, int B, int C, int topk, int cin, float* d_rows,
+                       void* d_scratch, dd3d_stream stream);
 int dd3d_op_stem_conv(const void* d_in4, const void* d_w, const float* d_scale, const float* d_bias, void* d_out,
                       int B, int H, int W, int ksize, int stride, int cout, int out_pitch, dd3d_stream stream);
 /* dd3d_op_dla_front: the fused DLA-34 front end (csrc/dla_front.cu; reference dla.py:271-283,346-350 base_layer -> level0
@@ -453,7 +473,7 @@ int dd3d_op_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsi
  * image in any order (cap <= 5750): per image a sort by (class, scores_3d descending, slot), the rotated-IoU bit matrix on
  * all SMs, one greedy scan per (image, class), then an order-preserving compaction (with detector_postprocess when
  * do_postprocess != 0).  d_scratch: dd3d_op_bev_nms_large_scratch_bytes(B, cap) bytes, any content (about
- * min(B, 256) * cap^2 / 8 bytes: the IoU bit matrix).  d_flags bit 6 (64): a count above cap. */
+ * min(B, 256) * cap^2 / 8 bytes: the IoU bit matrix).  Class ids 0..127.  d_flags bit 6 (64): a count above cap. */
 int64_t dd3d_op_bev_nms_large_scratch_bytes(int B, int cap);
 int dd3d_op_bev_nms_large(dd3d_det* d_dets, int32_t* d_counts, const float* d_intrinsics, const float* d_poses,
                           const int32_t* d_sizes, void* d_scratch, int32_t* d_flags, int B, int cap, float iou_thresh,
@@ -504,7 +524,7 @@ int dd3d_op_sample_aggregate(dd3d_det* d_dets, int32_t* d_counts, const float* d
  * dd3d_op_group_bev_nms_scratch_bytes(B, cap, max_group_images) bytes, any content (about
  * B * cap^2 * max_group_images / 8 bytes: the IoU bit matrix).  Arguments out of range return DD3D_ERR_INVALID before any
  * launch; d_flags bit 5 (32) is set when a count exceeds cap, a group holds more than max_group_images images, or a group
- * index, class (>= 64) or view index is out of range. */
+ * index, class (>= 128) or view index is out of range. */
 enum dd3d_pose_mode { DD3D_POSE_GLOBAL = 0, DD3D_POSE_CAMERA = 1 };
 int64_t dd3d_op_group_bev_nms_scratch_bytes(int B, int cap, int max_group_images);
 int dd3d_op_group_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_view_K, int num_views, const float* d_poses,
@@ -512,6 +532,8 @@ int dd3d_op_group_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_vi
                           void* d_scratch, int32_t* d_flags, int B, int cap, float iou_thresh, int max_dets,
                           dd3d_stream stream);
 /* decode + NMS on caller-provided head maps (layout documented in csrc/detect.cuh). */
+/* dd3d_op_detect_scratch_bytes sizes the NMS scratch for DD3D_MAX_CLASSES classes (dd3d_op_detect / _flags take at most that
+ * many); dd3d_op_detect_c takes up to DD3D_MAX_NUM_CLASSES with dd3d_op_detect_c_scratch_bytes(B, pre_nms_topk, num_classes). */
 int64_t dd3d_op_detect_scratch_bytes(int B, int pre_nms_topk);
 int dd3d_op_detect(const dd3d_model_desc* h_desc, int B, const int32_t* h_level_hw /*[5][2]*/,
                    const int32_t* h_strides /*[5]*/, const float* const* d_cls /*[5]*/, const float* const* d_box,
@@ -525,6 +547,15 @@ int dd3d_op_detect_flags(const dd3d_model_desc* h_desc, int B, const int32_t* h_
                          const float* const* d_b3d, int cls_pitch, int b3d_pitch, const float* d_intrinsics,
                          const int32_t* d_sizes, void* d_scratch, dd3d_det* d_pre_nms, int32_t* d_pre_counts,
                          dd3d_det* d_out, int32_t* d_counts, int32_t* d_flags /* or NULL */, dd3d_stream stream);
+/* dd3d_op_detect_flags for h_desc->num_classes up to DD3D_MAX_NUM_CLASSES: h_canonical_sizes = [num_classes][3] host array of
+ * FCOS3D.CANONICAL_BOX3D_SIZES (NULL: the desc's rows, num_classes <= DD3D_MAX_CLASSES); d_scratch:
+ * dd3d_op_detect_c_scratch_bytes(B, pre_nms_topk, num_classes) bytes.  The head map layout is dd3d_op_detect's. */
+int64_t dd3d_op_detect_c_scratch_bytes(int B, int pre_nms_topk, int num_classes);
+int dd3d_op_detect_c(const dd3d_model_desc* h_desc, const float* h_canonical_sizes, int B, const int32_t* h_level_hw /*[5][2]*/,
+                     const int32_t* h_strides /*[5]*/, const float* const* d_cls /*[5]*/, const float* const* d_box,
+                     const float* const* d_b3d, int cls_pitch, int b3d_pitch, const float* d_intrinsics,
+                     const int32_t* d_sizes, void* d_scratch, dd3d_det* d_pre_nms, int32_t* d_pre_counts,
+                     dd3d_det* d_out, int32_t* d_counts, int32_t* d_flags /* or NULL */, dd3d_stream stream);
 
 #ifdef __cplusplus
 }
