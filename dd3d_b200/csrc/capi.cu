@@ -225,9 +225,7 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value) {
                 throw EngineError(DD3D_ERR_INVALID, "do_nms = 0 needs out_cap >= 5 * pre_nms_topk (" +
                                                         std::to_string(kLevels * e.desc.pre_nms_topk) + "), engine has " +
                                                         std::to_string(e.desc.out_cap) + ": recreate the engine");
-            const int bev = e.bev_mode();
-            if (bev && bev_nms_path(value ? 1 : 0, e.desc.post_nms_topk) != bev) e.drop_plans();  // BEV kernel changes
-            e.desc.do_nms = value ? 1 : 0;
+            e.set_do_nms(value ? 1 : 0);
         } else if (n == "profile") {
             e.opt_profile = value ? 1 : 0;
         } else if (n == "workspace_reuse") {  // applies to plans made afterwards
@@ -298,10 +296,10 @@ int dd3d_get_profile(dd3d_handle h, double* h_ms, double* h_flops, double* h_byt
     return guarded(h, [&](Engine& e) { e.get_profile(h_ms, h_flops, h_bytes, h_launches); });
 }
 
-int dd3d_get_op_times(dd3d_handle h, float* h_ms, int32_t* h_cats, double* h_flops, int max_ops) {
+int dd3d_get_op_times(dd3d_handle h, float* h_ms, int32_t* h_cats, double* h_flops, int32_t* h_ops, int max_ops) {
     if (!h_ms || !h_cats || !h_flops || max_ops < 1) return DD3D_ERR_INVALID;
     int n = 0;
-    int st = guarded(h, [&](Engine& e) { n = e.get_op_times(h_ms, h_cats, h_flops, max_ops); });
+    int st = guarded(h, [&](Engine& e) { n = e.get_op_times(h_ms, h_cats, h_flops, h_ops, max_ops); });
     return st == DD3D_OK ? n : st;
 }
 
@@ -1007,9 +1005,8 @@ int dd3d_op_detect_c(const dd3d_model_desc* desc, const float* h_canon, int B, c
                         stream);
     }
     NmsParams np;
-    fill_nms_params(&np, *desc, dp, B);
-    // behind the canonical sizes at the tail of d_scratch (one 256-byte block at C <= 16)
-    np.scratch = reinterpret_cast<uint8_t*>(d_canon) + (static_cast<size_t>(C) * 3 * 4 + 255) / 256 * 256;
+    // scratch behind the canonical sizes at the tail of d_scratch (one 256-byte block at C <= 16)
+    fill_nms_params(&np, *desc, dp, B, reinterpret_cast<uint8_t*>(d_canon) + (static_cast<size_t>(C) * 3 * 4 + 255) / 256 * 256);
     np.sizes = d_sizes;
     np.out = reinterpret_cast<Det*>(d_out);
     np.out_count = d_counts;

@@ -117,8 +117,11 @@ struct NmsParams {
     int B, topk, out_cap;
     int do_nms, post_topk, do_postprocess;
     float nms_thresh;
-    void* scratch;    // nms_scratch_bytes(B, topk, num_classes) bytes, or nullptr: single-CTA kernel (one CTA per image)
-    int num_classes;  // with scratch: IoU bit matrix on all SMs + one scan CTA per (class, image)
+    void* scratch;    // nms_scratch_bytes(B, topk, num_classes) bytes, or nullptr (single-CTA kernel only)
+    int num_classes;
+    // 1: the multi-CTA path (sort / IoU bit matrix on all SMs / one scan CTA per (class, image) / finish), 0: one CTA per
+    // image does the whole NMS.  Chosen once with nms_class_parallel() by whoever fills the params.
+    int class_parallel;
 };
 
 size_t decode_scratch_bytes(int B, int topk);
@@ -127,11 +130,17 @@ void decode_finalize_params(DecodeParams* p);
 cudaError_t launch_decode(const DecodeParams& p, cudaStream_t stream);  // = select + final
 // the two halves: threshold / top-k / final candidate list (fin, cand_count), then the per-candidate 2-D + 3-D decode;
 // the sparse box3d predictor runs between them
+constexpr int kDecodeSelectLaunches = 5;  // clear, dense pass, select, dense pass, final select
+constexpr int kDecodeFinalLaunches = 1;
 cudaError_t launch_decode_select(const DecodeParams& p, cudaStream_t stream);
 cudaError_t launch_decode_final(const DecodeParams& p, cudaStream_t stream);
-cudaError_t launch_nms(const NmsParams& p, cudaStream_t stream);
+cudaError_t launch_nms(const NmsParams& p, cudaStream_t stream);  // the path p.class_parallel names
+int nms_launches(const NmsParams& p);
 size_t nms_scratch_bytes(int B, int topk, int num_classes);
-void nms_set_class_parallel(int mode);  // 0 single-CTA kernel, 1 multi-CTA path (sort / IoU bit matrix / scan / finish), -1 environment / default (1)
+void nms_set_class_parallel(int mode);  // 0 single-CTA kernel, 1 multi-CTA path, -1 environment / default (1)
+// The NMS path for params whose other fields are filled: the multi-CTA one when the policy above allows it, the params
+// have its scratch, there is something to suppress (do_nms, nms_thresh > 0) and 1 <= num_classes <= 255.
+int nms_class_parallel(const NmsParams& p);
 // BEV rotated NMS of DD3D.forward (DO_BEV_NMS, core.py:137-151).  The one-CTA kernel (launch_bev_nms) holds kBevNmsMax
 // boxes per image and relies on them arriving sorted by scores_3d: the output of the 2-D NMS with 0 < POST_NMS_TOPK <=
 // kBevNmsMax.  Every other configuration -- DO_NMS off (all 5 * PRE_NMS_TOPK candidates, level-major) or POST_NMS_TOPK

@@ -17,6 +17,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <optional>
 #include <stdexcept>
 
 namespace dd3d {
@@ -617,6 +618,7 @@ struct Builder {
         op.ksize = ksize;
         op.outs[0] = out;
         op.nouts = 1;
+        op.bytes = (static_cast<double>(B) * in.H * in.W + static_cast<double>(B) * out.H * out.W) * in.C * 2;
         P->ops.push_back(op);
     }
     void relu(View in, View out) {
@@ -630,6 +632,7 @@ struct Builder {
         op.out = out;
         op.outs[0] = out;
         op.nouts = 1;
+        op.bytes = static_cast<double>(B) * in.H * in.W * in.C * 4;
         P->ops.push_back(op);
     }
 
@@ -798,6 +801,9 @@ struct Builder {
         op.stem = &S;
         op.outs[0] = out;
         op.nouts = 1;
+        const double in_px = static_cast<double>(B) * in4.H * in4.W, out_px = static_cast<double>(B) * out.H * out.W;
+        op.flops = 2.0 * out_px * S.cout * 3 * ksize * ksize;
+        op.bytes = in_px * 8 + out_px * S.cout * 2;
         P->ops.push_back(op);
     }
 
@@ -971,9 +977,12 @@ struct Builder {
         op.ksize = T;
         op.outs[0] = dst;
         op.nouts = 1;
+        // pooling is fused into the concat conv, or behind a GroupNorm one more pass over the map
+        op.bytes = static_cast<double>(B) * xt.H * xt.W * xt.C * 2 * ((identity ? 3 : 2) + (fused ? 0 : 1));
         if (pooled) {  // outs[1]: the 3x3 / s2 ceil-mode max-pool of dst, written by the same pass
             op.outs[1] = *pooled;
             op.nouts = 2;
+            op.bytes += static_cast<double>(B) * pooled->H * pooled->W * xt.C * 2;
         }
         P->ops.push_back(op);
     }
@@ -1730,8 +1739,37 @@ void Engine::make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes) {
         cuda_check(cudaMemset(tt.dist, kTowerTileFar & 0xFF, static_cast<size_t>(tt.cap) * 4), "cudaMemset(box2d tile distances)");
         cuda_check(cudaDeviceSynchronize(), "cudaDeviceSynchronize");
     }
-    fill_nms_params(&plan.nms, desc, dp, B);
-    plan.nms.scratch = plan.nms_scratch;
+    plan_steps(&plan);
+}
+
+void Engine::plan_steps(Plan* P) {
+    fill_nms_params(&P->nms, desc, P->decode, P->B, P->nms_scratch);
+    std::vector<Step>& S = P->steps;
+    S.clear();
+    auto add = [&](Step::Kind kind, int cat, int launches) -> Step& {  // the reference lives until the next add
+        S.push_back(Step{kind, -1, cat, launches});
+        return S.back();
+    };
+    add(Step::PREPROCESS, 0, kOneLaunch).bytes =
+        static_cast<double>(P->B) * 3 * P->Hs * P->Ws + static_cast<double>(P->B) * P->Hp * P->Wp * 8;
+    for (int oi = 0; oi < static_cast<int>(P->ops.size()); ++oi) {
+        if (oi == P->box2d_begin) add(Step::BOX2D_TILES, 6, kOneLaunch + kOneLaunch);  // seeds, tile lists
+        if (oi == P->tower_begin) add(Step::BOX3D_TILES, 6, kDecodeSelectLaunches + kOneLaunch);
+        const Op& op = P->ops[oi];
+        // special-purpose conv kernels are counted with the stems, so category 2 stays wgmma-only
+        const int cat = (op.type == Op::STEM || op.type == Op::FRONT || op.type == Op::DW) ? 1 : op.type == Op::CONV ? 2
+                        : op.type == Op::POOL ? 3 : op.type == Op::ESE ? 4 : 5;
+        add(Step::OP, cat, op.type == Op::ESE ? kEseLaunches : op.type == Op::GN ? group_norm_launches(op.gn) : kOneLaunch).op = oi;
+    }
+    Step& det = add(Step::DETECT, 6, kDecodeFinalLaunches);
+    det.select = P->tower_begin < 0;
+    det.b3d = P->gather_b3d ? Step::kB3dGathered : P->sparse_b3d ? Step::kB3dSparse : 0;
+    det.launches += (det.select ? kDecodeSelectLaunches : 0) + (P->gather_b3d ? kB3dGatherLaunches : P->sparse_b3d ? kOneLaunch : 0);
+    for (int l = 0; l < kLevels; ++l)  // two dense passes over the fp32 logits + centerness
+        det.bytes += 2.0 * P->B * P->lvl_h[l] * P->lvl_w[l] * (static_cast<double>(desc.num_classes) + 1) * 4;
+    add(Step::NMS, 7, nms_launches(P->nms) + (P->bev == kBevPathOneCta     ? kOneLaunch
+                                              : P->bev == kBevPathMultiCta ? image_bev_nms_launches(P->B) : 0))
+        .bev = P->bev;
 }
 
 void fill_decode_params(DecodeParams* dp, const dd3d_model_desc& desc, int B, int cls_pitch, int b3d_pitch,
@@ -1757,8 +1795,9 @@ void fill_decode_params(DecodeParams* dp, const dd3d_model_desc& desc, int B, in
     dp->box3d_on = desc.box3d_on;
 }
 
-void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodeParams& dp, int B) {
+void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodeParams& dp, int B, void* scratch) {
     memset(np, 0, sizeof(*np));
+    np->scratch = scratch;
     np->cand = dp.cand;
     np->cand_count = dp.cand_count;
     np->flags = dp.flags;
@@ -1770,13 +1809,17 @@ void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodePar
     np->do_postprocess = 1;
     np->nms_thresh = desc.nms_thresh;
     np->num_classes = desc.num_classes;
+    np->class_parallel = nms_class_parallel(*np);
 }
 
 int Engine::bev_mode() const { return opt_bev_nms ? bev_nms_path(desc.do_nms, desc.post_nms_topk) : 0; }
 
-// kernel launches of the BEV NMS op of a plan
-static int bev_launches(const Plan& P) {
-    return P.bev == kBevPathOneCta ? 1 : P.bev == kBevPathMultiCta ? image_bev_nms_launches(P.B) : 0;
+void Engine::set_do_nms(int do_nms) {
+    if (do_nms == desc.do_nms) return;
+    if (bev_mode() && bev_nms_path(do_nms, desc.post_nms_topk) != bev_mode()) drop_plans();  // BEV kernel changes
+    desc.do_nms = do_nms;
+    if (plan.valid) plan_steps(&plan);
+    for (auto& kv : plan_cache) plan_steps(&kv.second);
 }
 
 void Engine::set_bev_nms(int enable, float thr) {
@@ -1797,9 +1840,8 @@ void Engine::set_host_poses(int slot, const float* h_poses) {
 }
 
 int Engine::launches_per_forward() const {
-    int n = bev_launches(plan) + 1 /*preprocess*/ + 6 /*decode: clear, 2 dense passes, 2 selects, final*/ + (plan.gather_b3d ? kB3dGatherLaunches : plan.sparse_b3d ? 1 : 0) +
-            (plan.tower_begin >= 0 ? 1 : 0) /*tower tile lists*/ + (plan.box2d_begin >= 0 ? 2 : 0) /*box2d mark + lists*/ + ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) /*nms: sort, IoU bit matrix, scan, finish*/;
-    for (const Op& op : plan.ops) n += (op.type == Op::ESE) ? 3 : (op.type == Op::GN && op.gn.gamma != nullptr) ? 2 : 1;
+    int n = 0;
+    for (const Step& s : plan.steps) n += s.launches;
     return n;
 }
 
@@ -1845,23 +1887,18 @@ void Engine::forward_resized(const uint8_t* d_raw, int raw_h, int raw_w, const i
     cuda_check(cudaMemcpyAsync(P.d_K, h_K, static_cast<size_t>(P.B) * 36, cudaMemcpyHostToDevice, stream), "H2D K");
     cuda_check(cudaMemcpyAsync(P.d_sizes, h_sizes4, static_cast<size_t>(P.B) * 16, cudaMemcpyHostToDevice, stream),
                "H2D sizes");
-    raw_pending = true;
-    raw_args = {d_raw, raw_h, raw_w, h_raw_sizes, h_new_sizes, h_flip};
-    forward(nullptr, DD3D_IMG_U8, P.d_K, P.d_sizes, d_out, d_counts, user_poses, stream);
+    const RawArgs raw = {d_raw, raw_h, raw_w, h_raw_sizes, h_new_sizes, h_flip};
+    forward(nullptr, DD3D_IMG_U8, P.d_K, P.d_sizes, d_out, d_counts, user_poses, stream, &raw);
 }
 
 void Engine::forward(const void* d_images, int img_dtype, const float* d_K, const int32_t* d_sizes, Det* d_out,
-                     int32_t* d_counts, const float* d_poses, cudaStream_t stream) {
+                     int32_t* d_counts, const float* d_poses, cudaStream_t stream, const RawArgs* raw) {
     if (!plan.valid) fail(DD3D_ERR_STATE, "forward before plan");
     const Plan& P = plan;
-    if (P.bev && d_poses == nullptr) {
-        raw_pending = false;
+    if (P.bev && d_poses == nullptr)
         fail(DD3D_ERR_STATE, "BEV NMS is on: the forward needs the poses (dd3d_set_poses / dd3d_set_host_poses)");
-    }
-    const bool raw = raw_pending;
-    raw_pending = false;
     size_t ev_i = 0;
-    auto mark = [&](int cat, int op = -1) {  // opt_profile: CUDA events on the launch stream around every op
+    auto mark = [&](int cat, int op) {  // opt_profile: CUDA events on the launch stream around every step
         if (!opt_profile) return;
         if (ev_i >= prof_ev.size()) {
             cudaEvent_t e;
@@ -1875,125 +1912,128 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
         cuda_check(cudaEventRecord(prof_ev[ev_i++], stream), "cudaEventRecord");
     };
     plan.ran = true;
-    mark(-1);
-    // sizes (h, w, out_h, out_w) -> the (h, w) pairs the preprocess kernel reads are its first two columns
-    if (raw) {
-        cuda_check(resize_tables.launch(raw_args.d_raw, raw_args.raw_h, raw_args.raw_w, raw_args.h_raw_sizes,
-                                        raw_args.h_new_sizes, raw_args.h_flip, P.input.ptr, P.B, P.Hp, P.Wp, desc.pixel_mean, desc.pixel_std,
-                                        stream, fp16),
-                   "resize + preprocess");
-    } else {
-        cuda_check(launch_preprocess(d_images, img_dtype == DD3D_IMG_U8, d_sizes, 4, P.input.ptr, P.B, P.Hs, P.Ws, P.Hp,
-                                     P.Wp, desc.pixel_mean, desc.pixel_std, stream, fp16),
-                   "preprocess");
-    }
-    mark(0);
-    // from here on every launch follows one of our kernels: the small kernels may use programmatic dependent launch (pdl.cuh)
-    PdlScope pdl_scope;
+    mark(-1, -1);
+    std::optional<PdlScope> pdl_scope;  // opened behind the preprocess: every later launch follows one of our kernels (pdl.cuh)
     DecodeParams dp = P.decode;
     dp.K = d_K;
-    for (const Op& op : P.ops) {
-        const int oi = static_cast<int>(&op - P.ops.data());
-        if (oi == P.box2d_begin) {  // sparse box2d tower: the pixels of the cls maps that pass the threshold, then the tiles
-            cuda_check(launch_tower_mark(P.box2d_tiles, stream), "box2d tower seeds");
-            cuda_check(launch_tower_tiles(P.box2d_tiles, stream), "box2d tower tile lists");
-            mark(6);
+    for (const Step& s : P.steps) {
+        switch (s.kind) {
+            case Step::PREPROCESS:
+                // sizes (h, w, out_h, out_w) -> the (h, w) pairs the preprocess kernel reads are its first two columns
+                if (raw)
+                    cuda_check(resize_tables.launch(raw->d_raw, raw->raw_h, raw->raw_w, raw->h_raw_sizes, raw->h_new_sizes,
+                                                    raw->h_flip, P.input.ptr, P.B, P.Hp, P.Wp, desc.pixel_mean,
+                                                    desc.pixel_std, stream, fp16),
+                               "resize + preprocess");
+                else
+                    cuda_check(launch_preprocess(d_images, img_dtype == DD3D_IMG_U8, d_sizes, 4, P.input.ptr, P.B, P.Hs, P.Ws,
+                                                 P.Hp, P.Wp, desc.pixel_mean, desc.pixel_std, stream, fp16),
+                               "preprocess");
+                pdl_scope.emplace();
+                break;
+            case Step::OP:
+                launch_op(P.ops[s.op], stream);
+                break;
+            case Step::BOX2D_TILES:  // the pixels of the cls maps that pass the threshold, then the tiles
+                cuda_check(launch_tower_mark(P.box2d_tiles, stream), "box2d tower seeds");
+                cuda_check(launch_tower_tiles(P.box2d_tiles, stream), "box2d tower tile lists");
+                break;
+            case Step::BOX3D_TILES:  // the final candidates first, then the tiles they need
+                cuda_check(launch_decode_select(dp, stream), "decode (threshold + top-k)");
+                cuda_check(launch_tower_tiles(P.tower_tiles, stream), "box3d tower tile lists");
+                break;
+            case Step::DETECT:
+                if (s.select) cuda_check(launch_decode_select(dp, stream), "decode (threshold + top-k)");
+                if (s.b3d == Step::kB3dGathered)
+                    cuda_check(launch_b3d_gather(P.b3d_gather, stream), "class-gathered box3d predictor");
+                else if (s.b3d == Step::kB3dSparse)
+                    cuda_check(launch_b3d_sparse(P.b3d_sparse, stream), "sparse box3d predictor");
+                cuda_check(launch_decode_final(dp, stream), "decode (boxes)");
+                break;
+            case Step::NMS: {
+                NmsParams np = P.nms;
+                np.do_postprocess = s.bev ? 0 : opt_do_postprocess;  // with BEV NMS detector_postprocess follows it (core.py:137-160)
+                np.sizes = d_sizes;
+                np.out = d_out;
+                np.out_count = d_counts;
+                cuda_check(launch_nms(np, stream), "nms");
+                if (s.bev == kBevPathOneCta)
+                    cuda_check(launch_bev_nms(d_out, d_counts, d_K, d_poses, d_sizes, P.decode.flags, P.B, desc.out_cap,
+                                              bev_nms_thresh, opt_do_postprocess, stream),
+                               "bev nms");
+                else if (s.bev == kBevPathMultiCta)
+                    cuda_check(launch_image_bev_nms(d_out, d_counts, d_K, d_poses, opt_do_postprocess ? d_sizes : nullptr,
+                                                    P.bev_scratch, P.decode.flags, P.B, desc.out_cap, bev_nms_thresh,
+                                                    desc.num_classes, stream),
+                               "bev nms (multi-CTA)");
+                break;
+            }
         }
-        if (oi == P.tower_begin) {  // sparse box3d tower: the final candidates first, then the tiles they need
-            cuda_check(launch_decode_select(dp, stream), "decode (threshold + top-k)");
-            cuda_check(launch_tower_tiles(P.tower_tiles, stream), "box3d tower tile lists");
-            mark(6);
-        }
-        switch (op.type) {
-            case Op::CONV:
-                cuda_check(launch_conv(op.conv, num_sms, stream), "conv");
+        mark(s.cat, s.op);
+    }
+    if (opt_profile) prof_used = ev_i;
+}
+
+void Engine::launch_op(const Op& op, cudaStream_t stream) {
+    switch (op.type) {
+        case Op::CONV:
+            cuda_check(launch_conv(op.conv, num_sms, stream), "conv");
+            break;
+        case Op::STEM:
+            if (op.stem->d_w_mma != nullptr && opt_stem_mma) {
+                cuda_check(launch_stem_s2_mma(op.in.ptr, op.stem->d_w_mma, op.stem->d_sb_mma, op.out.ptr, op.out.pitch, plan.B,
+                                              op.in.H, op.in.W, num_sms, stream, fp16, op.stem->relu ? 1 : 0),
+                           "stem conv (mma)");
                 break;
-            case Op::STEM:
-                if (op.stem->d_w_mma != nullptr && opt_stem_mma) {
-                    cuda_check(launch_stem_s2_mma(op.in.ptr, op.stem->d_w_mma, op.stem->d_sb_mma, op.out.ptr, op.out.pitch, P.B,
-                                                  op.in.H, op.in.W, num_sms, stream, fp16, op.stem->relu ? 1 : 0),
-                               "stem conv (mma)");
-                    break;
-                }
-                cuda_check(launch_stem_tc(op.in.ptr, op.stem->d_w, op.stem->epi.d_scale, op.stem->epi.d_bias, op.out.ptr,
-                                          P.B, op.in.H, op.in.W, op.ksize, op.stride, op.stem->cout, op.out.pitch, num_sms,
-                                          stream, fp16, op.stem->relu ? 1 : 0),
-                           "stem conv");
-                break;
-            case Op::POOL:
-                cuda_check(launch_maxpool(op.in.ptr, op.out.ptr, P.B, op.in.H, op.in.W, op.in.C, op.in.pitch, op.out.H,
-                                          op.out.W, op.out.pitch, op.ksize, num_sms, stream, fp16),
-                           "maxpool");
-                break;
-            case Op::ESE:
-                if (op.f2 == nullptr) {  // behind a GroupNorm: pool pass over the normalised map -> fc -> scale
-                    cuda_check(launch_ese(op.in.ptr, op.in.pitch, op.ese->d_w, op.ese->d_b,
-                                          op.has_identity ? op.identity.ptr : nullptr, op.has_identity ? op.identity.pitch : 0,
-                                          op.out.ptr, op.out.pitch, op.f0, op.f1, P.B, op.in.H * op.in.W, op.in.C, num_sms,
-                                          stream, fp16, op.nouts == 2 ? op.outs[1].ptr : nullptr,
-                                          op.nouts == 2 ? op.outs[1].pitch : 0, op.in.H, op.in.W),
-                               "eSE");
-                    break;
-                }
-                cuda_check(launch_ese_fused(op.in.ptr, op.in.pitch, op.f2, op.ksize, op.ese->d_w, op.ese->d_b,
-                                            op.has_identity ? op.identity.ptr : nullptr,
-                                            op.has_identity ? op.identity.pitch : 0, op.out.ptr, op.out.pitch, op.f0, op.f1,
-                                            P.B, op.in.H * op.in.W, op.in.C, num_sms, stream, fp16,
-                                            op.nouts == 2 ? op.outs[1].ptr : nullptr, op.nouts == 2 ? op.outs[1].pitch : 0,
-                                            op.in.H, op.in.W),
+            }
+            cuda_check(launch_stem_tc(op.in.ptr, op.stem->d_w, op.stem->epi.d_scale, op.stem->epi.d_bias, op.out.ptr,
+                                      plan.B, op.in.H, op.in.W, op.ksize, op.stride, op.stem->cout, op.out.pitch, num_sms,
+                                      stream, fp16, op.stem->relu ? 1 : 0),
+                       "stem conv");
+            break;
+        case Op::POOL:
+            cuda_check(launch_maxpool(op.in.ptr, op.out.ptr, plan.B, op.in.H, op.in.W, op.in.C, op.in.pitch, op.out.H,
+                                      op.out.W, op.out.pitch, op.ksize, num_sms, stream, fp16),
+                       "maxpool");
+            break;
+        case Op::ESE:
+            if (op.f2 == nullptr) {  // behind a GroupNorm: pool pass over the normalised map -> fc -> scale
+                cuda_check(launch_ese(op.in.ptr, op.in.pitch, op.ese->d_w, op.ese->d_b,
+                                      op.has_identity ? op.identity.ptr : nullptr, op.has_identity ? op.identity.pitch : 0,
+                                      op.out.ptr, op.out.pitch, op.f0, op.f1, plan.B, op.in.H * op.in.W, op.in.C, num_sms,
+                                      stream, fp16, op.nouts == 2 ? op.outs[1].ptr : nullptr,
+                                      op.nouts == 2 ? op.outs[1].pitch : 0, op.in.H, op.in.W),
                            "eSE");
                 break;
-            case Op::RELU:
-                cuda_check(launch_relu(op.in.ptr, op.out.ptr, static_cast<size_t>(P.B) * op.in.H * op.in.W * op.in.C,
-                                       num_sms, stream),
-                           "relu");
-                break;
-            case Op::FRONT:
-                cuda_check(launch_dla_front(op.in.ptr, op.front->d_w0, op.front->d_w1, op.front->d_w2, op.front->d_sb0,
-                                            op.front->d_sb1, op.front->d_sb2, op.out.ptr, op.out.pitch, op.identity.ptr,
-                                            op.identity.pitch, P.B, op.in.H, op.in.W, num_sms, stream, fp16),
-                           "dla front");
-                break;
-            case Op::DW:
-                cuda_check(launch_dwconv3x3(op.in.ptr, P.B, op.in.H, op.in.W, op.in.C, op.in.pitch, op.dw->d_w, op.stride,
-                                            op.out.ptr, op.out.pitch, stream, fp16),
-                           "depthwise conv");
-                break;
-            case Op::GN:
-                cuda_check(launch_group_norm(op.gn, stream), "group norm");
-                break;
-        }
-        mark((op.type == Op::STEM || op.type == Op::FRONT || op.type == Op::DW) ? 1 : op.type == Op::CONV ? 2 : op.type == Op::POOL ? 3 : op.type == Op::ESE ? 4 : 5,
-             oi);
+            }
+            cuda_check(launch_ese_fused(op.in.ptr, op.in.pitch, op.f2, op.ksize, op.ese->d_w, op.ese->d_b,
+                                        op.has_identity ? op.identity.ptr : nullptr,
+                                        op.has_identity ? op.identity.pitch : 0, op.out.ptr, op.out.pitch, op.f0, op.f1,
+                                        plan.B, op.in.H * op.in.W, op.in.C, num_sms, stream, fp16,
+                                        op.nouts == 2 ? op.outs[1].ptr : nullptr, op.nouts == 2 ? op.outs[1].pitch : 0,
+                                        op.in.H, op.in.W),
+                       "eSE");
+            break;
+        case Op::RELU:
+            cuda_check(launch_relu(op.in.ptr, op.out.ptr, static_cast<size_t>(plan.B) * op.in.H * op.in.W * op.in.C,
+                                   num_sms, stream),
+                       "relu");
+            break;
+        case Op::FRONT:
+            cuda_check(launch_dla_front(op.in.ptr, op.front->d_w0, op.front->d_w1, op.front->d_w2, op.front->d_sb0,
+                                        op.front->d_sb1, op.front->d_sb2, op.out.ptr, op.out.pitch, op.identity.ptr,
+                                        op.identity.pitch, plan.B, op.in.H, op.in.W, num_sms, stream, fp16),
+                       "dla front");
+            break;
+        case Op::DW:
+            cuda_check(launch_dwconv3x3(op.in.ptr, plan.B, op.in.H, op.in.W, op.in.C, op.in.pitch, op.dw->d_w, op.stride,
+                                        op.out.ptr, op.out.pitch, stream, fp16),
+                       "depthwise conv");
+            break;
+        case Op::GN:
+            cuda_check(launch_group_norm(op.gn, stream), "group norm");
+            break;
     }
-    if (P.sparse_b3d) {
-        if (P.tower_begin < 0) cuda_check(launch_decode_select(dp, stream), "decode (threshold + top-k)");
-        if (P.gather_b3d)
-            cuda_check(launch_b3d_gather(P.b3d_gather, stream), "class-gathered box3d predictor");
-        else
-            cuda_check(launch_b3d_sparse(P.b3d_sparse, stream), "sparse box3d predictor");
-        cuda_check(launch_decode_final(dp, stream), "decode (boxes)");
-    } else {
-        cuda_check(launch_decode(dp, stream), "decode");
-    }
-    mark(6);
-    NmsParams np = P.nms;
-    np.do_postprocess = P.bev ? 0 : opt_do_postprocess;  // with BEV NMS detector_postprocess follows it (core.py:137-160)
-    np.do_nms = desc.do_nms;
-    np.sizes = d_sizes;
-    np.out = d_out;
-    np.out_count = d_counts;
-    cuda_check(launch_nms(np, stream), "nms");
-    if (P.bev == kBevPathOneCta)
-        cuda_check(launch_bev_nms(d_out, d_counts, d_K, d_poses, d_sizes, P.decode.flags, P.B, desc.out_cap, bev_nms_thresh,
-                                  opt_do_postprocess, stream),
-                   "bev nms");
-    else if (P.bev == kBevPathMultiCta)
-        cuda_check(launch_image_bev_nms(d_out, d_counts, d_K, d_poses, opt_do_postprocess ? d_sizes : nullptr, P.bev_scratch,
-                                        P.decode.flags, P.B, desc.out_cap, bev_nms_thresh, desc.num_classes, stream),
-                   "bev nms (multi-CTA)");
-    mark(7);
-    if (opt_profile) prof_used = ev_i;
 }
 
 // Algorithmic FLOPs per plan op.  The convs of the sparse towers count the in-map pixels of the tiles the last forward ran,
@@ -2019,9 +2059,8 @@ std::vector<double> Engine::op_flops() {
     return f;
 }
 
-// per-op device time of the last profiled forward: entry 0 = preprocess, then plan.ops in order (with the sparse box3d
-// tower, the threshold / top-k and the tile lists before the tower convs), then decode, nms
-int Engine::get_op_times(float* ms, int32_t* cats, double* flops, int max_ops) {
+// per-step device time of the last profiled forward (Plan::steps in order), with the plan op each step ran (or -1)
+int Engine::get_op_times(float* ms, int32_t* cats, double* flops, int32_t* ops, int max_ops) {
     if (!plan.valid) fail(DD3D_ERR_STATE, "no plan");
     if (prof_used < 2) return 0;
     cuda_check(cudaEventSynchronize(prof_ev[prof_used - 1]), "cudaEventSynchronize");
@@ -2031,6 +2070,7 @@ int Engine::get_op_times(float* ms, int32_t* cats, double* flops, int max_ops) {
         cuda_check(cudaEventElapsedTime(&ms[n], prof_ev[i - 1], prof_ev[i]), "cudaEventElapsedTime");
         cats[n] = prof_cat[i];
         flops[n] = (prof_op[i] >= 0 && prof_op[i] < static_cast<int>(f.size())) ? f[prof_op[i]] : 0.0;
+        if (ops) ops[n] = prof_op[i];
     }
     return n;
 }
@@ -2046,53 +2086,12 @@ void Engine::get_profile(double* ms, double* flops, double* bytes, int32_t* laun
             ms[prof_cat[i]] += t;
         }
     }
-    const Plan& P = plan;
-    const double C = desc.num_classes;
     const std::vector<double> f = op_flops();
-    launches[0] = 1;
-    bytes[0] = static_cast<double>(P.B) * 3 * P.Hs * P.Ws + static_cast<double>(P.B) * P.Hp * P.Wp * 8;
-    for (const Op& op : P.ops) {
-        const double in_px = static_cast<double>(P.B) * op.in.H * op.in.W, out_px = static_cast<double>(P.B) * op.out.H * op.out.W;
-        switch (op.type) {
-            case Op::STEM:
-                launches[1] += 1;
-                flops[1] += 2.0 * out_px * op.stem->cout * 3 * op.ksize * op.ksize;
-                bytes[1] += in_px * 8 + out_px * op.stem->cout * 2;
-                break;
-            case Op::CONV:
-                launches[2] += 1;
-                flops[2] += f[&op - P.ops.data()];
-                break;
-            case Op::POOL:
-                launches[3] += 1;
-                bytes[3] += (in_px + out_px) * op.in.C * 2;
-                break;
-            case Op::ESE:
-                launches[4] += 3;
-                // pooling is fused into the concat conv, or behind a GroupNorm one more pass over the map
-                bytes[4] += in_px * op.in.C * 2 * ((op.has_identity ? 3 : 2) + (op.f2 == nullptr ? 1 : 0));
-                if (op.nouts == 2) bytes[4] += static_cast<double>(P.B) * op.outs[1].H * op.outs[1].W * op.in.C * 2;
-                break;
-            case Op::RELU:
-                launches[5] += 1;
-                bytes[5] += in_px * op.in.C * 4;
-                break;
-            case Op::GN:  // statistics + apply (one launch without the affine)
-                launches[5] += op.gn.gamma != nullptr ? 2 : 1;
-                bytes[5] += op.bytes;
-                break;
-            case Op::FRONT:
-            case Op::DW:  // special-purpose conv kernels are counted with the stems, so category 2 stays wgmma-only
-                launches[1] += 1;
-                flops[1] += op.flops;
-                bytes[1] += op.bytes;
-                break;
-        }
+    for (const Step& s : plan.steps) {
+        launches[s.cat] += s.launches;
+        flops[s.cat] += s.op >= 0 ? f[s.op] : 0.0;
+        bytes[s.cat] += s.op >= 0 ? plan.ops[s.op].bytes : s.bytes;
     }
-    launches[6] = 6 + (P.gather_b3d ? kB3dGatherLaunches : P.sparse_b3d ? 1 : 0) + (P.tower_begin >= 0 ? 1 : 0) + (P.box2d_begin >= 0 ? 2 : 0);
-    launches[7] = ((desc.do_nms && desc.nms_thresh > 0.f) ? 4 : 1) + bev_launches(P);
-    for (int l = 0; l < kLevels; ++l)  // two dense passes over the fp32 logits + centerness
-        bytes[6] += 2.0 * P.B * P.lvl_h[l] * P.lvl_w[l] * (C + 1) * 4;
 }
 
 void Engine::forward_host(const void* h_images, int img_dtype, const float* h_K, const int32_t* h_sizes, Det* h_out,

@@ -122,6 +122,27 @@ struct Op {
     double bytes = 0.0;  // algorithmic HBM bytes for the bandwidth-bound ops
 };
 
+// One step of the forward = one profile event (Engine::plan_steps).  The forward launches the steps in order; the launch
+// count and the profile are sums over them.
+struct Step {
+    enum Kind {
+        PREPROCESS,   // caller images or the raw-image resize -> padded input
+        OP,           // plan op `op`
+        BOX2D_TILES,  // sparse box2d tower: seeds (pixels passing the class-only threshold) + tile lists
+        BOX3D_TILES,  // sparse box3d tower: decode threshold / top-k + tile lists around the final candidates
+        DETECT,       // [decode threshold / top-k] [sparse or gathered box3d predictor] decode of the final candidates
+        NMS,          // NMS [+ BEV NMS]
+    } kind;
+    int op = -1;        // OP: index into Plan::ops, else -1
+    int cat = 0;        // profile category (Engine::get_profile)
+    int launches = 0;   // kernels the step enqueues
+    double bytes = 0.0;  // algorithmic HBM bytes of a non-op step (an op's are Op::bytes)
+    bool select = false;  // DETECT: the threshold / top-k half runs here (no BOX3D_TILES step ran it)
+    int b3d = 0;          // DETECT: box3d predictor at the final candidates: 0 none (dense maps), kB3dSparse, kB3dGathered
+    int bev = 0;          // NMS: 0, or the bev_nms_path() of the BEV NMS that follows
+    static constexpr int kB3dSparse = 1, kB3dGathered = 2;
+};
+
 struct Plan {
     bool valid = false;
     int B = 0, Hs = 0, Ws = 0, Hp = 0, Wp = 0;
@@ -177,12 +198,13 @@ struct Plan {
     // right before them); the box map holds stale workspace contents outside those tiles.  -1: dense.
     int box2d_begin = -1;
     TowerTilesParams box2d_tiles;
+    std::vector<Step> steps;  // what a forward of this plan launches, in order
     bool ran = false;  // a forward has run on this plan (the tile counts on the device are valid)
 };
 
 void fill_decode_params(DecodeParams* dp, const dd3d_model_desc& desc, int B, int cls_pitch, int b3d_pitch,
                         const float* d_canon);
-void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodeParams& dp, int B);
+void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodeParams& dp, int B, void* scratch);
 
 class Engine {
    public:
@@ -193,9 +215,16 @@ class Engine {
     int size_divisibility() const;
     size_t workspace_bytes(int B, int Hs, int Ws);
     void make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes);
-    // d_poses: [B][7] poses the BEV NMS reads (unused when it is off)
+    struct RawArgs {  // raw dataset images the preprocess resizes (forward_resized)
+        const uint8_t* d_raw;
+        int raw_h, raw_w;
+        const int32_t* h_raw_sizes;
+        const int32_t* h_new_sizes;
+        const int32_t* h_flip;
+    };
+    // d_poses: [B][7] poses the BEV NMS reads (unused when it is off); the preprocess reads `raw` when given, else d_images
     void forward(const void* d_images, int img_dtype, const float* d_K, const int32_t* d_sizes, Det* d_out,
-                 int32_t* d_counts, const float* d_poses, cudaStream_t stream);
+                 int32_t* d_counts, const float* d_poses, cudaStream_t stream, const RawArgs* raw = nullptr);
     void forward_host(const void* h_images, int img_dtype, const float* h_K, const int32_t* h_sizes, Det* h_out,
                       int32_t* h_counts, cudaStream_t stream);
     // double-buffered host path: H2D of one slot on a private copy stream while the other slot computes
@@ -212,6 +241,7 @@ class Engine {
                          const int32_t* h_flip, const float* h_K, const int32_t* h_sizes4, Det* d_out, int32_t* d_counts,
                          cudaStream_t stream);
     void drop_plans();  // frees the active and the cached plans (an option that changes the op graph was flipped)
+    void set_do_nms(int do_nms);  // DO_NMS at run time: the plans' NMS steps follow it
     int launches_per_forward() const;
     // BEV NMS (DO_BEV_NMS): on / off and its IoU threshold; the poses of dd3d_forward / dd3d_forward_raw (device) and of
     // the host paths (copied per slot)
@@ -220,7 +250,7 @@ class Engine {
     void set_host_poses(int slot, const float* h_poses);
     // categories: 0 preprocess, 1 stem and depthwise conv, 2 conv (wgmma), 3 pool, 4 eSE, 5 relu and GroupNorm, 6 decode, 7 nms
     void get_profile(double* ms, double* flops, double* bytes, int32_t* launches);
-    int get_op_times(float* ms, int32_t* cats, double* flops, int max_ops);
+    int get_op_times(float* ms, int32_t* cats, double* flops, int32_t* ops, int max_ops);  // ops may be null
 
     // layer factories (cached by key)
     const HostTensor& weight(const std::string& name) const;
@@ -301,19 +331,13 @@ class Engine {
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t h2d_done[2] = {nullptr, nullptr}, all_done[2] = {nullptr, nullptr};
     bool slot_busy[2] = {false, false};
-    struct RawArgs {
-        const uint8_t* d_raw;
-        int raw_h, raw_w;
-        const int32_t* h_raw_sizes;
-        const int32_t* h_new_sizes;
-        const int32_t* h_flip;
-    } raw_args{};
-    bool raw_pending = false;  // set by forward_raw for the forward() call it makes
 
    private:
+    void launch_op(const Op& op, cudaStream_t stream);
     void* dev_alloc(size_t bytes);
     float* upload_f32(const std::vector<float>& v);
     size_t build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry);
+    void plan_steps(Plan* P);  // the NMS params and the step list of a built plan
     void release_plan();
     static void free_plan(Plan* P);
     std::vector<double> op_flops();

@@ -313,4 +313,6 @@ cudaError_t launch_group_norm(GroupNormParams p, cudaStream_t stream) {
     }
 }
 
+int group_norm_launches(const GroupNormParams& p) { return p.gamma != nullptr ? 2 : 1; }
+
 }  // namespace dd3d

@@ -37,5 +37,6 @@ int group_norm_chunks(int H, int W);
 size_t group_norm_scratch_bytes(int B, int H, int W);
 // One launch of the statistics kernel (skipped when gamma == nullptr) and one of the apply kernel over every segment.
 cudaError_t launch_group_norm(GroupNormParams p, cudaStream_t stream);
+int group_norm_launches(const GroupNormParams& p);
 
 }  // namespace dd3d

@@ -617,6 +617,17 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_finish_kernel(const __grid
 static int g_class_parallel = -1;
 void nms_set_class_parallel(int mode) { g_class_parallel = (mode == 0 || mode == 1) ? mode : -1; }
 
+int nms_class_parallel(const NmsParams& p) {
+    if (g_class_parallel < 0) {  // DD3D_NMS_CLASS_PARALLEL=0 / dd3d_set_conv_policy("nms_class_parallel", 0): single-CTA kernel
+        const char* e = getenv("DD3D_NMS_CLASS_PARALLEL");
+        g_class_parallel = (e && atoi(e) == 0) ? 0 : 1;
+    }
+    return g_class_parallel && p.scratch != nullptr && p.do_nms && p.nms_thresh > 0.f && p.num_classes >= 1 &&
+           p.num_classes <= 255;
+}
+
+int nms_launches(const NmsParams& p) { return p.class_parallel ? 4 : 1; }
+
 size_t nms_scratch_bytes(int B, int topk, int num_classes) {
     const int cap = kLevels * topk;
     const NmsScratch sc = bind_nms_scratch(nullptr, B, cap, num_classes);
@@ -643,11 +654,7 @@ cudaError_t launch_nms(const NmsParams& p, cudaStream_t stream) {
         }
         attr_smem = smem;
     }
-    if (g_class_parallel < 0) {  // DD3D_NMS_CLASS_PARALLEL=0 / dd3d_set_conv_policy("nms_class_parallel", 0): single-CTA kernel
-        const char* e = getenv("DD3D_NMS_CLASS_PARALLEL");
-        g_class_parallel = (e && atoi(e) == 0) ? 0 : 1;
-    }
-    if (g_class_parallel && p.scratch != nullptr && p.do_nms && p.nms_thresh > 0.f && p.num_classes >= 1 && p.num_classes <= 255) {
+    if (p.class_parallel) {
         cudaError_t e = launch_pdl(nms_sort_kernel, dim3(kSortCtasPerImage, p.B), dim3(kSortThreads), smem_sort, stream, p);
         if (e == cudaSuccess) e = launch_pdl(nms_mask_kernel, dim3(kMaskCtasPerImage, p.B), dim3(kMaskThreads), 0, stream, p);
         if (e == cudaSuccess) e = launch_pdl(nms_scan_kernel, dim3(p.num_classes, p.B), dim3(kScanThreads), 0, stream, p);

@@ -24,6 +24,11 @@
 
 namespace dd3d {
 
+// Kernels a launch wrapper without a count of its own enqueues (launch_conv, the preprocess / stem / pool / relu / depthwise
+// wrappers, the resize, the sparse predictor, the tile lists, the one-CTA BEV NMS).  Multi-kernel wrappers name their count
+// next to their declaration (kDecodeSelectLaunches, kEseLaunches, kB3dGatherLaunches, nms_launches, ...).
+constexpr int kOneLaunch = 1;
+
 inline bool pdl_enabled() {
     static int on = -1;
     if (on < 0) {

@@ -39,6 +39,7 @@ cudaError_t launch_maxpool(const __nv_bfloat16* in, __nv_bfloat16* out, int B, i
                            int Ho, int Wo, int out_pitch, int ksize, int num_sms, cudaStream_t stream, int fp16 = 0);
 
 int ese_nsplit(int HW);
+constexpr int kEseLaunches = 3;  // either form: pool (or reduce), fc, scale
 // partial: [B][ese_nsplit(HW)][C] fp32 scratch, gate: [B][C] fp32 scratch.
 cudaError_t launch_ese(const __nv_bfloat16* x, int x_pitch, const float* fc_w, const float* fc_b,
                        const __nv_bfloat16* identity, int id_pitch, __nv_bfloat16* out, int out_pitch, float* partial,

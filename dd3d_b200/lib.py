@@ -118,7 +118,8 @@ SIGNATURES = {
     "dd3d_num_ops": (_I, [_P]),
     "dd3d_get_profile": (_I, [_P, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double),
                                C.POINTER(C.c_int32)]),
-    "dd3d_get_op_times": (_I, [_P, C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_double), _I]),
+    "dd3d_get_op_times": (_I, [_P, C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_double),
+                                  C.POINTER(C.c_int32), _I]),
     "dd3d_get_conv_info": (_I, [_P, C.POINTER(C.c_int32), _I]),
     "dd3d_get_tensor": (_I, [_P, C.c_char_p, C.POINTER(_P), C.POINTER(C.c_int32 * 6)]),
     "dd3d_op_conv2d": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _I, _I, _P]),

@@ -472,11 +472,13 @@ class DD3DB200(nn.Module):
         _lib.check(_lib.load().dd3d_get_profile(self._handle, ms, fl, by, ln), self._handle)
         return {n: dict(ms=ms[i], flops=fl[i], bytes=by[i], launches=ln[i]) for i, n in enumerate(self.PROFILE_CATEGORIES)}
 
-    def get_op_times(self, max_ops=1024):
-        """[(category, ms, algorithmic flops)] per engine op of the last profiled forward, in launch order."""
-        ms, cats, fl = (C.c_float * max_ops)(), (C.c_int32 * max_ops)(), (C.c_double * max_ops)()
-        n = _lib.check(_lib.load().dd3d_get_op_times(self._handle, ms, cats, fl, max_ops), self._handle)
-        return [(self.PROFILE_CATEGORIES[cats[i]], ms[i], fl[i]) for i in range(n)]
+    def get_op_times(self, max_ops=1024, with_op=False):
+        """[(category, ms, algorithmic flops)] per step of the last profiled forward, in launch order.  with_op: each entry
+        also carries the engine op the step ran (the index of get_conv_info), or -1 for the preprocess, tile-list, decode
+        and NMS steps."""
+        ms, cats, fl, ops = (C.c_float * max_ops)(), (C.c_int32 * max_ops)(), (C.c_double * max_ops)(), (C.c_int32 * max_ops)()
+        n = _lib.check(_lib.load().dd3d_get_op_times(self._handle, ms, cats, fl, ops, max_ops), self._handle)
+        return [(self.PROFILE_CATEGORIES[cats[i]], ms[i], fl[i]) + ((ops[i],) if with_op else ()) for i in range(n)]
 
     def get_conv_info(self, max_ops=1024):
         """Per engine op of the current plan, in launch order: None, or the conv's dict(taps, stride, cin, cout_pad, halo,

@@ -261,7 +261,8 @@ int dd3d_bev_nms_path(const dd3d_model_desc* h_desc);
 /* Process-wide kernel-selection policy for plans / operator calls made afterwards (tests, A/B measurements):
  * "op_fp16" = 1: the dd3d_op_* entry points below treat their 16-bit buffers as fp16 (default 0: bf16).
  * "nms_class_parallel" = 0: one CTA per image does the whole NMS instead of the multi-CTA path (rank sort, IoU bit matrix on
- * all SMs, one scan CTA per (class, image), finish; default 1; same kept set and order).
+ * all SMs, one scan CTA per (class, image), finish; default 1; same kept set and order).  A plan also reads it again when
+ * option "do_nms" changes.
  * "taps" = 0: 3x3 convs with <= 16 output channels use the per-tap kernels instead of the taps-in-N kernel (default 1).
  * "wstat" = 0: 3x3 layers whose whole weight tensor fits in shared memory next to the activation patches (64 -> 64 channels)
  * stream it per tile like every other layer instead of keeping it resident (default 1; bit-identical results either way).
@@ -272,7 +273,8 @@ int dd3d_bev_nms_path(const dd3d_model_desc* h_desc);
  * one (tile pair, 128-channel block) per SM, otherwise the 128-pixel tile and the N-split keep the machine filled; 1: wherever
  * eligible; 0 (or environment DD3D_CONV_PAIR=0): never.  Bit-identical results either way. */
 int dd3d_set_conv_policy(const char* name, int value);
-/* Number of kernel launches one dd3d_forward enqueues (for the bench's gpu_launches claim). */
+/* Number of kernel launches one dd3d_forward of the current plan enqueues (for the bench's gpu_launches claim): the sum over
+ * the steps the plan will launch (0 without a plan). */
 int dd3d_launches_per_forward(dd3d_handle h);
 
 /* Per-category device time of the LAST dd3d_forward issued with option "profile" = 1 (CUDA events recorded on the
@@ -281,12 +283,14 @@ int dd3d_launches_per_forward(dd3d_handle h);
  * depthwise 3x3 convs of the VoVNet -dw variants), 2 wgmma implicit-GEMM conv, 3 max-pool, 4 eSE, 5 relu and GroupNorm (the
  * elementwise passes over a map), 6 decode, 7 NMS. */
 int dd3d_get_profile(dd3d_handle h, double* h_ms, double* h_flops, double* h_bytes, int32_t* h_launches);
-/* Same events, per op in launch order (entry 0 = preprocess, then every engine op, then decode, NMS): device ms,
- * category and algorithmic FLOPs.  Returns the number of entries written (<= max_ops). */
-int dd3d_get_op_times(dd3d_handle h, float* h_ms, int32_t* h_cats, double* h_flops, int max_ops);
-/* Kernel choice of every engine op of the current plan, in launch order (entry i = entry i + 1 of dd3d_get_op_times): 8
- * int32 per op = {implicit-GEMM conv: 1 dense, 2 grouped block-diagonal mode; taps, stride, cin, padded cout, halo variant,
- * pair tile, block_n}, all 0 for other ops.  Returns the number of ops written (<= max_ops). */
+/* Same events, one entry per step in launch order: the preprocess, every engine op (with the sparse box2d / box3d towers,
+ * their tile lists in front of them), the decode, the NMS.  Per entry: device ms, category, algorithmic FLOPs and, when
+ * h_ops is not null, the engine op it timed (the index of dd3d_get_conv_info / dd3d_get_tensor "op<i>"), or -1 for the
+ * preprocess, tile-list, decode and NMS entries.  Returns the number of entries written (<= max_ops). */
+int dd3d_get_op_times(dd3d_handle h, float* h_ms, int32_t* h_cats, double* h_flops, int32_t* h_ops, int max_ops);
+/* Kernel choice of every engine op of the current plan, in op order (dd3d_get_op_times names the op of each of its
+ * entries): 8 int32 per op = {implicit-GEMM conv: 1 dense, 2 grouped block-diagonal mode; taps, stride, cin, padded cout,
+ * halo variant, pair tile, block_n}, all 0 for other ops.  Returns the number of ops written (<= max_ops). */
 int dd3d_get_conv_info(dd3d_handle h, int32_t* h_info, int max_ops);
 
 /* ---- GPU input pipeline (SURVEY.md 8f row 3) ------------------------------------------------------------------

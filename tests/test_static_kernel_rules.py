@@ -80,7 +80,7 @@ def _src(name):
         return f.read()
 
 
-def test_pdl_rule_in_the_sources():
+def test_pdl_rule_in_the_step_loop():
     pdl = _src("pdl.cuh")
     assert "g_pdl_scope_depth > 0" in pdl and "struct PdlScope" in pdl
     launched, defined = set(), {}
@@ -98,8 +98,10 @@ def test_pdl_rule_in_the_sources():
         assert k in defined, f"{k}: definition not found"
         assert defined[k].startswith("DD3D_PDL_PROLOGUE();"), f"{k} is launched programmatically but does not start with the prologue"
     eng = _src("engine.cu")
-    i_pre, i_scope, i_ops = eng.index('"preprocess");'), eng.index("PdlScope pdl_scope;"), eng.index("for (const Op& op : P.ops) {", eng.index("PdlScope pdl_scope;"))
-    assert i_pre < i_scope < i_ops, "the scope must open after the first kernel of the forward and before the op loop"
+    i_pre, i_scope, i_ops = eng.index('"preprocess");'), eng.index("pdl_scope.emplace();"), eng.index("case Step::OP:")
+    assert i_pre < i_scope < i_ops, "the scope must open right after the preprocess kernel, in its step"
+    steps = eng[eng.index("void Engine::plan_steps("):]
+    assert steps.index("add(Step::PREPROCESS") == steps.index("add("), "the preprocess must be the first step of the forward"
     assert eng.count("PdlScope") == 1 and "PdlScope" not in _src("capi.cu"), "operator-level entry points never open a PdlScope"
 
 

@@ -65,24 +65,23 @@ def main():
         for name, m in models.items():
             m.set_profile(True)
             m(inp)
-            t = m.get_op_times()
+            t = m.get_op_times(with_op=True)
             m.set_profile(False)
-            times[name].append([ms for _, ms, _ in t])
-            steps[name].append(sum(ms for _, ms, _ in t))
-            flops = [f for _, _, f in t]
+            times[name].append({op: ms for _, ms, _, op in t if op >= 0})
+            steps[name].append(sum(ms for _, ms, _, _ in t))
+            flops = {op: f for _, _, f, op in t if op >= 0}
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             m(inp)
             e1.record()
             torch.cuda.synchronize()
             walls[name].append(e0.elapsed_time(e1))
-    med = {n: [statistics.median(col) for col in zip(*times[n])] for n in modes}
+    med = {n: {op: statistics.median(r[op] for r in times[n]) for op in times[n][0]} for n in modes}
     rows, groups = [], {}
     for i, (c_old, c_new) in enumerate(zip(info["old"], info["pair"])):
         if c_old is None:
             continue
-        j = i + 1  # op-time entry 0 is the preprocess
-        a, b, f = med["old"][j], med["pair"][j], flops[j]
+        a, b, f = med["old"][i], med["pair"][i], flops[i]
         k = tag(c_old)
         rows.append(dict(op=i, shape=k, pair=int(c_new["pair"]), old_ms=a, new_ms=b, gflop=f / 1e9))
         g = groups.setdefault((k, int(c_new["pair"])), [0, 0.0, 0.0, 0.0])

@@ -76,11 +76,10 @@ def main():
         step()
         torch.cuda.synchronize()
         prof = model.get_profile()
-        ops = model.get_op_times()
+        ops = model.get_op_times(with_op=True)
         model.set_profile(False)
-        conv_info = model.get_conv_info()
-        # op entries: 0 = preprocess, 1.. = engine ops; the depthwise ops are the category-1 ops after stem_1 (engine op 0)
-        dw_ms = sum(t for i, (cat, t, _) in enumerate(ops) if cat == "stem_conv" and i >= 2 and i - 1 < len(conv_info))
+        # the depthwise ops are the category-1 engine ops after stem_1 (engine op 0)
+        dw_ms = sum(t for cat, t, _, op in ops if cat == "stem_conv" and op >= 1)
         dw_bytes = prof["stem_conv"]["bytes"] - _stem1_bytes(B, model)
         line = {"arch": arch, "name": VOVNET_SPECS[arch][0], "batch": B, "shape": [H, W], "dtype": args.dtype,
                 "images_per_s": B / (ms / 1e3), "ms_per_step": ms,
@@ -96,7 +95,7 @@ def main():
 
 
 def _stem1_bytes(B, model):
-    """Bytes dd3d_get_profile books for VoVNet stem_1 (engine.cu get_profile, Op::STEM): 8 B per input pixel, 2 B per output
+    """Bytes dd3d_get_profile books for VoVNet stem_1 (engine.cu Builder::stem): 8 B per input pixel, 2 B per output
     channel and pixel."""
     Hp, Wp = model._plan_key[1], model._plan_key[2]
     d = model.backbone.size_divisibility

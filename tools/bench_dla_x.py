@@ -78,16 +78,16 @@ def main():
         step()
         torch.cuda.synchronize()
         prof = model.get_profile()
-        ops = model.get_op_times()
+        ops = model.get_op_times(with_op=True)
         model.set_profile(False)
         conv_info = model.get_conv_info()
-        # op entries: 0 = preprocess, 1.. = engine ops (conv_info[i - 1])
+        by_op = {op: (t, fl) for _, t, fl, op in ops if op >= 0}
         g_ms = g_bytes = g_flops = 0.0
         per_cpg = {}
         for i, c in enumerate(conv_info):
             if c is None or not c["grouped"]:
                 continue
-            _, t, fl = ops[i + 1]
+            t, fl = by_op[i]
             o = model.get_tensor(f"op{i}")  # [B, Ho, Wo, C]
             nb = o.shape[0] * o.shape[1] * o.shape[2] * o.shape[3] * 2.0 * (1 + c["stride"] ** 2)  # input + output maps
             g_ms, g_bytes, g_flops = g_ms + t, g_bytes + nb, g_flops + fl

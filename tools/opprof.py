@@ -14,10 +14,10 @@ for _ in range(3): m(inp)
 m.set_profile(True)
 acc = None
 for _ in range(3):
-    m(inp); t = m.get_op_times()
-    acc = t if acc is None else [(a[0], a[1] + b[1], a[2]) for a, b in zip(acc, t)]
+    m(inp); t = m.get_op_times(with_op=True)
+    acc = t if acc is None else [(a[0], a[1] + b[1], a[2], a[3]) for a, b in zip(acc, t)]
 k = 0
-for i, (c, ms, fl) in enumerate(acc):
+for i, (c, ms, fl, _) in enumerate(acc):
     ms /= 3
     tf = fl / (ms * 1e-3) / 1e12 if ms > 0 and fl else 0
     if c == "conv_igemm":
