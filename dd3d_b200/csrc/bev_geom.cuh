@@ -155,6 +155,14 @@ __device__ void box_to_global(const Det& D, const float* iK, const float* Rw, co
     rect[4] = atan2f(fx, fy) * 57.29577951308232f;
 }
 
+// Rectangles whose bounding circles are apart (with a relative margin far above fp32 rounding) are disjoint: their IoU is
+// exactly 0 in the polygon clipper as well, so for iou_thresh >= 0 the pair never suppresses and needs no clipping.
+__device__ __forceinline__ bool circles_apart(const float* a, const float* b) {
+    const float ra = 0.5f * sqrtf(a[2] * a[2] + a[3] * a[3]), rb = 0.5f * sqrtf(b[2] * b[2] + b[3] * b[3]);
+    const float dx = a[0] - b[0], dy = a[1] - b[1], r = (ra + rb) * 1.001f + 1e-4f;
+    return dx * dx + dy * dy > r * r;
+}
+
 }  // namespace
 
 }  // namespace dd3d

@@ -261,14 +261,6 @@ __global__ void __launch_bounds__(kGbSortThreads) gbev_sort_kernel(const GbParam
     }
 }
 
-// Rectangles whose bounding circles are apart (with a relative margin far above fp32 rounding) are disjoint: their IoU is
-// exactly 0 in the polygon clipper as well, so for iou_thresh >= 0 the pair never suppresses and needs no clipping.
-__device__ __forceinline__ bool circles_apart(const float* a, const float* b) {
-    const float ra = 0.5f * sqrtf(a[2] * a[2] + a[3] * a[3]), rb = 0.5f * sqrtf(b[2] * b[2] + b[3] * b[3]);
-    const float dx = a[0] - b[0], dy = a[1] - b[1], r = (ra + rb) * 1.001f + 1e-4f;
-    return dx * dx + dy * dy > r * r;
-}
-
 __global__ void __launch_bounds__(kGbThreads) gbev_mask_kernel(const GbParams p) {
     DD3D_PDL_PROLOGUE();
     const int total = *p.total;

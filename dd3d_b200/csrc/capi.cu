@@ -894,6 +894,29 @@ int dd3d_op_tta_merge(const dd3d_det* d_dets, const int32_t* d_counts, const dd3
                        nullptr);
 }
 
+int dd3d_op_tta_merged_cap_large(int num_views, int cap) {
+    const int n = tta_merged_cap_large(num_views, cap);
+    return n < 0 ? DD3D_ERR_INVALID : n;
+}
+
+int64_t dd3d_op_tta_merge_large_scratch_bytes(int num_views, int cap) {
+    const size_t bytes = tta_large_scratch_bytes(num_views, cap);
+    return bytes ? static_cast<int64_t>(bytes) : DD3D_ERR_INVALID;
+}
+
+int dd3d_op_tta_merge_large(const dd3d_det* d_dets, const int32_t* d_counts, const dd3d_tta_view* h_views, int num_views,
+                            int cap, float nms_thresh, int do_nms, void* d_scratch, dd3d_det* d_out, int32_t* d_out_count,
+                            int32_t* d_flags, dd3d_stream stream) {
+    if (!d_dets || !d_counts || !h_views || !d_scratch || !d_out || !d_out_count || !d_flags ||
+        tta_merged_cap_large(num_views, cap) < 0)
+        return DD3D_ERR_INVALID;
+    return cuda_status(launch_tta_merge_large(reinterpret_cast<const Det*>(d_dets), d_counts,
+                                              reinterpret_cast<const TtaView*>(h_views), num_views, cap, nms_thresh,
+                                              do_nms, d_scratch, reinterpret_cast<Det*>(d_out), d_out_count, d_flags,
+                                              static_cast<cudaStream_t>(stream)),
+                       nullptr);
+}
+
 int dd3d_forward_resized(dd3d_handle h, const uint8_t* d_raw, int raw_h, int raw_w, const int32_t* h_raw_sizes,
                          const int32_t* h_new_sizes, const int32_t* h_flip, const float* h_intrinsics,
                          const int32_t* h_sizes, dd3d_det* d_out, int32_t* d_counts, dd3d_stream stream) {
@@ -947,6 +970,26 @@ int dd3d_op_group_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_vi
     return cuda_status(launch_group_bev_nms(reinterpret_cast<Det*>(d_dets), d_counts, d_view_K, num_views, d_poses,
                                             pose_mode, d_group, num_groups, max_group_images, d_global, d_scratch,
                                             d_flags, B, cap, iou_thresh, max_dets, static_cast<cudaStream_t>(stream)),
+                       nullptr);
+}
+
+int64_t dd3d_op_group_bev_nms_large_scratch_bytes(int B, int cap, int max_group_images) {
+    const size_t bytes = group_bev_nms_large_scratch_bytes(B, cap, max_group_images);
+    return bytes ? static_cast<int64_t>(bytes) : DD3D_ERR_INVALID;
+}
+
+int dd3d_op_group_bev_nms_large(dd3d_det* d_dets, int32_t* d_counts, const float* d_view_K, int num_views,
+                                const float* d_poses, int pose_mode, const int32_t* d_group, int num_groups,
+                                int max_group_images, float* d_global, void* d_scratch, int32_t* d_flags, int B, int cap,
+                                float iou_thresh, int max_dets, dd3d_stream stream) {
+    if (!d_dets || !d_counts || !d_view_K || !d_group || !d_scratch || !d_flags || num_views < 1 ||
+        group_bev_nms_large_scratch_bytes(B, cap, max_group_images) == 0 || num_groups < 1 || num_groups > B ||
+        (pose_mode != DD3D_POSE_GLOBAL && pose_mode != DD3D_POSE_CAMERA) || (pose_mode == DD3D_POSE_GLOBAL && !d_poses))
+        return DD3D_ERR_INVALID;
+    return cuda_status(launch_group_bev_nms_large(reinterpret_cast<Det*>(d_dets), d_counts, d_view_K, num_views, d_poses,
+                                                  pose_mode, d_group, num_groups, max_group_images, d_global, d_scratch,
+                                                  d_flags, B, cap, iou_thresh, max_dets,
+                                                  static_cast<cudaStream_t>(stream)),
                        nullptr);
 }
 

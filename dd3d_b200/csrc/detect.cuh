@@ -47,6 +47,17 @@ static_assert(sizeof(Det) == 96, "Det must be 24 words");
 
 __device__ __forceinline__ float sigmoidf(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// Axis-aligned IoU of (x1, y1, x2, y2) boxes exactly as torchvision computes it: the 2-D NMS kernels (nms.cu, tta_large.cu)
+__device__ __forceinline__ float iou_tv(const float4 a, const float4 b) {
+    const float area_a = __fmul_rn(__fsub_rn(a.z, a.x), __fsub_rn(a.w, a.y));
+    const float area_b = __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y));
+    const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y);
+    const float xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
+    const float w = fmaxf(0.f, __fsub_rn(xx2, xx1)), h = fmaxf(0.f, __fsub_rn(yy2, yy1));
+    const float inter = __fmul_rn(w, h);
+    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
+}
+
 // The class-only threshold: some class column c < C of a pixel's logits (a 16-byte aligned cls map row) has
 // sigmoid(logit) > thresh.  The decode reads a pixel's box2d map row only when this holds: with THRESH_WITH_CTR the
 // thresholded score is RN(sigmoid(cls) * sigmoid(ctr)) <= sigmoid(cls), since sigmoid(ctr) <= 1 (or NaN) and rounding is
@@ -173,6 +184,15 @@ cudaError_t launch_tta_merge(const Det* dets, const int32_t* counts, const TtaVi
                              float nms_thresh, int do_nms, void* scratch, Det* out, int32_t* out_count, int32_t* flags,
                              cudaStream_t stream);
 
+// The same merge for large sets (tta_large.cu): no kTtaMergedMax clamp, A * cap merged slots (cap <= kLevels *
+// kMaxPreNmsTopk, so up to 92 000 per image), multi-CTA transform, blocked class-aware NMS with O(A * cap) scratch; -1 /
+// 0 bytes / cudaErrorInvalidValue for arguments out of range.
+int tta_merged_cap_large(int A, int cap);
+size_t tta_large_scratch_bytes(int A, int cap);
+cudaError_t launch_tta_merge_large(const Det* dets, const int32_t* counts, const TtaView* h_views, int A, int cap,
+                                   float nms_thresh, int do_nms, void* scratch, Det* out, int32_t* out_count,
+                                   int32_t* flags, cudaStream_t stream);
+
 // NuscenesDD3D sample aggregation: BEV rotated NMS jointly over the images of each sample group, then the cap on the
 // survivors of the call; in place; global: [B][cap][10] pred_boxes3d_global rows; cap <= 256.
 size_t sample_aggregate_scratch_bytes(int B, int cap);
@@ -198,5 +218,13 @@ cudaError_t launch_group_bev_nms(Det* dets, int32_t* counts, const float* view_K
                                  int pose_mode, const int32_t* group, int num_groups, int max_group_images, float* global,
                                  void* scratch, int32_t* flags, int B, int cap, float thr, int max_dets,
                                  cudaStream_t stream);
+
+// launch_group_bev_nms on the blocked NMS of tta_large.cu: the same arguments, outputs and flags for cap <= 92 000 slots
+// per image, scratch O(B * cap) (0 bytes: arguments out of range).
+size_t group_bev_nms_large_scratch_bytes(int B, int cap, int max_group_images);
+cudaError_t launch_group_bev_nms_large(Det* dets, int32_t* counts, const float* view_K, int num_views, const float* poses,
+                                       int pose_mode, const int32_t* group, int num_groups, int max_group_images,
+                                       float* global, void* scratch, int32_t* flags, int B, int cap, float thr,
+                                       int max_dets, cudaStream_t stream);
 
 }  // namespace dd3d

@@ -23,16 +23,6 @@ namespace {
 constexpr int kNmsThreads = 1024;
 constexpr int kMaxCand = kNmsSortCap;  // bitonic sort capacity (>= L * topk)
 
-__device__ __forceinline__ float iou_tv(const float4 a, const float4 b) {
-    const float area_a = __fmul_rn(__fsub_rn(a.z, a.x), __fsub_rn(a.w, a.y));
-    const float area_b = __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y));
-    const float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y);
-    const float xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-    const float w = fmaxf(0.f, __fsub_rn(xx2, xx1)), h = fmaxf(0.f, __fsub_rn(yy2, yy1));
-    const float inter = __fmul_rn(w, h);
-    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
-}
-
 // ascending bitonic sort of n2 (power of two) 64-bit keys with a 16-bit payload, in shared memory
 __device__ void bitonic_sort(uint64_t* key, uint16_t* val, int n2) {
     for (int k = 2; k <= n2; k <<= 1) {

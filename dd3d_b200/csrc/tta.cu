@@ -11,7 +11,7 @@
 //               Boxes3D.from_vectors (tridet/structures/boxes3d.py:176-216) re-projects tvec to (proj_ctr, depth) --
 // then concatenated in view order and reduced by ONE class-aware NMS on scores_3d (detectron2 batched_nms), output in
 // descending scores_3d order (merged_instances[keep]).
-#include "detect.cuh"
+#include "tta_view.cuh"
 
 #include <string.h>
 
@@ -30,21 +30,6 @@ struct TtaParams {
     int32_t* flags;          // bit 4: more merged detections than merged_cap
     int A, cap, merged_cap;
 };
-
-__device__ void inv3(const float* K, float* iK) {  // adjugate in double like decode.cu
-    const double a = K[0], b = K[1], c = K[2], d = K[3], e = K[4], f = K[5], g = K[6], h = K[7], i = K[8];
-    const double A = e * i - f * h, B = -(d * i - f * g), C = d * h - e * g;
-    const double r = 1.0 / (a * A + b * B + c * C);
-    iK[0] = static_cast<float>(A * r);
-    iK[1] = static_cast<float>(-(b * i - c * h) * r);
-    iK[2] = static_cast<float>((b * f - c * e) * r);
-    iK[3] = static_cast<float>(B * r);
-    iK[4] = static_cast<float>((a * i - c * g) * r);
-    iK[5] = static_cast<float>(-(a * f - c * d) * r);
-    iK[6] = static_cast<float>(C * r);
-    iK[7] = static_cast<float>(-(a * h - b * g) * r);
-    iK[8] = static_cast<float>((a * e - b * d) * r);
-}
 
 __global__ void __launch_bounds__(kTtaThreads) tta_merge_kernel(const TtaParams p) {
     __shared__ int s_off[kTtaMaxViews + 1];
@@ -67,49 +52,10 @@ __global__ void __launch_bounds__(kTtaThreads) tta_merge_kernel(const TtaParams 
         const TtaView& V = p.view[a];
         const int n = s_off[a + 1] - s_off[a];
         float iK[9];
-        inv3(V.K_view, iK);
+        tta_inv3(V.K_view, iK);
         for (int i = threadIdx.x; i < n; i += blockDim.x) {
             Det d = p.dets[static_cast<size_t>(a) * p.cap + i];
-            // ---- 2-D box: inverse transforms in reverse order, each in fp32 (fvcore apply_box = 4 corners -> min / max)
-            float x1 = d.box[0], y1 = d.box[1], x2 = d.box[2], y2 = d.box[3];
-            if (V.flip) {
-                const float nx1 = V.view_w - x2, nx2 = V.view_w - x1;
-                x1 = nx1;
-                x2 = nx2;
-            }
-#pragma unroll
-            for (int s = 0; s < 2; ++s) {  // un-resize view -> input, then input -> original
-                x1 *= V.inv_sx[s];
-                x2 *= V.inv_sx[s];
-                y1 *= V.inv_sy[s];
-                y2 *= V.inv_sy[s];
-            }
-            d.box[0] = fminf(x1, x2);
-            d.box[1] = fminf(y1, y2);
-            d.box[2] = fmaxf(x1, x2);
-            d.box[3] = fmaxf(y1, y2);
-            // ---- 3-D box: camera-frame translation of the view (Boxes3D.tvec), mirror if flipped
-            const float u = d.proj_ctr[0], v = d.proj_ctr[1];
-            float tx = (iK[0] * u + iK[1] * v + iK[2]) * d.depth;
-            const float ty = (iK[3] * u + iK[4] * v + iK[5]) * d.depth;
-            const float tz = (iK[6] * u + iK[7] * v + iK[8]) * d.depth;
-            if (V.flip) {
-                const float q0 = d.quat[0], q1 = d.quat[1], q2 = d.quat[2], q3 = d.quat[3];
-                d.quat[0] = q3;
-                d.quat[1] = -q2;
-                d.quat[2] = -q1;
-                d.quat[3] = q0;
-                tx = -tx;
-            }
-            // ---- Boxes3D.from_vectors with the recovered original intrinsics: proj_ctr = (K t)[:2] / (K t)[2], depth = t.z
-            const float* K = V.K_orig;
-            const float px = K[0] * tx + K[1] * ty + K[2] * tz;
-            const float py = K[3] * tx + K[4] * ty + K[5] * tz;
-            const float pz = K[6] * tx + K[7] * ty + K[8] * tz;
-            d.proj_ctr[0] = px / pz;
-            d.proj_ctr[1] = py / pz;
-            d.depth = tz;
-            d.level = a;  // the view the detection came from (the merged Instances carry no fpn_levels)
+            tta_invert_det(d, V, iK, a);
             p.cand[s_off[a] + i] = d;
         }
     }

@@ -155,11 +155,16 @@ SIGNATURES = {
     "dd3d_op_tta_merged_cap": (_I, [_I, _I]),
     "dd3d_op_tta_merge_scratch_bytes": (_I64, [_I, _I]),
     "dd3d_op_tta_merge": (_I, [_P, _P, _P, _I, _I, C.c_float, _I, _P, _P, _P, _P, _P]),
+    "dd3d_op_tta_merged_cap_large": (_I, [_I, _I]),
+    "dd3d_op_tta_merge_large_scratch_bytes": (_I64, [_I, _I]),
+    "dd3d_op_tta_merge_large": (_I, [_P, _P, _P, _I, _I, C.c_float, _I, _P, _P, _P, _P, _P]),
     "dd3d_op_resize_preprocess": (_I, [_P, _I, _I, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P]),
     "dd3d_op_sample_aggregate_scratch_bytes": (_I64, [_I, _I]),
     "dd3d_op_sample_aggregate": (_I, [_P, _P, _P, _P, _P, _I, _P, _P, _P, _I, _I, C.c_float, _I, _P]),
     "dd3d_op_group_bev_nms_scratch_bytes": (_I64, [_I, _I, _I]),
     "dd3d_op_group_bev_nms": (_I, [_P, _P, _P, _I, _P, _I, _P, _I, _I, _P, _P, _P, _I, _I, C.c_float, _I, _P]),
+    "dd3d_op_group_bev_nms_large_scratch_bytes": (_I64, [_I, _I, _I]),
+    "dd3d_op_group_bev_nms_large": (_I, [_P, _P, _P, _I, _P, _I, _P, _I, _I, _P, _P, _P, _I, _I, C.c_float, _I, _P]),
     "dd3d_op_detect_scratch_bytes": (_I64, [_I, _I]),
     "dd3d_op_detect": (_I, [C.POINTER(ModelDesc), _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P),
                             C.POINTER(_P), C.POINTER(_P), _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -18,6 +18,9 @@ from . import lib as _lib
 from .meta_arch import DD3DB200, NuscenesDD3DB200, group_indices
 from .structures import Boxes, Boxes3D, GenericBoxes3D, Instances
 
+TTA_MERGED_MAX = 1024  # merged detections per image dd3d_op_tta_merge holds (kTtaMergedMax, csrc/detect.cuh)
+BEV_NMS_MAX = 256      # score-sorted boxes per image dd3d_op_bev_nms holds (kBevNmsMax)
+
 
 def build_views(image_hw, orig_hw, K_input, min_sizes, max_size, flip):
     """DatasetMapperTTA.__call__ (test_time_augmentation.py:50-87) + the inverse bookkeeping of
@@ -75,14 +78,48 @@ class _DeviceTTA(nn.Module):
 
     def _do_bev_nms(self):
         """`not model.only_box2d and model.do_bev_nms` (core.py:137, nuscenes_dd3d_tta.py), read at call time like the
-        reference.  The BEV kernels expect score-sorted sets: the engine's rule of DD3DB200._sync_options."""
+        reference."""
         model = self.model
-        bev = bool(model.do_bev_nms) and not model.only_box2d
-        if bev and not model.do_nms:
-            raise NotImplementedError("DO_BEV_NMS without DO_NMS: the BEV kernels expect the score-sorted output of the 2-D NMS")
-        return bev
+        return bool(model.do_bev_nms) and not model.only_box2d
 
-    def _merge_image(self, x, out, n_out, bev, stream):
+    def per_view_bound(self):
+        """Detections one view can contribute: POST_NMS_TOPK after the 2-D NMS, else every 5 * PRE_NMS_TOPK candidate."""
+        inf = self.cfg.DD3D.FCOS2D.INFERENCE
+        if self.model.do_nms and inf.POST_NMS_TOPK > 0:
+            return int(inf.POST_NMS_TOPK)
+        return 5 * int(inf.PRE_NMS_TOPK)
+
+    def large_path(self):
+        """True when the merged sets need the large-set ops (csrc/tta_large.cu): more merged detections than the
+        dd3d_op_tta_merge slots (TTA_MERGED_MAX), or DO_BEV_NMS without DO_NMS (unsorted views of up to 5 * PRE_NMS_TOPK
+        boxes).  Read from the config and the model's switches only; the shipped configurations keep the one-CTA ops."""
+        bev_alone = self._do_bev_nms() and not self.model.do_nms
+        return self.num_views * self.per_view_bound() > TTA_MERGED_MAX or bev_alone
+
+    def _fit_out_cap(self):
+        """Without the 2-D NMS (or its top-k) every view may return 5 * PRE_NMS_TOPK candidates: grow the engine's output
+        buffer to that (the rule of DD3DB200._sync_options) without touching its other options, so the plans stay."""
+        model, inf = self.model, self.cfg.DD3D.FCOS2D.INFERENCE
+        need = 5 * inf.PRE_NMS_TOPK if (not model.do_nms or inf.POST_NMS_TOPK <= 0) else 0
+        if need > model._desc.out_cap:
+            model._release()
+            model._desc.out_cap = need
+
+    def _merge_mode(self, bev, large):
+        """do_nms of the merge.  Without the 2-D NMS the reference's merged BEV NMS returns its survivors in descending
+        scores_3d order (merged_instances[keep], keep from batched_nms_rotated); the BEV ops keep the order of their input,
+        so the large merge then sorts the concatenation by scores_3d (mode 2, ties in view order)."""
+        if large and bev and self.merged_bev_nms_in_inference and not self.model.do_nms:
+            return 2
+        return int(self.model.do_nms)
+
+    def _merged_cap(self, large):
+        L, cap = _lib.load(), self.model._desc.out_cap
+        if large:
+            return int(_lib.check(L.dd3d_op_tta_merged_cap_large(self.num_views, cap)))
+        return int(L.dd3d_op_tta_merged_cap(self.num_views, cap))
+
+    def _merge_image(self, x, out, n_out, bev, stream, large=False):
         """Runs the views of one image and merges them into `out` [merged_cap][DET_WORDS] / `n_out` [1] (device, no sync).
         Returns (original (h, w), views)."""
         model, L = self.model, _lib.load()
@@ -128,30 +165,43 @@ class _DeviceTTA(nn.Module):
             if bev:
                 d_K, d_sizes = K.to(device, non_blocking=True), sizes4.to(device, non_blocking=True)
                 d_pose = pose.expand(B, 7).contiguous()
+                if large and not (model.do_nms and 0 < self.cfg.DD3D.FCOS2D.INFERENCE.POST_NMS_TOPK <= BEV_NMS_MAX):
+                    # unsorted views (DO_NMS off) or more than the one-CTA kernel's boxes: the multi-CTA image-mode op
+                    bev_scratch = torch.empty(int(_lib.check(L.dd3d_op_bev_nms_large_scratch_bytes(B, cap))),
+                                              dtype=torch.uint8, device=device)
+                    _lib.check(
+                        L.dd3d_op_bev_nms_large(C.c_void_p(dets[a0].data_ptr()), C.c_void_p(counts[a0:].data_ptr()),
+                                                C.c_void_p(d_K.data_ptr()), C.c_void_p(d_pose.data_ptr()),
+                                                C.c_void_p(d_sizes.data_ptr()), C.c_void_p(bev_scratch.data_ptr()),
+                                                C.c_void_p(self._flags.data_ptr()), B, cap,
+                                                float(model.bev_nms_iou_thresh), 0, C.c_void_p(stream)), model._handle)
+                    continue
                 _lib.check(
                     L.dd3d_op_bev_nms(C.c_void_p(dets[a0].data_ptr()), C.c_void_p(counts[a0:].data_ptr()),
                                       C.c_void_p(d_K.data_ptr()), C.c_void_p(d_pose.data_ptr()),
                                       C.c_void_p(d_sizes.data_ptr()), C.c_void_p(self._flags.data_ptr()), B, cap,
                                       float(model.bev_nms_iou_thresh), 0, C.c_void_p(stream)), model._handle)
-        scratch = torch.empty(int(L.dd3d_op_tta_merge_scratch_bytes(A, cap)), dtype=torch.uint8, device=device)
         varr = (_lib.TtaView * A)(*[v[3] for v in views])
+        merge_scratch_bytes, merge = ((L.dd3d_op_tta_merge_large_scratch_bytes, L.dd3d_op_tta_merge_large) if large else
+                                      (L.dd3d_op_tta_merge_scratch_bytes, L.dd3d_op_tta_merge))
+        scratch = torch.empty(int(_lib.check(merge_scratch_bytes(A, cap))), dtype=torch.uint8, device=device)
         _lib.check(
-            L.dd3d_op_tta_merge(C.c_void_p(dets.data_ptr()), C.c_void_p(counts.data_ptr()), varr, A, cap,
-                                float(self.nms_thresh), int(model.do_nms), C.c_void_p(scratch.data_ptr()),
-                                C.c_void_p(out.data_ptr()), C.c_void_p(n_out.data_ptr()),
-                                C.c_void_p(self._flags.data_ptr()), C.c_void_p(stream)), model._handle)
+            merge(C.c_void_p(dets.data_ptr()), C.c_void_p(counts.data_ptr()), varr, A, cap, float(self.nms_thresh),
+                  self._merge_mode(bev, large), C.c_void_p(scratch.data_ptr()), C.c_void_p(out.data_ptr()),
+                  C.c_void_p(n_out.data_ptr()), C.c_void_p(self._flags.data_ptr()), C.c_void_p(stream)), model._handle)
         return orig, views
 
     def _group_bev_nms(self, out, counts, view_K, pose_mode, d_group, num_groups, group_images, d_poses=None,
-                       d_global=None, max_dets=0, stream=None):
-        """dd3d_op_group_bev_nms on out [B][merged_cap] / counts [B] (device, in place, no sync); groups of at most
-        `group_images` images, which sizes the IoU bit matrix."""
+                       d_global=None, max_dets=0, stream=None, large=False):
+        """dd3d_op_group_bev_nms (large: dd3d_op_group_bev_nms_large) on out [B][merged_cap] / counts [B] (device, in
+        place, no sync); groups of at most `group_images` images, which sizes the IoU bit matrix of the first."""
         L = _lib.load()
         B, mcap = int(out.shape[0]), int(out.shape[1])
-        scratch = torch.empty(int(_lib.check(L.dd3d_op_group_bev_nms_scratch_bytes(B, mcap, group_images))),
-                              dtype=torch.uint8, device=out.device)
+        scratch_bytes, op = ((L.dd3d_op_group_bev_nms_large_scratch_bytes, L.dd3d_op_group_bev_nms_large) if large else
+                             (L.dd3d_op_group_bev_nms_scratch_bytes, L.dd3d_op_group_bev_nms))
+        scratch = torch.empty(int(_lib.check(scratch_bytes(B, mcap, group_images))), dtype=torch.uint8, device=out.device)
         _lib.check(
-            L.dd3d_op_group_bev_nms(C.c_void_p(out.data_ptr()), C.c_void_p(counts.data_ptr()), C.c_void_p(view_K.data_ptr()),
+            op(C.c_void_p(out.data_ptr()), C.c_void_p(counts.data_ptr()), C.c_void_p(view_K.data_ptr()),
                                     int(view_K.shape[1]), C.c_void_p(d_poses.data_ptr()) if d_poses is not None else None,
                                     pose_mode, C.c_void_p(d_group.data_ptr()), num_groups, group_images,
                                     C.c_void_p(d_global.data_ptr()) if d_global is not None else None,
@@ -195,21 +245,31 @@ class DD3DB200WithTTA(_DeviceTTA):
 
     @torch.no_grad()
     def _inference_one_image(self, x):
-        model, L = self.model, _lib.load()
+        model = self.model
         device = model.device
         bev = self._do_bev_nms()
+        large = self.large_path()
+        if large:
+            self._fit_out_cap()
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            mcap = int(L.dd3d_op_tta_merged_cap(self.num_views, model._desc.out_cap))
+            mcap = self._merged_cap(large)
             out = torch.empty((1, mcap, _lib.DET_WORDS), dtype=torch.float32, device=device)
-            n_out = torch.zeros(1, dtype=torch.int32, device=device)
+            n_out = torch.zeros(2 if large else 1, dtype=torch.int32, device=device)  # large: [count, overflow word]
             self._flags = torch.zeros(1, dtype=torch.int32, device=device)
-            orig, views = self._merge_image(x, out[0], n_out, bev, stream)
+            # the large path folds the engine's overflow word of every view forward into the call's word
+            self._engine_flags = torch.zeros(1, dtype=torch.int32, device=device) if large else None
+            orig, views = self._merge_image(x, out[0], n_out[:1], bev, stream, large)
             if bev and self.merged_bev_nms_in_inference:  # bev_nms(merged_instances.pred_boxes3d, ...), camera frame
                 view_K = self._view_K(views).unsqueeze(0).to(device, non_blocking=True)
                 group = torch.zeros(1, dtype=torch.int32).to(device, non_blocking=True)
-                self._group_bev_nms(out, n_out, view_K, _lib.POSE_CAMERA, group, 1, 1, stream=stream)
-            n = int(n_out.item())  # the only synchronisation
+                self._group_bev_nms(out, n_out[:1], view_K, _lib.POSE_CAMERA, group, 1, 1, stream=stream, large=large)
+            if large:
+                n_out[1:] = self._flags
+                n, flags = n_out.tolist()  # the only synchronisation: the count and the overflow word
+                model._check_flags(flags)
+            else:
+                n = int(n_out.item())  # the only synchronisation
         d, di = out[0, :n], out[0].view(torch.int32)[:n]
         inv_K = self._inv_K(views, device)
         inst = Instances(orig)
@@ -255,17 +315,20 @@ class NuscenesDD3DB200WithTTA(_DeviceTTA):
             raise ValueError(f"NuscenesDD3DB200WithTTA: at most {self.MAX_IMAGES} images per call, got {B}")
         poses = model._gather_poses([{"pose": x["pose"]} for x in batched_inputs])
         bev = self._do_bev_nms()
+        large = self.large_path()
+        if large:
+            self._fit_out_cap()
         device = model.device
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            mcap = int(L.dd3d_op_tta_merged_cap(self.num_views, model._desc.out_cap))
+            mcap = self._merged_cap(large)
             out = torch.empty((B, mcap, _lib.DET_WORDS), dtype=torch.float32, device=device)
             counts = torch.zeros((B + 1, ), dtype=torch.int32, device=device)  # [B] counts + overflow word
             self._flags = torch.zeros(1, dtype=torch.int32, device=device)
             self._engine_flags = torch.zeros(1, dtype=torch.int32, device=device)
             origs, all_views = [], []
             for b, x in enumerate(batched_inputs):
-                orig, views = self._merge_image(x, out[b], counts[b:b + 1], bev, stream)
+                orig, views = self._merge_image(x, out[b], counts[b:b + 1], bev, stream, large)
                 origs.append(orig)
                 all_views.append(views)
             # nuscenes_sample_aggregate concatenates the Instances of the call: detectron2's Instances.cat asserts one
@@ -274,14 +337,15 @@ class NuscenesDD3DB200WithTTA(_DeviceTTA):
             view_K = torch.stack([self._view_K(v) for v in all_views]).to(device, non_blocking=True)
             if bev and self.merged_bev_nms_in_inference:  # per image: group = image, camera-frame pose, no cap
                 self._group_bev_nms(out, counts, view_K, _lib.POSE_CAMERA,
-                                    torch.arange(B, dtype=torch.int32).to(device, non_blocking=True), B, 1, stream=stream)
+                                    torch.arange(B, dtype=torch.int32).to(device, non_blocking=True), B, 1, stream=stream,
+                                    large=large)
             glob = None
             if model.sample_aggregate_in_inference:
                 glob = torch.zeros((B, mcap, 10), dtype=torch.float32, device=device)
                 self._group_bev_nms(out, counts, view_K, _lib.POSE_GLOBAL,
                                     torch.tensor(groups, dtype=torch.int32).to(device, non_blocking=True), max(groups) + 1,
                                     model.num_images_per_sample, d_poses=poses.to(device, non_blocking=True), d_global=glob,
-                                    max_dets=int(model.max_num_dets_per_sample or 0), stream=stream)
+                                    max_dets=int(model.max_num_dets_per_sample or 0), stream=stream, large=large)
             counts[B:] |= self._flags
             host = counts.cpu()  # the only synchronisation: B counts + the overflow word
         self._last_flags = int(host[-1])

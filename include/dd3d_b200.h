@@ -502,6 +502,20 @@ int64_t dd3d_op_tta_merge_scratch_bytes(int num_views, int cap);
 int dd3d_op_tta_merge(const dd3d_det* d_dets, const int32_t* d_counts, const dd3d_tta_view* h_views, int num_views, int cap,
                       float nms_thresh, int do_nms, void* d_scratch, dd3d_det* d_out, int32_t* d_out_count,
                       int32_t* d_flags, dd3d_stream stream);
+/* dd3d_op_tta_merge for merged sets beyond its 1024 slots: the same arguments, transforms and output contract (descending
+ * scores_3d after the class-aware NMS; do_nms = 0: the plain concatenation in view order; `level` = view index) with
+ * dd3d_op_tta_merged_cap_large(num_views, cap) = num_views * cap slots in d_out, cap <= 5 * 1150 per view (so up to
+ * 16 * 5750 = 92 000 per image).  Equal scores_3d are ordered by the detection's `index`, then by view order.  The NMS is
+ * a blocked greedy pass per class on all SMs (csrc/tta_large.cu); d_scratch: dd3d_op_tta_merge_large_scratch_bytes bytes,
+ * any content, linear in num_views * cap.  Arguments out of range return DD3D_ERR_INVALID before any launch; d_flags bit 4
+ * (16): a view count above cap.  do_nms = 2 (this operator only): no NMS, the concatenation sorted by scores_3d descending
+ * with ties in view order -- the order of bev_nms's keep when the merged BEV NMS follows without the 2-D NMS
+ * (test_time_augmentation.py:172-181): dd3d_op_group_bev_nms(_large) keeps the order of its input. */
+int dd3d_op_tta_merged_cap_large(int num_views, int cap);
+int64_t dd3d_op_tta_merge_large_scratch_bytes(int num_views, int cap);
+int dd3d_op_tta_merge_large(const dd3d_det* d_dets, const int32_t* d_counts, const dd3d_tta_view* h_views, int num_views,
+                            int cap, float nms_thresh, int do_nms, void* d_scratch, dd3d_det* d_out, int32_t* d_out_count,
+                            int32_t* d_flags, dd3d_stream stream);
 /* NuscenesDD3D sample aggregation (nuscenes_dd3d.py:449-463 -> postprocessing.py:58-108 nuscenes_sample_aggregate with
  * get_group_idxs groups, :111-129): BEV rotated NMS (scores_3d order, class aware) jointly over the images that share a
  * sample group, then -- like the reference's keep[:max_num_dets_per_sample] on the concatenation of the whole call -- only
@@ -535,6 +549,16 @@ int dd3d_op_group_bev_nms(dd3d_det* d_dets, int32_t* d_counts, const float* d_vi
                           int pose_mode, const int32_t* d_group, int num_groups, int max_group_images, float* d_global,
                           void* d_scratch, int32_t* d_flags, int B, int cap, float iou_thresh, int max_dets,
                           dd3d_stream stream);
+/* dd3d_op_group_bev_nms for merged sets beyond its limits: the same arguments, modes, survivors, order, d_global rows and
+ * flags (bit 5, 32) for B <= 256 images of cap <= 92 000 slots and groups of up to max_group_images <= 16 images, on the
+ * blocked NMS of csrc/tta_large.cu.  d_scratch: dd3d_op_group_bev_nms_large_scratch_bytes(B, cap, max_group_images)
+ * bytes, any content, linear in B * cap (no IoU bit matrix).  Arguments out of range return DD3D_ERR_INVALID before any
+ * launch. */
+int64_t dd3d_op_group_bev_nms_large_scratch_bytes(int B, int cap, int max_group_images);
+int dd3d_op_group_bev_nms_large(dd3d_det* d_dets, int32_t* d_counts, const float* d_view_K, int num_views,
+                                const float* d_poses, int pose_mode, const int32_t* d_group, int num_groups,
+                                int max_group_images, float* d_global, void* d_scratch, int32_t* d_flags, int B, int cap,
+                                float iou_thresh, int max_dets, dd3d_stream stream);
 /* decode + NMS on caller-provided head maps (layout documented in csrc/detect.cuh). */
 /* dd3d_op_detect_scratch_bytes sizes the NMS scratch for DD3D_MAX_CLASSES classes (dd3d_op_detect / _flags take at most that
  * many); dd3d_op_detect_c takes up to DD3D_MAX_NUM_CLASSES with dd3d_op_detect_c_scratch_bytes(B, pre_nms_topk, num_classes). */
