@@ -190,7 +190,8 @@ def param_specs(cfg):
         _conv(specs, "backbone.top_block.p7", F, F, 3, bias=True, role="linear")
 
     C = cfg.DD3D.NUM_CLASSES
-    L = 5
+    L = len(in_feature_levels(cfg))  # num_levels = len(in_features): fcos2d.py:36, fcos3d.py:60
+    ND = len(cfg.DD3D.FCOS3D.MEAN_DEPTH_PER_LEVEL)  # scales_depth / offsets_depth: one per entry (fcos3d.py:136-139)
     f2, f3 = cfg.DD3D.FCOS2D, cfg.DD3D.FCOS3D
     box3d_on = bool(cfg.MODEL.BOX3D_ON)  # core.py:34-40: no FCOS3D head at all when off
     # fcos2d.py:46-91, fcos3d.py:75-112: NUM_*_CONVS x Conv2d(bias = no norm, norm); BN / FrozenBN one per level
@@ -216,20 +217,22 @@ def param_specs(cfg):
     if box3d_on:
         C3 = 1 if f3.CLASS_AGNOSTIC_BOX3D else C          # fcos3d.py:103
         NL = L if f3.PER_LEVEL_PREDICTORS else 1           # fcos3d.py:104
-        specs["fcos3d_head.mean_depth_per_level"] = ((L, ), "buffer")
-        specs["fcos3d_head.std_depth_per_level"] = ((L, ), "buffer")
+        specs["fcos3d_head.mean_depth_per_level"] = ((ND, ), "buffer")
+        specs["fcos3d_head.std_depth_per_level"] = ((ND, ), "buffer")
         for name, mult, role, bias in (("quat", 4, "quat", True), ("ctr", 2, "ctr", True),
                                        ("depth", 1, "depth", not f3.USE_SCALE),  # fcos3d.py:116
                                        ("size", 3, "size", True), ("conf", 1, "conf", True)):
             for li in range(NL):
                 _conv(specs, f"fcos3d_head.box3d_{name}.{li}", mult * C3, F, 3, bias=bias, role=role)
         if f3.USE_SCALE:  # fcos3d.py:128-139
-            for l in range(L):
-                specs[f"fcos3d_head.scales_proj_ctr.{l}.scale"] = ((1, ), "scalar:ctr")
-                specs[f"fcos3d_head.scales_size.{l}.scale"] = ((1, ), "scalar:one")
-                specs[f"fcos3d_head.scales_conf.{l}.scale"] = ((1, ), "scalar:one")
-                specs[f"fcos3d_head.scales_depth.{l}.scale"] = ((1, ), "scalar:depth")
-                specs[f"fcos3d_head.offsets_depth.{l}.bias"] = ((1, ), "scalar:depth_offset")
+            for l in range(max(L, ND)):
+                if l < L:
+                    specs[f"fcos3d_head.scales_proj_ctr.{l}.scale"] = ((1, ), "scalar:ctr")
+                    specs[f"fcos3d_head.scales_size.{l}.scale"] = ((1, ), "scalar:one")
+                    specs[f"fcos3d_head.scales_conf.{l}.scale"] = ((1, ), "scalar:one")
+                if l < ND:
+                    specs[f"fcos3d_head.scales_depth.{l}.scale"] = ((1, ), "scalar:depth")
+                    specs[f"fcos3d_head.offsets_depth.{l}.bias"] = ((1, ), "scalar:depth_offset")
     if is_nuscenes_arch(cfg):  # nuscenes_dd3d.py:311-312 (appended last: the synthetic generator stream of the rest is unchanged)
         _conv(specs, "attr_logits", MAX_NUM_ATTRIBUTES, F, 3, bias=True, role="attr")
         _conv(specs, "speed", 1, F, 3, bias=True, role="speed")
@@ -294,8 +297,34 @@ def backbone_norm(cfg):
     return norm
 
 
+def fpn_output_names(cfg):
+    """The FPN's outputs in order (backbone.output_shape()): p3..p7 for the DLA p67 builder (dla.py:536-561), p2..p6 for the
+    VoVNet p6 builder (vovnet.py:428-454)."""
+    return ["p3", "p4", "p5", "p6", "p7"] if arch_of(cfg) in DLA_SPECS else ["p2", "p3", "p4", "p5", "p6"]
+
+
+def in_feature_levels(cfg):
+    """DD3D.IN_FEATURES as FPN output indices (0..4) in head order: `cfg.DD3D.IN_FEATURES or list(backbone_output_shape)`
+    (core.py:25-26).  An unknown name raises KeyError like the reference's `backbone_output_shape[f]`; a repeated level, which
+    the reference builds but has no use, raises NotImplementedError."""
+    names = fpn_output_names(cfg)
+    dd3d = cfg.DD3D
+    sel = dd3d.get("IN_FEATURES") if hasattr(dd3d, "get") else getattr(dd3d, "IN_FEATURES", None)
+    sel = list(sel or names)
+    for f in sel:
+        if f not in names:
+            raise KeyError(f)
+    for f in sel:
+        if sel.count(f) > 1:
+            raise NotImplementedError(f"DD3D.IN_FEATURES lists {f!r} {sel.count(f)} times: the engine runs each FPN "
+                                      "level at most once")
+    return [names.index(f) for f in sel]
+
+
 def level_strides(cfg):
-    return [8, 16, 32, 64, 128] if arch_of(cfg) in DLA_SPECS else [4, 8, 16, 32, 64]
+    """Strides of the head levels, in DD3D.IN_FEATURES order (compute_locations, core.py:166-174)."""
+    strides = [8, 16, 32, 64, 128] if arch_of(cfg) in DLA_SPECS else [4, 8, 16, 32, 64]
+    return [strides[i] for i in in_feature_levels(cfg)]
 
 
 def size_divisibility(cfg):

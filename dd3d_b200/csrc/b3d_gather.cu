@@ -56,7 +56,7 @@ __device__ __forceinline__ void stage_slab(const __nv_bfloat16* w, int C, int c,
 __global__ void __launch_bounds__(kGroupThreads) b3d_group_kernel(const B3dGatherParams p) {
     DD3D_PDL_PROLOGUE();
     __shared__ int s_cnt[kB3dGatherMaxC], s_pos[kB3dGatherMaxC];
-    const int bl = blockIdx.y * kLevels + blockIdx.x;
+    const int bl = blockIdx.y * p.num_levels + blockIdx.x;
     const int count = min(p.cand_count[bl], p.topk);
     const uint2* fin = p.fin + static_cast<size_t>(bl) * p.topk;
     for (int c = threadIdx.x; c < p.C; c += blockDim.x) s_cnt[c] = 0;
@@ -82,7 +82,7 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel_gathered(const B3d
     DD3D_PDL_PROLOGUE();
     extern __shared__ __align__(16) uint8_t smem[];
     const int c = blockIdx.x, l = blockIdx.y, b = blockIdx.z;
-    const int bl = b * kLevels + l;
+    const int bl = b * p.num_levels + l;
     const int2 sg = p.seg[static_cast<size_t>(bl) * p.C + c];
     if (sg.y == 0) return;  // block-uniform
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -166,7 +166,7 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel_gathered(const B3d
 template <int KCS>
 cudaError_t launch_gathered(const B3dGatherParams& p, cudaStream_t stream) {
     constexpr int smem = 2 * kSlabRows * 128;
-    const dim3 grid(p.C, kLevels, p.B);
+    const dim3 grid(p.C, p.num_levels, p.B);
     if (p.fp16) return launch_pdl(b3d_sparse_kernel_gathered<true, KCS>, grid, dim3(kThreads), smem, stream, p);
     return launch_pdl(b3d_sparse_kernel_gathered<false, KCS>, grid, dim3(kThreads), smem, stream, p);
 }
@@ -175,13 +175,13 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 }  // namespace
 
-size_t b3d_gather_scratch_bytes(int B, int C, int topk) {
-    const size_t bl = static_cast<size_t>(B) * kLevels;
+size_t b3d_gather_scratch_bytes(int B, int C, int topk, int num_levels) {
+    const size_t bl = static_cast<size_t>(B) * num_levels;
     return align_up(bl * topk * 4, 256) + align_up(bl * C * 8, 256);
 }
 
 void b3d_gather_bind_scratch(B3dGatherParams* p, void* scratch) {
-    const size_t bl = static_cast<size_t>(p->B) * kLevels;
+    const size_t bl = static_cast<size_t>(p->B) * p->num_levels;
     uint8_t* s = static_cast<uint8_t*>(scratch);
     p->order = reinterpret_cast<int32_t*>(s);
     p->seg = reinterpret_cast<int2*>(s + align_up(bl * p->topk * 4, 256));
@@ -191,11 +191,12 @@ cudaError_t launch_b3d_gather(const B3dGatherParams& p, cudaStream_t stream) {
     if (p.B < 1 || p.topk < 1 || p.C < 1 || p.C > kB3dGatherMaxC || p.order == nullptr || p.seg == nullptr)
         return cudaErrorInvalidValue;
     if (p.cin < kChunk || p.cin % kChunk || p.cin > kB3dSparseMaxCin) return cudaErrorInvalidValue;
-    for (int l = 0; l < kLevels; ++l)
+    if (p.num_levels < 1 || p.num_levels > kLevels) return cudaErrorInvalidValue;
+    for (int l = 0; l < p.num_levels; ++l)
         if (p.lvl[l].pitch % 8 || p.lvl[l].pitch < p.cin || p.lvl[l].in == nullptr || p.lvl[l].w == nullptr ||
             p.lvl[l].scale == nullptr || p.lvl[l].bias == nullptr)
             return cudaErrorInvalidValue;
-    cudaError_t e = launch_pdl(b3d_group_kernel, dim3(kLevels, p.B), dim3(kGroupThreads), 0, stream, p);
+    cudaError_t e = launch_pdl(b3d_group_kernel, dim3(p.num_levels, p.B), dim3(kGroupThreads), 0, stream, p);
     if (e != cudaSuccess) return e;
     return p.cin == 256 ? launch_gathered<4>(p, stream) : launch_gathered<0>(p, stream);
 }

@@ -53,7 +53,7 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel(const B3dSparsePar
     DD3D_PDL_PROLOGUE();
     extern __shared__ __align__(16) uint8_t smem[];
     const int b = blockIdx.z, l = blockIdx.y, r0 = blockIdx.x * kRowsPerCta;
-    const int bl = b * kLevels + l;
+    const int bl = b * p.num_levels + l;
     const int count = min(p.cand_count[bl], p.topk);
     if (r0 >= count) return;  // block-uniform
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -137,7 +137,7 @@ __global__ void __launch_bounds__(kThreads) b3d_sparse_kernel(const B3dSparsePar
 template <int NT, int KCS>
 cudaError_t launch_nt(const B3dSparseParams& p, cudaStream_t stream) {
     const int smem = 2 * p.n_pad * 128;
-    dim3 grid((p.topk + kRowsPerCta - 1) / kRowsPerCta, kLevels, p.B);
+    dim3 grid((p.topk + kRowsPerCta - 1) / kRowsPerCta, p.num_levels, p.B);
     if (p.fp16) return launch_pdl(b3d_sparse_kernel<NT, true, KCS>, grid, dim3(kThreads), smem, stream, p);
     return launch_pdl(b3d_sparse_kernel<NT, false, KCS>, grid, dim3(kThreads), smem, stream, p);
 }
@@ -153,7 +153,8 @@ cudaError_t launch_b3d_sparse(const B3dSparseParams& p, cudaStream_t stream) {
     if (p.n_pad < 8 || p.n_pad % 8 || p.n_pad > kB3dSparseMaxN || p.out_pitch < p.n_pad || p.out_pitch % 2 || p.B < 1 || p.topk < 1)
         return cudaErrorInvalidValue;
     if (p.cin < kChunk || p.cin % kChunk || p.cin > kB3dSparseMaxCin) return cudaErrorInvalidValue;
-    for (int l = 0; l < kLevels; ++l)
+    if (p.num_levels < 1 || p.num_levels > kLevels) return cudaErrorInvalidValue;
+    for (int l = 0; l < p.num_levels; ++l)
         if (p.lvl[l].pitch % 8 || p.lvl[l].pitch < p.cin || p.lvl[l].in == nullptr || p.lvl[l].w == nullptr)
             return cudaErrorInvalidValue;
     if (p.n_pad <= 64) return launch_cin<8>(p, stream);   // C3 <= 5 (KITTI: 5 classes -> 55 -> 64), class-agnostic (11 -> 16)

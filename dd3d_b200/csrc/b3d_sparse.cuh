@@ -21,6 +21,7 @@ struct B3dSparseParams {
     const uint2* fin;           // [B][L][topk] (score bits, pixel * C + class): DecodeParams::fin
     const int32_t* cand_count;  // [B][L]
     float* rows;                // [B][L][topk][out_pitch] fp32, channel layout of a dense map pixel
+    int num_levels;             // L: lvl[0 .. L) are read (DecodeParams::num_levels)
     int B, C, topk, n_pad, out_pitch, fp16;
     int cin;  // tower width (FE.FPN.OUT_CHANNELS): a multiple of 64 in [64, kB3dSparseMaxCin]
 };
@@ -45,9 +46,10 @@ struct B3dGatherParams {
     float* rows;                // [B][L][topk][kB3dGatherPitch]
     int32_t* order;             // scratch [B][L][topk]: the slots of each (image, level), grouped by class
     int2* seg;                  // scratch [B][L][C]: (first entry in `order`, count) of each class
+    int num_levels;             // L: lvl[0 .. L) are read (DecodeParams::num_levels)
     int B, C, topk, fp16, cin;
 };
-size_t b3d_gather_scratch_bytes(int B, int C, int topk);
+size_t b3d_gather_scratch_bytes(int B, int C, int topk, int num_levels = kLevels);
 void b3d_gather_bind_scratch(B3dGatherParams* p, void* scratch);
 constexpr int kB3dGatherLaunches = 2;  // class grouping + predictor
 cudaError_t launch_b3d_gather(const B3dGatherParams& p, cudaStream_t stream);
@@ -78,6 +80,7 @@ struct TowerTilesParams {
     const int32_t* cand_count;  // [B][L]
     int32_t* dist;              // mark pass: [cap] tile distances, (level, image) regions at the offsets of a layer's list;
                                 // kTowerTileFar between launches (tower_tiles_kernel reads and resets them)
+    int num_levels;             // L: lvl[0 .. L) (DecodeParams::num_levels)
     int B, C, topk, depth, reach;
     int cls_pitch, mark_blocks;  // mark pass
     float thresh;                // mark pass: PRE_NMS_THRESH

@@ -90,6 +90,11 @@ int dd3d_set_fpn_channels(dd3d_handle h, int32_t channels) {
     return guarded(h, [&](Engine& e) { e.set_fpn_channels(channels); });
 }
 
+int dd3d_set_in_features(dd3d_handle h, const int32_t* h_fpn_levels, int n) {
+    if (h_fpn_levels == nullptr) return DD3D_ERR_INVALID;
+    return guarded(h, [&](Engine& e) { e.set_in_features(h_fpn_levels, n); });
+}
+
 int dd3d_set_canonical_sizes(dd3d_handle h, int32_t num_classes, const float* h_sizes) {
     if (h_sizes == nullptr) return DD3D_ERR_INVALID;
     return guarded(h, [&](Engine& e) { e.set_canonical_sizes(num_classes, h_sizes); });
@@ -220,10 +225,12 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value) {
         if (n == "do_postprocess") {
             e.opt_do_postprocess = value ? 1 : 0;
         } else if (n == "do_nms") {
-            // without NMS up to 5 * PRE_NMS_TOPK detections per image survive: refuse a buffer that would truncate them
-            if (!value && e.desc.out_cap < kLevels * e.desc.pre_nms_topk)
-                throw EngineError(DD3D_ERR_INVALID, "do_nms = 0 needs out_cap >= 5 * pre_nms_topk (" +
-                                                        std::to_string(kLevels * e.desc.pre_nms_topk) + "), engine has " +
+            // without NMS up to L * PRE_NMS_TOPK detections per image survive (L head levels): refuse a buffer that would
+            // truncate them
+            const int L = e.num_levels();
+            if (!value && e.desc.out_cap < L * e.desc.pre_nms_topk)
+                throw EngineError(DD3D_ERR_INVALID, "do_nms = 0 needs out_cap >= " + std::to_string(L) + " * pre_nms_topk (" +
+                                                        std::to_string(L * e.desc.pre_nms_topk) + "), engine has " +
                                                         std::to_string(e.desc.out_cap) + ": recreate the engine");
             e.set_do_nms(value ? 1 : 0);
         } else if (n == "profile") {
@@ -331,6 +338,12 @@ int dd3d_get_tensor(dd3d_handle h, const char* name, void** d_ptr, int32_t dims[
             if (l < 0 || l >= kLevels) throw EngineError(DD3D_ERR_INVALID, "unknown tensor: " + n);
             return l;
         };
+        auto position = [&](size_t prefix_len) {  // head maps: by DD3D.IN_FEATURES position
+            const int l = level(prefix_len);
+            if (l >= P.num_levels) throw EngineError(DD3D_ERR_INVALID, "unknown tensor: " + n + " (head levels: " +
+                                                                            std::to_string(P.num_levels) + ")");
+            return l;
+        };
         if (n.rfind("op", 0) == 0) {  // "op<i>" / "op<i>:<seg>": bf16 output view of engine op i (launch order)
             const size_t colon = n.find(':');
             const int i = atoi(n.substr(2, colon == std::string::npos ? std::string::npos : colon - 2).c_str());
@@ -347,16 +360,17 @@ int dd3d_get_tensor(dd3d_handle h, const char* name, void** d_ptr, int32_t dims[
             memcpy(dims, d, sizeof(d));
         } else if (n[0] == 'p') {
             const View& v = P.fpn[level(1)];
+            if (v.ptr == nullptr) throw EngineError(DD3D_ERR_INVALID, "FPN output " + n + " is not built: no head reads it");
             *d_ptr = v.ptr;
             const int32_t d[6] = {v.B, v.H, v.W, v.C, v.pitch, 2};
             memcpy(dims, d, sizeof(d));
         } else if (n.rfind("cls", 0) == 0) {
-            const int l = level(3);
+            const int l = position(3);
             *d_ptr = P.cls_map[l];
             const int32_t d[6] = {P.B, P.lvl_h[l], P.lvl_w[l], e.desc.num_classes, P.cls_pitch, 4};
             memcpy(dims, d, sizeof(d));
         } else if (n.rfind("box", 0) == 0) {
-            const int l = level(3);
+            const int l = position(3);
             if (P.box2d_begin >= 0)
                 throw EngineError(DD3D_ERR_INVALID, "the box2d map is computed only around the pixels that pass the threshold "
                                                     "with option sparse_box2d_tower: " + n);
@@ -364,7 +378,7 @@ int dd3d_get_tensor(dd3d_handle h, const char* name, void** d_ptr, int32_t dims[
             const int32_t d[6] = {P.B, P.lvl_h[l], P.lvl_w[l], 5, 16, 4};
             memcpy(dims, d, sizeof(d));
         } else if (n.rfind("b3d", 0) == 0) {
-            const int l = level(3);
+            const int l = position(3);
             if (P.b3d_map[l] == nullptr)
                 throw EngineError(DD3D_ERR_INVALID, P.sparse_b3d ? "dense box3d maps are not computed with option sparse_box3d = 1: " + n
                                                                  : "no 3-D head (box3d_on = 0): " + n);
@@ -644,6 +658,7 @@ int dd3d_op_b3d_sparse_c(const void* const* d_in, const int32_t* h_level_hw, con
     p.fin = static_cast<const uint2*>(d_fin);
     p.cand_count = d_counts;
     p.rows = d_rows;
+    p.num_levels = kLevels;
     p.B = B;
     p.C = C;
     p.topk = topk;
@@ -682,6 +697,7 @@ int dd3d_op_b3d_gather(const void* const* d_in, const int32_t* h_level_hw, const
     p.fin = static_cast<const uint2*>(d_fin);
     p.cand_count = d_counts;
     p.rows = d_rows;
+    p.num_levels = kLevels;
     p.B = B;
     p.C = C;
     p.topk = topk;

@@ -30,7 +30,7 @@ __device__ __forceinline__ int find_level(const DecodeParams& p, int blk) {
     int l = 0;
 #pragma unroll
     for (int i = 1; i < kLevels; ++i)
-        if (blk >= p.lvl[i].block_begin) l = i;
+        if (i < p.num_levels && blk >= p.lvl[i].block_begin) l = i;
     return l;
 }
 
@@ -76,7 +76,7 @@ __global__ void __launch_bounds__(kDenseThreads) dense_kernel(const __grid_const
     const int b = blockIdx.y;
     const int hw = L.H * L.W;
     const int pix = (blockIdx.x - L.block_begin) * kDenseThreads + threadIdx.x;
-    const int bl = b * kLevels + l;
+    const int bl = b * p.num_levels + l;
     if (MODE == 0) {
         for (int i = threadIdx.x; i < kHistBins; i += kDenseThreads) shist[i] = 0;
         __syncthreads();
@@ -114,7 +114,7 @@ __global__ void __launch_bounds__(kDenseThreads) dense_kernel(const __grid_const
 __global__ void __launch_bounds__(256) select_kernel(const __grid_constant__ DecodeParams p) {
     DD3D_PDL_PROLOGUE();
     __shared__ uint32_t chunk[256];
-    const int bl = blockIdx.y * kLevels + blockIdx.x;
+    const int bl = blockIdx.y * p.num_levels + blockIdx.x;
     const uint32_t* gh = p.hist + static_cast<size_t>(bl) * kHistBins;
     constexpr int per = kHistBins / 256;
     uint32_t loc = 0;
@@ -455,7 +455,7 @@ __device__ void select_overflow(const DecodeParams& p, int b, int l, uint32_t T,
 __global__ void __launch_bounds__(kSelectThreads) select_final_kernel(const __grid_constant__ DecodeParams p) {
     DD3D_PDL_PROLOGUE();
     const int l = blockIdx.x, b = blockIdx.y;
-    const int bl = b * kLevels + l;
+    const int bl = b * p.num_levels + l;
     const int* sel = p.sel + bl * 4;
     const int n_sure = min(p.counters[bl * 2 + 0], p.topk);
     const int nb_raw = p.counters[bl * 2 + 1];
@@ -488,11 +488,11 @@ constexpr int kFinalSplit = 8, kFinalThreads = 128;
 __global__ void __launch_bounds__(kFinalThreads) decode_final_kernel(const __grid_constant__ DecodeParams p) {
     DD3D_PDL_PROLOGUE();
     const int l = blockIdx.x / kFinalSplit, part = blockIdx.x % kFinalSplit, b = blockIdx.y;
-    const int bl = b * kLevels + l;
+    const int bl = b * p.num_levels + l;
     const int n = p.cand_count[bl];
     const DecodeLevel& L = p.lvl[l];
     const uint2* fin = p.fin + static_cast<size_t>(bl) * p.topk;
-    Det* out = p.cand + (static_cast<size_t>(b) * kLevels + l) * p.topk;
+    Det* out = p.cand + static_cast<size_t>(bl) * p.topk;
     const size_t hw = static_cast<size_t>(L.H) * L.W;
     for (int i = part * kFinalThreads + threadIdx.x; i < n; i += kFinalSplit * kFinalThreads) {
         const uint2 me = fin[i];
@@ -518,8 +518,8 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 }  // namespace
 
 // scratch layout: [hist | counters | flags(1 word + pad)] (cleared every forward) then sel, sure, boundary, cand, cand_count
-size_t decode_scratch_bytes(int B, int topk) {
-    const size_t bl = static_cast<size_t>(B) * kLevels;
+size_t decode_scratch_bytes(int B, int topk, int num_levels) {
+    const size_t bl = static_cast<size_t>(B) * num_levels;
     size_t n = 0;
     n += align_up(bl * kHistBins * 4, 256);
     n += align_up(bl * 2 * 4, 256);
@@ -534,7 +534,7 @@ size_t decode_scratch_bytes(int B, int topk) {
 }
 
 void decode_bind_scratch(DecodeParams* p, void* scratch) {
-    const size_t bl = static_cast<size_t>(p->B) * kLevels;
+    const size_t bl = static_cast<size_t>(p->B) * p->num_levels;
     uint8_t* s = static_cast<uint8_t*>(scratch);
     p->hist = reinterpret_cast<uint32_t*>(s);
     s += align_up(bl * kHistBins * 4, 256);
@@ -557,7 +557,7 @@ void decode_bind_scratch(DecodeParams* p, void* scratch) {
 
 void decode_finalize_params(DecodeParams* p) {
     int blk = 0;
-    for (int l = 0; l < kLevels; ++l) {
+    for (int l = 0; l < p->num_levels; ++l) {
         p->lvl[l].block_begin = blk;
         blk += (p->lvl[l].H * p->lvl[l].W + kDenseThreads - 1) / kDenseThreads;
     }
@@ -575,19 +575,21 @@ void decode_finalize_params(DecodeParams* p) {
 }
 
 cudaError_t launch_decode_select(const DecodeParams& p, cudaStream_t stream) {
-    const size_t bl = static_cast<size_t>(p.B) * kLevels;
+    if (p.num_levels < 1 || p.num_levels > kLevels) return cudaErrorInvalidValue;
+    const size_t bl = static_cast<size_t>(p.B) * p.num_levels;
     const size_t clear_words = (align_up(bl * kHistBins * 4, 256) + align_up(bl * 2 * 4, 256) + 256) / 4;
     cudaError_t e = launch_pdl(clear_kernel, dim3(148), dim3(256), 0, stream, p.hist, clear_words);
     dim3 dgrid(p.total_blocks, p.B);
     if (e == cudaSuccess) e = launch_pdl(dense_kernel<0>, dgrid, dim3(kDenseThreads), 0, stream, p);
-    if (e == cudaSuccess) e = launch_pdl(select_kernel, dim3(kLevels, p.B), dim3(256), 0, stream, p);
+    if (e == cudaSuccess) e = launch_pdl(select_kernel, dim3(p.num_levels, p.B), dim3(256), 0, stream, p);
     if (e == cudaSuccess) e = launch_pdl(dense_kernel<1>, dgrid, dim3(kDenseThreads), 0, stream, p);
-    if (e == cudaSuccess) e = launch_pdl(select_final_kernel, dim3(kLevels, p.B), dim3(kSelectThreads), 0, stream, p);
+    if (e == cudaSuccess) e = launch_pdl(select_final_kernel, dim3(p.num_levels, p.B), dim3(kSelectThreads), 0, stream, p);
     return e;
 }
 
 cudaError_t launch_decode_final(const DecodeParams& p, cudaStream_t stream) {
-    return launch_pdl(decode_final_kernel, dim3(kLevels * kFinalSplit, p.B), dim3(kFinalThreads), 0, stream, p);
+    if (p.num_levels < 1 || p.num_levels > kLevels) return cudaErrorInvalidValue;
+    return launch_pdl(decode_final_kernel, dim3(p.num_levels * kFinalSplit, p.B), dim3(kFinalThreads), 0, stream, p);
 }
 
 cudaError_t launch_decode(const DecodeParams& p, cudaStream_t stream) {

@@ -82,7 +82,8 @@ struct DecodeLevel {
 };
 
 struct DecodeParams {
-    DecodeLevel lvl[kLevels];
+    DecodeLevel lvl[kLevels];  // positions 0 .. num_levels - 1 (DD3D.IN_FEATURES order)
+    int num_levels;            // head levels (1 .. kLevels): the per-(image, level) scratch and the grids follow it
     int B, C, cls_pitch, b3d_pitch;
     int attr_off;       // NuscenesDD3D: channel of the first attribute logit in the cls map (speed follows), else -1
     int num_attr;
@@ -106,7 +107,7 @@ struct DecodeParams {
     int32_t* counters;    // [B][L][2] : sure, boundary
     uint2* sure;          // [B][L][topk]          (score bits, index)
     uint2* boundary;      // [B][L][kBoundaryCap]
-    Det* cand;            // [B][L*topk]           decoded candidates
+    Det* cand;            // [B][L*topk]           decoded candidates (L = num_levels)
     int32_t* cand_count;  // [B][L]
     int32_t* flags;       // [1] overflow word (the decode sets no bit; NMS: bit1)
     uint2* fin;           // [B][L][topk] final candidates (score bits, index): slot order of `cand`
@@ -126,6 +127,7 @@ struct NmsParams {
     int32_t* out_count;         // [B]
     int32_t* flags;             // bit1: output overflow
     int B, topk, out_cap;
+    int num_levels;             // L of cand / cand_count: the DecodeParams' num_levels
     int do_nms, post_topk, do_postprocess;
     float nms_thresh;
     void* scratch;    // nms_scratch_bytes(B, topk, num_classes) bytes, or nullptr (single-CTA kernel only)
@@ -135,7 +137,7 @@ struct NmsParams {
     int class_parallel;
 };
 
-size_t decode_scratch_bytes(int B, int topk);
+size_t decode_scratch_bytes(int B, int topk, int num_levels = kLevels);
 void decode_bind_scratch(DecodeParams* p, void* scratch);
 void decode_finalize_params(DecodeParams* p);
 cudaError_t launch_decode(const DecodeParams& p, cudaStream_t stream);  // = select + final
@@ -147,7 +149,7 @@ cudaError_t launch_decode_select(const DecodeParams& p, cudaStream_t stream);
 cudaError_t launch_decode_final(const DecodeParams& p, cudaStream_t stream);
 cudaError_t launch_nms(const NmsParams& p, cudaStream_t stream);  // the path p.class_parallel names
 int nms_launches(const NmsParams& p);
-size_t nms_scratch_bytes(int B, int topk, int num_classes);
+size_t nms_scratch_bytes(int B, int topk, int num_classes, int num_levels = kLevels);
 void nms_set_class_parallel(int mode);  // 0 single-CTA kernel, 1 multi-CTA path, -1 environment / default (1)
 // The NMS path for params whose other fields are filled: the multi-CTA one when the policy above allows it, the params
 // have its scratch, there is something to suppress (do_nms, nms_thresh > 0) and 1 <= num_classes <= 255.

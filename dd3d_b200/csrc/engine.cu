@@ -249,6 +249,23 @@ void Engine::set_fpn_channels(int C) {
     fpn_channels = C;
 }
 
+void Engine::set_in_features(const int32_t* fpn_levels, int n) {
+    if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_in_features after finalize");
+    if (fpn_levels == nullptr || n < 1 || n > kLevels) fail(DD3D_ERR_INVALID, "dd3d_set_in_features needs 1 to 5 FPN levels");
+    std::vector<int> v(fpn_levels, fpn_levels + n);
+    for (int i = 0; i < n; ++i) {
+        if (v[i] < 0 || v[i] >= kLevels) fail(DD3D_ERR_INVALID, "FPN level " + std::to_string(v[i]) + " outside 0..4");
+        for (int j = 0; j < i; ++j)
+            if (v[j] == v[i]) fail(DD3D_ERR_INVALID, "FPN level " + std::to_string(v[i]) + " repeated");
+    }
+    in_features = v;
+    if (n == kLevels) {  // all five in order is the default graph
+        bool identity = true;
+        for (int i = 0; i < n; ++i) identity = identity && v[i] == i;
+        if (identity) in_features.clear();
+    }
+}
+
 void Engine::set_canonical_sizes(int num_classes, const float* sizes) {
     if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_canonical_sizes after finalize");
     if (num_classes != desc.num_classes || sizes == nullptr)
@@ -998,12 +1015,25 @@ struct Builder {
         const bool gn = norm == DD3D_NORM_GN, bn = norm == DD3D_NORM_BN_SHARED || norm == DD3D_NORM_BN_PER_LEVEL;
         const bool avg = E->layout.fpn_fuse_avg != 0;
         const int width = E->fpn_channels;  // FE.FPN.OUT_CHANNELS: laterals, outputs, P6 / P7
+        // outputs the heads read (DD3D.IN_FEATURES): stage outputs 0 .. n-1, then P6 (n) and P7 (n + 1).  P6 reads output
+        // n - 1 and P7 reads P6; lateral i feeds output i and every lateral below it, so the laterals below the lowest output
+        // read are skipped too.  The reference still computes them; nothing reads them.
+        const bool dla = dla_spec(E->desc.arch) != nullptr;
+        bool read[kLevels + 1] = {};
+        for (int l = 0; l < E->num_levels(); ++l) read[E->head_level(l)] = true;
+        const bool want_p7 = dla && read[n + 1], want_p6 = read[n] || want_p7;
+        std::vector<bool> need(n);
+        int lowest = n;
+        for (int i = n - 1; i >= 0; --i) {
+            need[i] = read[i] || (i == n - 1 && want_p6);
+            if (need[i]) lowest = i;
+        }
         auto conv_norm = [&](const std::string& name, View in, View out, int ksize, const View* res) {
             conv1(name, bn ? name + ".norm" : "", norm == DD3D_NORM_NONE, in, out, ksize, 1, false, res, res != nullptr);
         };
         std::vector<View> res(n);
         View prev;
-        for (int i = n - 1; i >= 0; --i) {
+        for (int i = n - 1; i >= lowest; --i) {
             const std::string st = std::to_string(first_stage + i);
             const std::string lname = p + ".fpn_lateral" + st, oname = p + ".fpn_output" + st;
             const View& c = feats[i];
@@ -1017,18 +1047,23 @@ struct Builder {
                 conv_norm(lname, c, lat, 1, &prev);
             }
             prev = lat;
+            if (!need[i]) continue;
             res[i] = alloc(c.H, c.W, width);
             persist(res[i]);
             conv_norm(oname, lat, res[i], 3, nullptr);
             if (gn) group_norm({res[i]}, &E->gn_affine(oname + ".norm", width), false, nullptr, false);
         }
         *outs = res;
+        if (!want_p6) {
+            outs->resize(kLevels);
+            return;
+        }
         const View& p5 = res[n - 1];
         View p6 = alloc(p5.H / 2, p5.W / 2, width);
         persist(p6);
         conv1(p + ".top_block.p6", "", true, p5, p6, 3, 2, false);
         outs->push_back(p6);
-        if (dla_spec(E->desc.arch) != nullptr) {  // LastLevelP6P7
+        if (want_p7) {  // LastLevelP6P7
             View r6 = alloc(p6.H, p6.W, width);
             relu(p6, r6);
             View p7 = alloc(p6.H / 2, p6.W / 2, width);
@@ -1036,6 +1071,7 @@ struct Builder {
             conv1(p + ".top_block.p7", "", true, r6, p7, 3, 2, false);
             outs->push_back(p7);
         }
+        outs->resize(kLevels);  // VoVNet: P6 is the last; a skipped output stays an empty view
     }
 
     // ---- heads ------------------------------------------------------------------------------------------------
@@ -1080,6 +1116,7 @@ struct Builder {
     bool tower_tile_lists(TowerTilesParams& tt, const std::vector<View>& feats, int depth, int reach) {
         memset(&tt, 0, sizeof(tt));
         const int L = static_cast<int>(feats.size());
+        tt.num_levels = L;
         int hs[kMaxSeg], ws[kMaxSeg];
         for (int l = 0; l < L; ++l) {
             hs[l] = feats[l].H;
@@ -1175,9 +1212,10 @@ struct Builder {
         const int rows_pitch = gather3 ? kB3dGatherPitch : b3d_pitch;
         P->sparse_b3d = sparse3;
         P->gather_b3d = sparse3 && gather3;
-        P->b3d_rows = sparse3 ? alloc_f32(static_cast<size_t>(B) * kLevels * E->desc.pre_nms_topk * rows_pitch) : nullptr;
+        P->b3d_rows = sparse3 ? alloc_f32(static_cast<size_t>(B) * L * E->desc.pre_nms_topk * rows_pitch) : nullptr;
         P->b3d_gather_scratch =
-            P->gather_b3d ? alloc_bytes(b3d_gather_scratch_bytes(B, C, E->desc.pre_nms_topk)) : nullptr;
+            P->gather_b3d ? alloc_bytes(b3d_gather_scratch_bytes(B, C, E->desc.pre_nms_topk, L)) : nullptr;
+        P->num_levels = L;
         P->cls_pitch = cls_pitch;
         P->b3d_pitch = b3d_pitch;
         // each tower is followed at once by its predictor, so that its ping-pong buffers die before the next tower starts
@@ -1358,6 +1396,7 @@ struct Builder {
                 }
                 ++op_idx;
                 gp.rows = P->b3d_rows;
+                gp.num_levels = L;
                 gp.B = B;
                 gp.C = C;
                 gp.topk = E->desc.pre_nms_topk;
@@ -1383,6 +1422,7 @@ struct Builder {
                 }
                 ++op_idx;
                 sp.rows = P->b3d_rows;
+                sp.num_levels = L;
                 sp.B = B;
                 sp.C = C;
                 sp.topk = E->desc.pre_nms_topk;
@@ -1588,10 +1628,12 @@ size_t Engine::build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry) 
         }
         if (static_cast<int>(fpn.size()) != kLevels) fail(DD3D_ERR_STATE, "internal: expected 5 FPN levels");
         for (int l = 0; l < kLevels; ++l) P->fpn[l] = fpn[l];
-        bld.build_heads(fpn);
+        std::vector<View> heads(num_levels());  // the FPN outputs in DD3D.IN_FEATURES order
+        for (int l = 0; l < num_levels(); ++l) heads[l] = fpn[head_level(l)];
+        bld.build_heads(heads);
         // detection scratch + staging for the host-facing path
-        P->detect_scratch = bld.alloc_bytes(decode_scratch_bytes(B, desc.pre_nms_topk));
-        P->nms_scratch = bld.alloc_bytes(nms_scratch_bytes(B, desc.pre_nms_topk, desc.num_classes));
+        P->detect_scratch = bld.alloc_bytes(decode_scratch_bytes(B, desc.pre_nms_topk, num_levels()));
+        P->nms_scratch = bld.alloc_bytes(nms_scratch_bytes(B, desc.pre_nms_topk, desc.num_classes, num_levels()));
         P->d_K = static_cast<float*>(bld.alloc_bytes(static_cast<size_t>(B) * 9 * 4));
         P->d_sizes = static_cast<int32_t*>(bld.alloc_bytes(static_cast<size_t>(B) * 4 * 4));
         P->d_out = static_cast<Det*>(bld.alloc_bytes(static_cast<size_t>(B) * desc.out_cap * sizeof(Det)));
@@ -1698,15 +1740,15 @@ void Engine::make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes) {
     static const int strides_dla[5] = {8, 16, 32, 64, 128};
     static const int strides_vov[5] = {4, 8, 16, 32, 64};
     const int* strides = dla_spec(desc.arch) != nullptr ? strides_dla : strides_vov;
-    for (int l = 0; l < kLevels; ++l) {
+    for (int l = 0; l < plan.num_levels; ++l) {  // compute_locations with the strides of the selected levels
         dp.lvl[l].cls = plan.cls_map[l];
         dp.lvl[l].box = plan.box_map[l];
         dp.lvl[l].b3d = plan.b3d_map[l];
         dp.lvl[l].H = plan.lvl_h[l];
         dp.lvl[l].W = plan.lvl_w[l];
-        dp.lvl[l].stride = strides[l];
+        dp.lvl[l].stride = strides[head_level(l)];
     }
-    fill_decode_params(&dp, desc, B, plan.cls_pitch, plan.b3d_pitch, d_canon);
+    fill_decode_params(&dp, desc, B, plan.cls_pitch, plan.b3d_pitch, d_canon, plan.num_levels);
     decode_bind_scratch(&dp, plan.detect_scratch);
     decode_finalize_params(&dp);
     if (plan.gather_b3d) {
@@ -1765,7 +1807,7 @@ void Engine::plan_steps(Plan* P) {
     det.select = P->tower_begin < 0;
     det.b3d = P->gather_b3d ? Step::kB3dGathered : P->sparse_b3d ? Step::kB3dSparse : 0;
     det.launches += (det.select ? kDecodeSelectLaunches : 0) + (P->gather_b3d ? kB3dGatherLaunches : P->sparse_b3d ? kOneLaunch : 0);
-    for (int l = 0; l < kLevels; ++l)  // two dense passes over the fp32 logits + centerness
+    for (int l = 0; l < P->num_levels; ++l)  // two dense passes over the fp32 logits + centerness
         det.bytes += 2.0 * P->B * P->lvl_h[l] * P->lvl_w[l] * (static_cast<double>(desc.num_classes) + 1) * 4;
     add(Step::NMS, 7, nms_launches(P->nms) + (P->bev == kBevPathOneCta     ? kOneLaunch
                                               : P->bev == kBevPathMultiCta ? image_bev_nms_launches(P->B) : 0))
@@ -1773,7 +1815,8 @@ void Engine::plan_steps(Plan* P) {
 }
 
 void fill_decode_params(DecodeParams* dp, const dd3d_model_desc& desc, int B, int cls_pitch, int b3d_pitch,
-                        const float* d_canon) {
+                        const float* d_canon, int num_levels) {
+    dp->num_levels = num_levels;
     dp->B = B;
     dp->C = desc.num_classes;
     dp->cls_pitch = cls_pitch;
@@ -1802,6 +1845,7 @@ void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodePar
     np->cand_count = dp.cand_count;
     np->flags = dp.flags;
     np->B = B;
+    np->num_levels = dp.num_levels;
     np->topk = desc.pre_nms_topk;
     np->out_cap = desc.out_cap;
     np->do_nms = desc.do_nms;

@@ -157,7 +157,8 @@ struct Plan {
     int32_t* s1_counts = nullptr;
     float* s1_poses = nullptr;  // BEV NMS on: slot 1's copy of the host poses
     View input;
-    View fpn[kLevels];
+    View fpn[kLevels];  // by FPN output index; an output no head reads is not built (null ptr)
+    int num_levels = kLevels;  // head positions; the per-level arrays below are by position
     float* cls_map[kLevels] = {};
     float* box_map[kLevels] = {};
     float* b3d_map[kLevels] = {};
@@ -203,7 +204,7 @@ struct Plan {
 };
 
 void fill_decode_params(DecodeParams* dp, const dd3d_model_desc& desc, int B, int cls_pitch, int b3d_pitch,
-                        const float* d_canon);
+                        const float* d_canon, int num_levels = kLevels);
 void fill_nms_params(NmsParams* np, const dd3d_model_desc& desc, const DecodeParams& dp, int B, void* scratch);
 
 class Engine {
@@ -272,10 +273,16 @@ class Engine {
     void set_backbone_norm(int norm);
     void set_fpn_channels(int C);
     void set_canonical_sizes(int num_classes, const float* sizes);
+    void set_in_features(const int32_t* fpn_levels, int n);
+    int num_levels() const { return in_features.empty() ? kLevels : static_cast<int>(in_features.size()); }
+    int head_level(int l) const { return in_features.empty() ? l : in_features[l]; }  // FPN output read at position l
 
     dd3d_model_desc desc;
     // FCOS3D.CANONICAL_BOX3D_SIZES rows 0..num_classes-1 (dd3d_set_canonical_sizes); empty: the desc's rows (num_classes <= 16)
     std::vector<float> canonical_sizes;
+    // DD3D.IN_FEATURES (dd3d_set_in_features): the FPN output (0 .. 4) each head position reads, distinct; empty: all five in
+    // order.  Per-level BN, Scale / Offset and PER_LEVEL_PREDICTORS predictors are taken by position.
+    std::vector<int> in_features;
     // FPN / head layout (dd3d_set_layout); the default is the shipped one
     dd3d_layout_desc layout = {DD3D_NORM_BN_PER_LEVEL, DD3D_NORM_BN_PER_LEVEL, DD3D_NORM_BN_SHARED, 4, 4, 4, 0};
     // FE.BACKBONE.NORM (dd3d_set_backbone_norm): BN folded into the conv epilogues (default), DD3D_NORM_NONE (DLA-34: conv bias)

@@ -104,13 +104,13 @@ __device__ __forceinline__ NmsSmem carve(uint8_t* raw, int cap) {
 }
 
 // 1. keys (score3d desc, level asc, index asc) -> bitonic sort (when do_nms) -> val[i] = candidate slot of sorted position i.
-//    Returns n.  s_lvl_off: [kLevels + 1] shared ints.
+//    Returns n.  s_lvl_off: [kLevels + 1] shared ints; positions num_levels and up are empty.
 __device__ int sort_candidates(const NmsParams& p, int b, const Det* cand, NmsSmem m, int* s_lvl_off) {
     if (threadIdx.x == 0) {
         int off = 0;
         for (int l = 0; l < kLevels; ++l) {
             s_lvl_off[l] = off;
-            off += min(p.cand_count[b * kLevels + l], p.topk);
+            if (l < p.num_levels) off += min(p.cand_count[b * p.num_levels + l], p.topk);
         }
         s_lvl_off[kLevels] = off;
     }
@@ -288,7 +288,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_kernel(const __grid_consta
     DD3D_PDL_PROLOGUE();
     extern __shared__ uint8_t smem_raw[];
     const int b = blockIdx.x;
-    const int cap = kLevels * p.topk;
+    const int cap = p.num_levels * p.topk;
     NmsSmem m = carve(smem_raw, cap);
     __shared__ int s_warp_sums[33];
     __shared__ int s_base;
@@ -377,7 +377,7 @@ __global__ void __launch_bounds__(kSortThreads) nms_sort_kernel(const __grid_con
     DD3D_PDL_PROLOGUE();
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const int b = blockIdx.y;
-    const int cap = kLevels * p.topk, C = p.num_classes;
+    const int cap = p.num_levels * p.topk, C = p.num_classes;
     uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);       // [cap]
     uint16_t* slots = reinterpret_cast<uint16_t*>(keys + cap);    // [cap]
     uint8_t* scls = reinterpret_cast<uint8_t*>(slots + cap);      // [cap]
@@ -389,7 +389,7 @@ __global__ void __launch_bounds__(kSortThreads) nms_sort_kernel(const __grid_con
         int off = 0;
         for (int l = 0; l < kLevels; ++l) {
             s_lvl_off[l] = off;
-            off += min(p.cand_count[b * kLevels + l], p.topk);
+            if (l < p.num_levels) off += min(p.cand_count[b * p.num_levels + l], p.topk);
         }
         s_lvl_off[kLevels] = off;
     }
@@ -465,7 +465,7 @@ constexpr int kMaskCtasPerImage = 64;
 __global__ void __launch_bounds__(kMaskThreads) nms_mask_kernel(const __grid_constant__ NmsParams p) {
     DD3D_PDL_PROLOGUE();
     const int b = blockIdx.y;
-    const int cap = kLevels * p.topk, C = p.num_classes;
+    const int cap = p.num_levels * p.topk, C = p.num_classes;
     const NmsScratch sc = bind_nms_scratch(p.scratch, p.B, cap, C);
     __shared__ int s_first[257];  // first pair index of class c
     __shared__ float4 s_col[64];
@@ -522,7 +522,7 @@ constexpr int kScanThreads = 128;  // >= W (cap <= 8192)
 __global__ void __launch_bounds__(kScanThreads) nms_scan_kernel(const __grid_constant__ NmsParams p) {
     DD3D_PDL_PROLOGUE();
     const int c = blockIdx.x, b = blockIdx.y;
-    const int cap = kLevels * p.topk, C = p.num_classes;
+    const int cap = p.num_levels * p.topk, C = p.num_classes;
     const NmsScratch sc = bind_nms_scratch(p.scratch, p.B, cap, C);
     const int nc = sc.seg_cnt[b * C + c];
     if (nc <= 1) return;
@@ -584,7 +584,7 @@ __global__ void __launch_bounds__(kNmsThreads, 1) nms_finish_kernel(const __grid
     DD3D_PDL_PROLOGUE();
     extern __shared__ uint8_t smem_raw[];
     const int b = blockIdx.x;
-    const int cap = kLevels * p.topk;
+    const int cap = p.num_levels * p.topk;
     NmsSmem m = carve(smem_raw, cap);
     __shared__ int s_warp_sums[33];
     __shared__ int s_base;
@@ -618,16 +618,16 @@ int nms_class_parallel(const NmsParams& p) {
 
 int nms_launches(const NmsParams& p) { return p.class_parallel ? 4 : 1; }
 
-size_t nms_scratch_bytes(int B, int topk, int num_classes) {
-    const int cap = kLevels * topk;
+size_t nms_scratch_bytes(int B, int topk, int num_classes, int num_levels) {
+    const int cap = num_levels * topk;
     const NmsScratch sc = bind_nms_scratch(nullptr, B, cap, num_classes);
     return static_cast<size_t>(reinterpret_cast<uintptr_t>(sc.mask)) /* offset: bound at address 0 */ +
            up256(static_cast<size_t>(B) * sc.capP * sc.W * 8);
 }
 
 cudaError_t launch_nms(const NmsParams& p, cudaStream_t stream) {
-    const int cap = kLevels * p.topk;
-    if (p.topk > kMaxPreNmsTopk || p.B <= 0) return cudaErrorInvalidValue;
+    const int cap = p.num_levels * p.topk;
+    if (p.topk > kMaxPreNmsTopk || p.B <= 0 || p.num_levels < 1 || p.num_levels > kLevels) return cudaErrorInvalidValue;
     const size_t smem = nms_smem_bytes(cap);  // key 8 + val 2 per sort entry; box 16 + list 4 + list2 4 + cls 1 + flag 1
     const size_t smem_sort = static_cast<size_t>(cap) * (8 + 2 + 1) + 16;
     static size_t attr_smem_dev[64] = {};  // per device; the limit is 227 KiB minus the static shared memory: ask for what we use

@@ -77,7 +77,7 @@ __global__ void __launch_bounds__(kMarkThreads) tower_mark_kernel(const __grid_c
     int l = 0;
 #pragma unroll
     for (int i = 1; i < kLevels; ++i)
-        if (static_cast<int>(blockIdx.x) >= p.lvl[i].mark_begin) l = i;
+        if (i < p.num_levels && static_cast<int>(blockIdx.x) >= p.lvl[i].mark_begin) l = i;
     const TowerTilesLevel& L = p.lvl[l];
     const int b = blockIdx.y;
     const int pix = (static_cast<int>(blockIdx.x) - L.mark_begin) * kMarkThreads + static_cast<int>(threadIdx.x);
@@ -103,7 +103,7 @@ __global__ void __launch_bounds__(kThreads) tower_tiles_kernel(const TowerTilesP
     if (p.fin != nullptr) {
         for (int t = threadIdx.x; t < T; t += kThreads) s_dist[t] = kTowerTileFar;
         __syncthreads();
-        const int bl = b * kLevels + l;  // fin / cand_count order
+        const int bl = b * p.num_levels + l;  // fin / cand_count order
         const int n = min(p.cand_count[bl], p.topk);
         for (int c = threadIdx.x; c < n; c += kThreads) {
             const int pix = static_cast<int>(p.fin[static_cast<size_t>(bl) * p.topk + c].y / static_cast<uint32_t>(p.C));
@@ -205,7 +205,7 @@ size_t tower_tiles_smem_bytes(int max_tiles) { return static_cast<size_t>(max_ti
 
 cudaError_t launch_tower_mark(const TowerTilesParams& p, cudaStream_t stream) {
     if (p.dist == nullptr || p.fin != nullptr || p.B < 1 || p.C < 1 || p.cls_pitch < p.C || p.cls_pitch % 4 ||
-        p.mark_blocks < 1 || p.reach < 0)
+        p.mark_blocks < 1 || p.reach < 0 || p.num_levels < 1 || p.num_levels > kLevels)
         return cudaErrorInvalidValue;
     return launch_pdl(tower_mark_kernel, dim3(p.mark_blocks, p.B), dim3(kMarkThreads), 0, stream, p);
 }
@@ -213,9 +213,9 @@ cudaError_t launch_tower_mark(const TowerTilesParams& p, cudaStream_t stream) {
 cudaError_t launch_tower_tiles(const TowerTilesParams& p, cudaStream_t stream) {
     if (p.depth < 1 || p.reach < p.depth - 1 || p.B < 1 || p.B > kTileListMaxImages || p.C < 1 ||
         (p.fin != nullptr ? p.topk < 1 : p.dist == nullptr) || p.max_tiles >= kTileListMaxTiles ||
-        tower_tiles_smem_bytes(p.max_tiles) > 48 * 1024)
+        tower_tiles_smem_bytes(p.max_tiles) > 48 * 1024 || p.num_levels < 1 || p.num_levels > kLevels)
         return cudaErrorInvalidValue;
-    return launch_pdl(tower_tiles_kernel, dim3(kLevels * p.B), dim3(kThreads), tower_tiles_smem_bytes(p.max_tiles), stream, p);
+    return launch_pdl(tower_tiles_kernel, dim3(p.num_levels * p.B), dim3(kThreads), tower_tiles_smem_bytes(p.max_tiles), stream, p);
 }
 
 }  // namespace dd3d

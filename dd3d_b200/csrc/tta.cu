@@ -96,6 +96,7 @@ cudaError_t launch_tta_merge(const Det* dets, const int32_t* counts, const TtaVi
     np.out_count = out_count;
     np.flags = flags;
     np.B = 1;
+    np.num_levels = kLevels;
     np.topk = total;
     np.out_cap = total;
     np.do_nms = do_nms;

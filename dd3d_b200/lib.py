@@ -90,6 +90,7 @@ SIGNATURES = {
     "dd3d_set_backbone_norm": (_I, [_P, C.c_int32]),
     "dd3d_set_fpn_channels": (_I, [_P, C.c_int32]),
     "dd3d_set_canonical_sizes": (_I, [_P, C.c_int32, C.POINTER(C.c_float)]),
+    "dd3d_set_in_features": (_I, [_P, C.POINTER(C.c_int32), _I]),
     "dd3d_load_weight": (_I, [_P, C.c_char_p, _P, C.POINTER(_I64), _I]),
     "dd3d_finalize": (_I, [_P]),
     "dd3d_workspace_bytes": (_I64, [_P, _I, _I, _I]),
@@ -228,12 +229,28 @@ def desc_from_cfg(cfg, out_cap=None):
         for k in range(3):
             d.canonical_box3d_sizes[c * 3 + k] = sizes[c][k]
     if out_cap is None:
-        out_cap = ((inf.POST_NMS_TOPK + 28 + 31) // 32 * 32) if cfg.DD3D.INFERENCE.DO_NMS else 5 * inf.PRE_NMS_TOPK
+        out_cap = ((inf.POST_NMS_TOPK + 28 + 31) // 32 * 32) if cfg.DD3D.INFERENCE.DO_NMS else max_candidates(cfg)
     d.out_cap = out_cap
     from .arch import is_nuscenes_arch
     d.nuscenes_heads = int(is_nuscenes_arch(cfg))
     d.act_dtype = act_dtype_of(cfg)
     return d
+
+
+def max_candidates(cfg):
+    """Detections one image can have before the 2-D NMS: PRE_NMS_TOPK per head level (DD3D.IN_FEATURES)."""
+    from .arch import in_feature_levels
+    return len(in_feature_levels(cfg)) * int(cfg.DD3D.FCOS2D.INFERENCE.PRE_NMS_TOPK)
+
+
+def in_features_from_cfg(cfg):
+    """DD3D.IN_FEATURES as the int32 array of dd3d_set_in_features, or None for all five FPN outputs in order (the default
+    graph, which needs no call)."""
+    from .arch import in_feature_levels
+    levels = in_feature_levels(cfg)
+    if levels == list(range(5)):
+        return None
+    return (C.c_int32 * len(levels))(*levels), len(levels)
 
 
 def canonical_sizes_from_cfg(cfg):

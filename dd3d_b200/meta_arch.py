@@ -51,6 +51,7 @@ class DD3DB200(nn.Module):
         self._device = torch.device("cpu")
         self._desc = _lib.desc_from_cfg(cfg)
         self._layout = _lib.layout_from_cfg(cfg)
+        self._in_features = _lib.in_features_from_cfg(cfg)  # KeyError / NotImplementedError for lists the engine cannot run
         if cfg.DD3D.FCOS2D.USE_DEFORMABLE or (cfg.MODEL.BOX3D_ON and cfg.DD3D.FCOS3D.USE_DEFORMABLE):
             raise ValueError("Not supported yet.")  # fcos2d.py:51-52, fcos3d.py:77-78
         # param_specs raised the reference's errors for the FE.BACKBONE.NORM values it cannot build
@@ -137,6 +138,8 @@ class DD3DB200(nn.Module):
             _lib.check(L.dd3d_set_layout(handle, C.byref(self._layout)), handle)
             _lib.check(L.dd3d_set_backbone_norm(handle, self._backbone_norm), handle)
             _lib.check(L.dd3d_set_fpn_channels(handle, self._fpn_channels), handle)
+            if self._in_features is not None:
+                _lib.check(L.dd3d_set_in_features(handle, *self._in_features), handle)
             if self._canon is not None:
                 _lib.check(L.dd3d_set_canonical_sizes(handle, self.num_classes, self._canon), handle)
             for name, t in self._state.items():
@@ -163,13 +166,13 @@ class DD3DB200(nn.Module):
     def _sync_options(self, postprocess_in_forward):
         """Pushes the attributes callers toggle at run time (postprocess_in_inference, do_nms, do_bev_nms:
         scripts/train.py:206-209, core.py:134-137) to the engine.  Without NMS (or without a post-NMS top-k) up to
-        5 * PRE_NMS_TOPK detections per image survive: an engine planned with the small NMS-sized output buffer is rebuilt
+        L * PRE_NMS_TOPK detections per image survive (L head levels): an engine planned with the small NMS-sized output buffer is rebuilt
         with the large one instead of silently truncating (the reference never truncates).  With do_bev_nms the engine
         runs the BEV NMS as its last op, then detector_postprocess (core.py:137-160)."""
         inf = self.cfg.DD3D.FCOS2D.INFERENCE
         if self.do_bev_nms and self.only_box2d:
             self.do_bev_nms = False  # core.py:137: the BEV NMS needs the 3-D boxes
-        need = 5 * inf.PRE_NMS_TOPK if (not self.do_nms or inf.POST_NMS_TOPK <= 0) else 0
+        need = _lib.max_candidates(self.cfg) if (not self.do_nms or inf.POST_NMS_TOPK <= 0) else 0
         if need > self._desc.out_cap:
             self._release()
             self._desc.out_cap = need

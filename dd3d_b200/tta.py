@@ -83,24 +83,25 @@ class _DeviceTTA(nn.Module):
         return bool(model.do_bev_nms) and not model.only_box2d
 
     def per_view_bound(self):
-        """Detections one view can contribute: POST_NMS_TOPK after the 2-D NMS, else every 5 * PRE_NMS_TOPK candidate."""
+        """Detections one view can contribute: POST_NMS_TOPK after the 2-D NMS, else every candidate, PRE_NMS_TOPK per head
+        level (DD3D.IN_FEATURES)."""
         inf = self.cfg.DD3D.FCOS2D.INFERENCE
         if self.model.do_nms and inf.POST_NMS_TOPK > 0:
             return int(inf.POST_NMS_TOPK)
-        return 5 * int(inf.PRE_NMS_TOPK)
+        return _lib.max_candidates(self.cfg)
 
     def large_path(self):
         """True when the merged sets need the large-set ops (csrc/tta_large.cu): more merged detections than the
-        dd3d_op_tta_merge slots (TTA_MERGED_MAX), or DO_BEV_NMS without DO_NMS (unsorted views of up to 5 * PRE_NMS_TOPK
+        dd3d_op_tta_merge slots (TTA_MERGED_MAX), or DO_BEV_NMS without DO_NMS (unsorted views of up to L * PRE_NMS_TOPK
         boxes).  Read from the config and the model's switches only; the shipped configurations keep the one-CTA ops."""
         bev_alone = self._do_bev_nms() and not self.model.do_nms
         return self.num_views * self.per_view_bound() > TTA_MERGED_MAX or bev_alone
 
     def _fit_out_cap(self):
-        """Without the 2-D NMS (or its top-k) every view may return 5 * PRE_NMS_TOPK candidates: grow the engine's output
+        """Without the 2-D NMS (or its top-k) every view may return L * PRE_NMS_TOPK candidates: grow the engine's output
         buffer to that (the rule of DD3DB200._sync_options) without touching its other options, so the plans stay."""
         model, inf = self.model, self.cfg.DD3D.FCOS2D.INFERENCE
-        need = 5 * inf.PRE_NMS_TOPK if (not model.do_nms or inf.POST_NMS_TOPK <= 0) else 0
+        need = _lib.max_candidates(self.cfg) if (not model.do_nms or inf.POST_NMS_TOPK <= 0) else 0
         if need > model._desc.out_cap:
             model._release()
             model._desc.out_cap = need

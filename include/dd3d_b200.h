@@ -176,6 +176,14 @@ int dd3d_set_fpn_channels(dd3d_handle h, int32_t channels);
  * replaces them.  Class-specific heads above 16 classes run the box3d predictor at the final candidates only, 11 channels
  * each, on the class-gathered kernel (csrc/b3d_gather.cu) under the "sparse_box3d" rule of dd3d_set_option. */
 int dd3d_set_canonical_sizes(dd3d_handle h, int32_t num_classes, const float* h_sizes);
+/* Sets DD3D.IN_FEATURES before dd3d_finalize (DD3D_ERR_STATE afterwards): h_fpn_levels[0 .. n) are the FPN outputs the heads
+ * run on, in head order, as indices 0..4 into the FPN's outputs (DLA: p3..p7, VoVNet: p2..p6), 1 <= n <= DD3D_NUM_LEVELS,
+ * no index twice (DD3D_ERR_INVALID otherwise, leaving the selection unchanged).  Every per-level tensor is taken by position:
+ * tower norm l, Scale l, Offset l and (PER_LEVEL_PREDICTORS) predictor l serve the head at position l, and dd3d_det.level is
+ * the position.  FPN outputs no head reads are not computed (dd3d_get_tensor refuses their "p<i>"); the head maps
+ * "cls<l>" / "box<l>" / "b3d<l>" are by position.  Without DO_NMS up to n * pre_nms_topk detections per image survive.  An
+ * engine that never receives the call runs all five levels in order. */
+int dd3d_set_in_features(dd3d_handle h, const int32_t* h_fpn_levels, int n);
 
 /* ---- weights: one call per tensor of the reference state_dict (Checkpointer.load, scripts/train.py:52) ----- */
 /* h_data: host fp32, contiguous, `ndim` dims in h_shape.  Unknown names are ignored (return DD3D_OK, e.g.
