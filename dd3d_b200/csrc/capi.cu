@@ -125,7 +125,7 @@ int dd3d_forward(dd3d_handle h, const void* d_images, int img_dtype, const float
     if (!d_images || !d_intrinsics || !d_sizes || !d_out || !d_counts) return DD3D_ERR_INVALID;
     return guarded(h, [&](Engine& e) {
         e.forward(d_images, img_dtype, d_intrinsics, d_sizes, reinterpret_cast<Det*>(d_out), d_counts, e.user_poses,
-                  static_cast<cudaStream_t>(stream));
+                  e.device_agg_args(), static_cast<cudaStream_t>(stream));
     });
 }
 
@@ -281,6 +281,40 @@ int dd3d_set_host_poses(dd3d_handle h, int slot, const float* h_poses) {
 int dd3d_bev_nms_path(const dd3d_model_desc* h_desc) {
     if (!h_desc) return DD3D_ERR_INVALID;
     return bev_nms_path(h_desc->do_nms, h_desc->post_nms_topk);
+}
+
+int dd3d_set_sample_aggregate(dd3d_handle h, int enable, float iou_thresh, int max_dets) {
+    return guarded(h, [&](Engine& e) { e.set_sample_aggregate(enable, iou_thresh, max_dets); });
+}
+
+int dd3d_set_groups(dd3d_handle h, const int32_t* d_group, int num_groups) {
+    if (d_group && num_groups < 1) return DD3D_ERR_INVALID;
+    return guarded(h, [&](Engine& e) {
+        e.user_groups = d_group;
+        e.user_num_groups = d_group ? num_groups : 0;
+    });
+}
+
+int dd3d_set_host_groups(dd3d_handle h, int slot, const int32_t* h_group, int num_groups) {
+    if (!h_group) return DD3D_ERR_INVALID;
+    return guarded(h, [&](Engine& e) { e.set_host_groups(slot, h_group, num_groups); });
+}
+
+int dd3d_set_global_out(dd3d_handle h, float* d_global) {
+    return guarded(h, [&](Engine& e) { e.user_global = d_global; });
+}
+
+int dd3d_set_host_global_out(dd3d_handle h, int slot, float* h_global) {
+    return guarded(h, [&](Engine& e) {
+        if (slot < 0 || slot > 1) throw EngineError(DD3D_ERR_INVALID, "slot must be 0 or 1");
+        if (e.slot_busy[slot]) throw EngineError(DD3D_ERR_STATE, "slot has a pending dd3d_submit_host");
+        e.host_global[slot] = h_global;
+    });
+}
+
+int dd3d_sample_aggregate_path(const dd3d_model_desc* h_desc) {
+    if (!h_desc) return DD3D_ERR_INVALID;
+    return sample_aggregate_path(h_desc->do_nms, h_desc->post_nms_topk, h_desc->out_cap);
 }
 
 int dd3d_num_ops(dd3d_handle h) {

@@ -2,7 +2,8 @@
 //
 // Replaces detectron2 comm.gather of pickled prediction lists in the reference evaluators
 // (tridet/evaluators/kitti_3d_evaluator.py:152-164, nuscenes_evaluator.py:255): every rank contributes its fixed-stride
-// buffer  [B][out_cap] dd3d_det | counts[B] | flags[1]  (dd3d_packed_bytes) and receives all ranks' buffers.  Images are
+// buffer  [B][out_cap] dd3d_det | counts[B] | flags[1]  (dd3d_packed_bytes; NuscenesDD3D appends the pred_boxes3d_global
+// rows [B][out_cap][10] of its sample aggregation, dd3d_packed_bytes_global) and receives all ranks' buffers.  Images are
 // independent (eval BN, per-image NMS), so this is the only exchange of the path (SURVEY.md 8e); 295 KB per rank at
 // B = 32 -- latency, not bandwidth, so it is issued on a side stream and overlaps the next batch's forward.
 //
@@ -85,6 +86,13 @@ int64_t dd3d_packed_bytes(int B, int out_cap) {
     const int64_t dets = static_cast<int64_t>(B) * out_cap * static_cast<int64_t>(sizeof(dd3d_det));
     const int64_t tail = (static_cast<int64_t>(B + 1) * 4 + 255) / 256 * 256;  // counts[B] + flags[1], padded
     return dets + tail;
+}
+
+int64_t dd3d_packed_bytes_global(int B, int out_cap) {
+    const int64_t head = dd3d_packed_bytes(B, out_cap);
+    if (head < 0) return head;
+    const int64_t global = (static_cast<int64_t>(B) * out_cap * 10 * 4 + 255) / 256 * 256;  // float [B][out_cap][10], padded
+    return head + global;
 }
 
 const char* dd3d_comm_last_error(void) { return g_comm_error.c_str(); }

@@ -228,5 +228,22 @@ cudaError_t launch_group_bev_nms_large(Det* dets, int32_t* counts, const float* 
                                        int pose_mode, const int32_t* group, int num_groups, int max_group_images,
                                        float* global, void* scratch, int32_t* flags, int B, int cap, float thr,
                                        int max_dets, cudaStream_t stream);
+// Kernels launch_group_bev_nms_large enqueues for these arguments (the radix sort's pass count follows num_groups).
+int group_bev_nms_large_launches(int num_groups);
+constexpr int kGroupBevNmsLargeMaxB = 256;          // images per call of launch_group_bev_nms_large
+constexpr int kGroupBevNmsLargeGroupImages = 16;    // images per group it holds
+
+// NuscenesDD3D sample aggregation as a step of the forward (Engine::set_sample_aggregate).  The one-CTA pair of
+// launch_sample_aggregate holds kSampleAggOneCtaTopk boxes of each of 6 cameras (its 768-box group) and out_cap <=
+// kBevNmsMax slots: the 2-D NMS output with 0 < POST_NMS_TOPK <= 128.  Every other configuration -- DO_NMS off (all
+// L * PRE_NMS_TOPK candidates per image) or a larger top-k -- runs the blocked kernels of launch_group_bev_nms_large in
+// global pose mode, up to 6 * 5 * 1150 = 34 500 boxes per sample.
+constexpr int kSampleAggOneCtaTopk = 128;
+constexpr int kAggPathOneCta = 1, kAggPathBlocked = 2;
+inline int sample_aggregate_path(int do_nms, int post_nms_topk, int out_cap) {
+    return (do_nms && post_nms_topk > 0 && post_nms_topk <= kSampleAggOneCtaTopk && out_cap <= kBevNmsMax) ? kAggPathOneCta
+                                                                                                       : kAggPathBlocked;
+}
+constexpr int kSampleAggOneCtaLaunches = 2;  // sample_nms_kernel + sample_compact_kernel
 
 }  // namespace dd3d

@@ -1641,8 +1641,19 @@ size_t Engine::build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry) 
         P->d_images = bld.alloc_bytes(static_cast<size_t>(B) * 3 * Hs * Ws * 4);
         P->d_canon = nullptr;
         P->bev = bev_mode();
-        if (P->bev) P->d_poses = static_cast<float*>(bld.alloc_bytes(static_cast<size_t>(B) * 7 * 4));
+        P->agg = agg_mode();
+        if (P->bev || P->agg) P->d_poses = static_cast<float*>(bld.alloc_bytes(static_cast<size_t>(B) * 7 * 4));
         if (P->bev == kBevPathMultiCta) P->bev_scratch = bld.alloc_bytes(image_bev_nms_scratch_bytes(B, desc.out_cap, desc.num_classes));
+        if (P->agg) {
+            if (P->agg == kAggPathBlocked && B > kGroupBevNmsLargeMaxB)
+                fail(DD3D_ERR_INVALID, "the blocked sample aggregation holds at most " + std::to_string(kGroupBevNmsLargeMaxB) +
+                                           " images per call, plan has " + std::to_string(B));
+            P->d_group = static_cast<int32_t*>(bld.alloc_bytes(static_cast<size_t>(B) * 4));
+            P->d_global = static_cast<float*>(bld.alloc_bytes(static_cast<size_t>(B) * desc.out_cap * 10 * 4));
+            P->agg_scratch = bld.alloc_bytes(P->agg == kAggPathOneCta
+                                                 ? sample_aggregate_scratch_bytes(B, desc.out_cap)
+                                                 : group_bev_nms_large_scratch_bytes(B, desc.out_cap, kGroupBevNmsLargeGroupImages));
+        }
         if (tracing) {
             arena_bytes = plan_arena(bufs, opt_workspace_reuse != 0);
             total = arena_bytes + bld.off;
@@ -1812,6 +1823,10 @@ void Engine::plan_steps(Plan* P) {
     add(Step::NMS, 7, nms_launches(P->nms) + (P->bev == kBevPathOneCta     ? kOneLaunch
                                               : P->bev == kBevPathMultiCta ? image_bev_nms_launches(P->B) : 0))
         .bev = P->bev;
+    // the blocked kernels run with one group per image of the call (num_groups = B), so their launches follow the plan
+    if (P->agg)
+        add(Step::AGGREGATE, 7, P->agg == kAggPathOneCta ? kSampleAggOneCtaLaunches : group_bev_nms_large_launches(P->B)).agg =
+            P->agg;
 }
 
 void fill_decode_params(DecodeParams* dp, const dd3d_model_desc& desc, int B, int cls_pitch, int b3d_pitch,
@@ -1861,6 +1876,7 @@ int Engine::bev_mode() const { return opt_bev_nms ? bev_nms_path(desc.do_nms, de
 void Engine::set_do_nms(int do_nms) {
     if (do_nms == desc.do_nms) return;
     if (bev_mode() && bev_nms_path(do_nms, desc.post_nms_topk) != bev_mode()) drop_plans();  // BEV kernel changes
+    if (agg_mode() && sample_aggregate_path(do_nms, desc.post_nms_topk, desc.out_cap) != agg_mode()) drop_plans();
     desc.do_nms = do_nms;
     if (plan.valid) plan_steps(&plan);
     for (auto& kv : plan_cache) plan_steps(&kv.second);
@@ -1875,6 +1891,28 @@ void Engine::set_bev_nms(int enable, float thr) {
     if (after != bev_mode()) drop_plans();
     opt_bev_nms = enable ? 1 : 0;
     bev_nms_thresh = thr;
+}
+
+int Engine::agg_mode() const {
+    return opt_sample_agg ? sample_aggregate_path(desc.do_nms, desc.post_nms_topk, desc.out_cap) : 0;
+}
+
+void Engine::set_sample_aggregate(int enable, float thr, int max_dets) {
+    if (enable && !desc.box3d_on) fail(DD3D_ERR_INVALID, "the sample aggregation needs the 3-D head (box3d_on)");
+    if (!(thr == thr)) fail(DD3D_ERR_INVALID, "sample aggregation IoU threshold is NaN");
+    const int after = enable ? sample_aggregate_path(desc.do_nms, desc.post_nms_topk, desc.out_cap) : 0;
+    if (after != agg_mode()) drop_plans();  // the step list and the workspace change (as set_bev_nms)
+    opt_sample_agg = enable ? 1 : 0;
+    agg_thresh = thr;
+    agg_max_dets = max_dets;
+}
+
+void Engine::set_host_groups(int slot, const int32_t* h_group, int num_groups) {
+    if (!plan.valid) fail(DD3D_ERR_STATE, "set_host_groups before plan");
+    if (slot < 0 || slot > 1) fail(DD3D_ERR_INVALID, "slot must be 0 or 1");
+    if (num_groups < 1 || num_groups > plan.B) fail(DD3D_ERR_INVALID, "num_groups must be in 1..B");
+    host_groups[slot].assign(h_group, h_group + plan.B);
+    host_num_groups[slot] = num_groups;
 }
 
 void Engine::set_host_poses(int slot, const float* h_poses) {
@@ -1932,15 +1970,21 @@ void Engine::forward_resized(const uint8_t* d_raw, int raw_h, int raw_w, const i
     cuda_check(cudaMemcpyAsync(P.d_sizes, h_sizes4, static_cast<size_t>(P.B) * 16, cudaMemcpyHostToDevice, stream),
                "H2D sizes");
     const RawArgs raw = {d_raw, raw_h, raw_w, h_raw_sizes, h_new_sizes, h_flip};
-    forward(nullptr, DD3D_IMG_U8, P.d_K, P.d_sizes, d_out, d_counts, user_poses, stream, &raw);
+    forward(nullptr, DD3D_IMG_U8, P.d_K, P.d_sizes, d_out, d_counts, user_poses, device_agg_args(), stream, &raw);
 }
 
 void Engine::forward(const void* d_images, int img_dtype, const float* d_K, const int32_t* d_sizes, Det* d_out,
-                     int32_t* d_counts, const float* d_poses, cudaStream_t stream, const RawArgs* raw) {
+                     int32_t* d_counts, const float* d_poses, const AggArgs& agg, cudaStream_t stream, const RawArgs* raw) {
     if (!plan.valid) fail(DD3D_ERR_STATE, "forward before plan");
     const Plan& P = plan;
     if (P.bev && d_poses == nullptr)
         fail(DD3D_ERR_STATE, "BEV NMS is on: the forward needs the poses (dd3d_set_poses / dd3d_set_host_poses)");
+    if (P.agg) {
+        if (d_poses == nullptr || agg.d_group == nullptr || agg.d_global == nullptr)
+            fail(DD3D_ERR_STATE, "sample aggregation is on: the forward needs the poses, the group indices and the global rows "
+                                 "(dd3d_set_poses / dd3d_set_groups / dd3d_set_global_out or their host forms)");
+        if (agg.num_groups < 1 || agg.num_groups > P.B) fail(DD3D_ERR_INVALID, "num_groups must be in 1..B");
+    }
     size_t ev_i = 0;
     auto mark = [&](int cat, int op) {  // opt_profile: CUDA events on the launch stream around every step
         if (!opt_profile) return;
@@ -2012,6 +2056,19 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
                                "bev nms (multi-CTA)");
                 break;
             }
+            case Step::AGGREGATE:  // in place on the detector_postprocess'ed detections, like the reference's order
+                if (s.agg == kAggPathOneCta)
+                    cuda_check(launch_sample_aggregate(d_out, d_counts, d_K, d_poses, agg.d_group, agg.num_groups,
+                                                       agg.d_global, P.agg_scratch, P.decode.flags, P.B, desc.out_cap,
+                                                       agg_thresh, agg_max_dets, stream),
+                               "sample aggregation");
+                else
+                    cuda_check(launch_group_bev_nms_large(d_out, d_counts, d_K, 1, d_poses, 0, agg.d_group, P.B,
+                                                          kGroupBevNmsLargeGroupImages, agg.d_global, P.agg_scratch,
+                                                          P.decode.flags, P.B, desc.out_cap, agg_thresh, agg_max_dets,
+                                                          stream),
+                               "sample aggregation (blocked)");
+                break;
         }
         mark(s.cat, s.op);
     }
@@ -2142,20 +2199,30 @@ void Engine::forward_host(const void* h_images, int img_dtype, const float* h_K,
                           int32_t* h_counts, cudaStream_t stream) {
     if (!plan.valid) fail(DD3D_ERR_STATE, "forward before plan");
     const Plan& P = plan;
+    check_host_agg(0);
     const size_t img_bytes = static_cast<size_t>(P.B) * 3 * P.Hs * P.Ws * (img_dtype == DD3D_IMG_U8 ? 1 : 4);
     cuda_check(cudaMemcpyAsync(P.d_images, h_images, img_bytes, cudaMemcpyHostToDevice, stream), "H2D images");
     cuda_check(cudaMemcpyAsync(P.d_K, h_K, static_cast<size_t>(P.B) * 36, cudaMemcpyHostToDevice, stream), "H2D K");
     cuda_check(cudaMemcpyAsync(P.d_sizes, h_sizes, static_cast<size_t>(P.B) * 16, cudaMemcpyHostToDevice, stream),
                "H2D sizes");
-    if (P.bev) {
-        if (host_poses[0].size() != static_cast<size_t>(P.B) * 7) fail(DD3D_ERR_STATE, "BEV NMS is on: dd3d_set_host_poses(0, ...) first");
+    if (P.bev || P.agg) {
+        if (host_poses[0].size() != static_cast<size_t>(P.B) * 7)
+            fail(DD3D_ERR_STATE, std::string(P.bev ? "BEV NMS" : "sample aggregation") + " is on: dd3d_set_host_poses(0, ...) first");
         cuda_check(cudaMemcpyAsync(P.d_poses, host_poses[0].data(), host_poses[0].size() * 4, cudaMemcpyHostToDevice, stream),
                    "H2D poses");
     }
-    forward(P.d_images, img_dtype, P.d_K, P.d_sizes, P.d_out, P.d_counts, P.d_poses, stream);
+    if (P.agg)
+        cuda_check(cudaMemcpyAsync(P.d_group, host_groups[0].data(), host_groups[0].size() * 4, cudaMemcpyHostToDevice, stream),
+                   "H2D groups");
+    forward(P.d_images, img_dtype, P.d_K, P.d_sizes, P.d_out, P.d_counts, P.d_poses, {P.d_group, host_num_groups[0], P.d_global},
+            stream);
     cuda_check(cudaMemcpyAsync(h_out, P.d_out, static_cast<size_t>(P.B) * desc.out_cap * sizeof(Det),
                                cudaMemcpyDeviceToHost, stream),
                "D2H dets");
+    if (P.agg)
+        cuda_check(cudaMemcpyAsync(host_global[0], P.d_global, static_cast<size_t>(P.B) * desc.out_cap * 40,
+                                   cudaMemcpyDeviceToHost, stream),
+                   "D2H global rows");
     cuda_check(cudaMemcpyAsync(h_counts, P.d_counts, static_cast<size_t>(P.B) * 4, cudaMemcpyDeviceToHost, stream),
                "D2H counts");
     cuda_check(cudaStreamSynchronize(stream), "sync");
@@ -2182,7 +2249,9 @@ void Engine::submit_host(int slot, const void* h_images, int img_dtype, const fl
     if (slot == 1 && P.slot1 == nullptr) {
         const size_t a = 1024;
         auto up = [&](size_t n) { return (n + a - 1) / a * a; };
-        const size_t total = up(img_cap) + up(P.B * 36) + up(P.B * 16) + up(out_bytes) + up(P.B * 4) + (P.bev ? up(P.B * 28) : 0);
+        const size_t glob_bytes = static_cast<size_t>(P.B) * desc.out_cap * 40;
+        const size_t total = up(img_cap) + up(P.B * 36) + up(P.B * 16) + up(out_bytes) + up(P.B * 4) +
+                             (P.bev || P.agg ? up(P.B * 28) : 0) + (P.agg ? up(P.B * 4) + up(glob_bytes) : 0);
         cuda_check(cudaMalloc(&P.slot1, total), "cudaMalloc(slot 1 staging)");
         uint8_t* q = static_cast<uint8_t*>(P.slot1);
         P.s1_images = q; q += up(img_cap);
@@ -2190,7 +2259,13 @@ void Engine::submit_host(int slot, const void* h_images, int img_dtype, const fl
         P.s1_sizes = reinterpret_cast<int32_t*>(q); q += up(P.B * 16);
         P.s1_out = reinterpret_cast<Det*>(q); q += up(out_bytes);
         P.s1_counts = reinterpret_cast<int32_t*>(q); q += up(P.B * 4);
-        if (P.bev) P.s1_poses = reinterpret_cast<float*>(q);
+        if (P.bev || P.agg) {
+            P.s1_poses = reinterpret_cast<float*>(q); q += up(P.B * 28);
+        }
+        if (P.agg) {
+            P.s1_group = reinterpret_cast<int32_t*>(q); q += up(P.B * 4);
+            P.s1_global = reinterpret_cast<float*>(q);
+        }
     }
     void* d_img = slot ? P.s1_images : P.d_images;
     float* d_K = slot ? P.s1_K : P.d_K;
@@ -2198,23 +2273,43 @@ void Engine::submit_host(int slot, const void* h_images, int img_dtype, const fl
     Det* d_out = slot ? P.s1_out : P.d_out;
     int32_t* d_cnt = slot ? P.s1_counts : P.d_counts;
     float* d_poses = slot ? P.s1_poses : P.d_poses;
-    if (P.bev && host_poses[slot].size() != static_cast<size_t>(P.B) * 7)
-        fail(DD3D_ERR_STATE, "BEV NMS is on: dd3d_set_host_poses(slot, ...) first");
+    int32_t* d_group = slot ? P.s1_group : P.d_group;
+    float* d_global = slot ? P.s1_global : P.d_global;
+    if ((P.bev || P.agg) && host_poses[slot].size() != static_cast<size_t>(P.B) * 7)
+        fail(DD3D_ERR_STATE, std::string(P.bev ? "BEV NMS" : "sample aggregation") + " is on: dd3d_set_host_poses(slot, ...) first");
+    check_host_agg(slot);
     const size_t img_bytes = static_cast<size_t>(P.B) * 3 * P.Hs * P.Ws * (img_dtype == DD3D_IMG_U8 ? 1 : 4);
     cuda_check(cudaMemcpyAsync(d_img, h_images, img_bytes, cudaMemcpyHostToDevice, copy_stream), "H2D images");
     cuda_check(cudaMemcpyAsync(d_K, h_K, static_cast<size_t>(P.B) * 36, cudaMemcpyHostToDevice, copy_stream), "H2D K");
     cuda_check(cudaMemcpyAsync(d_sz, h_sizes, static_cast<size_t>(P.B) * 16, cudaMemcpyHostToDevice, copy_stream), "H2D sizes");
-    if (P.bev)  // pageable source: staged before the call returns, so the next dd3d_set_host_poses may overwrite it
+    if (P.bev || P.agg)  // pageable source: staged before the call returns, so the next dd3d_set_host_poses may overwrite it
         cuda_check(cudaMemcpyAsync(d_poses, host_poses[slot].data(), host_poses[slot].size() * 4, cudaMemcpyHostToDevice,
                                    copy_stream),
                    "H2D poses");
+    if (P.agg)  // pageable as well
+        cuda_check(cudaMemcpyAsync(d_group, host_groups[slot].data(), host_groups[slot].size() * 4, cudaMemcpyHostToDevice,
+                                   copy_stream),
+                   "H2D groups");
     cuda_check(cudaEventRecord(h2d_done[slot], copy_stream), "cudaEventRecord");
     cuda_check(cudaStreamWaitEvent(stream, h2d_done[slot], 0), "cudaStreamWaitEvent");
-    forward(d_img, img_dtype, d_K, d_sz, d_out, d_cnt, d_poses, stream);
+    forward(d_img, img_dtype, d_K, d_sz, d_out, d_cnt, d_poses, {d_group, host_num_groups[slot], d_global}, stream);
     cuda_check(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, stream), "D2H dets");
+    if (P.agg)
+        cuda_check(cudaMemcpyAsync(host_global[slot], d_global, static_cast<size_t>(P.B) * desc.out_cap * 40,
+                                   cudaMemcpyDeviceToHost, stream),
+                   "D2H global rows");
     cuda_check(cudaMemcpyAsync(h_counts, d_cnt, static_cast<size_t>(P.B) * 4, cudaMemcpyDeviceToHost, stream), "D2H counts");
     cuda_check(cudaEventRecord(all_done[slot], stream), "cudaEventRecord");
     slot_busy[slot] = true;
+}
+
+// the host group indices and the global-row buffer of a host slot, before anything is enqueued
+void Engine::check_host_agg(int slot) const {
+    if (!plan.agg) return;
+    if (host_groups[slot].size() != static_cast<size_t>(plan.B))
+        fail(DD3D_ERR_STATE, "sample aggregation is on: dd3d_set_host_groups(" + std::to_string(slot) + ", ...) first");
+    if (host_global[slot] == nullptr)
+        fail(DD3D_ERR_STATE, "sample aggregation is on: dd3d_set_host_global_out(" + std::to_string(slot) + ", ...) first");
 }
 
 void Engine::wait_host(int slot) {

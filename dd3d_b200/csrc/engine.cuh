@@ -132,6 +132,7 @@ struct Step {
         BOX3D_TILES,  // sparse box3d tower: decode threshold / top-k + tile lists around the final candidates
         DETECT,       // [decode threshold / top-k] [sparse or gathered box3d predictor] decode of the final candidates
         NMS,          // NMS [+ BEV NMS]
+        AGGREGATE,    // NuscenesDD3D sample aggregation over the call's images (after detector_postprocess)
     } kind;
     int op = -1;        // OP: index into Plan::ops, else -1
     int cat = 0;        // profile category (Engine::get_profile)
@@ -140,6 +141,7 @@ struct Step {
     bool select = false;  // DETECT: the threshold / top-k half runs here (no BOX3D_TILES step ran it)
     int b3d = 0;          // DETECT: box3d predictor at the final candidates: 0 none (dense maps), kB3dSparse, kB3dGathered
     int bev = 0;          // NMS: 0, or the bev_nms_path() of the BEV NMS that follows
+    int agg = 0;          // AGGREGATE: the sample_aggregate_path() it runs
     static constexpr int kB3dSparse = 1, kB3dGathered = 2;
 };
 
@@ -155,7 +157,9 @@ struct Plan {
     int32_t* s1_sizes = nullptr;
     Det* s1_out = nullptr;
     int32_t* s1_counts = nullptr;
-    float* s1_poses = nullptr;  // BEV NMS on: slot 1's copy of the host poses
+    float* s1_poses = nullptr;  // BEV NMS or sample aggregation on: slot 1's copy of the host poses
+    int32_t* s1_group = nullptr;  // sample aggregation on: slot 1's copy of the host group indices
+    float* s1_global = nullptr;   // and its pred_boxes3d_global rows [B][out_cap][10]
     View input;
     View fpn[kLevels];  // by FPN output index; an output no head reads is not built (null ptr)
     int num_levels = kLevels;  // head positions; the per-level arrays below are by position
@@ -179,6 +183,11 @@ struct Plan {
     int bev = 0;
     float* d_poses = nullptr;      // [B][7] staging of the host poses (host paths, slot 0)
     void* bev_scratch = nullptr;   // image_bev_nms_scratch_bytes(B, out_cap, num_classes) (multi-CTA path only)
+    // sample aggregation as the last step (dd3d_set_sample_aggregate): 0 off, else sample_aggregate_path() at plan time
+    int agg = 0;
+    int32_t* d_group = nullptr;   // [B] staging of the host group indices (host paths, slot 0)
+    float* d_global = nullptr;    // [B][out_cap][10] pred_boxes3d_global staging (host paths, slot 0)
+    void* agg_scratch = nullptr;  // sample_aggregate_scratch_bytes / group_bev_nms_large_scratch_bytes of the path
     // sparse FCOS3D predictor (b3d_sparse.cu): the fused box3d conv runs only at the final 2-D candidates, between the two
     // halves of the decode; the dense fp32 maps b3d_map[] then do not exist
     bool sparse_b3d = false;
@@ -224,8 +233,15 @@ class Engine {
         const int32_t* h_flip;
     };
     // d_poses: [B][7] poses the BEV NMS reads (unused when it is off); the preprocess reads `raw` when given, else d_images
+    // sample aggregation operands: [B] group indices of num_groups groups, [B][out_cap][10] pred_boxes3d_global rows
+    struct AggArgs {
+        const int32_t* d_group;
+        int num_groups;
+        float* d_global;
+    };
     void forward(const void* d_images, int img_dtype, const float* d_K, const int32_t* d_sizes, Det* d_out,
-                 int32_t* d_counts, const float* d_poses, cudaStream_t stream, const RawArgs* raw = nullptr);
+                 int32_t* d_counts, const float* d_poses, const AggArgs& agg, cudaStream_t stream,
+                 const RawArgs* raw = nullptr);
     void forward_host(const void* h_images, int img_dtype, const float* h_K, const int32_t* h_sizes, Det* h_out,
                       int32_t* h_counts, cudaStream_t stream);
     // double-buffered host path: H2D of one slot on a private copy stream while the other slot computes
@@ -249,6 +265,13 @@ class Engine {
     void set_bev_nms(int enable, float thr);
     int bev_mode() const;  // 0 off, else the bev_nms_path() the current options select
     void set_host_poses(int slot, const float* h_poses);
+    // NuscenesDD3D sample aggregation (dd3d_set_sample_aggregate) as the last step of every forward; its group indices and
+    // global rows: device (dd3d_set_groups / dd3d_set_global_out) and per host slot (dd3d_set_host_groups /
+    // dd3d_set_host_global_out)
+    void set_sample_aggregate(int enable, float thr, int max_dets);
+    int agg_mode() const;  // 0 off, else the sample_aggregate_path() the current options select
+    void set_host_groups(int slot, const int32_t* h_group, int num_groups);
+    AggArgs device_agg_args() const { return {user_groups, user_num_groups, user_global}; }
     // categories: 0 preprocess, 1 stem and depthwise conv, 2 conv (wgmma), 3 pool, 4 eSE, 5 relu and GroupNorm, 6 decode, 7 nms
     void get_profile(double* ms, double* flops, double* bytes, int32_t* launches);
     int get_op_times(float* ms, int32_t* cats, double* flops, int32_t* ops, int max_ops);  // ops may be null
@@ -314,6 +337,15 @@ class Engine {
     float bev_nms_thresh = 0.f;
     const float* user_poses = nullptr;   // dd3d_set_poses
     std::vector<float> host_poses[2];    // dd3d_set_host_poses, per slot
+    int opt_sample_agg = 0;
+    float agg_thresh = 0.f;
+    int agg_max_dets = 0;                 // <= 0: no cap
+    const int32_t* user_groups = nullptr;  // dd3d_set_groups
+    int user_num_groups = 0;
+    float* user_global = nullptr;          // dd3d_set_global_out
+    std::vector<int32_t> host_groups[2];   // dd3d_set_host_groups, per slot
+    int host_num_groups[2] = {0, 0};
+    float* host_global[2] = {nullptr, nullptr};  // dd3d_set_host_global_out, per slot
     std::vector<cudaEvent_t> prof_ev;
     std::vector<int> prof_cat;
     std::vector<int> prof_op;  // plan op that ends at event i, or -1
@@ -345,6 +377,7 @@ class Engine {
     float* upload_f32(const std::vector<float>& v);
     size_t build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry);
     void plan_steps(Plan* P);  // the NMS params and the step list of a built plan
+    void check_host_agg(int slot) const;
     void release_plan();
     static void free_plan(Plan* P);
     std::vector<double> op_flops();

@@ -812,6 +812,14 @@ cudaError_t launch_tta_merge_large(const Det* dets, const int32_t* counts, const
     return e;
 }
 
+static_assert(kTlMaxB == kGroupBevNmsLargeMaxB && kTlGroupImages == kGroupBevNmsLargeGroupImages, "detect.cuh limits");
+
+// layout + prep, the radix passes over (segment, score) keys, bounds, NMS, select, compact: what the launcher enqueues
+int group_bev_nms_large_launches(int num_groups) {
+    const int key_bits = 32 + bit_length(static_cast<unsigned>(num_groups * kTlMaxCls));
+    return 2 + 3 * ((key_bits + 7) / 8) + 4;
+}
+
 size_t group_bev_nms_large_scratch_bytes(int B, int cap, int max_group_images) {
     if (B < 1 || B > kTlMaxB || cap < 1 || cap > kTtaMaxViews * kLevels * kMaxPreNmsTopk || max_group_images < 1 ||
         max_group_images > kTlGroupImages)

@@ -6,7 +6,12 @@ Every rank owns one PACKED buffer (include/dd3d_b200.h dd3d_packed_bytes):
     dd3d_det[B][out_cap] | int32 counts[B] | int32 flags | pad to 256 B
 
 whose first two parts are handed to dd3d_forward as d_out / d_counts, so the detections, their counts and the overflow
-flags travel in a single fixed-size all-gather:
+flags travel in a single fixed-size all-gather.  NuscenesDD3D uses the extended layout (dd3d_packed_bytes_global), the same
+three parts at the same offsets followed by
+
+    float global[B][out_cap][10] | pad to 256 B
+
+the pred_boxes3d_global rows the engine's sample aggregation writes (dd3d_set_global_out), in the same collective:
   * on GPUs through the C ABI (dd3d_comm_* / dd3d_allgather = ncclAllGather, NCCL resolved at run time), on a SIDE stream
     ordered after the producing forward by an event -- the 295 KB exchange of batch k overlaps the forward of batch k+1 and
     no host synchronisation happens per step;
@@ -23,30 +28,44 @@ from . import lib as _lib
 
 class PackedDetections:
     """One packed per-rank buffer (uint8 storage) with typed views: .out [B, cap, 24] fp32, .counts [B] int32,
-    .flags [1] int32 (all aliases of .buf)."""
-    def __init__(self, B, cap, device, buf=None):
-        self.B, self.cap = int(B), int(cap)
-        self.nbytes = self.packed_bytes(B, cap)
+    .flags [1] int32 and, with with_global, .global_rows [B, cap, 10] fp32 (all aliases of .buf)."""
+    def __init__(self, B, cap, device, buf=None, with_global=False):
+        self.B, self.cap, self.with_global = int(B), int(cap), bool(with_global)
+        self.nbytes = self.packed_bytes(B, cap, with_global)
         self.buf = buf if buf is not None else torch.zeros(self.nbytes, dtype=torch.uint8, device=device)
         assert self.buf.numel() == self.nbytes and self.buf.dtype == torch.uint8
         det_bytes = self.B * self.cap * _lib.DET_WORDS * 4
         self.out = self.buf[:det_bytes].view(torch.float32).view(self.B, self.cap, _lib.DET_WORDS)
-        tail = self.buf[det_bytes:].view(torch.int32)
+        head = self.packed_bytes(B, cap)
+        tail = self.buf[det_bytes:head].view(torch.int32)
         self.counts = tail[:self.B]
         self.flags = tail[self.B:self.B + 1]
+        self.global_rows = None
+        if self.with_global:
+            glob_bytes = self.B * self.cap * _lib.GLOBAL_WORDS * 4
+            self.global_rows = self.buf[head:head + glob_bytes].view(torch.float32).view(self.B, self.cap, _lib.GLOBAL_WORDS)
 
     @staticmethod
-    def packed_bytes(B, cap):
+    def packed_bytes(B, cap, with_global=False):
+        """== dd3d_packed_bytes, or dd3d_packed_bytes_global with with_global (checked in the gather tests)."""
         det = int(B) * int(cap) * _lib.DET_WORDS * 4
-        return det + ((int(B) + 1) * 4 + 255) // 256 * 256  # == dd3d_packed_bytes (checked in tests/test_gather_gloo.py)
+        n = det + ((int(B) + 1) * 4 + 255) // 256 * 256
+        if with_global:
+            n += (int(B) * int(cap) * _lib.GLOBAL_WORDS * 4 + 255) // 256 * 256
+        return n
 
 
-def split_gathered(g_buf, world, B, cap):
-    """[world * packed_bytes] uint8 -> ([world*B, cap, 24] fp32, [world*B] int32 counts, [world] int32 flags)."""
-    n = PackedDetections.packed_bytes(B, cap)
-    parts = [PackedDetections(B, cap, g_buf.device, buf=g_buf[r * n:(r + 1) * n]) for r in range(world)]
-    return (torch.cat([p.out for p in parts], 0), torch.cat([p.counts for p in parts], 0),
-            torch.cat([p.flags for p in parts], 0))
+def split_gathered(g_buf, world, B, cap, with_global=False):
+    """[world * packed_bytes] uint8 -> ([world*B, cap, 24] fp32, [world*B] int32 counts, [world] int32 flags), and with
+    with_global the [world*B, cap, 10] fp32 global rows as a fourth element."""
+    n = PackedDetections.packed_bytes(B, cap, with_global)
+    parts = [PackedDetections(B, cap, g_buf.device, buf=g_buf[r * n:(r + 1) * n], with_global=with_global)
+             for r in range(world)]
+    res = (torch.cat([p.out for p in parts], 0), torch.cat([p.counts for p in parts], 0),
+           torch.cat([p.flags for p in parts], 0))
+    if with_global:
+        res += (torch.cat([p.global_rows for p in parts], 0), )
+    return res
 
 
 def unpack(g_out, g_cnt):
@@ -55,12 +74,14 @@ def unpack(g_out, g_cnt):
 
 
 class DetectionGatherer:
-    """All-gather of PackedDetections buffers.  device "cuda": NCCL through the C ABI on a side stream; "cpu": gloo."""
-    def __init__(self, B, cap, device, rank=None, world=None, group=None):
+    """All-gather of PackedDetections buffers.  device "cuda": NCCL through the C ABI on a side stream; "cpu": gloo.
+    with_global: the extended NuscenesDD3D layout, whose global rows travel in the same single collective."""
+    def __init__(self, B, cap, device, rank=None, world=None, group=None, with_global=False):
         self.B, self.cap, self.device, self.group = int(B), int(cap), torch.device(device), group
+        self.with_global = bool(with_global)
         self.rank = dist.get_rank(group) if rank is None else rank
         self.world = dist.get_world_size(group) if world is None else world
-        self.nbytes = PackedDetections.packed_bytes(B, cap)
+        self.nbytes = PackedDetections.packed_bytes(B, cap, with_global)
         self.comm = None
         self.side = None
         if self.device.type == "cuda":
@@ -105,12 +126,13 @@ class DetectionGatherer:
         return done
 
     def gather(self, packed, recv=None):
-        """Blocking convenience: returns (g_out, g_counts, g_flags) of all ranks."""
+        """Blocking convenience: returns (g_out, g_counts, g_flags) of all ranks, and g_global with with_global."""
+        assert packed.nbytes == self.nbytes, "packed buffer layout differs from the gatherer's"
         recv = recv if recv is not None else self.new_recv()
         done = self.gather_async(packed, recv)
         if done is not None:
             done.synchronize()
-        return split_gathered(recv, self.world, self.B, self.cap)
+        return split_gathered(recv, self.world, self.B, self.cap, self.with_global)
 
     def close(self):
         if self.comm is not None:

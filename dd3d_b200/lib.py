@@ -19,6 +19,8 @@ ARCH_IDS = {"dla34": ARCH_DLA34, "v2_99": ARCH_V2_99, "v2_19_slim_dw": 2, "v2_19
 IMG_U8, IMG_F32 = 0, 1
 ACT_BF16, ACT_FP16 = 0, 1
 POSE_GLOBAL, POSE_CAMERA = 0, 1
+AGG_PATH_ONE_CTA, AGG_PATH_BLOCKED = 1, 2  # dd3d_sample_aggregate_path
+GLOBAL_WORDS = 10  # pred_boxes3d_global row: quat (w, x, y, z), tvec, size
 NORM_BN_PER_LEVEL, NORM_BN_SHARED, NORM_GN, NORM_NONE = 0, 1, 2, 3  # dd3d_norm
 # NORM value -> dd3d_norm (get_norm's table: any other string raises KeyError like its dict lookup).  In a head tower BN /
 # FrozenBN are per level (ModuleListDial, fcos2d.py:73-80); the FPN's norms are one per conv, so every BN is "shared" there.
@@ -107,7 +109,14 @@ SIGNATURES = {
     "dd3d_set_poses": (_I, [_P, _P]),
     "dd3d_set_host_poses": (_I, [_P, _I, _P]),
     "dd3d_bev_nms_path": (_I, [C.POINTER(ModelDesc)]),
+    "dd3d_set_sample_aggregate": (_I, [_P, _I, C.c_float, _I]),
+    "dd3d_set_groups": (_I, [_P, _P, _I]),
+    "dd3d_set_host_groups": (_I, [_P, _I, _P, _I]),
+    "dd3d_set_global_out": (_I, [_P, _P]),
+    "dd3d_set_host_global_out": (_I, [_P, _I, _P]),
+    "dd3d_sample_aggregate_path": (_I, [C.POINTER(ModelDesc)]),
     "dd3d_packed_bytes": (_I64, [_I, _I]),
+    "dd3d_packed_bytes_global": (_I64, [_I, _I]),
     "dd3d_comm_unique_id": (_I, [_P]),
     "dd3d_comm_create": (_I, [_P, _I, _I, C.POINTER(_P)]),
     "dd3d_comm_from_nccl": (_I, [_P, _I, _I, C.POINTER(_P)]),

@@ -401,7 +401,7 @@ class DD3DB200(nn.Module):
                                     C.c_void_p(hb["sizes"].data_ptr()), C.c_void_p(hb["out"].data_ptr()),
                                     C.c_void_p(hb["counts"].data_ptr()), C.c_void_p(stream)), self._handle)
         self._check_flags(self.overflow_flags())
-        return self._wrap(hb["out"], hb["counts"], K, sizes, torch.device("cpu"))
+        return self._wrap(hb["out"], hb["counts"], K, sizes, torch.device("cpu"), self._host_global_rows(0))
 
     @torch.no_grad()
     def submit_host(self, batched_inputs, slot=0):
@@ -440,7 +440,13 @@ class DD3DB200(nn.Module):
         _lib.check(_lib.load().dd3d_wait_host(self._handle, int(slot)), self._handle)
         self._check_flags(self.overflow_flags())
         K, sizes = hb["ctx"]
-        return self._wrap(hb["out"].clone(), hb["counts"].clone(), K, sizes, torch.device("cpu"))
+        glob = self._host_global_rows(slot)
+        return self._wrap(hb["out"].clone(), hb["counts"].clone(), K, sizes, torch.device("cpu"),
+                          None if glob is None else glob.clone())
+
+    def _host_global_rows(self, slot):
+        """pred_boxes3d_global rows a host slot received (NuscenesDD3DB200 with the sample aggregation), else None."""
+        return None
 
     # ------------------------------------------------------------------ introspection (stage-level parity tests)
     def get_tensor(self, name):
@@ -520,7 +526,8 @@ class NuscenesDD3DB200(DD3DB200):
     """Mirror of ``tridet.modeling.dd3d.nuscenes_dd3d.NuscenesDD3D`` (nuscenes_dd3d.py:300-469) for inference: DD3D plus
     the attribute / speed predictors on the cls tower (fused into the cls predictor GEMM), ``pred_attributes`` /
     ``pred_speeds`` on every detection, and -- when ``postprocess_in_inference`` -- the cross-camera BEV NMS over the 6
-    images of each nuScenes sample with at most MAX_NUM_DETS_PER_SAMPLE survivors (``pred_boxes3d_global`` added).
+    images of each nuScenes sample with at most MAX_NUM_DETS_PER_SAMPLE survivors (``pred_boxes3d_global`` added), run by
+    the engine as the last step of every forward path (forward, forward_host, submit_host / wait_host, forward_raw).
     Inputs additionally carry "sample_token" and the global camera "pose"."""
     def __init__(self, cfg):
         super().__init__(cfg)
@@ -529,45 +536,83 @@ class NuscenesDD3DB200(DD3DB200):
         assert cfg.DATALOADER.TEST.NUM_IMAGES_PER_GROUP == 6
         self.max_num_dets_per_sample = cfg.DD3D.NUSC.INFERENCE.MAX_NUM_DETS_PER_SAMPLE
         self.sample_aggregate_in_inference = True  # test hook: False returns the per-image detections before the aggregation
+        self._groups = None  # group index of every image of the current call while the aggregation runs
+        self._host_glob, self._host_glob_live = {}, {}  # per host slot: pinned global rows, filled by its last call
+
+    def _aggregating(self, postprocess_in_forward=None):
+        post = self.postprocess_in_inference if postprocess_in_forward is None else postprocess_in_forward
+        return bool(post) and self.sample_aggregate_in_inference and not self.only_box2d
+
+    def _check_groups(self, batched_inputs, out_sizes):
+        """get_group_idxs (postprocessing.py:111-123) and the one common output size that detectron2's Instances.cat asserts
+        when nuscenes_sample_aggregate concatenates the Instances of the call (postprocessing.py:95): host checks, raised
+        before any device work.  Returns the group index of every image (None without the aggregation)."""
+        if not self._aggregating():
+            return None
+        groups = group_indices([x["sample_token"] for x in batched_inputs], self.num_images_per_sample)
+        assert len({tuple(int(v) for v in s) for s in out_sizes}) == 1, "images of one call must share the output size"
+        return groups
+
+    def _gather_inputs(self, batched_inputs, device):
+        r = super()._gather_inputs(batched_inputs, device)
+        self._groups = self._check_groups(batched_inputs, r[2][:, 2:].tolist())
+        return r
+
+    @torch.no_grad()
+    def forward_raw(self, raw_inputs):
+        # with postprocess_in_inference the output size of every image is its original (file) resolution
+        self._groups = self._check_groups(raw_inputs, [tuple(x["image_hwc"].shape[:2]) for x in raw_inputs])
+        return super().forward_raw(raw_inputs)
+
+    def _sync_options(self, postprocess_in_forward):
+        """The base switches, then the sample aggregation (nuscenes_dd3d.py:449-463) as the engine's last step whenever
+        postprocess_in_inference is on; the engine drops its plans when the step turns on or off."""
+        super()._sync_options(postprocess_in_forward)
+        h = self._handle
+        _lib.check(_lib.load().dd3d_set_sample_aggregate(h, int(self._aggregating(postprocess_in_forward)),
+                                                         float(self.bev_nms_iou_thresh),
+                                                         int(self.max_num_dets_per_sample or 0)), h)
+
+    def _set_device_poses(self, batched_inputs):
+        """With the sample aggregation: poses, group indices and the [B][cap][10] global-row buffer on the device, handed to
+        the engine for the next forward.  Returns what must stay alive until that forward has run."""
+        d_poses = super()._set_device_poses(batched_inputs)
+        if self._groups is None:
+            return SimpleNamespace(poses=d_poses, glob=None)
+        L, h, device = _lib.load(), self._handle, self._device
+        if d_poses is None:  # the BEV NMS did not hand them over already
+            d_poses = self._gather_poses(batched_inputs).to(device, non_blocking=True)
+            _lib.check(L.dd3d_set_poses(h, C.c_void_p(d_poses.data_ptr())), h)
+        d_group = torch.tensor(self._groups, dtype=torch.int32).to(device, non_blocking=True)
+        glob = torch.zeros((len(batched_inputs), self._desc.out_cap, _lib.GLOBAL_WORDS), dtype=torch.float32, device=device)
+        _lib.check(L.dd3d_set_groups(h, C.c_void_p(d_group.data_ptr()), max(self._groups) + 1), h)
+        _lib.check(L.dd3d_set_global_out(h, C.c_void_p(glob.data_ptr())), h)
+        return SimpleNamespace(poses=d_poses, group=d_group, glob=glob)
+
+    def _set_host_poses(self, batched_inputs, slot):
+        """Host paths: poses and group indices copied by the engine, the slot's pinned global-row buffer registered."""
+        self._host_glob_live[slot] = self._groups is not None
+        if self._groups is None:
+            return super()._set_host_poses(batched_inputs, slot)
+        L, h = _lib.load(), self._handle
+        poses = self._gather_poses(batched_inputs).contiguous()
+        _lib.check(L.dd3d_set_host_poses(h, int(slot), C.c_void_p(poses.data_ptr())), h)
+        groups = torch.tensor(self._groups, dtype=torch.int32)
+        _lib.check(L.dd3d_set_host_groups(h, int(slot), C.c_void_p(groups.data_ptr()), max(self._groups) + 1), h)
+        shape = (len(batched_inputs), self._desc.out_cap, _lib.GLOBAL_WORDS)
+        glob = self._host_glob.get(slot)
+        if glob is None or tuple(glob.shape) != shape:
+            glob = torch.zeros(shape, dtype=torch.float32).pin_memory()
+            self._host_glob[slot] = glob
+        _lib.check(L.dd3d_set_host_global_out(h, int(slot), C.c_void_p(glob.data_ptr())), h)
+
+    def _host_global_rows(self, slot):
+        return self._host_glob.get(slot) if self._host_glob_live.get(slot) else None
 
     def _finish(self, r, batched_inputs):
-        glob = None
-        if self.postprocess_in_inference and self.sample_aggregate_in_inference:
-            L = _lib.load()
-            device, B, cap = self._device, r["B"], r["cap"]
-            groups = group_indices([x["sample_token"] for x in batched_inputs], self.num_images_per_sample)
-            # nuscenes_sample_aggregate concatenates the Instances of the call (postprocessing.py:95); detectron2's
-            # Instances.cat asserts one common (output) image size
-            assert len({tuple(s[2:].tolist()) for s in r["sizes"]}) == 1, "images of one call must share the output size"
-            with torch.cuda.device(device):
-                d_poses = self._gather_poses([{"pose": x["pose"]} for x in batched_inputs]).to(device, non_blocking=True)
-                d_group = torch.tensor(groups, dtype=torch.int32).to(device, non_blocking=True)
-                glob = torch.zeros((B, cap, 10), dtype=torch.float32, device=device)
-                scratch = torch.empty(int(L.dd3d_op_sample_aggregate_scratch_bytes(B, cap)), dtype=torch.uint8, device=device)
-                self._agg_flags = torch.zeros(1, dtype=torch.int32, device=device)
-                _lib.check(
-                    L.dd3d_op_sample_aggregate(C.c_void_p(r["out"].data_ptr()), C.c_void_p(r["counts"].data_ptr()),
-                                               C.c_void_p(r["d_K"].data_ptr()), C.c_void_p(d_poses.data_ptr()),
-                                               C.c_void_p(d_group.data_ptr()), max(groups) + 1,
-                                               C.c_void_p(glob.data_ptr()), C.c_void_p(scratch.data_ptr()),
-                                               C.c_void_p(self._agg_flags.data_ptr()), B, cap,
-                                               float(self.bev_nms_iou_thresh), int(self.max_num_dets_per_sample or 0),
-                                               C.c_void_p(r["stream"])), self._handle)
-            r["counts"][B:] |= self._agg_flags  # bit 3 rides in the same overflow word
-        host = r["counts"].cpu()
+        host = r["counts"].cpu()  # the only sync: B counts + the overflow word (bits 3 / 5: the aggregation's capacity)
         self._check_flags(int(host[-1]))
-        return self._wrap(r["out"], host[:-1], r["K"], r["sizes"], self._device, glob)
-
-    def forward_host(self, batched_inputs):
-        """Host-buffer path: the sample aggregation needs the detections of all cameras on the device, so this is the
-        device forward followed by the device->host copy of the results."""
-        return [{"instances": o["instances"].to("cpu")} for o in self.forward(batched_inputs)]
-
-    def overflow_flags(self):
-        f = super().overflow_flags()
-        if getattr(self, "_agg_flags", None) is not None:
-            f |= int(self._agg_flags.item())
-        return f
+        return self._wrap(r["out"], host[:-1], r["K"], r["sizes"], self._device, r["d_poses"].glob)
 
 
 class _DevArray:

@@ -139,6 +139,8 @@ class _DeviceTTA(nn.Module):
             pose = model._gather_poses([x]).to(device, non_blocking=True)
         # that BEV NMS runs below, after each chunk of views, with the views' intrinsics: not as the engine's last op
         _lib.check(L.dd3d_set_bev_nms(model._engine(), 0, float(model.bev_nms_iou_thresh)), model._handle)
+        # nor does a NuscenesDD3DB200's sample aggregation: the wrapper aggregates the merged per-image results itself
+        _lib.check(L.dd3d_set_sample_aggregate(model._handle, 0, float(model.bev_nms_iou_thresh), 0), model._handle)
         # chunks of `batch_size` views, each padded to the chunk's largest view like ImageList.from_tensors does for
         # one model(inputs) call (test_time_augmentation.py:118-133)
         for a0 in range(0, A, self.batch_size):

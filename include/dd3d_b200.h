@@ -221,7 +221,9 @@ int dd3d_submit_host(dd3d_handle h, int slot, const void* h_images, int img_dtyp
 int dd3d_wait_host(dd3d_handle h, int slot);
 /* bit 0: unused (the pre-NMS top-k is exact for every input and sets no bit); bit 1: more than out_cap detections
  * survived; with the BEV NMS on (dd3d_set_bev_nms), bit 2: more than 256 boxes reached the one-CTA BEV kernel of an
- * image, bit 6: a count above out_cap reached the multi-CTA one.  Reads a device word (synchronises `stream`). */
+ * image, bit 6: a count above out_cap reached the multi-CTA one; with the sample aggregation on
+ * (dd3d_set_sample_aggregate), bit 3 (one-CTA path) / bit 5 (blocked path): a sample group beyond the kernel's capacity.
+ * Reads a device word (synchronises `stream`). */
 int dd3d_overflow_flags(dd3d_handle h, dd3d_stream stream, int32_t* h_flags);
 /* Runtime switches the reference's callers toggle on the meta-arch: "do_postprocess" (postprocess_in_inference,
  * scripts/train.py:206-209, test_time_augmentation.py:107), "do_nms" (core.py:134), "profile" (see
@@ -266,6 +268,37 @@ int dd3d_set_host_poses(dd3d_handle h, int slot, const float* h_poses);
  * 0 < post_nms_topk <= 256: at most 256 score-sorted boxes per image), 2 = the multi-CTA kernels of dd3d_op_bev_nms_large
  * (every other config: up to 5 * pre_nms_topk unsorted boxes per image). */
 int dd3d_bev_nms_path(const dd3d_model_desc* h_desc);
+/* ---- NuscenesDD3D sample aggregation (nuscenes_dd3d.py:449-463 -> postprocessing.py:58-108) as the last step of every
+ * forward -------------------------------------------------------------------------------------------------------------
+ * dd3d_set_sample_aggregate(h, 1, thr, max_dets): every following dd3d_forward / dd3d_forward_host / dd3d_submit_host /
+ * dd3d_forward_raw ends, after the NMS (and BEV NMS) step with detector_postprocess applied, with the reference's
+ * nuscenes_sample_aggregate on the detections of the call: boxes to the global frame through each image's pose, one
+ * class-aware rotated BEV NMS on scores_3d (IoU threshold thr, BEV_NMS_IOU_THRESH) per sample group, then only the
+ * max_dets best survivors OF THE CALL stay (keep[:MAX_NUM_DETS_PER_SAMPLE]; max_dets <= 0: no cap) -- per rank under
+ * multi-GPU, as the reference's per-rank forward; survivors keep their order, and the pred_boxes3d_global rows (quat w, x,
+ * y, z, tvec, size) of the survivors, compacted like the detections, go to the global-row buffer.  Same results as
+ * dd3d_op_sample_aggregate after the forward.  A sample's images must all be in one call.  Needs box3d_on.  The kernel is
+ * chosen from the config (dd3d_sample_aggregate_path); turning the step on or off, or a "do_nms" change that switches the
+ * kernel, drops the engine's plans (call dd3d_plan again).  With it off the op list, the launches and the workspace are
+ * those of an engine that never had it.  Overflow: flags bit 3 (one-CTA path: a group above 768 boxes or 16 images), bit 5
+ * (blocked path: a count above out_cap or a group above 16 images / out of range).
+ * Poses: dd3d_set_poses / dd3d_set_host_poses (the BEV NMS's).  Group indices: [B] int32, 0..num_groups-1 (get_group_idxs,
+ * postprocessing.py:111-123), 1 <= num_groups <= B: dd3d_set_groups, a DEVICE buffer read by every following dd3d_forward /
+ * dd3d_forward_raw (kept until replaced; NULL clears it); dd3d_set_host_groups, a HOST array copied at the call for the
+ * host paths' slot 0 / 1 (needs a plan).  Global rows: dd3d_set_global_out, a DEVICE buffer [B][out_cap][10] fp32 the
+ * device forwards write; dd3d_set_host_global_out, a HOST buffer (pinned) of the same shape per slot, filled by
+ * dd3d_forward_host (slot 0) or by the time dd3d_wait_host(slot) returns.  A forward with the step on and no poses, groups
+ * or global-row buffer returns DD3D_ERR_STATE. */
+int dd3d_set_sample_aggregate(dd3d_handle h, int enable, float iou_thresh, int max_dets);
+int dd3d_set_groups(dd3d_handle h, const int32_t* d_group, int num_groups);
+int dd3d_set_host_groups(dd3d_handle h, int slot, const int32_t* h_group, int num_groups);
+int dd3d_set_global_out(dd3d_handle h, float* d_global);
+int dd3d_set_host_global_out(dd3d_handle h, int slot, float* h_global);
+/* The sample aggregation kernels a config runs (no device needed): 1 = the one-CTA pair of dd3d_op_sample_aggregate (do_nms,
+ * 0 < post_nms_topk <= 128 and out_cap <= 256: six cameras fit its 768-box group), 2 = the blocked kernels of
+ * dd3d_op_group_bev_nms_large in global mode (every other config: up to 6 * 5 * 1150 = 34 500 boxes per sample, at most 256
+ * images per call). */
+int dd3d_sample_aggregate_path(const dd3d_model_desc* h_desc);
 /* Process-wide kernel-selection policy for plans / operator calls made afterwards (tests, A/B measurements):
  * "op_fp16" = 1: the dd3d_op_* entry points below treat their 16-bit buffers as fp16 (default 0: bf16).
  * "nms_class_parallel" = 0: one CTA per image does the whole NMS instead of the multi-CTA path (rank sort, IoU bit matrix on
@@ -289,10 +322,10 @@ int dd3d_launches_per_forward(dd3d_handle h);
  * launch stream around every op), with the algorithmic FLOPs / HBM bytes and launch counts of one forward.
  * Categories (arrays of 8): 0 preprocess, 1 special-purpose conv kernels (stem convs, the fused DLA-34 front end and the
  * depthwise 3x3 convs of the VoVNet -dw variants), 2 wgmma implicit-GEMM conv, 3 max-pool, 4 eSE, 5 relu and GroupNorm (the
- * elementwise passes over a map), 6 decode, 7 NMS. */
+ * elementwise passes over a map), 6 decode, 7 NMS (with the BEV NMS and the sample aggregation). */
 int dd3d_get_profile(dd3d_handle h, double* h_ms, double* h_flops, double* h_bytes, int32_t* h_launches);
 /* Same events, one entry per step in launch order: the preprocess, every engine op (with the sparse box2d / box3d towers,
- * their tile lists in front of them), the decode, the NMS.  Per entry: device ms, category, algorithmic FLOPs and, when
+ * their tile lists in front of them), the decode, the NMS, the sample aggregation when it is on.  Per entry: device ms, category, algorithmic FLOPs and, when
  * h_ops is not null, the engine op it timed (the index of dd3d_get_conv_info / dd3d_get_tensor "op<i>"), or -1 for the
  * preprocess, tile-list, decode and NMS entries.  Returns the number of entries written (<= max_ops). */
 int dd3d_get_op_times(dd3d_handle h, float* h_ms, int32_t* h_cats, double* h_flops, int32_t* h_ops, int max_ops);
@@ -334,6 +367,10 @@ int dd3d_forward_resized(dd3d_handle h, const uint8_t* d_raw, int raw_h, int raw
  * DD3D_ERR_CUDA and dd3d_comm_last_error() says why.  One process per GPU. */
 typedef struct dd3d_comm_s* dd3d_comm;
 int64_t dd3d_packed_bytes(int B, int out_cap);
+/* Extended layout for NuscenesDD3D (dd3d_set_sample_aggregate): the three parts above at the same offsets, then
+ * float global[B][out_cap][10] (the global-row buffer of the forward) at byte offset dd3d_packed_bytes(B, out_cap), padded to
+ * 256 bytes -- detections, counts, flags and pred_boxes3d_global in ONE buffer for ONE all-gather. */
+int64_t dd3d_packed_bytes_global(int B, int out_cap);
 /* device word of the overflow flags of the last forward (bits as dd3d_overflow_flags) -> d_dst, on `stream`, no sync */
 int dd3d_copy_flags(dd3d_handle h, int32_t* d_dst, dd3d_stream stream);
 int dd3d_comm_unique_id(uint8_t* h_id128);          /* rank 0: ncclGetUniqueId; ship the 128 bytes to the other ranks */
