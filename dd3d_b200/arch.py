@@ -6,6 +6,7 @@ tridet/modeling/feature_extractor/vovnet.py:19-143,188-336; FPN + top blocks dla
 heads fcos2d.py:55-108, fcos3d.py:81-139).  tests/test_cpu_oracle.py::test_inventory_and_oracle_vs_live_reference checks this inventory against the
 reference's own state_dict when /root/reference is present.
 """
+import math
 from collections import OrderedDict
 
 # kind tags: "conv" (weight, fan-in init), "bias", "bn_w", "bn_b", "bn_mean", "bn_var", "nbt", "gn_w", "gn_b", "scalar",
@@ -102,7 +103,7 @@ def _dla(specs, arch, norm):
     _dla_tree(specs, p + ".level2", levels[2], ch[1], ch[2], False, norm=norm, cardinality=card)
     for lvl in (3, 4, 5):
         _dla_tree(specs, p + f".level{lvl}", levels[lvl], ch[lvl - 1], ch[lvl], True, norm=norm, cardinality=card)
-    return {"level3": ch[3], "level4": ch[4], "level5": ch[5]}
+    return {f"level{lvl}": ch[lvl] for lvl in range(6)}  # channels of every output (dla.py:309-312)
 
 
 V99_STAGE_CONV_CH = [128, 160, 192, 224]
@@ -162,7 +163,7 @@ def _vovnet(specs, arch, norm):
             _norm(specs, f"{q}.concat.{name}_concat/norm", oc, norm)
             _conv(specs, f"{q}.ese.fc", oc, oc, 1, bias=True, role="ese")
             in_ch = oc
-    return {f"stage{si}": oc for si, oc in enumerate(out_ch, start=2)}
+    return dict(stem=stem[2], **{f"stage{si}": oc for si, oc in enumerate(out_ch, start=2)})
 
 
 def param_specs(cfg):
@@ -172,17 +173,12 @@ def param_specs(cfg):
     specs["pixel_std"] = ((3, 1, 1), "buffer")
     arch = arch_of(cfg)
     norm = backbone_norm(cfg)
-    if arch in DLA_SPECS:
-        feats = _dla(specs, arch, norm)
-        stages = {"level3": 3, "level4": 4, "level5": 5}
-    else:
-        feats = _vovnet(specs, arch, norm)
-        stages = {"stage2": 2, "stage3": 3, "stage4": 4, "stage5": 5}
+    feats = _dla(specs, arch, norm) if arch in DLA_SPECS else _vovnet(specs, arch, norm)
     fpn_norm = cfg.FE.FPN.NORM  # detectron2 FPN: bias only without a norm; one norm per conv
     F = fpn_channels(cfg)  # the FPN's width is every head's width too (fcos2d.py:43-45, fcos3d.py:70-72)
-    for name, ch in feats.items():
-        st = stages[name]
-        for conv, cin, k in ((f"backbone.fpn_lateral{st}", ch, 1), (f"backbone.fpn_output{st}", F, 3)):
+    for name, stride in fpn_inputs(cfg):  # registered in FE.FPN.IN_FEATURES order, named by log2 stride
+        st = int(math.log2(stride))
+        for conv, cin, k in ((f"backbone.fpn_lateral{st}", feats[name], 1), (f"backbone.fpn_output{st}", F, 3)):
             _conv(specs, conv, F, cin, k, bias=fpn_norm == "", role="linear")
             _norm(specs, conv + ".norm", F, fpn_norm)
     _conv(specs, "backbone.top_block.p6", F, F, 3, bias=True, role="linear")
@@ -297,14 +293,70 @@ def backbone_norm(cfg):
     return norm
 
 
+# Stride of every backbone output the reference names: DLA level<k> is 2**k (dla.py:309-312); the VoVNet stem and stage2 are 4,
+# each later stage doubles it (vovnet.py:306-333)
+DLA_OUTPUT_STRIDES = {f"level{k}": 2**k for k in range(6)}
+VOVNET_OUTPUT_STRIDES = {"stem": 4, "stage2": 4, "stage3": 8, "stage4": 16, "stage5": 32}
+# The FPN inputs without a configured FE.FPN.IN_FEATURES list (configs/feature_extractors/{dla34,v2_99}_fpn.yaml)
+DEFAULT_FPN_INPUTS = {True: ["level3", "level4", "level5"], False: ["stage2", "stage3", "stage4", "stage5"]}
+
+
+def fpn_inputs(cfg):
+    """FE.FPN.IN_FEATURES as [(backbone output, stride)], with the errors the reference raises while it builds the backbone
+    and the FPN: the DLA's assert on an output that is not one of its children and KeyError for base_layer (dla.py:300-315),
+    KeyError for a VoVNet output it does not have (VoVNet.output_shape), KeyError for an FPN input the backbone does not
+    return (``input_shapes[f]``), and detectron2's AssertionErrors for an empty list and for strides that do not double
+    from one input to the next (FPN.__init__, _assert_strides_are_log2_contiguous)."""
+    dla = arch_of(cfg) in DLA_SPECS
+    out = cfg.FE.BACKBONE.OUT_FEATURES
+    if dla:
+        out = ["level5"] if out is None else list(out)
+        assert len(out)
+        children = ["base_layer"] + list(DLA_OUTPUT_STRIDES)
+        for f in out:
+            assert f in children, "Available children: {}".format(", ".join(children))
+        shapes = {f: DLA_OUTPUT_STRIDES[f] for f in out}
+    else:
+        shapes = {f: VOVNET_OUTPUT_STRIDES[f] for f in out}
+    in_features = list(cfg.FE.FPN.IN_FEATURES)
+    assert in_features, in_features
+    strides = [shapes[f] for f in in_features]
+    for i, stride in enumerate(strides[1:], 1):
+        assert stride == 2 * strides[i - 1], "Strides {} {} are not log2 contiguous".format(stride, strides[i - 1])
+    return list(zip(in_features, strides))
+
+
 def fpn_output_names(cfg):
-    """The FPN's outputs in order (backbone.output_shape()): p3..p7 for the DLA p67 builder (dla.py:536-561), p2..p6 for the
-    VoVNet p6 builder (vovnet.py:428-454)."""
-    return ["p3", "p4", "p5", "p6", "p7"] if arch_of(cfg) in DLA_SPECS else ["p2", "p3", "p4", "p5", "p6"]
+    """The FPN's outputs in order (backbone.output_shape()): p<log2 stride> of every FPN input, then the top block's p6 and p7
+    for the DLA p67 builder (dla.py:536-561) or p6 for the VoVNet p6 builder (vovnet.py:428-454).  The defaults give p3..p7 and
+    p2..p6."""
+    stages = [int(math.log2(s)) for _, s in fpn_inputs(cfg)]
+    top = 2 if arch_of(cfg) in DLA_SPECS else 1
+    return [f"p{s}" for s in stages] + [f"p{stages[-1] + k}" for k in range(1, top + 1)]
+
+
+def check_fpn_inputs(cfg):
+    """The errors of an FE.FPN.IN_FEATURES list that builds in the reference but cannot run: the top block reads
+    ``results[self._out_features.index("p5")]`` at the first forward, ValueError without a p5 output and IndexError when p5 is
+    a top-block output; then NotImplementedError for what the engine does not build: inputs below stride 4 (DLA level0 /
+    level1, which its fused front end never stores) and more than DD3D_NUM_LEVELS (5) head levels, the bound of the decode
+    and of the NMS shared memory at PRE_NMS_TOPK.  Call it after param_specs, which raises the construction errors."""
+    inputs = fpn_inputs(cfg)
+    idx = fpn_output_names(cfg).index("p5")
+    if idx >= len(inputs):
+        raise IndexError("list index out of range")
+    low = [f for f, s in inputs if s < 4]
+    if low:
+        raise NotImplementedError(f"FE.FPN.IN_FEATURES {low} below stride 4 are not supported: the engine builds the FPN on "
+                                  "DLA level2..level5 and VoVNet stem / stage2..stage5")
+    n = len(in_feature_levels(cfg))
+    if n > 5:
+        raise NotImplementedError(f"{n} head levels are not supported: the engine runs at most 5 (set DD3D.IN_FEATURES to at "
+                                  f"most 5 of {fpn_output_names(cfg)})")
 
 
 def in_feature_levels(cfg):
-    """DD3D.IN_FEATURES as FPN output indices (0..4) in head order: `cfg.DD3D.IN_FEATURES or list(backbone_output_shape)`
+    """DD3D.IN_FEATURES as FPN output indices in head order: `cfg.DD3D.IN_FEATURES or list(backbone_output_shape)`
     (core.py:25-26).  An unknown name raises KeyError like the reference's `backbone_output_shape[f]`; a repeated level, which
     the reference builds but has no use, raises NotImplementedError."""
     names = fpn_output_names(cfg)
@@ -323,7 +375,7 @@ def in_feature_levels(cfg):
 
 def level_strides(cfg):
     """Strides of the head levels, in DD3D.IN_FEATURES order (compute_locations, core.py:166-174)."""
-    strides = [8, 16, 32, 64, 128] if arch_of(cfg) in DLA_SPECS else [4, 8, 16, 32, 64]
+    strides = [2**int(name[1:]) for name in fpn_output_names(cfg)]
     return [strides[i] for i in in_feature_levels(cfg)]
 
 

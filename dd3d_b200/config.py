@@ -96,15 +96,19 @@ for _key, _spec in DLA_SPECS.items():
 
 
 def get_cfg(backbone="dla34", dataset="kitti_3d", nms_thresh=0.75, meta_arch="DD3D", act_dtype="bf16", fpn_channels=256,
-            in_features=None):
+            in_features=None, fpn_in_features=None):
     """backbone: a DLA key of dd3d_b200.arch.DLA_SPECS ("dla34", "dla_x_46_c", "dla_x_60_c", "dla_x_60", "dla_x_102",
     "dla_x_102_64") or a VoVNet key of VOVNET_SPECS ("v2_19_slim_dw", "v2_19_dw", "v2_19_slim", "v2_19", "v2_39", "v2_57",
     "v2_99"), which sets FE.BACKBONE.NAME; dataset in {"kitti_3d", "nuscenes"} (head constants only); meta_arch in
     {"DD3D", "NuscenesDD3D"} (configs/experiments/dd3d_nusc_{dla34,v99}.yaml:9,30-36); fpn_channels sets FE.FPN.OUT_CHANNELS,
     the width of the FPN and of the FCOS heads (256 in every shipped config); in_features sets DD3D.IN_FEATURES, the FPN
-    outputs the heads run on in head order (None: every FPN output, core.py:25)."""
+    outputs the heads run on in head order (None: every FPN output, core.py:25); fpn_in_features sets FE.BACKBONE.OUT_FEATURES
+    and FE.FPN.IN_FEATURES, the backbone outputs the FPN reads (None: the feature extractor's list, dla34_fpn.yaml /
+    v2_99_fpn.yaml)."""
     ds = _DATASETS[dataset]
     fe = copy.deepcopy(_FEATURE_EXTRACTORS[backbone])
+    if fpn_in_features is not None:
+        fe["BACKBONE"]["OUT_FEATURES"] = list(fpn_in_features)
     fe["FPN"] = dict(IN_FEATURES=list(fe["BACKBONE"]["OUT_FEATURES"]), OUT_FEATURES=None, OUT_CHANNELS=fpn_channels,
                      NORM="FrozenBN", FUSE_TYPE="sum")
     fe["OUT_FEATURES"] = None

@@ -90,6 +90,11 @@ int dd3d_set_fpn_channels(dd3d_handle h, int32_t channels) {
     return guarded(h, [&](Engine& e) { e.set_fpn_channels(channels); });
 }
 
+int dd3d_set_fpn_inputs(dd3d_handle h, const int32_t* h_inputs, int n) {
+    if (h_inputs == nullptr) return DD3D_ERR_INVALID;
+    return guarded(h, [&](Engine& e) { e.set_fpn_inputs(h_inputs, n); });
+}
+
 int dd3d_set_in_features(dd3d_handle h, const int32_t* h_fpn_levels, int n) {
     if (h_fpn_levels == nullptr) return DD3D_ERR_INVALID;
     return guarded(h, [&](Engine& e) { e.set_in_features(h_fpn_levels, n); });
@@ -392,8 +397,10 @@ int dd3d_get_tensor(dd3d_handle h, const char* name, void** d_ptr, int32_t dims[
             *d_ptr = P.input.ptr;
             const int32_t d[6] = {P.B, P.Hp, P.Wp, 4, 4, 2};
             memcpy(dims, d, sizeof(d));
-        } else if (n[0] == 'p') {
-            const View& v = P.fpn[level(1)];
+        } else if (n[0] == 'p') {  // "p<i>": FPN output i, i < the FPN's output count
+            const int l = n.size() == 2 ? n[1] - '0' : -1;
+            if (l < 0 || l >= e.fpn_outputs()) throw EngineError(DD3D_ERR_INVALID, "unknown tensor: " + n);
+            const View& v = P.fpn[l];
             if (v.ptr == nullptr) throw EngineError(DD3D_ERR_INVALID, "FPN output " + n + " is not built: no head reads it");
             *d_ptr = v.ptr;
             const int32_t d[6] = {v.B, v.H, v.W, v.C, v.pitch, 2};

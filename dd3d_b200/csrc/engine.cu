@@ -249,17 +249,52 @@ void Engine::set_fpn_channels(int C) {
     fpn_channels = C;
 }
 
+// VoVNet: the stem and stage2 share stride 4, so the stem stands in for stage 2 of the stride order
+static int fpn_input_stage(int v) { return v == DD3D_FPN_IN_STEM ? 2 : v; }
+
+std::vector<int> Engine::fpn_input_list() const {
+    if (!fpn_inputs.empty()) return fpn_inputs;
+    if (dla_spec(desc.arch) != nullptr) return {3, 4, 5};
+    return {2, 3, 4, 5};
+}
+
+int Engine::fpn_first_stage() const { return fpn_input_stage(fpn_input_list()[0]); }
+
+int Engine::fpn_outputs() const {
+    return static_cast<int>(fpn_input_list().size()) + (dla_spec(desc.arch) != nullptr ? 2 : 1);
+}
+
+void Engine::set_fpn_inputs(const int32_t* inputs, int n) {
+    if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_fpn_inputs after finalize");
+    if (!in_features.empty()) fail(DD3D_ERR_STATE, "dd3d_set_fpn_inputs after dd3d_set_in_features");
+    if (inputs == nullptr || n < 1 || n > 4) fail(DD3D_ERR_INVALID, "dd3d_set_fpn_inputs needs 1 to 4 backbone outputs");
+    const bool dla = dla_spec(desc.arch) != nullptr;
+    std::vector<int> v(inputs, inputs + n);
+    for (int i = 0; i < n; ++i) {
+        // DLA level2..5 (level0 / level1 are stride 1 / 2: the fused front end never stores them); VoVNet stem, stage2..5
+        const bool known = dla ? (v[i] >= 2 && v[i] <= 5) : (v[i] == DD3D_FPN_IN_STEM || (v[i] >= 2 && v[i] <= 5));
+        if (!known) fail(DD3D_ERR_INVALID, "backbone output " + std::to_string(v[i]) + " cannot feed the FPN");
+        if (i > 0 && fpn_input_stage(v[i]) != fpn_input_stage(v[i - 1]) + 1)
+            fail(DD3D_ERR_INVALID, "FPN input strides must double from one input to the next");
+    }
+    if (v.back() != 5) fail(DD3D_ERR_INVALID, "the FPN inputs must end at stride 32 (the top block reads p5)");
+    fpn_inputs.clear();
+    if (v != fpn_input_list()) fpn_inputs = v;  // the default list is the default graph
+}
+
 void Engine::set_in_features(const int32_t* fpn_levels, int n) {
     if (finalized) fail(DD3D_ERR_STATE, "dd3d_set_in_features after finalize");
     if (fpn_levels == nullptr || n < 1 || n > kLevels) fail(DD3D_ERR_INVALID, "dd3d_set_in_features needs 1 to 5 FPN levels");
+    const int outs = fpn_outputs();
     std::vector<int> v(fpn_levels, fpn_levels + n);
     for (int i = 0; i < n; ++i) {
-        if (v[i] < 0 || v[i] >= kLevels) fail(DD3D_ERR_INVALID, "FPN level " + std::to_string(v[i]) + " outside 0..4");
+        if (v[i] < 0 || v[i] >= outs)
+            fail(DD3D_ERR_INVALID, "FPN level " + std::to_string(v[i]) + " outside 0.." + std::to_string(outs - 1));
         for (int j = 0; j < i; ++j)
             if (v[j] == v[i]) fail(DD3D_ERR_INVALID, "FPN level " + std::to_string(v[i]) + " repeated");
     }
     in_features = v;
-    if (n == kLevels) {  // all five in order is the default graph
+    if (n == outs) {  // every FPN output in order is the default graph
         bool identity = true;
         for (int i = 0; i < n; ++i) identity = identity && v[i] == i;
         if (identity) in_features.clear();
@@ -775,11 +810,14 @@ struct Builder {
             maxpool(a2, bottom, 2);
         }
         const int* ch = S.channels;
+        // the FPN inputs (FE.FPN.IN_FEATURES): level<first> .. level5
+        const int first = E->fpn_first_stage();
         View x = dla_level(p + ".level2", a2, S.levels[2], ch[1], ch[2], false, &bottom);
         feats->clear();
+        if (first == 2) feats->push_back(x);
         for (int l = 3; l <= 5; ++l) {
             x = dla_level(p + ".level" + std::to_string(l), x, S.levels[l], ch[l - 1], ch[l], true, nullptr);
-            feats->push_back(x);
+            if (l >= first) feats->push_back(x);
         }
     }
 
@@ -891,6 +929,11 @@ struct Builder {
         int in_ch = S.stem[2];
         View cat = alloc(h, w, in_ch + nl * stage_ch[0]);
         vov_conv3x3(p + ".stem.stem_3", s2, slice(cat, 0, in_ch), 2, S.dw);
+        // the FPN inputs (FE.FPN.IN_FEATURES): the stem (a slice of stage 2's first concat buffer, which nothing overwrites)
+        // and stage<first> .. stage5
+        const std::vector<int> fpn_in = E->fpn_input_list();
+        feats->clear();
+        if (fpn_in[0] == DD3D_FPN_IN_STEM) feats->push_back(slice(cat, 0, in_ch));
         View stage_out;
         View pooled_cat;  // next stage's concat buffer when its pooled slice was produced by the previous stage's eSE pass
         for (int si = 0; si < 4; ++si) {
@@ -954,7 +997,7 @@ struct Builder {
                 in_ch = oc;
             }
             pooled_cat = pooled_next;
-            feats->push_back(stage_out);
+            if (std::find(fpn_in.begin(), fpn_in.end(), si + 2) != fpn_in.end()) feats->push_back(stage_out);
         }
     }
 
@@ -1019,7 +1062,7 @@ struct Builder {
         // n - 1 and P7 reads P6; lateral i feeds output i and every lateral below it, so the laterals below the lowest output
         // read are skipped too.  The reference still computes them; nothing reads them.
         const bool dla = dla_spec(E->desc.arch) != nullptr;
-        bool read[kLevels + 1] = {};
+        bool read[kFpnMaxOutputs + 1] = {};
         for (int l = 0; l < E->num_levels(); ++l) read[E->head_level(l)] = true;
         const bool want_p7 = dla && read[n + 1], want_p6 = read[n] || want_p7;
         std::vector<bool> need(n);
@@ -1055,7 +1098,7 @@ struct Builder {
         }
         *outs = res;
         if (!want_p6) {
-            outs->resize(kLevels);
+            outs->resize(E->fpn_outputs());
             return;
         }
         const View& p5 = res[n - 1];
@@ -1071,7 +1114,7 @@ struct Builder {
             conv1(p + ".top_block.p7", "", true, r6, p7, 3, 2, false);
             outs->push_back(p7);
         }
-        outs->resize(kLevels);  // VoVNet: P6 is the last; a skipped output stays an empty view
+        outs->resize(E->fpn_outputs());  // VoVNet: P6 is the last; a skipped output stays an empty view
     }
 
     // ---- heads ------------------------------------------------------------------------------------------------
@@ -1619,15 +1662,13 @@ size_t Engine::build(Plan* P, int B, int Hs, int Ws, void* workspace, bool dry) 
         bld.off += round_up_sz(static_cast<size_t>(B) * Hp * Wp * 4 * 2, 1024);
         P->input = input;
         std::vector<View> feats, fpn;
-        if (dla_spec(desc.arch) != nullptr) {
+        if (dla_spec(desc.arch) != nullptr)
             bld.build_dla(input, &feats);
-            bld.build_fpn(feats, 3, &fpn);
-        } else {
+        else
             bld.build_vovnet(*vovnet_spec(desc.arch), input, &feats);
-            bld.build_fpn(feats, 2, &fpn);
-        }
-        if (static_cast<int>(fpn.size()) != kLevels) fail(DD3D_ERR_STATE, "internal: expected 5 FPN levels");
-        for (int l = 0; l < kLevels; ++l) P->fpn[l] = fpn[l];
+        bld.build_fpn(feats, fpn_first_stage(), &fpn);
+        if (static_cast<int>(fpn.size()) != fpn_outputs()) fail(DD3D_ERR_STATE, "internal: FPN output count");
+        for (int l = 0; l < fpn_outputs(); ++l) P->fpn[l] = fpn[l];
         std::vector<View> heads(num_levels());  // the FPN outputs in DD3D.IN_FEATURES order
         for (int l = 0; l < num_levels(); ++l) heads[l] = fpn[head_level(l)];
         bld.build_heads(heads);
@@ -1668,6 +1709,9 @@ void Engine::finalize() {
     // dry graph walk with the smallest legal shape: creates (packs + uploads) every layer and names the first
     // missing tensor, without needing a workspace.
     Plan tmp;
+    if (num_levels() > kLevels)
+        fail(DD3D_ERR_INVALID, std::to_string(fpn_outputs()) + " FPN outputs need dd3d_set_in_features with at most " +
+                                   std::to_string(kLevels) + " of them");
     if (canonical_sizes.empty() && desc.num_classes > DD3D_MAX_CLASSES && desc.box3d_on)
         fail(DD3D_ERR_STATE, "num_classes " + std::to_string(desc.num_classes) + " > " + std::to_string(DD3D_MAX_CLASSES) +
                                  " needs dd3d_set_canonical_sizes before dd3d_finalize");
@@ -1748,16 +1792,13 @@ void Engine::make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes) {
     // decode / NMS parameter blocks
     DecodeParams& dp = plan.decode;
     memset(&dp, 0, sizeof(dp));
-    static const int strides_dla[5] = {8, 16, 32, 64, 128};
-    static const int strides_vov[5] = {4, 8, 16, 32, 64};
-    const int* strides = dla_spec(desc.arch) != nullptr ? strides_dla : strides_vov;
     for (int l = 0; l < plan.num_levels; ++l) {  // compute_locations with the strides of the selected levels
         dp.lvl[l].cls = plan.cls_map[l];
         dp.lvl[l].box = plan.box_map[l];
         dp.lvl[l].b3d = plan.b3d_map[l];
         dp.lvl[l].H = plan.lvl_h[l];
         dp.lvl[l].W = plan.lvl_w[l];
-        dp.lvl[l].stride = strides[head_level(l)];
+        dp.lvl[l].stride = 1 << (fpn_first_stage() + head_level(l));  // FPN output i has stride 2^(first stage + i)
     }
     fill_decode_params(&dp, desc, B, plan.cls_pitch, plan.b3d_pitch, d_canon, plan.num_levels);
     decode_bind_scratch(&dp, plan.detect_scratch);

@@ -17,6 +17,8 @@
 
 namespace dd3d {
 
+constexpr int kFpnMaxOutputs = DD3D_FPN_MAX_OUTPUTS;  // FPN outputs (p<first> .. P6 / P7); the heads run at most kLevels
+
 struct EngineError {
     int status;
     std::string msg;
@@ -161,7 +163,7 @@ struct Plan {
     int32_t* s1_group = nullptr;  // sample aggregation on: slot 1's copy of the host group indices
     float* s1_global = nullptr;   // and its pred_boxes3d_global rows [B][out_cap][10]
     View input;
-    View fpn[kLevels];  // by FPN output index; an output no head reads is not built (null ptr)
+    View fpn[kFpnMaxOutputs];  // by FPN output index; an output no head reads is not built (null ptr)
     int num_levels = kLevels;  // head positions; the per-level arrays below are by position
     float* cls_map[kLevels] = {};
     float* box_map[kLevels] = {};
@@ -296,14 +298,21 @@ class Engine {
     void set_backbone_norm(int norm);
     void set_fpn_channels(int C);
     void set_canonical_sizes(int num_classes, const float* sizes);
+    void set_fpn_inputs(const int32_t* inputs, int n);
     void set_in_features(const int32_t* fpn_levels, int n);
-    int num_levels() const { return in_features.empty() ? kLevels : static_cast<int>(in_features.size()); }
+    std::vector<int> fpn_input_list() const;  // FE.FPN.IN_FEATURES as dd3d_set_fpn_inputs numbers (the default when unset)
+    int fpn_first_stage() const;  // log2 of the stride of FPN output 0
+    int fpn_outputs() const;      // inputs + the top block's P6 (VoVNet) or P6 and P7 (DLA): 2 .. kFpnMaxOutputs
+    int num_levels() const { return in_features.empty() ? fpn_outputs() : static_cast<int>(in_features.size()); }
     int head_level(int l) const { return in_features.empty() ? l : in_features[l]; }  // FPN output read at position l
 
     dd3d_model_desc desc;
     // FCOS3D.CANONICAL_BOX3D_SIZES rows 0..num_classes-1 (dd3d_set_canonical_sizes); empty: the desc's rows (num_classes <= 16)
     std::vector<float> canonical_sizes;
-    // DD3D.IN_FEATURES (dd3d_set_in_features): the FPN output (0 .. 4) each head position reads, distinct; empty: all five in
+    // FE.FPN.IN_FEATURES (dd3d_set_fpn_inputs): backbone outputs feeding the FPN, stride-contiguous and ending at stride 32;
+    // empty: the builder's default (DLA level3..5, VoVNet stage2..5)
+    std::vector<int> fpn_inputs;
+    // DD3D.IN_FEATURES (dd3d_set_in_features): the FPN output each head position reads, distinct; empty: every FPN output in
     // order.  Per-level BN, Scale / Offset and PER_LEVEL_PREDICTORS predictors are taken by position.
     std::vector<int> in_features;
     // FPN / head layout (dd3d_set_layout); the default is the shipped one

@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "_lib", "libdd3d_b200.so")
 MAX_CLASSES = 16        # DD3D_MAX_CLASSES: canonical-size rows of ModelDesc
 MAX_NUM_CLASSES = 128   # DD3D_MAX_NUM_CLASSES: largest DD3D.NUM_CLASSES (rows past 16 go through dd3d_set_canonical_sizes)
 NUM_LEVELS = 5
+FPN_IN_STEM = 1  # DD3D_FPN_IN_STEM: dd3d_set_fpn_inputs number of the VoVNet stem
 ARCH_DLA34, ARCH_V2_99 = 0, 1
 # dd3d_arch of every arch key (dd3d_b200.arch.ARCH_KEYS)
 ARCH_IDS = {"dla34": ARCH_DLA34, "v2_99": ARCH_V2_99, "v2_19_slim_dw": 2, "v2_19_dw": 3, "v2_19_slim": 4, "v2_19": 5,
@@ -92,6 +93,7 @@ SIGNATURES = {
     "dd3d_set_backbone_norm": (_I, [_P, C.c_int32]),
     "dd3d_set_fpn_channels": (_I, [_P, C.c_int32]),
     "dd3d_set_canonical_sizes": (_I, [_P, C.c_int32, C.POINTER(C.c_float)]),
+    "dd3d_set_fpn_inputs": (_I, [_P, C.POINTER(C.c_int32), _I]),
     "dd3d_set_in_features": (_I, [_P, C.POINTER(C.c_int32), _I]),
     "dd3d_load_weight": (_I, [_P, C.c_char_p, _P, C.POINTER(_I64), _I]),
     "dd3d_finalize": (_I, [_P]),
@@ -252,12 +254,23 @@ def max_candidates(cfg):
     return len(in_feature_levels(cfg)) * int(cfg.DD3D.FCOS2D.INFERENCE.PRE_NMS_TOPK)
 
 
+def fpn_inputs_from_cfg(cfg):
+    """FE.FPN.IN_FEATURES as the int32 array of dd3d_set_fpn_inputs (level<k> / stage<k> -> k, the VoVNet stem ->
+    FPN_IN_STEM), or None for the builder's default list (the default graph, which needs no call)."""
+    from .arch import DEFAULT_FPN_INPUTS, DLA_SPECS, arch_of, fpn_inputs
+    names = [name for name, _ in fpn_inputs(cfg)]
+    if names == DEFAULT_FPN_INPUTS[arch_of(cfg) in DLA_SPECS]:
+        return None
+    nums = [FPN_IN_STEM if name == "stem" else int(name[-1]) for name in names]
+    return (C.c_int32 * len(nums))(*nums), len(nums)
+
+
 def in_features_from_cfg(cfg):
-    """DD3D.IN_FEATURES as the int32 array of dd3d_set_in_features, or None for all five FPN outputs in order (the default
+    """DD3D.IN_FEATURES as the int32 array of dd3d_set_in_features, or None for every FPN output in order (the default
     graph, which needs no call)."""
-    from .arch import in_feature_levels
+    from .arch import fpn_output_names, in_feature_levels
     levels = in_feature_levels(cfg)
-    if levels == list(range(5)):
+    if levels == list(range(len(fpn_output_names(cfg)))):
         return None
     return (C.c_int32 * len(levels))(*levels), len(levels)
 

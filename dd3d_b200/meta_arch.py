@@ -14,7 +14,7 @@ import torch
 from torch import nn
 
 from . import lib as _lib
-from .arch import arch_of, check_fpn_channels, is_nuscenes_arch, param_specs, size_divisibility
+from .arch import arch_of, check_fpn_channels, check_fpn_inputs, is_nuscenes_arch, param_specs, size_divisibility
 from .structures import Boxes, Boxes3D, GenericBoxes3D, Instances
 
 try:  # register next to the reference's DD3D when detectron2 is present (scripts/train.py:48 build_model)
@@ -38,6 +38,7 @@ class DD3DB200(nn.Module):
         self.bev_nms_iou_thresh = cfg.DD3D.INFERENCE.BEV_NMS_IOU_THRESH
         self.backbone = SimpleNamespace(size_divisibility=size_divisibility(cfg))
         self._specs = param_specs(cfg)  # the reference's own errors first (nn.GroupNorm's ValueError for GN widths)
+        check_fpn_inputs(cfg)  # the top block's p5 lookup; FPN inputs of stride >= 4 and at most 5 head levels
         self._fpn_channels = check_fpn_channels(cfg)  # FE.FPN.OUT_CHANNELS: a multiple of 64 in [64, 512]
         if not 1 <= self.num_classes <= _lib.MAX_NUM_CLASSES:
             raise NotImplementedError(f"DD3D.NUM_CLASSES = {self.num_classes} is not supported: the engine builds 1 to "
@@ -51,6 +52,7 @@ class DD3DB200(nn.Module):
         self._device = torch.device("cpu")
         self._desc = _lib.desc_from_cfg(cfg)
         self._layout = _lib.layout_from_cfg(cfg)
+        self._fpn_inputs = _lib.fpn_inputs_from_cfg(cfg)  # FE.FPN.IN_FEATURES
         self._in_features = _lib.in_features_from_cfg(cfg)  # KeyError / NotImplementedError for lists the engine cannot run
         if cfg.DD3D.FCOS2D.USE_DEFORMABLE or (cfg.MODEL.BOX3D_ON and cfg.DD3D.FCOS3D.USE_DEFORMABLE):
             raise ValueError("Not supported yet.")  # fcos2d.py:51-52, fcos3d.py:77-78
@@ -138,6 +140,8 @@ class DD3DB200(nn.Module):
             _lib.check(L.dd3d_set_layout(handle, C.byref(self._layout)), handle)
             _lib.check(L.dd3d_set_backbone_norm(handle, self._backbone_norm), handle)
             _lib.check(L.dd3d_set_fpn_channels(handle, self._fpn_channels), handle)
+            if self._fpn_inputs is not None:  # before dd3d_set_in_features, whose indices range over the FPN's outputs
+                _lib.check(L.dd3d_set_fpn_inputs(handle, *self._fpn_inputs), handle)
             if self._in_features is not None:
                 _lib.check(L.dd3d_set_in_features(handle, *self._in_features), handle)
             if self._canon is not None:

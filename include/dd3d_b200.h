@@ -64,7 +64,9 @@ enum dd3d_act_dtype { DD3D_ACT_BF16 = 0, DD3D_ACT_FP16 = 1 };
 
 #define DD3D_MAX_CLASSES 16      /* rows of dd3d_model_desc.canonical_box3d_sizes */
 #define DD3D_MAX_NUM_CLASSES 128 /* largest DD3D.NUM_CLASSES: above DD3D_MAX_CLASSES the sizes come from dd3d_set_canonical_sizes */
-#define DD3D_NUM_LEVELS 5
+#define DD3D_NUM_LEVELS 5      /* most head levels (DD3D.IN_FEATURES entries) one engine runs */
+#define DD3D_FPN_MAX_OUTPUTS 6 /* most FPN outputs: DLA level2..5 give p2..p7 */
+#define DD3D_FPN_IN_STEM 1     /* dd3d_set_fpn_inputs number of the VoVNet stem output */
 
 /* Mirrors the cfg values DD3D.__init__ / FCOS2DInference / FCOS3DInference read
  * (core.py:20-55, fcos2d.py:242-249, fcos3d.py:302-313; defaults configs/models/dd3d.yaml). */
@@ -154,7 +156,9 @@ typedef struct dd3d_tta_view {
 int dd3d_create(const dd3d_model_desc* h_desc, dd3d_handle* out);
 void dd3d_destroy(dd3d_handle h);
 const char* dd3d_last_error(dd3d_handle h); /* h may be NULL: error of the last failed dd3d_create */
-int dd3d_size_divisibility(dd3d_handle h);  /* backbone.size_divisibility: 128 (DLA p67) / 64 (V2-99 p6) */
+/* backbone.size_divisibility: 128 (DLA p67) / 64 (VoVNet p6).  Every FPN input list the engine builds ends at stride 32
+ * (dd3d_set_fpn_inputs), so the FPN inputs never change it. */
+int dd3d_size_divisibility(dd3d_handle h);
 /* Sets the FPN / head layout (dd3d_layout_desc) before dd3d_finalize (DD3D_ERR_STATE afterwards).  An unknown dd3d_norm value,
  * a depth outside 0..16 or fpn_fuse_avg other than 0 / 1 returns DD3D_ERR_INVALID and leaves the layout unchanged. */
 int dd3d_set_layout(dd3d_handle h, const dd3d_layout_desc* h_layout);
@@ -176,13 +180,23 @@ int dd3d_set_fpn_channels(dd3d_handle h, int32_t channels);
  * replaces them.  Class-specific heads above 16 classes run the box3d predictor at the final candidates only, 11 channels
  * each, on the class-gathered kernel (csrc/b3d_gather.cu) under the "sparse_box3d" rule of dd3d_set_option. */
 int dd3d_set_canonical_sizes(dd3d_handle h, int32_t num_classes, const float* h_sizes);
+/* Sets FE.FPN.IN_FEATURES before dd3d_finalize and before dd3d_set_in_features (DD3D_ERR_STATE otherwise): h_inputs[0 .. n)
+ * are the backbone outputs the FPN reads, by number: DLA level<k> is k, VoVNet stage<k> is k and the VoVNet stem is
+ * DD3D_FPN_IN_STEM.  Their strides (DLA 2^k; VoVNet stem and stage2 4, stage<k> 2^k) must double from one input to the next
+ * and end at 32, where the top block reads p5, with the first stride at least 4: DLA level2..5 and VoVNet stem / stage2..5.
+ * The FPN outputs are p<log2 first stride> .. p5, then P6 (and P7 for a DLA): 2 to DD3D_FPN_MAX_OUTPUTS outputs; lateral /
+ * output convs are named fpn_lateral<log2 stride> / fpn_output<log2 stride>.  Any other list returns DD3D_ERR_INVALID and
+ * leaves the inputs unchanged.  An engine that never receives the call builds DLA level3..5 / VoVNet stage2..5.  With more
+ * than DD3D_NUM_LEVELS FPN outputs, dd3d_set_in_features must select at most DD3D_NUM_LEVELS of them (dd3d_finalize returns
+ * DD3D_ERR_INVALID otherwise). */
+int dd3d_set_fpn_inputs(dd3d_handle h, const int32_t* h_inputs, int n);
 /* Sets DD3D.IN_FEATURES before dd3d_finalize (DD3D_ERR_STATE afterwards): h_fpn_levels[0 .. n) are the FPN outputs the heads
- * run on, in head order, as indices 0..4 into the FPN's outputs (DLA: p3..p7, VoVNet: p2..p6), 1 <= n <= DD3D_NUM_LEVELS,
- * no index twice (DD3D_ERR_INVALID otherwise, leaving the selection unchanged).  Every per-level tensor is taken by position:
+ * run on, in head order, as indices into the FPN's outputs (by default DLA: p3..p7, VoVNet: p2..p6; dd3d_set_fpn_inputs
+ * changes them), 1 <= n <= DD3D_NUM_LEVELS, no index twice (DD3D_ERR_INVALID otherwise, leaving the selection unchanged).  Every per-level tensor is taken by position:
  * tower norm l, Scale l, Offset l and (PER_LEVEL_PREDICTORS) predictor l serve the head at position l, and dd3d_det.level is
  * the position.  FPN outputs no head reads are not computed (dd3d_get_tensor refuses their "p<i>"); the head maps
  * "cls<l>" / "box<l>" / "b3d<l>" are by position.  Without DO_NMS up to n * pre_nms_topk detections per image survive.  An
- * engine that never receives the call runs all five levels in order. */
+ * engine that never receives the call runs every FPN output in order. */
 int dd3d_set_in_features(dd3d_handle h, const int32_t* h_fpn_levels, int n);
 
 /* ---- weights: one call per tensor of the reference state_dict (Checkpointer.load, scripts/train.py:52) ----- */
