@@ -161,6 +161,10 @@ int dd3d_set_conv_policy(const char* name, int value) {
         conv_set_n_split(value);
         return DD3D_OK;
     }
+    if (!strcmp(name, "stagger")) {
+        conv_set_stagger(value);
+        return DD3D_OK;
+    }
     if (!strcmp(name, "pair_tile")) {
         conv_set_pair(value);
         return DD3D_OK;
@@ -493,7 +497,7 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
         ok = ok && make_act_map_s2(&g.in_map[0], d_in, 0, B, H, W, cin, in_pitch, g.th, g.tw, g_op_fp16) &&
              make_act_map_s2(&g.in_map[1], d_in, 1, B, H, W, cin, in_pitch, g.th, g.tw, g_op_fp16);
     }
-    if (!out_f32) ok = ok && make_act_map(&g.out_map, d_out, B, Ho, Wo, cout, out_pitch, g.th, g.tw, g_op_fp16);
+    if (!out_f32) ok = ok && make_out_map(&g.out_map, d_out, B, Ho, Wo, cout, out_pitch, g.tw, g_op_fp16);
     if (!ok) {
         fprintf(stderr, "dd3d_op_conv2d: %s\n", conv_last_error());
         return DD3D_ERR_CUDA;
@@ -567,7 +571,7 @@ int dd3d_op_conv2d_grouped(const void* d_in, int B, int H, int W, int C, int in_
         ok = make_act_map_s2(&g.in_map[0], d_in, 0, B, H, W, C, in_pitch, g.th, g.tw, g_op_fp16) &&
              make_act_map_s2(&g.in_map[1], d_in, 1, B, H, W, C, in_pitch, g.th, g.tw, g_op_fp16);
     }
-    ok = ok && make_act_map(&g.out_map, d_out, B, Ho, Wo, C, out_pitch, g.th, g.tw, g_op_fp16) &&
+    ok = ok && make_out_map(&g.out_map, d_out, B, Ho, Wo, C, out_pitch, g.tw, g_op_fp16) &&
          make_weight_map(&p.w_map, d_w, 9 * kBlockK, C, kBlockK, g_op_fp16);
     if (!ok) {
         fprintf(stderr, "dd3d_op_conv2d_grouped: %s\n", conv_last_error());
@@ -613,7 +617,7 @@ int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_
     g.tw = kHaloTw;
     if (((H + kHaloTh - 1) / kHaloTh) * ((W + kHaloTw - 1) / kHaloTw) >= kTileListMaxTiles) return DD3D_ERR_INVALID;
     if (!make_act_map_halo(&g.in_map[0], d_in, B, H, W, cin, in_pitch, g_op_fp16) ||
-        !make_act_map(&g.out_map, d_out, B, H, W, cout, out_pitch, g.th, g.tw, g_op_fp16) ||
+        !make_out_map(&g.out_map, d_out, B, H, W, cout, out_pitch, g.tw, g_op_fp16) ||
         !make_weight_map(&p.w_map, d_w, 9 * kchunks * kBlockK, cout, p.block_n, g_op_fp16)) {
         fprintf(stderr, "dd3d_op_conv2d_tiles: %s\n", conv_last_error());
         return DD3D_ERR_CUDA;

@@ -313,6 +313,11 @@ bool conv_prefer_halo(int taps, int stride, int block_n, int nseg, const int* Hs
     return halo_tiles * 100 <= gen_tiles * 110;  // fixed 16x8 tiling may cost at most 10 % more tiles
 }
 
+bool make_out_map(CUtensorMap* map, const void* base, int B, int H, int W, int C, int pitch, int tw, int fp16) {
+    const int bw = std::min(tw, 64);
+    return make_act_map(map, base, B, H, W, C, pitch, 64 / bw, bw, fp16);
+}
+
 bool make_weight_map(CUtensorMap* map, const void* base, int ktot, int cout_pad, int block_n, int fp16) {
     cuuint64_t dims[2] = {(cuuint64_t)ktot, (cuuint64_t)cout_pad};
     cuuint64_t strides[1] = {(cuuint64_t)ktot * 2};
@@ -346,12 +351,16 @@ static int conv_units_per_image(const ConvParams& p, const ConvSeg& g) {
     return p.pair ? (tiles + 1) / 2 : tiles;
 }
 
-// Dynamic shared memory of everything but the B ring: staging tiles, alignment slack, barriers, (scale, bias) vectors and
-// the A patches (pair tile: two staging tiles per consumer warpgroup, two patches per A stage).
+// Dynamic shared memory of everything but the B ring: staging tiles, alignment slack, barriers, (scale, bias) vectors, the
+// eSE partials hand-over (generic variant) and the A patches (pair tile: two staging tiles per consumer warpgroup, two
+// patches per A stage).
 static int conv_fixed_smem(const ConvParams& p) {
-    return (p.pair ? 4 : 2) * kStagingBytes + 1024 /*alignment slack*/ + kBarBytes + kSbBytes +
+    return (p.pair ? 4 : 2) * kStagingBytes + 1024 /*alignment slack*/ + kBarBytes + kSbBytes + (p.halo ? 0 : kPoolXBytes) +
            p.a_stages * (p.pair ? 2 : 1) * kHaloABytes;
 }
+
+static int g_stagger = -1;
+void conv_set_stagger(int mode) { g_stagger = mode >= 0 ? mode : -1; }
 
 void conv_finalize_params(ConvParams* p) {
     int unit = 0;
@@ -389,6 +398,12 @@ void conv_finalize_params(ConvParams* p) {
     }
     int stages = (kSmemBudget - conv_fixed_smem(*p)) / stage_bytes;
     p->num_stages = p->wstat ? 2 : std::max(2, std::min(kMaxStages, stages));
+    // Consumer skew: the leading warpgroup may run at most (ring depth - 1) k-blocks ahead of the other one, and one more slot
+    // keeps a TMA load in flight ahead of it, so stagger <= num_stages - 2.  Weight-stationary layers have no B ring: there
+    // the A patches (9 k-blocks each) bound it, and a_stages >= 3 leaves more than kMaxStagger.
+    const int bound = std::min(kMaxStagger, p->wstat ? 9 * (p->a_stages - 2) : p->num_stages - 2);
+    // (and at most one item's k-blocks: warpgroup 1 signals the skew from its first item)
+    p->stagger = std::max(0, std::min(p->taps * p->kchunks, g_stagger < 0 ? bound : std::min(g_stagger, bound)));
 }
 
 static int g_n_split = -1;

@@ -68,6 +68,9 @@ struct ConvParams {
     // *tile_count entries, read on the device after griddepcontrol.wait.  total_work then only sizes the grid.
     const uint32_t* tile_list;
     const int32_t* tile_count;
+    // k-blocks consumer warpgroup 2 starts behind warpgroup 1 (0: both start together); conv_finalize_params picks it so
+    // that num_stages >= stagger + 2 and the leading warpgroup keeps TMA lookahead
+    int stagger;
 };
 constexpr int kTileListMaxImages = 1 << 13, kTileListMaxTiles = 1 << 16;  // field widths of a tile_list entry
 static_assert(sizeof(ConvParams) <= 4096, "kernel parameter space");
@@ -77,6 +80,9 @@ const char* conv_last_error();
 bool make_act_map(CUtensorMap* map, const void* base, int B, int H, int W, int C, int pitch, int th, int tw, int fp16 = 0);
 bool make_act_map_s2(CUtensorMap* map, const void* base, int wp, int B, int H, int W, int C, int pitch, int th,
                      int tw, int fp16 = 0);
+// Output map of the conv kernel (out_mode 0) for tiles tw pixels wide: the box is one consumer warpgroup's half of the
+// 128-pixel tile, its first 64 pixels in row-major order (64 / tw rows of tw pixels, or 1 x 64 for the 1 x 128 tile).
+bool make_out_map(CUtensorMap* map, const void* base, int B, int H, int W, int C, int pitch, int tw, int fp16 = 0);
 bool make_weight_map(CUtensorMap* map, const void* base, int ktot, int cout_pad, int block_n, int fp16 = 0);
 void choose_tile(int H, int W, int* th, int* tw);
 int conv_tiles_per_image(int H, int W);  // M-tiles per image of the generic tiling
@@ -105,6 +111,9 @@ void conv_set_n_split(int mode);  // 0 off, 1 on, -1 environment / default (on)
 // the 128-pixel tile and the N-split.  conv_set_pair / DD3D_CONV_PAIR=0: 0 off, 1 on wherever eligible, -1 default.
 bool conv_select_pair(ConvParams* p, int cout_pad, int num_sms);
 void conv_set_pair(int mode);
+// Consumer-warpgroup skew (ConvParams::stagger): -1 the default rule of conv_finalize_params, >= 0 that many k-blocks
+// (clamped to the same bound).  dd3d_set_conv_policy("stagger", v); for A/B runs and tests.
+void conv_set_stagger(int mode);
 // N tile of a layer with cout_pad output channels: cout_pad itself up to 256, 256 for multiples of 256, otherwise the
 // largest multiple of 64 that is <= 256 and divides cout_pad (384 -> 192: every 64-channel store box stays inside its
 // n-block).  0: no such tile (the width is refused).

@@ -58,6 +58,7 @@ namespace {
 
 constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KiB
 constexpr int kStagingBytes = kBlockM * 128;    // one 64-channel bf16 output chunk
+constexpr int kHalfStagingBytes = kStagingBytes / 2;  // its 64 rows of one consumer warpgroup (one TMA store box)
 constexpr int kMaxStages = 8;
 constexpr int kSmemBudget = 227 * 1024;
 // halo variant: per 64-channel block the A operand is ONE (16+2)x(8+2)-pixel patch = 180 rows of 128 B (64 channels),
@@ -68,8 +69,12 @@ constexpr int kHaloAStages = 3;   // default number of A patches in flight
 constexpr int kMaxAStages = 5;    // weight-stationary layers (ConvParams::wstat) spend the freed B ring on deeper A prefetch
 constexpr int kPairAStages = 2;   // pair tile: one patch pair feeds 9 k-blocks, so two pairs in flight suffice
 constexpr int kBarBytes = 512;
-constexpr int kSbBytes = 2 * 256 * 4;  // staged (scale, bias) vectors of the current (segment, n-block)
-constexpr int kConsumerWarps = 8, kEpiThreads = kConsumerWarps * 32;
+constexpr int kSbBytes = 2 * 2 * 256 * 4;  // per consumer warpgroup: staged (scale, bias) of its current (segment, n-block)
+// generic variant: the eSE pool partials handed from warpgroup 1 (rows 0..63) to warpgroup 2 (rows 64..127), per staging
+// buffer parity: 128 threads x 8 fp32
+constexpr int kPoolXBytes = 2 * 128 * 8 * 4;
+constexpr int kMaxStagger = 6;  // k-blocks by which consumer warpgroup 1 leads warpgroup 2 (ConvParams::stagger)
+constexpr int kConsumerWarps = 8;
 
 struct TileCoord {
     int seg, img, y0, x0, n_blk;
@@ -208,10 +213,14 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
     uint64_t* afull_bar = bars + 2 * kMaxStages;   // [kMaxAStages]
     uint64_t* aempty_bar = afull_bar + kMaxAStages;
     uint64_t* wfull_bar = aempty_bar + kMaxAStages;  // [1] resident weights landed (wstat)
-    // shared-window addresses of the epilogue's staging tiles and of the staged folded-BN vectors (explicit LDS / STS)
+    uint64_t* skew_bar = wfull_bar + 1;              // [1] warpgroup 1 has issued p.stagger k-blocks of its first item
+    uint64_t* poolx_full = skew_bar + 1;             // [2] eSE partials of rows 0..63 handed over (per staging parity)
+    uint64_t* poolx_empty = poolx_full + 2;          // [2] ... and taken
+    // shared-window addresses of the epilogue's staging tiles, the staged folded-BN vectors (per consumer warpgroup) and
+    // the eSE partials hand-over (explicit LDS / STS)
     const uint32_t staging_u32 = ptx::smem_u32(staging);
-    const uint32_t s_scale_u32 = ptx::smem_u32(reinterpret_cast<uint8_t*>(bars) + kBarBytes);  // [256] fp32 scale
-    const uint32_t s_bias_u32 = s_scale_u32 + 256 * 4;                                          // [256] fp32 bias
+    const uint32_t sb_u32 = ptx::smem_u32(reinterpret_cast<uint8_t*>(bars) + kBarBytes);
+    const uint32_t poolx_u32 = sb_u32 + kSbBytes;
 
     const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);  // provably warp-uniform
     const int lane = threadIdx.x & 31;
@@ -231,6 +240,11 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             ptx::mbar_init(&aempty_bar[i], kConsumerWarps);
         }
         ptx::mbar_init(wfull_bar, 1);
+        ptx::mbar_init(skew_bar, 1);
+        for (int i = 0; i < 2; ++i) {
+            ptx::mbar_init(&poolx_full[i], 128);
+            ptx::mbar_init(&poolx_empty[i], 128);
+        }
         ptx::fence_barrier_init();
     }
     __syncthreads();
@@ -365,24 +379,30 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
         }
     } else if (warp >= 4) {
         // ---------------------------------------------------------------- consumer warpgroups 1, 2
+        // Each warpgroup runs its epilogue on its own: its own staging buffers, named barrier, store leader and copy of the
+        // folded-BN vectors, so neither waits for the other between work items.  Warpgroup 2 starts p.stagger k-blocks
+        // behind warpgroup 1; the shared ring then keeps them staggered (DESIGN.md section 3): one warpgroup's epilogue
+        // runs while the other one's wgmmas keep the tensor pipe busy.
         const int wgi = (warp >> 2) - 1;                                 // rows 64 * wgi .. (PAIR: sub-tile wgi)
-        const int et = static_cast<int>(threadIdx.x) - 128;              // 0 .. kEpiThreads - 1
-        const int wl = (et >> 5) & 3;
-        // PAIR: each warpgroup stages and stores its own sub-tile, synchronised on its own named barrier
-        const bool store_leader = PAIR ? (et & 127) == 0 : (et == 0);
-        const uint32_t epi_bar = PAIR ? 2 + wgi : 1;
-        const uint32_t epi_threads = PAIR ? 128 : kEpiThreads;
+        const int wt = static_cast<int>(threadIdx.x) & 127;              // thread of the warpgroup
+        const int wl = warp & 3;
+        const bool store_leader = wt == 0;
+        const uint32_t epi_bar = 2 + wgi;
+        const uint32_t s_scale_u32 = sb_u32 + wgi * (kSbBytes / 2);  // [256] fp32 scale
+        const uint32_t s_bias_u32 = s_scale_u32 + 256 * 4;           // [256] fp32 bias
         const int out_mode = PAIR ? 0 : p.out_mode;
         const uint64_t desc_hi = ptx::make_sw128_desc(0, HALO ? kHaloPW * 128 : 1024) & ~0x3FFFull;
         const uint64_t bdesc_hi = ptx::make_sw128_desc(0, 1024) & ~0x3FFFull;
         const uint32_t smem_lo = ptx::smem_u32(smem) >> 4;
         const uint32_t halo_lo = ptx::smem_u32(halo_a) >> 4;
         const uint32_t stage_units = static_cast<uint32_t>(stage_bytes) >> 4;
-        // the rows of this thread's accumulator row-halves within the 128-pixel tile (2 per 64-row half)
+        // the rows of this thread's accumulator row-halves within the warpgroup's staging tile (2 per 64-row half); row0 + row
+        // is the pixel within the 128-pixel tile
+        const int row0 = PAIR ? 0 : 64 * wgi;
         int row[2 * MH];
 #pragma unroll
         for (int m = 0; m < MH; ++m) {
-            row[2 * m] = 64 * (PAIR ? m : wgi) + 16 * wl + (lane >> 2);
+            row[2 * m] = 64 * m + 16 * wl + (lane >> 2);
             row[2 * m + 1] = row[2 * m] + 8;
         }
         const int qc = 2 * (lane & 3);  // first of this thread's two columns in every 8-column group
@@ -392,8 +412,18 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
         int as = 0;
         uint32_t aphase = 0;
         int sbuf = 0;
+        uint32_t poolx_phase = 0;  // bit b: phase of the eSE hand-over of staging parity b
         int sb_key = -1;  // (segment, n-block) whose folded-BN vectors are staged in s_scale / s_bias
         if (wstat) ptx::mbar_wait(wfull_bar, 0);
+        if (wgi == 1 && p.stagger > 0 && w_first < w_total) ptx::mbar_wait(skew_bar, 0);
+        // warpgroup 1 releases warpgroup 2 once it has issued k-block p.stagger - 1 (<= kblocks - 1) of its first item
+        bool skew_pending = wgi == 0 && wt == 0 && p.stagger > 0;
+        auto skew_arrive = [&](int i) {
+            if (skew_pending && i + 1 == p.stagger) {
+                ptx::mbar_arrive(skew_bar);
+                skew_pending = false;
+            }
+        };
         for (int work = w_first; work < w_total; work += w_step) {
             const TileCoord t = decode_tile<PAIR, LIST>(p, work, PAIR ? wgi : 0);
             const ConvSeg& g = p.seg[t.seg];
@@ -425,6 +455,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                                                  bdesc_hi | b_lo, (kc | tap) == 0);
                         else
                             mma_kblock<BN, F16>(acc[0], desc_hi | a_tap, bdesc_hi | b_lo, (kc | tap) == 0);
+                        skew_arrive(9 * kc + tap);
                         wg::wait<1>();
                         release();
                         rel_stage = wstat ? -1 : stage;
@@ -445,6 +476,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                     const uint32_t a_lo = smem_lo + static_cast<uint32_t>(stage) * stage_units + wgi * (64 * 128 / 16);
                     const uint32_t b_lo = smem_lo + static_cast<uint32_t>(stage) * stage_units + (kABytes >> 4);
                     mma_kblock<BN, F16>(acc[0], desc_hi | a_lo, bdesc_hi | b_lo, kb == 0);
+                    skew_arrive(kb);
                     wg::wait<1>();
                     release();
                     rel_stage = stage;
@@ -461,13 +493,15 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
 
             // ---- epilogue of this warpgroup's 64 rows (PAIR: of its 128-row sub-tile)
             const int n_base = t.n_blk * BN;
+            const int tw = HALO ? kHaloTw : g.tw, tw_shift = HALO ? 3 : g.tw_shift;  // the halo tile is 16 x 8
+            static_assert(kHaloTw == 8, "tw_shift of the halo tile");
             bool in_img[2 * MH];
             const __nv_bfloat16* res_ptr[2 * MH];
             float* f32_ptr[2 * MH];
 #pragma unroll
             for (int h = 0; h < 2 * MH; ++h) {
-                const int ly = row[h] >> g.tw_shift;
-                const int lx = row[h] - (ly << g.tw_shift);
+                const int ly = (row0 + row[h]) >> tw_shift;
+                const int lx = (row0 + row[h]) - (ly << tw_shift);
                 const int oy = t.y0 + ly, ox = t.x0 + lx;
                 in_img[h] = (oy < g.H) && (ox < g.W);
                 res_ptr[h] = nullptr;
@@ -481,30 +515,35 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                 if (out_mode == 1 && in_img[h])
                     f32_ptr[h] = g.out_f32 + (static_cast<size_t>(t.img * g.H + oy) * g.W + ox) * g.out_pitch + n_base + qc;
             }
-            // per-channel (scale, bias) of this (segment, n-block) in shared memory: broadcast LDS instead of LDG with their
-            // 64-bit address arithmetic.  The previous tile's readers are past the closing barrier of its last chunk.
+            // per-channel (scale, bias) of this (segment, n-block) in this warpgroup's shared copy: broadcast LDS instead of LDG
+            // with their 64-bit address arithmetic.  The first barrier waits for the warpgroup's readers of the previous copy.
             const int key = t.seg * 64 + t.n_blk;
             if (key != sb_key) {
-                ptx::named_bar_sync(1, kEpiThreads);
+                ptx::named_bar_sync(epi_bar, 128);
                 sb_key = key;
-                if (et < BN) {
-                    ptx::st_shared_f32(s_scale_u32 + et * 4, __ldg(g.scale + n_base + et));
-                    ptx::st_shared_f32(s_bias_u32 + et * 4, __ldg(g.bias + n_base + et));
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int ch = wt + 128 * i;
+                    if (ch < BN) {
+                        ptx::st_shared_f32(s_scale_u32 + ch * 4, __ldg(g.scale + n_base + ch));
+                        ptx::st_shared_f32(s_bias_u32 + ch * 4, __ldg(g.bias + n_base + ch));
+                    }
                 }
-                ptx::named_bar_sync(1, kEpiThreads);
+                ptx::named_bar_sync(epi_bar, 128);
             }
             const bool has_res = g.residual != nullptr;
 
 #pragma unroll
             for (int c = 0; c < (BN + 63) / 64; ++c) {
                 const int c0 = 64 * c;
-                const int sb = PAIR ? 2 * wgi + sbuf : sbuf;
-                uint8_t* stag = staging + sb * kStagingBytes;
-                const uint32_t stag_u32 = staging_u32 + sb * kStagingBytes;
+                // this warpgroup's staging buffer of parity sbuf: MH x 64 rows
+                const int sb_off = (2 * wgi + sbuf) * MH * kHalfStagingBytes;
+                uint8_t* stag = staging + sb_off;
+                const uint32_t stag_u32 = staging_u32 + sb_off;
                 if (out_mode == 0) {
                     // the TMA store that last read this staging buffer must have drained
                     if (store_leader) ptx::tma_store_wait_read<1>();
-                    ptx::named_bar_sync(epi_bar, epi_threads);
+                    ptx::named_bar_sync(epi_bar, 128);
                 }
 #pragma unroll
                 for (int jj = 0; jj < 8; ++jj) {
@@ -544,23 +583,40 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                 }
                 if (out_mode == 0) {
                     ptx::fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the TMA engine
-                    ptx::named_bar_sync(epi_bar, epi_threads);
+                    ptx::named_bar_sync(epi_bar, 128);
                     if (store_leader) {
-                        ptx::tma_store_4d(&g.out_map, stag, n_base + c0, t.x0, t.y0, t.img);
+                        // one box per 64-pixel half: the out map's box is the first 64 pixels of a tile in row-major order
+#pragma unroll
+                        for (int m = 0; m < MH; ++m) {
+                            const int px = 64 * (PAIR ? m : wgi);
+                            ptx::tma_store_4d(&g.out_map, stag + m * kHalfStagingBytes, n_base + c0, t.x0 + (px & (tw - 1)),
+                                              t.y0 + (px >> tw_shift), t.img);
+                        }
                         ptx::tma_store_commit();
                     }
-                    if (!PAIR && g.pool_partial != nullptr && et < 128) {
+                    if (!HALO && !PAIR && g.pool_partial != nullptr) {
                         // eSE global-average-pool, fused: per-tile channel sums of the 16-bit tile just staged (exactly the
                         // values the reference pools, vovnet.py:181).  Thread e covers channels 8*(e&7).. of rows
                         // (e>>3) + 16*i; the 4 row-groups of a warp are shuffle-reduced; one fp32 partial per
-                        // (tile, warp, channel) -> deterministic reduction later (no atomics).
-                        const int e = et;
+                        // (tile, warp, channel) -> deterministic reduction later (no atomics).  Rows i < 4 are warpgroup 1's:
+                        // thread e of warpgroup 1 hands its running sums to thread e of warpgroup 2, which adds rows i >= 4 in
+                        // the same order, reduces and stores.
+                        const int e = wt;
                         const int cg = e & 7;
+                        const uint32_t px_u32 = poolx_u32 + sbuf * (kPoolXBytes / 2) + e * 16;
+                        const uint32_t par = (poolx_phase >> sbuf) & 1;
                         float ps[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+                        if (wgi == 1) {
+                            ptx::mbar_wait(&poolx_full[sbuf], par);
+                            const float4 a = ptx::ld_shared_f4(px_u32), b = ptx::ld_shared_f4(px_u32 + 128 * 16);
+                            ps[0] = a.x, ps[1] = a.y, ps[2] = a.z, ps[3] = a.w;
+                            ps[4] = b.x, ps[5] = b.y, ps[6] = b.z, ps[7] = b.w;
+                            ptx::mbar_arrive(&poolx_empty[sbuf]);
+                        }
 #pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const int r = (e >> 3) + 16 * i;
-                            const int ry = t.y0 + (r >> g.tw_shift), rx = t.x0 + (r & (g.tw - 1));
+                        for (int i = 0; i < 4; ++i) {
+                            const int r = (e >> 3) + 16 * i;  // row of the staging buffer, row0 + r of the tile
+                            const int ry = t.y0 + ((row0 + r) >> g.tw_shift), rx = t.x0 + ((row0 + r) & (g.tw - 1));
                             if (ry < g.H && rx < g.W) {
                                 const uint4 u = ptx::ld_shared_v4(stag_u32 + r * 128 + ((cg ^ (r & 7)) << 4));
                                 const uint32_t* b2 = reinterpret_cast<const uint32_t*>(&u);
@@ -572,19 +628,28 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                                 }
                             }
                         }
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            ps[j] += __shfl_xor_sync(0xffffffffu, ps[j], 8);
-                            ps[j] += __shfl_xor_sync(0xffffffffu, ps[j], 16);
+                        if (wgi == 0) {
+                            ptx::mbar_wait(&poolx_empty[sbuf], par ^ 1);
+                            ptx::st_shared_f4(px_u32, make_float4(ps[0], ps[1], ps[2], ps[3]));
+                            ptx::st_shared_f4(px_u32 + 128 * 16, make_float4(ps[4], ps[5], ps[6], ps[7]));
+                            ptx::mbar_arrive(&poolx_full[sbuf]);
                         }
-                        if (lane < 8 && c0 + cg * 8 < BN) {
-                            const int tile_in_img = (t.y0 / g.th) * g.tiles_x + (t.x0 / g.tw);
-                            float* dst = g.pool_partial +
-                                         ((static_cast<size_t>(t.img) * (g.tiles_x * g.tiles_y) + tile_in_img) * 4 + (et >> 5)) *
-                                             g.pool_pitch +
-                                         n_base + c0 + cg * 8;
-                            *reinterpret_cast<float4*>(dst) = make_float4(ps[0], ps[1], ps[2], ps[3]);
-                            *reinterpret_cast<float4*>(dst + 4) = make_float4(ps[4], ps[5], ps[6], ps[7]);
+                        poolx_phase ^= 1u << sbuf;
+                        if (wgi == 1) {
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) {
+                                ps[j] += __shfl_xor_sync(0xffffffffu, ps[j], 8);
+                                ps[j] += __shfl_xor_sync(0xffffffffu, ps[j], 16);
+                            }
+                            if (lane < 8 && c0 + cg * 8 < BN) {
+                                const int tile_in_img = (t.y0 / g.th) * g.tiles_x + (t.x0 / g.tw);
+                                float* dst = g.pool_partial +
+                                             ((static_cast<size_t>(t.img) * (g.tiles_x * g.tiles_y) + tile_in_img) * 4 + (e >> 5)) *
+                                                 g.pool_pitch +
+                                             n_base + c0 + cg * 8;
+                                *reinterpret_cast<float4*>(dst) = make_float4(ps[0], ps[1], ps[2], ps[3]);
+                                *reinterpret_cast<float4*>(dst + 4) = make_float4(ps[4], ps[5], ps[6], ps[7]);
+                            }
                         }
                     }
                     sbuf ^= 1;

@@ -546,7 +546,7 @@ struct Builder {
             } else {
                 if (sp.out.H != Ho || sp.out.W != Wo || sp.out.C != L.cout)
                     fail(DD3D_ERR_INVALID, "conv output view mismatch");
-                if (!make_act_map(&g.out_map, sp.out.ptr, B, Ho, Wo, sp.out.C, sp.out.pitch, g.th, g.tw, E->fp16))
+                if (!make_out_map(&g.out_map, sp.out.ptr, B, Ho, Wo, sp.out.C, sp.out.pitch, g.tw, E->fp16))
                     fail(DD3D_ERR_CUDA, conv_last_error());
                 g.out16 = sp.out.ptr;
                 g.out_pitch = sp.out.pitch;

@@ -1,8 +1,10 @@
-"""A/B of the conv tile policy: interleaved V2-99 forwards with the 256 x 128 pair tile off (policy "pair_tile" 0) and on by
-the default rule (-1), in one process.  Prints per conv launch (tagged by layer shape) the median device ms and TFLOP/s of
-both, per-shape group totals, the step totals and their spread over the rounds.
+"""A/B of a conv policy (dd3d_set_conv_policy) in one process: interleaved V2-99 forwards under two values of it, by default
+the 256 x 128 pair tile off (policy "pair_tile" 0) against the default rule (-1); --policy stagger --old 0 times the
+consumer-warpgroup skew off against its default.  Prints per conv launch (tagged by layer shape) the median device ms and
+TFLOP/s of both, per-shape group totals, the step totals and their spread over the rounds.
 
-    python tools/ab_conv_tile.py [--workload v2_99] [--batch 32] [--rounds 5] [--json out.json]
+    python tools/ab_conv_tile.py [--policy pair_tile] [--old 0] [--new -1] [--workload v2_99] [--batch 32] [--rounds 5]
+                                 [--json out.json]
 """
 import argparse
 import json
@@ -36,6 +38,9 @@ def main():
     ap.add_argument("--batch", type=int, default=0, help="0: the workload's batch size")
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--policy", default="pair_tile", help="dd3d_set_conv_policy name")
+    ap.add_argument("--old", type=int, default=0, help="policy value of the 'old' leg")
+    ap.add_argument("--new", type=int, default=-1, help="policy value of the 'new' leg (-1: the default)")
     args = ap.parse_args()
     arch, ds, B, H, W, focal, _ = WORKLOADS[args.workload]
     B = args.batch or B
@@ -43,11 +48,12 @@ def main():
     sd = make_state_dict(cfg)
     inp = make_inputs(B, H, W, focal)
     L = lib.load()
-    modes = {"old": 0, "pair": -1}
+    modes = {"old": args.old, "new": args.new}
+    policy = args.policy.encode()
     models, info = {}, {}
     try:
         for name, mode in modes.items():  # the policy is read when the plan is made: one model (plan) per policy
-            assert L.dd3d_set_conv_policy(b"pair_tile", mode) == 0
+            assert L.dd3d_set_conv_policy(policy, mode) == 0
             m = DD3DB200(cfg).to("cuda")
             m.load_state_dict(sd)
             for _ in range(3):
@@ -56,7 +62,7 @@ def main():
             info[name] = m.get_conv_info()
             models[name] = m
     finally:
-        L.dd3d_set_conv_policy(b"pair_tile", -1)
+        L.dd3d_set_conv_policy(policy, -1)
     times = {n: [] for n in modes}
     steps = {n: [] for n in modes}
     walls = {n: [] for n in modes}
@@ -78,10 +84,10 @@ def main():
             walls[name].append(e0.elapsed_time(e1))
     med = {n: {op: statistics.median(r[op] for r in times[n]) for op in times[n][0]} for n in modes}
     rows, groups = [], {}
-    for i, (c_old, c_new) in enumerate(zip(info["old"], info["pair"])):
+    for i, (c_old, c_new) in enumerate(zip(info["old"], info["new"])):
         if c_old is None:
             continue
-        a, b, f = med["old"][i], med["pair"][i], flops[i]
+        a, b, f = med["old"][i], med["new"][i], flops[i]
         k = tag(c_old)
         rows.append(dict(op=i, shape=k, pair=int(c_new["pair"]), old_ms=a, new_ms=b, gflop=f / 1e9))
         g = groups.setdefault((k, int(c_new["pair"])), [0, 0.0, 0.0, 0.0])
@@ -89,7 +95,8 @@ def main():
         g[1] += a
         g[2] += b
         g[3] += f
-    print(json.dumps(dict(gpu=gpu_info(0), workload=args.workload, batch=B, rounds=args.rounds)))
+    print(json.dumps(dict(gpu=gpu_info(0), workload=args.workload, batch=B, rounds=args.rounds, policy=args.policy,
+                          old=args.old, new=args.new)))
     print(f"{'op':>4} {'shape':18} {'pair':>4} {'old ms':>8} {'new ms':>8} {'old TF/s':>8} {'new TF/s':>8} {'gain':>6}")
     for r in rows:
         tf = lambda ms: r["gflop"] / ms if ms > 0 else 0.0  # noqa: E731  GFLOP / ms = TFLOP/s
