@@ -246,11 +246,6 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value) {
             e.opt_profile = value ? 1 : 0;
         } else if (n == "workspace_reuse") {  // applies to plans made afterwards
             e.opt_workspace_reuse = value ? 1 : 0;
-        } else if (n == "ese_pool") {  // 1: stage-final eSE pass fused with the next stage's max-pool; 0 (default): separate kernels
-            if (e.opt_ese_pool != (value ? 1 : 0)) e.drop_plans();
-            e.opt_ese_pool = value ? 1 : 0;
-        } else if (n == "stem_mma") {  // 1 (default): VoVNet stem_1 on stem_mma.cu; 0: stem_tc.cu (same op graph)
-            e.opt_stem_mma = value ? 1 : 0;
         } else if (n == "sparse_box3d") {  // 2 (default): auto by head size; 1: always sparse; 0: dense fp32 maps
             const int v = value < 0 ? 0 : (value > 2 ? 2 : value);
             if (e.opt_sparse_box3d != v) e.drop_plans();
@@ -263,9 +258,6 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value) {
             const int v = value < 0 ? 0 : (value > 2 ? 2 : value);
             if (e.opt_sparse_box2d_tower != v) e.drop_plans();
             e.opt_sparse_box2d_tower = v;
-        } else if (n == "dla_front") {  // 1 (default): fused DLA-34 front end (dla_front.cu); 0: layer by layer
-            if (e.opt_dla_front != (value ? 1 : 0)) e.drop_plans();
-            e.opt_dla_front = value ? 1 : 0;
         } else if (n == "workspace_fill") {
             e.opt_workspace_fill = (value >= 0 && value <= 255) ? value : -1;
         } else {
@@ -486,7 +478,7 @@ int dd3d_op_conv2d(const void* d_in, int B, int H, int W, int cin, int in_pitch,
     g.W = Wo;
     choose_tile(Ho, Wo, &g.th, &g.tw);
     bool ok = true;
-    p.halo = conv_prefer_halo(taps, stride, block_n, 1, &Ho, &Wo) ? conv_halo_mode() : 0;
+    p.halo = conv_prefer_halo(taps, stride, block_n, 1, &Ho, &Wo) ? 1 : 0;
     if (p.halo) {
         g.th = kHaloTh;
         g.tw = kHaloTw;
@@ -560,7 +552,7 @@ int dd3d_op_conv2d_grouped(const void* d_in, int B, int H, int W, int C, int in_
     g.W = Wo;
     choose_tile(Ho, Wo, &g.th, &g.tw);
     bool ok = true;
-    p.halo = conv_prefer_halo(9, stride, kBlockK, 1, &Ho, &Wo) ? conv_halo_mode() : 0;
+    p.halo = conv_prefer_halo(9, stride, kBlockK, 1, &Ho, &Wo) ? 1 : 0;
     if (p.halo) {
         g.th = kHaloTh;
         g.tw = kHaloTw;
@@ -604,7 +596,7 @@ int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_
     p.relu = relu;
     p.fp16 = g_op_fp16;
     // the pair tile in work-list mode, whatever the pair / halo policies choose for dd3d_op_conv2d
-    p.halo = conv_halo_mode();
+    p.halo = 1;
     p.pair = 1;
     p.block_n = 128;
     p.n_blocks = cout / 128;
@@ -653,7 +645,7 @@ int dd3d_op_conv2d_taps_tiles(const void* d_in, int B, int H, int W, int cin, in
     p.out_mode = out_f32 ? 1 : 0;
     p.fp16 = g_op_fp16;
     // the taps-in-N kernel in work-list mode, whatever the taps / halo policies choose for dd3d_op_conv2d
-    p.halo = conv_halo_mode();
+    p.halo = 1;
     p.taps_n = 1;
     p.tile_list = d_tiles;
     p.tile_count = d_count;
@@ -758,14 +750,6 @@ int dd3d_op_b3d_sparse(const void* const* d_in, const int32_t* h_level_hw, const
                        int B, int C, int topk, int n_pad, float* d_rows, int out_pitch, dd3d_stream stream) {
     return dd3d_op_b3d_sparse_c(d_in, h_level_hw, h_pitch, d_w, d_scale, d_bias, d_fin, d_counts, B, C, topk, n_pad, d_rows,
                                 out_pitch, 256, stream);
-}
-
-int dd3d_op_stem_conv(const void* d_in4, const void* d_w, const float* d_scale, const float* d_bias, void* d_out, int B,
-                      int H, int W, int ksize, int stride, int cout, int out_pitch, dd3d_stream stream) {
-    return cuda_status(launch_stem_tc(static_cast<const __nv_bfloat16*>(d_in4), static_cast<const __nv_bfloat16*>(d_w),
-                                      d_scale, d_bias, static_cast<__nv_bfloat16*>(d_out), B, H, W, ksize, stride, cout,
-                                      out_pitch, device_sms(), static_cast<cudaStream_t>(stream), g_op_fp16),
-                       nullptr);
 }
 
 int dd3d_op_dla_front(const void* d_in4, const void* d_w0, const void* d_w1, const void* d_w2, const float* d_sb0,
@@ -877,19 +861,6 @@ int dd3d_op_maxpool(const void* d_in, void* d_out, int B, int H, int W, int C, i
 
 int64_t dd3d_op_ese_scratch_bytes(int B, int HW, int C) {
     return static_cast<int64_t>(B) * (ese_nsplit(HW) + 1) * C * 4;
-}
-
-int dd3d_op_ese_pool(const void* d_x, int x_pitch, const float* d_fc_w, const float* d_fc_b, const void* d_identity, int id_pitch,
-                     void* d_out, int out_pitch, void* d_pool, int pool_pitch, float* d_scratch, int B, int H, int W, int C,
-                     dd3d_stream stream) {
-    if (C % 8 || !d_pool) return DD3D_ERR_INVALID;
-    float* partial = d_scratch;
-    float* gate = d_scratch + static_cast<size_t>(B) * ese_nsplit(H * W) * C;
-    return cuda_status(launch_ese(static_cast<const __nv_bfloat16*>(d_x), x_pitch, d_fc_w, d_fc_b,
-                                  static_cast<const __nv_bfloat16*>(d_identity), id_pitch, static_cast<__nv_bfloat16*>(d_out),
-                                  out_pitch, partial, gate, B, H * W, C, device_sms(), static_cast<cudaStream_t>(stream),
-                                  g_op_fp16, static_cast<__nv_bfloat16*>(d_pool), pool_pitch, H, W),
-                       nullptr);
 }
 
 int dd3d_op_ese(const void* d_x, int x_pitch, const float* d_fc_w, const float* d_fc_b, const void* d_identity,

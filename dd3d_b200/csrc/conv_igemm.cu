@@ -1,7 +1,6 @@
 // Implicit-GEMM convolution: host side (tensor maps, tiling policy, launch) and the taps-in-N kernel.  The main kernel and its
 // design notes are in conv_igemm_kernel.cuh.
 #include <stdlib.h>
-#include <string.h>
 
 #include <algorithm>
 #include <string>
@@ -284,8 +283,6 @@ bool conv_taps_eligible(int taps, int stride, int cout_pad, int nseg, const int*
     return mode && taps == 9 && stride == 1 && cout_pad == 16 && conv_prefer_halo(taps, stride, cout_pad, nseg, Hs, Ws);
 }
 
-int conv_halo_mode() { return 2; }  // one 128B-swizzled [18][10][64ch] box per 64-channel block
-
 bool make_act_map_halo(CUtensorMap* map, const void* base, int B, int H, int W, int C, int pitch, int fp16) {
     cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)pitch * 2, (cuuint64_t)W * pitch * 2, (cuuint64_t)H * W * pitch * 2};
@@ -296,13 +293,6 @@ bool make_act_map_halo(CUtensorMap* map, const void* base, int B, int H, int W, 
 bool conv_prefer_halo(int taps, int stride, int block_n, int nseg, const int* Hs, const int* Ws) {
     if (taps != 9 || stride != 1) return false;
     (void)block_n;
-    static int mode = -1;  // 0 auto, 1 generic, 2 halo
-    if (mode < 0) {
-        const char* e = getenv("DD3D_CONV_MODE");
-        mode = (e && !strcmp(e, "generic")) ? 1 : (e && !strcmp(e, "halo")) ? 2 : 0;
-    }
-    if (mode == 1) return false;
-    if (mode == 2) return true;
     long halo_tiles = 0, gen_tiles = 0;
     for (int s = 0; s < nseg; ++s) {
         int th, tw;

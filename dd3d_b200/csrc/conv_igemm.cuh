@@ -88,10 +88,9 @@ void choose_tile(int H, int W, int* th, int* tw);
 int conv_tiles_per_image(int H, int W);  // M-tiles per image of the generic tiling
 // Halo variant (3x3, stride 1): one 128B-swizzled [18][10][64 ch] patch per 64-channel block serves all nine taps.
 constexpr int kHaloTh = 16, kHaloTw = 8;
-int conv_halo_mode();
 bool make_act_map_halo(CUtensorMap* map, const void* base, int B, int H, int W, int C, int pitch, int fp16 = 0);
 // Policy: use the halo variant when its fixed 16x8 tiling costs at most 10 % more tiles than the best generic
-// tiling over all segments (env DD3D_CONV_MODE=generic|halo overrides, for tests).
+// tiling over all segments.
 bool conv_prefer_halo(int taps, int stride, int block_n, int nseg, const int* Hs, const int* Ws);
 // Taps-in-N variant (3x3, stride 1, cout_pad == 16): the nine taps become GEMM columns -- ONE [180 patch pixels] x [9 x 16]
 // GEMM per 64-channel block instead of nine N = 16 GEMMs (an N = 16 wgmma runs far below the tensor-core rate), then the

@@ -16,9 +16,9 @@
 // rounding happens there, so there is no im2col copy, no shared-memory round trip of the accumulators and no CTA-wide
 // barrier inside a layer.  The kernel is bound by shared-memory wavefronts and the mma.sync path, not by HBM or wgmma peak.
 //
-// Numerics are those of the layer-by-layer path (and of the oracle's 16-bit emulation): every intermediate is rounded to
-// the storage type, conv padding is zero OUTSIDE THE IMAGE (halo positions beyond the border are forced to 0 after the
-// epilogue, they are not "the conv evaluated out there").
+// Numerics are those of the three layers run one by one (and of the oracle's 16-bit emulation): every intermediate is
+// rounded to the storage type, conv padding is zero OUTSIDE THE IMAGE (halo positions beyond the border are forced to 0
+// after the epilogue, they are not "the conv evaluated out there").
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

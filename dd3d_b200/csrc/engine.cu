@@ -58,12 +58,9 @@ Engine::Engine(const dd3d_model_desc& d) : desc(d) {
                                 std::to_string(prop.major) + std::to_string(prop.minor));
     }
     num_sms = prop.multiProcessorCount;
-    if (const char* e = getenv("DD3D_DLA_FRONT")) opt_dla_front = atoi(e) ? 1 : 0;  // A/B runs of bench.py; default 1
     if (const char* e = getenv("DD3D_SPARSE_BOX3D")) opt_sparse_box3d = std::max(0, std::min(2, atoi(e)));
     if (const char* e = getenv("DD3D_SPARSE_TOWER")) opt_sparse_tower = std::max(0, std::min(2, atoi(e)));
     if (const char* e = getenv("DD3D_SPARSE_BOX2D_TOWER")) opt_sparse_box2d_tower = std::max(0, std::min(2, atoi(e)));
-    if (const char* e = getenv("DD3D_STEM_MMA")) opt_stem_mma = atoi(e) ? 1 : 0;
-    if (const char* e = getenv("DD3D_ESE_POOL")) opt_ese_pool = atoi(e) ? 1 : 0;
 }
 
 Engine::~Engine() {
@@ -507,7 +504,7 @@ struct Builder {
                 hs[s] = segs[s].in.H / stride;
                 ws[s] = segs[s].in.W / stride;
             }
-            p.halo = conv_prefer_halo(L.taps, stride, L.block_n, p.nseg, hs, ws) ? conv_halo_mode() : 0;
+            p.halo = conv_prefer_halo(L.taps, stride, L.block_n, p.nseg, hs, ws) ? 1 : 0;
             p.taps_n = (L.d_w_taps != nullptr && conv_taps_eligible(L.taps, stride, L.cout_pad, p.nseg, hs, ws)) ? 1 : 0;
         }
         for (int s = 0; s < p.nseg; ++s) {
@@ -782,33 +779,12 @@ struct Builder {
         const DlaSpec& S = *dla_spec(E->desc.arch);
         const std::string p = "backbone.bottom_up";
         const int H = input.H, W = input.W;
-        // both forms of the front end are packed at finalize (host weights are dropped afterwards), so that the
-        // "dla_front" option can be flipped on a finalized engine.  base_layer / level0 / level1 have DLA-34's shapes in
-        // every variant (channels 16, 16, 32).
-        const FrontLayer& F = E->front_layer(p);
-        const auto n0 = dla_norm(p + ".base_layer"), n1 = dla_norm(p + ".level0.0"), n2 = dla_norm(p + ".level1.0");
-        E->stem_layer(p + ".base_layer", n0.first, n0.second, 7, 1);
-        E->conv_layer(p + ".level0.0", {p + ".level0.0"}, 16, 3);
-        E->bn_epilogue(p + ".level0.0|" + n1.first, n1.first, n1.second, 16);
-        E->conv_layer(p + ".level1.0", {p + ".level1.0"}, 16, 3);
-        E->bn_epilogue(p + ".level1.0|" + n2.first, n2.first, n2.second, 32);
-        View a2, bottom;
-        if (E->opt_dla_front && H % 4 == 0 && W % 4 == 0) {
-            // base_layer -> level0 -> level1 -> 2x2 max-pool in one kernel (dla_front.cu); the two full-resolution
-            // 16-channel maps never reach HBM
-            a2 = alloc(H / 2, W / 2, 32);
-            bottom = alloc(H / 4, W / 4, 32);
-            front(F, input, a2, bottom);
-        } else {
-            View a0 = alloc(H, W, 16);
-            stem(p + ".base_layer", n0.first, n0.second, input, a0, 7, 1);
-            View a1 = alloc(H, W, 16);
-            dla_conv(p + ".level0.0", a0, a1, 3, 1, true);
-            a2 = alloc(H / 2, W / 2, 32);
-            dla_conv(p + ".level1.0", a1, a2, 3, 2, true);
-            bottom = alloc(H / 4, W / 4, 32);
-            maxpool(a2, bottom, 2);
-        }
+        // base_layer -> level0 -> level1 -> 2x2 max-pool in one kernel (dla_front.cu); the two full-resolution 16-channel
+        // maps never reach HBM.  base_layer / level0 / level1 have DLA-34's shapes in every variant (channels 16, 16, 32).
+        if (H % 4 || W % 4) fail(DD3D_ERR_STATE, "internal: the DLA front end needs H and W divisible by 4");
+        View a2 = alloc(H / 2, W / 2, 32);
+        View bottom = alloc(H / 4, W / 4, 32);
+        front(E->front_layer(p), input, a2, bottom);
         const int* ch = S.channels;
         // the FPN inputs (FE.FPN.IN_FEATURES): level<first> .. level5
         const int first = E->fpn_first_stage();
@@ -841,9 +817,9 @@ struct Builder {
         P->ops.push_back(op);
     }
 
-    void stem(const std::string& wname, const std::string& bn, const std::string& bias, View in4, View out, int ksize, int stride,
-              bool relu = true) {
-        const StemLayer& S = E->stem_layer(wname, bn, bias, ksize, stride, relu);
+    // VoVNet stem_1: 3x3 / stride 2, 3 -> 64 channels (stem_mma.cu)
+    void stem(const std::string& wname, const std::string& bn, const std::string& bias, View in4, View out, bool relu = true) {
+        const StemLayer& S = E->stem_layer(wname, bn, bias, relu);
         touch(out);
         ++op_idx;
         if (dry) return;
@@ -851,14 +827,12 @@ struct Builder {
         op.type = Op::STEM;
         op.in = in4;
         op.out = out;
-        op.ksize = ksize;
-        op.stride = stride;
         op.stem = &S;
         op.outs[0] = out;
         op.nouts = 1;
         const double in_px = static_cast<double>(B) * in4.H * in4.W, out_px = static_cast<double>(B) * out.H * out.W;
-        op.flops = 2.0 * out_px * S.cout * 3 * ksize * ksize;
-        op.bytes = in_px * 8 + out_px * S.cout * 2;
+        op.flops = 2.0 * out_px * 64 * 3 * 9;
+        op.bytes = in_px * 8 + out_px * 64 * 2;
         P->ops.push_back(op);
     }
 
@@ -918,10 +892,10 @@ struct Builder {
         const int nl = S.layers;
         View s1 = alloc(H / 2, W / 2, S.stem[0]);
         if (E->backbone_norm == DD3D_NORM_GN) {
-            stem(p + ".stem.stem_1/conv", "", "", input, s1, 3, 2, false);
+            stem(p + ".stem.stem_1/conv", "", "", input, s1, false);
             group_norm({s1}, &E->gn_affine(p + ".stem.stem_1/norm", s1.C), true, nullptr, false);
         } else {
-            stem(p + ".stem.stem_1/conv", p + ".stem.stem_1/norm", "", input, s1, 3, 2);
+            stem(p + ".stem.stem_1/conv", p + ".stem.stem_1/norm", "", input, s1);
         }
         View s2 = alloc(H / 2, W / 2, S.stem[1]);
         vov_conv3x3(p + ".stem.stem_2", s1, s2, 1, S.dw);
@@ -935,21 +909,15 @@ struct Builder {
         feats->clear();
         if (fpn_in[0] == DD3D_FPN_IN_STEM) feats->push_back(slice(cat, 0, in_ch));
         View stage_out;
-        View pooled_cat;  // next stage's concat buffer when its pooled slice was produced by the previous stage's eSE pass
         for (int si = 0; si < 4; ++si) {
             const int sc = stage_ch[si], oc = out_ch[si];
             if (si > 0) {
                 const int hp = (h - 3 + 1) / 2 + 1, wp = (w - 3 + 1) / 2 + 1;  // 3x3 / s2, ceil_mode (vovnet.py:249)
-                if (pooled_cat.ptr != nullptr || pooled_cat.buf >= 0) {
-                    cat = pooled_cat;  // the previous stage's last eSE pass already wrote the pooled map (ese_scale_pool_kernel)
-                } else {
-                    cat = alloc(hp, wp, in_ch + nl * sc);
-                    maxpool(stage_out, slice(cat, 0, in_ch), 3);
-                }
+                cat = alloc(hp, wp, in_ch + nl * sc);
+                maxpool(stage_out, slice(cat, 0, in_ch), 3);
                 h = hp;
                 w = wp;
             }
-            View pooled_next;  // stays empty unless this stage's last module fuses the next stage's pool
             for (int b = 0; b < blocks[si]; ++b) {
                 const std::string name = "OSA" + std::to_string(si + 2) + "_" + std::to_string(b + 1);
                 const std::string q = p + ".stage" + std::to_string(si + 2) + "." + name;
@@ -976,19 +944,13 @@ struct Builder {
                 View dst;
                 View next_cat;
                 const bool last = (b == blocks[si] - 1);
-                View pooled;
                 if (last) {
                     dst = alloc(h, w, oc);
-                    if (si < 3 && E->opt_ese_pool && h >= 3 && w >= 3) {
-                        // the eSE scale pass of a stage's last module also writes the next stage's 3x3 / s2 pooled input
-                        pooled_next = alloc((h - 3 + 1) / 2 + 1, (w - 3 + 1) / 2 + 1, oc + nl * stage_ch[si + 1]);
-                        pooled = slice(pooled_next, 0, oc);
-                    }
                 } else {
                     next_cat = alloc(h, w, oc + nl * sc);
                     dst = slice(next_cat, 0, oc);
                 }
-                ese(q + ".ese.fc", xt, b > 0 ? &x : nullptr, dst, pooled.buf >= 0 ? &pooled : nullptr);
+                ese(q + ".ese.fc", xt, b > 0 ? &x : nullptr, dst);
                 if (last) {
                     stage_out = dst;
                 } else {
@@ -996,12 +958,11 @@ struct Builder {
                 }
                 in_ch = oc;
             }
-            pooled_cat = pooled_next;
             if (std::find(fpn_in.begin(), fpn_in.end(), si + 2) != fpn_in.end()) feats->push_back(stage_out);
         }
     }
 
-    void ese(const std::string& fc, View xt, const View* identity, View dst, const View* pooled = nullptr) {
+    void ese(const std::string& fc, View xt, const View* identity, View dst) {
         const EseLayer& L = E->ese_layer(fc, xt.C);
         // The concat conv (the op just emitted) writes per-tile channel sums from its epilogue: [B][T][C], T = 4 * tiles.
         // Behind a GroupNorm the eSE pools the normalised map itself (launch_ese): [B][ese_nsplit(HW)][C] partial sums.
@@ -1013,7 +974,6 @@ struct Builder {
         touch(xt);
         if (identity) touch(*identity);
         touch(dst);
-        if (pooled) touch(*pooled);
         ++op_idx;
         if (dry) return;
         if (fused) {
@@ -1039,11 +999,6 @@ struct Builder {
         op.nouts = 1;
         // pooling is fused into the concat conv, or behind a GroupNorm one more pass over the map
         op.bytes = static_cast<double>(B) * xt.H * xt.W * xt.C * 2 * ((identity ? 3 : 2) + (fused ? 0 : 1));
-        if (pooled) {  // outs[1]: the 3x3 / s2 ceil-mode max-pool of dst, written by the same pass
-            op.outs[1] = *pooled;
-            op.nouts = 2;
-            op.bytes += static_cast<double>(B) * pooled->H * pooled->W * xt.C * 2;
-        }
         P->ops.push_back(op);
     }
 
@@ -1160,7 +1115,7 @@ struct Builder {
         memset(&tt, 0, sizeof(tt));
         const int L = static_cast<int>(feats.size());
         tt.num_levels = L;
-        int hs[kMaxSeg], ws[kMaxSeg];
+        int hs[kMaxSeg] = {}, ws[kMaxSeg] = {};
         for (int l = 0; l < L; ++l) {
             hs[l] = feats[l].H;
             ws[l] = feats[l].W;
@@ -1191,7 +1146,7 @@ struct Builder {
         memset(&cp, 0, sizeof(cp));
         cp.nseg = L;
         cp.B = B;
-        cp.halo = halo ? conv_halo_mode() : 0;
+        cp.halo = halo ? 1 : 0;
         for (int l = 0; l < L; ++l) {
             cp.seg[l].H = hs[l];
             cp.seg[l].W = ws[l];
@@ -1487,43 +1442,29 @@ struct Builder {
 
 // ------------------------------------------------------------------------------------------------ misc layers
 
-const StemLayer& Engine::stem_layer(const std::string& wname, const std::string& bn, const std::string& conv_bias_name, int ksize,
-                                    int stride, bool relu) {
+// VoVNet stem_1 in the layout stem_mma.cu reads: [64][3][4][4] (cout, ky, kx, c; kernel column 3 and the 4th input channel
+// are zero); folded BN as scale[64] | bias[64].
+const StemLayer& Engine::stem_layer(const std::string& wname, const std::string& bn, const std::string& conv_bias_name,
+                                    bool relu) {
     auto it = stems.find(wname);
     if (it != stems.end()) return it->second;
     const HostTensor& w = weight(wname + ".weight");
-    if (w.shape.size() != 4 || w.shape[1] != 3 || w.shape[2] != ksize || w.shape[0] % 16)
+    if (w.shape.size() != 4 || w.shape[0] != 64 || w.shape[1] != 3 || w.shape[2] != 3 || w.shape[3] != 3)
         fail(DD3D_ERR_INVALID, "bad stem weight: " + wname);
     StemLayer S;
-    S.ksize = ksize;
-    S.stride = stride;
-    S.cout = static_cast<int>(w.shape[0]);
     S.relu = relu;
-    // tensor-core stem layout: bf16 [cout][kpad], k = (ky*ksize + kx)*4 + c, zero padded (4th channel and K tail)
-    const int kpad = stem_tc_kpad(ksize);
-    std::vector<uint16_t> packed(static_cast<size_t>(S.cout) * kpad, 0);
-    for (int co = 0; co < S.cout; ++co)
+    std::vector<uint16_t> pm(64 * 3 * 4 * 4, 0);
+    for (int co = 0; co < 64; ++co)
         for (int c = 0; c < 3; ++c)
-            for (int t = 0; t < ksize * ksize; ++t)
-                packed[static_cast<size_t>(co) * kpad + t * 4 + c] =
-                    host_f32_to_act(w.data[(static_cast<size_t>(co) * 3 + c) * ksize * ksize + t], fp16);
-    S.d_w = static_cast<__nv_bfloat16*>(dev_alloc(packed.size() * 2));
-    cuda_check(cudaMemcpy(S.d_w, packed.data(), packed.size() * 2, cudaMemcpyHostToDevice), "upload stem weights");
-    S.epi = bn_epilogue(wname + "|" + bn, bn, conv_bias_name, S.cout);
-    if (ksize == 3 && stride == 2 && S.cout == 64) {
-        std::vector<uint16_t> pm(64 * 3 * 4 * 4, 0);
-        for (int co = 0; co < 64; ++co)
-            for (int c = 0; c < 3; ++c)
-                for (int ky = 0; ky < 3; ++ky)
-                    for (int kx = 0; kx < 3; ++kx)
-                        pm[((co * 3 + ky) * 4 + kx) * 4 + c] = host_f32_to_act(w.data[((co * 3 + c) * 3 + ky) * 3 + kx], fp16);
-        S.d_w_mma = static_cast<__nv_bfloat16*>(dev_alloc(pm.size() * 2));
-        cuda_check(cudaMemcpy(S.d_w_mma, pm.data(), pm.size() * 2, cudaMemcpyHostToDevice), "upload stem weights (mma)");
-        std::vector<float> sc, bi;
-        bn_fold(bn, conv_bias_name, 64, &sc, &bi);
-        sc.insert(sc.end(), bi.begin(), bi.end());
-        S.d_sb_mma = upload_f32(sc);
-    }
+            for (int ky = 0; ky < 3; ++ky)
+                for (int kx = 0; kx < 3; ++kx)
+                    pm[((co * 3 + ky) * 4 + kx) * 4 + c] = host_f32_to_act(w.data[((co * 3 + c) * 3 + ky) * 3 + kx], fp16);
+    S.d_w = static_cast<__nv_bfloat16*>(dev_alloc(pm.size() * 2));
+    cuda_check(cudaMemcpy(S.d_w, pm.data(), pm.size() * 2, cudaMemcpyHostToDevice), "upload stem weights");
+    std::vector<float> sc, bi;
+    bn_fold(bn, conv_bias_name, 64, &sc, &bi);
+    sc.insert(sc.end(), bi.begin(), bi.end());
+    S.d_sb = upload_f32(sc);
     return stems.emplace(wname, S).first->second;
 }
 
@@ -2122,15 +2063,8 @@ void Engine::launch_op(const Op& op, cudaStream_t stream) {
             cuda_check(launch_conv(op.conv, num_sms, stream), "conv");
             break;
         case Op::STEM:
-            if (op.stem->d_w_mma != nullptr && opt_stem_mma) {
-                cuda_check(launch_stem_s2_mma(op.in.ptr, op.stem->d_w_mma, op.stem->d_sb_mma, op.out.ptr, op.out.pitch, plan.B,
-                                              op.in.H, op.in.W, num_sms, stream, fp16, op.stem->relu ? 1 : 0),
-                           "stem conv (mma)");
-                break;
-            }
-            cuda_check(launch_stem_tc(op.in.ptr, op.stem->d_w, op.stem->epi.d_scale, op.stem->epi.d_bias, op.out.ptr,
-                                      plan.B, op.in.H, op.in.W, op.ksize, op.stride, op.stem->cout, op.out.pitch, num_sms,
-                                      stream, fp16, op.stem->relu ? 1 : 0),
+            cuda_check(launch_stem_s2_mma(op.in.ptr, op.stem->d_w, op.stem->d_sb, op.out.ptr, op.out.pitch, plan.B, op.in.H,
+                                          op.in.W, num_sms, stream, fp16, op.stem->relu ? 1 : 0),
                        "stem conv");
             break;
         case Op::POOL:
@@ -2143,17 +2077,14 @@ void Engine::launch_op(const Op& op, cudaStream_t stream) {
                 cuda_check(launch_ese(op.in.ptr, op.in.pitch, op.ese->d_w, op.ese->d_b,
                                       op.has_identity ? op.identity.ptr : nullptr, op.has_identity ? op.identity.pitch : 0,
                                       op.out.ptr, op.out.pitch, op.f0, op.f1, plan.B, op.in.H * op.in.W, op.in.C, num_sms,
-                                      stream, fp16, op.nouts == 2 ? op.outs[1].ptr : nullptr,
-                                      op.nouts == 2 ? op.outs[1].pitch : 0, op.in.H, op.in.W),
+                                      stream, fp16),
                            "eSE");
                 break;
             }
             cuda_check(launch_ese_fused(op.in.ptr, op.in.pitch, op.f2, op.ksize, op.ese->d_w, op.ese->d_b,
                                         op.has_identity ? op.identity.ptr : nullptr,
                                         op.has_identity ? op.identity.pitch : 0, op.out.ptr, op.out.pitch, op.f0, op.f1,
-                                        plan.B, op.in.H * op.in.W, op.in.C, num_sms, stream, fp16,
-                                        op.nouts == 2 ? op.outs[1].ptr : nullptr, op.nouts == 2 ? op.outs[1].pitch : 0,
-                                        op.in.H, op.in.W),
+                                        plan.B, op.in.H * op.in.W, op.in.C, num_sms, stream, fp16),
                        "eSE");
             break;
         case Op::RELU:

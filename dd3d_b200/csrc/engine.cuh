@@ -59,13 +59,10 @@ struct Epilogue {
     float* d_bias;
     float* d_lo;
 };
-struct StemLayer {
-    __nv_bfloat16* d_w;
-    int ksize, stride, cout;
-    Epilogue epi;
-    __nv_bfloat16* d_w_mma = nullptr;  // 3x3 stride-2 64-channel stem (VoVNet stem_1): [64][3][4][4] for stem_mma.cu
-    float* d_sb_mma = nullptr;         // scale[64] | bias[64]
-    bool relu = true;                  // false: raw output (VoVNet stem_1 in front of its GroupNorm)
+struct StemLayer {  // VoVNet stem_1 (3x3 / stride 2, 3 -> 64) packed for stem_mma.cu
+    __nv_bfloat16* d_w;  // [64][3][4][4]
+    float* d_sb;         // scale[64] | bias[64]
+    bool relu = true;    // false: raw output (VoVNet stem_1 in front of its GroupNorm)
 };
 struct FrontLayer {  // DLA-34 base_layer + level0 + level1 packed for dla_front.cu
     __nv_bfloat16 *d_w0, *d_w1, *d_w2;
@@ -287,8 +284,7 @@ class Engine {
                              const std::vector<float>* lo);
     const Epilogue& bn_epilogue(const std::string& key, const std::string& bn_prefix, const std::string& conv_bias_name,
                                 int cout);
-    const StemLayer& stem_layer(const std::string& wname, const std::string& bn, const std::string& conv_bias_name, int ksize,
-                                int stride, bool relu = true);
+    const StemLayer& stem_layer(const std::string& wname, const std::string& bn, const std::string& conv_bias_name, bool relu);
     const EseLayer& ese_layer(const std::string& fc, int C);
     const FrontLayer& front_layer(const std::string& prefix);
     const DwLayer& dw_layer(const std::string& wname, int C);
@@ -330,9 +326,6 @@ class Engine {
     int opt_do_postprocess = 1;
     int opt_profile = 0;
     int opt_workspace_reuse = 1;  // 0: bump allocation, every op output keeps its own memory (stage-level tests / debugging)
-    int opt_ese_pool = 0;  // 1: a VoVNet stage's last eSE scale pass also writes the next stage's max-pooled input; 0 (default):
-                           // separate pool kernel (the fused pass re-reads each pooling window's inputs 2.25 times)
-    int opt_stem_mma = 1;  // 1: VoVNet stem_1 on the register-fragment kernel (stem_mma.cu); 0: wgmma im2col kernel (stem_tc.cu)
     int opt_sparse_box3d = 2;  // box3d predictor at the final candidates only (b3d_sparse.cu): 0 never (dense maps), 1 always, 2 auto (by head size)
     int opt_sparse_tower = 2;  // box3d tower on the tiles the sparse predictor reads (tower_tiles.cu): 0 never, 1 whenever the
                                // sparse predictor runs and the tower norm is not GN, 2 auto (as 1, for heads of >= 50 000 pixels)
@@ -340,7 +333,6 @@ class Engine {
                                      // threshold (tower_tiles.cu): 0 never, 1 whenever the tower norm is not GN and the tower
                                      // convs use the pair tile, 2 auto (as 1, with the sparse box3d predictor and heads of
                                      // >= 50 000 pixels)
-    int opt_dla_front = 1;  // 1: DLA-34 base_layer + level0 + level1 (+ pool) as ONE kernel (dla_front.cu); 0: layer by layer
     int opt_workspace_fill = -1;  // >= 0: byte the whole arena is filled with at dd3d_plan (poison test)
     int opt_bev_nms = 0;
     float bev_nms_thresh = 0.f;

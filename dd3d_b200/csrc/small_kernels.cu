@@ -1,6 +1,5 @@
 // Bandwidth-bound kernels of the DD3D backbone (NHWC bf16, 128-bit vector accesses):
 //   preprocess   : (x - mean) / std, zero pad, NCHW -> NHWC(4)        reference core.py:61-72, image_list.py:93-158
-//   (the Cin=3 stem convs live in stem_tc.cu)
 //   max-pool     : 2x2/s2 (DLA Tree.downsample, dla.py:224-225), 3x3/s2 ceil (VoVNet, vovnet.py:248-249)
 //   eSE          : global avg-pool -> fc -> hsigmoid -> channel scale (+identity)   vovnet.py:169-185,233-236
 //   relu         : p7 input (detectron2 LastLevelP6P7)
@@ -271,77 +270,6 @@ __global__ void __launch_bounds__(256) ese_scale_kernel(const __nv_bfloat16* __r
     }
 }
 
-// eSE scale pass of the LAST module of a stage fused with the 3x3 / stride-2 ceil-mode max-pool that opens the next stage
-// (vovnet.py:249 `Pooling` after vovnet.py:233-236): one thread per (pooled pixel, 8-channel chunk) computes the up-to-nine
-// window values out = 16-bit(x * gate (+ identity)), writes the ones it OWNS (the 2x2 block at the window's origin, plus the
-// odd last row / column of the map) to the full-resolution output that the FPN lateral reads, and their maximum to the pooled
-// output.  The separate pool re-read the whole stage output from HBM (1.57 GB for V2-99 stage2 at B = 32); here the window
-// overlap (2.25 loads per input element) is served by L1 / L2.  max of rounded values == the pool of the stored tensor.
-__global__ void __launch_bounds__(256) ese_scale_pool_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gate,
-                                                             const __nv_bfloat16* __restrict__ identity,
-                                                             __nv_bfloat16* __restrict__ out, __nv_bfloat16* __restrict__ pool,
-                                                             int B, int H, int W, int C, int x_pitch, int id_pitch,
-                                                             int out_pitch, int pool_pitch, int Ho, int Wo, int fp16) {
-    DD3D_PDL_PROLOGUE();
-    const int vc = C >> 3;
-    const size_t total = static_cast<size_t>(B) * Ho * Wo * vc;
-    for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-        const int v = static_cast<int>(i % vc);
-        size_t pix = i / vc;
-        const int ox = static_cast<int>(pix % Wo);
-        pix /= Wo;
-        const int oy = static_cast<int>(pix % Ho);
-        const int b = static_cast<int>(pix / Ho);
-        const float4 g0 = __ldg(reinterpret_cast<const float4*>(gate + static_cast<size_t>(b) * C + v * 8));
-        const float4 g1 = __ldg(reinterpret_cast<const float4*>(gate + static_cast<size_t>(b) * C + v * 8 + 4));
-        uint4 u[9], q[9];
-        bool ok[9];
-#pragma unroll
-        for (int k = 0; k < 9; ++k) {
-            const int iy = 2 * oy + k / 3, ix = 2 * ox + k % 3;
-            ok[k] = iy < H && ix < W;  // ceil_mode: windows are clipped to the input
-            if (ok[k]) {
-                const size_t p = (static_cast<size_t>(b) * H + iy) * W + ix;
-                u[k] = __ldg(reinterpret_cast<const uint4*>(x + p * x_pitch + v * 8));
-                if (identity != nullptr) q[k] = __ldg(reinterpret_cast<const uint4*>(identity + p * id_pitch + v * 8));
-            }
-        }
-        uint4 m = make_uint4(0u, 0u, 0u, 0u);
-        bool first = true;
-#pragma unroll
-        for (int k = 0; k < 9; ++k) {
-            if (!ok[k]) continue;
-            const int dy = k / 3, dx = k % 3;
-            float f[8];
-            float2 t;
-            t = unpack2_act(u[k].x, fp16); f[0] = t.x * g0.x; f[1] = t.y * g0.y;
-            t = unpack2_act(u[k].y, fp16); f[2] = t.x * g0.z; f[3] = t.y * g0.w;
-            t = unpack2_act(u[k].z, fp16); f[4] = t.x * g1.x; f[5] = t.y * g1.y;
-            t = unpack2_act(u[k].w, fp16); f[6] = t.x * g1.z; f[7] = t.y * g1.w;
-            if (identity != nullptr) {
-                t = unpack2_act(q[k].x, fp16); f[0] += t.x; f[1] += t.y;
-                t = unpack2_act(q[k].y, fp16); f[2] += t.x; f[3] += t.y;
-                t = unpack2_act(q[k].z, fp16); f[4] += t.x; f[5] += t.y;
-                t = unpack2_act(q[k].w, fp16); f[6] += t.x; f[7] += t.y;
-            }
-            uint4 o;
-            o.x = pack2_act(f[0], f[1], fp16); o.y = pack2_act(f[2], f[3], fp16); o.z = pack2_act(f[4], f[5], fp16);
-            o.w = pack2_act(f[6], f[7], fp16);
-            // owner of input pixel (2 oy + dy, 2 ox + dx): the window whose 2x2 origin block holds it; the odd last row / column
-            // (never inside an origin block) belongs to the last window
-            const bool own_y = dy < 2 || oy == Ho - 1, own_x = dx < 2 || ox == Wo - 1;
-            if (own_y && own_x) {
-                const size_t p = (static_cast<size_t>(b) * H + 2 * oy + dy) * W + 2 * ox + dx;
-                *reinterpret_cast<uint4*>(out + p * out_pitch + v * 8) = o;
-            }
-            m = first ? o : max8(m, o, fp16);
-            first = false;
-        }
-        *reinterpret_cast<uint4*>(pool + (static_cast<size_t>(b * Ho + oy) * Wo + ox) * pool_pitch + v * 8) = m;
-    }
-}
-
 // relu on packed 16-bit floats: a set sign bit (negative, -0) -> +0; identical for bf16 and fp16
 __global__ void relu_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ out, size_t nvec) {
     DD3D_PDL_PROLOGUE();
@@ -395,18 +323,10 @@ int ese_nsplit(int HW) {
 }
 
 namespace {
-// the scale pass shared by both eSE forms: plain, or fused with the next stage's 3x3 / s2 ceil-mode max-pool
+// the scale pass shared by both eSE forms
 cudaError_t launch_ese_scale(const __nv_bfloat16* x, int x_pitch, const float* gate, const __nv_bfloat16* identity, int id_pitch,
-                             __nv_bfloat16* out, int out_pitch, int B, int HW, int C, int num_sms, cudaStream_t stream, int fp16,
-                             __nv_bfloat16* pool, int pool_pitch, int H, int W) {
-    const int vc = C / 8;
-    if (pool != nullptr) {
-        const int Ho = (H - 3 + 1) / 2 + 1, Wo = (W - 3 + 1) / 2 + 1;
-        const size_t tp = static_cast<size_t>(B) * Ho * Wo * vc;
-        return launch_pdl(ese_scale_pool_kernel, dim3(grid_for(tp, 256, num_sms)), dim3(256), 0, stream, x, gate, identity, out, pool,
-                          B, H, W, C, x_pitch, id_pitch, out_pitch, pool_pitch, Ho, Wo, fp16);
-    }
-    const size_t total = static_cast<size_t>(B) * HW * vc;
+                             __nv_bfloat16* out, int out_pitch, int B, int HW, int C, int num_sms, cudaStream_t stream, int fp16) {
+    const size_t total = static_cast<size_t>(B) * HW * (C / 8);
     return launch_pdl(ese_scale_kernel, dim3(grid_for((total + kEseUnroll - 1) / kEseUnroll, 256, num_sms)), dim3(256), 0, stream, x,
                       gate, identity, out, B, HW, C, x_pitch, id_pitch, out_pitch, fp16);
 }
@@ -414,9 +334,7 @@ cudaError_t launch_ese_scale(const __nv_bfloat16* x, int x_pitch, const float* g
 
 cudaError_t launch_ese(const __nv_bfloat16* x, int x_pitch, const float* fc_w, const float* fc_b,
                        const __nv_bfloat16* identity, int id_pitch, __nv_bfloat16* out, int out_pitch, float* partial,
-                       float* gate, int B, int HW, int C, int num_sms, cudaStream_t stream, int fp16, __nv_bfloat16* pool,
-                       int pool_pitch, int H, int W) {
-    if (pool != nullptr && (H * W != HW || H < 3 || W < 3)) return cudaErrorInvalidValue;
+                       float* gate, int B, int HW, int C, int num_sms, cudaStream_t stream, int fp16) {
     const int vc = C / 8;
     int rows = 256 / vc;
     if (rows < 1) rows = 1;
@@ -427,23 +345,20 @@ cudaError_t launch_ese(const __nv_bfloat16* x, int x_pitch, const float* fc_w, c
     e = launch_pdl(ese_fc_kernel, dim3((C + 7) / 8, B), dim3(256), C * sizeof(float), stream, static_cast<const float*>(partial),
                    fc_w, fc_b, gate, C, nsplit, 1.0f / static_cast<float>(HW));
     if (e != cudaSuccess) return e;
-    return launch_ese_scale(x, x_pitch, gate, identity, id_pitch, out, out_pitch, B, HW, C, num_sms, stream, fp16, pool, pool_pitch,
-                            H, W);
+    return launch_ese_scale(x, x_pitch, gate, identity, id_pitch, out, out_pitch, B, HW, C, num_sms, stream, fp16);
 }
 
 // eSE with the pooling partials produced by the conv epilogue: reduce -> fc -> scale (2 tensor passes instead of 3)
 cudaError_t launch_ese_fused(const __nv_bfloat16* x, int x_pitch, const float* tile_partial, int T, const float* fc_w,
                              const float* fc_b, const __nv_bfloat16* identity, int id_pitch, __nv_bfloat16* out,
                              int out_pitch, float* sums, float* gate, int B, int HW, int C, int num_sms,
-                             cudaStream_t stream, int fp16, __nv_bfloat16* pool, int pool_pitch, int H, int W) {
-    if (pool != nullptr && (H * W != HW || H < 3 || W < 3)) return cudaErrorInvalidValue;
+                             cudaStream_t stream, int fp16) {
     cudaError_t e = launch_pdl(ese_reduce_kernel, dim3((C + 63) / 64, B), dim3(256), 0, stream, tile_partial, sums, T, C, C);
     if (e != cudaSuccess) return e;
     e = launch_pdl(ese_fc_kernel, dim3((C + 7) / 8, B), dim3(256), C * sizeof(float), stream, static_cast<const float*>(sums), fc_w,
                    fc_b, gate, C, 1, 1.0f / static_cast<float>(HW));
     if (e != cudaSuccess) return e;
-    return launch_ese_scale(x, x_pitch, gate, identity, id_pitch, out, out_pitch, B, HW, C, num_sms, stream, fp16, pool, pool_pitch,
-                            H, W);
+    return launch_ese_scale(x, x_pitch, gate, identity, id_pitch, out, out_pitch, B, HW, C, num_sms, stream, fp16);
 }
 
 cudaError_t launch_relu(const __nv_bfloat16* x, __nv_bfloat16* out, size_t n_elems, int num_sms, cudaStream_t stream) {

@@ -2,8 +2,8 @@
 // as a register-fragment kernel.
 //
 // The layer is a pure streaming problem: 0.39 GB of normalised input in, 1.57 GB of 64-channel output out per 32-image batch
-// around 75 GFLOP.  The wgmma form (stem_tc.cu) builds a K-major im2col tile in shared memory per 128 pixels
-// (thread-gathered, 9 predicated 8-byte loads + swizzled stores per pixel, then wgmma).  Here a CTA copies the 17 x 66
+// around 75 GFLOP.  A wgmma form has to build a K-major im2col tile in shared memory per 128 pixels (thread-gathered, 9
+// predicated 8-byte loads + swizzled stores per pixel) before every MMA.  Here a CTA copies the 17 x 66
 // input patch of an 8 x 32 output tile with cp.async (double buffered), and every warp feeds mma.sync.m16n8k16 straight from it: one K step per kernel row, its 16 k slots = 4
 // consecutive input pixels x 4 channels (4th pixel / 4th channel carry zero weights), so lane t's fragment registers are ONE
 // 8-byte shared-memory load of input pixel 2x - 1 + t.  The 64 x 48 weight fragments stay in registers for the whole kernel.

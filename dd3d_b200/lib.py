@@ -147,7 +147,6 @@ SIGNATURES = {
                                 C.POINTER(_P), _P, _P, _I, _I, _I, _I, _P, _P, _P]),
     "dd3d_op_dla_front": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_stem_s2_mma": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
-    "dd3d_op_stem_conv": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "dd3d_op_dwconv3x3": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _I, _P]),
     "dd3d_op_group_norm_scratch_bytes": (_I64, [_I, _I, _I]),
     "dd3d_op_group_norm": (_I, [_P, _I, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _I, _P, _P]),
@@ -155,7 +154,6 @@ SIGNATURES = {
     "dd3d_op_preprocess": (_I, [_P, _I, _P, _P, _I, _I, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
     "dd3d_op_maxpool": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "dd3d_op_ese": (_I, [_P, _I, _P, _P, _P, _I, _P, _I, _P, _I, _I, _I, _P]),
-    "dd3d_op_ese_pool": (_I, [_P, _I, _P, _P, _P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _P]),
     "dd3d_op_ese_scratch_bytes": (_I64, [_I, _I, _I]),
     "dd3d_op_bev_nms": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, C.c_float, _I, _P]),
     "dd3d_op_bev_nms_large_scratch_bytes": (_I64, [_I, _I]),

@@ -469,7 +469,7 @@ class DD3DB200(nn.Module):
     PROFILE_CATEGORIES = ("preprocess", "stem_conv", "conv_igemm", "maxpool", "ese", "relu", "decode", "nms")
 
     def set_engine_option(self, name, value):
-        """dd3d_set_option pass-through for the switches that change the op graph or the workspace ("dla_front",
+        """dd3d_set_option pass-through for the switches that change the op graph or the workspace ("sparse_box3d",
         "workspace_reuse", "workspace_fill"): the next forward re-plans."""
         _lib.check(_lib.load().dd3d_set_option(self._engine(), name.encode(), int(value)), self._handle)
         self._plan_key = None

@@ -241,9 +241,7 @@ int dd3d_wait_host(dd3d_handle h, int slot);
 int dd3d_overflow_flags(dd3d_handle h, dd3d_stream stream, int32_t* h_flags);
 /* Runtime switches the reference's callers toggle on the meta-arch: "do_postprocess" (postprocess_in_inference,
  * scripts/train.py:206-209, test_time_augmentation.py:107), "do_nms" (core.py:134), "profile" (see
- * dd3d_get_profile), "ese_pool" (default 0; 1: the eSE scale pass of a VoVNet stage's last module also writes the 3x3 / stride-2 max-pooled input of
- * the next stage instead of a separate pool kernel re-reading the stage output -- bit-identical, measured ~10 % slower than the
- * two kernels, kept as a tested alternative; changing it drops the plans), "stem_mma" (default 1: VoVNet stem_1 runs on csrc/stem_mma.cu, 0: on csrc/stem_tc.cu), "sparse_box3d" (2 = auto, the default: the fused FCOS3D predictor conv is evaluated only at the pixels that survive the 2-D
+ * dd3d_get_profile), "sparse_box3d" (2 = auto, the default: the fused FCOS3D predictor conv is evaluated only at the pixels that survive the 2-D
  * threshold and per-level top-k, between the two halves of the decode, when the head maps of one image hold >= 50 000 pixels (a per-image rule: batch-independent results) -- the dense
  * "b3d<l>" maps of dd3d_get_tensor then do not exist; 1: always; 0: never (dense fp32 maps, for stage-level tests); changing
  * it drops the engine's plans), "sparse_tower" (2 = auto, the default: with the sparse predictor, a non-GN box3d tower on
@@ -255,8 +253,7 @@ int dd3d_overflow_flags(dd3d_handle h, dd3d_stream stream, int32_t* h_flags);
  * only on the conv tiles around the pixels where some class score passes PRE_NMS_THRESH -- bit-identical detections;
  * "box0".."box4" of dd3d_get_tensor then refuse (the map is stale elsewhere) and the "op<i>" outputs of that tower hold
  * stale values; 1: whenever the head qualifies; 0: dense; environment DD3D_SPARSE_BOX2D_TOWER; changing it drops the
- * engine's plans), "dla_front" (default 1: DLA-34 base_layer + level0 + level1 + pool run as one kernel; 0: layer by layer; flipping it
- * drops the engine's plans), "workspace_reuse" (default 1: activation buffers with disjoint lifetimes share workspace memory --
+ * engine's plans), "workspace_reuse" (default 1: activation buffers with disjoint lifetimes share workspace memory --
  * after a forward only "input", "p0".."p4" and the head maps of dd3d_get_tensor are intact; 0: every op output keeps its own
  * memory, for stage-level tests; applies to plans made afterwards), and "workspace_fill" (0..255: dd3d_plan fills the whole workspace with that byte first, -1 = off;
  * the poison test of tests/test_determinism_gpu.py: results must not depend on what the arena held). */
@@ -406,9 +403,6 @@ int dd3d_num_ops(dd3d_handle h);
 
 /* ---- single operators (same kernels the engine launches; used by the kernel-level parity tests) ----------- */
 /* The 16-bit element type of the operator entry points is process-wide: dd3d_set_conv_policy("op_fp16", 0 | 1). */
-/* dd3d_op_stem_conv: Cin=3 stem conv on tensor cores; d_in4 = bf16 [B][H][W][4] (dd3d_op_preprocess output), d_w =
- * bf16 [cout][kpad] with k = (ky*ksize + kx)*4 + c, kpad = ksize*ksize*4 rounded up to 64; (ksize, stride, cout) in
- * {(7,1,16), (3,2,64)}. */
 /* NHWC bf16 conv via the wgmma implicit-GEMM kernel.  d_w: bf16 [cout_pad][ksize*ksize][cin_pad64];
  * d_scale/d_bias: fp32 [cout_pad]; d_residual (optional) NHWC bf16 with res_pitch channels, res_up2: residual is
  * the 2x coarser map; out: bf16 (out_f32 == 0, pitch out_pitch) or fp32. */
@@ -471,19 +465,17 @@ int dd3d_op_b3d_gather(const void* const* d_in /*[5]*/, const int32_t* h_level_h
                        const void* const* d_w /*[5]*/, const float* const* d_scale /*[5]*/, const float* const* d_bias /*[5]*/,
                        const void* d_fin, const int32_t* d_counts, int B, int C, int topk, int cin, float* d_rows,
                        void* d_scratch, dd3d_stream stream);
-int dd3d_op_stem_conv(const void* d_in4, const void* d_w, const float* d_scale, const float* d_bias, void* d_out,
-                      int B, int H, int W, int ksize, int stride, int cout, int out_pitch, dd3d_stream stream);
 /* dd3d_op_dla_front: the fused DLA-34 front end (csrc/dla_front.cu; reference dla.py:271-283,346-350 base_layer -> level0
- * -> level1, each conv + FrozenBN + ReLU, plus the 2x2 max-pool of level1's output, dla.py:235).  d_in4 as for
- * dd3d_op_stem_conv; d_w0 = 16-bit [16][7][8][4] (ky, kx padded to 8, c padded to 4), d_w1 = [16][9][16], d_w2 = [32][9][16]
+ * -> level1, each conv + FrozenBN + ReLU, plus the 2x2 max-pool of level1's output, dla.py:235).  d_in4 = 16-bit
+ * [B][H][W][4] (dd3d_op_preprocess output); d_w0 = 16-bit [16][7][8][4] (ky, kx padded to 8, c padded to 4), d_w1 = [16][9][16], d_w2 = [32][9][16]
  * (cout, tap, cin); d_sb* = fp32 scale[cout] | bias[cout]; d_out = [B][H/2][W/2][out_pitch], d_pool (may be NULL) =
  * [B][H/4][W/4][pool_pitch].  H, W multiples of 4. */
 int dd3d_op_dla_front(const void* d_in4, const void* d_w0, const void* d_w1, const void* d_w2, const float* d_sb0,
                       const float* d_sb1, const float* d_sb2, void* d_out, int out_pitch, void* d_pool, int pool_pitch,
                       int B, int H, int W, dd3d_stream stream);
 /* dd3d_op_stem_s2_mma: VoVNet stem_1 (3x3 stride 2, 3 -> 64, FrozenBN + ReLU; vovnet.py:302,357-359) on the register-fragment
- * kernel (csrc/stem_mma.cu), the engine's default for that layer.  d_w = 16-bit [64][3][4][4] (cout, ky, kx, c; kx = 3 and
- * c = 3 zero), d_sb = fp32 scale[64] | bias[64], d_out = [B][ceil(H/2)][ceil(W/2)][out_pitch]. */
+ * kernel (csrc/stem_mma.cu), the kernel the engine runs for that layer.  d_in4 = 16-bit [B][H][W][4] (dd3d_op_preprocess
+ * output), d_w = 16-bit [64][3][4][4] (cout, ky, kx, c; kx = 3 and c = 3 zero), d_sb = fp32 scale[64] | bias[64], d_out = [B][ceil(H/2)][ceil(W/2)][out_pitch]. */
 int dd3d_op_stem_s2_mma(const void* d_in4, const void* d_w, const float* d_sb, void* d_out, int out_pitch, int B, int H, int W,
                         dd3d_stream stream);
 /* dd3d_op_dwconv3x3: depthwise 3x3 conv (groups = C, padding 1, no bias; vovnet.py:100-121 dw_conv3x3) on the kernel the
@@ -518,11 +510,6 @@ int dd3d_op_maxpool(const void* d_in, void* d_out, int B, int H, int W, int C, i
 int dd3d_op_ese(const void* d_x, int x_pitch, const float* d_fc_w, const float* d_fc_b, const void* d_identity,
                 int id_pitch, void* d_out, int out_pitch, float* d_scratch, int B, int HW, int C, dd3d_stream stream);
 int64_t dd3d_op_ese_scratch_bytes(int B, int HW, int C);
-/* dd3d_op_ese_pool: dd3d_op_ese whose scale pass also writes d_pool = the 3x3 / stride-2 ceil-mode max-pool of d_out
- * ([B][(H-2)/2+1][(W-2)/2+1][pool_pitch]; vovnet.py:249 after :233-236), the engine's form for the last module of a stage. */
-int dd3d_op_ese_pool(const void* d_x, int x_pitch, const float* d_fc_w, const float* d_fc_b, const void* d_identity, int id_pitch,
-                     void* d_out, int out_pitch, void* d_pool, int pool_pitch, float* d_scratch, int B, int H, int W, int C,
-                     dd3d_stream stream);
 /* Bird's-eye-view rotated NMS (reference DO_BEV_NMS branch, core.py:137-151 -> postprocessing.py:22-108 ->
  * tridet/layers/bev_nms.py:51-133 -> detectron2 batched_nms_rotated), in place on the detections a dd3d_forward run
  * with option "do_postprocess" = 0 produced: d_dets [B][cap], d_counts [B].  d_poses: [B][7] sensor->global pose of

@@ -201,28 +201,6 @@ def _input4(B, H, W, mode, K, g):
 
 
 @pytest.mark.parametrize("mode", MODES)
-@pytest.mark.parametrize("ksize,stride,cout", [(7, 1, 16), (3, 2, 64)])
-def test_stem_conv_exact(ksize, stride, cout, mode, act):
-    """dd3d_op_stem_conv (csrc/stem_tc.cu) on exact tiles and a ragged multi-tile map."""
-    L = lib.load()
-    for B, H, W in ((2, 64, 128), (1, 46, 90)):
-        g = X._gen(ksize * H + W)
-        K = 3 * ksize * ksize
-        x4 = _input4(B, H, W, mode, K, g)
-        w = X.operand((cout, 3, ksize, ksize), mode, K, g)
-        scale, bias = X.epilogue(cout, mode, K, g)
-        kpad = (ksize * ksize * 4 + 63) // 64 * 64
-        wpk = torch.zeros(cout, kpad)
-        wpk[:, :ksize * ksize * 4].view(cout, ksize * ksize, 4)[:, :, :3] = w.permute(0, 2, 3, 1).reshape(cout, -1, 3)
-        d_w, d_sc, d_bi = _dev(wpk), scale.cuda(), bias.cuda()
-        out = torch.full((B, H // stride, W // stride, cout), 7.0, dtype=gpu_ops.ACT, device="cuda")
-        assert L.dd3d_op_stem_conv(gpu_ops._p(x4), gpu_ops._p(d_w), gpu_ops._p(d_sc), gpu_ops._p(d_bi), gpu_ops._p(out), B, H, W,
-                                   ksize, stride, cout, cout, gpu_ops._stream()) == 0
-        torch.cuda.synchronize()
-        X.assert_exact(out, X.stem_ref64(x4[..., :3], w, scale, bias, stride), f"stem k{ksize} {B}x{H}x{W} {mode}")
-
-
-@pytest.mark.parametrize("mode", MODES)
 def test_stem_s2_mma_exact(mode, act):
     """dd3d_op_stem_s2_mma (csrc/stem_mma.cu): odd sizes, partial tiles, a pitch with the 128-bit store path, and more
     tiles than CTAs."""

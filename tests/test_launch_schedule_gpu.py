@@ -35,14 +35,11 @@ _GN_AVG = {"FE.BACKBONE.NORM": "GN", "FE.FPN.NORM": "GN", "DD3D.FCOS2D.NORM": "G
 # name -> (cfg or (model, inputs) factory, inputs factory, engine options, tile-list steps the plan must have)
 CONFIGS = {
     "dla34": (lambda: _plain("dla34"), lambda: case_inputs("dla34"), {}, 0),
-    "dla34_layer_by_layer": (lambda: _plain("dla34"), lambda: case_inputs("dla34"), {"dla_front": 0}, 0),
     # the V2-99 benchmark config at one image: sparse predictor, sparse box2d and box3d towers
     "v2_99_900x1600": (lambda: _plain("v2_99", "nuscenes"), lambda: make_inputs(1, 900, 1600, 1266.4), {}, 2),
     "v2_99_900x1600_dense_box3d": (lambda: _plain("v2_99", "nuscenes"), lambda: make_inputs(1, 900, 1600, 1266.4),
                                    {"sparse_box3d": 0}, 0),
     "v2_39_gn_avg": (lambda: _plain("v2_39", "nuscenes", _GN_AVG), lambda: make_inputs(2, 128, 192, 1266.4), {}, 0),
-    "v2_39_ese_pool_stem_tc": (lambda: _plain("v2_39", "nuscenes"), lambda: make_inputs(2, 128, 192, 1266.4),
-                               {"ese_pool": 1, "stem_mma": 0}, 0),
     "c128_gathered": (lambda: num_classes_oracle.case_cfg("v2_19_slim_c128"),
                       lambda: num_classes_oracle.case_inputs("v2_19_slim_c128"), {"sparse_box3d": 1}, 0),
     "bev_one_cta": (lambda: _bev("default"), None, {}, 0),
