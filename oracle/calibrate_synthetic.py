@@ -2,8 +2,11 @@
 
 Runs the CPU oracle once per architecture on a small synthetic batch with unit gains, rescales each conv so its raw
 (pre-BN) output has unit standard deviation on first use, then picks ``cls_logits`` gain/bias so that the fraction
-of (pixel, class) scores above the 0.05 threshold is ~TARGET.  Writes dd3d_b200/data/synth_gains.json (a few hundred
-scalars).  Usage:  python -m oracle.calibrate_synthetic
+of (pixel, class) scores above the 0.05 threshold is ~TARGET.  Every DLA takes the DLA-34 recipe and every VoVNet the
+V2-99 one (RECIPES).  Merges each arch's entry (a few hundred scalars) into dd3d_b200/data/synth_gains.json.  Usage:
+
+    python -m oracle.calibrate_synthetic                       # dla34 and v2_99
+    python -m oracle.calibrate_synthetic --calibrate dla_x_60  # any arch key
 """
 import json
 import os
@@ -13,6 +16,7 @@ import torch
 import torch.nn.functional as F
 
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), ".."))
+from dd3d_b200.arch import DLA_SPECS  # noqa: E402
 from dd3d_b200.config import get_cfg  # noqa: E402
 from dd3d_b200.synthetic import make_inputs, make_state_dict  # noqa: E402
 from oracle.dd3d_oracle import DD3DOracle  # noqa: E402
@@ -27,7 +31,7 @@ class CalibOracle(DD3DOracle):
         key = wkey or prefix
         if key not in self.gains:
             w = self.sd[key + ".weight"]
-            y = F.conv2d(x, w, None, stride, (w.shape[-1] - 1) // 2)
+            y = F.conv2d(x, w, None, stride, (w.shape[-1] - 1) // 2, 1, x.shape[1] // w.shape[1])
             std = float(y.std())
             gain = 1.0 / std if std > 0 else 1.0
             self.gains[key] = gain
@@ -36,7 +40,7 @@ class CalibOracle(DD3DOracle):
             # per-level tower BN (ModuleListDial): record the level's raw-output statistics so the recipe can
             # centre the level's running stats on them (a trained BN would) -> every level yields candidates.
             w = self.sd[key + ".weight"]
-            y = F.conv2d(x, w, None, stride, (w.shape[-1] - 1) // 2)
+            y = F.conv2d(x, w, None, stride, (w.shape[-1] - 1) // 2, 1, x.shape[1] // w.shape[1])
             m, v = float(y.mean()), float(y.var())
             self.gains[norm] = [m, v]
             self.sd[norm + ".running_mean"] = m + (v**0.5) * self.sd[norm + ".running_mean"]
@@ -44,7 +48,12 @@ class CalibOracle(DD3DOracle):
         return super().conv(x, prefix, stride, relu, norm, residual, quant_out, wkey)
 
 
-def calibrate(arch, dataset, h, w, focal, target_frac):
+# is a DLA -> (dataset, H, W, focal, target candidate fraction): the DLA-34 and V2-99 recipes
+RECIPES = {True: ("kitti_3d", 384, 640, 721.5, 0.01), False: ("nuscenes", 384, 640, 1266.4, 0.002)}
+
+
+def calibrate(arch):
+    dataset, h, w, focal, target_frac = RECIPES[arch in DLA_SPECS]
     cfg = get_cfg(arch, dataset)
     sd = make_state_dict(cfg, seed=0, gains={})
     orc = CalibOracle(cfg, sd)
@@ -89,15 +98,25 @@ def calibrate(arch, dataset, h, w, focal, target_frac):
     return {k: (round(v, 6) if isinstance(v, float) else [round(t, 6) for t in v]) for k, v in gains.items()}
 
 
-def main():
-    out = {}
-    out["dla34"] = calibrate("dla34", "kitti_3d", 384, 640, 721.5, target_frac=0.01)
-    out["v2_99"] = calibrate("v2_99", "nuscenes", 384, 640, 1266.4, target_frac=0.002)
+def merge_gains(arch):
+    """Calibrates `arch` and writes its entry into dd3d_b200/data/synth_gains.json; the other entries are written back
+    unchanged (same json layout), so the file's diff holds only that entry."""
     path = os.path.join(os.path.dirname(__file__), "..", "dd3d_b200", "data", "synth_gains.json")
-    os.makedirs(os.path.dirname(path), exist_ok=True)
+    with open(path) as f:
+        out = json.load(f)
+    out[arch] = calibrate(arch)
     with open(path, "w") as f:
         json.dump(out, f, indent=0, sort_keys=True)
     print("wrote", os.path.abspath(path))
+
+
+def main():
+    import argparse
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--calibrate", metavar="ARCH", nargs="+", default=["dla34", "v2_99"],
+                    help="arch keys to calibrate and merge into synth_gains.json (default: dla34 v2_99)")
+    for arch in ap.parse_args().calibrate:
+        merge_gains(arch)
 
 
 if __name__ == "__main__":

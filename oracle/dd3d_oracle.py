@@ -6,20 +6,26 @@ module, and only as the checker / the CPU baseline.  The product path (dd3d_b200
 It is a plain-PyTorch (CPU, fp32) restatement of the reference's eval-mode ``DD3D.forward``
 (/root/reference/tridet/modeling/dd3d/core.py:64-164) written functionally over the reference's
 ``state_dict`` key names.  Each function cites the reference file:line it follows.  Third-party arithmetic that
-is NOT vendored under /root/reference (detectron2 FPN / FrozenBN / batched_nms / detector_postprocess,
+is NOT vendored under /root/reference (detectron2 FPN / FrozenBN / GroupNorm / batched_nms / detector_postprocess,
 pytorch3d quaternion conversions, torchvision nms) is restated from the published semantics listed in
 SURVEY.md Appendix A.
+
+``DD3DOracle`` follows every config key the engine builds: FE.BACKBONE.NAME (every DLA and VoVNetV2-eSE of the tables
+below) and FE.BACKBONE.NORM; FE.FPN.IN_FEATURES, NORM, FUSE_TYPE and OUT_CHANNELS; the FCOS2D / FCOS3D NORM and tower
+depths; DD3D.IN_FEATURES and DD3D.NUM_CLASSES.  Every width and class count is read from the state_dict.
 
 Pinning: the reference ships no tests or golden vectors (SURVEY.md 4).  The oracle is pinned instead against
 the reference's OWN modules executed in the build container under oracle/ref_standin.py
 (tests/test_oracle_vs_reference.py, skipped where /root/reference is absent) and against the fixtures those
-runs produced (tests/golden/*.npz, written by oracle/gen_golden.py).  The third-party pieces themselves remain
-"parity unpinned" upstream (no pinned versions in the reference's Dockerfile) -- see DESIGN.md.
+runs produced (tests/golden/*.npz, written by oracle/gen_golden.py and the oracle/*_oracle.py generators).  The
+third-party pieces themselves remain "parity unpinned" upstream (no pinned versions in the reference's Dockerfile) --
+see DESIGN.md.
 
 ``emulate="bf16" | "fp16"`` (``emulate_bf16=True``) reproduces the CUDA engine's storage precision: conv weights
 and every stored activation are rounded to that 16-bit type at the points where the engine stores it (after each conv
-epilogue, after eSE scaling, after preprocessing); accumulation, BN affine, predictors' outputs, decode and NMS stay
-fp32.  ``threads=1`` makes that emulation reproducible across processes (VERDICT r1 weak #4).
+epilogue, after eSE scaling, after preprocessing, the raw conv output in front of a GroupNorm and the output of every
+norm / FPN add pass); accumulation, BN affine, predictors' outputs, decode and NMS stay fp32.  ``threads=1`` makes that
+emulation reproducible across processes (VERDICT r1 weak #4).
 """
 import math
 
@@ -27,11 +33,41 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from dd3d_b200.arch import fpn_inputs, in_feature_levels, level_strides
+
 EPS = 1e-7
 BN_EPS = 1e-5
+GN_GROUPS, GN_EPS = 32, 1e-5  # get_norm("GN") = nn.GroupNorm(32, C), eps 1e-5
 
 
 _EMU_DTYPES = {"bf16": torch.bfloat16, "fp16": torch.float16}
+
+# vovnet.py:19-97 _STAGE_SPECS restated (the "eSE" flag is dead: _OSA_module always applies eSE, :216,233)
+VOVNET = {
+    name: dict(stem=stem, stage_ch=sc, out_ch=oc, layers=nl, blocks=nb, dw=dw)
+    for name, stem, sc, oc, nl, nb, dw in (
+        ("V-19-slim-dw-eSE", (64, 64, 64), (64, 80, 96, 112), (112, 256, 384, 512), 3, (1, 1, 1, 1), True),
+        ("V-19-dw-eSE", (64, 64, 64), (128, 160, 192, 224), (256, 512, 768, 1024), 3, (1, 1, 1, 1), True),
+        ("V-19-slim-eSE", (64, 64, 128), (64, 80, 96, 112), (112, 256, 384, 512), 3, (1, 1, 1, 1), False),
+        ("V-19-eSE", (64, 64, 128), (128, 160, 192, 224), (256, 512, 768, 1024), 3, (1, 1, 1, 1), False),
+        ("V-39-eSE", (64, 64, 128), (128, 160, 192, 224), (256, 512, 768, 1024), 5, (1, 1, 2, 2), False),
+        ("V-57-eSE", (64, 64, 128), (128, 160, 192, 224), (256, 512, 768, 1024), 5, (1, 1, 4, 3), False),
+        ("V-99-eSE", (64, 64, 128), (128, 160, 192, 224), (256, 512, 768, 1024), 5, (1, 3, 9, 3), False),
+    )
+}
+
+# dla.py:358-441 restated: FE.BACKBONE.NAME -> (levels, channels, BottleneckX, residual_root, cardinality)
+DLA = {
+    name: dict(levels=lv, channels=ch, bottleneck_x=bx, root_residual=rr, cardinality=card)
+    for name, lv, ch, bx, rr, card in (
+        ("DLA-34", (1, 1, 1, 2, 2, 1), (16, 32, 64, 128, 256, 512), False, False, 0),
+        ("DLA-X-46-C", (1, 1, 1, 2, 2, 1), (16, 32, 64, 64, 128, 256), True, False, 32),
+        ("DLA-X-60-C", (1, 1, 1, 2, 3, 1), (16, 32, 64, 64, 128, 256), True, False, 32),
+        ("DLA-X-60", (1, 1, 1, 2, 3, 1), (16, 32, 128, 256, 512, 1024), True, False, 32),
+        ("DLA-X-102", (1, 1, 1, 3, 4, 1), (16, 32, 128, 256, 512, 1024), True, True, 32),
+        ("DLA-X-102-64", (1, 1, 1, 3, 4, 1), (16, 32, 128, 256, 512, 1024), True, True, 64),
+    )
+}
 
 
 class DD3DOracle:
@@ -47,15 +83,15 @@ class DD3DOracle:
         if self.emu is not None and self.emu not in _EMU_DTYPES:
             raise ValueError(f"emulate must be None, 'bf16' or 'fp16', got {self.emu!r}")
         self.threads = threads
-        self.arch = "dla34" if cfg.FE.BUILDER == "build_fcos_dla_fpn_backbone_p67" else "v2_99"
+        is_dla = cfg.FE.BUILDER == "build_fcos_dla_fpn_backbone_p67"
+        self.dla = DLA[cfg.FE.BACKBONE.NAME] if is_dla else None
+        self.vov = None if is_dla else VOVNET[cfg.FE.BACKBONE.NAME]
+        self.size_divisibility = 128 if is_dla else 64  # FPN 32 * 4 (dla.py:559) / 32 * 2 (vovnet.py:452)
         self.num_classes = cfg.DD3D.NUM_CLASSES
-        if self.arch == "dla34":
-            self.strides = [8, 16, 32, 64, 128]  # p3..p7 (dla.py:536-561)
-            self.size_divisibility = 128  # FPN 32 * 4 (dla.py:559)
-        else:
-            self.strides = [4, 8, 16, 32, 64]  # p2..p6 (vovnet.py:428-454)
-            self.size_divisibility = 64  # FPN 32 * 2 (vovnet.py:452)
-        self.num_levels = 5
+        self.fpn_in = fpn_inputs(cfg)  # FE.FPN.IN_FEATURES as (backbone output, stride)
+        self.fpn_index = in_feature_levels(cfg)  # DD3D.IN_FEATURES as FPN output indices, in head order
+        self.strides = level_strides(cfg)
+        self.num_levels = len(self.fpn_index)
         self.nuscenes = cfg.MODEL.META_ARCHITECTURE == "NuscenesDD3D"  # nuscenes_dd3d.py:300-335
 
     # ------------------------------------------------------------------------------------------
@@ -73,13 +109,12 @@ class DD3DOracle:
 
     def conv(self, x, prefix, stride=1, relu=False, norm=None, residual=None, quant_out=True, wkey=None):
         """detectron2 ``Conv2d`` wrapper: conv -> norm -> (+residual) -> activation.
-        `norm`: state_dict prefix of the BN to apply (default `<prefix>.norm` if present)."""
+        `norm`: state_dict prefix of the BN to apply (default `<prefix>.norm` if present).  A weight of C / groups input
+        channels (BottleneckX conv2, dla.py:113-124) is a grouped conv."""
         sd = self.sd
         w = sd[(wkey or prefix) + ".weight"]
         k = w.shape[-1]
-        if self.emu:
-            w = self._q(w)
-        y = F.conv2d(x, w, None, stride, (k - 1) // 2)
+        y = F.conv2d(x, self._q(w), None, stride, (k - 1) // 2, 1, x.shape[1] // w.shape[1])
         cout = w.shape[0]
         scale = torch.ones(cout)
         bias = torch.zeros(cout)
@@ -96,6 +131,25 @@ class DD3DOracle:
         if relu:
             y = F.relu(y)
         return self._q(y) if quant_out else y
+
+    def _gn(self, y, prefix, relu=False, add=None, avg=False):
+        y = F.group_norm(y, GN_GROUPS, self.sd[prefix + ".weight"], self.sd[prefix + ".bias"], GN_EPS)
+        if add is not None:
+            y = y + add
+        if avg:
+            y = y * 0.5
+        return F.relu(y) if relu else y
+
+    def _conv_norm(self, x, prefix, norm, lvl=None, relu=False):
+        """FPN / head Conv2d(bias = no norm, norm = get_norm(norm)) -> optional ReLU; for GN the pre-norm output is
+        rounded."""
+        if norm in ("BN", "FrozenBN") and lvl is not None:  # ModuleListDial: level lvl uses norm lvl
+            return self.conv(x, prefix, relu=relu, norm=f"{prefix}.norm.{lvl}")
+        if norm == "GN":
+            y = self.conv(x, prefix, norm=prefix + ".no_norm")  # raw conv (GN convs have no bias), stored
+            return self._q(self._gn(y, prefix + ".norm", relu))
+        {"BN": 0, "FrozenBN": 0, "SyncBN": 0, "": 0}[norm]  # KeyError like get_norm
+        return self.conv(x, prefix, relu=relu)  # shared BN at <prefix>.norm, or the conv bias alone
 
     # ------------------------------------------------------------------------------------------
     # preprocessing: core.py:61-72 + image_list.py:93-158
@@ -119,18 +173,22 @@ class DD3DOracle:
         return self._q(batch), sizes, intrinsics
 
     # ------------------------------------------------------------------------------------------
-    # DLA-34: dla.py:24-62 (BasicBlock), 146-167 (Root), 170-247 (Tree), 250-355 (DLA)
+    # DLA: dla.py:24-62 (BasicBlock), 104-143 (BottleneckX), 146-167 (Root), 170-247 (Tree), 250-355 (DLA)
     # ------------------------------------------------------------------------------------------
     def _dla_block(self, x, p, stride, residual=None):
         if residual is None:
             residual = x
-        out = self.conv(x, p + ".conv1", stride=stride, relu=True)
-        out = self.conv(out, p + ".conv2", relu=True, residual=residual)
-        return out
+        if not self.dla["bottleneck_x"]:
+            out = self.conv(x, p + ".conv1", stride=stride, relu=True)
+            return self.conv(out, p + ".conv2", relu=True, residual=residual)
+        # BottleneckX.forward (dla.py:128-143): the stride is on the grouped 3x3
+        out = self.conv(x, p + ".conv1", relu=True)
+        out = self.conv(out, p + ".conv2", stride=stride, relu=True)
+        return self.conv(out, p + ".conv3", relu=True, residual=residual)
 
     def _dla_root(self, p, xs):
-        # root_residual is False for DLA-34 (dla.py:359-361 passes no residual_root)
-        return self.conv(torch.cat(xs, 1), p + ".conv", relu=True)
+        # Root.forward (dla.py:160-167): + children[0] (= x2) before the ReLU when residual_root
+        return self.conv(torch.cat(xs, 1), p + ".conv", relu=True, residual=xs[0] if self.dla["root_residual"] else None)
 
     def _dla_tree(self, x, p, levels, stride, level_root, in_ch, out_ch, children=None, residual=None):
         children = [] if children is None else children
@@ -147,25 +205,38 @@ class DD3DOracle:
         children.append(x1)
         return self._dla_tree(x1, p + ".tree2", levels - 1, 1, False, out_ch, out_ch, children=children)
 
-    def dla34(self, x):
+    def _dla_forward(self, x):
+        """level2..level5, the outputs the FPN may read."""
         p = "backbone.bottom_up"
-        ch = [16, 32, 64, 128, 256, 512]
-        levels = [1, 1, 1, 2, 2, 1]
+        ch, levels = self.dla["channels"], self.dla["levels"]
         x = self.conv(x, p + ".base_layer", relu=True)
         x = self.conv(x, p + ".level0.0", relu=True)
         x = self.conv(x, p + ".level1.0", stride=2, relu=True)
-        outs = {}
         x = self._dla_tree(x, p + ".level2", levels[2], 2, False, ch[1], ch[2])
+        outs = {"level2": x}
         for lvl in (3, 4, 5):
             x = self._dla_tree(x, p + f".level{lvl}", levels[lvl], 2, True, ch[lvl - 1], ch[lvl])
             outs[f"level{lvl}"] = x
         return outs
 
     # ------------------------------------------------------------------------------------------
-    # VoVNetV2-99-eSE: vovnet.py:79-87 (spec), 173-185 (eSE), 188-238 (OSA), 241-273 (stage), 276-367
+    # VoVNetV2-eSE: vovnet.py:79-87 (spec), 100-159 (convs), 173-185 (eSE), 188-238 (OSA), 241-273 (stage), 276-367
     # ------------------------------------------------------------------------------------------
+    def _bb_conv(self, x, conv, norm, stride=1):
+        """VoVNet conv -> get_norm(FE.BACKBONE.NORM) -> ReLU; for GN the raw conv output is stored (rounded), then normalised."""
+        if self.cfg.FE.BACKBONE.NORM != "GN":
+            return self.conv(x, conv, stride=stride, relu=True, norm=norm)
+        y = self.conv(x, conv, stride=stride, norm=norm + ".no_norm")
+        return self._q(self._gn(y, norm, relu=True))
+
     def _vov_conv(self, x, p, name, stride=1):
-        return self.conv(x, f"{p}.{name}/conv", stride=stride, relu=True, norm=f"{p}.{name}/norm")
+        if not self.vov["dw"]:
+            return self._bb_conv(x, f"{p}.{name}/conv", f"{p}.{name}/norm", stride)
+        # dw_conv3x3 (vovnet.py:100-121): depthwise 3x3 (groups = C, no bias, no norm) -> pointwise 1x1 -> pw_norm -> ReLU.
+        # The depthwise output is a stored activation in the engine: rounded in the storage emulation.
+        w = self.sd[f"{p}.{name}/dw_conv3x3.weight"]
+        y = self._q(F.conv2d(x, self._q(w), None, stride, 1, 1, x.shape[1]))
+        return self._bb_conv(y, f"{p}.{name}/pw_conv1x1", f"{p}.{name}/pw_norm")
 
     def _ese(self, x, p):
         sd = self.sd
@@ -175,24 +246,29 @@ class DD3DOracle:
         return x * y
 
     def _osa(self, x, p, name, identity):
+        """_OSA_module.forward (vovnet.py:218-236) with `layers` layers and the -dw conv_reduction."""
         outs = [x]
         ident = x
-        for i in range(5):
+        if self.vov["dw"] and x.shape[1] != self.vov["stage_ch"][int(name[3]) - 2]:  # vovnet.py:200-205,221-222
+            r = f"{p}.conv_reduction.{name}_reduction_0"
+            x = self._bb_conv(x, r + "/conv", r + "/norm")
+        for i in range(self.vov["layers"]):
             x = self._vov_conv(x, f"{p}.layers.{i}", f"{name}_{i}")
             outs.append(x)
-        xt = self._vov_conv(torch.cat(outs, 1), f"{p}.concat", f"{name}_concat")
+        xt = self._bb_conv(torch.cat(outs, 1), f"{p}.concat.{name}_concat/conv", f"{p}.concat.{name}_concat/norm")
         xt = self._ese(xt, p + ".ese")
         if identity:
             xt = xt + ident
         return self._q(xt)
 
-    def v2_99(self, x):
+    def _vovnet_forward(self, x):
+        """stem and stage2..stage5, the outputs the FPN may read."""
         p = "backbone.bottom_up"
-        x = self._vov_conv(x, p + ".stem", "stem_1", 2)
+        x = self._bb_conv(x, f"{p}.stem.stem_1/conv", f"{p}.stem.stem_1/norm", 2)
         x = self._vov_conv(x, p + ".stem", "stem_2", 1)
         x = self._vov_conv(x, p + ".stem", "stem_3", 2)
-        outs = {}
-        for si, nblocks in zip((2, 3, 4, 5), (1, 3, 9, 3)):
+        outs = {"stem": x}
+        for si, nblocks in zip((2, 3, 4, 5), self.vov["blocks"]):
             if si != 2:
                 x = F.max_pool2d(x, kernel_size=3, stride=2, ceil_mode=True)
             for b in range(nblocks):
@@ -202,35 +278,46 @@ class DD3DOracle:
         return outs
 
     # ------------------------------------------------------------------------------------------
-    # FPN: detectron2 FPN.forward (SURVEY Appendix A), LastLevelP6P7 / LastLevelP6 (vovnet.py:411-425)
+    # FPN: detectron2 FPN.forward with norm and fuse_type (SURVEY Appendix A, oracle/ref_standin.py FPN),
+    # LastLevelP6P7 / LastLevelP6 (vovnet.py:411-425)
     # ------------------------------------------------------------------------------------------
     def fpn(self, feats):
+        """One lateral / output conv pair per FE.FPN.IN_FEATURES input, named by log2 of its stride; the top-down pass from
+        the last input, the top block on its output.  Returns every FPN output in backbone.output_shape() order."""
         p = "backbone"
-        if self.arch == "dla34":
-            names, stages = ["level3", "level4", "level5"], [3, 4, 5]
-        else:
-            names, stages = ["stage2", "stage3", "stage4", "stage5"], [2, 3, 4, 5]
+        norm, avg = self.cfg.FE.FPN.NORM, self.cfg.FE.FPN.FUSE_TYPE == "avg"
+        names = [n for n, _ in self.fpn_in]
+        stages = [int(math.log2(s)) for _, s in self.fpn_in]
         results = {}
         prev = None
         for name, st in zip(names[::-1], stages[::-1]):
-            if prev is None:
-                prev = self.conv(feats[name], f"{p}.fpn_lateral{st}")
+            lat = f"{p}.fpn_lateral{st}"
+            td = None if prev is None else F.interpolate(prev, scale_factor=2.0, mode="nearest")
+            if norm == "GN":
+                raw = self.conv(feats[name], lat, norm=lat + ".no_norm")
+                prev = self._q(self._gn(raw, lat + ".norm", add=td, avg=avg and td is not None))
+            elif td is not None and avg:
+                prev = self._q((self._conv_norm(feats[name], lat, norm) + td) * 0.5)
+            elif td is not None:
+                prev = self.conv(feats[name], lat, residual=td)  # the add fused into the lateral conv, one rounding
             else:
-                td = F.interpolate(prev, scale_factor=2.0, mode="nearest")
-                prev = self.conv(feats[name], f"{p}.fpn_lateral{st}", residual=td)
-            results[st] = self.conv(prev, f"{p}.fpn_output{st}")
-        p6 = self.conv(results[5], f"{p}.top_block.p6", stride=2)
+                prev = self._conv_norm(feats[name], lat, norm)
+            results[st] = self._conv_norm(prev, f"{p}.fpn_output{st}", norm)
+        p6 = self.conv(results[stages[-1]], f"{p}.top_block.p6", stride=2)
         outs = [results[s] for s in stages] + [p6]
-        if self.arch == "dla34":
+        if self.dla:
             outs.append(self.conv(self._q(F.relu(p6)), f"{p}.top_block.p7", stride=2))
         return outs
 
     # ------------------------------------------------------------------------------------------
-    # heads: fcos2d.py:130-156, fcos3d.py:160-188 (ModuleListDial: level l uses norm l, normalization.py:30-40)
+    # heads: fcos2d.py:46-91,130-156, fcos3d.py:75-112,160-188 (ModuleListDial: level l uses norm l, normalization.py:30-40)
     # ------------------------------------------------------------------------------------------
     def _tower(self, x, p, lvl):
-        for i in range(4):
-            x = self.conv(x, f"{p}.{i}", relu=True, norm=f"{p}.{i}.norm.{lvl}")
+        f2, f3 = self.cfg.DD3D.FCOS2D, self.cfg.DD3D.FCOS3D
+        depth, norm = {"fcos2d_head.cls_tower": (f2.NUM_CLS_CONVS, f2.NORM), "fcos2d_head.box2d_tower": (f2.NUM_BOX_CONVS, f2.NORM),
+                       "fcos3d_head.box3d_tower": (f3.NUM_CONVS, f3.NORM)}[p]
+        for i in range(depth):
+            x = self._conv_norm(x, f"{p}.{i}", norm, lvl, relu=True)
         return x
 
     def heads(self, features):
@@ -376,8 +463,10 @@ class DD3DOracle:
     # whole forward
     # ------------------------------------------------------------------------------------------
     def backbone(self, batch):
-        feats = self.dla34(batch) if self.arch == "dla34" else self.v2_99(batch)
-        return self.fpn(feats)
+        """The FPN outputs DD3D.IN_FEATURES selects, in head order."""
+        feats = self._dla_forward(batch) if self.dla else self._vovnet_forward(batch)
+        outs = self.fpn(feats)
+        return [outs[i] for i in self.fpn_index]
 
     @torch.no_grad()
     def forward(self, batched_inputs, return_intermediates=False, do_postprocess=True):

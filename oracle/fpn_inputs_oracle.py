@@ -1,34 +1,29 @@
-"""TEST INFRASTRUCTURE ONLY -- the CPU oracle and reference fixtures for FE.FPN.IN_FEATURES, the backbone outputs the FPN reads
+"""TEST INFRASTRUCTURE ONLY -- the cases and reference fixtures for FE.FPN.IN_FEATURES, the backbone outputs the FPN reads
 (build_fcos_dla_fpn_backbone_p67, dla.py:537-561; build_fcos_vovnet_fpn_backbone_p6, vovnet.py:428-454; detectron2's FPN,
 oracle/ref_standin.py FPN): one lateral / output conv pair per input, named by log2 of its stride, the top-down pass from the
 last input, then the top block on p5.  The FPN outputs are p<log2 first stride> .. p5 and P6 (and P7 for a DLA);
 DD3D.IN_FEATURES picks the head levels among them as before.
 
     python -m oracle.fpn_inputs_oracle --golden   # tests/golden/golden_fpn_inputs.npz + fpn_inputs_inventory.json
-
-``FpnInputsOracle(cfg, state_dict, ...)`` takes the same arguments as ``DD3DOracle``: oracle/in_features_oracle.py's arithmetic
-with the FPN built on the listed backbone outputs (the DLA's level2 and the VoVNet's stem included).
 """
 import json
-import math
 import os
 import sys
 
 import numpy as np
 import torch
-import torch.nn.functional as F
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
-from dd3d_b200.arch import fpn_inputs, fpn_output_names  # noqa: E402
 from dd3d_b200.config import get_cfg  # noqa: E402
-from dd3d_b200.synthetic import make_inputs, make_state_dict  # noqa: E402
-from oracle.head_norm_oracle import set_key  # noqa: E402
-from oracle.in_features_oracle import InFeaturesOracle  # noqa: E402
+from dd3d_b200.synthetic import make_state_dict  # noqa: E402
+# DD3DOracle, by the name the code that imports the cases of this module uses for their oracle
+from oracle.dd3d_oracle import DD3DOracle as FpnInputsOracle  # noqa: E402,F401
+from oracle.gen_golden import PRE_NMS_THRESH as _THRESH  # noqa: E402
+from oracle.gen_golden import inventory_digest, ragged_inputs, reference_fields, set_key  # noqa: E402
 
 # ragged fixture case: dataset, B, H, W, focal, crop (dh, dw) of the last image (as oracle/in_features_oracle.py)
 FPN_INPUTS_CASE = ("kitti_3d", 2, 128, 192, 721.5, (21, 34))
-_THRESH = "DD3D.FCOS2D.INFERENCE.PRE_NMS_THRESH"
 # name -> (backbone, FE.FPN.IN_FEATURES, DD3D.IN_FEATURES or None, meta-architecture, {cfg path: value}); PRE_NMS_THRESH is
 # lowered where the synthetic weights give too few candidates.  Small VoVNets keep the reference's CPU forward short; the -dw
 # variant reads its 64-channel stem.
@@ -78,67 +73,7 @@ def case_cfg(case, **kw):
 
 
 def case_inputs(case):
-    _, B, H, W, focal, (dh, dw) = FPN_INPUTS_CASE
-    inputs = make_inputs(B, H, W, focal)
-    inputs[-1]["image"] = inputs[-1]["image"][:, :H - dh, :W - dw].contiguous()
-    return inputs
-
-
-class FpnInputsOracle(InFeaturesOracle):
-    """DD3DOracle following FE.FPN.IN_FEATURES and DD3D.IN_FEATURES on top of the FE.* and head keys of FpnWidthOracle."""
-
-    def __init__(self, cfg, state_dict, **kw):
-        super().__init__(cfg, state_dict, **kw)
-        self.fpn_in = fpn_inputs(cfg)
-        all_strides = [2**int(n[1:]) for n in fpn_output_names(cfg)]
-        self.strides = [all_strides[i] for i in self.fpn_index]
-
-    # the backbone outputs the parents' backbones compute but do not return: DLA level2 and the VoVNet stem
-    def _dla_tree(self, x, p, *args, **kw):
-        y = super()._dla_tree(x, p, *args, **kw)
-        if p == "backbone.bottom_up.level2":
-            self._extra["level2"] = y
-        return y
-
-    def _vov_conv(self, x, p, name, stride=1):
-        y = super()._vov_conv(x, p, name, stride)
-        if name == "stem_3":
-            self._extra["stem"] = y
-        return y
-
-    def backbone(self, batch):
-        self._extra = {}
-        feats = self.dla34(batch) if self.arch == "dla34" else self.v2_99(batch)
-        feats.update(self._extra)
-        outs = self.fpn(feats)
-        return [outs[i] for i in self.fpn_index]
-
-    def fpn(self, feats):
-        """HeadNormOracle.fpn on the listed inputs: the top-down pass from the last input, the top block on its output."""
-        p = "backbone"
-        norm, avg = self.cfg.FE.FPN.NORM, self.cfg.FE.FPN.FUSE_TYPE == "avg"
-        names = [n for n, _ in self.fpn_in]
-        stages = [int(math.log2(s)) for _, s in self.fpn_in]
-        results = {}
-        prev = None
-        for name, st in zip(names[::-1], stages[::-1]):
-            lat = f"{p}.fpn_lateral{st}"
-            td = None if prev is None else F.interpolate(prev, scale_factor=2.0, mode="nearest")
-            if norm == "GN":
-                raw = self.conv(feats[name], lat, norm=lat + ".no_norm")
-                prev = self._q(self._gn(raw, lat + ".norm", add=td, avg=avg and td is not None))
-            elif td is not None and avg:
-                prev = self._q((self._conv_norm(feats[name], lat, norm) + td) * 0.5)
-            elif td is not None:
-                prev = self.conv(feats[name], lat, residual=td)  # the add fused into the lateral conv, one rounding
-            else:
-                prev = self._conv_norm(feats[name], lat, norm)
-            results[st] = self._conv_norm(prev, f"{p}.fpn_output{st}", norm)
-        p6 = self.conv(results[stages[-1]], f"{p}.top_block.p6", stride=2)
-        outs = [results[s] for s in stages] + [p6]
-        if self.arch == "dla34":
-            outs.append(self.conv(self._q(F.relu(p6)), f"{p}.top_block.p7", stride=2))
-        return outs
+    return ragged_inputs(*FPN_INPUTS_CASE[1:])
 
 
 # ------------------------------------------------------------------------------------------------ fixtures
@@ -163,7 +98,6 @@ def gen_goldens(out_dir):
     fpn_inputs_inventory.json: case -> inventory_digest of the reference's state_dict, for every case (NuscenesDD3D:
     inventory only, as in oracle/in_features_oracle.py), and under "refused" the reference's [exception type, message] for every
     list of FPN_INPUTS_REFUSED."""
-    from oracle.gen_golden import inventory_digest
     blob, inventory = {}, {}
     torch.set_num_threads(1)
     for case, (_, _, _, meta_arch, _) in FPN_INPUTS_CASES.items():
@@ -176,17 +110,7 @@ def gen_goldens(out_dir):
         model.load_state_dict(make_state_dict(cfg))
         with torch.no_grad():
             outs = model(case_inputs(case))
-        for b, o in enumerate(outs):
-            inst = o["instances"]
-            b3 = inst.pred_boxes3d
-            blob.update({f"{case}/{k}": v for k, v in {
-                f"boxes{b}": inst.pred_boxes.tensor.numpy(), f"scores{b}": inst.scores.numpy(),
-                f"scores_3d{b}": inst.scores_3d.numpy(), f"classes{b}": inst.pred_classes.numpy(),
-                f"levels{b}": inst.fpn_levels.numpy(), f"locations{b}": inst.locations.numpy(),
-                f"quat{b}": b3.quat.numpy(), f"proj_ctr{b}": b3.proj_ctr.numpy(), f"depth{b}": b3.depth.numpy(),
-                f"size{b}": b3.size.numpy(), f"tvec{b}": b3.tvec.numpy(), f"image_size{b}": np.array(inst.image_size),
-            }.items()})
-            print(case, "image", b, "detections", len(inst), "levels", np.bincount(inst.fpn_levels.numpy()).tolist())
+        blob.update(reference_fields(case, outs))
     refused = {}
     for backbone, out, fpn_in in FPN_INPUTS_REFUSED:
         try:

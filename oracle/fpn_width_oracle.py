@@ -1,12 +1,9 @@
-"""TEST INFRASTRUCTURE ONLY -- the CPU oracle and reference fixtures for FE.FPN.OUT_CHANNELS, the width of the FPN and of every
+"""TEST INFRASTRUCTURE ONLY -- the cases and reference fixtures for FE.FPN.OUT_CHANNELS, the width of the FPN and of every
 FCOS head (the reference's FPN builders pass it to the laterals, the outputs and the top block, dla.py:546-557,
 vovnet.py:438-450; FCOS2DHead / FCOS3DHead take their tower width from the backbone's output shape, fcos2d.py:43-45,
-fcos3d.py:70-72), across backbones and head / FPN norms, on top of oracle/backbone_norm_oracle.py and oracle/dla_oracle.py.
+fcos3d.py:70-72), across backbones and head / FPN norms.  DD3DOracle reads every width from the state_dict.
 
     python -m oracle.fpn_width_oracle --golden   # tests/golden/golden_fpn_width.npz + fpn_width_inventory.json
-
-``FpnWidthOracle(cfg, state_dict, ...)`` takes the same arguments as ``DD3DOracle``.  Its arithmetic reads every width from the
-state_dict, so it needs no width of its own: the class only combines the DLA-X, VoVNet and FPN / head norm oracles.
 """
 import json
 import os
@@ -18,14 +15,14 @@ import torch
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
 from dd3d_b200.config import get_cfg  # noqa: E402
-from dd3d_b200.synthetic import make_inputs, make_state_dict  # noqa: E402
-from oracle.backbone_norm_oracle import BackboneNormOracle  # noqa: E402
-from oracle.dla_oracle import DLAOracle  # noqa: E402
-from oracle.head_norm_oracle import set_key  # noqa: E402
+from dd3d_b200.synthetic import make_state_dict  # noqa: E402
+# DD3DOracle, by the name the code that imports the cases of this module uses for their oracle
+from oracle.dd3d_oracle import DD3DOracle as FpnWidthOracle  # noqa: E402,F401
+from oracle.gen_golden import PRE_NMS_THRESH as _THRESH  # noqa: E402
+from oracle.gen_golden import inventory_digest, ragged_inputs, reference_fields, set_key  # noqa: E402
 
 # ragged fixture case: dataset, B, H, W, focal, crop (dh, dw) of the last image (as oracle/head_norm_oracle.py)
 FPN_WIDTH_CASE = ("nuscenes", 2, 128, 192, 1266.4, (21, 34))
-_THRESH = "DD3D.FCOS2D.INFERENCE.PRE_NMS_THRESH"
 _GN = {"DD3D.FCOS2D.NORM": "GN", "DD3D.FCOS3D.NORM": "GN", "FE.FPN.NORM": "GN"}
 _BN = {"DD3D.FCOS2D.NORM": "BN", "DD3D.FCOS3D.NORM": "BN", "FE.FPN.NORM": "BN"}
 _NONE = {"DD3D.FCOS2D.NORM": "", "DD3D.FCOS3D.NORM": "", "FE.FPN.NORM": ""}
@@ -51,14 +48,7 @@ def case_cfg(case, **kw):
 
 
 def case_inputs(case):
-    _, B, H, W, focal, (dh, dw) = FPN_WIDTH_CASE
-    inputs = make_inputs(B, H, W, focal)
-    inputs[-1]["image"] = inputs[-1]["image"][:, :H - dh, :W - dw].contiguous()
-    return inputs
-
-
-class FpnWidthOracle(BackboneNormOracle, DLAOracle):
-    """DD3DOracle following FE.BACKBONE.NAME / NORM, FE.FPN.* (OUT_CHANNELS included) and the head NORM / depth keys."""
+    return ragged_inputs(*FPN_WIDTH_CASE[1:])
 
 
 # ------------------------------------------------------------------------------------------------ fixtures
@@ -68,7 +58,6 @@ def gen_goldens(out_dir):
     reference's state_dict, for every case (NuscenesDD3D included: its forward needs the 6-camera sample aggregation, so its
     detections are checked against the emulating oracle instead)."""
     from oracle import ref_standin
-    from oracle.gen_golden import inventory_digest
     blob, inventory = {}, {}
     torch.set_num_threads(1)
     for case, (_, _, meta_arch, _) in FPN_WIDTH_CASES.items():
@@ -80,17 +69,7 @@ def gen_goldens(out_dir):
         model.load_state_dict(make_state_dict(cfg))
         with torch.no_grad():
             outs = model(case_inputs(case))
-        for b, o in enumerate(outs):
-            inst = o["instances"]
-            b3 = inst.pred_boxes3d
-            blob.update({f"{case}/{k}": v for k, v in {
-                f"boxes{b}": inst.pred_boxes.tensor.numpy(), f"scores{b}": inst.scores.numpy(),
-                f"scores_3d{b}": inst.scores_3d.numpy(), f"classes{b}": inst.pred_classes.numpy(),
-                f"levels{b}": inst.fpn_levels.numpy(), f"locations{b}": inst.locations.numpy(),
-                f"quat{b}": b3.quat.numpy(), f"proj_ctr{b}": b3.proj_ctr.numpy(), f"depth{b}": b3.depth.numpy(),
-                f"size{b}": b3.size.numpy(), f"tvec{b}": b3.tvec.numpy(), f"image_size{b}": np.array(inst.image_size),
-            }.items()})
-            print(case, "image", b, "detections", len(inst))
+        blob.update(reference_fields(case, outs))
     np.savez_compressed(os.path.join(out_dir, "golden_fpn_width.npz"), **blob)
     with open(os.path.join(out_dir, "fpn_width_inventory.json"), "w") as f:
         json.dump(inventory, f, indent=1, sort_keys=True)

@@ -36,6 +36,45 @@ FULL_CASES = {
 NUSC_CASE = ("v2_99", 1, 128, 192, 1266.4)  # NuscenesDD3D: backbone, samples (x 6 cameras), H, W, focal
 
 
+# cfg path of the pre-NMS score threshold, which the fixture cases lower where the synthetic weights give too few candidates
+PRE_NMS_THRESH = "DD3D.FCOS2D.INFERENCE.PRE_NMS_THRESH"
+
+
+def set_key(cfg, path, value):
+    """cfg["A"]["B"]["C"] = value for path "A.B.C"."""
+    node = cfg
+    *parents, leaf = path.split(".")
+    for p in parents:
+        node = node[p]
+    node[leaf] = value
+
+
+def ragged_inputs(B, H, W, focal, crop):
+    """make_inputs(B, H, W, focal) with the last image cropped by crop = (dh, dw): a batch of ragged sizes."""
+    dh, dw = crop
+    inputs = make_inputs(B, H, W, focal)
+    inputs[-1]["image"] = inputs[-1]["image"][:, :H - dh, :W - dw].contiguous()
+    return inputs
+
+
+def reference_fields(name, outs, prefixed=True):
+    """The reference's per-image DD3D outputs -> {"<name>/<field><image>": array} (or "<field><image>" unprefixed)."""
+    blob = {}
+    p = f"{name}/" if prefixed else ""
+    for b, o in enumerate(outs):
+        inst = o["instances"]
+        b3 = inst.pred_boxes3d
+        blob.update({f"{p}{k}": v for k, v in {
+            f"boxes{b}": inst.pred_boxes.tensor.numpy(), f"scores{b}": inst.scores.numpy(),
+            f"scores_3d{b}": inst.scores_3d.numpy(), f"classes{b}": inst.pred_classes.numpy(),
+            f"levels{b}": inst.fpn_levels.numpy(), f"locations{b}": inst.locations.numpy(),
+            f"quat{b}": b3.quat.numpy(), f"proj_ctr{b}": b3.proj_ctr.numpy(), f"depth{b}": b3.depth.numpy(),
+            f"size{b}": b3.size.numpy(), f"tvec{b}": b3.tvec.numpy(), f"image_size{b}": np.array(inst.image_size),
+        }.items()})
+        print(name, "image", b, "detections", len(inst))
+    return blob
+
+
 TTA_CASE = dict(arch="dla34", dataset="kitti_3d", H=96, W=320, orig=(94, 313), focal=721.5, min_sizes=[64, 96, 128],
                 ims_per_batch=4, pre_nms_thresh=0.02)
 
@@ -119,9 +158,7 @@ def case_inputs(arch):
         _, _, B, H, W, focal = FULL_CASES[arch]
         return make_inputs(B, H, W, focal, with_size=True)
     ds, B, H, W, focal, (dh, dw), fac = CASES[arch]
-    inputs = make_inputs(B, H, W, focal)
-    if dh or dw:
-        inputs[-1]["image"] = inputs[-1]["image"][:, :H - dh, :W - dw].contiguous()
+    inputs = ragged_inputs(B, H, W, focal, (dh, dw))
     if fac != 1.0:
         inputs[-1]["height"] = int(round((H - dh) * fac))
         inputs[-1]["width"] = int(round((W - dw) * fac))
@@ -166,23 +203,9 @@ def gen_dd3d_goldens(names, out_dir):
         cfg = case_cfg(arch)
         model = ref_standin.build_reference_model(cfg).eval()
         model.load_state_dict(make_state_dict(cfg))
-        inputs = case_inputs(arch)
         with torch.no_grad():
-            outs = model(inputs)
-        blob = {}
-        for b, o in enumerate(outs):
-            inst = o["instances"]
-            b3 = inst.pred_boxes3d
-            blob.update({
-                f"boxes{b}": inst.pred_boxes.tensor.numpy(), f"scores{b}": inst.scores.numpy(),
-                f"scores_3d{b}": inst.scores_3d.numpy(), f"classes{b}": inst.pred_classes.numpy(),
-                f"levels{b}": inst.fpn_levels.numpy(), f"locations{b}": inst.locations.numpy(),
-                f"quat{b}": b3.quat.numpy(), f"proj_ctr{b}": b3.proj_ctr.numpy(), f"depth{b}": b3.depth.numpy(),
-                f"size{b}": b3.size.numpy(), f"tvec{b}": b3.tvec.numpy(),
-                f"image_size{b}": np.array(inst.image_size),
-            })
-            print(arch, "image", b, "detections", len(inst))
-        np.savez_compressed(os.path.join(out_dir, f"golden_{arch}.npz"), **blob)
+            outs = model(case_inputs(arch))
+        np.savez_compressed(os.path.join(out_dir, f"golden_{arch}.npz"), **reference_fields(arch, outs, prefixed=False))
 
 
 def inventory_digest(shapes):

@@ -1,13 +1,10 @@
-"""TEST INFRASTRUCTURE ONLY -- the CPU oracle and reference fixtures for DD3D.IN_FEATURES, the FPN outputs the heads run on:
+"""TEST INFRASTRUCTURE ONLY -- the cases and reference fixtures for DD3D.IN_FEATURES, the FPN outputs the heads run on:
 ``features = [features[f] for f in self.in_features]`` (core.py:25-26,82); every per-level module is sized by
 ``len(in_features)`` (fcos2d.py:35-36,68,77,102-108, fcos3d.py:60,86,104,128-134) and indexed by position, scales_depth /
 offsets_depth by MEAN_DEPTH_PER_LEVEL (fcos3d.py:136-139, also by position); compute_locations takes the strides of the
 selected levels (core.py:166-174) and ``fpn_levels`` is the position.
 
     python -m oracle.in_features_oracle --golden   # tests/golden/golden_in_features.npz + in_features_inventory.json
-
-``InFeaturesOracle(cfg, state_dict, ...)`` takes the same arguments as ``DD3DOracle``: oracle/fpn_width_oracle.py's arithmetic,
-with the backbone's five FPN outputs narrowed to the selected ones, in list order.
 """
 import json
 import os
@@ -18,15 +15,15 @@ import torch
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
-from dd3d_b200.arch import arch_of, in_feature_levels, DLA_SPECS  # noqa: E402
 from dd3d_b200.config import get_cfg  # noqa: E402
-from dd3d_b200.synthetic import make_inputs, make_state_dict  # noqa: E402
-from oracle.fpn_width_oracle import FpnWidthOracle  # noqa: E402
-from oracle.head_norm_oracle import set_key  # noqa: E402
+from dd3d_b200.synthetic import make_state_dict  # noqa: E402
+# DD3DOracle, by the name the code that imports the cases of this module uses for their oracle
+from oracle.dd3d_oracle import DD3DOracle as InFeaturesOracle  # noqa: E402,F401
+from oracle.gen_golden import PRE_NMS_THRESH as _THRESH  # noqa: E402
+from oracle.gen_golden import inventory_digest, ragged_inputs, reference_fields, set_key  # noqa: E402
 
 # ragged fixture case: dataset, B, H, W, focal, crop (dh, dw) of the last image (as oracle/fpn_width_oracle.py)
 IN_FEATURES_CASE = ("kitti_3d", 2, 128, 192, 721.5, (21, 34))
-_THRESH = "DD3D.FCOS2D.INFERENCE.PRE_NMS_THRESH"
 # name -> (backbone, DD3D.IN_FEATURES, meta-architecture, {cfg path: value}); PRE_NMS_THRESH is lowered where the synthetic
 # weights give too few candidates.  [p6, p3] runs PER_LEVEL_PREDICTORS, so predictor l serves position l.
 IN_FEATURES_CASES = {
@@ -51,25 +48,7 @@ def case_cfg(case, **kw):
 
 
 def case_inputs(case):
-    _, B, H, W, focal, (dh, dw) = IN_FEATURES_CASE
-    inputs = make_inputs(B, H, W, focal)
-    inputs[-1]["image"] = inputs[-1]["image"][:, :H - dh, :W - dw].contiguous()
-    return inputs
-
-
-class InFeaturesOracle(FpnWidthOracle):
-    """DD3DOracle following DD3D.IN_FEATURES on top of the FE.* and head keys of FpnWidthOracle."""
-
-    def __init__(self, cfg, state_dict, **kw):
-        super().__init__(cfg, state_dict, **kw)
-        self.fpn_index = in_feature_levels(cfg)
-        all_strides = [8, 16, 32, 64, 128] if arch_of(cfg) in DLA_SPECS else [4, 8, 16, 32, 64]
-        self.strides = [all_strides[i] for i in self.fpn_index]
-        self.num_levels = len(self.fpn_index)
-
-    def backbone(self, batch):
-        outs = super().backbone(batch)  # every FPN output, as the reference computes them
-        return [outs[i] for i in self.fpn_index]
+    return ragged_inputs(*IN_FEATURES_CASE[1:])
 
 
 # ------------------------------------------------------------------------------------------------ fixtures
@@ -78,7 +57,6 @@ def gen_goldens(out_dir):
     fields "<case>/<field><image>" as in golden_fpn_width.npz; in_features_inventory.json: case -> inventory_digest of the
     reference's state_dict, for every case (NuscenesDD3D: inventory only, as in oracle/fpn_width_oracle.py)."""
     from oracle import ref_standin
-    from oracle.gen_golden import inventory_digest
     blob, inventory = {}, {}
     torch.set_num_threads(1)
     for case, (_, _, meta_arch, _) in IN_FEATURES_CASES.items():
@@ -90,17 +68,7 @@ def gen_goldens(out_dir):
         model.load_state_dict(make_state_dict(cfg))
         with torch.no_grad():
             outs = model(case_inputs(case))
-        for b, o in enumerate(outs):
-            inst = o["instances"]
-            b3 = inst.pred_boxes3d
-            blob.update({f"{case}/{k}": v for k, v in {
-                f"boxes{b}": inst.pred_boxes.tensor.numpy(), f"scores{b}": inst.scores.numpy(),
-                f"scores_3d{b}": inst.scores_3d.numpy(), f"classes{b}": inst.pred_classes.numpy(),
-                f"levels{b}": inst.fpn_levels.numpy(), f"locations{b}": inst.locations.numpy(),
-                f"quat{b}": b3.quat.numpy(), f"proj_ctr{b}": b3.proj_ctr.numpy(), f"depth{b}": b3.depth.numpy(),
-                f"size{b}": b3.size.numpy(), f"tvec{b}": b3.tvec.numpy(), f"image_size{b}": np.array(inst.image_size),
-            }.items()})
-            print(case, "image", b, "detections", len(inst), "levels", np.bincount(inst.fpn_levels.numpy()).tolist())
+        blob.update(reference_fields(case, outs))
     np.savez_compressed(os.path.join(out_dir, "golden_in_features.npz"), **blob)
     with open(os.path.join(out_dir, "in_features_inventory.json"), "w") as f:
         json.dump(inventory, f, indent=1, sort_keys=True)

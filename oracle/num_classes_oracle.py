@@ -1,10 +1,10 @@
-"""TEST INFRASTRUCTURE ONLY -- the CPU oracle cases and reference fixtures for DD3D.NUM_CLASSES above the 16 the model desc
+"""TEST INFRASTRUCTURE ONLY -- the cases and reference fixtures for DD3D.NUM_CLASSES above the 16 the model desc
 holds: the reference sizes cls_logits at C (fcos2d.py:96), the five box3d predictors at 4C / 2C / C / 3C / C (fcos3d.py:
 103-124) and looks CANONICAL_BOX3D_SIZES up by predicted class (fcos3d.py:378).
 
     python -m oracle.num_classes_oracle --golden   # tests/golden/golden_num_classes.npz + num_classes_inventory.json
 
-The arithmetic is oracle/fpn_width_oracle.py's FpnWidthOracle, which reads every class count from the state_dict and the cfg.
+oracle/dd3d_oracle.py's DD3DOracle reads every class count from the state_dict and the cfg.
 """
 import json
 import os
@@ -16,13 +16,12 @@ import torch
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
 from dd3d_b200.config import get_cfg  # noqa: E402
-from dd3d_b200.synthetic import make_inputs, make_state_dict  # noqa: E402
-from oracle.fpn_width_oracle import FpnWidthOracle  # noqa: E402,F401  (the oracle of these cases)
-from oracle.head_norm_oracle import set_key  # noqa: E402
+from dd3d_b200.synthetic import make_state_dict  # noqa: E402
+from oracle.gen_golden import PRE_NMS_THRESH as _THRESH  # noqa: E402
+from oracle.gen_golden import inventory_digest, ragged_inputs, reference_fields, set_key  # noqa: E402
 
 # ragged fixture case: B, H, W, focal, crop (dh, dw) of the last image (as oracle/fpn_width_oracle.py)
 NUM_CLASSES_CASE = (2, 128, 192, 1266.4, (21, 34))
-_THRESH = "DD3D.FCOS2D.INFERENCE.PRE_NMS_THRESH"
 # name -> (backbone, DD3D.NUM_CLASSES, meta-architecture, {cfg path: value}).  PRE_NMS_THRESH is lowered where the synthetic
 # weights give too few candidates.
 NUM_CLASSES_CASES = {
@@ -58,10 +57,7 @@ def case_cfg(case, **kw):
 
 
 def case_inputs(case):
-    B, H, W, focal, (dh, dw) = NUM_CLASSES_CASE
-    inputs = make_inputs(B, H, W, focal)
-    inputs[-1]["image"] = inputs[-1]["image"][:, :H - dh, :W - dw].contiguous()
-    return inputs
+    return ragged_inputs(*NUM_CLASSES_CASE)
 
 
 # ------------------------------------------------------------------------------------------------ fixtures
@@ -70,7 +66,6 @@ def gen_goldens(out_dir):
     fields "<case>/<field><image>" as in golden_fpn_width.npz; num_classes_inventory.json: case -> inventory_digest of the
     reference's state_dict, for every case (NuscenesDD3D: inventory only, as in oracle/fpn_width_oracle.py)."""
     from oracle import ref_standin
-    from oracle.gen_golden import inventory_digest
     blob, inventory = {}, {}
     torch.set_num_threads(1)
     for case, (_, _, meta_arch, _) in NUM_CLASSES_CASES.items():
@@ -82,17 +77,7 @@ def gen_goldens(out_dir):
         model.load_state_dict(make_state_dict(cfg))
         with torch.no_grad():
             outs = model(case_inputs(case))
-        for b, o in enumerate(outs):
-            inst = o["instances"]
-            b3 = inst.pred_boxes3d
-            blob.update({f"{case}/{k}": v for k, v in {
-                f"boxes{b}": inst.pred_boxes.tensor.numpy(), f"scores{b}": inst.scores.numpy(),
-                f"scores_3d{b}": inst.scores_3d.numpy(), f"classes{b}": inst.pred_classes.numpy(),
-                f"levels{b}": inst.fpn_levels.numpy(), f"locations{b}": inst.locations.numpy(),
-                f"quat{b}": b3.quat.numpy(), f"proj_ctr{b}": b3.proj_ctr.numpy(), f"depth{b}": b3.depth.numpy(),
-                f"size{b}": b3.size.numpy(), f"tvec{b}": b3.tvec.numpy(), f"image_size{b}": np.array(inst.image_size),
-            }.items()})
-            print(case, "image", b, "detections", len(inst))
+        blob.update(reference_fields(case, outs))
     np.savez_compressed(os.path.join(out_dir, "golden_num_classes.npz"), **blob)
     with open(os.path.join(out_dir, "num_classes_inventory.json"), "w") as f:
         json.dump(inventory, f, indent=1, sort_keys=True)

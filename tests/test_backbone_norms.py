@@ -14,7 +14,8 @@ from dd3d_b200.arch import ARCH_KEYS, param_specs
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200
 from dd3d_b200.synthetic import make_state_dict
-from oracle.backbone_norm_oracle import BACKBONE_NORM_CASES, BackboneNormOracle, case_cfg, case_inputs
+from oracle.backbone_norm_oracle import BACKBONE_NORM_CASES, case_cfg, case_inputs
+from oracle.dd3d_oracle import DD3DOracle
 from oracle.gen_golden import inventory_digest
 from util import quat_dist
 
@@ -35,17 +36,6 @@ def test_param_specs_match_reference_inventory(case):
     assert inventory_digest(shapes) == want
     sd = DD3DB200(case_cfg(case)).state_dict()
     assert inventory_digest({k: tuple(v.shape) for k, v in sd.items()}) == want
-
-
-def test_gn_oracle_is_the_vovnet_oracle_without_gn():
-    """The GN overrides of BackboneNormOracle reproduce VoVNetOracle bit for bit when the backbone norm is BN."""
-    from oracle.vovnet_oracle import VoVNetOracle
-    cfg = case_cfg("v2_39_syncbn")
-    sd = make_state_dict(cfg)
-    inputs = case_inputs("v2_39_syncbn")
-    _, a = VoVNetOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs, return_intermediates=True)
-    _, b = BackboneNormOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs, return_intermediates=True)
-    assert all(x.equal(y) for x, y in zip(a["features"], b["features"]))
 
 
 def test_norm_keys_of_each_mode():
@@ -122,7 +112,7 @@ def test_oracle_matches_reference_golden(case):
     """Oracle (fp32) vs the reference's own DD3D.forward (oracle/backbone_norm_oracle.py --golden)."""
     g = np.load(os.path.join(GOLDEN_DIR, "golden_backbone_norms.npz"))
     cfg = case_cfg(case)
-    out = BackboneNormOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
+    out = DD3DOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
     total = 0
     for b, o in enumerate(out):
         p = f"{case}/"

@@ -15,7 +15,8 @@ from dd3d_b200 import lib
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200
 from dd3d_b200.synthetic import make_state_dict
-from oracle.backbone_norm_oracle import BACKBONE_NORM_CASES, BackboneNormOracle, case_cfg, case_inputs
+from oracle.backbone_norm_oracle import BACKBONE_NORM_CASES, case_cfg, case_inputs
+from oracle.dd3d_oracle import DD3DOracle
 from util import det_key, match_by_key, quat_dist
 
 pytestmark = pytest.mark.gpu
@@ -157,7 +158,7 @@ def test_forward_vs_emulating_oracle(case, act_dtype):
     out = model(inputs)
     torch.cuda.synchronize()
     assert model.overflow_flags() == 0
-    ref, inter = BackboneNormOracle(cfg, sd, emulate=act_dtype, threads=1).forward(inputs, return_intermediates=True)
+    ref, inter = DD3DOracle(cfg, sd, emulate=act_dtype, threads=1).forward(inputs, return_intermediates=True)
     bd = _bounds(case, act_dtype)
     fpn = max(_rel_l2(model.get_tensor(f"p{l}").float().cpu().permute(0, 3, 1, 2), inter["features"][l]) for l in range(5))
     print(f"\n{case} {act_dtype}: FPN rel L2 {fpn:.3e}")
@@ -295,7 +296,7 @@ def test_nuscenes_with_gn_backbone():
     inputs = make_nusc_inputs(1, 128, 192, 1266.4)
     out = model(inputs)
     assert model.overflow_flags() == 0
-    emu = BackboneNormOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs)
+    emu = DD3DOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs)
     matched = total = attr_same = 0
     worst = 0.0
     for o, e in zip(out, emu):

@@ -14,7 +14,8 @@ from dd3d_b200.arch import DLA_SPECS, arch_of, param_specs
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200
 from dd3d_b200.synthetic import make_state_dict
-from oracle.dla_oracle import DLA, DLA_X_ARCHS, DLAOracle, case_cfg, case_inputs
+from oracle.dd3d_oracle import DLA, DD3DOracle
+from oracle.dla_oracle import DLA_X_ARCHS, case_cfg, case_inputs
 from oracle.gen_golden import inventory_digest
 from util import quat_dist
 
@@ -77,7 +78,7 @@ def test_oracle_matches_reference_golden(arch):
     """Oracle (fp32) vs the reference's own DD3D.forward (oracle/dla_oracle.py --golden), the VoVNet family's bounds."""
     g = np.load(os.path.join(GOLDEN_DIR, "golden_dla_x.npz"))
     cfg = case_cfg(arch)
-    out = DLAOracle(cfg, make_state_dict(cfg)).forward(case_inputs(arch))
+    out = DD3DOracle(cfg, make_state_dict(cfg)).forward(case_inputs(arch))
     total = 0
     for b, o in enumerate(out):
         p = f"{arch}/"
@@ -93,19 +94,6 @@ def test_oracle_matches_reference_golden(arch):
         np.testing.assert_allclose(o["tvec"].numpy(), g[f"{p}tvec{b}"], rtol=1e-3, atol=1e-3)
         np.testing.assert_allclose(o["size"].numpy(), g[f"{p}size{b}"], rtol=1e-4)
     assert total > 0
-
-
-def test_dla_oracle_is_the_dla34_oracle_for_dla34():
-    """The generic DLA forward reproduces DD3DOracle's DLA-34 backbone bit for bit (storage emulation included)."""
-    from oracle.dd3d_oracle import DD3DOracle
-    from oracle.gen_golden import CASES
-    from oracle.gen_golden import case_inputs as dla34_inputs
-    cfg = get_cfg("dla34", CASES["dla34"][0])
-    sd = make_state_dict(cfg)
-    batch = DD3DOracle(cfg, sd, emulate="bf16").preprocess(dla34_inputs("dla34"))[0]
-    a = DD3DOracle(cfg, sd, emulate="bf16").backbone(batch)
-    b = DLAOracle(cfg, sd, emulate="bf16").backbone(batch)
-    assert len(a) == len(b) == 5 and all(x.equal(y) for x, y in zip(a, b))
 
 
 @pytest.mark.parametrize("arch", list(NAMES))

@@ -18,7 +18,8 @@ from dd3d_b200 import lib
 from dd3d_b200.arch import DLA_SPECS
 from dd3d_b200.meta_arch import DD3DB200
 from dd3d_b200.synthetic import make_state_dict
-from oracle.dla_oracle import DLA_X_ARCHS, DLAOracle, case_cfg, case_inputs
+from oracle.dd3d_oracle import DD3DOracle
+from oracle.dla_oracle import DLA_X_ARCHS, case_cfg, case_inputs
 from util import det_key, match_by_key, quat_dist
 
 pytestmark = pytest.mark.gpu
@@ -49,7 +50,7 @@ def _vs_emulating_oracle(cfg, sd, model, act_dtype, need_detections=True):
     out = model(inputs)
     torch.cuda.synchronize()
     assert model.overflow_flags() == 0
-    ref, inter = DLAOracle(cfg, sd, emulate=act_dtype, threads=1).forward(inputs, return_intermediates=True)
+    ref, inter = DD3DOracle(cfg, sd, emulate=act_dtype, threads=1).forward(inputs, return_intermediates=True)
     x = model.get_tensor("input")[..., :3].float().cpu().permute(0, 3, 1, 2)
     assert torch.equal(x, inter["batch"])
     for l in range(5):

@@ -17,7 +17,8 @@ from dd3d_b200.arch import (check_fpn_inputs, fpn_inputs, fpn_output_names, in_f
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_state_dict
-from oracle.fpn_inputs_oracle import (FPN_INPUTS_CASES, FPN_INPUTS_REFUSED, FpnInputsOracle, case_cfg, case_inputs, refused_cfg,
+from oracle.dd3d_oracle import DD3DOracle
+from oracle.fpn_inputs_oracle import (FPN_INPUTS_CASES, FPN_INPUTS_REFUSED, case_cfg, case_inputs, refused_cfg,
                                       refused_key)
 from oracle.gen_golden import inventory_digest
 from util import quat_dist
@@ -84,7 +85,7 @@ def test_oracle_matches_reference_golden(case):
     g = np.load(os.path.join(GOLDEN_DIR, "golden_fpn_inputs.npz"))
     cfg = case_cfg(case)
     assert list(g[f"{case}/fpn_outputs"]) == fpn_output_names(cfg)
-    out = FpnInputsOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
+    out = DD3DOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
     total = 0
     for b, o in enumerate(out):
         p = f"{case}/"

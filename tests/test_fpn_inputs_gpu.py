@@ -17,7 +17,8 @@ from dd3d_b200.arch import fpn_output_names, in_feature_levels
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_nusc_inputs, make_state_dict
-from oracle.fpn_inputs_oracle import FPN_INPUTS_CASES, FpnInputsOracle, case_cfg, case_inputs
+from oracle.dd3d_oracle import DD3DOracle
+from oracle.fpn_inputs_oracle import FPN_INPUTS_CASES, case_cfg, case_inputs
 from util import quat_dist
 
 pytestmark = pytest.mark.gpu
@@ -58,7 +59,7 @@ def _model(cfg, **opts):
 @functools.lru_cache(maxsize=None)
 def _oracle(case, act_dtype):
     cfg = case_cfg(case, act_dtype=act_dtype)
-    return FpnInputsOracle(cfg, make_state_dict(cfg), emulate=act_dtype, threads=1).forward(_inputs(case),
+    return DD3DOracle(cfg, make_state_dict(cfg), emulate=act_dtype, threads=1).forward(_inputs(case),
                                                                                             return_intermediates=True)
 
 

@@ -15,7 +15,8 @@ from dd3d_b200.arch import FPN_WIDTHS, param_specs
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_state_dict
-from oracle.fpn_width_oracle import FPN_WIDTH_CASES, FpnWidthOracle, case_cfg, case_inputs
+from oracle.dd3d_oracle import DD3DOracle
+from oracle.fpn_width_oracle import FPN_WIDTH_CASES, case_cfg, case_inputs
 from oracle.gen_golden import CASES, inventory_digest
 from util import quat_dist
 
@@ -90,7 +91,7 @@ def test_oracle_matches_reference_golden(case):
     fixtures."""
     g = np.load(os.path.join(GOLDEN_DIR, "golden_fpn_width.npz"))
     cfg = case_cfg(case)
-    out = FpnWidthOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
+    out = DD3DOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
     total = 0
     for b, o in enumerate(out):
         p = f"{case}/"

@@ -19,7 +19,8 @@ from dd3d_b200.arch import FPN_WIDTHS
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_inputs, make_nusc_inputs, make_state_dict
-from oracle.fpn_width_oracle import FPN_WIDTH_CASES, FpnWidthOracle, case_cfg, case_inputs
+from oracle.dd3d_oracle import DD3DOracle
+from oracle.fpn_width_oracle import FPN_WIDTH_CASES, case_cfg, case_inputs
 from util import quat_dist
 
 pytestmark = pytest.mark.gpu
@@ -58,7 +59,7 @@ def test_forward_vs_emulating_oracle(case, act_dtype):
     out = model(inputs)
     torch.cuda.synchronize()
     assert model.overflow_flags() == 0
-    ref = FpnWidthOracle(cfg, make_state_dict(cfg), emulate=act_dtype, threads=1).forward(inputs)
+    ref = DD3DOracle(cfg, make_state_dict(cfg), emulate=act_dtype, threads=1).forward(inputs)
     gn = act_dtype == "bf16" and cfg.FE.FPN.NORM == "GN"
     bounds = _BOUNDS_GN_BF16 if gn else _BOUNDS
     worst = {f: 0.0 for f in bounds}

@@ -1,6 +1,6 @@
 """CPU suite for the FPN / FCOS head structure keys (FCOS2D.NORM, FCOS3D.NORM, FE.FPN.NORM, the tower depths and
-FE.FPN.FUSE_TYPE): parameter inventory against the reference, the oracle against the reference's own forward, the default
-layout's bit-identity with DD3DOracle, the cfg -> dd3d_layout_desc round trip and the refusals."""
+FE.FPN.FUSE_TYPE): parameter inventory against the reference, the oracle against the reference's own forward, the
+cfg -> dd3d_layout_desc round trip and the refusals."""
 import json
 import os
 import re
@@ -14,8 +14,9 @@ from dd3d_b200.arch import param_specs
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200
 from dd3d_b200.synthetic import make_state_dict
+from oracle.dd3d_oracle import DD3DOracle
 from oracle.gen_golden import inventory_digest
-from oracle.head_norm_oracle import HEAD_NORM_CASES, HeadNormOracle, case_cfg, case_inputs
+from oracle.head_norm_oracle import HEAD_NORM_CASES, case_cfg, case_inputs
 from util import quat_dist
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -76,7 +77,7 @@ def test_oracle_matches_reference_golden(case):
     VoVNet fixtures."""
     g = np.load(os.path.join(GOLDEN_DIR, "golden_head_norms.npz"))
     cfg = case_cfg(case)
-    out = HeadNormOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
+    out = DD3DOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
     total = 0
     for b, o in enumerate(out):
         p = f"{case}/"
@@ -92,21 +93,6 @@ def test_oracle_matches_reference_golden(case):
         np.testing.assert_allclose(o["tvec"].numpy(), g[f"{p}tvec{b}"], rtol=1e-3, atol=1e-3)
         np.testing.assert_allclose(o["size"].numpy(), g[f"{p}size{b}"], rtol=1e-4)
     assert total > 0
-
-
-@pytest.mark.parametrize("backbone", ["dla34", "v2_99"])
-def test_head_norm_oracle_is_dd3d_oracle_on_defaults(backbone):
-    from oracle.dd3d_oracle import DD3DOracle
-    cfg = get_cfg(backbone, "nuscenes")
-    sd = make_state_dict(cfg)
-    inputs = case_inputs("dla34_gn")
-    a, ia = DD3DOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs, return_intermediates=True)
-    b, ib = HeadNormOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs, return_intermediates=True)
-    assert all(x.equal(y) for x, y in zip(ia["features"], ib["features"]))
-    for k, v in ia["maps"].items():
-        assert all(x.equal(y) for x, y in zip(v, ib["maps"][k])), k
-    for x, y in zip(a, b):
-        assert all(x[k].equal(y[k]) for k in x)
 
 
 def test_layout_round_trip():

@@ -15,7 +15,8 @@ from dd3d_b200 import lib
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_nusc_inputs, make_state_dict
-from oracle.head_norm_oracle import HEAD_NORM_CASES, HeadNormOracle, case_cfg, case_inputs
+from oracle.dd3d_oracle import DD3DOracle
+from oracle.head_norm_oracle import HEAD_NORM_CASES, case_cfg, case_inputs
 from util import det_key, match_by_key, quat_dist, rel_err
 
 pytestmark = pytest.mark.gpu
@@ -154,7 +155,7 @@ def test_forward_vs_emulating_oracle(case, act_dtype):
     out = model(inputs)
     torch.cuda.synchronize()
     assert model.overflow_flags() == 0
-    ref, inter = HeadNormOracle(cfg, sd, emulate=act_dtype, threads=1).forward(inputs, return_intermediates=True)
+    ref, inter = DD3DOracle(cfg, sd, emulate=act_dtype, threads=1).forward(inputs, return_intermediates=True)
     x = model.get_tensor("input")[..., :3].float().cpu().permute(0, 3, 1, 2)
     assert torch.equal(x, inter["batch"])
     m = inter["maps"]
@@ -246,7 +247,7 @@ def test_nuscenes_with_gn_heads():
     inputs = make_nusc_inputs(1, 128, 192, 1266.4)
     out = model(inputs)
     assert model.overflow_flags() == 0
-    emu = HeadNormOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs)
+    emu = DD3DOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs)
     matched = total = attr_same = 0
     for o, e in zip(out, emu):
         inst = o["instances"]

@@ -15,8 +15,9 @@ from dd3d_b200.arch import fpn_output_names, in_feature_levels, level_strides, p
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_state_dict
+from oracle.dd3d_oracle import DD3DOracle
 from oracle.gen_golden import CASES, inventory_digest
-from oracle.in_features_oracle import IN_FEATURES_CASES, InFeaturesOracle, case_cfg, case_inputs
+from oracle.in_features_oracle import IN_FEATURES_CASES, case_cfg, case_inputs
 from util import quat_dist
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -99,7 +100,7 @@ def test_oracle_matches_reference_golden(case):
     (the position) and the 3-D fields, whose depth takes scales_depth / offsets_depth by position."""
     g = np.load(os.path.join(GOLDEN_DIR, "golden_in_features.npz"))
     cfg = case_cfg(case)
-    out = InFeaturesOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
+    out = DD3DOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
     total = 0
     for b, o in enumerate(out):
         p = f"{case}/"
@@ -127,10 +128,10 @@ def test_depth_offset_is_taken_by_position():
     cfg.DD3D.FCOS3D.MIN_DEPTH, cfg.DD3D.FCOS3D.MAX_DEPTH = -1e6, 1e6  # no clamp: the offset shows through unchanged
     sd = make_state_dict(cfg)
     inputs = case_inputs("dla34_p6_p3")
-    _, a = InFeaturesOracle(cfg, sd).forward(inputs, return_intermediates=True)
+    _, a = DD3DOracle(cfg, sd).forward(inputs, return_intermediates=True)
     sd2 = dict(sd)
     sd2["fcos3d_head.offsets_depth.1.bias"] = sd["fcos3d_head.offsets_depth.1.bias"] + 7.0
-    _, b = InFeaturesOracle(cfg, sd2).forward(inputs, return_intermediates=True)
+    _, b = DD3DOracle(cfg, sd2).forward(inputs, return_intermediates=True)
     for da, db in zip(a["pre_nms"], b["pre_nms"]):
         on = da["level"] == 1
         assert on.any()

@@ -16,7 +16,8 @@ from dd3d_b200 import lib
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_nusc_inputs, make_state_dict
-from oracle.in_features_oracle import IN_FEATURES_CASES, InFeaturesOracle, case_cfg, case_inputs
+from oracle.dd3d_oracle import DD3DOracle
+from oracle.in_features_oracle import IN_FEATURES_CASES, case_cfg, case_inputs
 from util import quat_dist
 
 pytestmark = pytest.mark.gpu
@@ -55,7 +56,7 @@ def _pair_tile():
 @functools.lru_cache(maxsize=None)
 def _oracle(case, act_dtype):
     cfg = case_cfg(case, act_dtype=act_dtype)
-    return InFeaturesOracle(cfg, make_state_dict(cfg), emulate=act_dtype, threads=1).forward(_inputs(case))
+    return DD3DOracle(cfg, make_state_dict(cfg), emulate=act_dtype, threads=1).forward(_inputs(case))
 
 
 def _snap(out):
@@ -186,7 +187,7 @@ def test_do_nms_off_holds_every_level_candidate():
     m.postprocess_in_inference = False
     out = m(case_inputs("v2_99_p6_p3"))
     assert m.overflow_flags() == 0
-    _, inter = InFeaturesOracle(cfg, make_state_dict(cfg), emulate="bf16", threads=1).forward(
+    _, inter = DD3DOracle(cfg, make_state_dict(cfg), emulate="bf16", threads=1).forward(
         case_inputs("v2_99_p6_p3"), return_intermediates=True)
     for o, r in zip(out, inter["pre_nms"]):
         n_pre = r["box2d"].shape[0]
@@ -277,7 +278,7 @@ def test_tta_vs_emulating_oracle():
     inst = tta([x])[0]["instances"]
     assert tta.overflow_flags() == 0
     assert tuple(inst.image_size) == (x["height"], x["width"])
-    emu = T.tta_forward(InFeaturesOracle(cfg, sd, emulate="bf16"), x, cfg.TEST.AUG.MIN_SIZES, cfg.TEST.AUG.MAX_SIZE,
+    emu = T.tta_forward(DD3DOracle(cfg, sd, emulate="bf16"), x, cfg.TEST.AUG.MIN_SIZES, cfg.TEST.AUG.MAX_SIZE,
                         cfg.TEST.AUG.FLIP, cfg.TEST.IMS_PER_BATCH, cfg.DD3D.FCOS2D.INFERENCE.NMS_THRESH)
     n, m = len(inst), emu["score3d"].shape[0]
     assert m > 0 and abs(n - m) <= 0.1 * m

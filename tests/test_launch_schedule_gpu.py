@@ -10,8 +10,7 @@ from dd3d_b200 import lib
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200
 from dd3d_b200.synthetic import make_inputs, make_state_dict
-from oracle.gen_golden import case_inputs
-from oracle.head_norm_oracle import set_key
+from oracle.gen_golden import case_inputs, set_key
 from oracle import num_classes_oracle
 
 pytestmark = pytest.mark.gpu

@@ -14,7 +14,7 @@ from dd3d_b200 import lib
 from dd3d_b200.arch import param_specs
 from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_state_dict
-from oracle.fpn_width_oracle import FpnWidthOracle
+from oracle.dd3d_oracle import DD3DOracle
 from oracle.gen_golden import inventory_digest
 from oracle.num_classes_oracle import NUM_CLASSES_CASES, canonical_sizes, case_cfg, case_inputs, num_classes_cfg
 from util import quat_dist
@@ -52,7 +52,7 @@ def test_oracle_matches_reference_golden(case):
     tests/test_dla_x.py."""
     g = np.load(os.path.join(GOLDEN_DIR, "golden_num_classes.npz"))
     cfg = case_cfg(case)
-    out = FpnWidthOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
+    out = DD3DOracle(cfg, make_state_dict(cfg)).forward(case_inputs(case))
     total = 0
     for b, o in enumerate(out):
         p = f"{case}/"

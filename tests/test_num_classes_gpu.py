@@ -17,7 +17,7 @@ from conftest import GOLDEN_DIR
 from dd3d_b200 import lib
 from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_inputs, make_nusc_inputs, make_state_dict
-from oracle.fpn_width_oracle import FpnWidthOracle
+from oracle.dd3d_oracle import DD3DOracle
 from oracle.num_classes_oracle import NUM_CLASSES_CASES, case_cfg, case_inputs, num_classes_cfg
 from util import quat_dist
 
@@ -205,7 +205,7 @@ def test_forward_vs_emulating_oracle(case, act_dtype, sparse):
     out = model(inputs)
     torch.cuda.synchronize()
     assert model.overflow_flags() == 0
-    ref = FpnWidthOracle(cfg, make_state_dict(cfg), emulate=act_dtype, threads=1).forward(inputs)
+    ref = DD3DOracle(cfg, make_state_dict(cfg), emulate=act_dtype, threads=1).forward(inputs)
     worst = {f: 0.0 for f in _BOUNDS}
     n = 0
     for b, (o, r) in enumerate(zip(out, ref)):

@@ -13,8 +13,9 @@ from dd3d_b200.arch import VOVNET_SPECS, arch_of, param_specs
 from dd3d_b200.config import get_cfg
 from dd3d_b200.meta_arch import DD3DB200
 from dd3d_b200.synthetic import make_state_dict
+from oracle.dd3d_oracle import VOVNET, DD3DOracle
 from oracle.gen_golden import inventory_digest
-from oracle.vovnet_oracle import VOVNET, VOVNET_ARCHS, VOVNET_CASE, VoVNetOracle, case_inputs
+from oracle.vovnet_oracle import VOVNET_ARCHS, VOVNET_CASE, case_inputs
 from util import quat_dist
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
@@ -70,7 +71,7 @@ def test_oracle_matches_reference_golden(arch):
     """Oracle (fp32) vs the reference's own DD3D.forward (oracle/vovnet_oracle.py --golden), same bounds as for V2-99."""
     g = np.load(os.path.join(GOLDEN_DIR, "golden_vovnet.npz"))
     cfg = _cfg(arch)
-    out = VoVNetOracle(cfg, make_state_dict(cfg)).forward(case_inputs(arch))
+    out = DD3DOracle(cfg, make_state_dict(cfg)).forward(case_inputs(arch))
     total = 0
     for b, o in enumerate(out):
         p = f"{arch}/"
@@ -118,15 +119,3 @@ def test_v2_99_recipe_unchanged_by_the_family():
                            "backbone.bottom_up.stem.stem_1/norm.weight"]
     assert not any("dw_conv3x3" in k or "conv_reduction" in k for k in a)
 
-
-def test_vovnet_oracle_is_the_v2_99_oracle_for_v2_99():
-    """The generic VoVNet forward reproduces the V2-99 oracle bit for bit (storage emulation included)."""
-    from oracle.dd3d_oracle import DD3DOracle
-    from oracle.gen_golden import CASES
-    from oracle.gen_golden import case_inputs as v99_inputs
-    cfg = get_cfg("v2_99", CASES["v2_99"][0])
-    sd = make_state_dict(cfg)
-    batch = DD3DOracle(cfg, sd, emulate="bf16").preprocess(v99_inputs("v2_99"))[0]
-    a = DD3DOracle(cfg, sd, emulate="bf16").backbone(batch)
-    b = VoVNetOracle(cfg, sd, emulate="bf16").backbone(batch)
-    assert all(x.equal(y) for x, y in zip(a, b))

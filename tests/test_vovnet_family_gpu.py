@@ -17,7 +17,8 @@ from dd3d_b200.meta_arch import DD3DB200, NuscenesDD3DB200
 from dd3d_b200.synthetic import make_nusc_inputs, make_state_dict
 from oracle import bev_nms_oracle
 from oracle.dd3d_oracle import pose_of
-from oracle.vovnet_oracle import VOVNET_ARCHS, VOVNET_CASE, VoVNetOracle, case_inputs
+from oracle.dd3d_oracle import DD3DOracle
+from oracle.vovnet_oracle import VOVNET_ARCHS, VOVNET_CASE, case_inputs
 from util import det_key, match_by_key, quat_dist, rel_err
 
 pytestmark = pytest.mark.gpu
@@ -118,7 +119,7 @@ def test_forward_vs_emulating_oracle(arch, act_dtype):
     out = model(inputs)
     torch.cuda.synchronize()
     assert model.overflow_flags() == 0
-    ref, inter = VoVNetOracle(cfg, sd, emulate=act_dtype, threads=1).forward(inputs, return_intermediates=True)
+    ref, inter = DD3DOracle(cfg, sd, emulate=act_dtype, threads=1).forward(inputs, return_intermediates=True)
     x = model.get_tensor("input")[..., :3].float().cpu().permute(0, 3, 1, 2)
     assert torch.equal(x, inter["batch"])
     for l in range(5):
@@ -239,7 +240,7 @@ def test_nuscenes_sample_aggregation_v2_39():
         assert torch.equal(gd["score3d"], r["score3d"])
         assert quat_dist(gd["quat_global"], r["quat_global"]).max().item() < 1e-5 if len(gd["score3d"]) else True
         np.testing.assert_allclose(gd["tvec_global"].numpy(), r["tvec_global"].numpy(), rtol=1e-5, atol=1e-4)
-    emu = VoVNetOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs)
+    emu = DD3DOracle(cfg, sd, emulate="bf16", threads=1).forward(inputs)
     matched = total = 0
     for gd, e in zip(got, emu):
         ka = [det_key(l, loc, c) for l, loc, c in zip(gd["level"], gd["loc"], gd["cls"])]
