@@ -5,6 +5,7 @@
 #include <string>
 
 #include "engine.cuh"
+#include "model_file.cuh"
 
 using namespace dd3d;
 
@@ -74,6 +75,59 @@ void dd3d_destroy(dd3d_handle h) {
 }
 
 const char* dd3d_last_error(dd3d_handle h) { return h ? h->err.c_str() : g_create_error.c_str(); }
+
+int dd3d_create_from_file(const char* path, dd3d_handle* out) {
+    if (path == nullptr || out == nullptr) return DD3D_ERR_INVALID;
+    *out = nullptr;
+    ModelFile mf;
+    try {
+        if (!read_model_file(path, &mf, &g_create_error)) return DD3D_ERR_INVALID;
+    } catch (const std::exception& e) {  // std::bad_alloc for a file larger than memory
+        g_create_error = std::string("cannot read model file: ") + e.what();
+        return DD3D_ERR_INVALID;
+    }
+    // the calls DD3DB200._engine() makes, in its order
+    dd3d_handle h = nullptr;
+    int st = dd3d_create(&mf.desc, &h);
+    if (st != DD3D_OK) {
+        g_create_error = "dd3d_create: " + g_create_error;
+        return st;
+    }
+    std::string call;
+    const auto step = [&](const std::string& name, auto&& f) {
+        if (st != DD3D_OK) return;
+        call = name;
+        st = f();
+    };
+    step("dd3d_set_layout", [&] { return dd3d_set_layout(h, &mf.layout); });
+    step("dd3d_set_backbone_norm", [&] { return dd3d_set_backbone_norm(h, mf.backbone_norm); });
+    step("dd3d_set_fpn_channels", [&] { return dd3d_set_fpn_channels(h, mf.fpn_channels); });
+    if (!mf.fpn_inputs.empty())
+        step("dd3d_set_fpn_inputs", [&] { return dd3d_set_fpn_inputs(h, mf.fpn_inputs.data(), int(mf.fpn_inputs.size())); });
+    if (!mf.in_features.empty())
+        step("dd3d_set_in_features",
+             [&] { return dd3d_set_in_features(h, mf.in_features.data(), int(mf.in_features.size())); });
+    if (mf.canon_classes > 0)
+        step("dd3d_set_canonical_sizes", [&] { return dd3d_set_canonical_sizes(h, mf.canon_classes, mf.canon.data()); });
+    std::vector<float> data;  // a record's fp32 data need not be 4-byte aligned in the file
+    for (const ModelFileTensor& t : mf.tensors) {
+        step("dd3d_load_weight('" + t.name + "')", [&] {
+            data.resize(std::max<size_t>(t.count, 1));
+            memcpy(data.data(), mf.bytes.data() + t.data_offset, 4 * t.count);
+            return dd3d_load_weight(h, t.name.c_str(), data.data(), t.shape.data(), int(t.shape.size()));
+        });
+    }
+    step("dd3d_finalize", [&] { return dd3d_finalize(h); });
+    if (st != DD3D_OK) {
+        g_create_error = call + ": " + h->err;
+        dd3d_destroy(h);
+        return st;
+    }
+    *out = h;
+    return DD3D_OK;
+}
+
+int dd3d_out_cap(dd3d_handle h) { return (h && h->eng) ? h->eng->desc.out_cap : DD3D_ERR_INVALID; }
 
 int dd3d_size_divisibility(dd3d_handle h) { return (h && h->eng) ? h->eng->size_divisibility() : DD3D_ERR_INVALID; }
 

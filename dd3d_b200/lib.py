@@ -4,7 +4,11 @@ There is NO fallback: if the shared library has not been built (``python -c "imp
 or ``make -C dd3d_b200/csrc``) loading raises, and every compute entry point fails without a CUDA device.
 """
 import ctypes as C
+import hashlib
 import os
+import struct
+import sys
+from typing import Callable, NamedTuple, Optional
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_lib", "libdd3d_b200.so")
@@ -88,6 +92,8 @@ SIGNATURES = {
     "dd3d_create": (_I, [C.POINTER(ModelDesc), C.POINTER(_P)]),
     "dd3d_destroy": (None, [_P]),
     "dd3d_last_error": (C.c_char_p, [_P]),
+    "dd3d_create_from_file": (_I, [C.c_char_p, C.POINTER(_P)]),
+    "dd3d_out_cap": (_I, [_P]),
     "dd3d_size_divisibility": (_I, [_P]),
     "dd3d_set_layout": (_I, [_P, C.POINTER(LayoutDesc)]),
     "dd3d_set_backbone_norm": (_I, [_P, C.c_int32]),
@@ -307,6 +313,60 @@ def act_dtype_of(cfg):
     if name not in ("bf16", "fp16"):
         raise ValueError(f"B200.ACT_DTYPE must be 'bf16' or 'fp16', got {name!r}")
     return ACT_FP16 if name == "fp16" else ACT_BF16
+
+
+class EngineSpec(NamedTuple):
+    """What dd3d_create .. dd3d_finalize receive, in call order (DD3DB200._engine_spec): DD3DB200._engine makes the calls
+    from it, write_model_file stores it for dd3d_create_from_file, which makes the same calls."""
+    desc: ModelDesc
+    layout: LayoutDesc
+    backbone_norm: int                  # dd3d_set_backbone_norm
+    fpn_channels: int                   # dd3d_set_fpn_channels
+    fpn_inputs: Optional[tuple]         # (int32 array, n) of dd3d_set_fpn_inputs, or None: not called
+    in_features: Optional[tuple]        # (int32 array, n) of dd3d_set_in_features, or None: not called
+    canonical_sizes: Optional[tuple]    # (num_classes, float array) of dd3d_set_canonical_sizes, or None: not called
+    tensors: Callable                   # () -> iterable of (name, contiguous fp32 CPU tensor), one dd3d_load_weight each
+
+
+MODEL_FILE_MAGIC = b"DD3DB200"
+MODEL_FILE_VERSION = 1
+MODEL_FILE_HEADER = struct.Struct("<8sIIIIQ")  # magic, version, desc bytes, layout bytes, tensor records, file bytes
+
+
+def write_model_file(path, spec):
+    """Writes `spec` as the self-contained model file dd3d_create_from_file reads (layout: include/dd3d_b200.h): header,
+    dd3d_model_desc, dd3d_layout_desc, the dd3d_set_* values, one record per tensor, then the 8-byte BLAKE2b checksum of
+    everything before it.  Host only: no GPU is needed."""
+    if sys.byteorder != "little":
+        raise NotImplementedError("the model file is little-endian and written from the host's own struct layout")
+    tensors = list(spec.tensors())
+
+    def int_list(arg):
+        return struct.pack("<I", 0) if arg is None else struct.pack("<I", arg[1]) + bytes(arg[0])
+
+    canon = spec.canonical_sizes
+    body = (bytes(spec.desc) + bytes(spec.layout) + struct.pack("<ii", spec.backbone_norm, spec.fpn_channels) +
+            int_list(spec.fpn_inputs) + int_list(spec.in_features) +
+            (struct.pack("<I", 0) if canon is None else struct.pack("<I", canon[0]) + bytes(canon[1])))
+    heads = [struct.pack(f"<I{len(name.encode())}sI{t.dim()}q", len(name.encode()), name.encode(), t.dim(), *t.shape)
+             for name, t in tensors]
+    size = MODEL_FILE_HEADER.size + len(body) + sum(len(h) + 4 * t.numel() for h, (_, t) in zip(heads, tensors)) + 8
+    digest = hashlib.blake2b(digest_size=8)
+    with open(path, "wb") as f:
+        def put(data):
+            digest.update(data)
+            f.write(data)
+
+        put(MODEL_FILE_HEADER.pack(MODEL_FILE_MAGIC, MODEL_FILE_VERSION, C.sizeof(ModelDesc), C.sizeof(LayoutDesc),
+                                   len(tensors), size))
+        put(body)
+        for head, (name, t) in zip(heads, tensors):
+            data = t.reshape(-1).numpy()
+            if data.dtype.str != "<f4":
+                raise TypeError(f"tensor {name}: the model file holds fp32, got {data.dtype}")
+            put(head)
+            put(memoryview(data).cast("B"))
+        f.write(digest.digest())
 
 
 def check(status, handle=None):

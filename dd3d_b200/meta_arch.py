@@ -121,6 +121,25 @@ class DD3DB200(nn.Module):
         except Exception:  # noqa: BLE001
             pass
 
+    def _engine_spec(self):
+        """The config-to-ABI mapping: everything dd3d_create .. dd3d_finalize receive for this model, in call order
+        (_engine makes the calls, save_model_file stores them)."""
+        if self._state is None:
+            raise RuntimeError("DD3DB200: load_state_dict() must be called before forward() or save_model_file()")
+        # pixel mean/std travel in the state_dict like in the reference (core.py:54-55)
+        for i in range(3):
+            self._desc.pixel_mean[i] = float(self._state["pixel_mean"].reshape(-1)[i])
+            self._desc.pixel_std[i] = float(self._state["pixel_std"].reshape(-1)[i])
+        self._desc.do_nms = int(self.do_nms)
+
+        def tensors():
+            for name, t in self._state.items():
+                if t.is_floating_point():
+                    yield name, t.to(torch.float32).contiguous()
+
+        return _lib.EngineSpec(self._desc, self._layout, self._backbone_norm, self._fpn_channels, self._fpn_inputs,
+                               self._in_features, None if self._canon is None else (self.num_classes, self._canon), tensors)
+
     def _engine(self):
         if self._handle is not None:
             return self._handle
@@ -129,32 +148,36 @@ class DD3DB200(nn.Module):
         if self._device.type != "cuda":
             raise RuntimeError("DD3DB200 runs on CUDA sm_90a (H100) only (model.to('cuda')); there is no CPU path")
         L = _lib.load()
-        # pixel mean/std travel in the state_dict like in the reference (core.py:54-55)
-        for i in range(3):
-            self._desc.pixel_mean[i] = float(self._state["pixel_mean"].reshape(-1)[i])
-            self._desc.pixel_std[i] = float(self._state["pixel_std"].reshape(-1)[i])
-        self._desc.do_nms = int(self.do_nms)
+        spec = self._engine_spec()
         handle = C.c_void_p()
         with torch.cuda.device(self._device):
-            _lib.check(L.dd3d_create(C.byref(self._desc), C.byref(handle)))
-            _lib.check(L.dd3d_set_layout(handle, C.byref(self._layout)), handle)
-            _lib.check(L.dd3d_set_backbone_norm(handle, self._backbone_norm), handle)
-            _lib.check(L.dd3d_set_fpn_channels(handle, self._fpn_channels), handle)
-            if self._fpn_inputs is not None:  # before dd3d_set_in_features, whose indices range over the FPN's outputs
-                _lib.check(L.dd3d_set_fpn_inputs(handle, *self._fpn_inputs), handle)
-            if self._in_features is not None:
-                _lib.check(L.dd3d_set_in_features(handle, *self._in_features), handle)
-            if self._canon is not None:
-                _lib.check(L.dd3d_set_canonical_sizes(handle, self.num_classes, self._canon), handle)
-            for name, t in self._state.items():
-                if not t.is_floating_point():
-                    continue
-                t = t.to(torch.float32).contiguous()
+            _lib.check(L.dd3d_create(C.byref(spec.desc), C.byref(handle)))
+            _lib.check(L.dd3d_set_layout(handle, C.byref(spec.layout)), handle)
+            _lib.check(L.dd3d_set_backbone_norm(handle, spec.backbone_norm), handle)
+            _lib.check(L.dd3d_set_fpn_channels(handle, spec.fpn_channels), handle)
+            if spec.fpn_inputs is not None:  # before dd3d_set_in_features, whose indices range over the FPN's outputs
+                _lib.check(L.dd3d_set_fpn_inputs(handle, *spec.fpn_inputs), handle)
+            if spec.in_features is not None:
+                _lib.check(L.dd3d_set_in_features(handle, *spec.in_features), handle)
+            if spec.canonical_sizes is not None:
+                _lib.check(L.dd3d_set_canonical_sizes(handle, *spec.canonical_sizes), handle)
+            for name, t in spec.tensors():
                 shape = (C.c_int64 * max(t.dim(), 1))(*t.shape)
                 _lib.check(L.dd3d_load_weight(handle, name.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()), handle)
             _lib.check(L.dd3d_finalize(handle), handle)
         self._handle = handle
         return handle
+
+    def save_model_file(self, path):
+        """Writes this model -- the engine's config values and the loaded state_dict's tensors -- to one self-contained
+        file from which dd3d_create_from_file (include/dd3d_b200.h) builds the same engine in a C or C++ program, without
+        Python, torch or the checkpoint.  Needs load_state_dict; no GPU.  The file holds do_nms as it is now and the
+        output capacity the forward uses with it; postprocess_in_inference, do_bev_nms, the sample aggregation and the
+        poses are run-time switches the caller sets per call, as on this model."""
+        spec = self._engine_spec()
+        desc = _lib.ModelDesc.from_buffer_copy(spec.desc)
+        desc.out_cap = max(desc.out_cap, self._needed_out_cap())
+        _lib.write_model_file(path, spec._replace(desc=desc))
 
     def _plan(self, B, Hs, Ws):
         key = (B, Hs, Ws)
@@ -173,10 +196,9 @@ class DD3DB200(nn.Module):
         L * PRE_NMS_TOPK detections per image survive (L head levels): an engine planned with the small NMS-sized output buffer is rebuilt
         with the large one instead of silently truncating (the reference never truncates).  With do_bev_nms the engine
         runs the BEV NMS as its last op, then detector_postprocess (core.py:137-160)."""
-        inf = self.cfg.DD3D.FCOS2D.INFERENCE
         if self.do_bev_nms and self.only_box2d:
             self.do_bev_nms = False  # core.py:137: the BEV NMS needs the 3-D boxes
-        need = _lib.max_candidates(self.cfg) if (not self.do_nms or inf.POST_NMS_TOPK <= 0) else 0
+        need = self._needed_out_cap()
         if need > self._desc.out_cap:
             self._release()
             self._desc.out_cap = need
@@ -185,6 +207,12 @@ class DD3DB200(nn.Module):
         _lib.check(L.dd3d_set_option(h, b"do_postprocess", int(postprocess_in_forward)), h)
         _lib.check(L.dd3d_set_option(h, b"do_nms", int(self.do_nms)), h)
         _lib.check(L.dd3d_set_bev_nms(h, int(self.do_bev_nms), float(self.bev_nms_iou_thresh)), h)
+
+    def _needed_out_cap(self):
+        """Detection slots per image the forward needs at least under the current do_nms: every candidate without the NMS
+        or its post-NMS top-k, else 0 (the desc's NMS-sized buffer)."""
+        inf = self.cfg.DD3D.FCOS2D.INFERENCE
+        return _lib.max_candidates(self.cfg) if (not self.do_nms or inf.POST_NMS_TOPK <= 0) else 0
 
     def _check_flags(self, flags):
         """Overflow word of the last forward (folded into the counts D2H): any set bit means the output differs from the

@@ -155,7 +155,35 @@ typedef struct dd3d_tta_view {
 /* ---- lifetime ------------------------------------------------------------------------------------------- */
 int dd3d_create(const dd3d_model_desc* h_desc, dd3d_handle* out);
 void dd3d_destroy(dd3d_handle h);
-const char* dd3d_last_error(dd3d_handle h); /* h may be NULL: error of the last failed dd3d_create */
+const char* dd3d_last_error(dd3d_handle h); /* h may be NULL: error of the last failed dd3d_create or
+                                             * dd3d_create_from_file */
+
+/* ---- self-contained model file: a trained model without Python or the PyTorch checkpoint -----------------------------
+ * dd3d_create_from_file reads a model file written by DD3DB200.save_model_file (dd3d_b200/meta_arch.py) and builds the
+ * engine that model builds from its config and state_dict: dd3d_create, dd3d_set_layout, dd3d_set_backbone_norm,
+ * dd3d_set_fpn_channels, then dd3d_set_fpn_inputs / dd3d_set_in_features / dd3d_set_canonical_sizes when the file holds
+ * them, one dd3d_load_weight per tensor record, dd3d_finalize.  The whole file is read and validated on the host before
+ * the first CUDA call; a defect returns DD3D_ERR_INVALID with dd3d_last_error(NULL) naming it (unreadable file, bad magic,
+ * unknown version, struct size mismatch, truncation, checksum mismatch, a record overrunning the file, a name twice).  An
+ * error of one of the calls above is returned unchanged, its text prefixed with the call.  No handle survives an error.
+ *
+ * Layout, little-endian, no padding:
+ *   char[8] "DD3DB200" | u32 version (1) | u32 size of dd3d_model_desc | u32 size of dd3d_layout_desc |
+ *   u32 tensor records | u64 file size in bytes, checksum included
+ *   dd3d_model_desc: pixel_mean / pixel_std of the state_dict, do_nms and the out_cap of the model's forward
+ *   dd3d_layout_desc | i32 backbone dd3d_norm | i32 FPN width
+ *   u32 n + i32[n] FPN inputs (n = 0: not set) | u32 n + i32[n] head levels (n = 0: not set)
+ *   u32 n + f32[n][3] canonical sizes (n = 0: not set, the desc's 16 rows apply)
+ *   per record: u32 name length + name bytes (no terminator) | u32 ndim (0..8) + i64[ndim] shape | f32 data, row-major
+ *   u64 checksum: BLAKE2b (RFC 7693) with an 8-byte digest of every byte before it
+ * Records hold the reference state_dict's floating-point tensors as fp32, not packed device weights, so a file does not
+ * depend on the kernels' weight layouts.
+ * Run-time switches are not in the file: option "do_postprocess" (dd3d_set_option), dd3d_set_bev_nms,
+ * dd3d_set_sample_aggregate, the poses and groups stay per-call settings of the handle, as for an engine built call by
+ * call. */
+int dd3d_create_from_file(const char* path, dd3d_handle* out);
+/* Detection slots per image of the output buffers of the forwards: dd3d_model_desc.out_cap of the engine. */
+int dd3d_out_cap(dd3d_handle h);
 /* backbone.size_divisibility: 128 (DLA p67) / 64 (VoVNet p6).  Every FPN input list the engine builds ends at stride 32
  * (dd3d_set_fpn_inputs), so the FPN inputs never change it. */
 int dd3d_size_divisibility(dd3d_handle h);
