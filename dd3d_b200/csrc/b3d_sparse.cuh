@@ -57,13 +57,16 @@ cudaError_t launch_b3d_gather(const B3dGatherParams& p, cudaStream_t stream);
 // Sparse box3d tower (tower_tiles.cu): the sparse predictor reads the tower output only in the 3x3 neighbourhoods of the
 // final candidates, so tower layer i of `depth` (0-based) is needed only at the candidates dilated by depth - i pixels
 // (Chebyshev), clipped to the map.  tower_tiles_kernel lists, per layer, the conv tiles that meet that set; the tower convs
-// then run the pair tile in work-list mode (ConvParams::tile_list) on exactly those tiles; every (image, level) list is
-// padded to an even length with an out-of-image tile, so that a pair never spans two levels.
+// then run the pair tile in work-list mode (ConvParams::tile_list) on exactly those 8x8 tiles (kListTile); every (image, level)
+// list is padded to a multiple of 4 entries with the out-of-image tile, so that a work unit of four tiles never spans two
+// levels or images.
 //
 // Sparse box2d tower: the decode reads the [box2d_reg | centerness] map only at the pixels of P, where some class passes the
 // class-only threshold (class_passes, detect.cuh), and the predictor is a 3x3 conv of the last tower layer.  So list `depth`
 // - 1 (the predictor's) holds the tiles that meet P, and tower layer i the tiles within depth - 1 - i of it.  Its seeds come
-// from a pixel-parallel marking pass over the cls maps (launch_tower_mark), which lowers the tile distances in `dist`.
+// from a pixel-parallel marking pass over the cls maps (launch_tower_mark), which lowers the tile distances in `dist`.  The
+// predictor (the taps-in-N kernel) works on 16x8 tiles: its list (pred16) holds the 16x8 tiles one of whose two 8x8 halves
+// meets P, unpadded.
 //
 // List i holds the tiles at distance <= reach - i from a seed: reach = depth for the box3d tower (its predictor reads 3x3
 // neighbourhoods of the candidates), depth - 1 for the box2d tower and its predictor.
@@ -82,9 +85,10 @@ struct TowerTilesParams {
                                 // kTowerTileFar between launches (tower_tiles_kernel reads and resets them)
     int num_levels;             // L: lvl[0 .. L) (DecodeParams::num_levels)
     int B, C, topk, depth, reach;
+    int pred16;                  // 1: list depth - 1 is the box2d predictor's, on 16x8 tiles (2 th x tw)
     int cls_pitch, mark_blocks;  // mark pass
     float thresh;                // mark pass: PRE_NMS_THRESH
-    int cap;        // entries per layer: sum over levels of B * (tiles per image, rounded up to even)
+    int cap;        // entries per layer: sum over levels of B * (tiles per image, rounded up to a multiple of 4)
     int max_tiles;  // largest tiles per image of a level (shared memory)
     uint32_t* stage;     // [depth][cap] per-(image, level) lists at fixed offsets
     int32_t* bl_count;   // [depth][L][B] entries of each (image, level) list

@@ -631,9 +631,10 @@ int dd3d_op_conv2d_grouped(const void* d_in, int B, int H, int W, int C, int in_
     return cuda_status(launch_conv(p, device_sms(), static_cast<cudaStream_t>(stream)), nullptr);
 }
 
-int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
-                         const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch, const uint32_t* d_tiles,
-                         const int32_t* d_count, dd3d_stream stream) {
+// the work-list pair tile on tiles th x 8 (th = 16: dd3d_op_conv2d_tiles, kListTile: dd3d_op_conv2d_tiles8x8)
+static int conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
+                        const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch, const uint32_t* d_tiles,
+                        const int32_t* d_count, dd3d_stream stream, int th) {
     if (!d_in || !d_w || !d_scale || !d_bias || !d_out || !d_tiles || !d_count) return DD3D_ERR_INVALID;
     if (B < 1 || B > kTileListMaxImages || H < 1 || W < 1 || cin < 1 || in_pitch < cin || cout < 128 || cout % 128 ||
         out_pitch < cout)
@@ -659,10 +660,10 @@ int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_
     ConvSeg& g = p.seg[0];
     g.H = H;
     g.W = W;
-    g.th = kHaloTh;
-    g.tw = kHaloTw;
-    if (((H + kHaloTh - 1) / kHaloTh) * ((W + kHaloTw - 1) / kHaloTw) >= kTileListMaxTiles) return DD3D_ERR_INVALID;
-    if (!make_act_map_halo(&g.in_map[0], d_in, B, H, W, cin, in_pitch, g_op_fp16) ||
+    g.th = th;
+    g.tw = kListTile;
+    if (((H + th - 1) / th) * ((W + kListTile - 1) / kListTile) >= kTileListMaxTiles) return DD3D_ERR_INVALID;
+    if (!make_act_map(&g.in_map[0], d_in, B, H, W, cin, in_pitch, kListTile + 2, kListTile + 2, g_op_fp16) ||
         !make_out_map(&g.out_map, d_out, B, H, W, cout, out_pitch, g.tw, g_op_fp16) ||
         !make_weight_map(&p.w_map, d_w, 9 * kchunks * kBlockK, cout, p.block_n, g_op_fp16)) {
         fprintf(stderr, "dd3d_op_conv2d_tiles: %s\n", conv_last_error());
@@ -674,6 +675,20 @@ int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_
     conv_finalize_params(&p);
     const cudaError_t e = launch_conv(p, device_sms(), static_cast<cudaStream_t>(stream));
     return e == cudaErrorInvalidValue ? DD3D_ERR_INVALID : cuda_status(e, nullptr);
+}
+
+int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
+                         const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch, const uint32_t* d_tiles,
+                         const int32_t* d_count, dd3d_stream stream) {
+    return conv2d_tiles(d_in, B, H, W, cin, in_pitch, d_w, cout, d_scale, d_bias, relu, d_out, out_pitch, d_tiles, d_count,
+                        stream, 2 * kListTile);
+}
+
+int dd3d_op_conv2d_tiles8x8(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
+                            const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch,
+                            const uint32_t* d_tiles, const int32_t* d_count, dd3d_stream stream) {
+    return conv2d_tiles(d_in, B, H, W, cin, in_pitch, d_w, cout, d_scale, d_bias, relu, d_out, out_pitch, d_tiles, d_count,
+                        stream, kListTile);
 }
 
 int dd3d_op_conv2d_taps_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,

@@ -343,10 +343,11 @@ static int conv_units_per_image(const ConvParams& p, const ConvSeg& g) {
 
 // Dynamic shared memory of everything but the B ring: staging tiles, alignment slack, barriers, (scale, bias) vectors, the
 // eSE partials hand-over (generic variant) and the A patches (pair tile: two staging tiles per consumer warpgroup, two
-// patches per A stage).
+// patches per A stage; in work-list mode four 8x8-tile patches, which leaves room for three B stages).
 static int conv_fixed_smem(const ConvParams& p) {
+    const int a_slot = !p.pair ? kHaloABytes : p.tile_list != nullptr ? 4 * kListABytes : 2 * kHaloABytes;
     return (p.pair ? 4 : 2) * kStagingBytes + 1024 /*alignment slack*/ + kBarBytes + kSbBytes + (p.halo ? 0 : kPoolXBytes) +
-           p.a_stages * (p.pair ? 2 : 1) * kHaloABytes;
+           p.a_stages * a_slot;
 }
 
 static int g_stagger = -1;
@@ -460,6 +461,13 @@ cudaError_t launch_conv(const ConvParams& p, int num_sms, cudaStream_t stream) {
         return cudaErrorInvalidValue;  // block-diagonal mode: one 64-channel k-block per 64-channel n-block
     if (p.pair) {
         if (!p.halo || p.block_n != 128 || p.out_mode != 0) return cudaErrorInvalidValue;
+        // tiling the kernel decodes: 16x8 tiles; in work-list mode 8-wide tiles of one height, 8 or 16 rows
+        for (int s = 0; s < p.nseg; ++s) {
+            const int th = p.seg[s].th, tw = p.seg[s].tw;
+            if (list ? (tw != kListTile || th != p.seg[0].th || (th != kListTile && th != 2 * kListTile))
+                     : (th != kHaloTh || tw != kHaloTw))
+                return cudaErrorInvalidValue;
+        }
         kernel = conv_kernel_pair(p.fp16 != 0, list);
     }
     for (auto group : {conv_kernel_n16_64, conv_kernel_n80_128, conv_kernel_n144_192, conv_kernel_n208_256}) {

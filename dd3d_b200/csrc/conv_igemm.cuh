@@ -63,9 +63,11 @@ struct ConvParams {
     // operand of n-block j is input channels [64 j, 64 j + 64) -- the only channels its 64 output channels read.  Weights
     // [cout][9][64] hold each row's group at its position in the 64-channel block and zeros elsewhere (exact zeros).
     int grouped;
-    // Work-list mode (nullptr: every tile of every segment).  The M units are the entries of tile_list (pair tile: entries
-    // 2i, 2i + 1 form unit i and must lie in one segment), each (seg << 29) | (img << 16) | (row-major tile of the image);
-    // *tile_count entries, read on the device after griddepcontrol.wait.  total_work then only sizes the grid.
+    // Work-list mode (nullptr: every tile of every segment).  The M units come from the entries of tile_list, each
+    // (seg << 29) | (img << 16) | (row-major tile of the image); *tile_count entries, read on the device after
+    // griddepcontrol.wait.  total_work then only sizes the grid.  Taps-in-N: one 16x8 tile per entry and unit.  Pair tile:
+    // the segments' tiles are kListTile wide and th = kListTile (the sparse towers: entries 4i .. 4i + 3 form unit i) or 16
+    // rows high (two 8x8 tiles per entry: entries 2i, 2i + 1 form unit i); the entries of a unit lie in one (segment, image).
     const uint32_t* tile_list;
     const int32_t* tile_count;
     // k-blocks consumer warpgroup 2 starts behind warpgroup 1 (0: both start together); conv_finalize_params picks it so
@@ -88,6 +90,9 @@ void choose_tile(int H, int W, int* th, int* tw);
 int conv_tiles_per_image(int H, int W);  // M-tiles per image of the generic tiling
 // Halo variant (3x3, stride 1): one 128B-swizzled [18][10][64 ch] patch per 64-channel block serves all nine taps.
 constexpr int kHaloTh = 16, kHaloTw = 8;
+// Work-list pair tile: the unit of work is four 8x8 tiles, each read as one [10][10][64 ch] patch (make_act_map with a
+// (kListTile + 2)-square box)
+constexpr int kListTile = 8;
 bool make_act_map_halo(CUtensorMap* map, const void* base, int B, int H, int W, int C, int pitch, int fp16 = 0);
 // Policy: use the halo variant when its fixed 16x8 tiling costs at most 10 % more tiles than the best generic
 // tiling over all segments.

@@ -36,8 +36,12 @@
 // order per output element is unchanged, so results are bit-identical to the 128 x 256 tile.
 //
 // Work-list mode (LIST, pair tile only): the M units come from ConvParams::tile_list, whose length the kernel reads from the
-// device after griddepcontrol.wait, so a launch can cover a tile set an earlier kernel chose (the sparse box3d tower, engine.cu)
-// without a host round trip; the grid stays persistent.  Everything else, K order included, is the dense pair tile's.
+// device after griddepcontrol.wait, so a launch can cover a tile set an earlier kernel chose (the sparse towers, engine.cu)
+// without a host round trip; the grid stays persistent.  The unit is four listed 8x8 tiles (kListTile), so that a sparse tower
+// computes fewer pixels around its seeds than with 16x8 tiles: warpgroup 1 + w owns tiles 2w and 2w + 1, one per 64-row
+// half, each read from its own [10][10][64ch] patch (four patches per A stage, on one barrier).  The descriptor views are the
+// halo tile's (row-group stride of 10 pixels, taps as whole-pixel-row shifts), the weight tile and the K order the dense pair
+// tile's, so every computed pixel is bit-identical to it.  The four patches leave room for three B stages (stagger 1).
 //
 // The kernel is templated on (halo variant, fp16 storage, wgmma N = block_n, pair tile, work list); conv_igemm_n*.cu instantiate it, one
 // group of N values per translation unit so that the build compiles them in parallel; conv_igemm.cu holds the host side and
@@ -68,6 +72,10 @@ constexpr int kHaloABytes = (kHaloPW * kHaloPH * 128 + 1023) / 1024 * 1024;  // 
 constexpr int kHaloAStages = 3;   // default number of A patches in flight
 constexpr int kMaxAStages = 5;    // weight-stationary layers (ConvParams::wstat) spend the freed B ring on deeper A prefetch
 constexpr int kPairAStages = 2;   // pair tile: one patch pair feeds 9 k-blocks, so two pairs in flight suffice
+// work-list pair tile: one (8+2)x(8+2)-pixel patch per 8x8 tile, 1024-byte aligned like the halo patch
+constexpr int kListPW = kListTile + 2;
+static_assert(kListPW == kHaloPW, "the list patches share the halo descriptors' row-group stride");
+constexpr int kListABytes = (kListPW * kListPW * 128 + 1023) / 1024 * 1024;  // 13312
 constexpr int kBarBytes = 512;
 constexpr int kSbBytes = 2 * 2 * 256 * 4;  // per consumer warpgroup: staged (scale, bias) of its current (segment, n-block)
 // generic variant: the eSE pool partials handed from warpgroup 1 (rows 0..63) to warpgroup 2 (rows 64..127), per staging
@@ -89,7 +97,8 @@ __device__ __forceinline__ int fast_div(int x, int d, float inv_d) {
     return q;
 }
 
-// work item = (M-tile, n-block), n-block fastest.  PAIR: the M unit is a pair of tiles, `sub` selects tile 2i + sub.
+// work item = (M-tile, n-block), n-block fastest.  PAIR: the M unit is a pair of tiles, `sub` selects tile 2i + sub; with
+// LIST four 8x8 tiles, `sub` selects 8x8 tile 4i + sub of the list (half `sub & 1` of entry 2i + sub / 2 for 16-row tiles).
 // Called by whole warps (the list entry is broadcast from lane 0, so the coordinates stay provably warp-uniform).
 template <bool PAIR = false, bool LIST = false>
 __device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int work, int sub = 0) {
@@ -100,9 +109,15 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int work, 
         mt = fast_div(work, p.n_blocks, p.inv_n_blocks);
         t.n_blk = work - mt * p.n_blocks;
     }
-    int r;
+    int r, half = 0;
     if (LIST) {
-        const uint32_t e = __shfl_sync(0xffffffffu, __ldg(p.tile_list + (PAIR ? 2 * mt + sub : mt)), 0);
+        int q = mt;
+        if (PAIR) {
+            const int sh = p.seg[0].th >> 4;  // 8x8 tiles per entry: 1 (th 8) or 2 (th 16)
+            q = (4 * mt + sub) >> sh;
+            half = (4 * mt + sub) & sh;
+        }
+        const uint32_t e = __shfl_sync(0xffffffffu, __ldg(p.tile_list + q), 0);
         t.seg = static_cast<int>(e >> 29);
         t.img = static_cast<int>((e >> 16) & (kTileListMaxImages - 1));
         r = static_cast<int>(e & (kTileListMaxTiles - 1));
@@ -124,7 +139,7 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvParams& p, int work, 
     const ConvSeg& g = p.seg[t.seg];
     int ty = fast_div(r, g.tiles_x, g.inv_tiles_x);
     int tx = r - ty * g.tiles_x;
-    t.y0 = ty * g.th;
+    t.y0 = ty * g.th + (LIST && PAIR ? kListTile * half : 0);
     t.x0 = tx * g.tw;
     return t;
 }
@@ -194,12 +209,13 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
     static_assert(!PAIR || (HALO && BN == 128), "the pair tile is a halo variant with block_n 128");
     static_assert(!LIST || PAIR, "work-list mode is instantiated for the pair tile only");
     constexpr int MH = PAIR ? 2 : 1;                                   // 64-row halves per consumer warpgroup
-    constexpr int kASlot = PAIR ? 2 * kHaloABytes : kHaloABytes;       // one A stage: the patch of every sub-tile
+    // one A stage: the patch of every sub-tile (LIST: of every 8x8 tile)
+    constexpr int kASlot = LIST ? 4 * kListABytes : PAIR ? 2 * kHaloABytes : kHaloABytes;
     extern __shared__ uint8_t smem_raw[];
     // 128B-swizzled tiles need 1024-byte alignment
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     // generic: num_stages x [A 16 KiB | B block_n*128].  halo: num_stages x [B block_n*128], then a_stages x [A patch 23 KiB
-    // (PAIR: two patches)], then the staging tiles (PAIR: two per consumer warpgroup)
+    // (PAIR: two patches; LIST: four 13 KiB patches)], then the staging tiles (PAIR: two per consumer warpgroup)
     const int stage_bytes = (HALO ? 0 : kABytes) + BN * 128;
     // weight-stationary (HALO, one n-block, cin <= 64): ALL k-blocks of the weight tensor stay resident in the B region
     // (loaded once per CTA) instead of cycling through the stage ring for every tile
@@ -258,7 +274,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
     const int w_first = static_cast<int>(blockIdx.x), w_step = static_cast<int>(gridDim.x);
     int w_total = p.total_work;
     if (LIST) {  // work-list mode: the list was written by an earlier kernel of the stream
-        const int units = PAIR ? (__ldg(p.tile_count) >> 1) : __ldg(p.tile_count);
+        const int units = PAIR ? ((__ldg(p.tile_count) << (p.seg[0].th >> 4)) >> 2) : __ldg(p.tile_count);
         w_total = __shfl_sync(0xffffffffu, units, 0) * p.n_blocks;
     }
 
@@ -351,7 +367,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
         } else {
             // ------------------------------------------------------------ warp 2: halo A-patch producer: one box
             // [18][10][64 ch] (180 rows of 128 B, 128B-swizzled, zero-filled outside the image) per 64-channel block
-            // (PAIR: one per sub-tile, both on one barrier)
+            // (PAIR: one per sub-tile, both on one barrier; LIST: one [10][10] box per 8x8 tile, all four on one barrier)
             int as = 0;
             uint32_t aphase = 0;
             for (int work = w_first; work < w_total; work += w_step) {
@@ -359,15 +375,26 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                 const TileCoord t1 = PAIR ? decode_tile<PAIR, LIST>(p, work, 1) : t;
                 const ConvSeg& g = p.seg[t.seg];
                 const int a_c0 = p.grouped ? t.n_blk * kBlockK : 0;  // block-diagonal: n-block j reads channels 64 j..
+                // LIST: four [10][10] patches, one per listed 8x8 tile
+                const TileCoord t2 = LIST ? decode_tile<PAIR, LIST>(p, work, 2) : t;
+                const TileCoord t3 = LIST ? decode_tile<PAIR, LIST>(p, work, 3) : t;
+                constexpr int a_bytes = LIST ? 4 * kListPW * kListPW * 128 : MH * kHaloPW * kHaloPH * 128;
+                constexpr int patch = LIST ? kListABytes : kHaloABytes;  // patch spacing in the A stage
                 for (int kc = 0; kc < p.kchunks; ++kc) {
                     ptx::mbar_wait(&aempty_bar[as], aphase ^ 1);
                     if (elect_one()) {
-                        ptx::mbar_expect_tx(&afull_bar[as], MH * kHaloPW * kHaloPH * 128);
+                        ptx::mbar_expect_tx(&afull_bar[as], a_bytes);
                         ptx::tma_load_4d(halo_a + as * kASlot, &g.in_map[0], &afull_bar[as], a_c0 + kc * kBlockK, t.x0 - 1,
                                          t.y0 - 1, t.img);
                         if (PAIR)
-                            ptx::tma_load_4d(halo_a + as * kASlot + kHaloABytes, &g.in_map[0], &afull_bar[as], kc * kBlockK,
+                            ptx::tma_load_4d(halo_a + as * kASlot + patch, &g.in_map[0], &afull_bar[as], kc * kBlockK,
                                              t1.x0 - 1, t1.y0 - 1, t1.img);
+                        if (LIST) {
+                            ptx::tma_load_4d(halo_a + as * kASlot + 2 * patch, &g.in_map[0], &afull_bar[as], kc * kBlockK,
+                                             t2.x0 - 1, t2.y0 - 1, t2.img);
+                            ptx::tma_load_4d(halo_a + as * kASlot + 3 * patch, &g.in_map[0], &afull_bar[as], kc * kBlockK,
+                                             t3.x0 - 1, t3.y0 - 1, t3.img);
+                        }
                     }
                     __syncwarp();
                     if (++as == a_stages) {
@@ -425,7 +452,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             }
         };
         for (int work = w_first; work < w_total; work += w_step) {
-            const TileCoord t = decode_tile<PAIR, LIST>(p, work, PAIR ? wgi : 0);
+            const TileCoord t = decode_tile<PAIR, LIST>(p, work, LIST ? 2 * wgi : PAIR ? wgi : 0);
             const ConvSeg& g = p.seg[t.seg];
             // ---- main loop: one commit group per k-block; the slot (and halo patch) of group i is released after
             // group i + 1 has been issued and group i has retired (wait_group 1)
@@ -441,9 +468,13 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             if (HALO) {
                 for (int kc = 0; kc < p.kchunks; ++kc) {
                     ptx::mbar_wait(&afull_bar[as], aphase);
-                    // rows 64 * wgi.. of the tile's patch; PAIR: row 0 of sub-tile wgi's patch (rows 64.. are 8 patch rows on)
+                    // rows 64 * wgi.. of the tile's patch; PAIR: row 0 of sub-tile wgi's patch (rows 64.. are 8 patch rows on);
+                    // LIST: row 0 of 8x8 tile 2 wgi's patch (rows 64.. are those of tile 2 wgi + 1, the next patch)
                     const uint32_t a_lo = halo_lo + static_cast<uint32_t>(as) * (kASlot >> 4) +
-                                          (PAIR ? wgi * (kHaloABytes >> 4) : wgi * 8 * kHaloPW * 8);
+                                          (LIST   ? 2 * wgi * (kListABytes >> 4)
+                                           : PAIR ? wgi * (kHaloABytes >> 4)
+                                                  : wgi * 8 * kHaloPW * 8);
+                    constexpr uint32_t half1 = LIST ? kListABytes >> 4 : 8 * kHaloPW * 8;  // rows 64.. (PAIR)
                     for (int tap = 0; tap < 9; ++tap) {
                         if (!wstat) ptx::mbar_wait(&full_bar[stage], phase);
                         const int r = tap / 3, s = tap - 3 * r;
@@ -451,7 +482,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
                         const uint32_t b_lo =
                             smem_lo + static_cast<uint32_t>(wstat ? tap * p.kchunks + kc : stage) * stage_units;
                         if constexpr (PAIR)
-                            mma_kblock2<BN, F16>(acc[0], acc[MH - 1], desc_hi | a_tap, desc_hi | (a_tap + 8 * kHaloPW * 8),
+                            mma_kblock2<BN, F16>(acc[0], acc[MH - 1], desc_hi | a_tap, desc_hi | (a_tap + half1),
                                                  bdesc_hi | b_lo, (kc | tap) == 0);
                         else
                             mma_kblock<BN, F16>(acc[0], desc_hi | a_tap, bdesc_hi | b_lo, (kc | tap) == 0);
@@ -494,7 +525,20 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             // ---- epilogue of this warpgroup's 64 rows (PAIR: of its 128-row sub-tile)
             const int n_base = t.n_blk * BN;
             const int tw = HALO ? kHaloTw : g.tw, tw_shift = HALO ? 3 : g.tw_shift;  // the halo tile is 16 x 8
-            static_assert(kHaloTw == 8, "tw_shift of the halo tile");
+            static_assert(kHaloTw == 8 && kListTile == 8, "tw_shift of the halo and list tiles");
+            // origin of each 64-row half in the frame of rows (row0 + row) >> tw_shift.  LIST: half 1 is the warpgroup's second
+            // 8x8 tile, whose rows 64.. sit 8 tile rows below that origin
+            int y_org[MH], x_org[MH];
+#pragma unroll
+            for (int m = 0; m < MH; ++m) {
+                y_org[m] = t.y0;
+                x_org[m] = t.x0;
+            }
+            if constexpr (LIST) {
+                const TileCoord t1 = decode_tile<PAIR, LIST>(p, work, 2 * wgi + 1);
+                y_org[1] = t1.y0 - kListTile;
+                x_org[1] = t1.x0;
+            }
             bool in_img[2 * MH];
             const __nv_bfloat16* res_ptr[2 * MH];
             float* f32_ptr[2 * MH];
@@ -502,7 +546,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
             for (int h = 0; h < 2 * MH; ++h) {
                 const int ly = (row0 + row[h]) >> tw_shift;
                 const int lx = (row0 + row[h]) - (ly << tw_shift);
-                const int oy = t.y0 + ly, ox = t.x0 + lx;
+                const int oy = y_org[h >> 1] + ly, ox = x_org[h >> 1] + lx;
                 in_img[h] = (oy < g.H) && (ox < g.W);
                 res_ptr[h] = nullptr;
                 if (g.residual != nullptr && in_img[h]) {
@@ -589,8 +633,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_igemm_kernel(const __gri
 #pragma unroll
                         for (int m = 0; m < MH; ++m) {
                             const int px = 64 * (PAIR ? m : wgi);
-                            ptx::tma_store_4d(&g.out_map, stag + m * kHalfStagingBytes, n_base + c0, t.x0 + (px & (tw - 1)),
-                                              t.y0 + (px >> tw_shift), t.img);
+                            ptx::tma_store_4d(&g.out_map, stag + m * kHalfStagingBytes, n_base + c0, x_org[m] + (px & (tw - 1)),
+                                              y_org[m] + (px >> tw_shift), t.img);
                         }
                         ptx::tma_store_commit();
                     }

@@ -424,6 +424,7 @@ struct Builder {
     std::vector<ArenaBuf>* bufs = nullptr;
     bool tracing = false;
     int next_buf = 0, op_idx = 0;
+    bool list_tiles = false;  // the halo convs emitted meanwhile are sparse tower layers: kListTile x kListTile tiles
 
     View alloc(int H, int W, int C) {
         View v;
@@ -521,7 +522,11 @@ struct Builder {
             g.W = Wo;
             choose_tile(Ho, Wo, &g.th, &g.tw);
             bool ok;
-            if (p.halo) {
+            if (p.halo && list_tiles) {  // the work-list pair tile: one [10][10] patch per 8x8 tile (use_tile_lists)
+                g.th = g.tw = kListTile;
+                ok = make_act_map(&g.in_map[0], sp.in.ptr, B, sp.in.H, sp.in.W, sp.in.C, sp.in.pitch, kListTile + 2,
+                                  kListTile + 2, E->fp16);
+            } else if (p.halo) {
                 g.th = kHaloTh;
                 g.tw = kHaloTw;
                 ok = make_act_map_halo(&g.in_map[0], sp.in.ptr, B, sp.in.H, sp.in.W, sp.in.C, sp.in.pitch, E->fp16);
@@ -1107,11 +1112,12 @@ struct Builder {
         *out = cur;
     }
 
-    // Tile lists of a sparse tower (TowerTilesParams): `depth` lists, list i at distance <= reach - i; the tiling conv() gives
-    // the tower layers, and the staging, list and count areas in the persistent region.  false: the shapes exceed the list
-    // entry fields or the layers do not run the pair tile, the tower stays dense.  The pair tile needs a width that 128 divides,
-    // so at FPN widths 64, 192, 320 and 448 the sparse box2d / box3d towers always fall back to the dense tower.
-    bool tower_tile_lists(TowerTilesParams& tt, const std::vector<View>& feats, int depth, int reach) {
+    // Tile lists of a sparse tower (TowerTilesParams): `depth` lists, list i at distance <= reach - i, on 8x8 tiles (pred16:
+    // the last one on the box2d predictor's 16x8 tiles), and the staging, list and count areas in the persistent region.
+    // false: the shapes exceed the list entry fields or the layers would not run the pair tile, the tower stays dense.  The
+    // pair tile needs a width that 128 divides, so at FPN widths 64, 192, 320 and 448 the sparse box2d / box3d towers always
+    // fall back to the dense tower.
+    bool tower_tile_lists(TowerTilesParams& tt, const std::vector<View>& feats, int depth, int reach, bool pred16) {
         memset(&tt, 0, sizeof(tt));
         const int L = static_cast<int>(feats.size());
         tt.num_levels = L;
@@ -1126,22 +1132,18 @@ struct Builder {
             TowerTilesLevel& v = tt.lvl[l];
             v.H = hs[l];
             v.W = ws[l];
-            if (halo) {
-                v.th = kHaloTh;
-                v.tw = kHaloTw;
-            } else {
-                choose_tile(v.H, v.W, &v.th, &v.tw);
-            }
+            v.th = v.tw = kListTile;
             v.tiles_x = (v.W + v.tw - 1) / v.tw;
             v.tiles_y = (v.H + v.th - 1) / v.th;
             const int T = v.tiles_x * v.tiles_y;
             v.stage_begin = tt.cap;
-            tt.cap += B * (T + (T & 1));
+            tt.cap += B * ((T + 3) & ~3);
             tt.max_tiles = std::max(tt.max_tiles, T);
         }
         if (B > kTileListMaxImages || tt.max_tiles >= kTileListMaxTiles || tower_tiles_smem_bytes(tt.max_tiles) > 48 * 1024)
             return false;
-        // the work-list mode is built for the pair tile, which every filled halo layer of a 128-multiple width selects (conv())
+        // the work-list mode is built for the pair tile, which every filled halo layer of a 128-multiple width selects (conv());
+        // the fill rule looks at the dense tower's 16x8 tiles
         ConvParams cp;
         memset(&cp, 0, sizeof(cp));
         cp.nseg = L;
@@ -1150,13 +1152,14 @@ struct Builder {
         for (int l = 0; l < L; ++l) {
             cp.seg[l].H = hs[l];
             cp.seg[l].W = ws[l];
-            cp.seg[l].th = tt.lvl[l].th;
-            cp.seg[l].tw = tt.lvl[l].tw;
+            cp.seg[l].th = kHaloTh;
+            cp.seg[l].tw = kHaloTw;
         }
         if (!conv_select_pair(&cp, width, E->num_sms)) return false;
         tt.B = B;
         tt.depth = depth;
         tt.reach = reach;
+        tt.pred16 = pred16 ? 1 : 0;
         const size_t list_bytes = static_cast<size_t>(depth) * tt.cap * 4, bl_bytes = static_cast<size_t>(depth) * L * B * 4;
         tt.stage = static_cast<uint32_t*>(alloc_bytes(list_bytes));
         tt.list = static_cast<uint32_t*>(alloc_bytes(list_bytes));
@@ -1168,19 +1171,21 @@ struct Builder {
         return true;
     }
 
-    // Points plan ops [begin, begin + tt.depth) -- tower convs on the pair tile, then (box2d) the taps-in-N predictor -- at
-    // their tile lists.
+    // Points plan ops [begin, begin + tt.depth) -- tower convs on the pair tile (built with list_tiles), then (box2d) the
+    // taps-in-N predictor -- at their tile lists.
     void use_tile_lists(int begin, const TowerTilesParams& tt, int L, const char* what) {
         for (int j = 0; j < tt.depth; ++j) {
             Op& op = P->ops[begin + j];
             ConvParams& c = op.conv;
-            if (op.type != Op::CONV || c.nseg != L || !(c.pair || c.taps_n))
+            const bool pred = tt.pred16 && j == tt.depth - 1;
+            if (op.type != Op::CONV || c.nseg != L || !(pred ? c.taps_n : c.pair))
                 fail(DD3D_ERR_STATE, std::string("internal: sparse ") + what + " layout");
             for (int l = 0; l < L; ++l)
-                if (c.seg[l].th != tt.lvl[l].th || c.seg[l].tw != tt.lvl[l].tw)
+                if (c.seg[l].th != (pred ? 2 * tt.lvl[l].th : tt.lvl[l].th) || c.seg[l].tw != tt.lvl[l].tw)
                     fail(DD3D_ERR_STATE, std::string("internal: sparse ") + what + " tiling");
             c.tile_list = tt.list + static_cast<size_t>(j) * tt.cap;
             c.tile_count = tt.count + j;
+            conv_finalize_params(&c);  // the list-mode pair tile lays out its shared memory differently
         }
     }
 
@@ -1276,7 +1281,7 @@ struct Builder {
         const bool sparse_box2d =
             d2 > 0 && E->layout.fcos2d_norm != DD3D_NORM_GN &&
             (E->opt_sparse_box2d_tower == 1 || (E->opt_sparse_box2d_tower == 2 && sparse3 && head_px >= 50000)) &&
-            conv_taps_eligible(9, 1, 16, L, hs, ws) && tower_tile_lists(P->box2d_tiles, feats, d2 + 1, d2);
+            conv_taps_eligible(9, 1, 16, L, hs, ws) && tower_tile_lists(P->box2d_tiles, feats, d2 + 1, d2, true);
         P->box2d_begin = sparse_box2d ? static_cast<int>(P->ops.size()) : -1;
         if (sparse_box2d) {
             TowerTilesParams& tt = P->box2d_tiles;
@@ -1289,7 +1294,9 @@ struct Builder {
             }
         }
         // [box2d_reg (4) | centerness (1)] on the box2d tower: relu(scale_l * (conv + b)) / conv + b (fcos2d.py:143-152)
+        list_tiles = sparse_box2d;
         tower("fcos2d_head.box2d_tower", d2, E->layout.fcos2d_norm, feats, &box_t);
+        list_tiles = false;
         {
             const ConvLayer& Lb = E->conv_layer("fcos2d_head.box2d_reg+centerness",
                                                 {"fcos2d_head.box2d_reg", "fcos2d_head.centerness"}, width, 3);
@@ -1330,9 +1337,11 @@ struct Builder {
         const int d3 = E->layout.num_box3d_convs;
         const bool sparse_tower = sparse3 && d3 > 0 && E->layout.fcos3d_norm != DD3D_NORM_GN &&
                                   (E->opt_sparse_tower == 1 || (E->opt_sparse_tower == 2 && head_px >= 50000)) &&
-                                  tower_tile_lists(P->tower_tiles, feats, d3, d3);
+                                  tower_tile_lists(P->tower_tiles, feats, d3, d3, false);
         P->tower_begin = sparse_tower ? static_cast<int>(P->ops.size()) : -1;
+        list_tiles = sparse_tower;
         tower("fcos3d_head.box3d_tower", d3, E->layout.fcos3d_norm, feats, &b3d_t);
+        list_tiles = false;
         if (sparse_tower && !dry) use_tile_lists(P->tower_begin, P->tower_tiles, L, "box3d tower");
         // [quat 4C | ctr 2C | depth C | size 3C | conf C] on the box3d tower with the per-level Scale/Offset folded
         // (fcos3d.py:166-180).  PER_LEVEL_PREDICTORS False (shipped): predictor index 0 for every level, one launch over the

@@ -5,7 +5,8 @@
 // tower's seeds are the final candidates of the decode's `fin` list, read by the CTA itself into shared memory; the box2d
 // tower's are the pixels of P, marked by tower_mark_kernel (one thread per head pixel) in the global `dist` array, which the
 // CTA copies and resets.  List i holds the tiles with distance <= reach - i, in row-major order, written to the (level,
-// image) region of the staging area.  The last CTA to finish (atomic ticket, no waiting) concatenates the regions
+// image) region of the staging area, padded to a multiple of 4 entries (the work unit of the list-mode pair tile) with the
+// out-of-image tile; the box2d predictor's list (pred16) holds 16x8 tiles, unpadded.  The last CTA to finish (atomic ticket, no waiting) concatenates the regions
 // level-major, then image -- a fixed order, so the lists and the conv schedule do not depend on timing -- writes the counts
 // and resets the ticket.
 #include <cuda_runtime.h>
@@ -64,10 +65,11 @@ __device__ __forceinline__ void seed_tiles(int* dist, const TowerTilesLevel& L, 
     }
 }
 
-// (level, image) region of a layer's staging / list area, and of `dist`
+// (level, image) region of a layer's staging / list area, and of `dist`: the level's tiles per image rounded up to a
+// multiple of 4
+__device__ __forceinline__ int region_size(const TowerTilesLevel& L) { return (L.tiles_x * L.tiles_y + 3) & ~3; }
 __device__ __forceinline__ size_t region(const TowerTilesLevel& L, int b) {
-    const int T = L.tiles_x * L.tiles_y;
-    return L.stage_begin + static_cast<size_t>(b) * (T + (T & 1));
+    return L.stage_begin + static_cast<size_t>(b) * region_size(L);
 }
 
 // One thread per head pixel, the grid of the decode's dense passes: the pixels of P seed the tiles around them.
@@ -122,23 +124,32 @@ __global__ void __launch_bounds__(kThreads) tower_tiles_kernel(const TowerTilesP
     uint32_t* stage = p.stage + region(L, b);
     for (int i = 0; i < D; ++i) {
         if (threadIdx.x == 0) s_pix = 0;
+        // the box2d predictor's list: 16x8 tiles, each the 8x8 tiles 2 ty and 2 ty + 1 of a tile column
+        const bool pred = p.pred16 && i == D - 1;
+        const int th = pred ? 2 * L.th : L.th, Ti = (pred ? (L.tiles_y + 1) / 2 : L.tiles_y) * L.tiles_x;
         int written = 0;
-        for (int base = 0; base < T; base += kThreads) {
+        for (int base = 0; base < Ti; base += kThreads) {
             const int t = base + threadIdx.x;
-            const bool on = t < T && s_dist[t] <= p.reach - i;
+            const int ty = t / L.tiles_x, tx = t - ty * L.tiles_x;
+            int d = kTowerTileFar;
+            if (t < Ti) {
+                d = s_dist[pred ? 2 * ty * L.tiles_x + tx : t];
+                if (pred && 2 * ty + 1 < L.tiles_y) d = min(d, s_dist[(2 * ty + 1) * L.tiles_x + tx]);
+            }
+            const bool on = d <= p.reach - i;
             int total;
             const int at = written + block_exclusive_scan(on ? 1 : 0, s_warp, &total);
             if (on) {
                 stage[static_cast<size_t>(i) * p.cap + at] = tile_entry(l, b, t);
-                const int ty = t / L.tiles_x, tx = t - ty * L.tiles_x;
-                atomicAdd(&s_pix, min(L.th, L.H - ty * L.th) * min(L.tw, L.W - tx * L.tw));
+                atomicAdd(&s_pix, min(th, L.H - ty * th) * min(L.tw, L.W - tx * L.tw));
             }
             written += total;
         }
         __syncthreads();
         if (threadIdx.x == 0) {
-            // pair tile: an odd list gets the out-of-image tile T (tile row tiles_y), whose rows are never stored
-            if (written & 1) stage[static_cast<size_t>(i) * p.cap + written++] = tile_entry(l, b, T);
+            // pair tile: the list is padded to whole units with the out-of-image tile T (tile row tiles_y), whose rows are
+            // never stored
+            while (!pred && (written & 3)) stage[static_cast<size_t>(i) * p.cap + written++] = tile_entry(l, b, T);
             p.bl_count[i * nbl + k] = written;
             p.bl_pixels[i * nbl + k] = s_pix;
         }
@@ -167,9 +178,7 @@ __global__ void __launch_bounds__(kThreads) tower_tiles_kernel(const TowerTilesP
             __syncthreads();
             for (int s = warp; s < min(kThreads, nbl - k0); s += kWarps) {
                 const int k2 = k0 + s, l2 = k2 / p.B, b2 = k2 - l2 * p.B;
-                const int T2 = p.lvl[l2].tiles_x * p.lvl[l2].tiles_y;
-                const uint32_t* src = p.stage + static_cast<size_t>(i) * p.cap + p.lvl[l2].stage_begin +
-                                      static_cast<size_t>(b2) * (T2 + (T2 & 1));
+                const uint32_t* src = p.stage + static_cast<size_t>(i) * p.cap + region(p.lvl[l2], b2);
                 uint32_t* dst = p.list + static_cast<size_t>(i) * p.cap + s_at[s];
                 const int cnt = s_n[s];
                 for (int j0 = 0; j0 < cnt; j0 += 32 * kCopyBatch) {

@@ -143,6 +143,7 @@ SIGNATURES = {
     "dd3d_op_conv2d": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _I, _I, _P, _P, _I, _P, _I, _I, _P, _I, _I, _P]),
     "dd3d_op_conv2d_grouped": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _I, _P, _P, _I, _P, _I, _P]),
     "dd3d_op_conv2d_tiles": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _I, _P, _I, _P, _P, _P]),
+    "dd3d_op_conv2d_tiles8x8": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _I, _P, _I, _P, _P, _P]),
     "dd3d_op_conv2d_taps_tiles": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P, _P, _I, _P, _I, _I, _P, _P, _P]),
     "dd3d_op_b3d_sparse": (_I, [C.POINTER(_P), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(_P), C.POINTER(_P),
                                 C.POINTER(_P), _P, _P, _I, _I, _I, _I, _P, _I, _P]),

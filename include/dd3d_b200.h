@@ -448,14 +448,19 @@ int dd3d_op_conv2d_grouped(const void* d_in, int B, int H, int W, int C, int in_
                            int stride, const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch,
                            dd3d_stream stream);
 /* dd3d_op_conv2d_tiles: dd3d_op_conv2d (3x3, stride 1, 16-bit output, cout a multiple of 128, no residual) on the pair-tile
- * kernel in work-list mode, the form the engine runs the sparse box3d tower in: only the 16x8 output tiles listed in d_tiles
- * are computed, every other output pixel is left untouched.  d_tiles: device uint32 entries (img << 16) | tile, tile = the
- * row-major index of a 16x8 tile of one image (the tile count of an image, ceil(H/16) * ceil(W/8), names the out-of-image
- * tile, which writes nothing); consecutive entries 2i, 2i + 1 form one work item.  d_count: device int32, the number of
- * entries (even), read by the kernel. */
+ * kernel in work-list mode: only the 16x8 output tiles listed in d_tiles are computed, every other output pixel is left
+ * untouched.  d_tiles: device uint32 entries (img << 16) | tile, tile = the row-major index of a 16x8 tile of one image (the
+ * tile count of an image, ceil(H/16) * ceil(W/8), names the out-of-image tile, which writes nothing); consecutive entries
+ * 2i, 2i + 1 form one work item and name one image.  d_count: device int32, the number of entries (even), read by the kernel.
+ * dd3d_op_conv2d_tiles8x8: the same on 8x8 tiles (ceil(H/8) * ceil(W/8) per image), the form the engine runs the sparse
+ * towers in: consecutive entries 4i .. 4i + 3 form one work item and name one image; the number of entries is a multiple
+ * of 4. */
 int dd3d_op_conv2d_tiles(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
                          const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch, const uint32_t* d_tiles,
                          const int32_t* d_count, dd3d_stream stream);
+int dd3d_op_conv2d_tiles8x8(const void* d_in, int B, int H, int W, int cin, int in_pitch, const void* d_w, int cout,
+                            const float* d_scale, const float* d_bias, int relu, void* d_out, int out_pitch,
+                            const uint32_t* d_tiles, const int32_t* d_count, dd3d_stream stream);
 /* dd3d_op_conv2d_taps_tiles: the 3x3 stride-1 conv of dd3d_op_conv2d with cout <= 16 on the taps-in-N kernel in work-list
  * mode, the form the engine runs the sparse box2d tower's predictor in: only the 16x8 output tiles listed in d_tiles are
  * computed (entries as in dd3d_op_conv2d_tiles, one work item each, the out-of-image tile writes nothing), every other output
