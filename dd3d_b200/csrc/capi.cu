@@ -2,6 +2,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <set>
 #include <string>
 
 #include "engine.cuh"
@@ -12,6 +13,15 @@ using namespace dd3d;
 struct dd3d_engine {
     Engine* eng = nullptr;
     std::string err;
+    std::set<dd3d_graph_t*> graphs;  // live graphs of this handle: dd3d_destroy detaches them
+};
+
+// A captured forward; `h` is null once its handle is destroyed.
+struct dd3d_graph_t {
+    dd3d_engine* h = nullptr;
+    Engine::CapturedForward cf;
+    uint64_t generation = 0;  // Engine::generation at the capture
+    int device = 0;
 };
 
 namespace {
@@ -70,6 +80,7 @@ int dd3d_create(const dd3d_model_desc* h_desc, dd3d_handle* out) {
 
 void dd3d_destroy(dd3d_handle h) {
     if (h == nullptr) return;
+    for (dd3d_graph_t* g : h->graphs) g->h = nullptr;  // stale from now on; dd3d_graph_destroy still frees them
     delete h->eng;
     delete h;
 }
@@ -197,6 +208,60 @@ int dd3d_forward_host(dd3d_handle h, const void* h_images, int img_dtype, const 
     });
 }
 
+int dd3d_graph_create(dd3d_handle h, const void* d_images, int img_dtype, const float* d_intrinsics,
+                      const int32_t* d_sizes, dd3d_det* d_out, int32_t* d_counts, dd3d_stream stream, dd3d_graph* out) {
+    if (!out) return DD3D_ERR_INVALID;
+    *out = nullptr;
+    if (!d_images || !d_intrinsics || !d_sizes || !d_out || !d_counts) return DD3D_ERR_INVALID;
+    dd3d_graph_t* g = nullptr;
+    const int st = guarded(h, [&](Engine& e) {
+        const Engine::CapturedForward cf = e.capture_forward(d_images, img_dtype, d_intrinsics, d_sizes,
+                                                             reinterpret_cast<Det*>(d_out), d_counts,
+                                                             static_cast<cudaStream_t>(stream));
+        g = new dd3d_graph_t{h, cf, e.generation, e.device};
+    });
+    if (st != DD3D_OK) {
+        if (h) g_create_error = h->err;
+        return st;
+    }
+    h->graphs.insert(g);
+    *out = g;
+    return DD3D_OK;
+}
+
+int dd3d_graph_launch(dd3d_graph g, dd3d_stream stream) {
+    if (g == nullptr) return DD3D_ERR_INVALID;
+    const char* stale = g->h == nullptr                             ? "the handle was destroyed"
+                        : g->h->eng->generation != g->generation ? "dd3d_plan or a dd3d_set_* call since the capture"
+                                                                  : nullptr;
+    std::string err;
+    int st = DD3D_OK;
+    if (stale) {
+        err = std::string("stale graph: ") + stale + "; create a new one";
+        st = DD3D_ERR_STATE;
+    } else {
+        cudaSetDevice(g->device);
+        st = cuda_status(cudaGraphLaunch(g->cf.exec, static_cast<cudaStream_t>(stream)), &err);
+    }
+    if (st != DD3D_OK) {
+        g_create_error = err;
+        if (g->h) g->h->err = err;
+    }
+    return st;
+}
+
+void dd3d_graph_destroy(dd3d_graph g) {
+    if (g == nullptr) return;
+    if (g->h) g->h->graphs.erase(g);
+    cudaSetDevice(g->device);
+    cudaGraphExecDestroy(g->cf.exec);
+    delete g;
+}
+
+int dd3d_graph_kernel_nodes(dd3d_graph g) { return g ? g->cf.kernel_nodes : DD3D_ERR_INVALID; }
+
+int dd3d_graph_programmatic_edges(dd3d_graph g) { return g ? g->cf.programmatic_edges : DD3D_ERR_INVALID; }
+
 int dd3d_set_conv_policy(const char* name, int value) {
     if (!name) return DD3D_ERR_INVALID;
     if (!strcmp(name, "nms_class_parallel")) {
@@ -284,6 +349,7 @@ int dd3d_copy_flags(dd3d_handle h, int32_t* d_dst, dd3d_stream stream) {
 
 int dd3d_set_option(dd3d_handle h, const char* name, int value) {
     return guarded(h, [&](Engine& e) {
+        ++e.generation;
         const std::string n(name ? name : "");
         if (n == "do_postprocess") {
             e.opt_do_postprocess = value ? 1 : 0;
@@ -321,11 +387,17 @@ int dd3d_set_option(dd3d_handle h, const char* name, int value) {
 }
 
 int dd3d_set_bev_nms(dd3d_handle h, int enable, float iou_thresh) {
-    return guarded(h, [&](Engine& e) { e.set_bev_nms(enable, iou_thresh); });
+    return guarded(h, [&](Engine& e) {
+        ++e.generation;
+        e.set_bev_nms(enable, iou_thresh);
+    });
 }
 
 int dd3d_set_poses(dd3d_handle h, const float* d_poses) {
-    return guarded(h, [&](Engine& e) { e.user_poses = d_poses; });
+    return guarded(h, [&](Engine& e) {
+        ++e.generation;
+        e.user_poses = d_poses;
+    });
 }
 
 int dd3d_set_host_poses(dd3d_handle h, int slot, const float* h_poses) {
@@ -339,12 +411,16 @@ int dd3d_bev_nms_path(const dd3d_model_desc* h_desc) {
 }
 
 int dd3d_set_sample_aggregate(dd3d_handle h, int enable, float iou_thresh, int max_dets) {
-    return guarded(h, [&](Engine& e) { e.set_sample_aggregate(enable, iou_thresh, max_dets); });
+    return guarded(h, [&](Engine& e) {
+        ++e.generation;
+        e.set_sample_aggregate(enable, iou_thresh, max_dets);
+    });
 }
 
 int dd3d_set_groups(dd3d_handle h, const int32_t* d_group, int num_groups) {
     if (d_group && num_groups < 1) return DD3D_ERR_INVALID;
     return guarded(h, [&](Engine& e) {
+        ++e.generation;
         e.user_groups = d_group;
         e.user_num_groups = d_group ? num_groups : 0;
     });
@@ -356,7 +432,10 @@ int dd3d_set_host_groups(dd3d_handle h, int slot, const int32_t* h_group, int nu
 }
 
 int dd3d_set_global_out(dd3d_handle h, float* d_global) {
-    return guarded(h, [&](Engine& e) { e.user_global = d_global; });
+    return guarded(h, [&](Engine& e) {
+        ++e.generation;
+        e.user_global = d_global;
+    });
 }
 
 int dd3d_set_host_global_out(dd3d_handle h, int slot, float* h_global) {

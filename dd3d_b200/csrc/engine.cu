@@ -1689,6 +1689,7 @@ void Engine::release_plan() { free_plan(&plan); }
 
 void Engine::drop_plans() {
     if (slot_busy[0] || slot_busy[1]) fail(DD3D_ERR_STATE, "plan change with a pending dd3d_submit_host");
+    ++generation;
     release_plan();
     for (auto& kv : plan_cache) free_plan(&kv.second);
     plan_cache.clear();
@@ -1698,6 +1699,7 @@ void Engine::make_plan(int B, int Hs, int Ws, void* workspace, size_t bytes) {
     if (!finalized) fail(DD3D_ERR_STATE, "plan before finalize");
     if (B < 1 || Hs < 1 || Ws < 1) fail(DD3D_ERR_INVALID, "bad plan shape");
     if (slot_busy[0] || slot_busy[1]) fail(DD3D_ERR_STATE, "plan change with a pending dd3d_submit_host");
+    ++generation;  // even a same-shape call: captured forwards of the old plan are stale
     cuda_check(cudaSetDevice(device), "cudaSetDevice");
     if (workspace == nullptr && plan.valid && plan.owned_workspace && plan.B == B && plan.Hs == Hs && plan.Ws == Ws &&
         opt_workspace_fill < 0)
@@ -2064,6 +2066,62 @@ void Engine::forward(const void* d_images, int img_dtype, const float* d_K, cons
         mark(s.cat, s.op);
     }
     if (opt_profile) prof_used = ev_i;
+}
+
+// The forward above, recorded once.  Nothing in it synchronises, allocates or reads a device value back while profiling is
+// off, and the device state that outlives a forward (tile-list tickets, box2d tile distances, the flags word) is reset by
+// its own kernels, so a replay does what a new call would.  launch_pdl's attribute becomes a programmatic edge.
+Engine::CapturedForward Engine::capture_forward(const void* d_images, int img_dtype, const float* d_K,
+                                                const int32_t* d_sizes, Det* d_out, int32_t* d_counts,
+                                                cudaStream_t stream) {
+    if (!plan.valid) fail(DD3D_ERR_STATE, "graph capture before dd3d_plan");
+    if (opt_profile) fail(DD3D_ERR_STATE, "graph capture with option \"profile\" on: its per-step events are for dd3d_forward");
+    // the legacy default stream cannot be captured; a private one records the same launches
+    struct OwnStream {
+        cudaStream_t s = nullptr;
+        ~OwnStream() { if (s) cudaStreamDestroy(s); }
+    } own;
+    if (stream == nullptr || stream == cudaStreamLegacy) {
+        cuda_check(cudaStreamCreateWithFlags(&own.s, cudaStreamNonBlocking), "cudaStreamCreate");
+        stream = own.s;
+    }
+    cuda_check(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal), "cudaStreamBeginCapture");
+    int status = DD3D_OK;
+    std::string msg;
+    try {
+        forward(d_images, img_dtype, d_K, d_sizes, d_out, d_counts, user_poses, device_agg_args(), stream);
+    } catch (const EngineError& e) {
+        status = e.status;
+        msg = e.msg;
+    }
+    struct OwnGraph {
+        cudaGraph_t g = nullptr;
+        ~OwnGraph() { if (g) cudaGraphDestroy(g); }
+    } graph;
+    const cudaError_t end = cudaStreamEndCapture(stream, &graph.g);  // ends the capture whatever happened inside it
+    if (status != DD3D_OK || end != cudaSuccess) {
+        cudaGetLastError();  // a failed capture leaves no sticky error
+        if (status == DD3D_OK) status = DD3D_ERR_CUDA, msg = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(end);
+        fail(status, "graph capture: " + msg);
+    }
+    CapturedForward cf;
+    size_t n = 0;
+    cuda_check(cudaGraphGetNodes(graph.g, nullptr, &n), "cudaGraphGetNodes");
+    std::vector<cudaGraphNode_t> nodes(n);
+    cuda_check(cudaGraphGetNodes(graph.g, nodes.data(), &n), "cudaGraphGetNodes");
+    for (cudaGraphNode_t node : nodes) {
+        cudaGraphNodeType t;
+        cuda_check(cudaGraphNodeGetType(node, &t), "cudaGraphNodeGetType");
+        cf.kernel_nodes += t == cudaGraphNodeTypeKernel;
+    }
+    size_t ne = 0;
+    cuda_check(cudaGraphGetEdges_v2(graph.g, nullptr, nullptr, nullptr, &ne), "cudaGraphGetEdges");
+    std::vector<cudaGraphNode_t> from(ne), to(ne);
+    std::vector<cudaGraphEdgeData> edges(ne);
+    cuda_check(cudaGraphGetEdges_v2(graph.g, from.data(), to.data(), edges.data(), &ne), "cudaGraphGetEdges");
+    for (const cudaGraphEdgeData& e : edges) cf.programmatic_edges += e.type == cudaGraphDependencyTypeProgrammatic;
+    cuda_check(cudaGraphInstantiate(&cf.exec, graph.g, 0), "cudaGraphInstantiate");
+    return cf;
 }
 
 void Engine::launch_op(const Op& op, cudaStream_t stream) {

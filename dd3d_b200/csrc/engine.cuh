@@ -241,6 +241,15 @@ class Engine {
     void forward(const void* d_images, int img_dtype, const float* d_K, const int32_t* d_sizes, Det* d_out,
                  int32_t* d_counts, const float* d_poses, const AggArgs& agg, cudaStream_t stream,
                  const RawArgs* raw = nullptr);
+    // One forward of the current plan recorded by stream capture and instantiated (dd3d_graph_create): the launches of
+    // forward() with the device poses / groups / global rows and the options as they are now
+    struct CapturedForward {
+        cudaGraphExec_t exec = nullptr;
+        int kernel_nodes = 0;
+        int programmatic_edges = 0;  // edges the PDL launch attribute became
+    };
+    CapturedForward capture_forward(const void* d_images, int img_dtype, const float* d_K, const int32_t* d_sizes,
+                                    Det* d_out, int32_t* d_counts, cudaStream_t stream);
     void forward_host(const void* h_images, int img_dtype, const float* h_K, const int32_t* h_sizes, Det* h_out,
                       int32_t* h_counts, cudaStream_t stream);
     // double-buffered host path: H2D of one slot on a private copy stream while the other slot computes
@@ -323,6 +332,9 @@ class Engine {
     int num_sms = 132;
     int fp16 = 0;  // desc.act_dtype == DD3D_ACT_FP16: 16-bit storage of activations / weights is fp16 instead of bf16
     bool finalized = false;
+    // Bumped by every dd3d_plan, every plan drop and every dd3d_set_* call a forward reads (options, BEV NMS, poses, sample
+    // aggregation, groups, global rows): a captured forward is current while the counter still has its capture-time value
+    uint64_t generation = 0;
     int opt_do_postprocess = 1;
     int opt_profile = 0;
     int opt_workspace_reuse = 1;  // 0: bump allocation, every op output keeps its own memory (stage-level tests / debugging)

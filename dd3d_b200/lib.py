@@ -106,6 +106,11 @@ SIGNATURES = {
     "dd3d_workspace_bytes": (_I64, [_P, _I, _I, _I]),
     "dd3d_plan": (_I, [_P, _I, _I, _I, _P, _I64]),
     "dd3d_forward": (_I, [_P, _P, _I, _P, _P, _P, _P, _P]),
+    "dd3d_graph_create": (_I, [_P, _P, _I, _P, _P, _P, _P, _P, C.POINTER(_P)]),
+    "dd3d_graph_launch": (_I, [_P, _P]),
+    "dd3d_graph_destroy": (None, [_P]),
+    "dd3d_graph_kernel_nodes": (_I, [_P]),
+    "dd3d_graph_programmatic_edges": (_I, [_P]),
     "dd3d_forward_host": (_I, [_P, _P, _I, _P, _P, _P, _P, _P]),
     "dd3d_set_conv_policy": (_I, [C.c_char_p, _I]),
     "dd3d_submit_host": (_I, [_P, _I, _P, _I, _P, _P, _P, _P, _P]),

@@ -61,6 +61,7 @@ class DD3DB200(nn.Module):
         self._handle = None
         self._plan_key = None
         self._host_bufs = None
+        self._graph_synced = None  # attributes capture_forward last pushed to the engine
         self.training = False
 
     # ------------------------------------------------------------------ nn.Module surface the callers use
@@ -114,6 +115,7 @@ class DD3DB200(nn.Module):
             _lib.load().dd3d_destroy(self._handle)
         self._handle = None
         self._plan_key = None
+        self._graph_synced = None
 
     def __del__(self):
         try:
@@ -406,6 +408,62 @@ class DD3DB200(nn.Module):
         return self.forward(batched_inputs)
 
     @torch.no_grad()
+    def capture_forward(self, images_u8, intrinsics, sizes, poses=None, groups=None):
+        """Records the forward on device buffers the caller keeps as a CUDA graph (dd3d_graph_create) and returns a
+        CapturedForward: per frame, write the next images / intrinsics / sizes into the same tensors, then ``launch()``.
+        images_u8: [B][3][Hs][Ws] uint8 (or float32); intrinsics: [B][3][3] or [B][9] float32; sizes: [B][4] int32 =
+        (h, w, out_h, out_w) as dd3d_forward reads them.  With do_bev_nms (or the NuscenesDD3D sample aggregation) ``poses``
+        is a [B][7] float32 device tensor and, for the aggregation, ``groups`` the group index of every image.  The
+        attributes (postprocess_in_inference, do_nms, do_bev_nms) are taken as they are now; changing the engine's plan or
+        options afterwards makes the graph stale (launch raises) -- forward() and the other paths push the options again,
+        and with do_bev_nms or the aggregation so does every capture (it binds its poses)."""
+        B = int(images_u8.shape[0]) if images_u8.dim() == 4 else -1
+        tensors = dict(images=images_u8, intrinsics=intrinsics, sizes=sizes)
+        shapes_ok = (B > 0 and images_u8.shape[1] == 3 and intrinsics.numel() == 9 * B and tuple(sizes.shape) == (B, 4)
+                     and images_u8.dtype in (torch.uint8, torch.float32) and intrinsics.dtype == torch.float32
+                     and sizes.dtype == torch.int32)
+        if not shapes_ok:
+            raise ValueError("capture_forward: images [B][3][H][W] uint8 / float32, intrinsics [B][9] float32 and sizes "
+                             "[B][4] int32")
+        for name, t in tensors.items():
+            if t.device != self._device or not t.is_contiguous():
+                raise ValueError(f"capture_forward: {name} must be a contiguous tensor on {self._device}")
+        # every option call makes the engine's graphs stale: push the attributes only when they changed since the last
+        # capture, so that several graphs of one shape can live side by side
+        attrs = (self.postprocess_in_inference, self.do_nms, self.do_bev_nms, self.bev_nms_iou_thresh, self.only_box2d,
+                 getattr(self, "sample_aggregate_in_inference", None))
+        if self._handle is None or self._graph_synced != attrs:
+            self._sync_options(self.postprocess_in_inference)
+            self._graph_synced = attrs
+        self._plan(B, int(images_u8.shape[2]), int(images_u8.shape[3]))
+        L, h, cap = _lib.load(), self._handle, self._desc.out_cap
+        with torch.cuda.device(self._device):
+            keep = self._graph_bindings(B, poses, groups)
+            out = torch.empty((B, cap, _lib.DET_WORDS), dtype=torch.float32, device=self._device)
+            counts = torch.zeros((B + 1, ), dtype=torch.int32, device=self._device)  # [B] counts + overflow word
+            stream = torch.cuda.current_stream(self._device).cuda_stream
+            graph = C.c_void_p()
+            status = L.dd3d_graph_create(h, C.c_void_p(images_u8.data_ptr()),
+                                         _lib.IMG_U8 if images_u8.dtype == torch.uint8 else _lib.IMG_F32,
+                                         C.c_void_p(intrinsics.data_ptr()), C.c_void_p(sizes.data_ptr()),
+                                         C.c_void_p(out.data_ptr()), C.c_void_p(counts.data_ptr()), C.c_void_p(stream),
+                                         C.byref(graph))
+            _lib.check(status, None)
+        return CapturedForward(self, graph, out, counts, dict(tensors, **keep))
+
+    def _graph_bindings(self, B, poses, groups):
+        """The device buffers a captured forward reads besides its arguments, handed to the engine (dd3d_set_poses for the
+        BEV NMS); returns them so that the graph keeps them alive."""
+        return dict(poses=self._bind_poses(B, poses)) if self.do_bev_nms else {}
+
+    def _bind_poses(self, B, poses):
+        if poses is None or tuple(poses.shape) != (B, 7) or poses.dtype != torch.float32 or poses.device != self._device:
+            raise ValueError(f"capture_forward needs poses: a [{B}][7] float32 tensor on {self._device}")
+        poses = poses.contiguous()
+        _lib.check(_lib.load().dd3d_set_poses(self._handle, C.c_void_p(poses.data_ptr())), self._handle)
+        return poses
+
+    @torch.no_grad()
     def forward_host(self, batched_inputs):
         """End-to-end path through HOST buffers: pinned staging -> dd3d_forward_host (H2D, kernels, D2H, sync)."""
         batch, K, sizes, shape, is_u8 = self._gather_inputs(batched_inputs, self._device)
@@ -501,6 +559,7 @@ class DD3DB200(nn.Module):
         "workspace_reuse", "workspace_fill"): the next forward re-plans."""
         _lib.check(_lib.load().dd3d_set_option(self._engine(), name.encode(), int(value)), self._handle)
         self._plan_key = None
+        self._graph_synced = None
 
     def set_profile(self, on):
         """Record CUDA events around every engine op of the following forwards (dd3d_get_profile)."""
@@ -638,6 +697,24 @@ class NuscenesDD3DB200(DD3DB200):
             self._host_glob[slot] = glob
         _lib.check(L.dd3d_set_host_global_out(h, int(slot), C.c_void_p(glob.data_ptr())), h)
 
+    def _graph_bindings(self, B, poses, groups):
+        """With the sample aggregation: the poses, the group indices and a [B][cap][10] global-row buffer
+        (CapturedForward.global_rows) bound to the engine for the captured forward."""
+        keep = super()._graph_bindings(B, poses, groups)
+        if not self._aggregating():
+            return keep
+        if groups is None or len(groups) != B:
+            raise ValueError(f"capture_forward with the sample aggregation needs the group index of each of the {B} images")
+        L, h, device = _lib.load(), self._handle, self._device
+        if "poses" not in keep:  # the BEV NMS did not bind them already
+            keep["poses"] = self._bind_poses(B, poses)
+        groups = [int(g) for g in groups]
+        keep["group"] = torch.tensor(groups, dtype=torch.int32, device=device)
+        keep["global_rows"] = torch.zeros((B, self._desc.out_cap, _lib.GLOBAL_WORDS), dtype=torch.float32, device=device)
+        _lib.check(L.dd3d_set_groups(h, C.c_void_p(keep["group"].data_ptr()), max(groups) + 1), h)
+        _lib.check(L.dd3d_set_global_out(h, C.c_void_p(keep["global_rows"].data_ptr())), h)
+        return keep
+
     def _host_global_rows(self, slot):
         return self._host_glob.get(slot) if self._host_glob_live.get(slot) else None
 
@@ -645,6 +722,46 @@ class NuscenesDD3DB200(DD3DB200):
         host = r["counts"].cpu()  # the only sync: B counts + the overflow word (bits 3 / 5: the aggregation's capacity)
         self._check_flags(int(host[-1]))
         return self._wrap(r["out"], host[:-1], r["K"], r["sizes"], self._device, r["d_poses"].glob)
+
+
+class CapturedForward:
+    """A forward recorded as a CUDA graph (DD3DB200.capture_forward): thin wrapper over dd3d_graph_launch /
+    dd3d_graph_destroy.  ``launch(stream)`` replays it and copies the overflow word next to the counts; ``outputs()`` gives
+    the live output tensors (dets [B][cap][24] fp32 words, counts [B] int32, flags [1] int32), valid once the launch's stream
+    reaches them; ``global_rows`` is the [B][cap][10] pred_boxes3d_global buffer of the sample aggregation, or None."""
+    def __init__(self, model, graph, out, counts, buffers):
+        self._model, self._graph, self._out, self._counts, self._buffers = model, graph, out, counts, buffers
+        self._handle = model._handle
+        self.global_rows = buffers.get("global_rows")
+        L = _lib.load()
+        self.kernel_nodes = L.dd3d_graph_kernel_nodes(graph)
+        self.programmatic_edges = L.dd3d_graph_programmatic_edges(graph)
+
+    def launch(self, stream=None):
+        if self._graph is None:
+            raise RuntimeError("CapturedForward: launch after close()")
+        L, device = _lib.load(), self._model.device
+        if stream is None:
+            stream = torch.cuda.current_stream(device)
+        sp = C.c_void_p(stream.cuda_stream if isinstance(stream, torch.cuda.Stream) else stream)
+        _lib.check(L.dd3d_graph_launch(self._graph, sp), None)
+        B = self._out.shape[0]
+        _lib.check(L.dd3d_copy_flags(self._handle, C.c_void_p(self._counts[B:].data_ptr()), sp), self._handle)
+
+    def outputs(self):
+        B = self._out.shape[0]
+        return self._out, self._counts[:B], self._counts[B:]
+
+    def close(self):
+        if self._graph is not None:
+            _lib.load().dd3d_graph_destroy(self._graph)
+        self._graph = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:  # noqa: BLE001
+            pass
 
 
 class _DevArray:

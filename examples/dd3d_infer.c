@@ -1,7 +1,7 @@
 /*
  * dd3d_infer -- run DD3D on one image from a self-contained model file, through the C ABI alone.
  *
- *   dd3d_infer MODEL_FILE IMAGE H W fx s cx 0 fy cy 0 0 1
+ *   dd3d_infer [-g] MODEL_FILE IMAGE H W fx s cx 0 fy cy 0 0 1
  *
  * MODEL_FILE: written by DD3DB200.save_model_file.  IMAGE: H * W * 3 bytes, uint8 BGR in CHW order (the layout of the
  * Python model's input["image"]).  The nine numbers: the 3x3 intrinsics, row-major.  Prints one line per detection:
@@ -10,9 +10,16 @@
  *
  * with boxes in the pixel coordinates of the image (option "do_postprocess" on, output size = input size).  Floats print
  * with 9 significant digits, enough to read back the exact fp32 value.
+ *
+ * -g: the per-frame loop of a deployment instead of dd3d_forward_host: device buffers the program owns, one forward
+ * recorded as a CUDA graph (dd3d_graph_create), then per frame write the inputs, dd3d_graph_launch, read the detections
+ * back.  Same output.
  */
 #include <stdio.h>
 #include <stdlib.h>
+#include <string.h>
+
+#include <cuda_runtime.h>
 
 #include "dd3d_b200.h"
 
@@ -22,9 +29,59 @@ static int fail(const char* what, int status, dd3d_handle h) {
     return 1;
 }
 
+/* One frame through a captured forward: device buffers, dd3d_graph_create, H2D, dd3d_graph_launch, D2H. */
+static int run_graph(dd3d_handle h, const unsigned char* image, size_t image_bytes, const float* K, const int32_t* sizes,
+                     dd3d_det* dets, int cap, int32_t* count) {
+    void *d_image = NULL, *d_K = NULL, *d_sizes = NULL, *d_dets = NULL, *d_count = NULL;
+    dd3d_graph g = NULL;
+    int st = DD3D_ERR_CUDA;
+    if (cudaMalloc(&d_image, image_bytes) != cudaSuccess || cudaMalloc(&d_K, 9 * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&d_sizes, 4 * sizeof(int32_t)) != cudaSuccess ||
+        cudaMalloc(&d_dets, sizeof(dd3d_det) * (size_t)cap) != cudaSuccess ||
+        cudaMalloc(&d_count, sizeof(int32_t)) != cudaSuccess) {
+        fprintf(stderr, "dd3d_infer: cudaMalloc failed\n");
+        goto done;
+    }
+    if ((st = dd3d_graph_create(h, d_image, DD3D_IMG_U8, d_K, d_sizes, d_dets, d_count, NULL, &g)) != DD3D_OK) {
+        fprintf(stderr, "dd3d_infer: dd3d_graph_create failed (%d): %s\n", st, dd3d_last_error(h));
+        goto done;
+    }
+    /* the per-frame loop, here one frame: write the bound input buffers, launch, read back */
+    st = DD3D_ERR_CUDA;
+    if (cudaMemcpy(d_image, image, image_bytes, cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(d_K, K, 9 * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess ||
+        cudaMemcpy(d_sizes, sizes, 4 * sizeof(int32_t), cudaMemcpyHostToDevice) != cudaSuccess) {
+        fprintf(stderr, "dd3d_infer: cudaMemcpy failed\n");
+        goto done;
+    }
+    if ((st = dd3d_graph_launch(g, NULL)) != DD3D_OK) {
+        fprintf(stderr, "dd3d_infer: dd3d_graph_launch failed (%d): %s\n", st, dd3d_last_error(h));
+        goto done;
+    }
+    st = DD3D_ERR_CUDA;
+    if (cudaMemcpy(count, d_count, sizeof(int32_t), cudaMemcpyDeviceToHost) != cudaSuccess ||
+        cudaMemcpy(dets, d_dets, sizeof(dd3d_det) * (size_t)cap, cudaMemcpyDeviceToHost) != cudaSuccess) {
+        fprintf(stderr, "dd3d_infer: cudaMemcpy failed\n");
+        goto done;
+    }
+    st = DD3D_OK;
+done:
+    dd3d_graph_destroy(g);
+    cudaFree(d_image);
+    cudaFree(d_K);
+    cudaFree(d_sizes);
+    cudaFree(d_dets);
+    cudaFree(d_count);
+    return st;
+}
+
 int main(int argc, char** argv) {
+    const char* prog = argv[0];
+    const int graph = argc > 1 && strcmp(argv[1], "-g") == 0;
+    argv += graph;
+    argc -= graph;
     if (argc != 14) {
-        fprintf(stderr, "usage: %s MODEL_FILE IMAGE H W k00 k01 k02 k10 k11 k12 k20 k21 k22\n", argv[0]);
+        fprintf(stderr, "usage: %s [-g] MODEL_FILE IMAGE H W k00 k01 k02 k10 k11 k12 k20 k21 k22\n", prog);
         return 2;
     }
     const int H = atoi(argv[3]), W = atoi(argv[4]);
@@ -57,8 +114,15 @@ int main(int argc, char** argv) {
     const int32_t sizes[4] = {H, W, H, W}; /* valid size, size the boxes are rescaled to */
     int32_t count = 0, flags = 0;
     if (!dets) return fail("malloc", 0, h);
-    st = dd3d_forward_host(h, image, DD3D_IMG_U8, K, sizes, dets, &count, NULL);
-    if (st != DD3D_OK) return fail("dd3d_forward_host", st, h);
+    if (graph) {
+        if (run_graph(h, image, image_bytes, K, sizes, dets, cap, &count) != DD3D_OK) {
+            dd3d_destroy(h);
+            return 1;
+        }
+    } else {
+        st = dd3d_forward_host(h, image, DD3D_IMG_U8, K, sizes, dets, &count, NULL);
+        if (st != DD3D_OK) return fail("dd3d_forward_host", st, h);
+    }
     if ((st = dd3d_overflow_flags(h, NULL, &flags)) != DD3D_OK) return fail("dd3d_overflow_flags", st, h);
     if (flags != 0) {
         fprintf(stderr, "dd3d_infer: detection capacity exceeded (flags %d)\n", flags);

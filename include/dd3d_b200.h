@@ -155,8 +155,8 @@ typedef struct dd3d_tta_view {
 /* ---- lifetime ------------------------------------------------------------------------------------------- */
 int dd3d_create(const dd3d_model_desc* h_desc, dd3d_handle* out);
 void dd3d_destroy(dd3d_handle h);
-const char* dd3d_last_error(dd3d_handle h); /* h may be NULL: error of the last failed dd3d_create or
-                                             * dd3d_create_from_file */
+const char* dd3d_last_error(dd3d_handle h); /* h may be NULL: error of the last failed dd3d_create,
+                                             * dd3d_create_from_file, dd3d_graph_create or dd3d_graph_launch */
 
 /* ---- self-contained model file: a trained model without Python or the PyTorch checkpoint -----------------------------
  * dd3d_create_from_file reads a model file written by DD3DB200.save_model_file (dd3d_b200/meta_arch.py) and builds the
@@ -249,7 +249,35 @@ int dd3d_plan(dd3d_handle h, int B, int Hs, int Ws, void* d_workspace, int64_t w
  * d_out: [B][out_cap] dd3d_det, d_counts: [B] int32.  Enqueues on `stream`; no host sync, no allocation. */
 int dd3d_forward(dd3d_handle h, const void* d_images, int img_dtype, const float* d_intrinsics,
                  const int32_t* d_sizes, dd3d_det* d_out, int32_t* d_counts, dd3d_stream stream);
-/* Same through HOST buffers (pinned recommended): copies inputs H2D, runs, copies detections and counts D2H,
+/* ---- the forward as a CUDA graph: record once, replay every frame -------------------------------------------------
+ * dd3d_graph_create records one dd3d_forward of the current plan with these device buffers (stream capture on `stream` in
+ * cudaStreamCaptureModeThreadLocal; the legacy default stream NULL cannot be captured, so a private stream records it then)
+ * and instantiates it.  Nothing runs at the call.  The graph holds the launches the forward would make now: the buffers
+ * above, the poses / groups / global-row buffers of dd3d_set_poses / dd3d_set_groups / dd3d_set_global_out, the BEV NMS and
+ * sample aggregation settings and options "do_postprocess" / "do_nms".  Per frame the caller writes the new images,
+ * intrinsics and sizes into the same buffers and calls dd3d_graph_launch, which enqueues the whole forward on `stream` (any
+ * stream of the handle's device) with one cudaGraphLaunch: the same kernels as dd3d_forward, bit-identical results, the
+ * kernels' programmatic dependent launches kept as programmatic edges (needs CUDA 12.3 or later).  Device state one forward
+ * leaves for the next is reset by the forward's own kernels, so replays may follow each other and dd3d_forward calls freely;
+ * like two forwards of one handle, they must not run concurrently (they share the plan's workspace).
+ * Staleness: dd3d_plan (any shape), a plan drop, and every dd3d_set_option / dd3d_set_bev_nms / dd3d_set_poses /
+ * dd3d_set_sample_aggregate / dd3d_set_groups / dd3d_set_global_out call after the capture make the graph stale: its
+ * dd3d_graph_launch returns DD3D_ERR_STATE and launches nothing; create a new graph.  dd3d_destroy makes every graph of the
+ * handle stale the same way; dd3d_graph_destroy frees a graph before or after its handle.
+ * dd3d_graph_create returns DD3D_ERR_STATE before dd3d_plan or with option "profile" on (its events are for dd3d_forward),
+ * any status of dd3d_forward for its arguments, and DD3D_ERR_CUDA when the capture or the instantiation fails; a failed
+ * capture is ended and discarded, `stream` is not left capturing and *out is NULL.  The text of a failed dd3d_graph_create
+ * or dd3d_graph_launch is in dd3d_last_error(NULL), and in dd3d_last_error(h) while the handle lives. */
+typedef struct dd3d_graph_t* dd3d_graph;
+int dd3d_graph_create(dd3d_handle h, const void* d_images, int img_dtype, const float* d_intrinsics,
+                      const int32_t* d_sizes, dd3d_det* d_out, int32_t* d_counts, dd3d_stream stream, dd3d_graph* out);
+int dd3d_graph_launch(dd3d_graph g, dd3d_stream stream);
+void dd3d_graph_destroy(dd3d_graph g); /* NULL: no-op */
+/* Kernel nodes of the graph: dd3d_launches_per_forward of the plan it was captured from. */
+int dd3d_graph_kernel_nodes(dd3d_graph g);
+/* Programmatic (PDL) edges of the graph: one per launch made with the programmatic-serialization attribute. */
+int dd3d_graph_programmatic_edges(dd3d_graph g);
+/* dd3d_forward through HOST buffers (pinned recommended): copies inputs H2D, runs, copies detections and counts D2H,
  * then synchronises `stream`. */
 int dd3d_forward_host(dd3d_handle h, const void* h_images, int img_dtype, const float* h_intrinsics,
                       const int32_t* h_sizes, dd3d_det* h_out, int32_t* h_counts, dd3d_stream stream);
